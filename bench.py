@@ -1,6 +1,6 @@
-"""bench.py - learner frames/sec of the B200-native IMPALA learner hot path.
+"""bench.py - learner frames/sec of the H100-native IMPALA learner hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one full learn() step (AtariNet forward, fused V-trace + losses + their gradients,
@@ -15,6 +15,8 @@ Printed JSON (one line, rank 0):
           buffers: every step's inputs are copied host->device and the step's stats are read back
           inside the timed region.
   roofline / roofline_ops / vtrace / cpu_baseline / clocks / gpu_launches: see DESIGN.md section 5.
+--dump-outputs DIR writes what the last timed step computed (losses, V-trace targets, loss gradients, updated
+parameters) as DIR/<name>.npy, so that two builds can be compared output for output on identical seeded inputs.
 `--impl reference` times the CPU restatement of the reference's learner step (oracle/, kind
 "port") on the host cores: the reference itself is PyTorch-on-CPU code that cannot travel to the box.
 """
@@ -58,12 +60,19 @@ def parse():
                     help="BASELINE configs[2]: N synthetic host actor threads -> pinned slots -> learner queue -> "
                          "polybeast_learner.learn on --learner_threads threads; prints the end-to-end SPS line")
     ap.add_argument("--learner_threads", type=int, default=2)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32, <= 64 MB in all)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1 (the number of timed steps)")
+    if args.warmup < 0:
+        ap.error("--warmup must not be negative")
+    return args
 
 
 # what the arithmetic is, per backend (the line's `dtype`)
 DTYPE_NAMES = {
-    "bf16x3": "bf16x3 (split-bf16 hi+lo operands, 3 tcgen05 MMAs per product, fp32 accumulate; fp32 state/loss/optimizer)",
+    "bf16x3": "bf16x3 (split-bf16 hi+lo operands, 3 tensor-core MMAs per product, fp32 accumulate; fp32 state/loss/optimizer)",
     "bf16": "bf16 (single-plane bf16 operands, fp32 accumulate)",
     "fp32": "f32",
 }
@@ -94,7 +103,7 @@ def synthetic_host_batch(T, B, A, seed, pin):
 
 class ClockSampler:
     """nvidia-smi clocks/throttle reasons sampled every 50 ms.  Started before the warm-up (nvidia-smi needs ~0.2 s to
-    produce its first line and a step is ~2 ms) and filtered to the timed region by nvidia-smi's own timestamps; if
+    produce its first line and a step takes milliseconds) and filtered to the timed region by nvidia-smi's own timestamps; if
     that filter leaves nothing (clock skew, parse trouble) every collected sample is used."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -213,7 +222,8 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return dict(hbm=p["hbm_gbs"], tensor=p["bf16_tflops_sustained"], tensor_burst=p["bf16_tflops"], source="measured")
     except Exception:
-        return dict(hbm=6650.0, tensor=1400.0, tensor_burst=1590.0, source="fallback")
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16
+        return dict(hbm=3350.0, tensor=989.0, tensor_burst=989.0, source="H100 SXM data sheet")
 
 
 def gemm_flops_table(N, A, use_lstm):
@@ -337,7 +347,7 @@ def run_reference(args, world=1):
     shapes = (LT.resnet_param_shapes if net == "resnet" else LT.atarinet_param_shapes)(A, bool(args.use_lstm))
     p = LT.random_params(shapes, seed=0)
     # Thread count: the op-by-op CPU path is dispatch-bound and gets SLOWER with many threads
-    # (measured on the 128-thread B200 host: 250 s/step at 128 threads; SURVEY.md section 6), so pick
+    # (SURVEY.md section 6), so pick
     # the fastest of a few counts on a small calibration rollout and report it as `cores`.
     ncpu = os.cpu_count() or 1
     cal = synthetic_host_batch(8, 8, A, seed=2, pin=False)
@@ -567,7 +577,7 @@ def main():
     flags = flags_ns(T, B)
     flags.cuda_graph = bool(args.graph)
     state = model.initial_state(B)
-    NROT = 4  # distinct input batches: 4 x 73 MB > 126 MB L2
+    NROT = 4  # distinct input batches: 4 x 73 MB > 50 MB L2
     # N1: the rollouts live in the pinned slots of the package's RolloutStager (what the actors would write in place)
     example = synthetic_host_batch(T, B, A, seed=1000 * rank, pin=False)
     stager = staging.RolloutStager(staging.spec_like(example), dev, depth=NROT)
@@ -630,6 +640,8 @@ def main():
     launches = lib.tb_launch_count() - launches0
     ms = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     clocks = sampler.stop(t_region0, time.time()) if sampler else None
+    if args.dump_outputs and rank == 0:  # before anything else touches the model or the graph's output buffers
+        dump_outputs(args.dump_outputs, out, model)
     final_loss = float(out["losses"][3])
     assert np.isfinite(final_loss), "non-finite loss"
     if graphed is not None:  # launches per step: count one eager step (a graph replay launches the same kernels)
@@ -706,7 +718,7 @@ def main():
         warmup=args.warmup, ms_per_step=ms, higher_is_better=True, scaling=args.scaling, vs_baseline=None,
         dtype=DTYPE_NAMES.get(model.precision, model.precision),
         data="synthetic", config=config,
-        l2_policy="4 rotating input batches per rank (%.0f MB) > 126 MB L2; ~2.3 GB of activations written per step" % (
+        l2_policy="4 rotating input batches per rank (%.0f MB) > 50 MB L2; ~2.3 GB of activations written per step" % (
             NROT * h2d_bytes / 1e6),
         e2e=dict(value=frames / (e2e_ms * 1e-3), unit="frames/s", ms_per_step=e2e_ms, h2d_bytes_per_step=h2d_bytes,
                  d2h_bytes_per_step=d2h_bytes, h2d_gbs_measured=h2d_gbs, numa_node=numa, cuda_graph=graphed is not None,
@@ -719,8 +731,8 @@ def main():
         parity="default backend %s: tests/test_learner_baseline_gpu.py holds it to reference-generated T=80,B=32 fixtures "
                "(outputs, vs, pg_advantages, losses <= 1e-5)" % model.precision if args.net == "atari" else
                ("backend %s: tests/test_resnet_gpu.py holds it to the reference-generated T=80,B=8 fixture (one GPU's shard of "
-                "configs[3]): outputs, vs, pg_advantages, losses <= 1e-5; gradients relative L2 < 6e-3 per tensor "
-                "(profiles/parity_r2_resnet.txt)" % model.precision),
+                "configs[3]): outputs, vs, pg_advantages, losses <= 1e-5; gradients relative L2 < 6e-3 per tensor"
+                % model.precision),
     )
     if dp is not None:
         line["dp_check"] = dp
@@ -764,15 +776,9 @@ def main():
         prof_total = sum(o["ms_per_step"] for o in ops)
         line["roofline_ops"] = [dict(o, share=o["ms_per_step"] / prof_total) for o in ops[:12]]
         dom = next((o for o in ops if "achieved" in o), None)
-        try:
-            traffic_tab = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic_r2.json")))
-        except Exception:
-            traffic_tab = {}
         if dom is not None:
             line["roofline"] = dict(kernel=dom["op"], bound=dom["bound"], achieved=dom["achieved"], peak=dom["peak"],
-                                    unit=dom["unit"], frac=dom["frac"],
-                                    traffic=(traffic_tab.get(dom["op"], {}).get("dram_bytes_per_launch")),
-                                    launches_per_step=dom["launches_per_step"], peak_source=pk["source"],
+                                    unit=dom["unit"], frac=dom["frac"], launches_per_step=dom["launches_per_step"], peak_source=pk["source"],
                                     note=("latency-bound recurrence: T+1 dependent time steps, each a hand-off through L2 + tile "
                                           "all-gather + mma.sync products; neither roofline is approached - the algorithmic "
                                           "recurrent-product flops (2*M*N*K, not x3 for the split planes) are reported against the "
@@ -791,6 +797,39 @@ def main():
                                     **host_cpu_info())
     print(json.dumps(line))
     finish()
+
+
+DUMP_LIMIT = 64 << 20   # bytes written by --dump-outputs in all
+DUMP_SAMPLE = 1 << 20   # arrays larger than this many elements are stored as a fixed, seeded sample of this size
+
+
+def dump_outputs(path, out, model):
+    """The arrays a caller of the timed step receives: the step's losses, its V-trace / loss results and the updated
+    parameters, as float32 .npy files.  Large arrays are reduced to a fixed sample (seeded, so two runs with the same
+    arguments sample the same elements; the indices are stored beside it).  Nothing is written if the total would exceed
+    DUMP_LIMIT."""
+    tensors = {"losses": out["losses"]}
+    vt = out.get("vtrace")
+    if vt is not None:
+        for name in getattr(vt, "_fields", ()):
+            v = getattr(vt, name)
+            if torch.is_tensor(v):
+                tensors[name] = v
+    tensors["params"] = model.flat_params
+    files, total = {}, 0
+    for name, t in tensors.items():
+        a = t.detach().float().cpu().numpy().reshape(-1)  # .cpu() waits for the stream that produced t
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.RandomState(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            files[name + "_sample_index"] = idx.astype(np.float64)
+            a = a[idx]
+        files[name] = np.ascontiguousarray(a, dtype=np.float32)
+    total = sum(a.nbytes for a in files.values())
+    if total > DUMP_LIMIT:
+        raise SystemExit("--dump-outputs: %d bytes, more than the %d allowed" % (total, DUMP_LIMIT))
+    os.makedirs(path, exist_ok=True)
+    for name, a in files.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def vtrace_numbers(pk, T, B, A):

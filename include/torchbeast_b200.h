@@ -1,4 +1,4 @@
-/* torchbeast_b200 C-ABI: the drop-in boundary of the B200-native IMPALA learner hot path.
+/* torchbeast_b200 C-ABI: the drop-in boundary of the H100-native IMPALA learner hot path.
  *
  * Plain C, raw device pointers + sizes + a cudaStream_t passed as void*; no torch types.
  * The reference (facebookresearch/torchbeast) has NO FFI for this path - its boundary is
@@ -131,7 +131,7 @@ size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int u
  * -> policy_logits f32 [T1,B,A], baseline f32 [T1,B].  Activations stay in `workspace`.
  * precision: 0 = fp32 SIMT GEMMs (bit-comparable with the reference's fp32 CPU arithmetic);
  *            1 = bf16 operands with fp32 accumulation: conv/fc trunk (implicit-GEMM convolutions) and LSTM
- *                projections on tcgen05 tensor cores, LSTM recurrence products as bf16 mma.sync; LSTM state and
+ *                projections on wgmma tensor cores, LSTM recurrence products as bf16 mma.sync; LSTM state and
  *                gate math, heads, losses, optimizer, master weights and gradients stay fp32.             */
 int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* notdone,
                         const int64_t* last_action, const float* h0, const float* c0,
@@ -185,7 +185,7 @@ int64_t tb_resnet_param_count(int num_actions, int use_lstm);
 size_t tb_resnet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision);
 /* polybeast_learner.py:214-266 Net.forward without the action sampling: frame u8 [T1,B,4,84,84], reward f32
  * [T1,B], notdone f32 [T1,B] and h0,c0/hN,cN f32 [1,B,256] (LSTM only) -> policy_logits [T1,B,A], baseline [T1,B].
- * precision: 0 = fp32 SIMT patch-matrix GEMMs; 1 = bf16 activations + patch-matrix tcgen05 GEMMs (not parity-grade);
+ * precision: 0 = fp32 SIMT patch-matrix GEMMs; 1 = bf16 activations + patch-matrix wgmma GEMMs (not parity-grade);
  * 2 = split-bf16 (the Python default): fp32 activations, every 3x3 conv as a shifted-window implicit GEMM over padded
  * channel-chunk-planar hi/lo images (csrc/conv3x3_sw.cu), the H=256 LSTM on one thread-block cluster.  T1*B < 65536.
  * The same precision and workspace must be used for forward and backward.                                            */
@@ -221,7 +221,7 @@ int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, flo
                              const float* sumsq, float max_norm, const float* lr_device, float lr, float alpha,
                              float eps, float momentum, float* grad_norm_out, void* stream);
 
-/* ---- bf16 tensor-core GEMM (tcgen05 + TMEM + TMA), the throughput backend of the network -------- */
+/* ---- bf16 tensor-core GEMM (wgmma + TMA), the throughput backend of the network -------- */
 
 /* C[M,N] = relu?( scale * (A[M,K] . B[N,K]^T) + bias[N] );  A, B bf16 with K contiguous ("K-major"),
  * lda/ldb multiples of 8, 16-byte aligned; outputs fp32 C (ldc) and/or bf16 C_bf16 (ldc16), either may
@@ -237,11 +237,11 @@ int tb_gemm_bf16_ex(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N
                     int64_t ldb, int a_mn, int b_mn, float* C, int64_t ldc, int splits, float* partial,
                     void* stream);
 /* ---- implicit-GEMM convolutions (bf16 tensor-core backend) -------------------------------------------
- * The nn.Conv2d layers of AtariNet (monobeast.py:560-562: 8x8/4, 4x4/2, 3x3/1, no padding) as tcgen05 GEMMs whose
+ * The nn.Conv2d layers of AtariNet (monobeast.py:560-562: 8x8/4, 4x4/2, 3x3/1, no padding) as wgmma GEMMs whose
  * patch operand is read by TMA straight from the bf16 NHWC activation [Nf,H,W,C] (conv2/conv3) or gathered from a
  * bf16 image of the uint8 NCHW frames (conv1) - no patch matrix is materialised.  weight / dweight are fp32 in the
  * reference layout [O,C,KH,KW]; outputs bf16 NHWC.  *_scratch buffers are caller-owned device memory:
- * pack_scratch_bf16 >= max(O,4*C)*KH*KW*max(C,O) bf16, partial >= 148*O*KH*KW*C floats, image_bf16 = N*4*H*W bf16. */
+ * pack_scratch_bf16 >= max(O,4*C)*KH*KW*max(C,O) bf16, partial >= 132*O*KH*KW*C floats (one split per SM), image_bf16 = N*4*H*W bf16. */
 int tb_conv_nhwc_bf16_fwd(const void* act_bf16, const float* weight, const float* bias, int64_t Nf, int H, int W, int C,
                           int KH, int KW, int S, int O, int relu, void* out_bf16, void* pack_scratch_bf16, void* stream);
 /* dx = conv_transpose(dy, weight) * (act > 0)   (act_bf16 nullable: no ReLU mask); O must be 64, stride 1 or 2 (4x4) */

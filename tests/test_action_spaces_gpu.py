@@ -60,6 +60,6 @@ def test_forward_backward_other_action_spaces(A, use_lstm, B, precision):
     else:
         # bf16: same mechanism as test_learner_bf16_gpu.py (ReLU sign flips of pre-activations within 2^-9 of zero switch
         # whole gradient paths, error ~ sqrt(flip fraction)); with only N = 35 frames a handful of flips weighs more than in
-        # the fixtures, hence 0.2 / 0.98 here instead of 0.12 / 0.995 (measured worst: conv1 0.13 / 0.992 at A=18, no LSTM)
+        # the fixtures, hence 0.2 / 0.98 here instead of 0.12 / 0.995 (conv1 at A=18 without LSTM is the tightest case)
         bad = {n: v for n, v in report.items() if v[0] >= 0.2 or v[1] <= 0.98}
     assert not bad, (bad, report)

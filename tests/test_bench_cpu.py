@@ -1,9 +1,11 @@
-"""Host-side pieces of bench.py that can be checked without a GPU: the clock sampler's parsing / time-window filter."""
+"""Host-side pieces of bench.py that can be checked without a GPU: the clock sampler's parsing / time-window filter,
+--dump-outputs (identical files on identical inputs, sampling, size limit) and argument checks."""
 import datetime
 import importlib.util
 import os
 import sys
 import time
+import types
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -57,3 +59,56 @@ def test_clock_sampler_survives_garbage():
     s.rows = [["not a timestamp", "1950", "1965", "1", "Not Active", "Not Active", "Not Active", "Not Active"]]
     out = s.stop(now, now + 0.1)
     assert out["samples"] == 1 and out["in_timed_region"] is False
+
+
+def _dump_case(b):
+    import collections
+
+    import torch
+
+    g = torch.Generator().manual_seed(0)
+    VT = collections.namedtuple("VT", "vs grad_logits note")
+    out = dict(losses=torch.randn(4, generator=g),
+               vtrace=VT(torch.randn(80, 32, generator=g), torch.randn(81, 32, 6, generator=g), "not an array"))
+    model = types.SimpleNamespace(flat_params=torch.randn(b.DUMP_SAMPLE + 1000, generator=g))
+    return out, model
+
+
+def test_dump_outputs_writes_the_same_files_twice(tmp_path):
+    import numpy as np
+
+    b = _bench()
+    out, model = _dump_case(b)
+    for d in ("a", "b"):
+        b.dump_outputs(str(tmp_path / d), out, model)
+    names = sorted(os.listdir(tmp_path / "a"))
+    assert names == sorted(os.listdir(tmp_path / "b"))
+    assert names == ["grad_logits.npy", "losses.npy", "params.npy", "params_sample_index.npy", "vs.npy"]
+    for n in names:
+        x, y = np.load(tmp_path / "a" / n), np.load(tmp_path / "b" / n)
+        assert x.dtype in (np.float32, np.float64) and np.array_equal(x, y), n
+    # small arrays whole, the large one as a sample of its own elements at the stored indices
+    np.testing.assert_array_equal(np.load(tmp_path / "a" / "vs.npy"), out["vtrace"].vs.numpy().reshape(-1))
+    idx = np.load(tmp_path / "a" / "params_sample_index.npy").astype(np.int64)
+    assert idx.size == b.DUMP_SAMPLE and np.all(np.diff(idx) > 0)
+    np.testing.assert_array_equal(np.load(tmp_path / "a" / "params.npy"), model.flat_params.numpy()[idx])
+
+
+def test_dump_outputs_refuses_more_than_the_limit(tmp_path):
+    b = _bench()
+    out, model = _dump_case(b)
+    b.DUMP_LIMIT = 1024
+    try:
+        b.dump_outputs(str(tmp_path / "d"), out, model)
+    except SystemExit as e:
+        assert "more than" in str(e)
+    else:
+        raise AssertionError("no error above the limit")
+    assert not (tmp_path / "d").exists()
+
+
+def test_steps_must_be_positive():
+    import subprocess
+
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--steps", "0"], capture_output=True, text=True)
+    assert r.returncode != 0 and "--steps must be at least 1" in r.stderr

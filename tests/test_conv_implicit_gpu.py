@@ -1,4 +1,4 @@
-"""Implicit-GEMM convolutions (tcgen05 + TMA gather) against torch.nn.functional.conv2d / torch.nn.grad in fp64
+"""Implicit-GEMM convolutions (wgmma + TMA gather) against torch.nn.functional.conv2d / torch.nn.grad in fp64
 on the SAME bf16-rounded operands: the only differences left are fp32 accumulation order and the bf16 rounding
 of the output, so the tolerances are tight (2^-8 relative for bf16 outputs, 1e-4*sqrt(K) for fp32 sums).
 Shapes are AtariNet's conv2 / conv3 / conv1 (monobeast.py:560-562) with several frame counts (tile tails)."""
@@ -69,7 +69,7 @@ def test_conv_weight_gradient(H, W, C, K, S, O, N):
     act = _bf16(torch.randn(N, H, W, C, device="cuda", generator=g))
     dy = _bf16(torch.randn(N, OH, OH, O, device="cuda", generator=g))
     dw = torch.full((O, C, K, K), float("nan"), device="cuda")
-    part = torch.empty(148 * O * C * K * K, device="cuda")
+    part = torch.empty(132 * O * C * K * K, device="cuda")  # one split per SM
     _lib.check(_lib.lib().tb_conv_nhwc_bf16_wgrad(p(dy), p(act), N, H, W, C, K, K, S, O, p(dw), p(part), part.numel(), st), "wgrad")
     torch.cuda.synchronize()
     ref = torch.nn.grad.conv2d_weight(act.double().permute(0, 3, 1, 2), (O, C, K, K), dy.double().permute(0, 3, 1, 2), stride=S)
@@ -94,7 +94,7 @@ def test_conv1_from_uint8_frames(N):
     torch.testing.assert_close(out.double(), ref, rtol=2 ** -7, atol=1e-3)
     dy = _bf16(torch.randn(N, 20, 20, 32, device="cuda", generator=g))
     dw = torch.full((32, 4, 8, 8), float("nan"), device="cuda")
-    part = torch.empty(148 * 32 * 256, device="cuda")
+    part = torch.empty(132 * 32 * 256, device="cuda")
     _lib.check(_lib.lib().tb_conv1_u8_wgrad(p(dy), p(image), N, 84, 84, 4, p(dw), p(part), part.numel(), st), "conv1 wgrad")
     torch.cuda.synchronize()
     refw = torch.nn.grad.conv2d_weight(x, (32, 4, 8, 8), dy.double().permute(0, 3, 1, 2), stride=4)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMEM/TMA bf16 GEMM against a plain PyTorch fp32 reference of the same op
+"""GPU: the wgmma/TMA bf16 GEMM against a plain PyTorch fp32 reference of the same op
 (inputs rounded to bf16 first, so products are exact and only the fp32 accumulation order differs:
 tolerance rtol 1e-4 / atol 1e-4 x sqrt(K))."""
 import numpy as np

@@ -1,10 +1,9 @@
-"""GPU: the bf16 tensor-core backend (precision="bf16": tcgen05 GEMMs with bf16 operands and fp32
+"""GPU: the bf16 tensor-core backend (precision="bf16": wgmma GEMMs with bf16 operands and fp32
 accumulation for the conv/fc trunk and the LSTM projections) against the fp64 oracle.
 bf16 carries 8 mantissa bits (unit roundoff 2^-9 ~ 2e-3), so this is a mixed-precision tolerance,
-stated per quantity: learner outputs relative L2 error < 1e-2 (measured 1e-3), losses rtol 3e-2, and -
+stated per quantity: learner outputs relative L2 error < 1e-2, losses rtol 3e-2, and -
 for fixed cotangents - every parameter gradient relative L2 error < 0.12 with cosine similarity > 0.995.
-Measured (tools/bf16_report.py): heads/LSTM 1e-3, fc 2-5e-2, conv1 5-9e-2, cosine >= 0.9965.  The
-conv/fc figure is NOT GEMM rounding (that is ~3e-3): a bf16 forward flips the sign of the ~0.2% of
+tools/bf16_report.py prints the per-tensor errors.  The conv/fc error is NOT GEMM rounding (that is ~3e-3): a bf16 forward flips the sign of the ~0.2% of
 ReLU pre-activations that sit within 2^-9 of zero, and each flip switches a whole gradient path, so the
 L2 error is ~sqrt(flip fraction).  Any reduced-precision forward (incl. the reference's own TF32 cuDNN
 path on GPU) has this property; the same script shows the fp32 backend at 5e-7.  The fp32 backend holds

@@ -18,8 +18,8 @@ pytestmark = pytest.mark.gpu
 
 ATARI_CASES = ["learn_atari_T4_B2.npz", "learn_atari_T20_B4.npz", "learn_atari_T40_B6_clip10.npz"]
 # ReLU ties: in this case two conv2 pre-activations are |z| ~ 1e-8 (below fp32 resolution of the O(1)
-# sums that produce them), so fp32 implementations legitimately disagree on their sign (measured with
-# tools/debug_acts.py: forward max err 9e-7, 2 sign flips).  Each flip switches one unit's gradient on
+# sums that produce them), so fp32 implementations legitimately disagree on their sign (tools/debug_acts.py
+# shows them).  Each flip switches one unit's gradient on
 # or off, which moves conv1/conv2 gradients by ~1e-3 relative; the tolerances for this case allow it.
 TIE_CASES = {"learn_atari_T40_B6_clip10.npz": 10.0}
 LSTM_CASES = ["learn_atari_lstm_T4_B2.npz", "learn_atari_lstm_T20_B4.npz"]
@@ -125,7 +125,7 @@ def test_full_gradients_vs_oracle(fname, precision):
         ref = o["grads"][n].numpy()
         got = p.grad.cpu().numpy()
         # fp32 backend: 1e-4 x the tensor's largest gradient; split-bf16: 3e-3 x (its ~2^-17 products move the handful of
-        # ReLU pre-activations that sit at the rounding threshold, measured 1.2e-3 on conv1 at T=20,B=4)
+        # ReLU pre-activations that sit at the rounding threshold)
         tol = (1e-4 if precision == "fp32" else 3e-3) * max(np.abs(ref).max(), 1e-6)
         np.testing.assert_allclose(got, ref, rtol=1e-3, atol=tol, err_msg=n)
 

@@ -85,7 +85,7 @@ def test_learn_matches_reference(fname, precision):
         scale = max(float(g["grad_stats/" + n][2]), 1e-6)
         # split-bf16: conv outputs carry ~5e-6 relative rounding, enough to flip a handful of max-pool argmax / ReLU
         # decisions in this tiny case; every flip moves the gradients upstream of it by ~1e-3 of their norm while tensors
-        # with no flip upstream agree to 1e-5 (profiles/resnet_flips_r2.txt) - same bounds as the T=80 baseline tests
+        # with no flip upstream agree to 1e-5 (tools/resnet_flips.py) - same bounds as the T=80 baseline tests
         gatol, nrtol = (5e-4, 2e-3) if precision == "fp32" else (1.5e-2, 2e-2)
         np.testing.assert_allclose(gr.flatten()[:16].numpy(), g["grad_head/" + n], rtol=5e-3, atol=gatol * scale, err_msg=n)
         np.testing.assert_allclose(float(gr.double().norm()), float(g["grad_stats/" + n][2]), rtol=nrtol, atol=1e-6, err_msg=n)
@@ -124,7 +124,7 @@ def test_backward_vs_oracle_fixed_cotangents(fname, precision):
         report[n] = (round(rel(got, ref[n]), 5), round(cos, 6))
     # split-bf16 ("bf16x3"): hi.hi + hi.lo + lo.hi products, ~2^-17 relative each: 1e-5 where no max-pool / ReLU decision
     # flips upstream; in this 10-frame case ONE flipped ReLU / argmax moves a gradient tensor by up to ~1e-2 of its norm and
-    # which elements flip depends on the summation order (profiles/resnet_flips_r2.txt).  So: every tensor within 3e-2 with
+    # which elements flip depends on the summation order (tools/resnet_flips.py).  So: every tensor within 3e-2 with
     # cosine > 0.9995, and the MEDIAN tensor within 5e-3 (plain bf16 operands sit at 2e-2 .. 2e-1 on every tensor)
     lim = {"fp32": (1e-4, 0.999999), "bf16x3": (3e-2, 0.9995), "bf16": (0.2, 0.98)}[precision]
     bad = {n: v for n, v in report.items() if v[0] >= lim[0] or v[1] <= lim[1]}

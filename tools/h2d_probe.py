@@ -1,4 +1,4 @@
-"""Why is the pinned host->device rate 33 GB/s in a plain `python bench.py` but 55 GB/s under torchrun on the same node
+"""Why does the pinned host->device rate differ between a plain `python bench.py` and torchrun on the same node
 (VERDICT r1, Missing 1)?  Each variant runs in a fresh subprocess and prints its measured rate.
 usage: python tools/h2d_probe.py            (runs all variants)
        python tools/h2d_probe.py VARIANT    (one variant, used by the parent)"""

@@ -1,5 +1,5 @@
 """Two eager learn steps of the IMPALA ResNet (+LSTM) at T=80, B=8 (one GPU's shard of BASELINE configs[3]) - the target of
-the ncu captures under profiles/ (ncu -k regex:sw_conv ... python tools/resnet_step.py)."""
+ncu captures (ncu -k regex:sw_conv ... python tools/resnet_step.py)."""
 import sys
 import torch
 sys.path.insert(0, ".")

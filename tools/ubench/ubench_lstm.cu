@@ -1,8 +1,8 @@
-// Micro-benchmarks behind the LSTM recurrence design (DESIGN.md "LSTM recurrence"): measured on the B200 box, not guessed.
+// Micro-benchmarks behind the LSTM recurrence design (DESIGN.md "LSTM recurrence").
 //   1. mma.sync.m16n8k16 bf16 issue rate per SM (8 / 16 warps, 12 independent accumulators)
 //   2. all-gather cost: 130 CTAs each pulling the same 137 KB from L2 into shared memory (cp.async 16 B vs TMA 2D boxes)
 //   3. store -> remote-poll visibility latency through L2 (one CTA stores, another spins on ld.relaxed.gpu)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o ubench_lstm ubench_lstm.cu -lcuda
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o ubench_lstm ubench_lstm.cu -lcuda
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""torchbeast_b200: B200-native (sm_100a) IMPALA learner hot path behind torchbeast's API.
+"""torchbeast_b200: H100-native (sm_90a) IMPALA learner hot path behind torchbeast's API.
 
 Python surface mirrors the reference (facebookresearch/torchbeast):
     torchbeast_b200.core.vtrace        <- torchbeast/core/vtrace.py

@@ -83,7 +83,7 @@ def lib():
                 if not os.path.exists(LIB_PATH):
                     raise ImportError(
                         "torchbeast_b200: %s not found. Build it with `python -c 'import __graft_entry__ as g; "
-                        "g.build()'` (nvcc, sm_100a). There is no CPU/PyTorch fallback." % LIB_PATH)
+                        "g.build()'` (nvcc, sm_90a). There is no CPU/PyTorch fallback." % LIB_PATH)
                 h = ctypes.CDLL(LIB_PATH)
                 for name, (argtypes, restype) in _SIGNATURES.items():
                     fn = getattr(h, name)  # AttributeError if the .so lacks a declared symbol

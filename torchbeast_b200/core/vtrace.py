@@ -2,7 +2,7 @@
 
 Same names, signatures, return types and error text as the reference
 (/root/reference/torchbeast/core/vtrace.py:36-139); every function launches hand-written
-sm_100a kernels through the C-ABI (torchbeast_b200/csrc/vtrace.cu).  CUDA tensors only.
+sm_90a kernels through the C-ABI (torchbeast_b200/csrc/vtrace.cu).  CUDA tensors only.
 """
 import collections
 

@@ -1,11 +1,11 @@
-// AtariNet forward / backward for the IMPALA learner (sm_100a), behind the C ABI.
+// AtariNet forward / backward for the IMPALA learner (sm_90a), behind the C ABI.
 //
 // Replaces /root/reference/torchbeast/monobeast.py:582-632 (AtariNet.forward) and the autograd
 // graph torch builds behind it:   u8 frame -> /255 -> conv 8x8/4 -> conv 4x4/2 -> conv 3x3/1 ->
 // fc 3136->512 -> cat[x, clip(reward), onehot(last_action)] -> [2-layer LSTM] -> policy/baseline.
 //
 // Structure: every dense contraction (3 convs as patch-matrix GEMMs, fc, heads, LSTM projections;
-// forward, dgrad and wgrad) goes through ONE GEMM interface (gemm_simt.cuh today, the tcgen05
+// forward, dgrad and wgrad) goes through ONE GEMM interface (gemm_simt.cuh today, the wgmma
 // backend next); activations live in NHWC so that a GEMM's [rows, channels] output is the next
 // layer's input with no transpose; weights stay in the reference's state_dict layout in one flat
 // buffer and are re-packed per step into GEMM order (tiny); weight gradients are un-packed into
@@ -166,7 +166,7 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
 static int pick_splits(int64_t M, int64_t N, int64_t K) {
   const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
   const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMsB200 + tiles - 1) / tiles;
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
   const int64_t ktiles = (K + kGemmBK - 1) / kGemmBK;
   if (s > ktiles / 4) s = ktiles / 4;
   if (s * M * N > kSplitKScratchFloats) s = kSplitKScratchFloats / (M * N);
@@ -195,7 +195,7 @@ static int atarinet_forward(const uint8_t* frame, const float* reward, const flo
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
   if (precision) {
-    // ---- tensor-core trunk: tcgen05 GEMMs, bf16 (precision 1) or split-bf16 hi/lo (precision 2) activations, fp32 accumulation
+    // ---- tensor-core trunk: wgmma GEMMs, bf16 (precision 1) or split-bf16 hi/lo (precision 2) activations, fp32 accumulation
     const bool split = precision == 2;
     TB_REQUIRE(!split || (implicit_plan().conv1 && implicit_plan().conv2 && implicit_plan().conv3),
                "atarinet_forward: the split-bf16 backend needs the implicit-GEMM convolutions (TB_CONV*_IMPLICIT=0 set?)");
@@ -303,11 +303,11 @@ static int tc_splits(int64_t M, int64_t N, int64_t K) {
   const int64_t bn = N <= 64 ? 64 : 128;
   const int64_t tiles = ((M + 127) / 128) * ((N + bn - 1) / bn);
   const int64_t kb = (K + 63) / 64;
-  int64_t s = (2 * kNumSMsB200 + tiles - 1) / tiles;
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
   if (s > kb / 4) s = kb / 4;
   const int64_t Np = (N + 31) & ~int64_t(31);  // partial rows are padded to 32 floats (gemm_tc.cu)
   if (s * M * Np > kSplitKScratchFloats) s = kSplitKScratchFloats / (M * Np);
-  if (s > 148) s = 148;
+  if (s > kNumSMs) s = kNumSMs;
   if (s < 1) s = 1;
   return int(s);
 }

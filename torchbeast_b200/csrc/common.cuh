@@ -1,4 +1,4 @@
-// Shared host/device helpers for the torchbeast_b200 C-ABI library (sm_100a only).
+// Shared host/device helpers for the torchbeast_b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,7 +30,7 @@ struct ProfScope {
   } while (0)
 
 constexpr int kWarp = 32;
-constexpr int kNumSMsB200 = 148;
+constexpr int kNumSMs = 132;  // H100 SXM
 // workspace layout: [0] uint32 ticket counter (self-resetting), then kMaxPartialCtas x 4 doubles
 constexpr int kMaxPartialCtas = 4096;
 constexpr size_t kWorkspaceBytes = 64 + size_t(kMaxPartialCtas) * 4 * sizeof(double);
@@ -91,7 +91,7 @@ __device__ __forceinline__ bool grid_sum3(double s0, double s1, double s2, void*
   if (is_last && nblocks > 1) {
     // the last CTA folds the partials with ALL its threads: thread t takes CTAs t, t + nthreads, ... and the
     // per-thread sums are combined warp by warp - a fixed pattern, independent of which CTA arrived last
-    // (one thread walking 592 partials with dependent fp64 adds took 40 us in grad_sumsq_kernel)
+    // (one thread walking hundreds of partials with dependent fp64 adds was slow in grad_sumsq_kernel)
     __threadfence();
     double x = 0, y = 0, z = 0;
     for (unsigned i = tid; i < nblocks; i += nthreads) {

@@ -1,22 +1,21 @@
-// Shifted-window implicit-GEMM 3x3 convolutions (stride 1, pad 1) of the IMPALA ResNet trunk on tcgen05
-// (reference: /root/reference/torchbeast/polybeast_learner.py:141-199, nn.Conv2d(kernel_size=3, stride=1, padding=1)).
+// Shifted-window implicit-GEMM 3x3 convolutions (stride 1, pad 1) of the IMPALA ResNet trunk on wgmma
+// (reference: torchbeast/polybeast_learner.py:141-199, nn.Conv2d(kernel_size=3, stride=1, padding=1)).
 //
 // These convolutions have 16 / 32 channels: as GEMMs they are [pixels, 9*C] x [9*C, 16..32] - the A stream is everything.
 // A patch matrix (or a per-tap TMA box) moves every input element 9-12 times through the TMA -> shared-memory path, and
-// that path (~45-70 B/clk per SM measured), not HBM and not the tensor pipe, bounded the patch-matrix kernels (3.4-3.7 TB/s
-// aggregate).  Here the image is stored as zero-padded CHANNEL-CHUNK PLANES [frame][C/8][(H+2)*(W+2)][8] (split-bf16: hi
+// that path, not HBM and not the tensor pipe, bounds patch-matrix kernels.  Here the image is stored as zero-padded CHANNEL-CHUNK PLANES [frame][C/8][(H+2)*(W+2)][8] (split-bf16: hi
 // and lo planes).  A tile = 128 consecutive flattened padded pixels of one frame; its input window (128 + 2*(W+2) + 2
 // pixels of every chunk plane) is ONE contiguous 1-D bulk copy per plane.  In shared memory a chunk plane is a K-major
-// no-swizzle UMMA operand as it stands - row = pixel, 16 bytes = 8 channels, rows 16 bytes apart (canonical layout
+// no-swizzle wgmma operand as it stands - row = pixel, 16 bytes = 8 channels, rows 16 bytes apart (canonical layout
 // ((8,n),2):((1,SBO),LBO) in 16-byte units with SBO = 8 and LBO = the chunk-plane pitch) - and the operand of tap (kh, kw)
 // is the same rows shifted by (kh*(W+2) + kw)*16 bytes: 9 descriptors over one copy of the data.  Output rows that fall on
 // padding columns / rows are computed and dropped by the epilogue (2/(W+2) of the tile).
 //
-// Split-bf16 (see gemm_tc.cuh): x = hi + lo per operand, products x_hi.w_hi + x_hi.w_lo + x_lo.w_hi in fp32.  On tcgen05 the
-// weight rows are stored [w_hi | w_lo] so that x_hi.[w_hi | w_lo] is ONE MMA with N = 2*NO (an SS-mode MMA costs >= 32 cycles
-// for its A operand whatever N is); x_lo.w_hi accumulates onto the first half and the epilogue adds the halves.
+// Split-bf16 (see gemm_tc.cuh): x = hi + lo per operand, products x_hi.w_hi + x_hi.w_lo + x_lo.w_hi in fp32.  The
+// weight rows are stored [w_hi | w_lo] so that x_hi.[w_hi | w_lo] is ONE MMA with N = 2*NO (the A operand is read from
+// shared memory once for both products); x_lo.w_hi accumulates onto the first half and the epilogue adds the halves.
 // The epilogue can also write the NEXT conv's padded image (and per-tile column sums = its bias gradient in the backward
-// pass), so most fp32 -> image passes do not exist.  Weight gradients (M = 16..32 output channels: a shape the 128-row tcgen05
+// pass), so most fp32 -> image passes do not exist.  Weight gradients (M = 16..32 output channels: a shape the 64-row wgmma
 // atom cannot fill) run on mma.sync.m16n8k16 from the same planar tiles (sw_conv_wgrad_kernel).
 #include "conv3x3_sw.cuh"
 
@@ -39,7 +38,7 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 // K-major, no swizzle: rows 16 B apart inside an 8-row core matrix, 8-row groups `sbo` bytes apart, the second 8-element
 // k-chunk `lbo` bytes away
 __device__ __forceinline__ uint64_t desc_k_noswz(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(lbo >> 4) << 16) | (uint64_t(sbo >> 4) << 32) | (uint64_t(1) << 46);
+  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(lbo >> 4) << 16) | (uint64_t(sbo >> 4) << 32);  // layout 0: no swizzle
 }
 struct SwGeom {
   int H, W, Wp, Hp;
@@ -70,50 +69,39 @@ struct SwFwdArgs {
   int Nf; SwGeom g;
 };
 
-// persistent: CTA walks (frame, tile) work items; warp 0 = bulk-copy producer, warp 1 = MMA issuer, warps 2..9 = two epilogue
-// groups of four warps (one per TMEM lane quarter), group g owning accumulator buffer g = the CTA's even / odd tiles: with the
-// image and column-sum outputs the epilogue of a tile (global loads of mask / residual, ~10 16-byte stores per row) takes
-// longer than its 18 MMAs, and one group made the kernels epilogue-bound
-constexpr int kSwThreads = 64 + 8 * 32;
+// persistent: CTA walks (frame, tile) work items; warp 8 = bulk-copy producer, warps 0..7 = two consumer warpgroups, group g
+// owning the CTA's even / odd tiles: each issues the wgmma of its tile and runs its epilogue, so one group's epilogue (global
+// loads of mask / residual, ~10 16-byte stores per row) overlaps the other group's MMAs.  The accumulator fragments go
+// through a per-group shared-memory staging tile so that each thread of the group owns one row in the epilogue.
+constexpr int kSwThreads = 9 * 32;
 template <int CK, int NO>
 __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a) {
   constexpr int CH = CK / 8;                   // chunk planes per frame
   constexpr int KP = CK / 16;                  // k16 steps per tap
   constexpr uint32_t W_PLANE = 9u * CK * NO * 2u;   // bytes of one weight plane (the image interleaves hi and lo rows)
+  constexpr int LDS = NO + 4;                  // staging row pitch in floats
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 127u) & ~127u;
   const uint32_t chb = uint32_t(a.g.pin) * 16u;     // bytes of one chunk plane window
   const uint32_t stage_bytes = 2u * CH * chb;       // [plane hi / lo][chunk][pixel][16 B]
   const uint32_t sW = base;                         // [tap][kp][j][hi rows | lo rows][16 B]
   const uint32_t sX = sW + 2u * W_PLANE;
-  const uint32_t bars = sX + kSwStages * stage_bytes;  // full[kSt], empty[kSt], tmem_full[2], tmem_empty[2], wbar
+  const uint32_t bars = sX + kSwStages * stage_bytes;  // full[kSt], empty[kSt], wbar, then the two staging tiles
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kSwStages + s); };
-  auto tmem_full = [&](int b) { return bars + 8u * (2 * kSwStages + b); };
-  auto tmem_empty = [&](int b) { return bars + 8u * (2 * kSwStages + 2 + b); };
-  const uint32_t wbar = bars + 8u * (2 * kSwStages + 4);
-  const uint32_t tmem_slot = wbar + 8u;
-  constexpr uint32_t TMEM_COLS = 128;  // two accumulator buffers of 2*NO <= 64 columns
+  const uint32_t wbar = bars + 8u * (2 * kSwStages);
   __shared__ float csum_s[8][32][NO + 1];   // column-sum staging of the eight epilogue warps
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_work = a.Nf * a.g.tpf;
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kSwStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tmem_full(b), 1); mbar_init(tmem_empty(b), 4); }
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < kSwStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
     mbar_init(wbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(wbar, 2u * W_PLANE);
       bulk_g2s(sW, a.wk, 2u * W_PLANE, wbar);
@@ -133,46 +121,14 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a)
         if (++stage == kSwStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // An SS-mode MMA costs >= 32 cycles of the tensor pipe for its 128 x 16 A operand whatever N is (ncu: pipe_tc 87 % busy
-      // with three N = 16 MMAs per product), so the split product is issued as TWO MMAs: x_hi . [w_hi | w_lo] (N = 2*NO, the lo
-      // half lands in columns [NO, 2*NO)) and x_lo . w_hi accumulated onto columns [0, NO); the epilogue adds the halves.
-      constexpr uint32_t idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t((2 * NO) >> 3) << 17) | (uint32_t(kTile >> 4) << 24);
-      constexpr uint32_t idesc1 = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(NO >> 3) << 17) | (uint32_t(kTile >> 4) << 24);
-      mbar_wait(wbar, 0);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++it) {
-        const int ab = it & 1;
-        mbar_wait(tmem_empty(ab), ((it >> 1) & 1) ^ 1);
-        mbar_wait(full(stage), phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + uint32_t(ab * 64);
-        const uint32_t st = sX + stage * stage_bytes;
-#pragma unroll 1
-        for (int tap = 0; tap < 9; ++tap) {
-          const uint32_t shift = uint32_t((tap / 3) * a.g.Wp + (tap % 3)) * 16u;
-#pragma unroll
-          for (int kp = 0; kp < KP; ++kp) {
-            const uint32_t xa = st + uint32_t(2 * kp) * chb + shift;
-            const uint32_t wa = sW + uint32_t((tap * KP + kp) * 2 * 2 * NO) * 16u;
-            const uint64_t dah = desc_k_noswz(xa, chb, 128u), dal = desc_k_noswz(xa + CH * chb, chb, 128u);
-            const uint64_t dbw = desc_k_noswz(wa, 2u * NO * 16u, 128u);   // rows [0, NO) = hi, [NO, 2*NO) = lo
-            umma_bf16(tacc, dah, dbw, idesc2, (tap | kp) != 0 ? 1u : 0u);
-            umma_bf16(tacc, dal, dbw, idesc1, 1u);
-          }
-        }
-        umma_commit(empty(stage));
-        umma_commit(tmem_full(ab));
-        if (++stage == kSwStages) { stage = 0; phase ^= 1; }
-      }
-    }
   } else {
-    const int quarter = warp & 3, ew = warp - 2, grp = ew >> 2;
+    const int quarter = warp & 3, ew = warp, grp = ew >> 2;
     const int rl = quarter * 32 + lane;
+    float* stg = reinterpret_cast<float*>(smem_raw + (wbar + 16u - smem_addr(smem_raw))) + grp * kTile * LDS;
+    mbar_wait(wbar, 0);
     for (int w = blockIdx.x + grp * gridDim.x, it = grp; w < total_work; w += 2 * gridDim.x, it += 2) {
-      const int ab = it & 1;
+      const int stage = it % kSwStages;
+      const uint32_t phase = uint32_t(it / kSwStages) & 1u;
       const int n = w / a.g.tpf, p = (w - n * a.g.tpf) * kTile + rl;
       const int y = p / a.g.Wp, x = p - y * a.g.Wp;
       const bool valid = x < a.g.W && y < a.g.H;
@@ -181,21 +137,58 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a)
         if (a.mask) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.mask + r * NO));
         if (a.addend) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.addend + r * NO));
       }
-      mbar_wait(tmem_full(ab), (it >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t v[32], v2[32];
-      tmem_ld32(tmem_base + (uint32_t(quarter * 32) << 16) + uint32_t(ab * 64), v);
-      if (NO == 32) tmem_ld32(tmem_base + (uint32_t(quarter * 32) << 16) + uint32_t(ab * 64 + 32), v2);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      // The split product as TWO wgmmas per k-step: x_hi . [w_hi | w_lo] (N = 2*NO, the lo half lands in columns [NO, 2*NO))
+      // and x_lo . w_hi accumulated onto columns [0, NO) - the first NO/2 registers of the 2*NO-wide accumulator.
+      float acc[2][NO];  // rows [0, 64) and [64, 128) of the tile
+      mbar_wait(full(stage), phase);
+      wgmma_fence();
+      const uint32_t st = sX + stage * stage_bytes;
+      // fully unrolled: the first product's scale-d flag is then a constant - with a runtime flag in a rolled loop ptxas
+      // serialises the whole wgmma chain
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        const uint32_t shift = uint32_t((tap / 3) * a.g.Wp + (tap % 3)) * 16u;
+#pragma unroll
+        for (int kp = 0; kp < KP; ++kp) {
+          const uint32_t wa = sW + uint32_t((tap * KP + kp) * 2 * 2 * NO) * 16u;
+          const uint64_t dbw = desc_k_noswz(wa, 2u * NO * 16u, 128u);   // rows [0, NO) = hi, [NO, 2*NO) = lo
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {  // 64 pixel rows = 1024 B further
+            const uint32_t xa = st + uint32_t(2 * kp) * chb + shift + h * 1024u;
+            const uint64_t dah = desc_k_noswz(xa, chb, 128u), dal = desc_k_noswz(xa + CH * chb, chb, 128u);
+            wgmma_bf16<2 * NO>(acc[h], dah, dbw, (tap | kp) != 0);
+            wgmma_bf16<NO>(acc[h], dal, dbw, 1);
+          }
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty(ab));   // the values are in registers: the buffer can be refilled
+      if (lane == 0) mbar_arrive(empty(stage));   // the values are in registers: the stage can be refilled
+      named_sync(1 + grp, 128);  // this group's previous epilogue has read the staging tile
+      {
+        // lo.hi + hi.hi (columns [0, NO)) + hi.lo (columns [NO, 2*NO)): registers i and i + NO/2
+        const int fr = quarter * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < NO / 8; ++j) {
+            float* sp = stg + (h * 64 + fr) * LDS + 8 * j + fc;
+            *reinterpret_cast<float2*>(sp) = make_float2(acc[h][4 * j] + acc[h][4 * j + NO / 2], acc[h][4 * j + 1] + acc[h][4 * j + 1 + NO / 2]);
+            *reinterpret_cast<float2*>(sp + 8 * LDS) =
+                make_float2(acc[h][4 * j + 2] + acc[h][4 * j + 2 + NO / 2], acc[h][4 * j + 3] + acc[h][4 * j + 3 + NO / 2]);
+          }
+      }
+      named_sync(1 + grp, 128);
       float o[NO];
 #pragma unroll
       for (int j = 0; j < NO; ++j) o[j] = 0.f;
       if (valid) {
 #pragma unroll
-        for (int j = 0; j < NO; ++j)   // lo.hi + hi.hi (columns [0, NO)) + hi.lo (columns [NO, 2*NO))
-          o[j] = (__uint_as_float(v[j]) + __uint_as_float(NO == 32 ? v2[j] : v[(j + NO) & 31])) * a.scale;
+        for (int j = 0; j < NO; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(stg + rl * LDS + j);
+          o[j] = t.x * a.scale; o[j + 1] = t.y * a.scale; o[j + 2] = t.z * a.scale; o[j + 3] = t.w * a.scale;
+        }
         if (a.bias) {
 #pragma unroll
           for (int q = 0; q < NO / 4; ++q) {
@@ -282,16 +275,12 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a)
       }
     }
   }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 template <int CK, int NO>
 int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
-  const size_t smem = 128 + 2 * size_t(9) * CK * NO * 2 + size_t(kSwStages) * 2 * (CK / 8) * a.g.pin * 16 + 8 * (2 * kSwStages + 5) + 16;
+  const size_t smem = 128 + 2 * size_t(9) * CK * NO * 2 + size_t(kSwStages) * 2 * (CK / 8) * a.g.pin * 16 + 8 * (2 * kSwStages + 2) +
+                      2 * size_t(kTile) * (NO + 4) * sizeof(float) + 16;
   TB_REQUIRE(smem <= 227 * 1024, "sw_conv_fwd: shared memory");
   static size_t attr[64] = {0};
   int dev = 0;
@@ -304,7 +293,7 @@ int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
   int per_sm = int((224 * 1024) / (smem + sizeof(float) * 8 * 32 * (NO + 1) + 1024));   // + the static column-sum staging
   if (per_sm > 4) per_sm = 4;
   if (per_sm < 1) per_sm = 1;
-  int64_t grid = int64_t(kNumSMsB200) * per_sm;
+  int64_t grid = int64_t(kNumSMs) * per_sm;
   const int64_t total = int64_t(a.Nf) * a.g.tpf;
   if (grid > total) grid = total;
   sw_conv_fwd_kernel<CK, NO><<<(unsigned)grid, kSwThreads, smem, stream>>>(a);
@@ -313,10 +302,8 @@ int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
 
 // ---- weight gradient ------------------------------------------------------------------------------------------
 // dW[o, tap, c] = sum over pixels p of dY[p, o] * x[p + shift(tap), c]: M = O and N = C are 16..32 and the reduction runs
-// over pixels.  tcgen05 cannot run this shape: its atom is 128 rows and an SS-mode MMA costs >= 32 cycles whatever M and N
-// are (measured here: 35 cycles per M=128/64 x N=16 x K=16 MMA; 216 of them per tile = 7.7 k cycles, 267 us per conv).  The
-// warp-level mma.sync.m16n8k16 atom fits exactly (M = 16 channels of dY, N = 8 channels of x, K = 16 pixels; 2 cycles per
-// MMA per SM measured): A = dY^T and B = the x window both come straight out of the planar tiles with ldmatrix.trans (a
+// over pixels.  A wgmma atom is 64 rows, so three quarters of every MMA would be padding.  The
+// warp-level mma.sync.m16n8k16 atom fits exactly (M = 16 channels of dY, N = 8 channels of x, K = 16 pixels): A = dY^T and B = the x window both come straight out of the planar tiles with ldmatrix.trans (a
 // row of either tile is one pixel's 8 channels = 16 bytes, 8 consecutive pixels are one 8x8 matrix), the tap shift is a
 // 16-byte multiple in the row address, and the products are split-bf16 (lo.hi + hi.lo + hi.hi).
 // CTA = 9 MMA warps = 3 tap groups (one kernel row each) x 3 pixel groups (k16 steps kg, kg+3, kg+6 of a tile) + 1 producer
@@ -479,7 +466,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) sw_conv_wgrad_kernel(SwWgradArg
 }
 
 // dW[o, c, kh, kw] = scale * sum over CTAs of partial[cta][o][(kh*3 + kw)*C + c].  Block = 32 consecutive partial columns x 8
-// CTA groups (coalesced 128-byte reads; a 148-iteration per-thread loop with strided reads took 24 us per conv - more than
+// CTA groups (coalesced 128-byte reads; a per-thread loop over every CTA's partial with strided reads took longer than
 // a third of the weight-gradient kernels themselves); the 8 group sums are folded in a fixed order (deterministic).
 __global__ void __launch_bounds__(256) sw_wgrad_reduce_kernel(const float* __restrict__ partial, float* __restrict__ dW, int ctas,
                                                               int O, int C, int c_real, float scale) {
@@ -521,7 +508,7 @@ int launch_sw_wgrad(const SwWgradArgs& a, int grid, cudaStream_t stream) {
 
 static inline unsigned sgrid(int64_t work, int threads) {
   int64_t blocks = (work + threads - 1) / threads;
-  const int64_t cap = int64_t(kNumSMsB200) * 16;
+  const int64_t cap = int64_t(kNumSMs) * 16;
   if (blocks > cap) blocks = cap;
   return (unsigned)(blocks < 1 ? 1 : blocks);
 }
@@ -872,7 +859,7 @@ int sw_conv_wgrad(const __nv_bfloat16* dyimg, int64_t dy_lo, const __nv_bfloat16
   ProfScope prof(tag, stream);
   SwWgradArgs a;
   a.dy = dyimg; a.dy_lo = dy_lo; a.x = ximg; a.x_lo = x_lo; a.partial = partial; a.Nf = int(Nf); a.g = sw_geom(H, W);
-  int64_t grid = kNumSMsB200;
+  int64_t grid = kNumSMs;
   const int64_t total = Nf * a.g.tpf;
   if (grid > total) grid = total;
   TB_REQUIRE(grid * O * 9 * C <= partial_floats, "sw_conv_wgrad: partial buffer too small");

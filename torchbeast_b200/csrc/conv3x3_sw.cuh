@@ -14,7 +14,7 @@ namespace tb {
 int64_t sw_image_elems(int64_t Nf, int H, int W, int C);
 // fp32 NHWC [Nf, H, W, C] (optionally through ReLU) -> padded planar hi / lo image
 int sw_pad_split(const float* x, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int H, int W, int C, int relu_in, cudaStream_t stream);
-// same, and also db[C] = column sums of x (bias gradient when x is dL/d(conv output)); scratch >= 148*8*C floats
+// same, and also db[C] = column sums of x (bias gradient when x is dL/d(conv output)); scratch >= kNumSMs*8*C floats
 int sw_pad_split_colsum(const float* x, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int H, int W, int C, float* db,
                         float* scratch, int64_t scratch_floats, cudaStream_t stream);
 

@@ -2,11 +2,11 @@
 //
 // AtariNet's conv1 (monobeast.py:560, 8x8 stride 4 over [N,4,84,84] uint8) as a patch-matrix GEMM reads a
 // [N*400, 256] bf16 matrix that is 7x larger than the frames it was gathered from; materialising it costs
-// more HBM time than the product itself (profiles/launches_r1_summary.txt: im2col 229 us + GEMM 110 us +
-// wgrad 112 us, all bound by the 531 MB patch matrix).  Here the frames are converted ONCE to bf16 (exact:
+// more HBM time than the product itself (im2col, GEMM and wgrad are all bound by the 531 MB patch matrix).  Here the
+// frames are converted ONCE to bf16 (exact:
 // pixel values are integers <= 2^8; the 1/255 stays in the epilogue; 146 MB instead of 531 MB) and producer
 // warps gather each patch row straight from that image with per-thread async copies (cp.async 8 B, L1/L2
-// resident: every pixel is reused by 4 patches) into shared memory in the SWIZZLE_128B layout the UMMA
+// resident: every pixel is reused by 4 patches) into shared memory in the SWIZZLE_128B layout the wgmma
 // descriptors expect, so the patch matrix never exists in HBM.  (A first version converted u8 -> bf16 inside
 // the gather: ncu showed it issue-bound on the 4x redundant conversion, 23 instructions per 16-byte chunk.)
 //
@@ -30,13 +30,13 @@ using namespace tcd;
 
 namespace {
 
-constexpr int kProducers = 256;                 // 8 gather warps
-constexpr int kConvThreads = 192 + kProducers;  // warp 0: TMA, 1: MMA issue, 2-5: epilogue, 6-13: gather
+constexpr int kProducers = 256;                         // 8 gather warps
+constexpr int kGatherBase = 9 * 32;                     // warps 0-7: two wgmma + epilogue warpgroups, 8: TMA, 9-16: gather
+constexpr int kConvThreads = kGatherBase + kProducers;
 constexpr int kC = 4;                           // input channels = k-blocks of 64 (= KH*KW)
 constexpr int kO = 32;                          // output channels
-constexpr int kStagesF = 3;   // forward: a stage is a WHOLE 128-patch tile (4 k-blocks, 64 KB): with one k-block per stage
-                              // the single MMA-issuing thread paid an mbarrier wait + commit per 64 cycles of tensor work
-                              // and its latency, not the gather, bounded the kernel (63 us with the copies disabled)
+constexpr int kStagesF = 3;   // forward: a stage is a WHOLE 128-patch tile (4 k-blocks, 64 KB), so the consumers pay one
+                              // mbarrier wait and one wgmma wait per tile instead of one per k-block
 constexpr int kStagesW = 5;   // wgrad: 5 x (8 KB dY + 32 KB patches)
 
 struct ConvGeom {
@@ -94,109 +94,80 @@ __global__ void __launch_bounds__(kConvThreads, 1)
 conv_u8_fwd_implicit_kernel(const __nv_bfloat16* __restrict__ frame, const __grid_constant__ CUtensorMap tmB,
                             const __grid_constant__ CUtensorMap tmBl, TcEpilogue ep, ConvGeom g, int tiles_m) {
   constexpr uint32_t B_BYTES = kO * kBlockK * 2;  // 4 KB per k-block
-  constexpr uint32_t TMEM_COLS = 64;              // two 32-column accumulator buffers
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t kTileBytes = kC * kABytes;  // 64 KB
   const uint32_t sA = base, sB = base + kStagesF * kTileBytes;
-  const uint32_t bars = sB + (SPLIT ? 2 : 1) * kC * B_BYTES;  // full[kStagesF], empty[kStagesF], tmem_full[2], tmem_empty[2], wfull
-  const uint32_t tmem_slot = bars + 8 * (2 * kStagesF + 5);
+  const uint32_t bars = sB + (SPLIT ? 2 : 1) * kC * B_BYTES;  // full[kStagesF], empty[kStagesF], wfull
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kStagesF + s); };
-  auto tmem_full = [&](int b) { return bars + 8u * (2 * kStagesF + b); };
-  auto tmem_empty = [&](int b) { return bars + 8u * (2 * kStagesF + 2 + b); };
-  const uint32_t wfull = bars + 8u * (2 * kStagesF + 4);
+  const uint32_t wfull = bars + 8u * (2 * kStagesF);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStagesF; ++s) { mbar_init(full(s), kProducers / 32); mbar_init(empty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tmem_full(b), 1); mbar_init(tmem_empty(b), 4); }
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < kStagesF; ++s) { mbar_init(full(s), kProducers / 32); mbar_init(empty(s), 8); }
     mbar_init(wfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {  // the whole weight matrix [32, 256] stays resident: one box per k-block
       mbar_expect_tx(wfull, (SPLIT ? 2 : 1) * kC * B_BYTES);
       for (int c = 0; c < kC; ++c) tma_load_2d(sB + c * B_BYTES, &tmB, wfull, c * kBlockK, 0);
       if constexpr (SPLIT)
         for (int c = 0; c < kC; ++c) tma_load_2d(sB + (kC + c) * B_BYTES, &tmBl, wfull, c * kBlockK, 0);
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(kO >> 3) << 17) | (uint32_t(kBlockM >> 4) << 24);
-      mbar_wait(wfull, 0);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x, ++it) {
-        const int ab = it & 1;
-        mbar_wait(tmem_empty(ab), ((it >> 1) & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + uint32_t(ab * kO);
-        mbar_wait(full(stage), phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  } else if (warp < 8) {
+    // consumer warpgroup h: the 64-row half h of the tile, an m64n32 accumulator; the epilogue works on the fragments
+    // (rows fr, fr + 8, column pairs 8j + fc)
+    const int h = warp >> 2;
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+    float bias_r[8];
 #pragma unroll
-        for (int c = 0; c < kC; ++c)
+    for (int j = 0; j < 4; ++j) { bias_r[2 * j] = __ldg(ep.bias + 8 * j + fc); bias_r[2 * j + 1] = __ldg(ep.bias + 8 * j + fc + 1); }
+    mbar_wait(wfull, 0);
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x) {
+      float acc[kO / 2];
+      mbar_wait(full(stage), phase);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            const uint64_t da = make_smem_desc(sA + stage * kTileBytes + c * kABytes + k * 32);
-            if constexpr (SPLIT) {
-              umma_bf16(tacc, da, make_smem_desc(sB + (kC + c) * B_BYTES + k * 32), idesc, (c | k) != 0 ? 1u : 0u);
-              umma_bf16(tacc, da, make_smem_desc(sB + c * B_BYTES + k * 32), idesc, 1u);
-            } else {
-              umma_bf16(tacc, da, make_smem_desc(sB + c * B_BYTES + k * 32), idesc, (c | k) != 0 ? 1u : 0u);
-            }
+      for (int c = 0; c < kC; ++c)
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          const uint64_t da = make_smem_desc(sA + stage * kTileBytes + c * kABytes + h * 8192 + k * 32);
+          if constexpr (SPLIT) {
+            wgmma_bf16<kO>(acc, da, make_smem_desc(sB + (kC + c) * B_BYTES + k * 32), (c | k) != 0);
+            wgmma_bf16<kO>(acc, da, make_smem_desc(sB + c * B_BYTES + k * 32), 1);
+          } else {
+            wgmma_bf16<kO>(acc, da, make_smem_desc(sB + c * B_BYTES + k * 32), (c | k) != 0);
           }
-        umma_commit(empty(stage));
-        umma_commit(tmem_full(ab));
-        if (++stage == kStagesF) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp < 6) {
-    const int quarter = warp & 3;
-    float bias_r[32];
-#pragma unroll
-    for (int j = 0; j < 32; ++j) bias_r[j] = __ldg(ep.bias + j);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < tiles_m; tile += gridDim.x, ++it) {
-      const int ab = it & 1;
-      mbar_wait(tmem_full(ab), (it >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int64_t r = int64_t(tile) * kBlockM + quarter * 32 + lane;
-      uint32_t v[32];
-      tmem_ld32(tmem_base + (uint32_t(quarter * 32) << 16) + uint32_t(ab * kO), v);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty(ab));  // values are in registers: free the accumulator early
-      if (r < g.M) {
-        uint32_t pk[16], pl[16];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float x0 = __uint_as_float(v[j]) * ep.scale + bias_r[j];
-          float x1 = __uint_as_float(v[j + 1]) * ep.scale + bias_r[j + 1];
-          if (ep.relu) { x0 = fmaxf(x0, 0.0f); x1 = fmaxf(x1, 0.0f); }
-          split_bf16x2(x0, x1, pk[j >> 1], pl[j >> 1]);
         }
-        uint4* c = reinterpret_cast<uint4*>(ep.C16 + r * ep.ldc16);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(stage));  // values are in registers: free the stage early
+      if (++stage == kStagesF) { stage = 0; phase ^= 1; }
 #pragma unroll
-        for (int j = 0; j < 4; ++j) c[j] = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-        if (SPLIT && ep.c16_lo) {
-          uint4* cl = reinterpret_cast<uint4*>(ep.C16 + ep.c16_lo + r * ep.ldc16);
+      for (int e = 0; e < 2; ++e) {
+        const int64_t r = int64_t(tile) * kBlockM + h * 64 + fr + 8 * e;
+        if (r >= g.M) continue;
+        __nv_bfloat16* c = ep.C16 + r * ep.ldc16;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) cl[j] = make_uint4(pl[4 * j], pl[4 * j + 1], pl[4 * j + 2], pl[4 * j + 3]);
+        for (int j = 0; j < 4; ++j) {
+          float x0 = acc[4 * j + 2 * e] * ep.scale + bias_r[2 * j];
+          float x1 = acc[4 * j + 2 * e + 1] * ep.scale + bias_r[2 * j + 1];
+          if (ep.relu) { x0 = fmaxf(x0, 0.0f); x1 = fmaxf(x1, 0.0f); }
+          uint32_t hi, lo;
+          split_bf16x2(x0, x1, hi, lo);
+          *reinterpret_cast<uint32_t*>(c + 8 * j + fc) = hi;
+          if (SPLIT && ep.c16_lo) *reinterpret_cast<uint32_t*>(c + ep.c16_lo + 8 * j + fc) = lo;
         }
       }
     }
   } else {
-    const int p = threadIdx.x - 192;
+    const int p = threadIdx.x - kGatherBase;
     const int half = lane & 1;                       // which 8 bytes of every chunk
     const int row = (p >> 5) * 16 + (lane >> 1);     // 16 patch rows per gather warp
     const uint32_t row_off = uint32_t(row >> 3) * 1024u + uint32_t(row & 7) * 128u + 8u * half;
@@ -240,11 +211,6 @@ conv_u8_fwd_implicit_kernel(const __nv_bfloat16* __restrict__ frame, const __gri
       if (++sig == kStagesF) sig = 0;
     }
   }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
 }
 
 // ---- weight gradient -------------------------------------------------------------------------------
@@ -260,38 +226,26 @@ conv_u8_wgrad_implicit_kernel(const __nv_bfloat16* __restrict__ frame, const __g
                               int per) {
   constexpr int kStW = SPLIT ? kStagesW - 1 : kStagesW;  // 4 x 48 KB (split) / 5 x 40 KB
   constexpr uint32_t B_BYTES = kC * 8192;  // 32 KB
-  constexpr uint32_t TMEM_COLS = 256;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
-  constexpr uint32_t A_BOX = 8192;   // only the first 64-wide box of dY^T is loaded: accumulator rows >= 64 read
-                                     // whatever follows in shared memory and are never looked at
+  constexpr uint32_t A_BOX = 8192;   // one 64-wide box of dY^T: rows >= 32 of the m64 accumulator are zero fill
   constexpr uint32_t A_BYTES = (SPLIT ? 2u : 1u) * A_BOX;  // [hi][lo]
   const uint32_t sA = base, sB = base + kStW * A_BYTES;
-  const uint32_t bars = sB + kStW * B_BYTES;  // full[kStW], empty[kStW], tmem_full
-  const uint32_t tmem_slot = bars + 8 * (2 * kStW + 1);
+  const uint32_t bars = sB + kStW * B_BYTES;  // full[kStW], empty[kStW]
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kStW + s); };
-  const uint32_t tmem_full = bars + 8u * (2 * kStW);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kb0 = blockIdx.x * per;
   const int kb1 = (kb0 + per < total_kb) ? kb0 + per : total_kb;
   const int num_kb = kb1 > kb0 ? kb1 - kb0 : 0;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStW; ++s) { mbar_init(full(s), kProducers / 32 + 1); mbar_init(empty(s), 1); }
-    mbar_init(tmem_full, 1);
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < kStW; ++s) { mbar_init(full(s), kProducers / 32 + 1); mbar_init(empty(s), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int i = 0; i < num_kb; ++i) {
@@ -303,53 +257,46 @@ conv_u8_wgrad_implicit_kernel(const __nv_bfloat16* __restrict__ frame, const __g
         if (++stage == kStW) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && num_kb > 0) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | (uint32_t(256 >> 3) << 17) |
-                                 (uint32_t(kBlockM >> 4) << 24);
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full(stage), phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+  } else if (warp < 8) {
+    // D[o, k]: warpgroup q owns columns [128q, 128q + 128) (two of the four gathered 64-wide k groups, 8192 B apart) as
+    // an m64n128 accumulator, o < 32 real
+    constexpr int NQ = kC * 64 / 2;
+    const int q = warp >> 2;
+    float acc[NQ / 2];
 #pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) {
-          const uint64_t db = make_smem_desc_mn(sB + stage * B_BYTES + k * 2048);
-          if constexpr (SPLIT) {
-            umma_bf16(tmem_base, make_smem_desc_mn(sA + stage * A_BYTES + A_BOX + k * 2048), db, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_bf16(tmem_base, make_smem_desc_mn(sA + stage * A_BYTES + k * 2048), db, idesc, 1u);
-          } else {
-            umma_bf16(tmem_base, make_smem_desc_mn(sA + stage * A_BYTES + k * 2048), db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(empty(stage));
-        if (++stage == kStW) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
-  } else if (warp < 6) {
-    if ((warp & 3) == 0) {  // TMEM lanes 0..31 = the 32 real output channels
-      if (num_kb > 0) {
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      float* pz = partial + (int64_t(blockIdx.x) * kO + lane) * (kC * 64);
-#pragma unroll 1
-      for (int c0 = 0; c0 < kC * 64; c0 += 32) {
-        uint32_t v[32];
-        if (num_kb > 0) {
-          tmem_ld32(tmem_base + uint32_t(c0), v);
+    for (int j = 0; j < NQ / 2; ++j) acc[j] = 0.0f;
+    int stage = 0; uint32_t phase = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(full(stage), phase);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        const uint64_t db = make_smem_desc_mn(sB + stage * B_BYTES + q * 2 * 8192 + k * 2048);
+        if constexpr (SPLIT) {
+          wgmma_bf16<NQ, 1, 1>(acc, make_smem_desc_mn(sA + stage * A_BYTES + A_BOX + k * 2048), db, (kb | k) != 0);
+          wgmma_bf16<NQ, 1, 1>(acc, make_smem_desc_mn(sA + stage * A_BYTES + k * 2048), db, 1);
         } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
+          wgmma_bf16<NQ, 1, 1>(acc, make_smem_desc_mn(sA + stage * A_BYTES + k * 2048), db, (kb | k) != 0);
         }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(stage));
+      if (++stage == kStW) { stage = 0; phase ^= 1; }
+    }
+    if ((warp & 3) < 2) {  // fragment rows 0..31 = the 32 real output channels
+      const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(pz + c0 + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                 __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
+      for (int e = 0; e < 2; ++e) {
+        float* pz = partial + (int64_t(blockIdx.x) * kO + fr + 8 * e) * (kC * 64) + q * NQ;
+#pragma unroll
+        for (int j = 0; j < NQ / 8; ++j)
+          *reinterpret_cast<float2*>(pz + 8 * j + fc) = make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
       }
     }
   } else {
-    const int p = threadIdx.x - 192;
+    const int p = threadIdx.x - kGatherBase;
     const int half = lane & 1;
     const int c = p >> 6;                                      // two gather warps per channel
     const int row = ((p >> 5) & 1) * 32 + (lane >> 1);         // this thread's rows: row and row + 16
@@ -393,11 +340,6 @@ conv_u8_wgrad_implicit_kernel(const __nv_bfloat16* __restrict__ frame, const __g
       if (lane == 0) mbar_arrive(full(sig));
       if (++sig == kStW) sig = 0;
     }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -445,7 +387,7 @@ int frames_u8_to_bf16(const uint8_t* frame, void* frame_bf16, int64_t count, cud
   if (count == 0) return 0;
   ProfScope prof("frames_to_bf16", stream);
   int64_t blocks = ((count >> 4) + 255) / 256;
-  if (blocks > kNumSMsB200 * 16) blocks = kNumSMsB200 * 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   if (blocks < 1) blocks = 1;
   frames_u8_to_bf16_kernel<<<(unsigned)blocks, 256, 0, stream>>>(frame, static_cast<__nv_bfloat16*>(frame_bf16), count);
   return check_launch("frames_u8_to_bf16_kernel");
@@ -493,7 +435,7 @@ int conv_u8_fwd_implicit(const void* frame_bf16, const void* w_bf16, int64_t N, 
   }
   const int64_t tiles = (g.M + kBlockM - 1) / kBlockM;
   TB_REQUIRE(tiles < (int64_t(1) << 31), "conv_u8_fwd_implicit: too many tiles");
-  const int64_t grid = tiles < kNumSMsB200 ? tiles : kNumSMsB200;
+  const int64_t grid = tiles < kNumSMs ? tiles : kNumSMs;
   if (split) conv_u8_fwd_implicit_kernel<true><<<(unsigned)grid, kConvThreads, smem, stream>>>(frame, mb, mbl, ep, g, int(tiles));
   else conv_u8_fwd_implicit_kernel<false><<<(unsigned)grid, kConvThreads, smem, stream>>>(frame, mb, mbl, ep, g, int(tiles));
   return check_launch("conv_u8_fwd_implicit_kernel");
@@ -508,7 +450,7 @@ int conv_u8_wgrad_implicit(const void* dy_bf16, const void* frame_bf16, int64_t 
   const ConvGeom g = make_geom(N, H, W, S);
   const int64_t total_kb = (g.M + kBlockK - 1) / kBlockK;
   TB_REQUIRE(total_kb >= 1 && total_kb < (int64_t(1) << 31), "conv_u8_wgrad_implicit: bad size");
-  int64_t grid = total_kb < kNumSMsB200 ? total_kb : kNumSMsB200;
+  int64_t grid = total_kb < kNumSMs ? total_kb : kNumSMs;
   const int64_t per = (total_kb + grid - 1) / grid;
   grid = (total_kb + per - 1) / per;
   TB_REQUIRE(grid * kO * kC * 64 <= partial_floats, "conv_u8_wgrad_implicit: partial buffer too small");

@@ -4,7 +4,7 @@
 
 namespace tb {
 
-// true when the tcgen05 implicit-GEMM kernels cover this shape (8x8 kernel, 4 input / 32 output channels,
+// true when the wgmma implicit-GEMM kernels cover this shape (8x8 kernel, 4 input / 32 output channels,
 // W and stride multiples of 4) and TB_CONV1_IMPLICIT != 0
 bool conv_u8_implicit_applicable(int C, int H, int W, int KH, int KW, int S, int O);
 
@@ -18,7 +18,7 @@ int conv_u8_fwd_implicit(const void* frame_bf16, const void* w_bf16, int64_t N, 
                          cudaStream_t stream);
 
 // dW[32, 256] (fp32) = scale * dY^T . patches(frame); dy_bf16 [N*OH*OW, 32]; partial: split scratch
-// (>= 148*32*256 floats), reduced in fixed order
+// (>= kNumSMs*32*256 floats), reduced in fixed order
 int conv_u8_wgrad_implicit(const void* dy_bf16, const void* frame_bf16, int64_t N, int H, int W, int S, float* dW, float scale,
                            float* partial, int64_t partial_floats, const char* tag, cudaStream_t stream, int64_t dy_lo = 0);
 

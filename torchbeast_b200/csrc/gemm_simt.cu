@@ -27,8 +27,8 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, float* _
     const float* p = partial + m * ldp + n0;
     float v[4] = {0.f, 0.f, 0.f, 0.f};
     if (vec) {
-      // 16 loads in flight per thread (same summation order): with 148 splits and unroll 4 the conv1 reduce was 37 dependent
-      // L2 round trips = 26 us for a 4.8 MB read
+      // 16 loads in flight per thread (same summation order): with one split per SM and unroll 4 the conv1 reduce was 37 dependent
+      // L2 round trips for a 4.8 MB read
 #pragma unroll 16
       for (int z = 0; z < splits; ++z) {
         const float4 t = __ldg(reinterpret_cast<const float4*>(p + int64_t(z) * slice));
@@ -93,7 +93,7 @@ int gemm_simt(const AT* A, const BT* B, float* C, int64_t M, int64_t N, int64_t 
   if (via_scratch) {
     const int64_t total = M * N;
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
     rc = launch_splitk_reduce(splitk_scratch, C, M, N, ldc, splits, ep, N, stream);
   }
   return rc;

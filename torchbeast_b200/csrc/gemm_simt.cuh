@@ -1,4 +1,4 @@
-// fp32 SIMT GEMM for sm_100a: the exact-arithmetic ("fp32") backend of the network path.
+// fp32 SIMT GEMM for sm_90a: the exact-arithmetic ("fp32") backend of the network path.
 //
 //   C[M,N] (+)= sum_k A(m,k) * B(k,n)            fp32 accumulate, fp32 FFMA
 //   A(m,k) = TA ? A[k*lda + m] : A[m*lda + k]    (AT = float or uint8; uint8 is read as x/255.f,
@@ -11,7 +11,7 @@
 // `partial` ([z][M][N]) and splitk_reduce_kernel folds them in a fixed order (deterministic).
 //
 // This backend keeps the learner bit-comparable with the reference's fp32 CPU arithmetic
-// (parity tests); the tensor-core backend (tcgen05) replaces it for throughput.
+// (parity tests); the tensor-core backend (wgmma) replaces it for throughput.
 #pragma once
 #include "common.cuh"
 

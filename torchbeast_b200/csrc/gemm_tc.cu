@@ -1,15 +1,16 @@
-// bf16 tensor-core GEMM for sm_100a: tcgen05.mma + TMEM accumulators + TMA-staged operands.
+// bf16 tensor-core GEMM for sm_90a: wgmma.mma_async + register accumulators + TMA-staged operands.
 //
 //   C[M,N] = epilogue( sum_k A[m,k] * B[n,k] )     A [M,K], B [N,K] bf16, K contiguous ("K-major")
 //
-// One CTA computes a 128 x BLOCK_N tile.  Warp roles (192 threads):
-//   warp 0  TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 64 bf16 = 128 B) into a
-//                          4-stage shared-memory ring, mbarrier expect_tx / complete_tx
-//   warp 1  MMA issuer   : one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128,
-//                          N=BLOCK_N, K=16) x4 per 64-wide k-block, accumulating in TMEM;
-//                          tcgen05.commit frees the ring slot / signals the epilogue
-//   warps 2-5 epilogue   : tcgen05.ld 32x32b (each warp owns its 32 TMEM lanes = 32 output rows),
-//                          scale / bias / ReLU / ReLU-mask, fp32 and/or bf16 stores
+// One CTA computes a 128 x BLOCK_N tile.  Warp roles (160 threads):
+//   warp 4     TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 64 bf16 = 128 B) into a
+//                             shared-memory ring, mbarrier expect_tx / complete_tx
+//   warps 0-3  consumer     : one warpgroup issues wgmma.m64nNk16 (N = BLOCK_N) for both 64-row halves of
+//                             the tile, x4 per 64-wide k-block, keeping one wgmma group in flight; a ring slot
+//                             is handed back once the group that read it has completed.  The accumulator
+//                             fragments then go through a shared-memory staging tile so that each thread owns
+//                             one output row for the epilogue: scale / bias / ReLU / ReLU-mask, fp32 and/or
+//                             bf16 stores
 // M/N/K tails are handled by TMA out-of-bounds zero fill plus guarded stores.  Shared-memory
 // matrix descriptors: K-major, SWIZZLE_128B, SBO = 1024 B (8 rows x 128 B), advanced by 32 B per
 // K=16 step inside the swizzle atom (the CUTLASS/DeepGEMM canonical layout).
@@ -33,9 +34,8 @@ using namespace tcd;
 
 namespace {
 
-// Persistent: each CTA walks the work list (m tile, n tile, k split) with stride gridDim.x; the TMEM
-// accumulator is double-buffered so the epilogue of work item i overlaps the TMA/MMA main loop of item
-// i+1, and the per-CTA prologue (barrier init, TMEM alloc, descriptor fetch) is paid once.
+// Persistent: each CTA walks the work list (m tile, n tile, k split) with stride gridDim.x; the producer runs
+// ahead into the next work item while the consumers run the epilogue, and the per-CTA prologue is paid once.
 // EPI: 0 = store the accumulator as is; 1 = scale / bias / ReLU; 2 = + ReLU-mask / residual loads.
 // (compile-time so the common epilogues carry no predicated per-element loads - ncu showed the generic
 //  epilogue, not the MMA pipe, bounding the K=64 dgrad products)
@@ -74,16 +74,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                ImplicitConv ic = ImplicitConv()) {
   constexpr uint32_t B_BYTES = BLOCK_N * kBlockK * 2;
   constexpr uint32_t A_STAGE = (SPLIT ? 2u : 1u) * kABytes, B_STAGE = (SPLIT ? 2u : 1u) * B_BYTES;  // [hi][lo]
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N < 32 ? 32 : 2 * BLOCK_N;  // two accumulator buffers (power of two)
+  constexpr int LDS = BLOCK_N + 4;  // staging row pitch in floats (16-byte rows, conflict-free row reads)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t sA = base, sB = base + kStages * A_STAGE;
-  const uint32_t bars = sB + kStages * B_STAGE;  // full[kStages], empty[kStages], tmem_full[2], tmem_empty[2]
-  const uint32_t tmem_slot = bars + 8 * (2 * kStages + 4);
+  const uint32_t bars = sB + kStages * B_STAGE;  // full[kStages], empty[kStages], then the accumulator staging tile
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kStages + s); };
-  auto tmem_full = [&](int b) { return bars + 8u * (2 * kStages + b); };
-  auto tmem_empty = [&](int b) { return bars + 8u * (2 * kStages + 2 + b); };
+  // [128][LDS] fp32: the epilogue reads whole rows, the wgmma fragments are scattered over row pairs
+  float* stg = reinterpret_cast<float*>(smem_raw + (bars + 16u * kStages - smem_addr(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_kb = (K + kBlockK - 1) / kBlockK;
@@ -91,19 +90,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int tiles_mn = tiles_m * tiles_n;
   const int total_work = tiles_mn * splits;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(tmem_full(b), 1); mbar_init(tmem_empty(b), 4); }
+  if (warp == 4 && lane == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
   // work item -> tile coordinates (n fastest so that co-running CTAs share A tiles in L2)
   auto decode = [&](int w, int& m0, int& n0, int& kb0, int& num_kb, int& z) {
@@ -116,7 +107,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     num_kb = kb1 > kb0 ? kb1 - kb0 : 0;
   };
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
@@ -155,52 +146,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // instruction descriptor: D=f32, A=B=bf16, majorness bits, N>>3, M>>4
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(A_MN) << 15) | (uint32_t(B_MN) << 16) |
-                                 (uint32_t(BLOCK_N >> 3) << 17) | (uint32_t(kBlockM >> 4) << 24);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++it) {
-        int m0, n0, kb0, num_kb, z;
-        decode(w, m0, n0, kb0, num_kb, z);
-        const int ab = it & 1;
-        mbar_wait(tmem_empty(ab), ((it >> 1) & 1) ^ 1);  // epilogue has drained this accumulator buffer
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tacc = tmem_base + uint32_t(ab * BLOCK_N);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(full(stage), phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            const uint32_t aA = sA + stage * A_STAGE, aB = sB + stage * B_STAGE;
-            const uint64_t da = A_MN ? make_smem_desc_mn(aA + k * 2048) : make_smem_desc(aA + k * 32);
-            const uint64_t db = B_MN ? make_smem_desc_mn(aB + k * 2048) : make_smem_desc(aB + k * 32);
-            if constexpr (SPLIT) {  // small terms first: lo.hi, hi.lo, then hi.hi
-              const uint64_t dal = A_MN ? make_smem_desc_mn(aA + kABytes + k * 2048) : make_smem_desc(aA + kABytes + k * 32);
-              const uint64_t dbl = B_MN ? make_smem_desc_mn(aB + B_BYTES + k * 2048) : make_smem_desc(aB + B_BYTES + k * 32);
-              umma_bf16(tacc, dal, db, idesc, (kb | k) != 0 ? 1u : 0u);
-              umma_bf16(tacc, da, dbl, idesc, 1u);
-              umma_bf16(tacc, da, db, idesc, 1u);
-            } else {
-              umma_bf16(tacc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(empty(stage));  // slot free once these MMAs have read it
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tmem_full(ab));   // accumulator complete
-      }
-    }
-  } else {
-    const int quarter = warp & 3;   // TMEM lanes [32*quarter, 32*quarter+32) belong to this warp
-    int it = 0;
-    for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++it) {
+  } else if (warp < 4) {
+    int stage = 0; uint32_t phase = 0;
+    float acc[2][BLOCK_N / 2];  // rows [0, 64) and [64, 128) of the tile
+    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       int m0, n0, kb0, num_kb, z;
       decode(w, m0, n0, kb0, num_kb, z);
-      const int ab = it & 1;
-      const int rl = quarter * 32 + lane;
+      const int rl = threadIdx.x;
       const int64_t r = IMPL ? int64_t(m0 / kBlockM) * ic.rows + rl : int64_t(m0) + rl;
       const bool rvalid = r < M && (!IMPL || rl < ic.rows);
       // where this thread's 32 values of column chunk c0 live in memory: row pr, first column pc (== r, n0 + c0
@@ -218,7 +170,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       };
       // EPI 2: pull the ReLU-mask / residual rows of the WHOLE tile into L2 before waiting for the accumulator, so
       // their DRAM latency hides behind the MMA main loop (fetching them chunk by chunk after the wait made the
-      // stride-2 input gradient - 4 chunks, 4 k-blocks - epilogue-latency bound: 271 us)
+      // stride-2 input gradient - 4 chunks, 4 k-blocks - epilogue-latency bound)
       if constexpr (EPI >= 2) {
         if (rvalid) {
 #pragma unroll 1
@@ -230,15 +182,63 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-      mbar_wait(tmem_full(ab), (it >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+      // main loop: one k-block per stage; a stage is handed back once the wgmma group after it has been issued and
+      // its own group has completed (one group in flight)
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(full(stage), phase);
+        wgmma_fence();
+        const uint32_t aA = sA + stage * A_STAGE, aB = sB + stage * B_STAGE;
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          const uint64_t db = B_MN ? make_smem_desc_mn(aB + k * 2048) : make_smem_desc(aB + k * 32);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {  // the two 64-row halves of the tile (8192 B apart in both layouts)
+            const uint32_t ah = aA + h * 8192;
+            const uint64_t da = A_MN ? make_smem_desc_mn(ah + k * 2048) : make_smem_desc(ah + k * 32);
+            if constexpr (SPLIT) {  // small terms first: lo.hi, hi.lo, then hi.hi
+              const uint64_t dal = A_MN ? make_smem_desc_mn(ah + kABytes + k * 2048) : make_smem_desc(ah + kABytes + k * 32);
+              const uint64_t dbl = B_MN ? make_smem_desc_mn(aB + B_BYTES + k * 2048) : make_smem_desc(aB + B_BYTES + k * 32);
+              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], dal, db, (kb | k) != 0);
+              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, dbl, 1);
+              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, db, 1);
+            } else {
+              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, db, (kb | k) != 0);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty(prev)); }
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty(prev)); }
+      if (num_kb == 0) {  // nothing was accumulated (empty split)
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 2; ++j) { acc[0][j] = 0.0f; acc[1][j] = 0.0f; }
+      }
+      named_sync(1, kConsumers);  // the previous tile's epilogue has read the staging tile
+      {
+        const int fr = warp * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            float* sp = stg + (h * 64 + fr) * LDS + 8 * j + fc;
+            *reinterpret_cast<float2*>(sp) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+            *reinterpret_cast<float2*>(sp + 8 * LDS) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+          }
+      }
+      named_sync(1, kConsumers);
 #pragma unroll 1
       for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
         uint32_t v[32];
-        tmem_ld32(tmem_base + (uint32_t(quarter * 32) << 16) + uint32_t(ab * BLOCK_N + c0), v);
-        if (num_kb == 0) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;  // nothing was accumulated (empty split)
+        for (int j = 0; j < 32; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(stg + rl * LDS + c0 + j);
+          v[j] = __float_as_uint(t.x); v[j + 1] = __float_as_uint(t.y); v[j + 2] = __float_as_uint(t.z); v[j + 3] = __float_as_uint(t.w);
         }
         if (partial) {  // split-K: raw partial tile [z][M][N]; splitk_reduce_kernel applies the epilogue
           if (rvalid) {
@@ -265,7 +265,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           float o[32];
           const bool full_cols = nbase + 32 <= N;
           // EPI 2: the ReLU mask / residual rows are read as four 16-byte vectors per 32 columns when aligned
-          // (32 scalar 2-byte loads per thread made fc_dgrad epilogue-bound: 117 us for an 8 GFLOP product)
+          // (32 scalar 2-byte loads per thread made fc_dgrad epilogue-bound)
           uint32_t m16[16], a16[16];
           bool vm = false, va = false;
           if constexpr (EPI >= 2) {
@@ -429,16 +429,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-      // this warp is done reading the accumulator buffer: hand it back to the MMA issuer
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty(ab));
     }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -454,27 +445,43 @@ static inline bool attr_done(uint64_t* mask) {
   return false;
 }
 
+// dynamic shared memory of gemm_tc_kernel: 1 KB alignment slack, the stage ring, the barriers, the accumulator staging tile
+constexpr size_t tc_smem(int block_n, int stages, bool split) {
+  return 1024 + size_t(stages) * (split ? 2 : 1) * (kABytes + size_t(block_n) * kBlockK * 2) + 16 * stages +
+         size_t(kBlockM) * (block_n + 4) * 4 + 16;
+}
+// the deepest ring of at most `want` stages that fits beside the staging tile
+constexpr int tc_stages(int block_n, int want, bool split) {
+  return (want <= 2 || tc_smem(block_n, want, split) <= 227 * 1024) ? want : tc_stages(block_n, want - 1, split);
+}
+
+// CTAs of `kernel` resident per SM with `smem` bytes of dynamic shared memory: registers, not shared memory, are the
+// limit for most instantiations (a 128-column accumulator pair plus the epilogue needs > 204 registers per thread)
+template <typename Kernel>
+static int resident_per_sm(Kernel kernel, size_t smem) {
+  int n = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kThreads, smem) != cudaSuccess || n < 1) n = 1;
+  return n;
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool SPLIT>
 int launch_e(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
              float* partial, cudaStream_t stream) {
-  constexpr size_t smem = 1024 + kStages * (SPLIT ? 2 : 1) * (kABytes + size_t(BLOCK_N) * kBlockK * 2) + 8 * (2 * kStages + 4) + 16;
+  constexpr size_t smem = tc_smem(BLOCK_N, kStages, SPLIT);
   static_assert(smem <= 227 * 1024, "gemm_tc: stage ring exceeds shared memory");
   static uint64_t attr = 0;
+  static int per_sm = 1;
   if (!attr_done(&attr)) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT>, smem);
   }
   const int64_t tiles_m = (M + kBlockM - 1) / kBlockM, tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n * splits;
   TB_REQUIRE(total < (int64_t(1) << 31), "gemm_tc: too many tiles");
-  // persistent grid: as many CTAs as fit at once (shared memory and 512 TMEM columns per SM)
-  int per_sm = int((220 * 1024) / smem);
-  const int tmem_cols = 2 * BLOCK_N < 32 ? 32 : 2 * BLOCK_N;
-  if (per_sm > 512 / tmem_cols) per_sm = 512 / tmem_cols;
-  if (per_sm < 1) per_sm = 1;
-  if (per_sm > 3) per_sm = 3;
-  int64_t grid = int64_t(kNumSMsB200) * per_sm;
+  // persistent grid: as many CTAs as are resident at once
+  int64_t grid = int64_t(kNumSMs) * per_sm;
   if (ep.max_ctas > 0 && grid > ep.max_ctas) grid = ep.max_ctas;
   if (grid > total) grid = total;
   gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
@@ -493,9 +500,10 @@ int launch_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64
   return launch_e<BLOCK_N, A_MN, B_MN, kStages, 0, SPLIT>(mp, ep, M, N, K, splits, partial, stream);
 }
 
-// Few k-blocks per CTA (dgrad: K = 64 channels): a 2-stage ring keeps 3 CTAs resident per SM so the
-// per-CTA prologue (TMEM alloc, barrier init) of one tile overlaps the epilogue of another.
-// Split mode doubles the stage (hi + lo planes): 3 stages of 64 KB for 128-wide tiles, 4 otherwise.
+// Few k-blocks per CTA (dgrad: K = 64 channels): a deeper ring than 2 stages would only hold the next tile's data, so
+// the ring stays small.  Within a CTA the epilogue does not overlap the next tile's MMAs (the producer prefetches into
+// the ring meanwhile); overlap across CTAs happens only where registers allow two per SM.
+// Split mode doubles the stage (hi + lo planes); the ring is as deep as fits beside the accumulator staging tile.
 template <int BLOCK_N, bool A_MN, bool B_MN>
 int launch(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
            float* partial, cudaStream_t stream) {
@@ -503,10 +511,10 @@ int launch(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t
   const bool split = ep.a_lo != 0;
   if (split) {
     if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, true>(mp, ep, M, N, K, splits, partial, stream);
-    return launch_s<BLOCK_N, A_MN, B_MN, (BLOCK_N >= 128 ? 3 : 4), true>(mp, ep, M, N, K, splits, partial, stream);
+    return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(BLOCK_N, 4, true), true>(mp, ep, M, N, K, splits, partial, stream);
   }
   if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, false>(mp, ep, M, N, K, splits, partial, stream);
-  return launch_s<BLOCK_N, A_MN, B_MN, 4, false>(mp, ep, M, N, K, splits, partial, stream);
+  return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(BLOCK_N, 4, false), false>(mp, ep, M, N, K, splits, partial, stream);
 }
 
 
@@ -514,7 +522,7 @@ int launch(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t
 // patches read straight from the NHWC activation (same overlapping-dimension tensor map as the forward).
 // One stage = the `rows` patches of `fpt` whole frames: A = one 64(o) x rows box of dY (MN-major), B = two
 // 64(k) x rows boxes of patches (MN-major: the k-th 64-wide group is k-block n0/64 + j of the kernel window).
-// rows is padded to a multiple of 16 (the UMMA K step) with shared-memory rows that are zeroed once and
+// rows is padded to a multiple of 16 (the wgmma K step) with shared-memory rows that are zeroed once and
 // never written by TMA, so the padding contributes exact zeros.  CTAs split the frames; raw fp32 partial
 // tiles go to `partial` [z][O][K] and splitk_reduce_kernel folds them in a fixed order.
 struct ImplicitWgrad {
@@ -531,17 +539,14 @@ conv_wgrad_implicit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid
                            const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, int O, int Kdim,
                            float* __restrict__ partial, int tiles_n, ImplicitWgrad iw) {
   constexpr int BLOCK_N = 128;
-  constexpr uint32_t TMEM_COLS = BLOCK_N;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
   const uint32_t group = uint32_t(iw.rows_pad) * 128u;  // one 64-wide group: rows_pad x 128 B (multiple of 1024)
   const uint32_t stage_bytes = (SPLIT ? 6u : 3u) * group;  // [dY group][patch group 0][patch group 1]
   const uint32_t offB = (SPLIT ? 2u : 1u) * group;         // first patch group
-  const uint32_t bars = base + kSt * stage_bytes;       // full[kSt], empty[kSt], tmem_full
-  const uint32_t tmem_slot = bars + 8 * (2 * kSt + 1);
+  const uint32_t bars = base + kSt * stage_bytes;       // full[kSt], empty[kSt]
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kSt + s); };
-  const uint32_t tmem_full = bars + 8u * (2 * kSt);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nt = blockIdx.x % tiles_n, z = blockIdx.x / tiles_n;
   const int n0 = nt * BLOCK_N;
@@ -553,21 +558,13 @@ conv_wgrad_implicit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid
   for (uint32_t off = threadIdx.x * 16u; off < kSt * stage_bytes; off += kThreads * 16u)
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(base + off), "r"(0u) : "memory");
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kSt; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-    mbar_init(tmem_full, 1);
+  if (warp == 4 && lane == 0) {
+    for (int s = 0; s < kSt; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  } else if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       const int kbA = n0 / kBlockK, kbB = kbA + 1;
       const int eA = (kbA / iw.kbw) * iw.row_elems + (kbA % iw.kbw) * kBlockK;
@@ -589,89 +586,71 @@ conv_wgrad_implicit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid
         if (++stage == kSt) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && num > 0) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | (uint32_t(BLOCK_N >> 3) << 17) |
-                                 (uint32_t(kBlockM >> 4) << 24);
-      const int ksteps = iw.rows_pad / 16;
-      int stage = 0; uint32_t phase = 0;
-      for (int i = 0; i < num; ++i) {
-        mbar_wait(full(stage), phase);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t st = base + stage * stage_bytes;
-        for (int k = 0; k < ksteps; ++k) {  // A's second 64-wide group aliases the next group: accumulator rows >= 64 are junk
-          const uint64_t da = make_smem_desc_mn_lbo(st + k * 2048, group);
-          const uint64_t db = make_smem_desc_mn_lbo(st + offB + k * 2048, group);
-          if constexpr (SPLIT) {
-            umma_bf16(tmem_base, make_smem_desc_mn_lbo(st + group + k * 2048, group), db, idesc, (i | k) != 0 ? 1u : 0u);
-            umma_bf16(tmem_base, da, make_smem_desc_mn_lbo(st + 4 * group + k * 2048, group), idesc, 1u);
-            umma_bf16(tmem_base, da, db, idesc, 1u);
-          } else {
-            umma_bf16(tmem_base, da, db, idesc, (i | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(empty(stage));
-        if (++stage == kSt) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
   } else {
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;  // output channel
-    if (quarter < 2) {                   // TMEM lanes 0..63
-      if (num > 0) {
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t v[32];
-        if (num > 0) {
-          tmem_ld32(tmem_base + (uint32_t(quarter * 32) << 16) + uint32_t(c0), v);
+    // M = 64 output channels (O <= 64): one m64n128 accumulator per warpgroup
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.0f;
+    const int ksteps = iw.rows_pad / 16;
+    int stage = 0; uint32_t phase = 0;
+    for (int i = 0; i < num; ++i) {
+      mbar_wait(full(stage), phase);
+      wgmma_fence();
+      const uint32_t st = base + stage * stage_bytes;
+      for (int k = 0; k < ksteps; ++k) {
+        const uint64_t da = make_smem_desc_mn_lbo(st + k * 2048, group);
+        const uint64_t db = make_smem_desc_mn_lbo(st + offB + k * 2048, group);
+        if constexpr (SPLIT) {
+          wgmma_bf16<BLOCK_N, 1, 1>(acc, make_smem_desc_mn_lbo(st + group + k * 2048, group), db, (i | k) != 0);
+          wgmma_bf16<BLOCK_N, 1, 1>(acc, da, make_smem_desc_mn_lbo(st + 4 * group + k * 2048, group), 1);
+          wgmma_bf16<BLOCK_N, 1, 1>(acc, da, db, 1);
         } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0u;
+          wgmma_bf16<BLOCK_N, 1, 1>(acc, da, db, (i | k) != 0);
         }
-        if (r < O) {
-          float* pz = partial + (int64_t(z) * O + r) * Kdim + n0 + c0;
-          if (n0 + c0 + 32 <= Kdim && (Kdim & 3) == 0) {
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(stage));
+      if (++stage == kSt) { stage = 0; phase ^= 1; }
+    }
+    // fragment rows r and r + 8 (output channels), column pairs 8j + fc
+    const int r = warp * 16 + (lane >> 2), fc = 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(pz + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (n0 + c0 + j < Kdim) pz[j] = __uint_as_float(v[j]);
-          }
+    for (int e = 0; e < 2; ++e) {
+      const int o = r + 8 * e;
+      if (o >= O) continue;
+      float* pz = partial + (int64_t(z) * O + o) * Kdim + n0;
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int c = 8 * j + fc;
+        if (n0 + c + 2 <= Kdim && (Kdim & 1) == 0) {
+          *reinterpret_cast<float2*>(pz + c) = make_float2(acc[4 * j + 2 * e], acc[4 * j + 2 * e + 1]);
+        } else {
+          if (n0 + c < Kdim) pz[c] = acc[4 * j + 2 * e];
+          if (n0 + c + 1 < Kdim) pz[c + 1] = acc[4 * j + 2 * e + 1];
         }
       }
     }
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
 template <int BLOCK_N, int EPI, int kSt, bool SPLIT>
 int launch_conv_fwd_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K,
                       int64_t tiles_m, const ImplicitConv& ic, cudaStream_t stream) {
-  constexpr size_t smem = 1024 + kSt * (SPLIT ? 2 : 1) * (kABytes + size_t(BLOCK_N) * kBlockK * 2) + 8 * (2 * kSt + 4) + 16;
+  constexpr size_t smem = tc_smem(BLOCK_N, kSt, SPLIT);
   static_assert(smem <= 227 * 1024, "gemm_tc: stage ring exceeds shared memory");
   static uint64_t attr = 0;
+  static int per_sm = 1;
   if (!attr_done(&attr)) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT>, smem);
   }
   const int64_t tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n;
-  int per_sm = int((220 * 1024) / smem);
-  if (per_sm > 512 / (2 * BLOCK_N)) per_sm = 512 / (2 * BLOCK_N);
-  if (per_sm < 1) per_sm = 1;
-  if (per_sm > 3) per_sm = 3;
-  int64_t grid = int64_t(kNumSMsB200) * per_sm;
+  int64_t grid = int64_t(kNumSMs) * per_sm;
   if (grid > total) grid = total;
   gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
       mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), nullptr, int(tiles_m), int(tiles_n), 1, 0, ic);
@@ -681,9 +660,9 @@ int launch_conv_fwd_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t
 template <int BLOCK_N, int EPI = 1, int kSt = 4>
 int launch_conv_fwd(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int64_t tiles_m,
                     const ImplicitConv& ic, cudaStream_t stream) {
-  if (ep.a_lo != 0)  // split: 64 KB stages for 128-wide tiles
-    return launch_conv_fwd_s<BLOCK_N, EPI, (BLOCK_N >= 128 && kSt > 3 ? 3 : kSt), true>(mp, ep, M, N, K, tiles_m, ic, stream);
-  return launch_conv_fwd_s<BLOCK_N, EPI, kSt, false>(mp, ep, M, N, K, tiles_m, ic, stream);
+  if (ep.a_lo != 0)  // split: stages of twice the size
+    return launch_conv_fwd_s<BLOCK_N, EPI, tc_stages(BLOCK_N, kSt, true), true>(mp, ep, M, N, K, tiles_m, ic, stream);
+  return launch_conv_fwd_s<BLOCK_N, EPI, tc_stages(BLOCK_N, kSt, false), false>(mp, ep, M, N, K, tiles_m, ic, stream);
 }
 
 }  // namespace
@@ -799,7 +778,7 @@ int conv_tc_dgrad_implicit(const void* dy_nhwc_bf16, const void* wt_bf16, int64_
     rc = make_map(&mp.bl, wt_lo, 4 * C, K, K, 128);
     if (rc) return rc;
   }
-  // 4 k-blocks per tile: a 2-stage ring lets two CTAs share an SM so one tile's epilogue overlaps another's loads
+  // 4 k-blocks per tile: a 2-stage ring holds the next tile's operands while the epilogue runs
   return launch_conv_fwd<128, 2, 2>(mp, ep, M, 4 * C, K, Nf, ic, stream);
 }
 
@@ -847,7 +826,7 @@ int conv_tc_wgrad_implicit(const void* dy_bf16, const void* act_nhwc_bf16, int64
     const int64_t e_last = int64_t(kb_last / iw.kbw) * iw.row_elems + int64_t(kb_last % iw.kbw) * kBlockK;
     TB_REQUIRE(e_last + kBlockK <= int64_t(H) * W * C, "conv_tc_wgrad_implicit: window tail outside the frame");
   }
-  int64_t splits = kNumSMsB200 / tiles_n;
+  int64_t splits = kNumSMs / tiles_n;
   if (splits > iw.stages_total) splits = iw.stages_total;
   if (splits * O * K > partial_floats) splits = partial_floats / (int64_t(O) * K);
   TB_REQUIRE(splits >= 1, "conv_tc_wgrad_implicit: partial buffer too small");
@@ -956,7 +935,7 @@ int f32_to_bf16(const float* in, void* out, int64_t rows, int64_t cols, int64_t 
   if (total == 0) return 0;
   ProfScope prof("f32_to_bf16", stream);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > kNumSMsB200 * 16) blocks = kNumSMsB200 * 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   f32_to_bf16_kernel<<<(unsigned)blocks, 256, 0, stream>>>(in, static_cast<__nv_bfloat16*>(out), rows, cols, ld, ld16, lo_off);
   return check_launch("f32_to_bf16_kernel");
 }

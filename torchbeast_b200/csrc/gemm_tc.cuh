@@ -1,4 +1,4 @@
-// bf16 tcgen05 GEMM (see gemm_tc.cu): host interface.
+// bf16 wgmma GEMM (see gemm_tc.cu): host interface.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -11,7 +11,7 @@ struct TcEpilogue {
   __nv_bfloat16* C16 = nullptr; int64_t ldc16 = 0;   // bf16 output (nullable) - next GEMM's operand
   // Split-bf16 ("bf16x3") mode: every operand x is stored as TWO bf16 planes, hi = bf16(x) and lo = bf16(x - hi)
   // (16-17 significant bits together), and the product is accumulated as hi.hi + hi.lo + lo.hi in the same fp32
-  // TMEM accumulator - fp32-grade results (relative error ~2^-17 per product instead of 2^-9) at 3 MMAs per k-step.
+  // fp32 accumulator - fp32-grade results (relative error ~2^-17 per product instead of 2^-9) at 3 MMAs per k-step.
   // a_lo / b_lo: element offsets from the operand base pointers to their lo planes (both non-zero = split product,
   // both zero = plain bf16); c16_lo: element offset from C16 to the lo plane of the bf16 output (0 = hi only).
   int64_t a_lo = 0, b_lo = 0, c16_lo = 0;

@@ -9,7 +9,7 @@ constexpr int kMaxOut = 32;   // A + 1 outputs at most
 constexpr int kSlabRows = 64; // rows per partial block of the weight-gradient reduction
 
 // Block = 8 warps x kFwdRowsPerWarp rows each; the (A+1) x F weight matrix is staged once per block in shared memory
-// (the first version re-read it through L1 for every row: 46 us).  Lanes stride over F; 8 accumulators per pass.
+// (the first version re-read it through L1 for every row).  Lanes stride over F; 8 accumulators per pass.
 constexpr int kFwdRowsPerWarp = 2;  // 16 rows per block: ~160 blocks at N = 2592
 __global__ void heads_fwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ Wp,
                                  const float* __restrict__ bp, const float* __restrict__ Wb, const float* __restrict__ bb,

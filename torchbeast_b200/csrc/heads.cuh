@@ -1,6 +1,6 @@
 // Policy / baseline heads (monobeast.py:613-614, polybeast_learner.py:251-252): two tiny linear layers over the
 // core output, fused.  A GEMM tile is the wrong shape for [N, F] x [F, A+1] with A+1 ~ 7 outputs: the tiled
-// SIMT kernels spent 72 us forward and ~70 us backward here; these kernels stream core_out once.
+// GEMM would read core_out many times; these kernels stream it once.
 #pragma once
 #include "common.cuh"
 

@@ -1,4 +1,4 @@
-// Stacked LSTM over the unroll with per-step done-reset, forward + BPTT (sm_100a).
+// Stacked LSTM over the unroll with per-step done-reset, forward + BPTT (sm_90a).
 //
 // Replaces the reference's 81 seq_len-1 nn.LSTM calls and their autograd graph
 // (/root/reference/torchbeast/monobeast.py:603-611, polybeast_learner.py:241-249):
@@ -100,7 +100,7 @@ __global__ void add2_kernel(const float* __restrict__ a, const float* __restrict
 // forward step: one CTA = 4 hidden units (x 4 gates = 16 rows of W_hh) x a 32-row batch tile.
 // 512 threads: lane = batch row, warp = (gate q, k-quarter ks); each thread accumulates gate q of the
 // 4 units over a quarter of the reduction, partial sums are combined through shared memory (16 warps
-// per SM hide the LDS/FMA latency that a 4-warp CTA exposed: ncu 'No Eligible' 86% -> see profiles/).
+// per SM hide the LDS/FMA latency that a 4-warp CTA exposed: ncu 'No Eligible' 86%).
 // Operands are staged by the bulk-copy engine (cp.async.bulk -> UBLKCP, mbarrier complete_tx):
 // four 8 KB W_hh gate slices - issued BEFORE griddepcontrol.wait, so with programmatic
 // dependent launch they stream in while the previous time step is still finishing - and the
@@ -467,7 +467,7 @@ __device__ __forceinline__ void grid_wait(const unsigned* ctr, unsigned target) 
   // arrivals (or a later one in the same release sequence), which is what synchronizes this thread with every
   // arriving CTA.  History: acquire loads in the spin cost an L1 invalidation per poll (30 % of the step at the
   // barrier); relaxed spin + fence.acq_rel.gpu fixed that but the fence is a full MEMBAR.ALL.GPU - ncu showed the
-  // waiting thread spending as long in it (1.3 us) as in the release fence of the arrive.
+  // waiting thread spending as long in it as in the release fence of the arrive.
   while (ld_relaxed_u32(ctr) < target) {}
   (void)ld_acquire_u32(ctr);
   asm volatile("fence.proxy.async;" ::: "memory");  // generic-proxy writes of other CTAs -> our bulk copies
@@ -783,7 +783,7 @@ static int lstm_bwd_persistent(const LstmLayerWs& L, const LstmWs& ws, const flo
 
 // =========================================================================================
 // Tensor-core variants of the persistent recurrence (bf16 backend): the per-step recurrent products run
-// on mma.sync.m16n8k16 (bf16 x bf16 -> fp32).  tcgen05 needs M >= 64 and smem-resident B, so for this
+// on mma.sync.m16n8k16 (bf16 x bf16 -> fp32).  wgmma needs M >= 64 and smem-resident B, so for this
 // M = 32, N = 16/4, weights-in-registers product the warp-level MMA is the right tool: the CTA's W_hh
 // slice lives in REGISTERS as B fragments for all T+1 steps (nothing but the 34 KB bf16 h tile moves
 // per step), A fragments come from shared memory via ldmatrix.
@@ -1155,7 +1155,7 @@ constexpr int kBwdNT = kBwdCols / 8;
 
 // Every CTA needs ALL gate gradients of the step (4 x [32, H] bf16 = 137 KB, pulled L2 -> smem with all loads
 // of a thread in flight at once); 8 columns per CTA (65 CTAs) fill the n8 MMA tile and halve the per-step L2
-// traffic against 4 columns (measured: 4 cols 8.0 us/step, 16 cols 9.8 us/step with too few SMs pulling).
+// traffic against 4 columns (16 columns leave too few SMs pulling).
 __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_mma_kernel(PersistBwdMmaArgs a) {
   extern __shared__ __align__(128) unsigned char smem_b[];
   __nv_bfloat16* Xs = reinterpret_cast<__nv_bfloat16*>(smem_b);  // [4 gates][32][Hq]
@@ -1581,20 +1581,20 @@ __global__ void lstm_init_state_q_kernel(const float* __restrict__ h0, const flo
 // Same wavefront as lstm2_fwd_wave_mma_kernel (layer 0 at t = s, layer 1 at t = s-1 per wave step, the
 // layer-1 input projection riding on the pass), but every MMA operand is a hi/lo bf16 PAIR (x = hi + lo,
 // hi.hi + hi.lo + lo.hi in fp32: ~2^-17 relative per product, fp32-grade) so that the recurrence holds the
-// 1e-4 parity contract the bf16 kernel cannot.  What changed with the 3x MMA count (measured,
-// profiles/ubench_lstm_r2.txt: mma.sync.m16n8k16 runs at 2.0 cycles / MMA / SM = 2036 flop/clk/SM):
+// 1e-4 parity contract the bf16 kernel cannot.  What changed with the 3x MMA count (tools/ubench/ubench_lstm.cu
+// measures the mma.sync, gather and hand-off rates this layout is built around):
 //   * 11 MMA warps x 3 k16-steps cover K = 528 exactly (33 k-steps): no padded k-steps, weights of all three
 //     matrices as hi AND lo B fragments in registers (72 per thread) for all steps;
 //   * h is exchanged as two bf16 planes (hq: raw h, slot t+1 = h_t) written with 8-byte stores (4 units x
-//     bf16 of one row and plane) and pulled as 4 x 34 KB tiles per step with cp.async (77 B/clk/SM measured);
+//     bf16 of one row and plane) and pulled as 4 x 34 KB tiles per step with cp.async;
 //   * the cell state lives in a register of the thread that owns (layer, unit, row) for all steps;
 //   * the grid barrier is per-CTA FLAGS instead of one contended counter: producer = stores, bar.sync,
-//     fence.acq_rel.gpu (600 cycles measured), st flag[cta] = step; consumers = one thread per producer
+//     fence.acq_rel.gpu, st flag[cta] = step; consumers = one thread per producer
 //     spinning on its flag with relaxed loads, one acquire load, bar.sync.
 // CTA = kStepUnits hidden units x 4 gates of BOTH layers, B <= 32 rows, ceil(H/16) <= 33.
 // =========================================================================================
-constexpr int kFlagStride = 32;   // one flag per 128-byte line: 130 CTAs polling 130 flags packed into 5 lines made those
-                                  // lines' L2 slices the bottleneck (ncu: 36 % of the samples in the spin, loads ~3000 cycles)
+constexpr int kFlagStride = 32;   // one flag per 128-byte line: 130 CTAs polling 130 flags packed into 5 lines make those
+                                  // lines' L2 slices the bottleneck
 constexpr int kSplitWarps = 11;
 constexpr int kSplitThreads = kSplitWarps * 32;
 constexpr int kSplitK = 3;  // k16 steps per warp
@@ -1716,7 +1716,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
     // tiles (cp.async, one commit group per k-step) and starts its MMAs on k-step 0 while k-steps 1, 2 are still in
     // flight - no block-wide barrier between the hand-off and the products.  (History: 130 threads per CTA polling 130
     // flag words - 17 k pollers chip-wide on 5 cache lines - made the L2 slices of those lines the bottleneck: ncu
-    // showed 36 % of all samples in the spin and the step at 9.8 us.)
+    // showed over a third of all samples in the spin.)
     if (s > 0) {
       const int p0 = (ks0 * 16) / kStepUnits + lane;                   // producer CTA of this lane
       const int pend = (min((ks0 + kSplitK) * 16, H) + kStepUnits - 1) / kStepUnits;
@@ -2401,8 +2401,8 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
 
 // =========================================================================================
 // Single-layer recurrence on ONE thread-block cluster (precision 2, H = 256: the IMPALA ResNet's LSTM).
-// The cooperative kernels above pay 2-3 us per step for a grid-wide barrier through L2 although a [B, 256] x [256, 1024]
-// product is ~0.1 us of tensor-core time.  Here the 16 CTAs of one cluster own 16 hidden units x 4 gates each (64 gate
+// The cooperative kernels above pay a grid-wide barrier through L2 per step although a [B, 256] x [256, 1024]
+// product is a small fraction of that in tensor-core time.  Here the 16 CTAs of one cluster own 16 hidden units x 4 gates each (64 gate
 // rows of W_hh as hi / lo mma.sync B fragments in registers for all steps), h is exchanged through DISTRIBUTED SHARED
 // MEMORY (every CTA stores its 16 units of h_t - bf16 hi / lo - into the A tile of all 16 CTAs) and the step barrier is the
 // hardware cluster barrier.  Warp w multiplies k16 steps {2w, 2w+1} for all 8 n8 tiles (A is read once per CTA), partial
@@ -2600,7 +2600,7 @@ static int lstm_fwd_cluster(const LstmLayerWs& L, const float* w_hh, float* hs, 
 
 // ---- backward on the same cluster ---------------------------------------------------------------------------------
 // dL/dh_t needs dgates_{t+1} . W_hh over ALL 1024 gate rows.  Broadcasting the gate gradients (64 KB per CTA and step) would sit
-// on the DSMEM links (17-21 B/clk per SM measured); instead every CTA multiplies ITS 64 gate gradients (local, bf16 hi / lo
+// on the DSMEM links; instead every CTA multiplies ITS 64 gate gradients (local, bf16 hi / lo
 // in shared memory) with ITS 64 rows of W_hh (B fragments in registers) into a partial dh[rows, 256], and the partials are
 // reduce-scattered: the 16 columns of destination CTA d go into slot [source] of d's receive buffer (16 KB per CTA and
 // step), summed by d in source order (deterministic) at the start of the next step.  Buffers as lstm_bwd_persistent_kernel:
@@ -2893,7 +2893,7 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   return check_launch("lstm2_bwd_wave_split_kernel");
 }
 
-// Side stream for work that can run beside a recurrence kernel (which occupies only H/8 = 65 of the 148 SMs):
+// Side stream for work that can run beside a recurrence kernel (which occupies only H/8 = 65 of the 132 SMs):
 // forked from / joined into the caller's stream with events, so it is captured into the learner's CUDA graph.
 struct SideStream {
   cudaStream_t stream = nullptr;
@@ -2987,7 +2987,7 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
   }
   // (forward and backward are decided together: the split backward consumes the blocked saves only the split forward writes)
   if (precision == 2 && layers == 2 && wave_bwd_split_applicable(B, In, H)) {
-    // split-bf16 wavefront: layer 0's input projection is one split tcgen05 GEMM, everything sequential is ONE kernel
+    // split-bf16 wavefront: layer 0's input projection is one split wgmma GEMM, everything sequential is ONE kernel
     const int Hq = mma_hq(H);
     for (int l = 0; l < 2; ++l) {
       LstmLayerWs& L = ws.layer[l];
@@ -3092,7 +3092,7 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
 static int splits_for(int64_t M, int64_t N, int64_t K, int64_t scratch_floats) {
   const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
   const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMsB200 + tiles - 1) / tiles;
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
   const int64_t ktiles = (K + kGemmBK - 1) / kGemmBK;
   if (s > ktiles / 4) s = ktiles / 4;
   if (s * M * N > scratch_floats) s = scratch_floats / (M * N);
@@ -3224,7 +3224,7 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
       float* wscr = splitk;
       TcEpilogue te; te.tag = "lstm_wgrad";
       if (tail) {
-        static const int tail_ctas = [] { const char* e = getenv("TB_LSTM_TAIL_CTAS"); return e ? atoi(e) : 0; }();  // 0 = uncapped: measured best (cap 32/64/96/none: 2.13/2.11/2.09/2.08 ms)
+        static const int tail_ctas = [] { const char* e = getenv("TB_LSTM_TAIL_CTAS"); return e ? atoi(e) : 0; }();  // 0 = uncapped
         gs = tail->stream; wscr = ws.wg_scratch; te.max_ctas = tail_ctas;
       }
       if (side) {
@@ -3232,7 +3232,7 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
         if (ee == cudaSuccess) ee = cudaStreamWaitEvent(side->stream, side->fork, 0);
         TB_REQUIRE(ee == cudaSuccess, "lstm: side stream fork: %s", cudaGetErrorString(ee));
         gs = side->stream;
-        te.max_ctas = kNumSMsB200 - int((H + kBwdCols - 1) / kBwdCols) - 2;
+        te.max_ctas = kNumSMs - int((H + kBwdCols - 1) / kBwdCols) - 2;
         forked = true;
       }
       te.C = g.w_hh[l]; te.ldc = H;      // dW_hh[4H,H] = dgates^T . hm   (both operands stored [N, .]: MN-major)

@@ -58,8 +58,8 @@ struct LstmWs {
 size_t lstm_ws_bytes(int64_t T1, int64_t B, int In, int H, int layers, int precision);
 LstmWs lstm_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int precision);
 
-// precision: 0 = fp32 SIMT GEMMs; 1 = bf16 tcgen05 GEMMs for the hoisted projections and bf16 mma.sync operands in
-// the recurrence; 2 = split-bf16 (hi/lo planes, 3 MMAs) tcgen05 GEMMs with the recurrence in exact fp32.  State, gate
+// precision: 0 = fp32 SIMT GEMMs; 1 = bf16 wgmma GEMMs for the hoisted projections and bf16 mma.sync operands in
+// the recurrence; 2 = split-bf16 (hi/lo planes, 3 MMAs) wgmma GEMMs with the recurrence in exact fp32.  State, gate
 // activations and accumulation are fp32 in every mode.
 // x [T1*B, In] -> y [T1*B, H]; h0/c0/hN/cN [layers, B, H]; notdone [T1*B] (float, multiplies the state
 // before each step).  splitk: GEMM scratch (kSplitKScratchFloats).

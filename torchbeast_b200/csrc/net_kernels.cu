@@ -9,7 +9,7 @@ namespace tb {
 
 static inline unsigned grid_for(int64_t work_items, int threads) {
   int64_t blocks = (work_items + threads - 1) / threads;
-  const int64_t cap = int64_t(kNumSMsB200) * 16;
+  const int64_t cap = int64_t(kNumSMs) * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (unsigned)blocks;
@@ -187,7 +187,7 @@ __global__ void colsum_partial_kernel(const float* __restrict__ X, float* __rest
 }
 
 // block (32 x 8): 8 partial sums per column (slab s goes to row s % 8), folded in a fixed order.  (The first
-// version walked all slabs with one thread per column: 256 dependent L2 round trips, 16 us per call.)
+// version walked all slabs with one thread per column: 256 dependent L2 round trips per call.)
 __global__ void colsum_final_kernel(const float* __restrict__ part, float* __restrict__ out, int64_t ncols, int slabs) {
   __shared__ float sm[8][33];
   const int64_t n = int64_t(blockIdx.x) * 32 + threadIdx.x;
@@ -506,8 +506,8 @@ int colsum_bf16(const void* X, float* out, int64_t M, int64_t ncols, int64_t ld,
       (reinterpret_cast<uintptr_t>(X) & 15) == 0 && (lo_off & 7) == 0) {
     const int cg = int(ncols / 8);
     // partials [blocks][ncols] must fit the caller's scratch (colsum_scratch_floats(>= 512) = 256 * 512 floats): 6 CTAs per SM
-    // keep enough 16-byte loads in flight to stream at HBM rate (256 CTAs ran the 133 MB conv1 gradient at 2.3 TB/s)
-    int blocks = kNumSMsB200 * 6;
+    // keep enough 16-byte loads in flight to stream at HBM rate
+    int blocks = kNumSMs * 6;
     if (int64_t(blocks) * ncols > int64_t(kColsumSlabs) * 512) blocks = int(int64_t(kColsumSlabs) * 512 / ncols);
     colsum_dense_bf16_kernel<<<blocks, 256, 0, stream>>>(static_cast<const uint4*>(X), scratch, M * cg, cg, lo_off / 8);
     int rc = check_launch("colsum_dense_bf16_kernel");

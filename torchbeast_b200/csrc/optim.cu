@@ -84,7 +84,7 @@ int tb_grad_sumsq_f32(const float* grads, int64_t n, float* out_sumsq, void* wor
   TB_REQUIRE(n == 0 || grads, "tb_grad_sumsq_f32: null gradient buffer");
   TB_REQUIRE((reinterpret_cast<uintptr_t>(grads) & 15) == 0, "tb_grad_sumsq_f32: gradient buffer must be 16-byte aligned");
   int64_t blocks = (n / 4 + 255) / 256;
-  if (blocks > kNumSMsB200 * 4) blocks = kNumSMsB200 * 4;
+  if (blocks > kNumSMs * 4) blocks = kNumSMs * 4;
   if (blocks < 1) blocks = 1;
   ProfScope prof("grad_sumsq", (cudaStream_t)stream);
   grad_sumsq_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(grads, n, out_sumsq, workspace);
@@ -99,7 +99,7 @@ int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, flo
   TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_step_f32: null buffer");
   TB_REQUIRE(momentum == 0.0f || momentum_buf, "tb_clip_rmsprop_step_f32: momentum needs a buffer");
   int64_t blocks = (n + 255) / 256;
-  if (blocks > kNumSMsB200 * 8) blocks = kNumSMsB200 * 8;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   ProfScope prof("clip_rmsprop", (cudaStream_t)stream);
   clip_rmsprop_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       params, grads, square_avg, momentum != 0.0f ? momentum_buf : nullptr, n, sumsq, max_norm, lr_device, lr, alpha,

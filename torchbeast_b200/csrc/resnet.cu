@@ -4,7 +4,7 @@
 //   for ch in (16, 32, 32):  x = maxpool3x3/2(conv3x3(x));  x += conv(relu(conv(relu(x))));  x += conv(relu(conv(relu(x))))
 //   x = relu(x) -> fc 3872->256 -> relu -> cat[x, clip(reward)] -> [LSTM(257->256)] -> policy / baseline
 // Same construction as atarinet.cu: NHWC activations, every conv a patch-matrix GEMM through the shared
-// GEMM backends (fp32 SIMT for parity, bf16 tcgen05 for throughput - the activation element type T
+// GEMM backends (fp32 SIMT for parity, bf16 wgmma for throughput - the activation element type T
 // follows the backend), residual adds fused into the GEMM epilogue, ReLU-on-read fused into the patch
 // gather, ReLU masks and skip-gradients fused into the gather-form col2im, weights/gradients in ONE
 // flat buffer in state_dict order.  Patch matrices are recomputed in the backward pass (a gather is
@@ -227,7 +227,7 @@ ResWs<T> res_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int use_lst
 int splits_simt(int64_t M, int64_t N, int64_t K) {
   const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
   const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMsB200 + tiles - 1) / tiles;
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
   const int64_t kt = (K + kGemmBK - 1) / kGemmBK;
   if (s > kt / 4) s = kt / 4;
   if (s * M * N > kScratchFloats) s = kScratchFloats / (M * N);
@@ -237,12 +237,12 @@ int splits_simt(int64_t M, int64_t N, int64_t K) {
 int splits_tc(int64_t M, int64_t N, int64_t K) {
   const int64_t bn = N <= 64 ? 64 : 128;
   const int64_t tiles = ((M + 127) / 128) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMsB200 + tiles - 1) / tiles;
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
   const int64_t kb = (K + 63) / 64;
   if (s > kb / 4) s = kb / 4;
   const int64_t Np = (N + 31) & ~int64_t(31);  // partial rows are padded to 32 floats (gemm_tc.cu)
   if (s * M * Np > kScratchFloats) s = kScratchFloats / (M * Np);
-  if (s > 148) s = 148;
+  if (s > kNumSMs) s = kNumSMs;
   return int(s < 1 ? 1 : s);
 }
 

@@ -15,7 +15,7 @@ namespace tb {
 
 static inline unsigned rgrid(int64_t work, int threads) {
   int64_t blocks = (work + threads - 1) / threads;
-  const int64_t cap = int64_t(kNumSMsB200) * 16;
+  const int64_t cap = int64_t(kNumSMs) * 16;
   if (blocks > cap) blocks = cap;
   return (unsigned)(blocks < 1 ? 1 : blocks);
 }
@@ -146,7 +146,7 @@ int dy_split_colsum(const float* dy, __nv_bfloat16* out, int64_t lo_off, int64_t
   const int64_t units = M * (C / 4);
   if (units == 0) return 0;
   int64_t blocks = (units + 255) / 256;
-  if (blocks > int64_t(kNumSMsB200) * 8) blocks = int64_t(kNumSMsB200) * 8;
+  if (blocks > int64_t(kNumSMs) * 8) blocks = int64_t(kNumSMs) * 8;
   TB_REQUIRE(blocks * C <= scratch_floats, "dy_split_colsum: scratch too small");
   dy_split_colsum_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(dy), out, lo_off, units, C / 4, scratch);
   TB_TRY(check_launch("dy_split_colsum_kernel"));

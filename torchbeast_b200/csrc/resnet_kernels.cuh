@@ -44,7 +44,7 @@ int im2col3x3(const T* x, T* col, int64_t N, int H, int W, int C, int64_t ldk, i
 int im2col3x3_split(const float* x, __nv_bfloat16* col, int64_t lo_off, int64_t N, int H, int W, int C, int64_t ldk, int relu_in,
                     cudaStream_t stream);
 
-// dY fp32 [M, C] -> bf16 hi / lo planes + column sums db[C] (bias gradient) in one pass; scratch >= 148*8*C floats
+// dY fp32 [M, C] -> bf16 hi / lo planes + column sums db[C] (bias gradient) in one pass; scratch >= kNumSMs*8*C floats
 int dy_split_colsum(const float* dy, __nv_bfloat16* out, int64_t lo_off, int64_t M, int C, float* db, float* scratch,
                     int64_t scratch_floats, cudaStream_t stream);
 // weights [O, C, 3, 3] -> [C, ld >= 9*O] hi / lo planes with flipped taps: the input gradient as a convolution of dY

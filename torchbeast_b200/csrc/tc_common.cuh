@@ -1,17 +1,20 @@
-// Shared device/host helpers of the tcgen05 kernels (gemm_tc.cu, conv_implicit.cu): mbarrier, TMA, UMMA
-// descriptors, TMEM loads, tensor-map construction.  Internal header: include inside namespace-less scope.
+// Shared device/host helpers of the wgmma kernels (gemm_tc.cu, conv_implicit.cu, conv3x3_sw.cu): mbarrier, TMA,
+// wgmma descriptors, tensor-map construction.  Internal header: include inside namespace-less scope.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace tb {
 namespace tcd {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;           // 64 bf16 = 128 bytes = one swizzle atom row
-constexpr int kThreads = 192;
+// warps 0-3: the consumer warpgroup (wgmma issue + epilogue, one accumulator row pair per thread), warp 4: TMA producer
+constexpr int kConsumers = 128;
+constexpr int kThreads = kConsumers + 32;
 constexpr uint32_t kABytes = kBlockM * kBlockK * 2;  // 16 KB
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -45,44 +48,24 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// wgmma shared-memory matrix descriptor: start >> 4 | LBO >> 4 << 16 | SBO >> 4 << 32 | layout << 62 (1 = SWIZZLE_128B)
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  // K-major, SWIZZLE_128B: start>>4 | LBO(1)<<16 | SBO(1024>>4)<<32 | version(1)<<46 | layout(2)<<61
-  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
-}
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t saddr) {
-  // MN-major, SWIZZLE_128B: LBO = 8192 B (next 64-wide mn group), SBO = 1024 B (next 8 k rows)
-  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(8192 >> 4) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
+  // K-major, SWIZZLE_128B: SBO = 1024 B (8 rows x 128 B); LBO unused
+  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(1) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
 __device__ __forceinline__ uint64_t make_smem_desc_mn_lbo(uint32_t saddr, uint32_t lbo_bytes) {
-  // MN-major, SWIZZLE_128B with an explicit byte distance between the 64-wide mn groups
-  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(lbo_bytes >> 4) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 46) |
-         (uint64_t(2) << 61);
+  // MN-major, SWIZZLE_128B: LBO = byte distance between the 64-wide mn groups, SBO = 1024 B (next 8 k rows)
+  return uint64_t((saddr & 0x3FFFF) >> 4) | (uint64_t(lbo_bytes >> 4) << 16) | (uint64_t(1024 >> 4) << 32) | (uint64_t(1) << 62);
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t saddr) { return make_smem_desc_mn_lbo(saddr, 8192); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// barrier over the `threads` threads of one warpgroup role (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // split-bf16 planes of a float: hi = bf16(x), lo = bf16(x - hi); packed pairs for two consecutive elements

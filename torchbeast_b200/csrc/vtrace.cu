@@ -1,4 +1,4 @@
-// V-trace + IMPALA loss kernels for sm_100a (B200).
+// V-trace + IMPALA loss kernels for sm_90a (H100).
 //
 // Replaces the device-side work of (paths under /root/reference/torchbeast/):
 //   core/vtrace.py:50-55    action_log_probs           -> action_log_probs_kernel
@@ -33,7 +33,7 @@ static int sm_count() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       g_sm_count = n;
     else
-      g_sm_count = kNumSMsB200;
+      g_sm_count = kNumSMs;
   }
   return g_sm_count;
 }

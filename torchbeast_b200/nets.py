@@ -1,4 +1,4 @@
-"""Network modules whose forward/backward are the hand-written sm_100a kernels.
+"""Network modules whose forward/backward are the hand-written sm_90a kernels.
 
 `AtariNet` keeps the reference's constructor, `initial_state`, `forward` contract and
 state_dict keys/shapes (/root/reference/torchbeast/monobeast.py:545-635, BASELINE.md section 5) so
@@ -206,7 +206,7 @@ class AtariNet(FlatParamModule):
     """CUDA AtariNet (reference monobeast.py:545-635).  conv 8/4 -> 4/2 -> 3/1 -> fc 512 ->
     cat[reward, one-hot last action] -> optional 2-layer LSTM(519) -> policy / baseline heads."""
 
-    # "bf16x3" (default): every dense product on tcgen05 tensor cores with SPLIT bf16 operands - x = hi + lo, two bf16
+    # "bf16x3" (default): every dense product on wgmma tensor cores with SPLIT bf16 operands - x = hi + lo, two bf16
     #     planes, accumulated as hi.hi + hi.lo + lo.hi in fp32 (3 MMAs, ~2^-17 relative per product): holds the
     #     reference's fp32 results to the 1e-4 parity contract (tests/test_learner_baseline_gpu.py);
     # "bf16": single-plane bf16 operands (1 MMA, 2^-9): fastest, mixed-precision tolerances only;
