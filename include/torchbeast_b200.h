@@ -97,6 +97,25 @@ int tb_impala_loss_fwd_bwd_f32(const float* behavior_logits, const float* target
                                float* target_alp, float* losses_out, float* grad_logits,
                                float* grad_values, int zero_tail, void* workspace, void* stream);
 
+/* ---- seeded action sampling for the acting forward ------------------------------------ */
+
+/* monobeast.py:618-619 / polybeast_learner.py:256-257  torch.multinomial(F.softmax(policy_logits, dim=1), 1) as a
+ * stateless, counter-based sampler: an action depends only on (seed, step, stream id, logits row), never on batch
+ * composition, threads or torch's generator.  logits [T,B,A] f32 contiguous; stream_ids [B] i64, or NULL: column b
+ * uses stream id b; actions [T,B] i64 out.  For row (t,b), with sid = stream_ids[b]:
+ *   1. x = word 0 of Philox4x32-10(counter, key), counter = (lo32(step+t), hi32(step+t), lo32(sid), hi32(sid)),
+ *      key = (lo32(seed), hi32(seed))  (all arithmetic mod 2^64, sid taken as its two's-complement bits);
+ *   2. u = (x >> 8) * 2^-24, a 24-bit uniform in [0,1), exact in fp32;
+ *   3. m = the row's maximum; e_a = expf(l_a - m) (precise expf, not __expf); S = sum of e_a in fp32, in index order;
+ *   4. action = the smallest a whose fp32 running sum e_0 + ... + e_a is strictly greater than the fp32 product u*S;
+ *      if rounding leaves no such a, the last a with e_a > 0;
+ *   5. -inf logits are never chosen.  A row that contains a NaN, whose logits are all -inf, or that has a +inf logit
+ *      gets action -1 (the kernel does not trap).
+ * Because the counter is step + t, one [T,B] call gives the same actions as T calls of [1,B] at step, step+1, ...
+ * Sizes: T, B >= 0, A >= 1; T*B == 0 is a no-op success.                                                        */
+int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
+                          const int64_t* stream_ids, int64_t* actions, void* stream);
+
 /* ---- the three loss functions on their own (API mirror; tests pass float64) ---------- */
 
 /* monobeast.py:107-108 compute_baseline_loss: out[0] = 0.5*sum(adv^2); grad (nullable) = adv. */

@@ -56,6 +56,18 @@ class FlatParamModule(nn.Module):
     # sibling's flat buffer) and take the one-copy path without hanging anything on the dict itself
     _flat_owners = weakref.WeakValueDictionary()
 
+    # torchbeast_b200.sampling.ActionSampler used by training-mode forwards instead of torch.multinomial; None keeps the
+    # reference's sampling.  Not part of the state_dict: checkpoint its `seed` and `step` alongside.
+    action_sampler = None
+
+    def _sample(self, logits, inputs):
+        """Training-mode action [T, B] of the reference-compatible forwards (monobeast.py:618-619).  With a sampler,
+        an optional inputs["stream_ids"] (int64 [B], e.g. actor indices) names each column's random stream."""
+        T, B, A = logits.shape
+        if self.action_sampler is not None:
+            return self.action_sampler.sample(logits, inputs.get("stream_ids"))
+        return torch.multinomial(torch.softmax(logits.detach().view(T * B, A), dim=1), num_samples=1).view(T, B)
+
     def _build_flat(self, spec, device):
         self._spec = list(spec)
         total = sum(_numel(s) for _, s in self._spec)
@@ -360,11 +372,10 @@ class AtariNet(FlatParamModule):
                 self, frame, inputs["reward"], notdone, inputs["last_action"], h0, c0, *params)
         else:
             logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"], h0, c0)
-        flat_logits = logits.detach().view(T * B, self.num_actions)
         if self.training:
-            action = torch.multinomial(torch.softmax(flat_logits, dim=1), num_samples=1)
+            action = self._sample(logits, inputs)
         else:
-            action = torch.argmax(flat_logits, dim=1)  # don't sample when testing
+            action = torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
         out = dict(policy_logits=logits, baseline=baseline, action=action.view(T, B))
         return out, ((hN, cN) if self.use_lstm else tuple())
 
@@ -522,11 +533,10 @@ class ResNet(FlatParamModule):
             logits, baseline, hN, cN = _ResNetFunction.apply(self, frame, inputs["reward"], notdone, h0, c0, *params)
         else:
             logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, h0, c0)
-        flat_logits = logits.detach().view(T * B, self.num_actions)
         if self.training:
-            action = torch.multinomial(torch.softmax(flat_logits, dim=1), num_samples=1)
+            action = self._sample(logits, inputs)
         else:
-            action = torch.argmax(flat_logits, dim=1)  # don't sample when testing
+            action = torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
         return (action.view(T, B), logits, baseline), ((hN, cN) if self.use_lstm else tuple())
 
 

@@ -42,7 +42,12 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
     `(batched_env_outputs, agent_state)` with [T=1, B, ...] leaves, B = 1 .. 512 actors; the forward of the SAME CUDA
     kernels the learner uses runs under `lock` on flags.actor_device, and `batch.set_outputs(((action, policy_logits,
     baseline), core_state))` receives CPU tensors, like the reference.  Works for polybeast's Net (ResNet) and for AtariNet
-    (whose `last_action` input is batched_env_outputs[5] if the nest carries one, else zeros)."""
+    (whose `last_action` input is batched_env_outputs[5] if the nest carries one, else zeros).
+
+    A sampler attached as `model.action_sampler` (torchbeast_b200.sampling) replaces torch.multinomial in training mode;
+    its step advances by one per call, safely across inference threads because the forward runs under `lock`.  The
+    polybeast nest carries no actor id, so each row's stream id is its index in the batch: a run is reproducible for a
+    given sequence of batches, not per actor."""
     device = torch.device(getattr(flags, "actor_device", None) or model.flat_params.device)
     with torch.no_grad():
         for batch in inference_batcher:
