@@ -115,6 +115,11 @@ int tb_impala_loss_fwd_bwd_f32(const float* behavior_logits, const float* target
  * Sizes: T, B >= 0, A >= 1; T*B == 0 is a no-op success.                                                        */
 int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
                           const int64_t* stream_ids, int64_t* actions, void* stream);
+/* The same contract, bit for bit, with seed = seed_step[0] and step = seed_step[1] read from device memory when the
+ * kernel runs: a launch captured in a CUDA graph samples at whatever (seed, step) was written there before each
+ * replay.  Same host validation, and a null seed_step is rejected.                                              */
+int tb_sample_actions_dev_f32(const float* logits, int64_t T, int64_t B, int64_t A, const uint64_t* seed_step,
+                              const int64_t* stream_ids, int64_t* actions, void* stream);
 
 /* ---- the three loss functions on their own (API mirror; tests pass float64) ---------- */
 

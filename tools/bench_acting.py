@@ -1,11 +1,12 @@
 """Acting-forward timing: the training-mode forward an inference thread runs per environment step (T=1) at B in
-{1, 48, 512} actors, once with the seeded sampler attached (torchbeast_b200.sampling.ActionSampler) and once with the
-reference's torch.multinomial(softmax(.)), plus each sampling step on its own.
+{1, 48, 512} actors, once with the seeded sampler attached (torchbeast_b200.sampling.ActionSampler), once with the
+reference's torch.multinomial(softmax(.)) and once replayed as a CUDA graph with the sampler attached
+(torchbeast_b200.acting.GraphedActor), plus each sampling step on its own.
 
     python tools/bench_acting.py [--net atari|resnet] [--use_lstm 0|1] [--precision fp32|bf16|bf16x3] [--num_actions A]
 
-Eager calls back to back (host launch cost included, as an inference thread pays it), CUDA events around `--reps` calls;
-the four measurements alternate over `--rounds` rounds and each number is the median round.  Prints one JSON line with an
+Calls back to back (host launch cost included, as an inference thread pays it), CUDA events around `--reps` calls;
+the five measurements alternate over `--rounds` rounds and each number is the median round.  Prints one JSON line with an
 `acting` key, beside the card's name and power limit (an absolute time means nothing without them).  Writes no files.
 """
 import argparse
@@ -55,6 +56,7 @@ def main():
     assert torch.cuda.is_available(), "bench_acting.py needs a GPU (there is no CPU fallback)"
     torch.cuda.set_device(0)
     from torchbeast_b200 import monobeast, polybeast_learner
+    from torchbeast_b200.acting import GraphedActor
     from torchbeast_b200.sampling import ActionSampler
 
     A, use_lstm = args.num_actions, bool(args.use_lstm)
@@ -81,6 +83,14 @@ def main():
             return model(batch, state)
         return run
 
+    graphed = GraphedActor(model)
+
+    def graphed_with(s, batch, state):
+        def run():
+            model.action_sampler = s
+            return graphed(batch, state)
+        return run
+
     cases = []
     with torch.no_grad():
         for B in (1, 48, 512):
@@ -89,6 +99,7 @@ def main():
             logits = model.learner_forward(batch, state).policy_logits
             fns = dict(
                 acting_sampler=forward_with(sampler, batch, state), acting_torch=forward_with(None, batch, state),
+                acting_graphed=graphed_with(sampler, batch, state),
                 sample_sampler=lambda: sampler.sample(logits),
                 sample_torch=lambda: torch.multinomial(torch.softmax(logits.view(B, A), dim=1), num_samples=1))
             for fn in fns.values():  # warm-up: module loads, allocator, library heuristics
@@ -100,7 +111,7 @@ def main():
                     times[k].append(per_call_ms(fn))
             med = {k: float(np.median(v)) for k, v in times.items()}
             cases.append(dict(B=B, acting_ms_sampler=med["acting_sampler"], acting_ms_torch=med["acting_torch"],
-                              sample_us_sampler=med["sample_sampler"] * 1e3, sample_us_torch=med["sample_torch"] * 1e3,
+                              acting_ms_graphed=med["acting_graphed"], sample_us_sampler=med["sample_sampler"] * 1e3, sample_us_torch=med["sample_torch"] * 1e3,
                               logits_bytes=4 * B * A, actions_bytes=8 * B))
     model.action_sampler = None
     print(json.dumps(dict(acting=dict(

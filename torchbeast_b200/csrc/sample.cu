@@ -33,10 +33,18 @@ __device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, u
   return c0;
 }
 
+// kSeedStepOnDevice: seed and step are read from seed_step[0..1] when the kernel runs instead of the by-value
+// arguments, so a launch captured in a CUDA graph picks up whatever (seed, step) was written there before each replay.
+template <bool kSeedStepOnDevice>
 __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __restrict__ logits, int64_t N, int64_t B,
                                                              int64_t A, uint64_t seed, uint64_t step,
+                                                             const uint64_t* __restrict__ seed_step,
                                                              const int64_t* __restrict__ stream_ids,
                                                              int64_t* __restrict__ actions) {
+  if (kSeedStepOnDevice) {
+    seed = seed_step[0];
+    step = seed_step[1];
+  }
   const int64_t stride = int64_t(gridDim.x) * blockDim.x;
   for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < N; i += stride) {
     const int64_t t = i / B, b = i - t * B;
@@ -79,12 +87,9 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float* __rest
   }
 }
 
-}  // namespace tb
-
-using namespace tb;
-
-extern "C" int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
-                                     const int64_t* stream_ids, int64_t* actions, void* stream) {
+// Host validation and launch shared by both entries; seed_step is non-null exactly for the device-memory entry.
+static int sample_actions(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
+                          const uint64_t* seed_step, const int64_t* stream_ids, int64_t* actions, void* stream) {
   TB_REQUIRE(T >= 0 && B >= 0, "sample_actions: negative size T=%lld B=%lld", (long long)T, (long long)B);
   TB_REQUIRE(A >= 1, "sample_actions: A must be at least 1, got %lld", (long long)A);
   if (T == 0 || B == 0) return 0;
@@ -96,7 +101,26 @@ extern "C" int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, 
   int64_t blocks = (N + threads - 1) / threads;
   if (blocks > int64_t(kNumSMs) * 16) blocks = int64_t(kNumSMs) * 16;
   ProfScope prof("sample_actions", (cudaStream_t)stream);
-  sample_actions_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(logits, N, B, A, seed, step, stream_ids,
-                                                                                actions);
+  if (seed_step)
+    sample_actions_kernel<true><<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(logits, N, B, A, 0, 0, seed_step,
+                                                                                        stream_ids, actions);
+  else
+    sample_actions_kernel<false><<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(logits, N, B, A, seed, step,
+                                                                                         nullptr, stream_ids, actions);
   return check_launch("sample_actions_kernel");
+}
+
+}  // namespace tb
+
+using namespace tb;
+
+extern "C" int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
+                                     const int64_t* stream_ids, int64_t* actions, void* stream) {
+  return sample_actions(logits, T, B, A, seed, step, nullptr, stream_ids, actions, stream);
+}
+
+extern "C" int tb_sample_actions_dev_f32(const float* logits, int64_t T, int64_t B, int64_t A, const uint64_t* seed_step,
+                                         const int64_t* stream_ids, int64_t* actions, void* stream) {
+  TB_REQUIRE(seed_step, "sample_actions_dev: null seed_step");
+  return sample_actions(logits, T, B, A, 0, 0, seed_step, stream_ids, actions, stream);
 }

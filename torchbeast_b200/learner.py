@@ -328,6 +328,9 @@ class GraphedLearner:
         with torch.cuda.graph(self.graph):
             self.out = learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None,
                                   stats_sync=False)
+        # the graph writes into the model workspace it was captured with; the model replaces (and frees) that buffer when
+        # it runs another shape, e.g. while the GraphedLearner of another batch shape is captured: keep it alive here
+        self.workspace = getattr(model, "_ws", None)
         self.graph.replay()  # first replay uploads the graph to the device; keep that out of the training loop
         torch.cuda.synchronize()
         # undo the warm-up / capture-time updates so training starts from the caller's weights

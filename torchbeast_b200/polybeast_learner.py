@@ -14,10 +14,12 @@ from torchbeast_b200.losses import (  # noqa: F401
 )
 
 import collections  # noqa: E402
+import os  # noqa: E402
 import threading  # noqa: E402
 
 import torch  # noqa: E402
 
+from torchbeast_b200 import acting as _acting  # noqa: E402
 from torchbeast_b200 import learner as _learner  # noqa: E402
 from torchbeast_b200.nets import ResNet as Net  # noqa: E402,F401
 
@@ -47,8 +49,14 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
     A sampler attached as `model.action_sampler` (torchbeast_b200.sampling) replaces torch.multinomial in training mode;
     its step advances by one per call, safely across inference threads because the forward runs under `lock`.  The
     polybeast nest carries no actor id, so each row's stream id is its index in the batch: a run is reproducible for a
-    given sequence of batches, not per actor."""
+    given sequence of batches, not per actor.
+
+    With flags.inference_graph (or TB_INFERENCE_GRAPH=1) the forward is a CUDA-graph replay (torchbeast_b200.acting.
+    GraphedActor, one per model, shared by the inference threads); training mode then needs a sampler attached.  The
+    replay's outputs live in the graph's static buffers, which the next thread's replay overwrites, so their copy to
+    the host is enqueued before the lock is released."""
     device = torch.device(getattr(flags, "actor_device", None) or model.flat_params.device)
+    graphed = inference_graph_enabled(flags)
     with torch.no_grad():
         for batch in inference_batcher:
             batched_env_outputs, agent_state = batch.get_inputs()
@@ -59,12 +67,42 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
                 la = rest[2] if len(rest) > 2 else torch.zeros(reward.shape, dtype=torch.int64)
                 inputs["last_action"] = la.to(device, non_blocking=True)
             agent_state = _map_nest(lambda t: t.to(device, non_blocking=True), agent_state)
+            if graphed:
+                with lock:
+                    actor = model.__dict__.get("_tb_graphed_actor")
+                    if actor is None:
+                        actor = model._tb_graphed_actor = _acting.GraphedActor(model)
+                    host = _map_nest(_to_pinned_async, _net_outputs(actor(inputs, agent_state)))
+                    ready = torch.cuda.Event()
+                    ready.record()
+                ready.synchronize()
+                batch.set_outputs(host)
+                continue
             with lock:
                 outputs = model(inputs, agent_state)
-            if isinstance(outputs[0], dict):  # AtariNet returns a dict (monobeast.py:626-632): same tuple order as Net
-                o = outputs[0]
-                outputs = ((o["action"], o["policy_logits"], o["baseline"]), outputs[1])
+            outputs = _net_outputs(outputs)
             batch.set_outputs(_map_nest(lambda t: t.cpu(), outputs))
+
+
+def inference_graph_enabled(flags):
+    """The graphed inference forward is opt-in: flags.inference_graph (or TB_INFERENCE_GRAPH=1)."""
+    v = getattr(flags, "inference_graph", None)
+    if v is None:
+        v = os.environ.get("TB_INFERENCE_GRAPH", "0") not in ("0", "", "false")
+    return bool(v)
+
+
+def _net_outputs(outputs):
+    if isinstance(outputs[0], dict):  # AtariNet returns a dict (monobeast.py:626-632): same tuple order as Net
+        o = outputs[0]
+        outputs = ((o["action"], o["policy_logits"], o["baseline"]), outputs[1])
+    return outputs
+
+
+def _to_pinned_async(t):
+    """A fresh pinned host tensor receiving `t` by a copy enqueued on the current stream (the caching host allocator
+    does not hand the block out again while the copy is pending)."""
+    return torch.empty(t.shape, dtype=t.dtype, pin_memory=True).copy_(t, non_blocking=True)
 
 
 def _to_device(t, device):

@@ -22,7 +22,10 @@ class ActionSampler:
     a restored sampler continues the same sequence.
 
     Each `sample` call reads `step` on the host and passes it to the kernel by value, then advances it by T.  The call
-    is therefore not CUDA-graph safe: a captured launch would replay the same step forever.  Calls from several threads
+    itself is therefore not CUDA-graph safe: a captured launch would replay the same step forever.  To replay the acting
+    forward as a graph, use torchbeast_b200.acting.GraphedActor: it captures tb_sample_actions_dev_f32, which reads
+    (seed, step) from device memory, publishes this sampler's `seed` and `step` there before each replay and advances
+    `step` as an eager call does, so graphed and eager calls give one action sequence.  Calls from several threads
     must be serialised by the caller (polybeast_learner.inference already holds its lock around the forward)."""
 
     def __init__(self, seed, step=0):
