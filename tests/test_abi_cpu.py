@@ -56,3 +56,13 @@ def test_null_pointer_and_size_validation_host_side():
     # empty problems are a no-op success
     assert h.tb_vtrace_from_importance_weights_f32(None, None, None, None, None, 0, 4, 1.0, 1.0, None, None, None) == 0
     assert h.tb_action_log_probs_f32(None, None, 0, 6, None, None) == 0
+
+
+def test_cuda_sources_read_no_environment():
+    # the library chooses kernels from shapes alone: an environment switch would add a path no test runs, and could
+    # pair a forward with a backward (or a workspace size) chosen under a different setting
+    csrc = os.path.join(ROOT, "torchbeast_b200", "csrc")
+    sources = sorted(fn for fn in os.listdir(csrc) if fn.endswith((".cu", ".cuh")))
+    assert sources
+    offenders = [fn for fn in sources if "getenv" in open(os.path.join(csrc, fn)).read()]
+    assert not offenders, "getenv in %s" % ", ".join(offenders)

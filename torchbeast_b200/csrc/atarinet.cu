@@ -34,19 +34,16 @@ struct AtariGeom {
   static constexpr int KD3 = K3 * K3 * C2;  // 576
 };
 
-// Which convolutions run as implicit GEMMs (bf16 backend).  Decided ONCE per process (the environment switches are
-// read at the first call): the workspace layout depends on it - without patch matrices the conv-side buffers shrink
-// from 1.5 GB to 0.35 GB at N = 2592 - so forward, backward and tb_atarinet_workspace_bytes must agree.
-struct ImplicitPlan { bool conv1, conv2, conv3, dgrad2, dgrad3; };
-static const ImplicitPlan& implicit_plan() {
+// The tensor-core trunk runs every convolution as an implicit GEMM (no patch matrices); the fixed geometry must satisfy
+// all five kernels' shape predicates.
+static bool implicit_geometry_ok() {
   using G = AtariGeom;
-  static const ImplicitPlan p = {
-      conv_u8_implicit_applicable(G::C0, G::H0, G::W0, G::K1, G::K1, G::S1, G::C1),
-      conv_tc_implicit_applicable(G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2),
-      conv_tc_implicit_applicable(G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3),
-      conv_tc_dgrad_implicit_applicable(G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2),
-      conv_tc_dgrad_implicit_applicable(G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3)};
-  return p;
+  static const bool ok = conv_u8_implicit_applicable(G::C0, G::H0, G::W0, G::K1, G::K1, G::S1, G::C1) &&
+                         conv_tc_implicit_applicable(G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2) &&
+                         conv_tc_implicit_applicable(G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3) &&
+                         conv_tc_dgrad_implicit_applicable(G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2) &&
+                         conv_tc_dgrad_implicit_applicable(G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3);
+  return ok;
 }
 
 struct AtariParams {  // offsets (in floats) into the flat parameter / gradient buffers
@@ -96,8 +93,8 @@ struct AtariWs {  // bump-carved view of the caller's workspace
   float *dcore_out, *dcore_in, *dact3, *dcol3, *dact2, *dcol2, *dact1;
   float *splitk, *colsum_scratch;
   // tensor-core backends (precision 1: bf16, precision 2: split-bf16 hi/lo planes): operands / activations
-  HB col1b, act1b, col2b, act2b, col3b, act3b, w1b, w2b, w3b, wfcb;
-  HB dfcb, dact3b, dcol3b, dact2b, dcol2b, dact1b;
+  HB frameb, act1b, act2b, act3b, w1b, w2b, w3b, wfcb;
+  HB dfcb, dact3b, w3tb, dact2b, w2tb, dact1b;
   LstmWs lstm;
   size_t bytes;
 };
@@ -136,18 +133,15 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
     w.dact3 = takef(N * G::FC_IN); w.dcol3 = takef(M3 * G::KD3); w.dact2 = takef(M2 * G::C2);
     w.dcol2 = takef(M2 * G::KD2); w.dact1 = takef(M1 * G::C1);
   } else {
-    const ImplicitPlan& ip = implicit_plan();
-    // col1b: the bf16 frame image (implicit conv1) or the conv1 patch matrix; col2b/col3b exist only for the patch-matrix
-    // fallback; dcol2b/dcol3b hold the transposed weight packs of the implicit input gradients or the gradient matrices
-    // (the frame image / conv1 patch matrix holds integers <= 255: exact in bf16, no lo plane)
-    w.col1b = takeh(ip.conv1 ? N * G::C0 * G::H0 * G::W0 : M1 * G::KD1, false); w.act1b = takeh(M1 * G::C1);
-    w.col2b = takeh(ip.conv2 ? 8 : M2 * G::KD2); w.act2b = takeh(M2 * G::C2);
-    w.col3b = takeh(ip.conv3 ? 8 : M3 * G::KD3); w.act3b = takeh(N * G::FC_IN);
+    // frameb: the bf16 frame image conv1 gathers from (integers <= 255: exact in bf16, no lo plane); w2tb/w3tb: the
+    // transposed weight packs of the input-gradient convolutions
+    w.frameb = takeh(N * G::C0 * G::H0 * G::W0, false); w.act1b = takeh(M1 * G::C1);
+    w.act2b = takeh(M2 * G::C2); w.act3b = takeh(N * G::FC_IN);
     w.w1b = takeh(int64_t(G::C1) * G::KD1); w.w2b = takeh(int64_t(G::C2) * G::KD2); w.w3b = takeh(int64_t(G::C3) * G::KD3);
     w.wfcb = takeh(int64_t(G::FC_OUT) * G::FC_IN);
     w.dfcb = takeh(N * G::FC_OUT); w.dact3b = takeh(N * G::FC_IN);
-    w.dcol3b = takeh(ip.dgrad3 ? int64_t(G::C2) * G::KD3 : M3 * G::KD3);
-    w.dact2b = takeh(M2 * G::C2); w.dcol2b = takeh(ip.dgrad2 ? int64_t(4) * G::C1 * G::KD2 : M2 * G::KD2);
+    w.w3tb = takeh(int64_t(G::C2) * G::KD3);
+    w.dact2b = takeh(M2 * G::C2); w.w2tb = takeh(int64_t(4) * G::C1 * G::KD2);
     w.dact1b = takeh(M1 * G::C1);
   }
   w.splitk = takef(kSplitKScratchFloats);
@@ -196,9 +190,7 @@ static int atarinet_forward(const uint8_t* frame, const float* reward, const flo
   GemmEpilogue ep;
   if (precision) {
     // ---- tensor-core trunk: wgmma GEMMs, bf16 (precision 1) or split-bf16 hi/lo (precision 2) activations, fp32 accumulation
-    const bool split = precision == 2;
-    TB_REQUIRE(!split || (implicit_plan().conv1 && implicit_plan().conv2 && implicit_plan().conv3),
-               "atarinet_forward: the split-bf16 backend needs the implicit-GEMM convolutions (TB_CONV*_IMPLICIT=0 set?)");
+    TB_REQUIRE(implicit_geometry_ok(), "atarinet_forward: the trunk geometry does not fit the implicit-GEMM convolutions");
     TB_TRY(pack_weights_bf16(P + pp.conv1_w, w.w1b, G::C1, 1, G::KD1, G::KD1, st, w.w1b.lo));
     TB_TRY(pack_weights_bf16(P + pp.conv2_w, w.w2b, G::C2, G::K2 * G::K2, G::C1, G::KD2, st, w.w2b.lo));
     TB_TRY(pack_weights_bf16(P + pp.conv3_w, w.w3b, G::C3, G::K3 * G::K3, G::C2, G::KD3, st, w.w3b.lo));
@@ -206,35 +198,19 @@ static int atarinet_forward(const uint8_t* frame, const float* reward, const flo
     TcEpilogue te;
     te = TcEpilogue(); te.C16 = w.act1b.h(); te.ldc16 = G::C1; te.c16_lo = w.act1b.lo; te.bias = P + pp.conv1_b;
     te.scale = 1.0f / 255.0f; te.relu = 1; te.tag = "conv1_fwd";
-    if (implicit_plan().conv1) {
-      // implicit GEMM: frames -> bf16 image once (kept in col1b for the backward), producer warps gather the
-      // patches from it into the UMMA smem layout
-      te.b_lo = w.w1b.lo;  // the pixels are exact in bf16: only the weights have a lo plane
-      TB_TRY(frames_u8_to_bf16(frame, w.col1b, N * G::C0 * G::H0 * G::W0, st));
-      TB_TRY(conv_u8_fwd_implicit(w.col1b, w.w1b, N, G::H0, G::W0, G::S1, te, st));
-    } else {
-      TB_TRY(im2col_u8_nchw_bf16(frame, w.col1b, N, G::C0, G::H0, G::W0, G::K1, G::K1, G::S1, st));
-      TB_TRY(gemm_tc_bf16(w.col1b, w.w1b, M1, G::C1, G::KD1, G::KD1, G::KD1, te, st));
-    }
+    // implicit GEMM: frames -> bf16 image once (kept in frameb for the backward), producer warps gather the
+    // patches from it into the UMMA smem layout
+    te.b_lo = w.w1b.lo;  // the pixels are exact in bf16: only the weights have a lo plane
+    TB_TRY(frames_u8_to_bf16(frame, w.frameb, N * G::C0 * G::H0 * G::W0, st));
+    TB_TRY(conv_u8_fwd_implicit(w.frameb, w.w1b, N, G::H0, G::W0, G::S1, te, st));
     // conv2 / conv3: implicit GEMM - TMA gathers the patches from the NHWC activation (rank-4 map with
-    // overlapping dimensions); the patch matrices col2b / col3b are only materialised for the backward
-    const bool impl2 = implicit_plan().conv2, impl3 = implicit_plan().conv3;
+    // overlapping dimensions)
     te = TcEpilogue(); te.C16 = w.act2b.h(); te.ldc16 = G::C2; te.c16_lo = w.act2b.lo; te.bias = P + pp.conv2_b;
     te.relu = 1; te.tag = "conv2_fwd"; te.a_lo = w.act1b.lo; te.b_lo = w.w2b.lo;
-    if (impl2) {
-      TB_TRY(conv_tc_fwd_implicit(w.act1b, w.w2b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, te, st));
-    } else {
-      TB_TRY(im2col_bf16_nhwc(w.act1b, w.col2b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, st));
-      TB_TRY(gemm_tc_bf16(w.col2b, w.w2b, M2, G::C2, G::KD2, G::KD2, G::KD2, te, st));
-    }
+    TB_TRY(conv_tc_fwd_implicit(w.act1b, w.w2b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, te, st));
     te = TcEpilogue(); te.C16 = w.act3b.h(); te.ldc16 = G::C3; te.c16_lo = w.act3b.lo; te.bias = P + pp.conv3_b;
     te.relu = 1; te.tag = "conv3_fwd"; te.a_lo = w.act2b.lo; te.b_lo = w.w3b.lo;
-    if (impl3) {
-      TB_TRY(conv_tc_fwd_implicit(w.act2b, w.w3b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, te, st));
-    } else {
-      TB_TRY(im2col_bf16_nhwc(w.act2b, w.col3b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, st));
-      TB_TRY(gemm_tc_bf16(w.col3b, w.w3b, M3, G::C3, G::KD3, G::KD3, G::KD3, te, st));
-    }
+    TB_TRY(conv_tc_fwd_implicit(w.act2b, w.w3b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, te, st));
     te = TcEpilogue(); te.C = w.core_in; te.ldc = pp.core; te.bias = P + pp.fc_b; te.relu = 1; te.tag = "fc_fwd";
     te.a_lo = w.act3b.lo; te.b_lo = w.wfcb.lo;
     TB_TRY(gemm_tc_bf16(w.act3b, w.wfcb, N, G::FC_OUT, G::FC_IN, G::FC_IN, G::FC_IN, te, st));
@@ -334,60 +310,30 @@ static int atarinet_backward_trunk_bf16(const float* P, float* G_, const AtariPa
   te = TcEpilogue(); te.C16 = w.dact3b.h(); te.ldc16 = G::FC_IN; te.c16_lo = w.dact3b.lo;
   te.mask16 = w.act3b.h(); te.ldmask = G::FC_IN; te.tag = "fc_dgrad"; te.a_lo = w.dfcb.lo; te.b_lo = w.wfcb.lo;
   TB_TRY(gemm_tc_bf16_ex(w.dfcb, w.wfcb, N, G::FC_IN, G::FC_OUT, G::FC_OUT, G::FC_IN, false, true, te, 1, nullptr, st));
-  // conv3 (dact3b viewed as [M3, 64]); the implicit forward did not leave a patch matrix behind
-  if (implicit_plan().conv3) {
-    TB_TRY(conv_tc_wgrad_implicit(w.dact3b, w.act2b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, G_ + pp.conv3_w,
-                                  G::K3 * G::K3, G::C2, 1.0f, w.splitk, kSplitKScratchFloats, "conv3_wgrad", st, w.dact3b.lo,
-                                  w.act2b.lo));
-  } else {
-    TB_TRY(tc_wgrad(w.dact3b, G::C3, w.col3b, G::KD3, G_ + pp.conv3_w, M3, G::C3, G::KD3, G::K3 * G::K3, G::C2, 1.0f, w, st,
-                    "conv3_wgrad"));
-  }
+  // conv3 (dact3b viewed as [M3, 64]); the weight gradients gather their patches from the activations
+  TB_TRY(conv_tc_wgrad_implicit(w.dact3b, w.act2b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, G_ + pp.conv3_w,
+                                G::K3 * G::K3, G::C2, 1.0f, w.splitk, kSplitKScratchFloats, "conv3_wgrad", st, w.dact3b.lo,
+                                w.act2b.lo));
   TB_TRY(colsum_bf16(w.dact3b, G_ + pp.conv3_b, M3, G::C3, G::C3, w.colsum_scratch, st, w.dact3b.lo));
-  if (implicit_plan().dgrad3) {
-    // gather-form transposed convolution on tensor cores: dY boxes through TMA (zero fill = padding), ReLU mask in the
-    // epilogue; the transposed weight pack lives in the (otherwise unused) dcol3b buffer
-    TB_TRY(pack_dgrad_weights_bf16(P + pp.conv3_w, w.dcol3b, G::C3, G::C2, G::K3, G::K3, G::S3, st, w.dcol3b.lo));
-    te = TcEpilogue(); te.C16 = w.dact2b.h(); te.ldc16 = G::C2; te.c16_lo = w.dact2b.lo;
-    te.mask16 = w.act2b.h(); te.ldmask = G::C2; te.tag = "conv3_dgrad"; te.a_lo = w.dact3b.lo; te.b_lo = w.dcol3b.lo;
-    TB_TRY(conv_tc_dgrad_implicit(w.dact3b, w.dcol3b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, te, st));
-  } else {
-    TB_REQUIRE(!w.dact3b.lo, "atarinet_backward: split-bf16 needs the implicit input-gradient convolutions");
-    te = TcEpilogue(); te.C16 = w.dcol3b.h(); te.ldc16 = G::KD3; te.tag = "conv3_dgrad";
-    TB_TRY(gemm_tc_bf16_ex(w.dact3b, w.w3b, M3, G::KD3, G::C3, G::C3, G::KD3, false, true, te, 1, nullptr, st));
-    TB_TRY(col2im_bf16_nhwc(w.dcol3b, w.act2b, w.dact2b, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, st));
-  }
+  // gather-form transposed convolution on tensor cores: dY boxes through TMA (zero fill = padding), ReLU mask in the
+  // epilogue
+  TB_TRY(pack_dgrad_weights_bf16(P + pp.conv3_w, w.w3tb, G::C3, G::C2, G::K3, G::K3, G::S3, st, w.w3tb.lo));
+  te = TcEpilogue(); te.C16 = w.dact2b.h(); te.ldc16 = G::C2; te.c16_lo = w.dact2b.lo;
+  te.mask16 = w.act2b.h(); te.ldmask = G::C2; te.tag = "conv3_dgrad"; te.a_lo = w.dact3b.lo; te.b_lo = w.w3tb.lo;
+  TB_TRY(conv_tc_dgrad_implicit(w.dact3b, w.w3tb, N, G::H2, G::W2, G::C2, G::K3, G::K3, G::S3, G::C3, te, st));
   // conv2
-  if (implicit_plan().conv2) {
-    TB_TRY(conv_tc_wgrad_implicit(w.dact2b, w.act1b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, G_ + pp.conv2_w,
-                                  G::K2 * G::K2, G::C1, 1.0f, w.splitk, kSplitKScratchFloats, "conv2_wgrad", st, w.dact2b.lo,
-                                  w.act1b.lo));
-  } else {
-    TB_TRY(tc_wgrad(w.dact2b, G::C2, w.col2b, G::KD2, G_ + pp.conv2_w, M2, G::C2, G::KD2, G::K2 * G::K2, G::C1, 1.0f, w, st,
-                    "conv2_wgrad"));
-  }
+  TB_TRY(conv_tc_wgrad_implicit(w.dact2b, w.act1b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, G_ + pp.conv2_w,
+                                G::K2 * G::K2, G::C1, 1.0f, w.splitk, kSplitKScratchFloats, "conv2_wgrad", st, w.dact2b.lo,
+                                w.act1b.lo));
   TB_TRY(colsum_bf16(w.dact2b, G_ + pp.conv2_b, M2, G::C2, G::C2, w.colsum_scratch, st, w.dact2b.lo));
-  if (implicit_plan().dgrad2) {
-    TB_TRY(pack_dgrad_weights_bf16(P + pp.conv2_w, w.dcol2b, G::C2, G::C1, G::K2, G::K2, G::S2, st, w.dcol2b.lo));
-    te = TcEpilogue(); te.C16 = w.dact1b.h(); te.ldc16 = G::C1; te.c16_lo = w.dact1b.lo;
-    te.mask16 = w.act1b.h(); te.ldmask = G::C1; te.tag = "conv2_dgrad"; te.a_lo = w.dact2b.lo; te.b_lo = w.dcol2b.lo;
-    TB_TRY(conv_tc_dgrad_implicit(w.dact2b, w.dcol2b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, te, st));
-  } else {
-    TB_REQUIRE(!w.dact2b.lo, "atarinet_backward: split-bf16 needs the implicit input-gradient convolutions");
-    te = TcEpilogue(); te.C16 = w.dcol2b.h(); te.ldc16 = G::KD2; te.tag = "conv2_dgrad";
-    TB_TRY(gemm_tc_bf16_ex(w.dact2b, w.w2b, M2, G::KD2, G::C2, G::C2, G::KD2, false, true, te, 1, nullptr, st));
-    TB_TRY(col2im_bf16_nhwc(w.dcol2b, w.act1b, w.dact1b, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, st));
-  }
-  // conv1: the patch matrix holds raw pixel values, so the weight gradient carries the 1/255
-  if (implicit_plan().conv1) {
-    // w.col1b holds the bf16 frame image the forward left there (not a patch matrix)
-    TB_TRY(conv_u8_wgrad_implicit(w.dact1b, w.col1b, N, G::H0, G::W0, G::S1, G_ + pp.conv1_w, 1.0f / 255.0f, w.splitk,
-                                  kSplitKScratchFloats, "conv1_wgrad", st, w.dact1b.lo));
-  } else {
-    TB_REQUIRE(!w.dact1b.lo, "atarinet_backward: split-bf16 needs the implicit conv1");
-    TB_TRY(tc_wgrad(w.dact1b, G::C1, w.col1b, G::KD1, G_ + pp.conv1_w, M1, G::C1, G::KD1, 1, 1, 1.0f / 255.0f, w, st,
-                    "conv1_wgrad"));
-  }
+  TB_TRY(pack_dgrad_weights_bf16(P + pp.conv2_w, w.w2tb, G::C2, G::C1, G::K2, G::K2, G::S2, st, w.w2tb.lo));
+  te = TcEpilogue(); te.C16 = w.dact1b.h(); te.ldc16 = G::C1; te.c16_lo = w.dact1b.lo;
+  te.mask16 = w.act1b.h(); te.ldmask = G::C1; te.tag = "conv2_dgrad"; te.a_lo = w.dact2b.lo; te.b_lo = w.w2tb.lo;
+  TB_TRY(conv_tc_dgrad_implicit(w.dact2b, w.w2tb, N, G::H1, G::W1, G::C1, G::K2, G::K2, G::S2, G::C2, te, st));
+  // conv1: frameb holds the bf16 frame image the forward left there (raw pixel values), so the weight gradient carries
+  // the 1/255
+  TB_TRY(conv_u8_wgrad_implicit(w.dact1b, w.frameb, N, G::H0, G::W0, G::S1, G_ + pp.conv1_w, 1.0f / 255.0f, w.splitk,
+                                kSplitKScratchFloats, "conv1_wgrad", st, w.dact1b.lo));
   TB_TRY(colsum_bf16(w.dact1b, G_ + pp.conv1_b, M1, G::C1, G::C1, w.colsum_scratch, st, w.dact1b.lo));
   return 0;
 }

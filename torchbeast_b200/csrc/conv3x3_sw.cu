@@ -823,8 +823,6 @@ int sw_pack_weights(const float* w, __nv_bfloat16* out, int O, int C, int transp
 }
 
 bool sw_conv_applicable(int H, int W, int CK, int NO) {
-  const char* e = getenv("TB_RESNET_IMPLICIT");
-  if (e && e[0] == '0') return false;
   return (CK == 16 || CK == 32) && (NO == 16 || NO == 32) && H >= 3 && W >= 3 && W <= 126;
 }
 

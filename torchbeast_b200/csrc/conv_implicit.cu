@@ -394,8 +394,6 @@ int frames_u8_to_bf16(const uint8_t* frame, void* frame_bf16, int64_t count, cud
 }
 
 bool conv_u8_implicit_applicable(int C, int H, int W, int KH, int KW, int S, int O) {
-  const char* e = getenv("TB_CONV1_IMPLICIT");
-  if (e && e[0] == '0') return false;
   if (!(C == kC && KH == 8 && KW == 8 && O == kO && (W % 4) == 0 && (S % 4) == 0 && H >= 8 && W >= 8)) return false;
   const ConvGeom g = make_geom(1, H, W, S);
   if (g.per > 4096) return false;

@@ -5,7 +5,7 @@
 namespace tb {
 
 // true when the wgmma implicit-GEMM kernels cover this shape (8x8 kernel, 4 input / 32 output channels,
-// W and stride multiples of 4) and TB_CONV1_IMPLICIT != 0
+// W and stride multiples of 4)
 bool conv_u8_implicit_applicable(int C, int H, int W, int KH, int KW, int S, int O);
 
 // frames u8 NCHW -> bf16 NCHW (exact), the operand image of the two kernels below

@@ -668,8 +668,6 @@ int launch_conv_fwd(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N
 }  // namespace
 
 bool conv_tc_implicit_applicable(int H, int W, int C, int KH, int KW, int S, int O) {
-  const char* e = getenv("TB_CONV_IMPLICIT");
-  if (e && e[0] == '0') return false;
   if (H < KH || W < KW || S < 1) return false;
   const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
   return (KW * C) % kBlockK == 0 && (S * C * 2) % 16 == 0 && (C % 8) == 0 && OW * OH <= kBlockM && OW <= 256 && OH <= 256 &&
@@ -714,8 +712,6 @@ int conv_tc_fwd_implicit(const void* act_nhwc_bf16, const void* w_packed_bf16, i
 }
 
 bool conv_tc_dgrad_implicit_applicable(int H, int W, int C, int KH, int KW, int S, int O) {
-  const char* e = getenv("TB_CONV_IMPLICIT");
-  if (e && e[0] == '0') return false;
   if (O != 64 || H < KH || W < KW) return false;
   const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
   if (S == 1) return H * W <= kBlockM && (C == 32 || C == 64 || C == 128) && (OH - 1) + KH == H && (OW - 1) + KW == W;

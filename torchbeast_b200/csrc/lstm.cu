@@ -702,45 +702,52 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_kernel(Persi
   }
 }
 
-// returns 0 = ran, -1 = not applicable (caller falls back to the per-step kernels), > 0 = error
-static int persistent_ok(const void* kernel, dim3 grid, size_t smem) {
+// 1 if the whole grid of `kernel` (blocks of `threads`, `smem` bytes of dynamic shared memory) is co-resident on the
+// current device, as a cooperative launch needs; 0 otherwise
+static int persistent_ok(const void* kernel, dim3 grid, int threads, size_t smem) {
   int dev = 0, sms = 0, coop = 0, per_sm = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
   if (!coop) return 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kStepThreads, smem) != cudaSuccess) {
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
   return int64_t(per_sm) * sms >= int64_t(grid.x) * grid.y;
 }
 
-static bool persistent_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TB_LSTM_PERSISTENT");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
+// cudaFuncSetAttribute is per device: the attribute caches are indexed by the current device
+static inline size_t* per_device(size_t (&cache)[64]) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  return &cache[dev & 63];
 }
+
+// raises the kernel's dynamic shared-memory limit to `smem` (once per device; *attr_smem caches the limit already set),
+// then checks co-residency.  0: the kernel cannot run as one cooperative grid here
+template <typename Kernel>
+static int coop_fit(Kernel kernel, dim3 grid, size_t smem, int threads, size_t* attr_smem) {
+  if (*attr_smem < smem) {
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
+      cudaGetLastError();
+      return 0;
+    }
+    *attr_smem = smem;
+  }
+  return persistent_ok((const void*)kernel, grid, threads, smem);
+}
+
+static size_t g_fwd_persist_attr_dev[64] = {0}, g_bwd_persist_attr_dev[64] = {0};
 
 static int lstm_fwd_persistent(const LstmLayerWs& L, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
                                unsigned* counter, cudaStream_t st) {
-  if (!persistent_enabled() || B > 64) return -1;
+  if (B > 64) return -1;
   const int Hp = padded_h(H);
   const size_t smem = size_t(48) * Hp * sizeof(float) + 16;
   if (smem > 200 * 1024) return -1;
-  static size_t attr_smem = 0;
-  if (attr_smem < smem) {
-    if (cudaFuncSetAttribute(lstm_fwd_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();  // not applicable on this device: clear and fall back
-      return -1;
-    }
-    attr_smem = smem;
-  }
   dim3 grid((H + kStepUnits - 1) / kStepUnits, (unsigned)((B + 31) / 32));
-  if (!persistent_ok((const void*)lstm_fwd_persistent_kernel, grid, smem)) return -1;
+  if (!coop_fit(lstm_fwd_persistent_kernel, grid, smem, kStepThreads, per_device(g_fwd_persist_attr_dev))) return -1;
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   PersistFwdArgs a;
@@ -754,20 +761,12 @@ static int lstm_fwd_persistent(const LstmLayerWs& L, float* hs, const float* not
 
 static int lstm_bwd_persistent(const LstmLayerWs& L, const LstmWs& ws, const float* dy, const float* notdone, int64_t T1,
                                int64_t B, int H, unsigned* counter, cudaStream_t st) {
-  if (!persistent_enabled() || B > 32) return -1;
+  if (B > 32) return -1;
   const int Hp = padded_h(H);
   const size_t smem = size_t(80) * Hp * sizeof(float) + 32;
   if (smem > 220 * 1024) return -1;
-  static size_t attr_smem = 0;
-  if (attr_smem < smem) {
-    if (cudaFuncSetAttribute(lstm_bwd_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();
-      return -1;
-    }
-    attr_smem = smem;
-  }
   dim3 grid((H + 3) / 4, 1);
-  if (!persistent_ok((const void*)lstm_bwd_persistent_kernel, grid, smem)) return -1;
+  if (!coop_fit(lstm_bwd_persistent_kernel, grid, smem, kStepThreads, per_device(g_bwd_persist_attr_dev))) return -1;
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(ws.dgp, 0, sizeof(float) * 2 * 4 * B * Hp, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
@@ -1599,11 +1598,6 @@ constexpr int kSplitWarps = 11;
 constexpr int kSplitThreads = kSplitWarps * 32;
 constexpr int kSplitK = 3;  // k16 steps per warp
 
-// Debug timeline (TB_LSTM_TRACE=<file>): thread 0 of every CTA stamps clock64() at the phase boundaries of every wave step
-// into a device buffer that the launcher dumps after the kernel (synchronising - never enabled in production runs).
-constexpr int kTracePhases = 8;
-#define TB_TRACE(ph) do { if (a.trace && tid == 0) a.trace[(int64_t(blockIdx.x) * (a.T1 + 2) + s) * kTracePhases + (ph)] = clock64(); } while (0)
-
 struct WaveFwdSplitArgs {
   const float* w_hh0; const float* w_ih1; const float* w_hh1; const float* bias1;
   const float* c0;          // [2, B, H] initial cell state
@@ -1620,7 +1614,6 @@ struct WaveFwdSplitArgs {
   int64_t hq_lo, hmq_lo;
   const float* nd; unsigned* flags;
   int T1, B, H, Hq; unsigned nctas;
-  long long* trace;
 };
 
 __device__ __forceinline__ void split_pack(float v0, float v1, uint32_t& hi, uint32_t& lo) {
@@ -1697,7 +1690,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
   if (updthread) csb_u[int64_t(blockIdx.x) * 128 + (tid & 127)] = c_state;    // slot 0
   for (int s = 0; s <= a.T1; ++s) {
     const bool act0 = (s < a.T1), act1 = (s >= 1);
-    TB_TRACE(0);
     // inputs that do not depend on other CTAs: issued before the wait
     float preA = 0.f, preB = 0.f;
     if (act0) {
@@ -1726,7 +1718,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       }
       __syncwarp();
     }
-    TB_TRACE(1);
     float m0[2][2], m1[2][2];   // done masks of this thread's accumulator rows (layer 0 at t = s, layer 1 at t = s-1)
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt)
@@ -1770,7 +1761,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
           for (int e = 0; e < 4; ++e) { acc0[mt][nt][e] = 0.f; accI[mt][nt][e] = 0.f; acc1[mt][nt][e] = 0.f; }
       asm volatile("cp.async.wait_group 1;" ::: "memory");   // the h0 planes
       __syncwarp();
-      TB_TRACE(2);
 #pragma unroll
       for (int sk = 0; sk < kSplitK; ++sk) {
         if (ks0 + sk < ksteps) {
@@ -1793,7 +1783,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       }
       asm volatile("cp.async.wait_group 0;" ::: "memory");   // the h1 planes
       __syncwarp();
-      TB_TRACE(3);
       if (act1) {
 #pragma unroll
         for (int sk = 0; sk < kSplitK; ++sk) {
@@ -1826,9 +1815,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
         }
       }
     }
-    TB_TRACE(4);
     __syncthreads();
-    TB_TRACE(5);
     float g0A = 0.f, g0B = 0.f, g1A = 0.f, g1B = 0.f;
     if (actrole) {
       float d0A = 0.f, d0B = 0.f, d1A = 0.f, d1B = 0.f;
@@ -1873,12 +1860,10 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       }
     }
     __syncthreads();
-    TB_TRACE(6);
     if (tid == 0 && s < a.T1) {
       asm volatile("fence.acq_rel.gpu;" ::: "memory");
       st_relaxed_u32(a.flags + blockIdx.x * kFlagStride, unsigned(s + 1));
     }
-    TB_TRACE(7);
     // ---- everything below is consumed by this CTA or after the kernel: off the critical path ----
     // activated gates -> CTA-blocked [row][16] tiles, straight from act_s (rewritten only after the next step's barrier)
     for (int idx = tid; idx < 1024; idx += kSplitThreads) {
@@ -1937,7 +1922,6 @@ struct WaveBwdSplitArgs {
   float* dxb;                       // dL/dh_lower, blocked [T1][nc][32 rows][8 cols]: upper role -> lower role
   unsigned* flags;                  // [2 * nc]
   int T1, B, H, Hq; unsigned nc;
-  long long* trace;
 };
 
 __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(WaveBwdSplitArgs a) {
@@ -2060,7 +2044,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     const int64_t row0 = int64_t(active ? t : 0) * B;
     __nv_bfloat16* dgq_t = dgq + int64_t(it & 1) * 4 * gs;
     float p_i = 0.f, p_f = 0.f, p_g = 0.f, p_o = 0.f;
-    TB_TRACE(0);
     if (active) {
       if (actA) {   // (the prefetched operands were waited for, and made visible by the barrier, at the end of the previous step)
         const int gb = (q >> 2) * 512 + lane * 16 + (q & 3), cb = (q >> 2) * 128 + lane * 4 + (q & 3);
@@ -2105,12 +2088,10 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
       break;
     }
     __syncthreads();
-    TB_TRACE(1);
     if (tid == 0) {  // this CTA's tile columns of wave step s (and, upper role, its dxm of step s-1) are out
       asm volatile("fence.acq_rel.gpu;" ::: "memory");
       st_relaxed_u32(my_flag, unsigned(s + 1));
     }
-    TB_TRACE(2);
     if (active) store_dg(row0);
     prefetch(time_of(s + 1));  // forward-pass operands only: overlaps the wait
     // hand-off: this warp needs the tile columns of units [16*ks0, 16*ks0 + 48) -> the 6 CTAs of its own role that own
@@ -2127,7 +2108,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
       }
       __syncwarp();
     }
-    TB_TRACE(3);
     fetch_dxm(time_of(s + 1));  // written by the upper role before it published wave step s
     const bool need_rec = active && t > 0;
     const bool need_dx = active && upper;
@@ -2175,9 +2155,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         }
         __syncwarp();
         if (g + 2 < 4) issue(g + 2);
-        if (g == 0) TB_TRACE(4);
       }
-      TB_TRACE(5);
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         const int r = mt * 16 + (lane >> 2), c = (lane & 3) * 2;
@@ -2204,7 +2182,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");   // next step's prefetched pointwise operands (all threads' copies)
     __syncthreads();
-    TB_TRACE(6);
     if (active) ++it;
   }
   if (wrp < kBwdCols) {
@@ -2216,37 +2193,16 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   }
 }
 
-// cudaFuncSetAttribute is per device: the caches below are indexed by the current device (ADVICE r1)
-static inline size_t* per_device(size_t (&cache)[64]) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return &cache[dev & 63];
-}
-
-template <typename Kernel>
-static int coop_fit(Kernel kernel, dim3 grid, size_t smem, size_t* attr_smem) {
-  if (*attr_smem < smem) {
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();
-      return 0;
-    }
-    *attr_smem = smem;
-  }
-  return persistent_ok((const void*)kernel, grid, smem);
-}
-
 static size_t g_fwd_mma_attr_dev[64] = {0}, g_bwd_mma_attr_dev[64] = {0};
 
 // one decision for a (B, H) pair, used identically by forward and backward (the backward consumes the bf16
 // masked-h buffer only the tensor-core forward writes)
 static bool mma_recurrence_applicable(int64_t B, int H) {
-  const char* e = getenv("TB_LSTM_MMA");
-  if (e && e[0] == '0') return false;
-  if (!persistent_enabled() || B > 32 || H > 624) return false;  // tile copy: <= 5 x 16 B chunks per thread
+  if (B > 32 || H > 624) return false;  // tile copy: <= 5 x 16 B chunks per thread
   const int Hq = mma_hq(H);
   dim3 grid((H + kStepUnits - 1) / kStepUnits, 1), gridb((H + kBwdCols - 1) / kBwdCols, 1);
-  return coop_fit(lstm_fwd_persistent_mma_kernel, grid, size_t(32) * Hq * 2, per_device(g_fwd_mma_attr_dev)) &&
-         coop_fit(lstm_bwd_persistent_mma_kernel, gridb, size_t(4) * 32 * Hq * 2, per_device(g_bwd_mma_attr_dev));
+  return coop_fit(lstm_fwd_persistent_mma_kernel, grid, size_t(32) * Hq * 2, kStepThreads, per_device(g_fwd_mma_attr_dev)) &&
+         coop_fit(lstm_bwd_persistent_mma_kernel, gridb, size_t(4) * 32 * Hq * 2, kStepThreads, per_device(g_bwd_mma_attr_dev));
 }
 
 static int lstm_fwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, float* hs, const float* notdone, int64_t T1,
@@ -2254,7 +2210,7 @@ static int lstm_fwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, floa
   const int Hq = mma_hq(H);
   const size_t smem = size_t(32) * Hq * 2;
   dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
-  if (!coop_fit(lstm_fwd_persistent_mma_kernel, grid, smem, per_device(g_fwd_mma_attr_dev))) return -1;
+  if (!coop_fit(lstm_fwd_persistent_mma_kernel, grid, smem, kStepThreads, per_device(g_fwd_mma_attr_dev))) return -1;
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   PersistFwdMmaArgs a;
@@ -2270,12 +2226,10 @@ static int lstm_fwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, floa
 static size_t g_fwd_wave_attr_dev[64] = {0};
 static size_t wave_fwd_smem(int Hq) { return size_t(2) * 32 * Hq * 2 + sizeof(float) * 16 * 2 * 16 * 33; }
 static bool wave_fwd_applicable(int64_t B, int H) {
-  const char* e = getenv("TB_LSTM_WAVE");
-  if (e && e[0] == '0') return false;
   if (!mma_recurrence_applicable(B, H)) return false;
   if (((H + 15) / 16 + 15) / 16 > kWaveK) return false;
   dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
-  return coop_fit(lstm2_fwd_wave_mma_kernel, grid, wave_fwd_smem(mma_hq(H)), per_device(g_fwd_wave_attr_dev));
+  return coop_fit(lstm2_fwd_wave_mma_kernel, grid, wave_fwd_smem(mma_hq(H)), kStepThreads, per_device(g_fwd_wave_attr_dev));
 }
 
 static int lstm2_fwd_wave(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, int64_t T1, int64_t B, int H,
@@ -2300,33 +2254,6 @@ static int lstm2_fwd_wave(LstmWs& ws, const LstmParams& p, float* y, const float
   return check_launch("lstm2_fwd_wave_mma_kernel");
 }
 
-static long long* trace_buffer(unsigned ctas, int T1) {
-  static const char* path = getenv("TB_LSTM_TRACE");
-  if (!path) return nullptr;
-  long long* p = nullptr;
-  const size_t n = size_t(ctas) * (T1 + 2) * kTracePhases;
-  if (cudaMalloc(&p, n * sizeof(long long)) != cudaSuccess) return nullptr;
-  cudaMemset(p, 0, n * sizeof(long long));
-  return p;
-}
-static void trace_dump(const char* tag, long long* dev, unsigned ctas, int T1, cudaStream_t st) {
-  if (!dev) return;
-  const size_t n = size_t(ctas) * (T1 + 2) * kTracePhases;
-  long long* h = static_cast<long long*>(malloc(n * sizeof(long long)));
-  cudaStreamSynchronize(st);
-  cudaMemcpy(h, dev, n * sizeof(long long), cudaMemcpyDeviceToHost);
-  char name[512];
-  snprintf(name, sizeof(name), "%s.%s", getenv("TB_LSTM_TRACE"), tag);
-  if (FILE* f = fopen(name, "wb")) {
-    const int hdr[4] = {int(ctas), T1 + 2, kTracePhases, 0};
-    fwrite(hdr, sizeof(hdr), 1, f);
-    fwrite(h, sizeof(long long), n, f);
-    fclose(f);
-  }
-  free(h);
-  cudaFree(dev);
-}
-
 // slot 0 of the split recurrence's planes: hq = split(h0) (raw), hmq = split(h0 * nd_0); row padding zero
 __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const float* __restrict__ nd,
                                              __nv_bfloat16* __restrict__ hq, int64_t hq_lo, __nv_bfloat16* __restrict__ hmq,
@@ -2344,31 +2271,13 @@ __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const
 
 static size_t g_fwd_split_attr_dev[64] = {0};
 static size_t wave_fwd_split_smem(int Hq) { return size_t(4) * 32 * Hq * 2 + sizeof(float) * kSplitWarps * 2 * 16 * 33; }
-// precision 2, two layers: the split-bf16 wavefront kernel (TB_LSTM_SPLIT=0 keeps the exact-fp32 recurrence kernels)
+// precision 2, two layers: the split-bf16 wavefront kernel (other shapes run the exact-fp32 recurrence kernels)
 static bool wave_fwd_split_applicable(int64_t B, int In, int H) {
-  const char* e = getenv("TB_LSTM_SPLIT");
-  if (e && e[0] == '0') return false;
-  if (!persistent_enabled() || B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
+  if (B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
   dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
   if (int(grid.x) > kSplitThreads || grid.x > 512) return false;
-  if (*per_device(g_fwd_split_attr_dev) < wave_fwd_split_smem(mma_hq(H))) {
-    if (cudaFuncSetAttribute(lstm2_fwd_wave_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             int(wave_fwd_split_smem(mma_hq(H)))) != cudaSuccess) {
-      cudaGetLastError();
-      return false;
-    }
-    *per_device(g_fwd_split_attr_dev) = wave_fwd_split_smem(mma_hq(H));
-  }
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return false;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm2_fwd_wave_split_kernel, kSplitThreads,
-                                                             wave_fwd_split_smem(mma_hq(H))) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return int64_t(per_sm) * sms >= int64_t(grid.x);
+  return coop_fit(lstm2_fwd_wave_split_kernel, grid, wave_fwd_split_smem(mma_hq(H)), kSplitThreads,
+                  per_device(g_fwd_split_attr_dev));
 }
 
 static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, const float* c0, float* hN,
@@ -2390,12 +2299,10 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
   TB_REQUIRE(ws.layer[1].hq_lo == a.hq_lo && ws.layer[1].hmq_lo == a.hmq_lo && a.hq_lo > 0, "lstm: split planes missing");
   a.nd = notdone; a.flags = ws.flags;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = grid.x;
-  a.trace = trace_buffer(grid.x, int(T1));
   void* args[] = {&a};
   e = cudaLaunchCooperativeKernel((const void*)lstm2_fwd_wave_split_kernel, grid, dim3(kSplitThreads), args,
                                   wave_fwd_split_smem(Hq), st);
   TB_REQUIRE(e == cudaSuccess, "lstm2_fwd_wave_split_kernel: %s", cudaGetErrorString(e));
-  trace_dump("fwd", a.trace, grid.x, int(T1), st);
   return check_launch("lstm2_fwd_wave_split_kernel");
 }
 
@@ -2563,8 +2470,7 @@ static size_t cluster_fwd_smem(int MT) {
 
 static int lstm_fwd_cluster(const LstmLayerWs& L, const float* w_hh, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
                             cudaStream_t st) {
-  const char* env = getenv("TB_LSTM_CLUSTER");
-  if ((env && env[0] == '0') || H != kClH || B > 32 || B < 1) return -1;
+  if (H != kClH || B > 32 || B < 1) return -1;
   static int attr_ok[64] = {0};   // per device: 0 unknown, 1 ok, -1 unavailable
   int dev = 0;
   cudaGetDevice(&dev);
@@ -2735,8 +2641,7 @@ static size_t cluster_bwd_smem(int MT) {
 
 static int lstm_bwd_cluster(const LstmLayerWs& L, const float* w_hh, const float* dy, const float* notdone, int64_t T1, int64_t B,
                             int H, cudaStream_t st) {
-  const char* env = getenv("TB_LSTM_CLUSTER");
-  if ((env && env[0] == '0') || H != kClH || B > 32 || B < 1) return -1;
+  if (H != kClH || B > 32 || B < 1) return -1;
   static int attr_ok[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -2775,7 +2680,7 @@ static int lstm_bwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, cons
   const int Hq = mma_hq(H);
   const size_t smem = size_t(4) * 32 * Hq * 2;
   dim3 grid((H + kBwdCols - 1) / kBwdCols, 1);
-  if (!coop_fit(lstm_bwd_persistent_mma_kernel, grid, smem, per_device(g_bwd_mma_attr_dev))) return -1;
+  if (!coop_fit(lstm_bwd_persistent_mma_kernel, grid, smem, kStepThreads, per_device(g_bwd_mma_attr_dev))) return -1;
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(L.dgq, 0, size_t(2) * 4 * B * Hq * 2, st);  // zero the row padding
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
@@ -2796,11 +2701,9 @@ static size_t wave_bwd_smem(int H) {
   return size_t(4) * 32 * mma_hq(H) * 2 + size_t(16) * kper * 32 * 8;
 }
 static bool wave_bwd_applicable(int64_t B, int H) {
-  const char* e = getenv("TB_LSTM_WAVE_BWD");
-  if (e && e[0] == '0') return false;
   if (!mma_recurrence_applicable(B, H)) return false;
   dim3 grid(2 * ((H + kBwdCols - 1) / kBwdCols), 1);
-  return coop_fit(lstm2_bwd_wave_mma_kernel, grid, wave_bwd_smem(H), per_device(g_bwd_wave_attr_dev));
+  return coop_fit(lstm2_bwd_wave_mma_kernel, grid, wave_bwd_smem(H), kStepThreads, per_device(g_bwd_wave_attr_dev));
 }
 
 // both layers' backward recurrences in one launch; leaves dgb / bias gradients of both layers and
@@ -2842,23 +2745,8 @@ static bool wave_bwd_split_applicable(int64_t B, int In, int H) {
   if (!wave_fwd_split_applicable(B, In, H)) return false;  // consumes the planes the split forward leaves behind
   dim3 grid(2 * ((H + kBwdCols - 1) / kBwdCols), 1);
   if (int(grid.x / 2) + 1 > kSplitThreads || grid.x > 512) return false;
-  const size_t smem = wave_bwd_split_smem(mma_hq(H));
-  if (*per_device(g_bwd_split_attr_dev) < smem) {
-    if (cudaFuncSetAttribute(lstm2_bwd_wave_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();
-      return false;
-    }
-    *per_device(g_bwd_split_attr_dev) = smem;
-  }
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return false;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lstm2_bwd_wave_split_kernel, kSplitThreads, smem) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return int64_t(per_sm) * sms >= int64_t(grid.x);
+  return coop_fit(lstm2_bwd_wave_split_kernel, grid, wave_bwd_split_smem(mma_hq(H)), kSplitThreads,
+                  per_device(g_bwd_split_attr_dev));
 }
 
 static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone,
@@ -2884,12 +2772,10 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq); a.dgq_lo_off = U.dgq_lo;
   a.dxb = ws.dxb; a.flags = flags;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc;
-  a.trace = trace_buffer(2 * nc, int(T1));
   void* args[] = {&a};
   e = cudaLaunchCooperativeKernel((const void*)lstm2_bwd_wave_split_kernel, dim3(2 * nc), dim3(kSplitThreads), args,
                                   wave_bwd_split_smem(Hq), st);
   TB_REQUIRE(e == cudaSuccess, "lstm2_bwd_wave_split_kernel: %s", cudaGetErrorString(e));
-  trace_dump("bwd", a.trace, 2 * nc, int(T1), st);
   return check_launch("lstm2_bwd_wave_split_kernel");
 }
 
@@ -2920,8 +2806,6 @@ static SideStream* side_stream() {
     return &x;
   }
   if (!s.stream) {
-    const char* e = getenv("TB_LSTM_OVERLAP");
-    if (e && e[0] == '0') return nullptr;
     if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming) != cudaSuccess) {
@@ -3224,8 +3108,7 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
       float* wscr = splitk;
       TcEpilogue te; te.tag = "lstm_wgrad";
       if (tail) {
-        static const int tail_ctas = [] { const char* e = getenv("TB_LSTM_TAIL_CTAS"); return e ? atoi(e) : 0; }();  // 0 = uncapped
-        gs = tail->stream; wscr = ws.wg_scratch; te.max_ctas = tail_ctas;
+        gs = tail->stream; wscr = ws.wg_scratch;
       }
       if (side) {
         cudaError_t ee = cudaEventRecord(side->fork, st);

@@ -268,65 +268,6 @@ int relu_mask_inplace(float* X, const float* Y, int64_t M, int64_t ncols, int64_
 // =========================================================================================
 // bf16 operand staging (tensor-core backend)
 // =========================================================================================
-__global__ void im2col_u8_nchw_bf16_kernel(const uint8_t* __restrict__ frame, uint4* __restrict__ col, int64_t N, int C,
-                                           int H, int W, int KH, int S, int OH, int OW, int aligned4) {
-  // KW == 8: one thread converts one kernel row (8 pixels -> 8 bf16 = 16 bytes)
-  const int64_t rows_k = int64_t(C) * KH;
-  const int64_t total = N * OH * OW * rows_k;
-  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
-  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int64_t row = i / rows_k;
-    const int ck = int(i % rows_k);
-    const int c = ck / KH, kh = ck % KH;
-    const int64_t n = row / (OH * OW);
-    const int rem = int(row % (OH * OW));
-    const int oy = rem / OW, ox = rem % OW;
-    const uint8_t* src = frame + ((n * C + c) * H + (oy * S + kh)) * W + ox * S;
-    uint32_t lo, hi;
-    if (aligned4) {
-      lo = __ldg(reinterpret_cast<const uint32_t*>(src));
-      hi = __ldg(reinterpret_cast<const uint32_t*>(src) + 1);
-    } else {
-      lo = src[0] | (src[1] << 8) | (src[2] << 16) | (uint32_t(src[3]) << 24);
-      hi = src[4] | (src[5] << 8) | (src[6] << 16) | (uint32_t(src[7]) << 24);
-    }
-    auto pack2 = [](uint32_t a, uint32_t b) {
-      __nv_bfloat162 v = __floats2bfloat162_rn(float(a), float(b));
-      return *reinterpret_cast<uint32_t*>(&v);
-    };
-    uint4 o;
-    o.x = pack2(lo & 255u, (lo >> 8) & 255u); o.y = pack2((lo >> 16) & 255u, lo >> 24);
-    o.z = pack2(hi & 255u, (hi >> 8) & 255u); o.w = pack2((hi >> 16) & 255u, hi >> 24);
-    col[i] = o;  // row*K + ck*8 elements == i * 8 elements
-  }
-}
-
-int im2col_u8_nchw_bf16(const uint8_t* frame, void* col, int64_t N, int C, int H, int W, int KH, int KW, int S,
-                        cudaStream_t stream) {
-  ProfScope prof("im2col_u8_bf16", stream);
-  TB_REQUIRE(KW == 8, "im2col_u8_nchw_bf16: kernel width must be 8");
-  const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
-  const int64_t total = N * OH * OW * C * KH;
-  if (total == 0) return 0;
-  const int aligned4 = ((S & 3) == 0 && (W & 3) == 0 && (reinterpret_cast<uintptr_t>(frame) & 3) == 0);
-  im2col_u8_nchw_bf16_kernel<<<grid_for(total, 256), 256, 0, stream>>>(frame, static_cast<uint4*>(col), N, C, H, W, KH, S,
-                                                                         OH, OW, aligned4);
-  return check_launch("im2col_u8_nchw_bf16_kernel");
-}
-
-int im2col_bf16_nhwc(const void* act, void* col, int64_t N, int H, int W, int C, int KH, int KW, int S,
-                     cudaStream_t stream) {
-  ProfScope prof("im2col_bf16", stream);
-  TB_REQUIRE(C % 8 == 0, "im2col_bf16_nhwc: C must be a multiple of 8");
-  const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
-  const int64_t total = N * OH * OW * KH * KW * (C / 8);
-  if (total == 0) return 0;
-  // identical gather on 16-byte vectors: 8 bf16 per vector instead of 4 floats
-  im2col_f32_nhwc_kernel<<<grid_for(total, 256), 256, 0, stream>>>(
-      reinterpret_cast<const float4*>(act), reinterpret_cast<float4*>(col), N, H, W, C / 8, KH, KW, S, OH, OW);
-  return check_launch("im2col_bf16_nhwc_kernel");
-}
-
 __device__ __forceinline__ void acc_bf16x8(const uint4& v, float (&s)[8]) {
   const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
 #pragma unroll
@@ -334,62 +275,6 @@ __device__ __forceinline__ void acc_bf16x8(const uint4& v, float (&s)[8]) {
     const float2 f = __bfloat1622float2(h[j]);
     s[2 * j] += f.x; s[2 * j + 1] += f.y;
   }
-}
-
-__global__ void col2im_bf16_nhwc_kernel(const uint4* __restrict__ dcol, const uint4* __restrict__ act,
-                                        uint4* __restrict__ dact, int64_t N, int H, int W, int C8, int KH, int KW, int S,
-                                        int OH, int OW) {
-  const int64_t total = N * H * W * C8;
-  const int64_t K8 = int64_t(KH) * KW * C8;
-  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
-  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int c8 = int(i % C8);
-    int64_t t = i / C8;
-    const int ix = int(t % W); t /= W;
-    const int iy = int(t % H);
-    const int64_t n = t / H;
-    float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    for (int kh = iy % S; kh < KH; kh += S) {
-      if (iy - kh < 0) break;
-      const int oy = (iy - kh) / S;
-      if (oy >= OH) continue;
-      for (int kw = ix % S; kw < KW; kw += S) {
-        if (ix - kw < 0) break;
-        const int ox = (ix - kw) / S;
-        if (ox >= OW) continue;
-        acc_bf16x8(__ldg(dcol + ((n * OH + oy) * OW + ox) * K8 + (kh * KW + kw) * C8 + c8), s);
-      }
-    }
-    if (act) {
-      const uint4 a = __ldg(act + i);
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&a);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __bfloat1622float2(h[j]);
-        if (!(f.x > 0.f)) s[2 * j] = 0.f;
-        if (!(f.y > 0.f)) s[2 * j + 1] = 0.f;
-      }
-    }
-    uint4 o;
-    __nv_bfloat162 p0 = __floats2bfloat162_rn(s[0], s[1]), p1 = __floats2bfloat162_rn(s[2], s[3]);
-    __nv_bfloat162 p2 = __floats2bfloat162_rn(s[4], s[5]), p3 = __floats2bfloat162_rn(s[6], s[7]);
-    o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
-    o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
-    dact[i] = o;
-  }
-}
-
-int col2im_bf16_nhwc(const void* dcol, const void* act, void* dact, int64_t N, int H, int W, int C, int KH, int KW,
-                     int S, cudaStream_t stream) {
-  ProfScope prof("col2im_bf16", stream);
-  TB_REQUIRE(C % 8 == 0, "col2im_bf16_nhwc: C must be a multiple of 8");
-  const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
-  const int64_t total = N * H * W * (C / 8);
-  if (total == 0) return 0;
-  col2im_bf16_nhwc_kernel<<<grid_for(total, 256), 256, 0, stream>>>(
-      static_cast<const uint4*>(dcol), static_cast<const uint4*>(act), static_cast<uint4*>(dact), N, H, W, C / 8, KH, KW,
-      S, OH, OW);
-  return check_launch("col2im_bf16_nhwc_kernel");
 }
 
 __global__ void pack_weights_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, int64_t O, int P,

@@ -38,16 +38,6 @@ int relu_mask_inplace(float* X, const float* Y, int64_t M, int64_t ncols, int64_
                       cudaStream_t stream);
 
 // ---- bf16 operand staging for the tensor-core backend ---------------------------------------
-// frames u8 [N,C,H,W] -> bf16 patch matrix (pixel values 0..255 are exact in bf16; 1/255 is applied
-// in the GEMM epilogue)
-int im2col_u8_nchw_bf16(const uint8_t* frame, void* col_bf16, int64_t N, int C, int H, int W, int KH, int KW, int S,
-                        cudaStream_t stream);
-// bf16 NHWC -> bf16 patch matrix (C % 8 == 0); same gather as im2col_f32_nhwc on 16-byte vectors
-int im2col_bf16_nhwc(const void* act_bf16, void* col_bf16, int64_t N, int H, int W, int C, int KH, int KW, int S,
-                     cudaStream_t stream);
-// bf16 dcol -> bf16 d_act (fp32 accumulation), ReLU mask from the bf16 forward activation
-int col2im_bf16_nhwc(const void* dcol_bf16, const void* act_bf16, void* dact_bf16, int64_t N, int H, int W, int C,
-                     int KH, int KW, int S, cudaStream_t stream);
 // out_bf16[o*ld_out + p*Q + q] = in[o*P*Q + q*P + p]; columns [P*Q, ld_out) zero
 // lo_off != 0 (all three below): split-bf16 - also write / read the lo plane at +lo_off elements
 int pack_weights_bf16(const float* in, void* out_bf16, int64_t O, int P, int Q, int64_t ld_out, cudaStream_t stream,

@@ -76,34 +76,20 @@ struct ResWs {
   int64_t splitk_floats = 0;   // >= kScratchFloats; the split backend's per-tile column-sum partials grow with the frame count
   // split-bf16 backend (precision 2): activations stay fp32; only the GEMM operands are bf16 hi / lo planes
   // (lo plane = hi pointer + the *_lo element offset)
-  __nv_bfloat16 *colb = nullptr, *dyb = nullptr, *fcb = nullptr, *dfcb = nullptr;
-  // patch matrices of the 15 convolutions kept from the forward pass for the weight-gradient GEMMs (5.6 GB at T=80, B=8:
-  // HBM is 180 GB; TB_RESNET_KEEP_PATCHES=0 gathers them again in the backward pass instead), and the flipped /
-  // transposed weights of the input-gradient convolutions
-  __nv_bfloat16 *colk_feat[kSections] = {nullptr, nullptr, nullptr}, *colk_blk[kSections][4] = {};
-  int64_t colk_feat_lo[kSections] = {0, 0, 0}, colk_blk_lo[kSections][4] = {};
+  __nv_bfloat16 *fcb = nullptr, *dfcb = nullptr, *wb_fc = nullptr;
+  int64_t fcb_lo = 0, dfcb_lo = 0, wb_fc_lo = 0;
+  // every 3x3 conv is a shifted-window implicit GEMM (conv3x3_sw.cuh): the conv's input as a zero-padded
+  // channel-chunk-planar split-bf16 image, kept for the weight gradient; the images of dY (ping-pong); weights in the
+  // kernels' shared-memory layout (wi: forward, wd: flipped / transposed for the input-gradient convolution)
   __nv_bfloat16 *wd_feat[kSections] = {nullptr, nullptr, nullptr}, *wd_blk[kSections][4] = {};
   int64_t wd_feat_lo[kSections] = {0, 0, 0}, wd_blk_lo[kSections][4] = {};
-  // shifted-window implicit-GEMM path (conv3x3_sw.cuh; every 3x3 conv with 16 / 32 input channels): the conv's input as a
-  // zero-padded channel-chunk-planar split-bf16 image, kept for the weight gradient; the image of dY (shared); weights in
-  // the kernels' shared-memory layout
   __nv_bfloat16 *xp_feat[kSections] = {nullptr, nullptr, nullptr}, *xp_blk[kSections][4] = {}, *dyp = nullptr, *dyp2 = nullptr;
   int64_t xp_feat_lo[kSections] = {0, 0, 0}, xp_blk_lo[kSections][4] = {}, dyp_lo = 0, dyp2_lo = 0;
   __nv_bfloat16 *wi_feat[kSections] = {nullptr, nullptr, nullptr}, *wi_blk[kSections][4] = {};
   int64_t wi_feat_lo[kSections] = {0, 0, 0}, wi_blk_lo[kSections][4] = {};
-  __nv_bfloat16 *wb_feat[kSections] = {nullptr, nullptr, nullptr}, *wb_blk[kSections][4] = {}, *wb_fc = nullptr;
-  int64_t colb_lo = 0, dyb_lo = 0, fcb_lo = 0, dfcb_lo = 0, wb_feat_lo[kSections] = {0, 0, 0}, wb_blk_lo[kSections][4] = {}, wb_fc_lo = 0;
   LstmWs lstm;
   size_t bytes;
 };
-
-inline bool keep_patches() {
-  const char* e = getenv("TB_RESNET_KEEP_PATCHES");
-  return !(e && e[0] == '0');
-}
-
-// every 3x3 conv with 16 / 32 input channels as a shifted-window implicit GEMM (TB_RESNET_IMPLICIT=0: patch matrices)
-inline bool implicit3x3() { return sw_conv_applicable(kSecSo[0], kSecSo[0], 16, 16); }
 
 inline int64_t ldk_of(int cin, bool bf16) { const int64_t k = int64_t(cin) * 9; return bf16 ? ((k + 7) & ~int64_t(7)) : k; }
 
@@ -132,65 +118,38 @@ ResWs<T> res_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int use_lst
     if (a > maxcol) maxcol = a;
     if (b > maxcol) maxcol = b;
   }
-  w.col = split ? nullptr : takeT(maxcol);   // (the split backend gathers into colb instead)
-  w.dcol = split ? nullptr : takeT(maxcol);   // (the split backend's input gradients are convolutions of dY: no gradient patches)
+  w.col = split ? nullptr : takeT(maxcol);   // (the split backend's convolutions gather their own operands)
+  w.dcol = split ? nullptr : takeT(maxcol);
   if (split) {
     auto takeh = [&](int64_t n, int64_t& lo) {
       lo = (n + 127) & ~int64_t(127);
       return static_cast<__nv_bfloat16*>(take(size_t(2) * lo * sizeof(__nv_bfloat16)));
     };
-    int64_t maxcol16 = 0;
-    for (int i = 0; i < kSections; ++i) {
-      const int64_t a = N * kSecS[i] * kSecS[i] * ldk_of(kSecCin[i], true), b = N * kSecSo[i] * kSecSo[i] * ldk_of(kSecCh[i], true);
-      const int64_t c = i > 0 ? N * kSecS[i] * kSecS[i] * 9 * kSecCh[i] : 0;   // patches of dY (input gradient of the feat conv)
-      if (a > maxcol16) maxcol16 = a;
-      if (b > maxcol16) maxcol16 = b;
-      if (c > maxcol16) maxcol16 = c;
-    }
-    const bool patches = !implicit3x3();   // patch-matrix GEMMs only behind TB_RESNET_IMPLICIT=0
-    if (patches) {
-      w.colb = takeh(maxcol16, w.colb_lo);
-      w.dyb = takeh(maxact, w.dyb_lo);
-    }
     w.fcb = takeh(N * kFcIn, w.fcb_lo);
     w.dfcb = takeh(N * kFcOut, w.dfcb_lo);
-    for (int i = 0; i < kSections && patches; ++i) {
-      w.wb_feat[i] = takeh(int64_t(kSecCh[i]) * ldk_of(kSecCin[i], true), w.wb_feat_lo[i]);
-      for (int j = 0; j < 4; ++j) w.wb_blk[i][j] = takeh(int64_t(kSecCh[i]) * ldk_of(kSecCh[i], true), w.wb_blk_lo[i][j]);
-    }
     w.wb_fc = takeh(int64_t(kFcOut) * kFcIn, w.wb_fc_lo);
     for (int i = 0; i < kSections; ++i) {
       if (i > 0) w.wd_feat[i] = takeh(int64_t(kSecCin[i]) * 9 * kSecCh[i], w.wd_feat_lo[i]);
       for (int j = 0; j < 4; ++j) w.wd_blk[i][j] = takeh(int64_t(kSecCh[i]) * 9 * kSecCh[i], w.wd_blk_lo[i][j]);
     }
-    const bool impl = implicit3x3();
-    if (keep_patches()) {
-      for (int i = 0; i < kSections; ++i) {
-        if (!impl) w.colk_feat[i] = takeh(N * kSecS[i] * kSecS[i] * ldk_of(kSecCin[i], true), w.colk_feat_lo[i]);
-        for (int j = 0; j < 4 && !impl; ++j)
-          w.colk_blk[i][j] = takeh(N * kSecSo[i] * kSecSo[i] * ldk_of(kSecCh[i], true), w.colk_blk_lo[i][j]);
-      }
-    }
-    if (impl) {
-      int64_t maxp = 0;
-      for (int i = 0; i < kSections; ++i) {
-        {   // (the 4 frame channels of the first conv are padded to 16)
-          const int cin16 = kSecCin[i] < 16 ? 16 : kSecCin[i];
-          w.xp_feat[i] = takeh(sw_image_elems(N, kSecS[i], kSecS[i], cin16), w.xp_feat_lo[i]);
-          w.wi_feat[i] = takeh(sw_weight_elems(kSecCh[i], cin16) / 2, w.wi_feat_lo[i]);
-          const int64_t e = sw_image_elems(N, kSecS[i], kSecS[i], kSecCh[i]);
-          if (e > maxp) maxp = e;
-        }
-        for (int j = 0; j < 4; ++j) {
-          w.xp_blk[i][j] = takeh(sw_image_elems(N, kSecSo[i], kSecSo[i], kSecCh[i]), w.xp_blk_lo[i][j]);
-          w.wi_blk[i][j] = takeh(sw_weight_elems(kSecCh[i], kSecCh[i]) / 2, w.wi_blk_lo[i][j]);
-        }
-        const int64_t e = sw_image_elems(N, kSecSo[i], kSecSo[i], kSecCh[i]);
+    int64_t maxp = 0;
+    for (int i = 0; i < kSections; ++i) {
+      {   // (the 4 frame channels of the first conv are padded to 16)
+        const int cin16 = kSecCin[i] < 16 ? 16 : kSecCin[i];
+        w.xp_feat[i] = takeh(sw_image_elems(N, kSecS[i], kSecS[i], cin16), w.xp_feat_lo[i]);
+        w.wi_feat[i] = takeh(sw_weight_elems(kSecCh[i], cin16) / 2, w.wi_feat_lo[i]);
+        const int64_t e = sw_image_elems(N, kSecS[i], kSecS[i], kSecCh[i]);
         if (e > maxp) maxp = e;
       }
-      w.dyp = takeh(maxp, w.dyp_lo);     // dY images ping-pong: a conv's input-gradient epilogue writes the next conv's dY image
-      w.dyp2 = takeh(maxp, w.dyp2_lo);
+      for (int j = 0; j < 4; ++j) {
+        w.xp_blk[i][j] = takeh(sw_image_elems(N, kSecSo[i], kSecSo[i], kSecCh[i]), w.xp_blk_lo[i][j]);
+        w.wi_blk[i][j] = takeh(sw_weight_elems(kSecCh[i], kSecCh[i]) / 2, w.wi_blk_lo[i][j]);
+      }
+      const int64_t e = sw_image_elems(N, kSecSo[i], kSecSo[i], kSecCh[i]);
+      if (e > maxp) maxp = e;
     }
+    w.dyp = takeh(maxp, w.dyp_lo);     // dY images ping-pong: a conv's input-gradient epilogue writes the next conv's dY image
+    w.dyp2 = takeh(maxp, w.dyp2_lo);
   }
   for (int i = 0; i < kSections; ++i) {
     w.wfeat[i] = takeT(int64_t(kSecCh[i]) * ldk_of(kSecCin[i], kBf16));
@@ -432,10 +391,10 @@ struct Impl {
 
 
 // ---- split-bf16 backend (precision 2) ----------------------------------------------------------------------
-// The fp32 data flow of Impl<float> (fp32 NHWC activations, fp32 gradients, the same pool / ReLU / col2im kernels)
-// with every GEMM on the tensor cores in split-bf16: the patch gather writes hi / lo bf16 planes, the weights are
-// packed as hi / lo planes, products are hi.hi + hi.lo + lo.hi in fp32 (~2^-17 relative per product: fp32-grade,
-// holds the 1e-4 parity contract that plain bf16 operands do not).
+// The fp32 data flow of Impl<float> (fp32 NHWC activations, fp32 gradients, the same pool / ReLU kernels) with every
+// contraction on the tensor cores in split-bf16: the 3x3 convolutions are shifted-window implicit GEMMs over hi / lo
+// bf16 images, the fc GEMM reads hi / lo planes, products are hi.hi + hi.lo + lo.hi in fp32 (~2^-17 relative per
+// product: fp32-grade, holds the 1e-4 parity contract that plain bf16 operands do not).
 struct SplitImpl {
   using W = ResWs<float>;
   static int gemm_fwd(const __nv_bfloat16* a, int64_t a_lo, const __nv_bfloat16* b, int64_t b_lo, float* out, int64_t M, int cout,
@@ -453,16 +412,6 @@ struct SplitImpl {
     te.tag = tag;
     return gemm_tc_bf16_ex(dy, col, cout, K, M, cout, ldk, true, true, te, splits_tc(cout, K, M), scratch, st);
   }
-  // the first conv's patches are uint8 pixels: exact in the hi plane, the lo plane is zero
-  static int first_patches(const uint8_t* frame, __nv_bfloat16* col, int64_t col_lo, int64_t N, cudaStream_t st) {
-    const int S = kSecS[0];
-    const int64_t ldk = ldk_of(4, true);
-    TB_TRY(im2col3x3_u8_nchw<__nv_bfloat16>(frame, col, N, 4, S, S, ldk, st));
-    cudaError_t e = cudaMemsetAsync(col + col_lo, 0, size_t(N) * S * S * ldk * sizeof(__nv_bfloat16), st);
-    TB_REQUIRE(e == cudaSuccess, "resnet: memset: %s", cudaGetErrorString(e));
-    return 0;
-  }
-
   // shifted-window implicit GEMM: x fp32 NHWC -> padded planar split-bf16 image xp (kept for the weight gradient) -> out fp32
   // x == nullptr: the previous conv's epilogue already wrote this conv's input image into xp.  emit: the NEXT conv's input
   // image (this conv's output, through ReLU if emit_relu), written by the epilogue.
@@ -481,64 +430,32 @@ struct SplitImpl {
     const int64_t N = T1 * B;
     const ResParams pp = res_params(A, use_lstm);
     W w = res_ws<float>(workspace, N, T1, B, A, use_lstm, true);
-    if (w.wb_feat[0]) {   // patch-matrix fallback: K-major packed weights
-      TB_TRY(pack_weights_bf16(P + pp.feat[0].w, w.wb_feat[0], kSecCh[0], 1, 36, ldk_of(4, true), st, w.wb_feat_lo[0]));
-      for (int i = 0; i < kSections; ++i) {
-        if (i > 0)
-          TB_TRY(pack_weights_bf16(P + pp.feat[i].w, w.wb_feat[i], kSecCh[i], 9, kSecCin[i], ldk_of(kSecCin[i], true), st, w.wb_feat_lo[i]));
-        for (int j = 0; j < 4; ++j)
-          TB_TRY(pack_weights_bf16(P + pp.blk[i][j].w, w.wb_blk[i][j], kSecCh[i], 9, kSecCh[i], ldk_of(kSecCh[i], true), st, w.wb_blk_lo[i][j]));
-      }
-    }
     TB_TRY(pack_weights_bf16(P + pp.fc_w, w.wb_fc, kFcOut, 121, 32, kFcIn, st, w.wb_fc_lo));
-    const float* xin = nullptr;
     for (int i = 0; i < kSections; ++i) {
       const int S = kSecS[i], So = kSecSo[i], ch = kSecCh[i], cin = kSecCin[i];
-      const int64_t M = N * S * S, Mo = N * So * So;
-      const int64_t ldk_in = ldk_of(cin, true), ldk = ldk_of(ch, true);
-      __nv_bfloat16* cf = w.colk_feat[i] ? w.colk_feat[i] : w.colb;
-      const int64_t cf_lo = w.colk_feat[i] ? w.colk_feat_lo[i] : w.colb_lo;
-      if (i == 0 && w.xp_feat[0]) {
+      if (i == 0) {
         // the first conv through the same kernels: frame pixels (exact in bf16) as a 16-channel image, 1/255 in the epilogue
         TB_TRY(sw_pack_weights(P + pp.feat[0].w, w.wi_feat[0], ch, 16, 0, st, 4));
         TB_TRY(sw_frames_u8(frame, w.xp_feat[0], w.xp_feat_lo[0], N, 4, S, S, st));
         SwEpilogue ep; ep.scale = 1.0f / 255.0f; ep.bias = P + pp.feat[0].b; ep.tag = "feat_conv_fwd";
         TB_TRY(sw_conv_fwd(w.xp_feat[0], w.xp_feat_lo[0], w.wi_feat[0], w.s[0].P, N, S, S, 16, ch, ep, st));
-      } else if (i == 0) {
-        TB_TRY(first_patches(frame, cf, cf_lo, N, st));
-        TB_TRY(gemm_fwd(cf, cf_lo, w.wb_feat[0], w.wb_feat_lo[0], w.s[0].P, M, ch, 36, ldk_in, P + pp.feat[0].b, nullptr,
-                        1.0f / 255.0f, 0, ch, "feat_conv_fwd", st));
-      } else if (w.xp_feat[i]) {
+      } else {
         // (its input image was written by the epilogue of the previous section's last conv)
         TB_TRY(conv_impl(nullptr, 0, w.xp_feat[i], w.xp_feat_lo[i], P + pp.feat[i].w, w.wi_feat[i], w.wi_feat_lo[i], w.s[i].P, N, S, cin, ch,
                          P + pp.feat[i].b, nullptr, nullptr, 0, 0, "feat_conv_fwd", st));
-      } else {
-        TB_TRY(im2col3x3_split(xin, cf, cf_lo, N, S, S, cin, ldk_in, 0, st));
-        TB_TRY(gemm_fwd(cf, cf_lo, w.wb_feat[i], w.wb_feat_lo[i], w.s[i].P, M, ch, int64_t(cin) * 9, ldk_in,
-                        P + pp.feat[i].b, nullptr, 1.0f, 0, ch, "feat_conv_fwd", st));
       }
       TB_TRY(maxpool3x3s2_fwd<float>(w.s[i].P, w.s[i].X0, w.s[i].arg, N, S, S, ch, st));
-      const float* ins[4] = {w.s[i].X0, w.s[i].Y1, w.s[i].X1, w.s[i].Y2};
       float* outs[4] = {w.s[i].Y1, w.s[i].X1, w.s[i].Y2, w.s[i].X2};
       const float* adds[4] = {nullptr, w.s[i].X0, nullptr, w.s[i].X1};
       for (int j = 0; j < 4; ++j) {
-        if (w.xp_blk[i][j]) {
-          // conv j's epilogue writes relu(output) as conv j+1's input image; the section's last conv writes the next
-          // section's feat-conv input (no ReLU there)
-          __nv_bfloat16* emit = j < 3 ? w.xp_blk[i][j + 1] : (i + 1 < kSections ? w.xp_feat[i + 1] : nullptr);
-          const int64_t emit_lo = j < 3 ? w.xp_blk_lo[i][j + 1] : (i + 1 < kSections ? w.xp_feat_lo[i + 1] : 0);
-          TB_TRY(conv_impl(j == 0 ? ins[0] : nullptr, 1, w.xp_blk[i][j], w.xp_blk_lo[i][j], P + pp.blk[i][j].w, w.wi_blk[i][j],
-                           w.wi_blk_lo[i][j], outs[j], N, So, ch, ch, P + pp.blk[i][j].b, adds[j], emit, emit_lo, j < 3 ? 1 : 0,
-                           "res_conv_fwd", st));
-          continue;
-        }
-        __nv_bfloat16* cb = w.colk_blk[i][j] ? w.colk_blk[i][j] : w.colb;
-        const int64_t cb_lo = w.colk_blk[i][j] ? w.colk_blk_lo[i][j] : w.colb_lo;
-        TB_TRY(im2col3x3_split(ins[j], cb, cb_lo, N, So, So, ch, ldk, 1, st));
-        TB_TRY(gemm_fwd(cb, cb_lo, w.wb_blk[i][j], w.wb_blk_lo[i][j], outs[j], Mo, ch, int64_t(ch) * 9, ldk,
-                        P + pp.blk[i][j].b, adds[j], 1.0f, 0, ch, "res_conv_fwd", st));
+        // conv j's epilogue writes relu(output) as conv j+1's input image; the section's last conv writes the next
+        // section's feat-conv input (no ReLU there)
+        __nv_bfloat16* emit = j < 3 ? w.xp_blk[i][j + 1] : (i + 1 < kSections ? w.xp_feat[i + 1] : nullptr);
+        const int64_t emit_lo = j < 3 ? w.xp_blk_lo[i][j + 1] : (i + 1 < kSections ? w.xp_feat_lo[i + 1] : 0);
+        TB_TRY(conv_impl(j == 0 ? w.s[i].X0 : nullptr, 1, w.xp_blk[i][j], w.xp_blk_lo[i][j], P + pp.blk[i][j].w, w.wi_blk[i][j],
+                         w.wi_blk_lo[i][j], outs[j], N, So, ch, ch, P + pp.blk[i][j].b, adds[j], emit, emit_lo, j < 3 ? 1 : 0,
+                         "res_conv_fwd", st));
       }
-      xin = w.s[i].X2;
     }
     TB_TRY(relu_fwd<float>(w.s[2].X2, w.fcin, N * kFcIn, st));
     TB_TRY(f32_to_bf16(w.fcin, w.fcb, N, kFcIn, kFcIn, kFcIn, st, w.fcb_lo));
@@ -582,31 +499,6 @@ struct SplitImpl {
     return 0;
   }
 
-  // one 3x3 conv backward.  Bias gradient + the bf16 planes of dY in one pass; weight gradient against the patch matrix
-  // kept from the forward pass (colk; nullptr = gather it again); input gradient as a CONVOLUTION of dY with the flipped /
-  // transposed weights (wd) - patches of dY, one GEMM with N = cin whose epilogue applies the ReLU mask of the conv's input
-  // and adds the skip gradient: no [M, 9*cin] fp32 gradient patch matrix, no col2im pass.
-  static int conv_bwd(const float* x, bool relu_in, const float* dY, const float* Wsrc, const __nv_bfloat16* colk, int64_t colk_lo,
-                      __nv_bfloat16* wd, int64_t wd_lo, float* dW, float* db, float* dx, const float* addend, int64_t N, int S,
-                      int cin, int cout, W& w, cudaStream_t st) {
-    const int64_t M = N * S * S, K = int64_t(cin) * 9, ldk = ldk_of(cin, true);
-    TB_TRY(dy_split_colsum(dY, w.dyb, w.dyb_lo, M, cout, db, w.splitk, kScratchFloats, st));
-    if (!colk) {
-      TB_TRY(im2col3x3_split(x, w.colb, w.colb_lo, N, S, S, cin, ldk, relu_in ? 1 : 0, st));
-      colk = w.colb; colk_lo = w.colb_lo;
-    }
-    TB_TRY(gemm_wgrad(w.dyb, w.dyb_lo, colk, colk_lo, dW, M, cout, K, ldk, 9, cin, 1.0f, w.splitk, "res_conv_wgrad", st));
-    if (dx) {
-      const int64_t Kd = int64_t(cout) * 9;
-      TB_TRY(pack_dgrad3x3_weights(Wsrc, wd, wd_lo, cout, cin, Kd, st));
-      TB_TRY(im2col3x3_split(dY, w.colb, w.colb_lo, N, S, S, cout, Kd, 0, st));
-      TcEpilogue te; te.C = dx; te.ldc = cin; te.addend32 = addend; te.ldadd = cin; te.mask = relu_in ? x : nullptr; te.ldmask = cin;
-      te.a_lo = w.colb_lo; te.b_lo = wd_lo; te.tag = "res_conv_dgrad";
-      TB_TRY(gemm_tc_bf16(w.colb, wd, M, cin, Kd, Kd, Kd, te, st));
-    }
-    return 0;
-  }
-
   static int backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
                       const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st) {
     const int64_t N = T1 * B;
@@ -635,7 +527,7 @@ struct SplitImpl {
     }
     float* g0 = w.g[0]; float* g1 = w.g[1]; float* g2 = w.g[2];
     TB_TRY(relu_bwd<float>(w.s[2].X2, w.dfcin, g0, N * kFcIn, st));
-    __nv_bfloat16* dyi[2] = {w.dyp, w.dyp2};   // dY images (shifted-window path): dyi[dsel] is the one the next kernel reads
+    __nv_bfloat16* dyi[2] = {w.dyp, w.dyp2};   // dY images: dyi[dsel] is the one the next kernel reads
     const int64_t dyi_lo[2] = {w.dyp_lo, w.dyp2_lo};
     int dsel = 0;
     for (int i = kSections - 1; i >= 0; --i) {
@@ -646,51 +538,28 @@ struct SplitImpl {
       float* dxs[4] = {g1, g0, g2, g1};
       const float* skip[4] = {g2, nullptr, g0, nullptr};
       for (int j = 3; j >= 0; --j) {
-        if (w.xp_blk[i][j]) {
-          // the dY image of conv j: written by the previous kernel's epilogue, except for the very first conv of the pass
-          const bool ready = !(i == kSections - 1 && j == 3);
-          __nv_bfloat16* cur = dyi[dsel]; const int64_t cur_lo = dyi_lo[dsel];
-          __nv_bfloat16* nxt = j > 0 ? dyi[dsel ^ 1] : nullptr;   // conv j's dx is conv j-1's dY (j = 0: feeds the max-pool backward)
-          TB_TRY(conv_bwd_impl(xs[j], true, ready ? nullptr : dys[j], cur, cur_lo, P + pp.blk[i][j].w, w.xp_blk[i][j], w.xp_blk_lo[i][j],
-                               w.wd_blk[i][j], w.wd_blk_lo[i][j], G + pp.blk[i][j].w, G + pp.blk[i][j].b, dxs[j], skip[j], nxt,
-                               dyi_lo[dsel ^ 1], j > 0 ? G + pp.blk[i][j - 1].b : nullptr, N, So, ch, ch, w, "res_conv_wgrad", st));
-          if (nxt) dsel ^= 1;
-        } else {
-          TB_TRY(conv_bwd(xs[j], true, dys[j], P + pp.blk[i][j].w, w.colk_blk[i][j], w.colk_blk_lo[i][j], w.wd_blk[i][j], w.wd_blk_lo[i][j],
-                          G + pp.blk[i][j].w, G + pp.blk[i][j].b, dxs[j], skip[j], N, So, ch, ch, w, st));
-        }
+        // the dY image of conv j: written by the previous kernel's epilogue, except for the very first conv of the pass
+        const bool ready = !(i == kSections - 1 && j == 3);
+        __nv_bfloat16* cur = dyi[dsel]; const int64_t cur_lo = dyi_lo[dsel];
+        __nv_bfloat16* nxt = j > 0 ? dyi[dsel ^ 1] : nullptr;   // conv j's dx is conv j-1's dY (j = 0: feeds the max-pool backward)
+        TB_TRY(conv_bwd_impl(xs[j], true, ready ? nullptr : dys[j], cur, cur_lo, P + pp.blk[i][j].w, w.xp_blk[i][j], w.xp_blk_lo[i][j],
+                             w.wd_blk[i][j], w.wd_blk_lo[i][j], G + pp.blk[i][j].w, G + pp.blk[i][j].b, dxs[j], skip[j], nxt,
+                             dyi_lo[dsel ^ 1], j > 0 ? G + pp.blk[i][j - 1].b : nullptr, N, So, ch, ch, w, "res_conv_wgrad", st));
+        if (nxt) dsel ^= 1;
       }
-      // dL/dP (the feat conv's output gradient) is consumed only as that conv's dY image + bias gradient: with the
-      // shifted-window kernels the max-pool backward gathers straight into the image (never materialised in fp32)
-      if (w.xp_feat[i])
-        TB_TRY(sw_pool_bwd_image_colsum(s.arg, g1, dyi[dsel], dyi_lo[dsel], N, S, S, ch, G + pp.feat[i].b, w.splitk, w.splitk_floats, st));
-      else
-        TB_TRY(maxpool3x3s2_bwd<float>(s.arg, g1, g2, N, S, S, ch, st));   // g2 = dL/dP
-      const int64_t M = N * S * S;
-      if (i == 0 && w.xp_feat[0]) {
+      // dL/dP (the feat conv's output gradient) is consumed only as that conv's dY image + bias gradient: the max-pool
+      // backward gathers straight into the image (never materialised in fp32)
+      TB_TRY(sw_pool_bwd_image_colsum(s.arg, g1, dyi[dsel], dyi_lo[dsel], N, S, S, ch, G + pp.feat[i].b, w.splitk, w.splitk_floats, st));
+      if (i == 0) {
         TB_TRY(sw_conv_wgrad(dyi[dsel], dyi_lo[dsel], w.xp_feat[0], w.xp_feat_lo[0], G + pp.feat[0].w, N, S, S, 16, ch, w.splitk,
                              w.splitk_floats, "feat_conv_wgrad", st, 1.0f / 255.0f, 4));
-      } else if (i == 0) {
-        const int64_t ldk_in = ldk_of(4, true);
-        TB_TRY(dy_split_colsum(g2, w.dyb, w.dyb_lo, M, ch, G + pp.feat[0].b, w.splitk, kScratchFloats, st));
-        const __nv_bfloat16* cf = w.colk_feat[0];
-        int64_t cf_lo = w.colk_feat_lo[0];
-        if (!cf) {
-          TB_TRY(first_patches(frame, w.colb, w.colb_lo, N, st));
-          cf = w.colb; cf_lo = w.colb_lo;
-        }
-        TB_TRY(gemm_wgrad(w.dyb, w.dyb_lo, cf, cf_lo, G + pp.feat[0].w, M, ch, 36, ldk_in, 1, 1, 1.0f / 255.0f, w.splitk,
-                          "feat_conv_wgrad", st));
-      } else if (w.xp_feat[i]) {
-        // (image + bias gradient done by the fused max-pool backward above); its dx = dL/dX2 of section i-1 = the dY of that
-        // section's last conv: emitted as the image + bias gradient that conv's backward starts from
+      } else {
+        // its dx = dL/dX2 of section i-1 = the dY of that section's last conv: emitted as the image + bias gradient that
+        // conv's backward starts from
         TB_TRY(conv_bwd_impl(w.s[i - 1].X2, false, nullptr, dyi[dsel], dyi_lo[dsel], P + pp.feat[i].w, w.xp_feat[i], w.xp_feat_lo[i],
                              w.wd_feat[i], w.wd_feat_lo[i], G + pp.feat[i].w, G + pp.feat[i].b, g0, nullptr, dyi[dsel ^ 1], dyi_lo[dsel ^ 1],
                              G + pp.blk[i - 1][3].b, N, S, cin, ch, w, "res_conv_wgrad", st));
         dsel ^= 1;
-      } else {
-        TB_TRY(conv_bwd(w.s[i - 1].X2, false, g2, P + pp.feat[i].w, w.colk_feat[i], w.colk_feat_lo[i], w.wd_feat[i], w.wd_feat_lo[i],
-                        G + pp.feat[i].w, G + pp.feat[i].b, g0, nullptr, N, S, cin, ch, w, st));
       }
     }
     return 0;

@@ -3,15 +3,8 @@
 
 #include "gemm_tc.cuh"
 #include "net_kernels.cuh"
-#include "tc_common.cuh"
 
 namespace tb {
-
-#define TB_TRY(expr)        \
-  do {                      \
-    int _rc = (expr);       \
-    if (_rc) return _rc;    \
-  } while (0)
 
 static inline unsigned rgrid(int64_t work, int threads) {
   int64_t blocks = (work + threads - 1) / threads;
@@ -62,121 +55,6 @@ int im2col3x3(const T* x, T* col, int64_t N, int H, int W, int C, int64_t ldk, i
 }
 template int im2col3x3<float>(const float*, float*, int64_t, int, int, int, int64_t, int, cudaStream_t);
 template int im2col3x3<__nv_bfloat16>(const __nv_bfloat16*, __nv_bfloat16*, int64_t, int, int, int, int64_t, int, cudaStream_t);
-
-// fp32 activations -> split-bf16 patch matrix (hi plane at col, lo plane at col + lo_off): one thread = 8 channels of
-// one (pixel, tap), two 16-byte stores
-__global__ void im2col3x3_split_kernel(const float4* __restrict__ x, __nv_bfloat16* __restrict__ col, int64_t lo_off, int64_t N,
-                                       int H, int W, int C8, int64_t ldk, int relu_in) {
-  const int64_t total = N * H * W * 9 * C8;
-  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
-  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int cv = int(i % C8);
-    int64_t t = i / C8;
-    const int tap = int(t % 9); t /= 9;
-    const int ox = int(t % W); t /= W;
-    const int oy = int(t % H);
-    const int64_t n = t / H;
-    const int iy = oy + tap / 3 - 1, ix = ox + tap % 3 - 1;
-    float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
-      const float4* src = x + (((n * H + iy) * W + ix) * C8 + cv) * 2;
-      const float4 a = __ldg(src), b = __ldg(src + 1);
-      f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-      if (relu_in) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = fmaxf(f[j], 0.0f);
-      }
-    }
-    uint4 ph, pl;
-    tcd::split_bf16x2(f[0], f[1], ph.x, pl.x); tcd::split_bf16x2(f[2], f[3], ph.y, pl.y);
-    tcd::split_bf16x2(f[4], f[5], ph.z, pl.z); tcd::split_bf16x2(f[6], f[7], ph.w, pl.w);
-    __nv_bfloat16* dst = col + ((n * H + oy) * W + ox) * ldk + int64_t(tap) * C8 * 8 + cv * 8;
-    *reinterpret_cast<uint4*>(dst) = ph;
-    *reinterpret_cast<uint4*>(dst + lo_off) = pl;
-  }
-}
-
-int im2col3x3_split(const float* x, __nv_bfloat16* col, int64_t lo_off, int64_t N, int H, int W, int C, int64_t ldk, int relu_in,
-                    cudaStream_t stream) {
-  ProfScope prof("im2col3x3", stream);
-  TB_REQUIRE(C % 8 == 0 && ldk % 8 == 0 && lo_off % 8 == 0, "im2col3x3_split: C, ldk and the plane offset must be multiples of 8");
-  const int64_t total = N * H * W * 9 * (C / 8);
-  if (total == 0) return 0;
-  im2col3x3_split_kernel<<<rgrid(total, 256), 256, 0, stream>>>(reinterpret_cast<const float4*>(x), col, lo_off, N, H, W, C / 8,
-                                                               ldk, relu_in);
-  return check_launch("im2col3x3_split_kernel");
-}
-
-// dY fp32 [M, C] -> bf16 hi / lo planes (the MN-major operand of the weight-gradient GEMM) AND its column sums (the bias
-// gradient) in one pass: a thread keeps the same 4 channels for all of its rows (the grid stride is a multiple of C/4),
-// block partials go to scratch [blocks][C] and are folded in block order by dy_colsum_final_kernel (deterministic).
-__global__ void __launch_bounds__(256) dy_split_colsum_kernel(const float4* __restrict__ dy, __nv_bfloat16* __restrict__ out,
-                                                              int64_t lo_off, int64_t units, int CQ, float* __restrict__ partial) {
-  __shared__ float4 red[256];
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  const int64_t stride = int64_t(gridDim.x) * 256;
-  for (int64_t u = int64_t(blockIdx.x) * 256 + threadIdx.x; u < units; u += stride) {
-    const float4 v = __ldg(dy + u);
-    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-    uint2 ph, pl;
-    tcd::split_bf16x2(v.x, v.y, ph.x, pl.x); tcd::split_bf16x2(v.z, v.w, ph.y, pl.y);
-    *reinterpret_cast<uint2*>(out + u * 4) = ph;
-    *reinterpret_cast<uint2*>(out + lo_off + u * 4) = pl;
-  }
-  red[threadIdx.x] = acc;
-  __syncthreads();
-  if (int(threadIdx.x) < CQ) {   // thread t holds channels 4*(t % CQ) .. +3 (256 % CQ == 0)
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int t = threadIdx.x; t < 256; t += CQ) { s.x += red[t].x; s.y += red[t].y; s.z += red[t].z; s.w += red[t].w; }
-    *reinterpret_cast<float4*>(partial + (int64_t(blockIdx.x) * CQ + threadIdx.x) * 4) = s;
-  }
-}
-__global__ void dy_colsum_final_kernel(const float* __restrict__ partial, float* __restrict__ out, int blocks, int C) {
-  const int c = threadIdx.x;
-  if (c >= C) return;
-  float s = 0.f;
-  for (int b = 0; b < blocks; ++b) s += partial[int64_t(b) * C + c];
-  out[c] = s;
-}
-
-int dy_split_colsum(const float* dy, __nv_bfloat16* out, int64_t lo_off, int64_t M, int C, float* db, float* scratch,
-                    int64_t scratch_floats, cudaStream_t stream) {
-  ProfScope prof("bias_grad_colsum", stream);
-  TB_REQUIRE(C % 4 == 0 && 256 % (C / 4) == 0 && C <= 256 && lo_off % 4 == 0, "dy_split_colsum: C must be 4..256 with 256 %% (C/4) == 0");
-  const int64_t units = M * (C / 4);
-  if (units == 0) return 0;
-  int64_t blocks = (units + 255) / 256;
-  if (blocks > int64_t(kNumSMs) * 8) blocks = int64_t(kNumSMs) * 8;
-  TB_REQUIRE(blocks * C <= scratch_floats, "dy_split_colsum: scratch too small");
-  dy_split_colsum_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const float4*>(dy), out, lo_off, units, C / 4, scratch);
-  TB_TRY(check_launch("dy_split_colsum_kernel"));
-  dy_colsum_final_kernel<<<1, 256, 0, stream>>>(scratch, db, int(blocks), C);
-  return check_launch("dy_colsum_final_kernel");
-}
-
-// weights [O, C, 3, 3] fp32 -> B operand of the input gradient computed as a convolution of dY (stride 1, pad 1):
-// out[c, (a*3 + b)*O + o] = W[o, c, 2-a, 2-b] as bf16 hi / lo planes, row pitch ld (>= 9*O)
-__global__ void pack_dgrad3x3_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int64_t lo_off, int O, int C,
-                                     int64_t ld) {
-  const int64_t total = int64_t(C) * ld;
-  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-    const int c = int(i / ld), k = int(i % ld);
-    float v = 0.f;
-    if (k < 9 * O) {
-      const int tap = k / O, o = k - tap * O;
-      const int a = tap / 3, b = tap - a * 3;
-      v = w[((int64_t(o) * C + c) * 3 + (2 - a)) * 3 + (2 - b)];
-    }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    out[i] = h;
-    out[lo_off + i] = tcd::bf16_lo_of(v, h);
-  }
-}
-int pack_dgrad3x3_weights(const float* w, __nv_bfloat16* out, int64_t lo_off, int O, int C, int64_t ld, cudaStream_t stream) {
-  const int64_t total = int64_t(C) * ld;
-  pack_dgrad3x3_kernel<<<rgrid(total, 256), 256, 0, stream>>>(w, out, lo_off, O, C, ld);
-  return check_launch("pack_dgrad3x3_kernel");
-}
 
 template <typename TOut> __device__ __forceinline__ TOut from_u8(uint8_t v);
 template <> __device__ __forceinline__ uint8_t from_u8<uint8_t>(uint8_t v) { return v; }

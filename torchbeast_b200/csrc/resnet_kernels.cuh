@@ -40,16 +40,6 @@ template <> struct Vec16<__nv_bfloat16> {
 template <typename T>
 int im2col3x3(const T* x, T* col, int64_t N, int H, int W, int C, int64_t ldk, int relu_in, cudaStream_t stream);
 
-// split-bf16 backend: fp32 activations -> patch matrix as bf16 hi / lo planes (lo plane at col + lo_off elements)
-int im2col3x3_split(const float* x, __nv_bfloat16* col, int64_t lo_off, int64_t N, int H, int W, int C, int64_t ldk, int relu_in,
-                    cudaStream_t stream);
-
-// dY fp32 [M, C] -> bf16 hi / lo planes + column sums db[C] (bias gradient) in one pass; scratch >= kNumSMs*8*C floats
-int dy_split_colsum(const float* dy, __nv_bfloat16* out, int64_t lo_off, int64_t M, int C, float* db, float* scratch,
-                    int64_t scratch_floats, cudaStream_t stream);
-// weights [O, C, 3, 3] -> [C, ld >= 9*O] hi / lo planes with flipped taps: the input gradient as a convolution of dY
-int pack_dgrad3x3_weights(const float* w, __nv_bfloat16* out, int64_t lo_off, int O, int C, int64_t ld, cudaStream_t stream);
-
 // first conv of the net: frames u8 NCHW [N,C,H,W] -> patch matrix, k = (c*3 + kh)*3 + kw (the reference
 // weight's own flattening).  TOut = uint8_t (fp32 backend: x/255 applied on read) or bf16 (exact 0..255).
 template <typename TOut>

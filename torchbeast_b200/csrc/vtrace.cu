@@ -265,8 +265,6 @@ __global__ void __launch_bounds__(512) vtrace_scan_cluster_kernel(ScanArgs<F> p)
 
 // cluster size for the T-split across CTAs: the largest power of two <= 8 that leaves >= 4 time steps per warp (0: not worth it)
 static int pick_cluster(int64_t T, int64_t tiles, int W) {
-  const char* e = getenv("TB_VTRACE_CLUSTER");
-  if (e && e[0] == '0') return 0;
   if (W < 16 || tiles * 16 > int64_t(sm_count()) * 2) return 0;  // enough tiles to fill the chip without it
   int c = 8;
   while (c > 1 && (T < int64_t(16) * c * 4 || (T + int64_t(16) * c - 1) / (int64_t(16) * c) > 8)) c >>= 1;
