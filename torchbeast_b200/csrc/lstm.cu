@@ -18,6 +18,7 @@
 #include "gemm_simt.cuh"
 #include "gemm_tc.cuh"
 #include "net_kernels.cuh"
+#include "tc_common.cuh"
 
 namespace tb {
 
@@ -1585,7 +1586,8 @@ __global__ void lstm_init_state_q_kernel(const float* __restrict__ h0, const flo
 //   * 11 MMA warps x 3 k16-steps cover K = 528 exactly (33 k-steps): no padded k-steps, weights of all three
 //     matrices as hi AND lo B fragments in registers (72 per thread) for all steps;
 //   * h is exchanged as two bf16 planes (hq: raw h, slot t+1 = h_t) written with 8-byte stores (4 units x
-//     bf16 of one row and plane) and pulled as 4 x 34 KB tiles per step with cp.async;
+//     bf16 of one row and plane) and pulled per warp as TMA boxes of its 48 (+8) columns; the CTAs run as 2-CTA
+//     clusters and each CTA of a pair loads one 16-row half and multicasts it, so the pair reads each tile once;
 //   * the cell state lives in a register of the thread that owns (layer, unit, row) for all steps;
 //   * the grid barrier is per-CTA FLAGS instead of one contended counter: producer = stores, bar.sync,
 //     fence.acq_rel.gpu, st flag[cta] = step; consumers = one thread per producer
@@ -1626,6 +1628,64 @@ __device__ __forceinline__ void split_pack(float v0, float v1, uint32_t& hi, uin
 __device__ __forceinline__ void st_relaxed_u32(unsigned* p, unsigned v) {
   asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// ---- 2-CTA cluster tile exchange of the split kernels: each CTA of a pair loads one 16-row half of every tile box and
+// multicasts it into both CTAs' shared memory (halves the L2 -> SM traffic of the all-gather: tools/ubench/ubench_lstm.cu)
+constexpr int kTileRowE = kSplitK * 16 + 8;     // elements per tile row: a warp's 48 columns + 8 (112 B: conflict-free ldmatrix)
+constexpr int kHalfE = 2 * 16 * kTileRowE;      // one box: [hi, lo][16 rows][kTileRowE]
+constexpr uint32_t kSlotBytes = 2 * kHalfE * 2; // both row halves of one tile slot
+__device__ __forceinline__ uint32_t cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the peer CTA's copy of a local shared-memory mbarrier
+__device__ __forceinline__ uint32_t peer_addr(const void* p, uint32_t peer) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(peer));
+  return r;
+}
+__device__ __forceinline__ void mbar_arrive_local(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+}
+// wait on an mbarrier phase that the peer CTA's warp also arrives on (acquire at cluster scope)
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "LAB_WAIT_%=:\n"
+      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
+      "@p bra LAB_DONE_%=;\n"
+      "bra LAB_WAIT_%=;\n"
+      "LAB_DONE_%=:\n"
+      "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+// generic-proxy global writes (h / gate-gradient stores) vs the TMA reads of the same bytes
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// one box of a rank-4 / rank-5 map into the same shared-memory offset of both CTAs of the pair; completes tx on the
+// mbarrier at `bar`'s offset in each of them
+__device__ __forceinline__ void tma_multicast_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(
+          smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"((uint16_t)3)
+      : "memory");
+}
+__device__ __forceinline__ void tma_multicast_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;" ::"r"(
+          smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "h"((uint16_t)3)
+      : "memory");
+}
+// 128-byte aligned start of the dynamic shared memory (TMA destinations); the kernels request 128 bytes of slack
+__device__ __forceinline__ unsigned char* smem_align128(unsigned char* p) {
+  return p + ((128u - (smem_u32(p) & 127u)) & 127u);
+}
+
 // hi.hi + hi.lo + lo.hi (small terms first) of one m16n8k16 tile product
 __device__ __forceinline__ void mma3(float (&c)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint32_t bh0, uint32_t bh1,
                                      uint32_t bl0, uint32_t bl1) {
@@ -1634,16 +1694,30 @@ __device__ __forceinline__ void mma3(float (&c)[4], const uint32_t (&ah)[4], con
   mma_bf16_16816(c, ah, bh0, bh1);
 }
 
-__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(WaveFwdSplitArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_b[];
+// hq_map[l]: the hq planes of layer l as a rank-4 map {Hq, B, T1 + 1, plane}, box {kTileRowE, 16, 1, 2}: rows >= B and
+// columns >= Hq are zero-filled.  Launched as 2-CTA clusters; a padding CTA (index >= a.nctas, all units past H) only
+// takes part in the loads.
+__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(const __grid_constant__ CUtensorMap hq_map0,
+                                                                               const __grid_constant__ CUtensorMap hq_map1,
+                                                                               WaveFwdSplitArgs a) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  unsigned char* const smem_b = smem_align128(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
   const int H = a.H, Hq = a.Hq, B = a.B;
-  // tiles: [0] h0 hi, [1] h0 lo, [2] h1 hi, [3] h1 lo; each [32][Hq]
-  __nv_bfloat16* X = reinterpret_cast<__nv_bfloat16*>(smem_b);
-  const int tile = 32 * Hq;
+  const bool idle = blockIdx.x >= a.nctas;
+  // warp-private tiles [group: h0, h1][row half = CTA rank that loads it][hi, lo][16 rows][kTileRowE] of this warp's 48 columns
+  __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_b) + int64_t(wrp) * 4 * kHalfE;
   typedef float PartT[2][16][33];
-  PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(4) * tile * 2);  // [11 warps][set][col][row]
+  PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes);  // [11 warps][set][col][row]
   __shared__ float act_s[2][4][kStepUnits][33];
+  // per warp: full[group] (this CTA's expect_tx, both CTAs' bytes), empty (this warp + the peer CTA's warp done reading)
+  __shared__ __align__(8) uint64_t full_s[kSplitWarps][2], empty_s[kSplitWarps];
+  const uint32_t rank = cluster_rank();
+  if (lane == 0) {
+    mbar_init(&full_s[wrp][0], 1); mbar_init(&full_s[wrp][1], 1); mbar_init(&empty_s[wrp], 2);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  const uint32_t peer_empty = peer_addr(&empty_s[wrp], rank ^ 1u);
   const int j0 = blockIdx.x * kStepUnits;
   const int rows = (B < 32) ? B : 32;
   const int ksteps = (H + 15) / 16;
@@ -1687,7 +1761,8 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
   __nv_bfloat16* const hq_u = ul ? a.hq[1] : a.hq[0];
   __nv_bfloat16* const hmq_u = ul ? a.hmq[1] : a.hmq[0];
   float c_state = updrole ? a.c0[(int64_t(ul) * B + ur) * H + j0 + uu] : 0.f;  // c_{t-1} of this (layer, row, unit)
-  if (updthread) csb_u[int64_t(blockIdx.x) * 128 + (tid & 127)] = c_state;    // slot 0
+  if (updthread && !idle) csb_u[int64_t(blockIdx.x) * 128 + (tid & 127)] = c_state;    // slot 0
+  cluster_sync_all();   // the peer's mbarriers are initialised before any multicast or remote arrive
   for (int s = 0; s <= a.T1; ++s) {
     const bool act0 = (s < a.T1), act1 = (s >= 1);
     // inputs that do not depend on other CTAs: issued before the wait
@@ -1704,9 +1779,9 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       if (tu < a.T1 - 1) nd_n = __ldg(a.nd + int64_t(tu + 1) * B + ur);
     }
     // Every tile element is consumed by exactly ONE warp (K is split across the warps), so each warp waits only for the
-    // CTAs that produce ITS k-range (units [16*ks0, 16*ks0 + 48) -> 12 producer CTAs), pulls its own columns of the four
-    // tiles (cp.async, one commit group per k-step) and starts its MMAs on k-step 0 while k-steps 1, 2 are still in
-    // flight - no block-wide barrier between the hand-off and the products.  (History: 130 threads per CTA polling 130
+    // CTAs that produce ITS k-range (units [16*ks0, 16*ks0 + 48) -> 12 producer CTAs) and fetches its own columns of the
+    // four planes - no block-wide barrier between the hand-off and the products.  The same warp of the peer CTA needs the
+    // same columns: each loads one 16-row half and multicasts it to both.  (History: 130 threads per CTA polling 130
     // flag words - 17 k pollers chip-wide on 5 cache lines - made the L2 slices of those lines the bottleneck: ncu
     // showed over a third of all samples in the spin.)
     if (s > 0) {
@@ -1715,8 +1790,19 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       if (lane < 12 && p0 < pend && p0 < int(a.nctas)) {
         while (ld_relaxed_u32(a.flags + p0 * kFlagStride) < unsigned(s)) {}
         (void)ld_acquire_u32(a.flags + p0 * kFlagStride);
+        fence_proxy_async_global();
       }
       __syncwarp();
+    }
+    if (lane == 0) {
+      // Two groups: the h0 planes first, so the layer-0 / input-projection MMAs start while the h1 planes land.  At s = 0
+      // the h1 group (slot 0) is loaded but not used, which keeps one phase per step on every barrier.
+      if (s > 0) mbar_wait_cluster(&empty_s[wrp], (s - 1) & 1);   // both CTAs' warps have read step s-1's tiles
+      fence_proxy_async_global();
+      mbar_expect_tx(&full_s[wrp][0], kSlotBytes);
+      tma_multicast_4d(X + rank * kHalfE, &hq_map0, &full_s[wrp][0], ks0 * 16, 16 * int(rank), s, 0);
+      mbar_expect_tx(&full_s[wrp][1], kSlotBytes);
+      tma_multicast_4d(X + (2 + rank) * kHalfE, &hq_map1, &full_s[wrp][1], ks0 * 16, 16 * int(rank), s > 0 ? s - 1 : 0, 0);
     }
     float m0[2][2], m1[2][2];   // done masks of this thread's accumulator rows (layer 0 at t = s, layer 1 at t = s-1)
 #pragma unroll
@@ -1728,30 +1814,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
         m1[mt][hh] = (r < rows && act1) ? __ldg(a.nd + int64_t(s - 1) * B + r) : 0.f;
       }
     {
-      const __nv_bfloat16* src0 = a.hq[0] + int64_t(s) * B * Hq;
-      const __nv_bfloat16* src1 = a.hq[1] + int64_t(s > 0 ? s - 1 : 0) * B * Hq;
-      // this warp's 48 columns (96 contiguous bytes per row) of each plane: lanes walk (row, 16-byte chunk) with the chunk
-      // fastest - ~6 cache lines per warp instruction (a (row, half-k-step) walk touched 16 and ran the LSU 3x longer).
-      // Two commit groups: the h0 planes first, so the layer-0 / input-projection MMAs start while the h1 planes land.
-#pragma unroll
-      for (int grp = 0; grp < 2; ++grp) {
-        if (grp == 0 || act1) {
-          const __nv_bfloat16* src = (grp ? src1 : src0) + ks0 * 16;
-          __nv_bfloat16* dst = X + grp * 2 * tile + ks0 * 16;
-#pragma unroll
-          for (int i = 0; i < 6; ++i) {
-            const int j = lane + 32 * i;            // 192 (row, chunk) pairs
-            const int r = j / 6, c = j - r * 6;
-            if (r < rows && (ks0 * 16 + c * 8) < ksteps * 16) {
-              cp_async16(dst + r * Hq + c * 8, src + int64_t(r) * Hq + c * 8);
-              cp_async16(dst + tile + r * Hq + c * 8, src + a.hq_lo + int64_t(r) * Hq + c * 8);
-            }
-          }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-      }
-    }
-    {
       float acc0[2][2][4], accI[2][2][4], acc1[2][2][4];
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
@@ -1759,17 +1821,16 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
         for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
           for (int e = 0; e < 4; ++e) { acc0[mt][nt][e] = 0.f; accI[mt][nt][e] = 0.f; acc1[mt][nt][e] = 0.f; }
-      asm volatile("cp.async.wait_group 1;" ::: "memory");   // the h0 planes
-      __syncwarp();
+      mbar_wait(&full_s[wrp][0], s & 1);   // the h0 planes
 #pragma unroll
       for (int sk = 0; sk < kSplitK; ++sk) {
         if (ks0 + sk < ksteps) {
 #pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {
+          for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = the row half CTA rank mt loaded
             uint32_t ah[4], al[4];
-            const int off = (mt * 16 + (lane & 15)) * Hq + (ks0 + sk) * 16 + (lane >> 4) * 8;
+            const int off = mt * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
             ldmatrix_x4(ah, X + off);
-            ldmatrix_x4(al, X + tile + off);
+            ldmatrix_x4(al, X + 16 * kTileRowE + off);
             if (act0) {
               mma3(acc0[mt][0], ah, al, bh[0][sk][0][0], bh[0][sk][0][1], bl[0][sk][0][0], bl[0][sk][0][1]);
               mma3(acc0[mt][1], ah, al, bh[0][sk][1][0], bh[0][sk][1][1], bl[0][sk][1][0], bl[0][sk][1][1]);
@@ -1781,8 +1842,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
           }
         }
       }
-      asm volatile("cp.async.wait_group 0;" ::: "memory");   // the h1 planes
-      __syncwarp();
+      mbar_wait(&full_s[wrp][1], s & 1);   // the h1 planes
       if (act1) {
 #pragma unroll
         for (int sk = 0; sk < kSplitK; ++sk) {
@@ -1790,14 +1850,19 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
               uint32_t ah[4], al[4];
-              const int off = (mt * 16 + (lane & 15)) * Hq + (ks0 + sk) * 16 + (lane >> 4) * 8;
-              ldmatrix_x4(ah, X + 2 * tile + off);
-              ldmatrix_x4(al, X + 3 * tile + off);
+              const int off = (2 + mt) * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
+              ldmatrix_x4(ah, X + off);
+              ldmatrix_x4(al, X + 16 * kTileRowE + off);
               mma3(acc1[mt][0], ah, al, bh[2][sk][0][0], bh[2][sk][0][1], bl[2][sk][0][0], bl[2][sk][0][1]);
               mma3(acc1[mt][1], ah, al, bh[2][sk][1][0], bh[2][sk][1][1], bl[2][sk][1][0], bl[2][sk][1][1]);
             }
           }
         }
+      }
+      __syncwarp();
+      if (lane == 0) {   // this warp's tiles are read: free them for both loaders of step s+1
+        mbar_arrive_local(&empty_s[wrp]);
+        mbar_arrive_remote(peer_empty);
       }
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
@@ -1853,26 +1918,27 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       const uint32_t vh = uint32_t(__bfloat16_as_ushort(hh)), vl = uint32_t(__bfloat16_as_ushort(hl));
       const uint32_t ph = vh | (__shfl_down_sync(0xffffffffu, vh, 1) << 16), pl = vl | (__shfl_down_sync(0xffffffffu, vl, 1) << 16);
       const uint32_t ph2 = __shfl_down_sync(0xffffffffu, ph, 2), pl2 = __shfl_down_sync(0xffffffffu, pl, 2);
-      if (live && uu == 0 && ur < rows) {
+      if (live && !idle && uu == 0 && ur < rows) {
         __nv_bfloat16* d = hq_u + (int64_t(tu + 1) * B + ur) * Hq + j0;
         *reinterpret_cast<uint2*>(d) = make_uint2(ph, ph2);
         *reinterpret_cast<uint2*>(d + a.hq_lo) = make_uint2(pl, pl2);
+        fence_proxy_async_global();   // consumers read h through TMA
       }
     }
     __syncthreads();
-    if (tid == 0 && s < a.T1) {
+    if (tid == 0 && s < a.T1 && !idle) {
       asm volatile("fence.acq_rel.gpu;" ::: "memory");
       st_relaxed_u32(a.flags + blockIdx.x * kFlagStride, unsigned(s + 1));
     }
     // ---- everything below is consumed by this CTA or after the kernel: off the critical path ----
     // activated gates -> CTA-blocked [row][16] tiles, straight from act_s (rewritten only after the next step's barrier)
-    for (int idx = tid; idx < 1024; idx += kSplitThreads) {
+    for (int idx = tid; idx < 1024 && !idle; idx += kSplitThreads) {
       const int l = idx >> 9, e = idx & 511, row = e >> 4, c = e & 15;
       const int tl = s - l;
       if ((l ? act1 : act0) && row < rows)
         a.gact[l][(int64_t(tl) * a.nctas + blockIdx.x) * 512 + e] = act_s[l][c >> 2][c & 3][row];
     }
-    if (updthread) {
+    if (updthread && !idle) {
       // masked recurrent input of the NEXT step (h_t * notdone_{t+1}) for the weight-gradient GEMMs, as hi / lo planes
       const float hm = h_new * nd_n;
       const __nv_bfloat16 mh = __float2bfloat16_rn(hm);
@@ -1898,13 +1964,14 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       }
     }
   }
+  cluster_sync_all();   // no CTA exits with multicast writes or remote arrives into it still in flight
 }
 
 // ---- split-precision backward wavefront (precision 2) ----------------------------------------------
 // lstm2_bwd_wave_mma_kernel's role split (CTAs [0, nc): upper layer recurrence + dL/dh_lower from the same tile;
 // CTAs [nc, 2nc): lower layer two wave steps behind; 8 hidden units per CTA) with hi/lo operand planes:
 //   * the four gate-gradient tiles of a step are 4 x (hi + lo) x 34 KB = 274 KB - more than shared memory - so they
-//     stream through a 2-deep ring by gate (cp.async of gate g+1 under the MMAs of gate g);
+//     stream through a 2-deep ring by gate (the multicast TMA boxes of gate g+2 under the MMAs of gate g+1);
 //   * 11 MMA warps x 3 k16-steps cover one gate's K = 528 exactly; W_hh^T (and, upper role, W_ih_upper^T) as hi AND lo
 //     B fragments in registers (96 per thread);
 //   * per-CTA flags instead of the counter barrier (see lstm2_fwd_wave_split_kernel): a CTA waits for the CTAs of its
@@ -1919,28 +1986,44 @@ struct WaveBwdSplitArgs {
   __nv_bfloat16* dgb_up; __nv_bfloat16* dgb_lo; int lg; int64_t dgb_lo_off;   // gate gradients of all steps, hi plane (+ lo offset)
   float* db_up; float* db_lo;
   __nv_bfloat16* dgq_up; __nv_bfloat16* dgq_lo; int64_t dgq_lo_off;          // exchange planes: [2][4, B, Hq] (+ lo offset)
-  float* dxb;                       // dL/dh_lower, blocked [T1][nc][32 rows][8 cols]: upper role -> lower role
+  float* dxb;                       // dL/dh_lower, blocked [T1][ncol][32 rows][8 cols]: upper role -> lower role
   unsigned* flags;                  // [2 * nc]
-  int T1, B, H, Hq; unsigned nc;
+  int T1, B, H, Hq;
+  unsigned nc;                      // CTAs per role, padded to whole clusters
+  unsigned ncol;                    // CTAs per role that own columns < H (= ceil(H / 8))
 };
 
-__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(WaveBwdSplitArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_b[];
+// dgq_map[role]: that role's exchange planes as a rank-5 map {Hq, B, gate, ping-pong buffer, plane}, box
+// {kTileRowE, 16, 1, 1, 2}: rows >= B and columns >= Hq are zero-filled.  Launched as 2-CTA clusters, every pair within
+// one role; a role's padding CTA (index >= ncol, all columns past H) takes part in the loads and the flag protocol only.
+__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(const __grid_constant__ CUtensorMap dgq_map_up,
+                                                                               const __grid_constant__ CUtensorMap dgq_map_lo,
+                                                                               WaveBwdSplitArgs a) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  unsigned char* const smem_b = smem_align128(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
   const int H = a.H, Hq = a.Hq, B = a.B;
   // Every tile element is consumed by exactly one warp (K = (gate, unit) is split across the warps: this warp owns units
   // [16*ks0, 16*ks0 + 48) of every gate), so the tiles stream through WARP-PRIVATE 2-slot rings - slot = one gate,
-  // [hi, lo][32 rows][48 units], rows padded to 56 elements (112 B: conflict-free ldmatrix) - with no block barrier
-  // anywhere in the fetch / MMA phase.
-  constexpr int kRowE = kSplitK * 16 + 8;                        // elements per ring row
-  constexpr int kPlaneE = 32 * kRowE;                            // one plane of one slot
-  __nv_bfloat16* X = reinterpret_cast<__nv_bfloat16*>(smem_b) + int64_t(wrp) * 4 * kPlaneE;  // [2 slots][hi, lo][32][kRowE]
+  // [row half = CTA rank that loads it][hi, lo][16 rows][kTileRowE] - with no block barrier anywhere in the fetch / MMA
+  // phase.  The same warp of the peer CTA streams the same columns: each CTA loads one row half and multicasts it.
+  __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_b) + int64_t(wrp) * 4 * kHalfE;
   typedef float PartT[2][kBwdCols][33];
-  PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(kSplitWarps) * 4 * kPlaneE * 2);  // [11 warps][product][col][row]
+  PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes);  // [11 warps][product][col][row]
   __shared__ float dh_s[kBwdCols][33];
   __shared__ float dc_s[kBwdCols][33];
   __shared__ __align__(16) __nv_bfloat16 stg_s[2][4][32][kBwdCols];       // [plane][gate][row][col]
+  // per warp and ring slot: full (this CTA's expect_tx, both CTAs' bytes), empty (this warp + the peer CTA's warp done)
+  __shared__ __align__(8) uint64_t full_s[kSplitWarps][2], empty_s[kSplitWarps][2];
+  const uint32_t rank = cluster_rank();
+  if (lane == 0) {
+    mbar_init(&full_s[wrp][0], 1); mbar_init(&full_s[wrp][1], 1);
+    mbar_init(&empty_s[wrp][0], 2); mbar_init(&empty_s[wrp][1], 2);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  const uint32_t peer_empty0 = peer_addr(&empty_s[wrp][0], rank ^ 1u), peer_empty1 = peer_addr(&empty_s[wrp][1], rank ^ 1u);
   const bool upper = blockIdx.x < a.nc;
+  const CUtensorMap* const dgq_map = upper ? &dgq_map_up : &dgq_map_lo;
   const int cidx = int(upper ? blockIdx.x : blockIdx.x - a.nc);
   const int k0 = cidx * kBwdCols;
   const int rows = B < 32 ? B : 32;
@@ -1951,6 +2034,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   const float* const csb = upper ? a.csb_up : a.csb_lo;
   __nv_bfloat16* const dgb = upper ? a.dgb_up : a.dgb_lo;
   __nv_bfloat16* const dgq = upper ? a.dgq_up : a.dgq_lo;
+  const bool idle = cidx >= int(a.ncol);
   // B fragments: B[kk][n] = W[g*H + j][k0 + n] for kk = (gate g, j)
   uint32_t bh[4][kSplitK][2], bl[4][kSplitK][2], ih[4][kSplitK][2], il[4][kSplitK][2];
   // The pointwise operands of the NEXT step (forward saves: 4 gates, c, masked c_prev, dy, 2 done masks) are prefetched
@@ -1958,7 +2042,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   // to local memory (168-register cap with the 96 fragment registers) and their load latency landed on the critical path.
   // layout: [0,1024) activated gates of the two forward CTAs whose units this CTA owns ([2][32 rows][16]); [1024,1280) c_t
   // ([2][32][4]); [1280,1536) c_{t-1}; [1536,1792) dy ([32 rows][8 cols], upper role); [1792,1856) notdone_t, notdone_{t+1}
-  float* const pre_s = reinterpret_cast<float*>(smem_b + size_t(kSplitWarps) * 4 * kPlaneE * 2 + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33);
+  float* const pre_s = reinterpret_cast<float*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33);
   {
     const int n = lane >> 2;
 #pragma unroll
@@ -1982,7 +2066,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
       }
   }
   if (wrp < kBwdCols) { dh_s[wrp][lane] = 0.0f; dc_s[wrp][lane] = 0.0f; }
-  __syncthreads();
+  cluster_sync_all();   // also: the peer's mbarriers are initialised before any multicast or remote arrive
   const int64_t gs = int64_t(B) * Hq;      // one gate of one exchange buffer
   const int q = wrp;  // pointwise role: thread = (batch row lane, unit k0 + wrp), warps 0..7
   const bool actA = (wrp < kBwdCols && lane < rows && k0 + q < H);
@@ -2019,7 +2103,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   };
   auto fetch_dxm = [&](int t) {
     if (upper || !actA || t < 0 || t >= a.T1) return;
-    n_dy = __ldcg(a.dxb + (int64_t(t) * a.nc + cidx) * 256 + lane * 8 + q);
+    n_dy = __ldcg(a.dxb + (int64_t(t) * a.ncol + cidx) * 256 + lane * 8 + q);
   };
   // gate-gradient rows of all steps for the hoisted weight-gradient GEMMs ([N, lg] hi / lo planes): written from the staging
   // tile with 8 lanes per 16-byte run (4 cache lines per warp store; one 2-byte store per lane-row touched 32)
@@ -2038,6 +2122,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   unsigned* const my_flag = a.flags + blockIdx.x * kFlagStride;
   const unsigned* const role_flags = a.flags + (upper ? 0 : a.nc) * kFlagStride;
   int it = 0;  // this role's active-step counter
+  bool fetched = false;   // a tile fetch has run (the ring's empty barriers have completed phases)
   for (int s = 0; s <= last_s; ++s) {
     const int t = time_of(s);
     const bool active = (t >= 0 && t < a.T1);
@@ -2077,10 +2162,11 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         }
       }
       __syncthreads();
-      if (tid < 256 && (tid & 31) < rows) {
+      if (tid < 256 && (tid & 31) < rows && !idle) {
         const int pl = tid >> 7, g = (tid >> 5) & 3, bb = tid & 31;
         *reinterpret_cast<uint4*>(dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(bb) * Hq + k0) =
             *reinterpret_cast<const uint4*>(&stg_s[pl][g][bb][0]);
+        fence_proxy_async_global();   // consumers read the tiles through TMA
       }
     }
     if (s == last_s) {
@@ -2099,9 +2185,10 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     {
       const int p0 = (ks0 * 16) / kBwdCols + lane;
       const int pend = (min((ks0 + kSplitK) * 16, H) + kBwdCols - 1) / kBwdCols;
-      if (lane < 6 && p0 < pend && p0 < int(a.nc)) {
+      if (lane < 6 && p0 < pend && p0 < int(a.ncol)) {
         while (ld_relaxed_u32(role_flags + p0 * kFlagStride) < unsigned(s + 1)) {}
         (void)ld_acquire_u32(role_flags + p0 * kFlagStride);
+        fence_proxy_async_global();
       } else if (!upper && lane == 8 && wrp < kBwdCols) {
         while (ld_relaxed_u32(a.flags + cidx * kFlagStride) < unsigned(s + 1)) {}
         (void)ld_acquire_u32(a.flags + cidx * kFlagStride);
@@ -2112,50 +2199,47 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     const bool need_rec = active && t > 0;
     const bool need_dx = active && upper;
     if (need_rec || need_dx) {
-      auto issue = [&](int g) {   // this warp's 48 columns of gate g, hi and lo plane: 32 rows x 6 chunks x 2 = 12 per lane
-        const __nv_bfloat16* src = dgq_t + int64_t(g) * gs + ks0 * 16;
-        __nv_bfloat16* dst = X + int64_t(g & 1) * 2 * kPlaneE;
-#pragma unroll
-        for (int i = 0; i < 6; ++i) {
-          const int j = lane + 32 * i;            // 192 (row, chunk) pairs
-          const int r = j / 6, c = j - r * 6;
-          if (r < rows && (ks0 * 16 + c * 8) < kpg * 16) {
-            cp_async16(dst + r * kRowE + c * 8, src + int64_t(r) * Hq + c * 8);
-            cp_async16(dst + kPlaneE + r * kRowE + c * 8, src + a.dgq_lo_off + int64_t(r) * Hq + c * 8);
-          }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+      // Ring slot g & 1 holds gate g: its full and empty barriers complete twice per fetching step (gates g & 1 and
+      // (g & 1) + 2), so the phase parity of gate g is g >> 1 on the full barrier; before gate g is loaded, the empty
+      // barrier's previous phase (gate g - 2, or gate g + 2 of the previous fetching step) must have completed.
+      auto issue = [&](int g) {   // lane 0: this CTA's row half of this warp's columns of gate g, both planes
+        if (g >= 2 || fetched) mbar_wait_cluster(&empty_s[wrp][g & 1], g >= 2 ? 0u : 1u);
+        fence_proxy_async_global();
+        mbar_expect_tx(&full_s[wrp][g & 1], kSlotBytes);
+        tma_multicast_5d(X + ((g & 1) * 2 + rank) * kHalfE, dgq_map, &full_s[wrp][g & 1], ks0 * 16, 16 * int(rank), g, it & 1, 0);
       };
       float acc0[2][4], acc1[2][4];
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
         for (int e = 0; e < 4; ++e) { acc0[mt][e] = 0.f; acc1[mt][e] = 0.f; }
-      issue(0);
-      issue(1);
+      if (lane == 0) { issue(0); issue(1); }
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        if (g < 3) asm volatile("cp.async.wait_group 1;" ::: "memory");
-        else asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncwarp();
-        const __nv_bfloat16* Xg = X + int64_t(g & 1) * 2 * kPlaneE;
+        mbar_wait(&full_s[wrp][g & 1], uint32_t(g >> 1));
+        const __nv_bfloat16* Xg = X + (g & 1) * 2 * kHalfE;
 #pragma unroll
         for (int sk = 0; sk < kSplitK; ++sk) {
           if (ks0 + sk < kpg) {
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {
+            for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = the row half CTA rank mt loaded
               uint32_t ah[4], al[4];
-              const int off = (mt * 16 + (lane & 15)) * kRowE + sk * 16 + (lane >> 4) * 8;
+              const int off = mt * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
               ldmatrix_x4(ah, Xg + off);
-              ldmatrix_x4(al, Xg + kPlaneE + off);
+              ldmatrix_x4(al, Xg + 16 * kTileRowE + off);
               if (need_rec) mma3(acc0[mt], ah, al, bh[g][sk][0], bh[g][sk][1], bl[g][sk][0], bl[g][sk][1]);
               if (need_dx) mma3(acc1[mt], ah, al, ih[g][sk][0], ih[g][sk][1], il[g][sk][0], il[g][sk][1]);
             }
           }
         }
         __syncwarp();
-        if (g + 2 < 4) issue(g + 2);
+        if (lane == 0) {   // slot read: free it for both loaders
+          mbar_arrive_local(&empty_s[wrp][g & 1]);
+          mbar_arrive_remote((g & 1) ? peer_empty1 : peer_empty0);
+          if (g + 2 < 4) issue(g + 2);
+        }
       }
+      fetched = true;
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         const int r = mt * 16 + (lane >> 2), c = (lane & 3) * 2;
@@ -2176,7 +2260,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
           float d = 0.f;
 #pragma unroll
           for (int w = 0; w < kSplitWarps; ++w) d += part[w][1][wrp][lane];
-          if (lane < rows) a.dxb[(int64_t(t) * a.nc + cidx) * 256 + lane * 8 + wrp] = d;
+          if (lane < rows && !idle) a.dxb[(int64_t(t) * a.ncol + cidx) * 256 + lane * 8 + wrp] = d;
         }
       }
     }
@@ -2191,6 +2275,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
       db[k0 + q] = bs_i; db[H + k0 + q] = bs_f; db[2 * H + k0 + q] = bs_g; db[3 * H + k0 + q] = bs_o;
     }
   }
+  cluster_sync_all();   // no CTA exits with multicast writes or remote arrives into it still in flight
 }
 
 static size_t g_fwd_mma_attr_dev[64] = {0}, g_bwd_mma_attr_dev[64] = {0};
@@ -2269,21 +2354,60 @@ __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const
   hmq[i] = m; hmq[hmq_lo + i] = __float2bfloat16_rn(hm - __bfloat162float(m));
 }
 
+// The split kernels run as one cooperative grid of 2-CTA clusters: launch configuration with both attributes
+struct ClusterCoopLaunch {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[2];
+  ClusterCoopLaunch(dim3 grid, size_t smem, cudaStream_t st) {
+    cfg.gridDim = grid; cfg.blockDim = dim3(kSplitThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeCooperative; attr[1].val.cooperative = 1;
+    cfg.attrs = attr; cfg.numAttrs = 2;
+  }
+};
+// coop_fit for a grid of 2-CTA clusters: every cluster of the grid must be co-resident (the kernels spin on flags
+// written by other CTAs)
+template <typename Kernel>
+static int cluster_coop_fit(Kernel kernel, dim3 grid, size_t smem, size_t* attr_smem) {
+  int dev = 0, coop = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+  if (!coop) return 0;
+  if (*attr_smem < smem) {
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
+      cudaGetLastError();
+      return 0;
+    }
+    *attr_smem = smem;
+  }
+  ClusterCoopLaunch l(grid, smem, nullptr);
+  int clusters = 0;
+  if (cudaOccupancyMaxActiveClusters(&clusters, kernel, &l.cfg) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return int64_t(clusters) * 2 >= int64_t(grid.x);
+}
+
 static size_t g_fwd_split_attr_dev[64] = {0};
-static size_t wave_fwd_split_smem(int Hq) { return size_t(4) * 32 * Hq * 2 + sizeof(float) * kSplitWarps * 2 * 16 * 33; }
+static size_t wave_fwd_split_smem() {   // tiles + partial sums + alignment slack
+  return size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128;
+}
+// forward CTAs: kStepUnits units each, padded to whole clusters
+static dim3 wave_fwd_split_grid(int H) { return dim3(((H + kStepUnits - 1) / kStepUnits + 1) & ~1, 1); }
 // precision 2, two layers: the split-bf16 wavefront kernel (other shapes run the exact-fp32 recurrence kernels)
 static bool wave_fwd_split_applicable(int64_t B, int In, int H) {
   if (B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
+  const dim3 grid = wave_fwd_split_grid(H);
   if (int(grid.x) > kSplitThreads || grid.x > 512) return false;
-  return coop_fit(lstm2_fwd_wave_split_kernel, grid, wave_fwd_split_smem(mma_hq(H)), kSplitThreads,
-                  per_device(g_fwd_split_attr_dev));
+  return cluster_coop_fit(lstm2_fwd_wave_split_kernel, grid, wave_fwd_split_smem(), per_device(g_fwd_split_attr_dev));
 }
 
 static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, const float* c0, float* hN,
                                 float* cN, int64_t T1, int64_t B, int H, cudaStream_t st) {
   const int Hq = mma_hq(H);
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
+  const dim3 grid = wave_fwd_split_grid(H);
   cudaError_t e = cudaMemsetAsync(ws.flags, 0, sizeof(unsigned) * 512 * kFlagStride, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   WaveFwdSplitArgs a;
@@ -2298,10 +2422,16 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
   a.hq_lo = ws.layer[0].hq_lo; a.hmq_lo = ws.layer[0].hmq_lo;
   TB_REQUIRE(ws.layer[1].hq_lo == a.hq_lo && ws.layer[1].hmq_lo == a.hmq_lo && a.hq_lo > 0, "lstm: split planes missing");
   a.nd = notdone; a.flags = ws.flags;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = grid.x;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm2_fwd_wave_split_kernel, grid, dim3(kSplitThreads), args,
-                                  wave_fwd_split_smem(Hq), st);
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = unsigned((H + kStepUnits - 1) / kStepUnits);
+  CUtensorMap maps[2];
+  for (int l = 0; l < 2; ++l) {
+    const uint64_t dims[4] = {uint64_t(Hq), uint64_t(B), uint64_t(T1 + 1), 2};
+    const uint64_t strides[3] = {uint64_t(Hq) * 2, uint64_t(B) * Hq * 2, uint64_t(a.hq_lo) * 2};
+    const uint32_t box[4] = {kTileRowE, 16, 1, 2};
+    tcd::make_map_nd(&maps[l], a.hq[l], 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  ClusterCoopLaunch l(grid, wave_fwd_split_smem(), st);
+  e = cudaLaunchKernelEx(&l.cfg, lstm2_fwd_wave_split_kernel, maps[0], maps[1], a);
   TB_REQUIRE(e == cudaSuccess, "lstm2_fwd_wave_split_kernel: %s", cudaGetErrorString(e));
   return check_launch("lstm2_fwd_wave_split_kernel");
 }
@@ -2737,22 +2867,22 @@ static int lstm2_bwd_wave(LstmWs& ws, const LstmParams& p, const LstmGrads& g, c
 }
 
 static size_t g_bwd_split_attr_dev[64] = {0};
-static size_t wave_bwd_split_smem(int) {
-  return size_t(kSplitWarps) * 4 * 32 * (kSplitK * 16 + 8) * 2 + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33 +
-         sizeof(float) * 9 * 256;   // tile rings + partial sums + prefetched pointwise operands
+static size_t wave_bwd_split_smem() {   // tile rings + partial sums + prefetched pointwise operands + alignment slack
+  return size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33 + sizeof(float) * 9 * 256 + 128;
 }
+// CTAs per role: kBwdCols columns each, padded to whole clusters (a cluster never straddles the two roles)
+static unsigned wave_bwd_split_role_ctas(int H) { return unsigned(((H + kBwdCols - 1) / kBwdCols + 1) & ~1); }
 static bool wave_bwd_split_applicable(int64_t B, int In, int H) {
   if (!wave_fwd_split_applicable(B, In, H)) return false;  // consumes the planes the split forward leaves behind
-  dim3 grid(2 * ((H + kBwdCols - 1) / kBwdCols), 1);
+  dim3 grid(2 * wave_bwd_split_role_ctas(H), 1);
   if (int(grid.x / 2) + 1 > kSplitThreads || grid.x > 512) return false;
-  return coop_fit(lstm2_bwd_wave_split_kernel, grid, wave_bwd_split_smem(mma_hq(H)), kSplitThreads,
-                  per_device(g_bwd_split_attr_dev));
+  return cluster_coop_fit(lstm2_bwd_wave_split_kernel, grid, wave_bwd_split_smem(), per_device(g_bwd_split_attr_dev));
 }
 
 static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone,
                                 int64_t T1, int64_t B, int H, cudaStream_t st) {
   const int Hq = mma_hq(H);
-  const unsigned nc = unsigned((H + kBwdCols - 1) / kBwdCols);
+  const unsigned nc = wave_bwd_split_role_ctas(H);
   const LstmLayerWs& U = ws.layer[1];
   const LstmLayerWs& L = ws.layer[0];
   unsigned* flags = ws.flags + 512 * kFlagStride;
@@ -2771,10 +2901,16 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   a.db_up = g.b_ih[1]; a.db_lo = g.b_ih[0];
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq); a.dgq_lo_off = U.dgq_lo;
   a.dxb = ws.dxb; a.flags = flags;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm2_bwd_wave_split_kernel, dim3(2 * nc), dim3(kSplitThreads), args,
-                                  wave_bwd_split_smem(Hq), st);
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc; a.ncol = unsigned((H + kBwdCols - 1) / kBwdCols);
+  CUtensorMap maps[2];
+  for (int r = 0; r < 2; ++r) {
+    const uint64_t dims[5] = {uint64_t(Hq), uint64_t(B), 4, 2, 2};
+    const uint64_t strides[4] = {uint64_t(Hq) * 2, uint64_t(B) * Hq * 2, uint64_t(4) * B * Hq * 2, uint64_t(a.dgq_lo_off) * 2};
+    const uint32_t box[5] = {kTileRowE, 16, 1, 1, 2};
+    tcd::make_map_nd(&maps[r], r == 0 ? a.dgq_up : a.dgq_lo, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  }
+  ClusterCoopLaunch l(dim3(2 * nc), wave_bwd_split_smem(), st);
+  e = cudaLaunchKernelEx(&l.cfg, lstm2_bwd_wave_split_kernel, maps[0], maps[1], a);
   TB_REQUIRE(e == cudaSuccess, "lstm2_bwd_wave_split_kernel: %s", cudaGetErrorString(e));
   return check_launch("lstm2_bwd_wave_split_kernel");
 }

@@ -123,7 +123,7 @@ inline int make_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t col
 // multiples of 16).  Dimensions may overlap in memory - that is how the implicit-GEMM convolutions express
 // "patch (ox, oy) of frame n, kernel row offset e0" as plain TMA coordinates.
 inline int make_map_nd(CUtensorMap* map, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                       const uint32_t* box) {
+                       const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn fn = encode_fn();
   TB_REQUIRE(fn, "gemm_tc: cuTensorMapEncodeTiled is not available from the driver");
   TB_REQUIRE(rank >= 2 && rank <= 5 && (reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "gemm_tc: bad tensor map arguments");
@@ -135,7 +135,7 @@ inline int make_map_nd(CUtensorMap* map, const void* ptr, int rank, const uint64
     gstride[i] = strides_bytes[i];
   }
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstride, bx, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   TB_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled (rank %d) failed (%d)", rank, int(r));
   return 0;
