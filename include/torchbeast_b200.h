@@ -222,6 +222,50 @@ int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const flo
                        const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
                        int use_lstm, int precision, void* workspace, float* grads, void* stream);
 
+/* ---- unstacked rollouts: four-frame stacks rebuilt on the GPU ------------------------------------------------------
+ * Each frame sits in four consecutive stacks, so a stacked `frame` leaf u8 [T1,B,4,84,84] is three quarters copies.  An
+ * unstacked rollout of T1 = T+1 steps carries the same information as frames u8 [T1+3, B, HW] (HW = 84*84), contiguous:
+ *   rows 0..2 = channels 0..2 (oldest first) of step 0's stack;  row 3+t = the newest channel of step t's stack;
+ * with done [T1,B] bool or uint8, any non-zero value marking the first step of an episode (the environment reports
+ * done = 1 on an episode's first frame, and FrameStack.reset fills all four channels with it).  Channel c (0..3) of step t's
+ * stack in column b is
+ *   stack[t,b,c] = frames[3 + max(t - 3 + c, last_done(t,b)), b],
+ *   last_done(t,b) = the largest s in [0,t] with done[s,b] != 0, or -3 if there is none.
+ * An actor writes its current stack's four channels into rows 0..3 at the start of a rollout, then one newest frame per
+ * step; row 0 of a rollout repeats the previous rollout's last step, as for stacked leaves.  The LSTM's notdone
+ * ((~done).float(), a bitwise NOT for uint8) is unaffected: only the restack reads done as "non-zero".             */
+
+/* stacked_out u8 [T1,B,4,HW] = the stacks of frames u8 [T1+3,B,HW] / done [T1,B] (u8 or bool bytes).  HW % 16 == 0;
+ * frames and stacked_out 16-byte aligned.  One bandwidth-bound launch.                                               */
+int tb_restack_frames_u8(const uint8_t* frames, const uint8_t* done, int64_t T1, int64_t B, int64_t HW, uint8_t* stacked_out,
+                         void* stream);
+/* Bytes of stacked_scratch the *_forward_unstacked entries need for net (0 = AtariNet, 1 = ResNet) at this precision:
+ * 0 where the restack is fused into the backend's frame-image pass (AtariNet bf16 / bf16x3, ResNet bf16x3),
+ * T1*B*4*84*84 where the backend reads stacked frames (AtariNet fp32, ResNet fp32 / bf16).  SIZE_MAX for an unknown net,
+ * precision or a size < 1.                                                                                           */
+size_t tb_unstacked_scratch_bytes(int net, int64_t T1, int64_t B, int precision);
+/* tb_atarinet_forward / tb_resnet_forward on an unstacked rollout: the same arguments, with the stacked frame replaced
+ * by frames u8 [T1+3,B,84,84] + done [T1,B], and stacked_scratch (device memory of tb_unstacked_scratch_bytes bytes;
+ * NULL allowed, and not touched, when that is 0).  Logits, baseline, final state and the workspace contents are
+ * bit-identical to the stacked entry on the restacked frames.  tb_atarinet_backward / _phase follow this forward
+ * unchanged: they read only the workspace.                                                                          */
+int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                  const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                  int64_t T1, int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
+                                  void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
+                                  void* stream);
+int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
+                                int num_actions, int use_lstm, int precision, void* workspace, void* stacked_scratch,
+                                float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
+/* Backward of tb_resnet_forward_unstacked (gradients bit-identical to tb_resnet_backward after the stacked forward).
+ * It reads: the workspace, always; stacked_scratch only at precision 0 / 1, where it must still hold the frames that
+ * forward restacked into it (precision 2 reads the first conv's input image from the workspace, and stacked_scratch may
+ * be NULL).  No frames or done are read.                                                                            */
+int tb_resnet_backward_unstacked(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
+                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
+                                 int use_lstm, int precision, void* workspace, float* grads, void* stream);
+
 /* ---- learner-queue ingest, host side (SURVEY 8(f) N1) --------------------------------------------------
  * One actor writes its [T1, ...] rollout into batch column b of a pinned [T1, B, ...] slot (replaces the per-rollout
  * tensors + torch::cat of src/cc/actorpool.cc:49-55,493-506): leaf l of the slot starts at slot_base + leaf_offset[l], one

@@ -57,6 +57,11 @@ _SIGNATURES = {
     "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),
+    "tb_restack_frames_u8": ([_vp, _vp, _i64, _i64, _i64, _vp, _vp], _int),
+    "tb_unstacked_scratch_bytes": ([_int, _i64, _i64, _int], _c.c_size_t),
+    "tb_atarinet_forward_unstacked": ([_vp] * 8 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_resnet_forward_unstacked": ([_vp] * 7 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_resnet_backward_unstacked": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_host_write_rollout_column": ([_vp, _vp, _vp, _int, _i64, _i64, _i64, _vp], _int),
     "tb_lstm_workspace_bytes": ([_i64, _i64, _int, _int, _int, _int], _c.c_size_t),
     "tb_lstm_forward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 5, _int),

@@ -109,6 +109,9 @@ class GraphedActor:
 
     def __call__(self, inputs, core_state=()):
         model = self.model
+        if inputs["frame"].dim() != 5:
+            raise _lib.TorchBeastB200Error("GraphedActor takes stacked frames [1, B, 4, 84, 84]; unstacked rollouts are a "
+                                           "learner input, got frame %r" % (tuple(inputs["frame"].shape),))
         sampler = replay_sampler(model)
         _lib.require_cuda(model.flat_params)
         T, B = inputs["frame"].shape[:2]

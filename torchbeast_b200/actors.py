@@ -7,7 +7,12 @@ PINNED `[T+1, B, ...]` slot of a RolloutStager (N1: no per-rollout tensors, no t
 whose B columns are complete is handed to the learner threads through `LearnerQueue` as the reference's nest
 `((env_outputs, actor_outputs), initial_agent_state)` (SURVEY 8(b) B2) whose leaves ARE the slot's tensors, so
 polybeast_learner.learn() submits it with one async H2D copy.  Row 0 of every rollout repeats the last row of that
-actor's previous rollout (actorpool.cc:443).  Out of scope: real environments / inference (SURVEY section 2)."""
+actor's previous rollout (actorpool.cc:443).  Out of scope: real environments / inference (SURVEY section 2).
+
+Frames and `done` come from synthetic environment streams that follow the reference's actor side: done = 1 on the first
+frame of every episode (core/environment.py), and FrameStack(4) fills all four slots with that frame.  frame_format=
+"unstacked" hands over the same steps as one newest frame per step (staging.spec_for(..., frame_format="unstacked")), so
+one seed gives the same stacks in both formats."""
 import collections
 import queue
 import threading
@@ -44,8 +49,33 @@ class LearnerQueue:
         return item
 
 
+def _frame_stream(rs, steps, done_prob=0.01, hw=(84, 84)):
+    """One column's environment stream as a cycle: (stacks u8 [steps, 4, *hw], done bool [steps]).  Step 0 starts an
+    episode (initial()); the last step starts one on step 0's frame again, so its stack equals step 0's and the stream
+    can be handed over round and round with row 0 of each rollout repeating the previous rollout's last row."""
+    obs = rs.randint(0, 256, size=(steps,) + tuple(hw), dtype=np.uint8)
+    done = rs.rand(steps) < done_prob
+    done[0] = done[-1] = True
+    obs[-1] = obs[0]
+    stacks = np.empty((steps, 4) + tuple(hw), dtype=np.uint8)
+    slots = collections.deque(maxlen=4)
+    for s in range(steps):
+        if done[s]:
+            slots.extend([obs[s]] * 4)  # FrameStack.reset
+        else:
+            slots.append(obs[s])        # FrameStack.step
+        stacks[s] = np.stack(slots)
+    return torch.from_numpy(stacks), torch.from_numpy(done)
+
+
 class SyntheticActors:
-    def __init__(self, stager, num_actors, T, B, num_actions, learner_queue, state_shape=None, seed=0, frame_pool=8):
+    POOL = 4  # rollouts each actor hands over in turn
+
+    def __init__(self, stager, num_actors, T, B, num_actions, learner_queue, state_shape=None, seed=0, frame_pool=8,
+                 frame_format="stacked"):
+        if frame_format not in ("stacked", "unstacked"):
+            raise ValueError("frame_format must be 'stacked' or 'unstacked', got %r" % (frame_format,))
+        self.frame_format = frame_format
         self.stager, self.n, self.T, self.B, self.A = stager, num_actors, T, B, num_actions
         self.queue = learner_queue
         self.state_shape = state_shape  # (layers, H) or None
@@ -58,9 +88,18 @@ class SyntheticActors:
         self._threads = []
         self.rollouts = 0
         rs = np.random.RandomState(seed)
-        # a small pool of pre-rendered frame stacks per actor: the host work per rollout is the copy into the pinned column,
-        # as it is for a real actor handing over frames it received from its environment
-        self._frames = torch.from_numpy(rs.randint(0, 256, size=(frame_pool, T + 1, 4, 84, 84), dtype=np.uint8))
+        # `frame_pool` environment streams, each cut into POOL chained rollouts; actor k hands over those of stream
+        # k % frame_pool.  The host work per rollout is the copy into the pinned column, as it is for a real actor handing
+        # over frames it received from its environment.
+        T1 = T + 1
+        self._rollout_frames, self._rollout_done = [], []
+        for _ in range(frame_pool):
+            stacks, done = _frame_stream(rs, self.POOL * T + 1)
+            rolls = [stacks[j * T:j * T + T1] for j in range(self.POOL)]
+            if frame_format == "unstacked":
+                rolls = [torch.cat([r[0, :3], r[:, 3]]) for r in rolls]
+            self._rollout_frames.append(rolls)
+            self._rollout_done.append([done[j * T:j * T + T1] for j in range(self.POOL)])
         self._seed = seed
 
     def _claim(self):
@@ -94,29 +133,30 @@ class SyntheticActors:
                 state = tuple(torch.zeros(layers, self.B, H) for _ in range(2))
             self.queue.put(((env, agent), state))
 
-    def _make_pool(self, k, pool=4):
+    def _make_pool(self, k):
         """A few pre-generated rollouts per actor (what its environment steps would have produced): the per-rollout host work
         that remains is the hand-over into the pinned column, as for a real actor."""
         rs = np.random.RandomState(self._seed * 1000 + k)
-        T1, A = self.T + 1, self.A
+        T1, A, pool = self.T + 1, self.A, self.POOL
+        stream = k % len(self._rollout_frames)
         out = []
         for j in range(pool):
             out.append(dict(
-                frame=self._frames[(k + j) % self._frames.shape[0]],
+                frame=self._rollout_frames[stream][j],
                 reward=torch.from_numpy(rs.randn(T1).astype(np.float32)),
-                done=torch.from_numpy(rs.rand(T1) < 0.01),
+                done=self._rollout_done[stream][j],
                 episode_return=torch.from_numpy(rs.randn(T1).astype(np.float32)),
                 episode_step=torch.from_numpy(rs.randint(0, 1000, size=T1).astype(np.int32)),
                 policy_logits=torch.from_numpy(rs.randn(T1, A).astype(np.float32)),
                 baseline=torch.from_numpy(rs.randn(T1).astype(np.float32)),
                 action=torch.from_numpy(rs.randint(0, A, size=T1).astype(np.int64))))
         # row 0 of a rollout = last row of this actor's previous rollout (actorpool.cc:443): the pool is handed over cyclically,
-        # so that overlap is baked in once (own copies of the shared frame stacks: row 0 differs per actor)
-        out = [dict(r, frame=r["frame"].clone()) for r in out]
+        # so that overlap is baked in once (the shared frame / done streams are cycles that already have it)
         for j in range(pool):
             prev = out[(j - 1) % pool]
             for key, v in out[j].items():
-                v[0].copy_(prev[key][-1])
+                if key not in ("frame", "done"):
+                    v[0].copy_(prev[key][-1])
         return [self.stager.prepare_rollout(r) for r in out]
 
     def _actor(self, k):

@@ -16,6 +16,7 @@
 #include "heads.cuh"
 #include "lstm.cuh"
 #include "net_kernels.cuh"
+#include "restack.cuh"
 
 namespace tb {
 
@@ -178,7 +179,9 @@ static int pick_splits(int64_t M, int64_t N, int64_t K) {
 // ---------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------
-static int atarinet_forward(const uint8_t* frame, const float* reward, const float* notdone,
+// done == nullptr: frame is stacked u8 [T1,B,4,84,84]; otherwise frame is an unstacked rollout u8 [T1+3,B,84,84] whose stacks
+// the tensor-core backends rebuild in their frame-image pass (the fp32 backend is handed restacked frames by its caller)
+static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                             const int64_t* last_action, const float* h0, const float* c0, const float* P,
                             int64_t T1, int64_t B, int A, int use_lstm, int precision, void* workspace,
                             float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st) {
@@ -201,7 +204,10 @@ static int atarinet_forward(const uint8_t* frame, const float* reward, const flo
     // implicit GEMM: frames -> bf16 image once (kept in frameb for the backward), producer warps gather the
     // patches from it into the UMMA smem layout
     te.b_lo = w.w1b.lo;  // the pixels are exact in bf16: only the weights have a lo plane
-    TB_TRY(frames_u8_to_bf16(frame, w.frameb, N * G::C0 * G::H0 * G::W0, st));
+    if (done)
+      TB_TRY(frames_u8_unstacked_to_bf16(frame, done, T1, B, int64_t(G::H0) * G::W0, w.frameb, st));
+    else
+      TB_TRY(frames_u8_to_bf16(frame, w.frameb, N * G::C0 * G::H0 * G::W0, st));
     TB_TRY(conv_u8_fwd_implicit(w.frameb, w.w1b, N, G::H0, G::W0, G::S1, te, st));
     // conv2 / conv3: implicit GEMM - TMA gathers the patches from the NHWC activation (rank-4 map with
     // overlapping dimensions)
@@ -449,8 +455,31 @@ int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* 
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "atarinet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2,
              "atarinet_forward: precision must be 0 (fp32 SIMT), 1 (bf16 tensor cores) or 2 (split-bf16 tensor cores)");
-  return atarinet_forward(frame, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
+  return atarinet_forward(frame, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
                           workspace, policy_logits, baseline, hN, cN, (cudaStream_t)stream);
+}
+
+int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                  const int64_t* last_action, const float* h0, const float* c0, const float* params, int64_t T1,
+                                  int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
+                                  void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
+                                  void* stream) {
+  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward_unstacked: bad sizes T1=%lld B=%lld A=%d",
+             (long long)T1, (long long)B, num_actions);
+  TB_REQUIRE(frames && done && reward && last_action && params && workspace && policy_logits && baseline,
+             "atarinet_forward_unstacked: null pointer");
+  TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "atarinet_forward_unstacked: LSTM needs notdone/h0/c0/hN/cN");
+  TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_forward_unstacked: precision must be 0, 1 or 2");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision)  // fused: the frame-image pass reads the unstacked rows
+    return atarinet_forward(frames, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
+                            precision, workspace, policy_logits, baseline, hN, cN, st);
+  TB_REQUIRE(stacked_scratch, "atarinet_forward_unstacked: the fp32 backend needs stacked_scratch "
+                              "(tb_unstacked_scratch_bytes bytes)");
+  uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
+  TB_TRY(restack_frames_u8(frames, done, T1, B, int64_t(AtariGeom::H0) * AtariGeom::W0, stacked, st));
+  return atarinet_forward(stacked, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
+                          precision, workspace, policy_logits, baseline, hN, cN, st);
 }
 
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,

@@ -20,6 +20,7 @@
 #include "conv3x3_sw.cuh"
 
 #include "tc_common.cuh"
+#include "restack.cuh"
 
 namespace tb {
 
@@ -669,6 +670,36 @@ __global__ void sw_frames_u8_kernel(const uint8_t* __restrict__ frame, __nv_bflo
   }
 }
 
+// the same image (Cf = 4) from an unstacked rollout: channel c of frame n = (t, b) is row unstacked_row(t, b, c)
+__global__ void sw_frames_u8_unstacked_kernel(const uint8_t* __restrict__ frames, const uint8_t* __restrict__ done,
+                                              __nv_bfloat16* __restrict__ out, int64_t lo_off, int64_t T1, int64_t B, int H,
+                                              int W, int slack_units) {
+  const int Hp = H + 2, Wp = W + 2;
+  const int64_t total = T1 * B * 2 * Hp * Wp;
+  if (blockIdx.x == 0) zero_slack_units(out, lo_off, total * 8, slack_units);
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int px = int(i % Wp);
+    int64_t t = i / Wp;
+    const int py = int(t % Hp); t /= Hp;
+    const int cv = int(t & 1);
+    const int64_t n = t >> 1;
+    uint4 ph = make_uint4(0u, 0u, 0u, 0u);
+    if (cv == 0 && py >= 1 && py <= H && px >= 1 && px <= W) {
+      const int64_t ts = n / B, b = n - ts * B;
+      float f[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        f[c] = float(__ldg(frames + ((unstacked_row(done, ts, b, B, c) * B + b) * H + (py - 1)) * W + (px - 1)));
+      __nv_bfloat162 p0 = __floats2bfloat162_rn(f[0], f[1]), p1 = __floats2bfloat162_rn(f[2], f[3]);
+      ph.x = *reinterpret_cast<uint32_t*>(&p0); ph.y = *reinterpret_cast<uint32_t*>(&p1);
+    }
+    __nv_bfloat16* dst = out + i * 8;
+    *reinterpret_cast<uint4*>(dst) = ph;
+    *reinterpret_cast<uint4*>(dst + lo_off) = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 // column sums of the block partials [blocks][C] in two levels (fixed association: deterministic): level 1 = kColsumSlices
 // blocks, each folding a contiguous slice of rows with coalesced reads (thread = (row group, channel)); level 2 = one block
 constexpr int kColsumSlices = 128;
@@ -810,6 +841,17 @@ int sw_frames_u8(const uint8_t* frame, __nv_bfloat16* out, int64_t lo_off, int64
   if (total == 0) return 0;
   sw_frames_u8_kernel<<<sgrid(total, 256), 256, 0, stream>>>(frame, out, lo_off, Nf, Cf, H, W, sw_geom(H, W).pin + 8);
   return check_launch("sw_frames_u8_kernel");
+}
+
+int sw_frames_u8_unstacked(const uint8_t* frames, const uint8_t* done, __nv_bfloat16* out, int64_t lo_off, int64_t T1, int64_t B,
+                           int H, int W, cudaStream_t stream) {
+  ProfScope prof("frames_to_image", stream);
+  TB_REQUIRE(frames && done && lo_off % 8 == 0, "sw_frames_u8_unstacked: null pointer or misaligned lo plane");
+  const int64_t total = T1 * B * 2 * (H + 2) * (W + 2);
+  if (total == 0) return 0;
+  sw_frames_u8_unstacked_kernel<<<sgrid(total, 256), 256, 0, stream>>>(frames, done, out, lo_off, T1, B, H, W,
+                                                                       sw_geom(H, W).pin + 8);
+  return check_launch("sw_frames_u8_unstacked_kernel");
 }
 
 int64_t sw_weight_elems(int O, int C) { return int64_t(2) * 9 * O * C; }

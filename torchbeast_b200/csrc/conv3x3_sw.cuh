@@ -26,6 +26,9 @@ int sw_pool_bwd_image_colsum(const uint8_t* argmax, const float* dy_pooled, __nv
 // uint8 NCHW frames [Nf, Cf <= 8, H, W] -> padded planar image with 16 channels (channels >= Cf and the whole lo plane are
 // zero; pixel values 0..255 are exact in bf16): the first convolution of the net through the same kernels
 int sw_frames_u8(const uint8_t* frame, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int Cf, int H, int W, cudaStream_t stream);
+// the same image (Cf = 4, byte-identical) from an unstacked rollout: frames u8 [T1+3, B, H, W], done [T1, B] (restack.cuh)
+int sw_frames_u8_unstacked(const uint8_t* frames, const uint8_t* done, __nv_bfloat16* out, int64_t lo_off, int64_t T1, int64_t B,
+                           int H, int W, cudaStream_t stream);
 
 // weights [O, C, 3, 3] fp32 -> the shared-memory image of the B operand (sw_weight_elems(O, C) elements; R operand rows,
 // the hi rows of a block followed by its lo rows so that [w_hi | w_lo] is one 2R-row operand):

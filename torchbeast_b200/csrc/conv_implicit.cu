@@ -22,6 +22,7 @@
 #include "conv_implicit.cuh"
 
 #include "gemm_simt.cuh"  // splitk_reduce_kernel / GemmEpilogue
+#include "restack.cuh"
 #include "tc_common.cuh"
 
 namespace tb {
@@ -369,6 +370,30 @@ __global__ void frames_u8_to_bf16_kernel(const uint8_t* __restrict__ in, __nv_bf
     for (int64_t i = nvec << 4; i < count; ++i) out[i] = __float2bfloat16_rn(float(in[i]));
 }
 
+// the same image from an unstacked rollout: vector i of plane (n, c) is read from the row unstacked_row() names
+__global__ void frames_u8_unstacked_to_bf16_kernel(const uint8_t* __restrict__ frames, const uint8_t* __restrict__ done,
+                                                   int64_t T1, int64_t B, int64_t vpp, __nv_bfloat16* __restrict__ out) {
+  const int64_t nvec = T1 * B * 4 * vpp;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec; i += stride) {
+    const int64_t plane = i / vpp;
+    const int c = int(plane & 3);
+    const int64_t n = plane >> 2, t = n / B, b = n - t * B;
+    const int64_t row = unstacked_row(done, t, b, B, c);
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(frames) + (row * B + b) * vpp + (i - plane * vpp));
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      o[2 * j] = u8pair_to_bf16x2(w[j], 0x7650, 0x7651);
+      o[2 * j + 1] = u8pair_to_bf16x2(w[j], 0x7652, 0x7653);
+    }
+    uint4* dst = reinterpret_cast<uint4*>(out) + 2 * i;
+    dst[0] = make_uint4(o[0], o[1], o[2], o[3]);
+    dst[1] = make_uint4(o[4], o[5], o[6], o[7]);
+  }
+}
+
 ConvGeom make_geom(int64_t N, int H, int W, int S) {
   ConvGeom g;
   g.H = H; g.W = W; g.S = S; g.OH = (H - 8) / S + 1; g.OW = (W - 8) / S + 1;
@@ -391,6 +416,22 @@ int frames_u8_to_bf16(const uint8_t* frame, void* frame_bf16, int64_t count, cud
   if (blocks < 1) blocks = 1;
   frames_u8_to_bf16_kernel<<<(unsigned)blocks, 256, 0, stream>>>(frame, static_cast<__nv_bfloat16*>(frame_bf16), count);
   return check_launch("frames_u8_to_bf16_kernel");
+}
+
+int frames_u8_unstacked_to_bf16(const uint8_t* frames, const uint8_t* done, int64_t T1, int64_t B, int64_t HW,
+                                void* frame_bf16, cudaStream_t stream) {
+  TB_REQUIRE(frames && done && frame_bf16 && (reinterpret_cast<uintptr_t>(frames) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(frame_bf16) & 15) == 0,
+             "frames_u8_unstacked_to_bf16: null or unaligned pointer");
+  TB_REQUIRE(HW % 16 == 0, "frames_u8_unstacked_to_bf16: HW must be a multiple of 16");
+  ProfScope prof("frames_to_bf16", stream);
+  const int64_t vpp = HW / 16;
+  int64_t blocks = (T1 * B * 4 * vpp + 255) / 256;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  if (blocks < 1) blocks = 1;
+  frames_u8_unstacked_to_bf16_kernel<<<(unsigned)blocks, 256, 0, stream>>>(frames, done, T1, B, vpp,
+                                                                           static_cast<__nv_bfloat16*>(frame_bf16));
+  return check_launch("frames_u8_unstacked_to_bf16_kernel");
 }
 
 bool conv_u8_implicit_applicable(int C, int H, int W, int KH, int KW, int S, int O) {

@@ -10,6 +10,10 @@ bool conv_u8_implicit_applicable(int C, int H, int W, int KH, int KW, int S, int
 
 // frames u8 NCHW -> bf16 NCHW (exact), the operand image of the two kernels below
 int frames_u8_to_bf16(const uint8_t* frame, void* frame_bf16, int64_t count, cudaStream_t stream);
+// the same image [T1*B, 4, HW] (byte-identical) from an unstacked rollout: frames u8 [T1+3, B, HW], done [T1, B]
+// (restack.cuh); HW % 16 == 0
+int frames_u8_unstacked_to_bf16(const uint8_t* frames, const uint8_t* done, int64_t T1, int64_t B, int64_t HW,
+                                void* frame_bf16, cudaStream_t stream);
 
 // act[N*OH*OW, 32] (bf16, ep.C16) = relu(ep.scale * patches(frame) . W^T + ep.bias); w_bf16 [32, 256] with
 // k = (c*8 + kh)*8 + kw (the reference weight's own flattening).  Split-bf16: ep.b_lo = lo plane of the weights

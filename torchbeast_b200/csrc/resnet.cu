@@ -18,6 +18,7 @@
 #include "net_kernels.cuh"
 #include "resnet_kernels.cuh"
 #include "conv3x3_sw.cuh"
+#include "restack.cuh"
 
 namespace tb {
 
@@ -424,9 +425,11 @@ struct SplitImpl {
     return sw_conv_fwd(xp, xp_lo, wi, out, N, S, S, cin, cout, ep, st);
   }
 
-  static int forward(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                     const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* policy_logits,
-                     float* baseline, float* hN, float* cN, cudaStream_t st) {
+  // done == nullptr: frame is stacked u8 [T1,B,4,84,84]; otherwise an unstacked rollout u8 [T1+3,B,84,84], restacked by the
+  // pass that writes the first conv's input image
+  static int forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone, const float* h0,
+                     const float* c0, const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace,
+                     float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st) {
     const int64_t N = T1 * B;
     const ResParams pp = res_params(A, use_lstm);
     W w = res_ws<float>(workspace, N, T1, B, A, use_lstm, true);
@@ -436,7 +439,10 @@ struct SplitImpl {
       if (i == 0) {
         // the first conv through the same kernels: frame pixels (exact in bf16) as a 16-channel image, 1/255 in the epilogue
         TB_TRY(sw_pack_weights(P + pp.feat[0].w, w.wi_feat[0], ch, 16, 0, st, 4));
-        TB_TRY(sw_frames_u8(frame, w.xp_feat[0], w.xp_feat_lo[0], N, 4, S, S, st));
+        if (done)
+          TB_TRY(sw_frames_u8_unstacked(frame, done, w.xp_feat[0], w.xp_feat_lo[0], T1, B, S, S, st));
+        else
+          TB_TRY(sw_frames_u8(frame, w.xp_feat[0], w.xp_feat_lo[0], N, 4, S, S, st));
         SwEpilogue ep; ep.scale = 1.0f / 255.0f; ep.bias = P + pp.feat[0].b; ep.tag = "feat_conv_fwd";
         TB_TRY(sw_conv_fwd(w.xp_feat[0], w.xp_feat_lo[0], w.wi_feat[0], w.s[0].P, N, S, S, 16, ch, ep, st));
       } else {
@@ -499,8 +505,9 @@ struct SplitImpl {
     return 0;
   }
 
-  static int backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                      const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st) {
+  // reads no frames: the first conv's weight gradient uses the input image the forward left in the workspace
+  static int backward(const float* grad_logits, const float* grad_baseline, const float* notdone, const float* P, int64_t T1,
+                      int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st) {
     const int64_t N = T1 * B;
     const ResParams pp = res_params(A, use_lstm);
     W w = res_ws<float>(workspace, N, T1, B, A, use_lstm, true);
@@ -589,8 +596,8 @@ int tb_resnet_forward(const uint8_t* frame, const float* reward, const float* no
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
   if (precision == 2)
-    return SplitImpl::forward(frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace, policy_logits,
-                              baseline, hN, cN, (cudaStream_t)stream);
+    return SplitImpl::forward(frame, nullptr, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
+                              policy_logits, baseline, hN, cN, (cudaStream_t)stream);
   if (precision)
     return Impl<__nv_bfloat16>::forward(frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
                                         policy_logits, baseline, hN, cN, (cudaStream_t)stream);
@@ -606,13 +613,57 @@ int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const flo
   TB_REQUIRE(!use_lstm || notdone, "resnet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward: precision must be 0, 1 or 2");
   if (precision == 2)
-    return SplitImpl::backward(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
-                               grads, (cudaStream_t)stream);
+    return SplitImpl::backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads,
+                               (cudaStream_t)stream);
   if (precision)
     return Impl<__nv_bfloat16>::backward(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm,
                                          workspace, grads, (cudaStream_t)stream);
   return Impl<float>::backward(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
                                grads, (cudaStream_t)stream);
+}
+
+int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B, int num_actions,
+                                int use_lstm, int precision, void* workspace, void* stacked_scratch, float* policy_logits,
+                                float* baseline, float* hN, float* cN, void* stream) {
+  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward_unstacked: bad sizes");
+  TB_REQUIRE(frames && done && reward && params && workspace && policy_logits && baseline,
+             "resnet_forward_unstacked: null pointer");
+  TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward_unstacked: LSTM needs notdone/h0/c0/hN/cN");
+  TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward_unstacked: precision must be 0, 1 or 2");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision == 2)  // fused into the first conv's image pass
+    return SplitImpl::forward(frames, done, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
+                              policy_logits, baseline, hN, cN, st);
+  TB_REQUIRE(stacked_scratch, "resnet_forward_unstacked: the fp32 / bf16 backends need stacked_scratch "
+                              "(tb_unstacked_scratch_bytes bytes)");
+  uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
+  TB_TRY(restack_frames_u8(frames, done, T1, B, 84 * 84, stacked, st));
+  if (precision)
+    return Impl<__nv_bfloat16>::forward(stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
+                                        policy_logits, baseline, hN, cN, st);
+  return Impl<float>::forward(stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace, policy_logits,
+                              baseline, hN, cN, st);
+}
+
+int tb_resnet_backward_unstacked(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
+                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
+                                 int use_lstm, int precision, void* workspace, float* grads, void* stream) {
+  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward_unstacked: bad sizes");
+  TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "resnet_backward_unstacked: null pointer");
+  TB_REQUIRE(!use_lstm || notdone, "resnet_backward_unstacked: LSTM needs notdone");
+  TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward_unstacked: precision must be 0, 1 or 2");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision == 2)
+    return SplitImpl::backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads, st);
+  TB_REQUIRE(stacked_scratch, "resnet_backward_unstacked: the fp32 / bf16 backends re-read the restacked frames from "
+                              "stacked_scratch");
+  const uint8_t* stacked = static_cast<const uint8_t*>(stacked_scratch);
+  if (precision)
+    return Impl<__nv_bfloat16>::backward(stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm,
+                                         workspace, grads, st);
+  return Impl<float>::backward(stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
+                               grads, st);
 }
 
 }  // extern "C"

@@ -331,6 +331,9 @@ class GraphedLearner:
         # the graph writes into the model workspace it was captured with; the model replaces (and frees) that buffer when
         # it runs another shape, e.g. while the GraphedLearner of another batch shape is captured: keep it alive here
         self.workspace = getattr(model, "_ws", None)
+        # the same holds for the stacked scratch an unstacked rollout is restacked into (AtariNet fp32, ResNet fp32 / bf16):
+        # the graph writes it, its forward reads it, and the ResNet backward reads it again
+        self.scratch = getattr(model, "_scratch_buf", None)
         self.graph.replay()  # first replay uploads the graph to the device; keep that out of the training loop
         torch.cuda.synchronize()
         # undo the warm-up / capture-time updates so training starts from the caller's weights

@@ -42,6 +42,44 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4):
     return spec
 
 
+def frame_is_unstacked(frame, reward):
+    """False for a stacked frame u8 [T1, B, 4, 84, 84]; True for an unstacked rollout u8 [T1+3, B, 84, 84] with
+    T1 = reward.shape[0] (include/torchbeast_b200.h, "unstacked rollouts").  Anything else raises."""
+    if frame.dtype != torch.uint8 or frame.dim() not in (4, 5):
+        raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84] or unstacked [T+3,B,84,84], got %s %r"
+                                       % (frame.dtype, tuple(frame.shape)))
+    if frame.dim() == 5:
+        if tuple(frame.shape[2:]) != (4, 84, 84):
+            raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84], got %s %r" % (frame.dtype, tuple(frame.shape)))
+        return False
+    T1, B = reward.shape[:2]
+    if tuple(frame.shape) != (T1 + 3, B, 84, 84):
+        raise _lib.TorchBeastB200Error(
+            "an unstacked frame must be uint8 [T1+3, B, 84, 84] with [T1, B] = reward's shape %r, got %r"
+            % ((T1, B), tuple(frame.shape)))
+    return True
+
+
+def _done_bytes(done, T1, B):
+    """The restack's view of `done`: [T1, B] bool or uint8 as contiguous bytes (non-zero = an episode starts)."""
+    if done is None or done.dtype not in (torch.bool, torch.uint8) or tuple(done.shape) != (T1, B):
+        raise _lib.TorchBeastB200Error("done must be bool or uint8 [%d, %d] with an unstacked frame, got %s"
+                                       % (T1, B, None if done is None else "%s %r" % (done.dtype, tuple(done.shape))))
+    return done.contiguous().view(torch.uint8)
+
+
+def _scratch(module, net, T1, B):
+    """Caller-owned stacked scratch for the backends that read stacked frames; None where the restack is fused."""
+    nbytes = _lib.lib().tb_unstacked_scratch_bytes(net, T1, B, module.PRECISIONS[module.precision])
+    if nbytes == 0:
+        return None
+    key = (T1, B, module._flat.device, module.precision)
+    if module._scratch_key != key:
+        module._scratch_buf = torch.empty(nbytes, dtype=torch.uint8, device=module._flat.device)
+        module._scratch_key = key
+    return module._scratch_buf
+
+
 def _numel(shape):
     n = 1
     for d in shape:
@@ -192,11 +230,11 @@ class _AtariNetFunction(torch.autograd.Function):
     learn() does not go through autograd (it calls learner_forward/learner_backward)."""
 
     @staticmethod
-    def forward(ctx, module, frame, reward, notdone, last_action, h0, c0, *params):
-        logits, baseline, hN, cN = module._launch_forward(frame, reward, notdone, last_action, h0, c0)
+    def forward(ctx, module, frame, done, reward, notdone, last_action, h0, c0, *params):
+        logits, baseline, hN, cN = module._launch_forward(frame, reward, notdone, last_action, h0, c0, done)
         ctx.module = module
         ctx.notdone = notdone
-        ctx.shape = frame.shape[:2]
+        ctx.shape = baseline.shape
         ctx.mark_non_differentiable(hN, cN)
         return logits, baseline, hN, cN
 
@@ -211,7 +249,7 @@ class _AtariNetFunction(torch.autograd.Function):
         grads = torch.empty_like(module._flat)
         module._launch_backward(g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
         outs = tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
-        return (None,) * 7 + outs
+        return (None,) * 8 + outs
 
 
 class AtariNet(FlatParamModule):
@@ -250,6 +288,7 @@ class AtariNet(FlatParamModule):
             raise _lib.TorchBeastB200Error("precision must be one of %s" % sorted(self.PRECISIONS))
         self._ws = None
         self._ws_key = None
+        self._scratch_buf = self._scratch_key = None
         count = _lib.lib().tb_atarinet_param_count(num_actions, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
@@ -268,11 +307,14 @@ class AtariNet(FlatParamModule):
             self._ws_key = key
         return self._ws
 
-    def _launch_forward(self, frame, reward, notdone, last_action, h0, c0):
+    def _launch_forward(self, frame, reward, notdone, last_action, h0, c0, done=None):
+        """`done` is read only with an unstacked frame (frame_is_unstacked), to rebuild the stacks."""
         _lib.require_cuda(frame, reward, last_action, self._flat)
-        T1, B = frame.shape[:2]
-        if frame.dtype != torch.uint8 or tuple(frame.shape[2:]) != self.observation_shape:
-            raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84], got %s %r" % (frame.dtype, tuple(frame.shape)))
+        unstacked = frame_is_unstacked(frame, reward)
+        T1, B = reward.shape[:2] if unstacked else frame.shape[:2]
+        if unstacked:
+            _lib.require_cuda(done)
+            done = _done_bytes(done, T1, B)
         dev = self._flat.device
         frame = frame.contiguous()
         reward = reward.to(torch.float32).contiguous()
@@ -288,6 +330,15 @@ class AtariNet(FlatParamModule):
             h0 = c0 = notdone = None
         ws = self._workspace(T1, B)
         p = _lib.ptr
+        if unstacked:
+            _lib.check(
+                _lib.lib().tb_atarinet_forward_unstacked(
+                    p(frame), p(done), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
+                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)),
+                    p(logits), p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None,
+                    _lib.stream_ptr()),
+                "tb_atarinet_forward_unstacked")
+            return logits, baseline, hN, cN
         _lib.check(
             _lib.lib().tb_atarinet_forward(
                 p(frame), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
@@ -331,7 +382,7 @@ class AtariNet(FlatParamModule):
         notdone = self._notdone(inputs["done"]) if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
         logits, baseline, hN, cN = self._launch_forward(
-            inputs["frame"], inputs["reward"], notdone, inputs["last_action"], h0, c0)
+            inputs["frame"], inputs["reward"], notdone, inputs["last_action"], h0, c0, inputs.get("done"))
         self._saved_notdone = notdone
         return LearnerOutputs(logits, baseline, (hN, cN) if self.use_lstm else tuple())
 
@@ -362,16 +413,17 @@ class AtariNet(FlatParamModule):
 
     # ---- reference-compatible forward ---------------------------------------------------------
     def forward(self, inputs, core_state=()):
-        frame = inputs["frame"]
-        T, B = frame.shape[:2]
-        notdone = self._notdone(inputs["done"]) if self.use_lstm else None
+        frame, done = inputs["frame"], inputs.get("done")
+        notdone = self._notdone(done) if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
         params = [v[0] for v in self._views]
         if torch.is_grad_enabled() and any(q.requires_grad for q in params):
             logits, baseline, hN, cN = _AtariNetFunction.apply(
-                self, frame, inputs["reward"], notdone, inputs["last_action"], h0, c0, *params)
+                self, frame, done, inputs["reward"], notdone, inputs["last_action"], h0, c0, *params)
         else:
-            logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"], h0, c0)
+            logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"], h0, c0,
+                                                            done)
+        T, B = baseline.shape
         if self.training:
             action = self._sample(logits, inputs)
         else:
@@ -406,24 +458,24 @@ def resnet_param_spec(num_actions, use_lstm):
 
 class _ResNetFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, module, frame, reward, notdone, h0, c0, *params):
-        logits, baseline, hN, cN = module._launch_forward(frame, reward, notdone, h0, c0)
-        ctx.module, ctx.notdone, ctx.frame = module, notdone, frame
+    def forward(ctx, module, frame, done, reward, notdone, h0, c0, *params):
+        logits, baseline, hN, cN, saved = module._launch_forward(frame, reward, notdone, h0, c0, done)
+        ctx.module, ctx.notdone, ctx.saved, ctx.shape = module, notdone, saved, baseline.shape
         ctx.mark_non_differentiable(hN, cN)
         return logits, baseline, hN, cN
 
     @staticmethod
     def backward(ctx, g_logits, g_baseline, _ghn, _gcn):
         module = ctx.module
-        T1, B = ctx.frame.shape[:2]
+        T1, B = ctx.shape
         dev = module._flat.device
         if g_logits is None:
             g_logits = torch.zeros(T1, B, module.num_actions, device=dev)
         if g_baseline is None:
             g_baseline = torch.zeros(T1, B, device=dev)
         grads = torch.empty_like(module._flat)
-        module._launch_backward(ctx.frame, g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
-        return (None,) * 6 + tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
+        module._launch_backward(ctx.saved, g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
+        return (None,) * 7 + tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
 
 
 class ResNet(FlatParamModule):
@@ -452,6 +504,7 @@ class ResNet(FlatParamModule):
             raise _lib.TorchBeastB200Error("ResNet precision must be 'fp32', 'bf16' or 'bf16x3'")
         self._ws = None
         self._ws_key = None
+        self._scratch_buf = self._scratch_key = None
         count = _lib.lib().tb_resnet_param_count(num_actions, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
@@ -472,11 +525,15 @@ class ResNet(FlatParamModule):
             self._ws_key = key
         return self._ws
 
-    def _launch_forward(self, frame, reward, notdone, h0, c0):
+    def _launch_forward(self, frame, reward, notdone, h0, c0, done=None):
+        """Returns (logits, baseline, hN, cN, saved): `saved` is what _launch_backward re-reads - the stacked frame, or
+        ("unstacked", stacked scratch or None).  `done` is read only with an unstacked frame, to rebuild the stacks."""
         _lib.require_cuda(frame, reward, self._flat)
-        T1, B = frame.shape[:2]
-        if frame.dtype != torch.uint8 or tuple(frame.shape[2:]) != (4, 84, 84):
-            raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84], got %s %r" % (frame.dtype, tuple(frame.shape)))
+        unstacked = frame_is_unstacked(frame, reward)
+        T1, B = reward.shape[:2] if unstacked else frame.shape[:2]
+        if unstacked:
+            _lib.require_cuda(done)
+            done = _done_bytes(done, T1, B)
         dev = self._flat.device
         frame = frame.contiguous()
         reward = reward.to(torch.float32).contiguous()
@@ -490,17 +547,35 @@ class ResNet(FlatParamModule):
             hN = cN = torch.empty(0, device=dev)
             h0 = c0 = notdone = None
         p = _lib.ptr
+        if unstacked:
+            scratch = _scratch(self, 1, T1, B)
+            _lib.check(
+                _lib.lib().tb_resnet_forward_unstacked(
+                    p(frame), p(done), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions,
+                    int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(scratch), p(logits),
+                    p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
+                "tb_resnet_forward_unstacked")
+            return logits, baseline, hN, cN, ("unstacked", scratch)
         _lib.check(
             _lib.lib().tb_resnet_forward(
                 p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_resnet_forward")
-        return logits, baseline, hN, cN
+        return logits, baseline, hN, cN, frame
 
-    def _launch_backward(self, frame, g_logits, g_baseline, notdone, grads_out):
+    def _launch_backward(self, saved, g_logits, g_baseline, notdone, grads_out):
         T1, B = g_baseline.shape
         p = _lib.ptr
+        if isinstance(saved, tuple):  # ("unstacked", scratch): the backward reads the workspace (+ the restacked scratch)
+            _lib.check(
+                _lib.lib().tb_resnet_backward_unstacked(
+                    p(saved[1]), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
+                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
+                    p(grads_out), _lib.stream_ptr()),
+                "tb_resnet_backward_unstacked")
+            return
+        frame = saved
         _lib.check(
             _lib.lib().tb_resnet_backward(
                 p(frame.contiguous()), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
@@ -512,8 +587,9 @@ class ResNet(FlatParamModule):
     def learner_forward(self, inputs, core_state=()):
         notdone = (~inputs["done"]).float().contiguous() if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
-        logits, baseline, hN, cN = self._launch_forward(inputs["frame"], inputs["reward"], notdone, h0, c0)
-        self._saved = (inputs["frame"], notdone)
+        logits, baseline, hN, cN, saved = self._launch_forward(inputs["frame"], inputs["reward"], notdone, h0, c0,
+                                                               inputs.get("done"))
+        self._saved = (saved, notdone)
         return LearnerOutputs(logits, baseline, (hN, cN) if self.use_lstm else tuple())
 
     @torch.no_grad()
@@ -524,15 +600,15 @@ class ResNet(FlatParamModule):
         return fg
 
     def forward(self, inputs, core_state=()):
-        frame = inputs["frame"]
-        T, B = frame.shape[:2]
-        notdone = (~inputs["done"]).float().contiguous() if self.use_lstm else None
+        frame, done = inputs["frame"], inputs.get("done")
+        notdone = (~done).float().contiguous() if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
         params = [v[0] for v in self._views]
         if torch.is_grad_enabled() and any(q.requires_grad for q in params):
-            logits, baseline, hN, cN = _ResNetFunction.apply(self, frame, inputs["reward"], notdone, h0, c0, *params)
+            logits, baseline, hN, cN = _ResNetFunction.apply(self, frame, done, inputs["reward"], notdone, h0, c0, *params)
         else:
-            logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, h0, c0)
+            logits, baseline, hN, cN, _ = self._launch_forward(frame, inputs["reward"], notdone, h0, c0, done)
+        T, B = baseline.shape
         if self.training:
             action = self._sample(logits, inputs)
         else:

@@ -19,6 +19,7 @@ import threading  # noqa: E402
 
 import torch  # noqa: E402
 
+from torchbeast_b200 import _lib  # noqa: E402
 from torchbeast_b200 import acting as _acting  # noqa: E402
 from torchbeast_b200 import learner as _learner  # noqa: E402
 from torchbeast_b200.nets import ResNet as Net  # noqa: E402,F401
@@ -61,6 +62,9 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
         for batch in inference_batcher:
             batched_env_outputs, agent_state = batch.get_inputs()
             frame, reward, done, *rest = batched_env_outputs
+            if frame.dim() != 5:
+                raise _lib.TorchBeastB200Error("inference takes stacked frames [1, B, 4, 84, 84]; unstacked rollouts are a "
+                                               "learner input, got frame %r" % (tuple(frame.shape),))
             inputs = dict(frame=frame.to(device, non_blocking=True), reward=reward.to(device, non_blocking=True),
                           done=done.to(device, non_blocking=True))
             if getattr(model, "needs_last_action", False):

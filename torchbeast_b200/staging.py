@@ -29,11 +29,19 @@ from torchbeast_b200 import _lib
 LEAF_ORDER = ("frame", "reward", "done", "episode_return", "episode_step", "policy_logits", "baseline", "action", "last_action")
 
 
-def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), extra=()):
-    """Leaf name -> (shape, dtype) of one [T+1, B, ...] rollout batch (monobeast.py:299-316 buffers / the B2 nest)."""
+FRAME_FORMATS = ("stacked", "unstacked")
+
+
+def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), extra=(), frame_format="stacked"):
+    """Leaf name -> (shape, dtype) of one [T+1, B, ...] rollout batch (monobeast.py:299-316 buffers / the B2 nest).
+    frame_format="unstacked": the frame leaf is [T+4, B, H, W], one newest frame per step after step 0's first three
+    channels; the learner rebuilds the stacks on the GPU (include/torchbeast_b200.h, "unstacked rollouts")."""
+    if frame_format not in FRAME_FORMATS:
+        raise ValueError("frame_format must be one of %s, got %r" % (FRAME_FORMATS, frame_format))
     T1 = T + 1
+    frame = (T1, B) + tuple(frame_shape) if frame_format == "stacked" else (T1 + 3, B) + tuple(frame_shape[1:])
     spec = collections.OrderedDict(
-        frame=((T1, B) + tuple(frame_shape), torch.uint8),
+        frame=(frame, torch.uint8),
         reward=((T1, B), torch.float32),
         done=((T1, B), torch.bool),
         episode_return=((T1, B), torch.float32),
@@ -110,51 +118,49 @@ class RolloutStager:
         return i
 
     def column(self, i, b):
-        """Views `[T+1, ...]` of batch column b of host slot i: what ONE actor fills (actorpool.cc:493-506 per rollout)."""
+        """Views `[T+1, ...]` of batch column b of host slot i: what ONE actor fills (actorpool.cc:493-506 per rollout).
+        With an unstacked spec the frame view is `[T+4, H, W]`: rows 0..3 = the four channels of the stack at the rollout's
+        first step, row 3+t = the newest frame of step t (include/torchbeast_b200.h, "unstacked rollouts")."""
         return collections.OrderedDict((k, v[:, b]) for k, v in self.host[i].items())
 
-    def prepare_rollout(self, rollout):
-        """Pre-built argument block for write_column() when the same host arrays are handed over repeatedly (a fixed pool of
-        synthetic rollouts): keeps the per-rollout Python work to one C call."""
+    def prepare_rollout(self, rollout, what="prepare_rollout"):
+        """Pre-built argument block for write_prepared() when the same host arrays are handed over repeatedly (a fixed pool
+        of synthetic rollouts): keeps the per-rollout Python work to one C call per distinct leaf row count (one call; two
+        with an unstacked frame leaf, whose T+4 rows differ from the other leaves' T+1)."""
         import ctypes
         names = [k for k in self.spec if k in rollout]
-        n = len(names)
-        T1, B = self.spec[names[0]][0][:2]
         for k in names:
             t = rollout[k]
-            if t.is_cuda or not t.is_contiguous() or t.dtype != self.spec[k][1] or t.numel() * t.element_size() != self._offs[k][1] // B:
-                raise _lib.TorchBeastB200Error("prepare_rollout: leaf %r must be a contiguous CPU [T+1, ...] tensor of the slot's dtype" % k)
-        offs = (ctypes.c_int64 * n)(*[self._offs[k][0] for k in names])
-        rows = (ctypes.c_int64 * n)(*[self._offs[k][1] // (T1 * B) for k in names])
-        srcs = (ctypes.c_void_p * n)(*[rollout[k].data_ptr() for k in names])
-        return (ctypes.cast(offs, ctypes.c_void_p), ctypes.cast(rows, ctypes.c_void_p), n, T1, B, ctypes.cast(srcs, ctypes.c_void_p),
-                (offs, rows, srcs, rollout))  # keep the arrays and tensors alive
+            if t.is_cuda or not t.is_contiguous() or t.dtype != self.spec[k][1] or \
+                    t.numel() * t.element_size() != self._offs[k][1] // self.spec[k][0][1]:
+                raise _lib.TorchBeastB200Error("%s: leaf %r must be a contiguous CPU [%d, ...] tensor of the slot's dtype"
+                                               % (what, k, self.spec[k][0][0]))
+        groups = collections.OrderedDict()  # leaf row count -> leaf names
+        for k in names:
+            groups.setdefault(self.spec[k][0][0], []).append(k)
+        calls = []
+        for rows_t, ks in groups.items():
+            n, B = len(ks), self.spec[ks[0]][0][1]
+            offs = (ctypes.c_int64 * n)(*[self._offs[k][0] for k in ks])
+            rows = (ctypes.c_int64 * n)(*[self._offs[k][1] // (rows_t * B) for k in ks])
+            srcs = (ctypes.c_void_p * n)(*[rollout[k].data_ptr() for k in ks])
+            calls.append((ctypes.cast(offs, ctypes.c_void_p), ctypes.cast(rows, ctypes.c_void_p), n, rows_t, B,
+                          ctypes.cast(srcs, ctypes.c_void_p), (offs, rows, srcs)))
+        return calls, rollout  # keep the arrays and tensors alive
 
     def write_prepared(self, i, b, prep):
         import ctypes
-        offs, rows, n, T1, B, srcs, _keep = prep
-        rc = _lib.lib().tb_host_write_rollout_column(ctypes.c_void_p(self._host_raw[i].data_ptr()), offs, rows, n, T1, B, int(b), srcs)
-        if rc:
-            _lib.check(rc, "tb_host_write_rollout_column")
+        base = ctypes.c_void_p(self._host_raw[i].data_ptr())
+        for offs, rows, n, T, B, srcs, _keep in prep[0]:
+            rc = _lib.lib().tb_host_write_rollout_column(base, offs, rows, n, T, B, int(b), srcs)
+            if rc:
+                _lib.check(rc, "tb_host_write_rollout_column")
 
     def write_column(self, i, b, rollout):
-        """Native per-actor hand-over: copy `rollout` (dict leaf -> contiguous [T+1, ...] CPU tensor) into column b of pinned
-        slot i with ONE C call (tb_host_write_rollout_column) that runs without the GIL - N actor threads then copy in
-        parallel instead of serialising on the interpreter."""
-        import ctypes
-        names = [k for k in self.spec if k in rollout]
-        n = len(names)
-        offs = (ctypes.c_int64 * n)(*[self._offs[k][0] for k in names])
-        T1, B = self.spec[names[0]][0][:2]
-        rows = (ctypes.c_int64 * n)(*[self._offs[k][1] // (T1 * B) for k in names])
-        srcs = (ctypes.c_void_p * n)(*[rollout[k].data_ptr() for k in names])
-        for k in names:
-            t = rollout[k]
-            if t.is_cuda or not t.is_contiguous() or t.dtype != self.spec[k][1] or t.numel() * t.element_size() != self._offs[k][1] // B:
-                raise _lib.TorchBeastB200Error("write_column: leaf %r must be a contiguous CPU [T+1, ...] tensor of the slot's dtype" % k)
-        _lib.check(_lib.lib().tb_host_write_rollout_column(
-            ctypes.c_void_p(self._host_raw[i].data_ptr()), ctypes.cast(offs, ctypes.c_void_p), ctypes.cast(rows, ctypes.c_void_p), n,
-            T1, B, int(b), ctypes.cast(srcs, ctypes.c_void_p)), "tb_host_write_rollout_column")
+        """Native per-actor hand-over: copy `rollout` (dict leaf -> contiguous [T+1, ...] CPU tensor; [T+4, ...] for an
+        unstacked frame leaf) into column b of pinned slot i with native calls (tb_host_write_rollout_column) that run
+        without the GIL - N actor threads then copy in parallel instead of serialising on the interpreter."""
+        self.write_prepared(i, b, self.prepare_rollout(rollout, "write_column"))
 
     def submit(self, i):
         """Slot i is complete: one async H2D copy of the whole slot on the copy stream."""
