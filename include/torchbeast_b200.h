@@ -288,6 +288,23 @@ int tb_grad_sumsq_f32(const float* grads, int64_t n, float* out_sumsq, void* wor
 int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
                              const float* sumsq, float max_norm, const float* lr_device, float lr, float alpha,
                              float eps, float momentum, float* grad_norm_out, void* stream);
+/* The same clip fused with one torch.optim.Adam (decoupled = 0, L2 weight decay) or AdamW (decoupled = 1) step,
+ * non-amsgrad, in torch's op order:  g *= coef (written back);  Adam: g' = g + wd*p,  AdamW: p *= 1 - lr*wd;
+ *   exp_avg = beta1*exp_avg + (1-beta1)*g';  exp_avg_sq = beta2*exp_avg_sq + (1-beta2)*g'^2;
+ *   p -= lr/(1-beta1^t) * exp_avg / (sqrt(exp_avg_sq)/sqrt(1-beta2^t) + eps).
+ * step_device is a device int64 holding the number of completed steps: t = step_device[0] + 1, and the call
+ * increments it on the stream after the update (a second, one-thread launch).  No host read, so the call can be
+ * captured into a CUDA graph and every replay takes the next t.  Bias corrections are computed in double.    */
+int tb_clip_adam_step_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, const float* sumsq,
+                          float max_norm, const float* lr_device, float lr, double beta1, double beta2, float eps,
+                          float weight_decay, int decoupled, int64_t* step_device, float* grad_norm_out, void* stream);
+/* The same clip fused with torch.optim.RMSprop's remaining options: weight_decay (g' = g + wd*p after the clip) and
+ * centered (grad_avg != NULL: grad_avg = alpha*grad_avg + (1-alpha)*g', avg = sqrt(square_avg - grad_avg^2) + eps),
+ * combined with momentum as in tb_clip_rmsprop_step_f32.                                                         */
+int tb_clip_rmsprop_ex_step_f32(float* params, float* grads, float* square_avg, float* grad_avg, float* momentum_buf,
+                                int64_t n, const float* sumsq, float max_norm, const float* lr_device, float lr,
+                                float alpha, float eps, float weight_decay, float momentum, float* grad_norm_out,
+                                void* stream);
 
 /* ---- bf16 tensor-core GEMM (wgmma + TMA), the throughput backend of the network -------- */
 

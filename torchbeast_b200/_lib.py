@@ -54,6 +54,9 @@ _SIGNATURES = {
     "tb_resnet_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_grad_sumsq_f32": ([_vp, _i64, _vp, _vp, _vp], _int),
     "tb_clip_rmsprop_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _vp, _vp], _int),
+    "tb_clip_adam_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f64, _f64, _f32, _f32, _int, _vp, _vp, _vp],
+                              _int),
+    "tb_clip_rmsprop_ex_step_f32": ([_vp] * 5 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _f32, _vp, _vp], _int),
     "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),

@@ -144,8 +144,8 @@ def _backward_with_overlapped_all_reduce(model, grad_logits, grad_values):
 def optimizer_step(model, optimizer, max_grad_norm):
     from torchbeast_b200 import optim as _optim
 
-    if isinstance(optimizer, _optim.RMSprop):
-        optimizer.step(max_grad_norm=max_grad_norm)  # fused clip + RMSprop, 2 launches
+    if isinstance(optimizer, _optim.FusedOptimizer):
+        optimizer.step(max_grad_norm=max_grad_norm)  # fused clip + update on the flat buffers, 2-3 launches
     else:
         # foreign optimizer object: gradients are already in .grad (views of the flat buffer)
         torch.nn.utils.clip_grad_norm_(model.parameters(), max_grad_norm)
@@ -158,7 +158,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
       network forward -> fused V-trace + 3 losses + their gradients (1 launch) -> network
-      backward into the flat gradient -> [NCCL all-reduce] -> fused clip + RMSprop -> actor copy.
+      backward into the flat gradient -> [NCCL all-reduce] -> fused clip + optimizer step -> actor copy.
     """
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
@@ -293,8 +293,8 @@ class GraphedLearner:
     """The whole device side of learn() captured ONCE into a CUDA graph and replayed per step.
 
     One replay = network forward, fused V-trace/loss/grad kernel, network backward, [NCCL all-reduce],
-    fused clip + RMSprop, actor-weight publication: ~150 kernel launches become one cudaGraphLaunch, so
-    a learner that reads its stats back every step (like the reference, monobeast.py:279-287) is no longer
+    fused clip + optimizer update (any optim.FusedOptimizer), actor-weight publication: ~150 kernel launches
+    become one cudaGraphLaunch, so a learner that reads its stats back every step (like the reference, monobeast.py:279-287) is no longer
     exposed to per-launch CPU latency.  Inputs are copied into static device buffers before each replay;
     the learning rate is read from a device scalar so LambdaLR keeps working; stats are computed from the
     graph's static outputs after the replay."""
@@ -303,8 +303,9 @@ class GraphedLearner:
 
     def __init__(self, flags, model, actor_model, optimizer, example_batch, initial_agent_state=()):
         from torchbeast_b200 import optim as _optim
-        if not isinstance(optimizer, _optim.RMSprop):
-            raise _lib.TorchBeastB200Error("GraphedLearner needs torchbeast_b200.optim.RMSprop")
+        if not isinstance(optimizer, _optim.FusedOptimizer):
+            raise _lib.TorchBeastB200Error(
+                "GraphedLearner needs a fused optimizer from torchbeast_b200.optim (RMSprop, Adam or AdamW)")
         self.flags, self.model, self.actor, self.opt = flags, model, actor_model, optimizer
         self.static = {k: torch.empty_like(v) for k, v in example_batch.items() if k in self.KEYS}
         self.static_state = tuple(torch.empty_like(s) for s in initial_agent_state)
@@ -315,8 +316,7 @@ class GraphedLearner:
         optimizer.lr_from_device = True
         optimizer.sync_lr_to_device()
         # warm up on a side stream (allocations, one-time attribute calls), then capture
-        snapshot = (model.flat_params.clone(), optimizer.square_avg.clone(),
-                    None if optimizer.momentum_buffer is None else optimizer.momentum_buffer.clone(), optimizer._steps)
+        snapshot = (model.flat_params.clone(), optimizer.snapshot())
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -338,10 +338,7 @@ class GraphedLearner:
         torch.cuda.synchronize()
         # undo the warm-up / capture-time updates so training starts from the caller's weights
         model.flat_params.copy_(snapshot[0])
-        optimizer.square_avg.copy_(snapshot[1])
-        if snapshot[2] is not None:
-            optimizer.momentum_buffer.copy_(snapshot[2])
-        optimizer._steps = snapshot[3]
+        optimizer.restore(snapshot[1])  # state buffers and step count, the device step of Adam included
         if actor_model is not None and hasattr(actor_model, "copy_params_from"):
             actor_model.copy_params_from(model)
 
