@@ -189,9 +189,19 @@ int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_basel
  * bias_hh_l [4H] (gate order i, f, g, o); 1 or 2 layers; hidden size, input size, batch and unroll are free
  * (BASELINE configs[4]: T = 600, B = 128, H = 512).  x [T1*B, In], notdone [T1*B] (float 0/1), h0/c0/hN/cN [layers, B, H],
  * y [T1*B, H].  precision 0 = fp32 everywhere (any shape); 1 / 2 = bf16 / split-bf16 tensor-core products for the hoisted
- * projections.  tb_lstm_backward must follow tb_lstm_forward on the same workspace; grads[] mirrors params[] and is
- * overwritten; dx [T1*B, In].                                                                                        */
+ * projections, and in the recurrence where a tensor-core recurrence fits the shape (tb_lstm_plan).  tb_lstm_backward must
+ * follow tb_lstm_forward on the same workspace; grads[] mirrors params[] and is overwritten; dx [T1*B, In].             */
 size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision);
+/* The recurrence kinds tb_lstm_forward (*fwd_kind_host) and tb_lstm_backward (*bwd_kind_host) run for this shape on the
+ * current device; host query, runs no kernel.  The choice does not depend on the unroll length.                       */
+#define TB_LSTM_STEP 0            /* one step kernel per time step (any shape) */
+#define TB_LSTM_PERSISTENT 1      /* one cooperative fp32 kernel per layer */
+#define TB_LSTM_PERSISTENT_MMA 2  /* one cooperative kernel per layer, bf16 tensor-core products (precision 1) */
+#define TB_LSTM_CLUSTER 3         /* one 16-CTA thread-block cluster per layer, split-bf16 products (precision 2, H = 256) */
+#define TB_LSTM_WAVE_BF16 4       /* both layers in one wavefront kernel, bf16 products (precision 1) */
+#define TB_LSTM_WAVE_SPLIT 5      /* both layers in one wavefront kernel, split-bf16 products (precision 2) */
+int tb_lstm_plan(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kind_host,
+                 int* bwd_kind_host);
 int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const float* c0, const float* const* params,
                     int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision, void* workspace,
                     float* y, float* hN, float* cN, void* stream);

@@ -79,8 +79,6 @@ static AtariParams atari_params(int A, int use_lstm) {
   return p;
 }
 
-constexpr int64_t kSplitKScratchFloats = int64_t(8) << 20;  // 32 MB
-
 // bf16 operand buffer of the tensor-core backends; lo != 0 (precision 2, split-bf16): element offset of the lo plane
 struct HB {
   void* p = nullptr; int64_t lo = 0;
@@ -156,25 +154,6 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
   w.bytes = off;
   return w;
 }
-
-// choose split-K so the grid is ~2 waves and the scratch fits
-static int pick_splits(int64_t M, int64_t N, int64_t K) {
-  const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
-  const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
-  const int64_t ktiles = (K + kGemmBK - 1) / kGemmBK;
-  if (s > ktiles / 4) s = ktiles / 4;
-  if (s * M * N > kSplitKScratchFloats) s = kSplitKScratchFloats / (M * N);
-  if (s > 128) s = 128;
-  if (s < 1) s = 1;
-  return int(s);
-}
-
-#define TB_TRY(expr)        \
-  do {                      \
-    int _rc = (expr);       \
-    if (_rc) return _rc;    \
-  } while (0)
 
 // ---------------------------------------------------------------------------------------
 // forward
@@ -252,8 +231,8 @@ static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const flo
       lp.w_ih[l] = P + pp.lstm[l][0]; lp.w_hh[l] = P + pp.lstm[l][1];
       lp.b_ih[l] = P + pp.lstm[l][2]; lp.b_hh[l] = P + pp.lstm[l][3];
     }
-    TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core, pp.core, 2, w.lstm, w.core_out, hN, cN,
-                        w.splitk, precision, st));
+    TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core, pp.core, 2, w.lstm, w.core_out, hN, cN, precision,
+                        st));
   }
   // heads (fused skinny kernel: one pass over core_out for all A+1 outputs)
   TB_TRY(heads_forward(w.core_out, pp.core, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N, pp.core,
@@ -269,7 +248,7 @@ static int wgrad(const float* dY, int64_t ldy, const void* X, bool x_is_u8, int6
   // dW[nout, kin] = dY[rows, nout]^T . X[rows, kin]
   GemmEpilogue ep;
   ep.permP = permP; ep.permQ = permQ; ep.tag = tag;
-  const int splits = pick_splits(nout, kin, rows);
+  const int splits = simt_splits(nout, kin, rows, kSplitKScratchFloats, 128);
   if (x_is_u8)
     return gemm_simt<float, uint8_t, true, false>(dY, static_cast<const uint8_t*>(X), dW, nout, kin, rows, ldy, ldx,
                                                    kin, ep, splits, w.splitk, st);

@@ -29,6 +29,13 @@ struct ProfScope {
     }                              \
   } while (0)
 
+// forwards a non-zero status (the callee has already set the error message)
+#define TB_TRY(expr)     \
+  do {                   \
+    int _rc = (expr);    \
+    if (_rc) return _rc; \
+  } while (0)
+
 constexpr int kWarp = 32;
 constexpr int kNumSMs = 132;  // H100 SXM
 // workspace layout: [0] uint32 ticket counter (self-resetting), then kMaxPartialCtas x 4 doubles

@@ -187,6 +187,20 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ partial, float* _
 int launch_splitk_reduce(const float* partial, float* C, int64_t M, int64_t N, int64_t ldc, int splits, const GemmEpilogue& ep,
                          int64_t ldp, cudaStream_t stream);
 
+// Split-K count for C[M,N] over K: about two waves of CTA tiles, at least four K tiles per split, the partials within
+// `scratch_floats`, at most `cap` splits.
+inline int simt_splits(int64_t M, int64_t N, int64_t K, int64_t scratch_floats, int64_t cap) {
+  const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
+  const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
+  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
+  const int64_t ktiles = (K + kGemmBK - 1) / kGemmBK;
+  if (s > ktiles / 4) s = ktiles / 4;
+  if (s * M * N > scratch_floats) s = scratch_floats / (M * N);
+  if (s > cap) s = cap;
+  if (s < 1) s = 1;
+  return int(s);
+}
+
 // Host launcher.  `splitk_scratch` must hold splits*M*N floats when splits > 1.
 template <typename AT, typename BT, bool TA, bool TB>
 int gemm_simt(const AT* A, const BT* B, float* C, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,

@@ -4,10 +4,13 @@
 // (/root/reference/torchbeast/monobeast.py:603-611, polybeast_learner.py:241-249):
 //     for t: state *= notdone_t;  out_t, state = LSTM(x_t, state)         (all layers per t)
 // Re-ordered layer-major: layer l only depends on layer l-1's outputs, so for each layer the
-// input projection of ALL T+1 steps is hoisted into one [N,In]x[In,4H] GEMM, the recurrence runs
-// as T+1 fused step kernels (recurrent product + gate non-linearities + state update + next
-// step's masked state, W_hh slice and h tile staged in shared memory), and BPTT accumulates
-// the weight gradients with two [4H,N]x[N,*] GEMMs after the time loop instead of per step.
+// input projection of ALL T+1 steps is hoisted into one [N,In]x[In,4H] GEMM, only the recurrence
+// itself runs step by step, and BPTT accumulates the weight gradients with two [4H,N]x[N,*] GEMMs
+// after the time loop instead of per step.
+// The recurrence has six implementations, and lstm_plan (near the end of this file) picks one per
+// shape and direction: T+1 fused step kernels (any shape), one persistent cooperative kernel per
+// layer in fp32 or with bf16 tensor-core products, one 16-CTA cluster per layer (H = 256), and
+// two-layer wavefront kernels (bf16 or split-bf16) that run both layers in one launch.
 // torch.nn.LSTM conventions: gate order i,f,g,o; weight_ih [4H,In], weight_hh [4H,H]; two biases.
 #include "lstm.cuh"
 
@@ -703,81 +706,149 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_kernel(Persi
   }
 }
 
-// 1 if the whole grid of `kernel` (blocks of `threads`, `smem` bytes of dynamic shared memory) is co-resident on the
-// current device, as a cooperative launch needs; 0 otherwise
-static int persistent_ok(const void* kernel, dim3 grid, int threads, size_t smem) {
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  if (!coop) return 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  return int64_t(per_sm) * sms >= int64_t(grid.x) * grid.y;
-}
-
-// cudaFuncSetAttribute is per device: the attribute caches are indexed by the current device
-static inline size_t* per_device(size_t (&cache)[64]) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return &cache[dev & 63];
-}
-
-// raises the kernel's dynamic shared-memory limit to `smem` (once per device; *attr_smem caches the limit already set),
-// then checks co-residency.  0: the kernel cannot run as one cooperative grid here
-template <typename Kernel>
-static int coop_fit(Kernel kernel, dim3 grid, size_t smem, int threads, size_t* attr_smem) {
-  if (*attr_smem < smem) {
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();
-      return 0;
+// Launch configuration of the recurrence kernels: `cluster` > 1 groups the CTAs into thread-block clusters of that size;
+// `coop` makes the grid cooperative (every CTA co-resident: the kernels wait on barriers and flags other CTAs release).
+// Not copyable: cfg points at attr.
+struct Launch {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[2];
+  unsigned cluster;
+  Launch(dim3 grid, int threads, size_t smem, cudaStream_t st, unsigned cluster_size, bool coop) : cluster(cluster_size) {
+    cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st; cfg.attrs = attr;
+    if (cluster > 1) {
+      cudaLaunchAttribute& a = attr[cfg.numAttrs++];
+      a.id = cudaLaunchAttributeClusterDimension;
+      a.val.clusterDim.x = cluster; a.val.clusterDim.y = 1; a.val.clusterDim.z = 1;
     }
-    *attr_smem = smem;
+    if (coop) {
+      cudaLaunchAttribute& a = attr[cfg.numAttrs++];
+      a.id = cudaLaunchAttributeCooperative; a.val.cooperative = 1;
+    }
   }
-  return persistent_ok((const void*)kernel, grid, threads, smem);
+  Launch(const Launch&) = delete;
+};
+
+// Whether `Kernel` can run as configured by `l` on the current device.  Raises the kernel's dynamic shared-memory limit
+// to what `l` asks for (and allows a non-portable cluster size above 8) once per device, then checks that the whole grid
+// - every cluster of it - is co-resident.
+template <auto Kernel>
+static bool fits(const Launch& l) {
+  static size_t attr_smem[64] = {0};  // per device: the shared-memory limit already set
+  const void* k = (const void*)Kernel;
+  int dev = 0, coop = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return false;
+  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (!coop) return false;
+  const size_t smem = l.cfg.dynamicSmemBytes;
+  if (attr_smem[dev & 63] < smem) {
+    if ((l.cluster > 8 && cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) ||
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
+      cudaGetLastError();
+      return false;
+    }
+    attr_smem[dev & 63] = smem;
+  }
+  int n = 0;
+  const cudaError_t e = l.cluster > 1 ? cudaOccupancyMaxActiveClusters(&n, k, &l.cfg)
+                                      : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, int(l.cfg.blockDim.x), smem);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return int64_t(n) * (l.cluster > 1 ? l.cluster : sms) >= int64_t(l.cfg.gridDim.x) * l.cfg.gridDim.y;
 }
 
-static size_t g_fwd_persist_attr_dev[64] = {0}, g_bwd_persist_attr_dev[64] = {0};
+template <typename Kernel, typename... Args>
+static int launch(const Launch& l, const char* what, Kernel kernel, const Args&... args) {
+  const cudaError_t e = cudaLaunchKernelEx(&l.cfg, kernel, args...);
+  TB_REQUIRE(e == cudaSuccess, "%s: %s", what, cudaGetErrorString(e));
+  return check_launch(what);
+}
+
+static Launch persistent_fwd_launch(int64_t B, int H, cudaStream_t st) {
+  return Launch(dim3((H + kStepUnits - 1) / kStepUnits, unsigned((B + 31) / 32)), kStepThreads,
+                size_t(48) * padded_h(H) * sizeof(float) + 16, st, 1, true);
+}
+static Launch persistent_bwd_launch(int H, cudaStream_t st) {
+  return Launch(dim3((H + 3) / 4), kStepThreads, size_t(80) * padded_h(H) * sizeof(float) + 32, st, 1, true);
+}
+static bool persistent_fwd_fits(int64_t B, int H) {
+  const Launch l = persistent_fwd_launch(B, H, nullptr);
+  return B <= 64 && l.cfg.dynamicSmemBytes <= 200 * 1024 && fits<lstm_fwd_persistent_kernel>(l);
+}
+static bool persistent_bwd_fits(int64_t B, int H) {
+  const Launch l = persistent_bwd_launch(H, nullptr);
+  return B <= 32 && l.cfg.dynamicSmemBytes <= 220 * 1024 && fits<lstm_bwd_persistent_kernel>(l);
+}
 
 static int lstm_fwd_persistent(const LstmLayerWs& L, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
                                unsigned* counter, cudaStream_t st) {
-  if (B > 64) return -1;
-  const int Hp = padded_h(H);
-  const size_t smem = size_t(48) * Hp * sizeof(float) + 16;
-  if (smem > 200 * 1024) return -1;
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, (unsigned)((B + 31) / 32));
-  if (!coop_fit(lstm_fwd_persistent_kernel, grid, smem, kStepThreads, per_device(g_fwd_persist_attr_dev))) return -1;
+  const Launch l = persistent_fwd_launch(B, H, st);
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   PersistFwdArgs a;
   a.wp = L.wp; a.gates = L.gates; a.hs = hs; a.cs = L.cs; a.hm = L.hm; a.cm = L.cm; a.nd = notdone; a.counter = counter;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hp = Hp; a.nctas = grid.x * grid.y;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm_fwd_persistent_kernel, grid, dim3(kStepThreads), args, smem, st);
-  TB_REQUIRE(e == cudaSuccess, "lstm_fwd_persistent_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm_fwd_persistent_kernel");
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hp = padded_h(H); a.nctas = l.cfg.gridDim.x * l.cfg.gridDim.y;
+  return launch(l, "lstm_fwd_persistent_kernel", lstm_fwd_persistent_kernel, a);
 }
 
 static int lstm_bwd_persistent(const LstmLayerWs& L, const LstmWs& ws, const float* dy, const float* notdone, int64_t T1,
                                int64_t B, int H, unsigned* counter, cudaStream_t st) {
-  if (B > 32) return -1;
+  const Launch l = persistent_bwd_launch(H, st);
   const int Hp = padded_h(H);
-  const size_t smem = size_t(80) * Hp * sizeof(float) + 32;
-  if (smem > 220 * 1024) return -1;
-  dim3 grid((H + 3) / 4, 1);
-  if (!coop_fit(lstm_bwd_persistent_kernel, grid, smem, kStepThreads, per_device(g_bwd_persist_attr_dev))) return -1;
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(ws.dgp, 0, sizeof(float) * 2 * 4 * B * Hp, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   PersistBwdArgs a;
   a.wtp = L.w_hh_t; a.dy = dy; a.nd = notdone; a.gates = L.gates; a.cs = L.cs; a.cm = L.cm; a.dgates = L.dgates;
-  a.dgp = ws.dgp; a.counter = counter; a.T1 = int(T1); a.B = int(B); a.H = H; a.Hp = Hp; a.nctas = grid.x;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm_bwd_persistent_kernel, grid, dim3(kStepThreads), args, smem, st);
-  TB_REQUIRE(e == cudaSuccess, "lstm_bwd_persistent_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm_bwd_persistent_kernel");
+  a.dgp = ws.dgp; a.counter = counter; a.T1 = int(T1); a.B = int(B); a.H = H; a.Hp = Hp; a.nctas = l.cfg.gridDim.x;
+  return launch(l, "lstm_bwd_persistent_kernel", lstm_bwd_persistent_kernel, a);
+}
+
+// the step kernels: one launch per time step (any shape)
+static int lstm_fwd_steps(const LstmLayerWs& L, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
+                          cudaStream_t st) {
+  const int Hp = padded_h(H);
+  for (int64_t t = 0; t < T1; ++t) {
+    StepArgs a;
+    a.hm = L.hm + t * B * Hp;
+    a.cm = L.cm + t * B * H;
+    const bool last = (t == T1 - 1);
+    a.nd_next = last ? nullptr : notdone + (t + 1) * B;
+    a.wp = L.wp;
+    a.gates = L.gates + t * B * 4 * H;
+    a.hs = hs + t * B * H; a.cs = L.cs + t * B * H;
+    a.hm_next = last ? nullptr : L.hm + (t + 1) * B * Hp;
+    a.cm_next = last ? nullptr : L.cm + (t + 1) * B * H;
+    a.B = int(B); a.H = H; a.Hp = Hp;
+    TB_TRY(launch_step_fwd(a, st));
+  }
+  return 0;
+}
+
+static int lstm_bwd_steps(const LstmLayerWs& L, const LstmWs& ws, const float* dy, const float* notdone, int64_t T1,
+                          int64_t B, int H, cudaStream_t st) {
+  const int Hp = padded_h(H);
+  for (int64_t t = T1 - 1; t >= 0; --t) {
+    BwdPointArgs a;
+    a.dy = dy + t * B * H;
+    a.first = (t == T1 - 1);
+    a.dh_raw = ws.dh; a.nd_next = a.first ? nullptr : notdone + (t + 1) * B;
+    a.nd = notdone + t * B;
+    a.gates = L.gates + t * B * 4 * H; a.cs = L.cs + t * B * H; a.cm = L.cm + t * B * H;
+    a.dc = ws.dc; a.dgates = L.dgates + t * B * 4 * H; a.B = int(B); a.H = H; a.dgp = ws.dgp; a.Hp = Hp;
+    const int64_t total = B * H;
+    lstm_step_bwd_point_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
+    TB_TRY(check_launch("lstm_step_bwd_point_kernel"));
+    if (t > 0) {
+      // dh_raw[B,H] = dgates_t[B,4H] . W_hh[4H,H]   (masked by notdone_t when consumed at t-1)
+      DhArgs d;
+      d.dgp = ws.dgp; d.wtp = L.w_hh_t; d.dh_raw = ws.dh; d.B = int(B); d.H = H; d.Hp = Hp;
+      TB_TRY(launch_step_bwd_dh(d, st));
+    }
+  }
+  return 0;
 }
 
 
@@ -2278,50 +2349,42 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   cluster_sync_all();   // no CTA exits with multicast writes or remote arrives into it still in flight
 }
 
-static size_t g_fwd_mma_attr_dev[64] = {0}, g_bwd_mma_attr_dev[64] = {0};
-
-// one decision for a (B, H) pair, used identically by forward and backward (the backward consumes the bf16
-// masked-h buffer only the tensor-core forward writes)
-static bool mma_recurrence_applicable(int64_t B, int H) {
+static Launch mma_fwd_launch(int H, cudaStream_t st) {
+  return Launch(dim3((H + kStepUnits - 1) / kStepUnits), kStepThreads, size_t(32) * mma_hq(H) * 2, st, 1, true);
+}
+static Launch mma_bwd_launch(int H, cudaStream_t st) {
+  return Launch(dim3((H + kBwdCols - 1) / kBwdCols), kStepThreads, size_t(4) * 32 * mma_hq(H) * 2, st, 1, true);
+}
+// both tensor-core kernels: the precision 1 layers run both of them or neither
+static bool mma_fits(int64_t B, int H) {
   if (B > 32 || H > 624) return false;  // tile copy: <= 5 x 16 B chunks per thread
-  const int Hq = mma_hq(H);
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1), gridb((H + kBwdCols - 1) / kBwdCols, 1);
-  return coop_fit(lstm_fwd_persistent_mma_kernel, grid, size_t(32) * Hq * 2, kStepThreads, per_device(g_fwd_mma_attr_dev)) &&
-         coop_fit(lstm_bwd_persistent_mma_kernel, gridb, size_t(4) * 32 * Hq * 2, kStepThreads, per_device(g_bwd_mma_attr_dev));
+  return fits<lstm_fwd_persistent_mma_kernel>(mma_fwd_launch(H, nullptr)) &&
+         fits<lstm_bwd_persistent_mma_kernel>(mma_bwd_launch(H, nullptr));
 }
 
 static int lstm_fwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, float* hs, const float* notdone, int64_t T1,
                                    int64_t B, int H, unsigned* counter, cudaStream_t st) {
-  const int Hq = mma_hq(H);
-  const size_t smem = size_t(32) * Hq * 2;
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
-  if (!coop_fit(lstm_fwd_persistent_mma_kernel, grid, smem, kStepThreads, per_device(g_fwd_mma_attr_dev))) return -1;
+  const Launch l = mma_fwd_launch(H, st);
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   PersistFwdMmaArgs a;
   a.w_hh = w_hh; a.gates = L.gates; a.hs = hs; a.cs = L.cs; a.cm = L.cm; a.nd = notdone;
   a.hmq = static_cast<__nv_bfloat16*>(L.hmq); a.counter = counter;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = grid.x;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm_fwd_persistent_mma_kernel, grid, dim3(kStepThreads), args, smem, st);
-  TB_REQUIRE(e == cudaSuccess, "lstm_fwd_persistent_mma_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm_fwd_persistent_mma_kernel");
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = mma_hq(H); a.nctas = l.cfg.gridDim.x;
+  return launch(l, "lstm_fwd_persistent_mma_kernel", lstm_fwd_persistent_mma_kernel, a);
 }
 
-static size_t g_fwd_wave_attr_dev[64] = {0};
-static size_t wave_fwd_smem(int Hq) { return size_t(2) * 32 * Hq * 2 + sizeof(float) * 16 * 2 * 16 * 33; }
-static bool wave_fwd_applicable(int64_t B, int H) {
-  if (!mma_recurrence_applicable(B, H)) return false;
-  if (((H + 15) / 16 + 15) / 16 > kWaveK) return false;
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
-  return coop_fit(lstm2_fwd_wave_mma_kernel, grid, wave_fwd_smem(mma_hq(H)), kStepThreads, per_device(g_fwd_wave_attr_dev));
+static Launch wave_fwd_launch(int H, cudaStream_t st) {
+  return Launch(dim3((H + kStepUnits - 1) / kStepUnits), kStepThreads,
+                size_t(2) * 32 * mma_hq(H) * 2 + sizeof(float) * 16 * 2 * 16 * 33, st, 1, true);
+}
+static bool wave_fwd_fits(int64_t B, int H) {
+  return mma_fits(B, H) && ((H + 15) / 16 + 15) / 16 <= kWaveK && fits<lstm2_fwd_wave_mma_kernel>(wave_fwd_launch(H, nullptr));
 }
 
 static int lstm2_fwd_wave(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, int64_t T1, int64_t B, int H,
                           cudaStream_t st) {
-  const int Hq = mma_hq(H);
-  const size_t smem = wave_fwd_smem(Hq);
-  dim3 grid((H + kStepUnits - 1) / kStepUnits, 1);
+  const Launch l = wave_fwd_launch(H, st);
   cudaError_t e = cudaMemsetAsync(ws.sync, 0, sizeof(unsigned), st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   WaveFwdArgs a;
@@ -2332,11 +2395,8 @@ static int lstm2_fwd_wave(LstmWs& ws, const LstmParams& p, float* y, const float
     a.hq[l] = static_cast<__nv_bfloat16*>(L.hq); a.hmq[l] = static_cast<__nv_bfloat16*>(L.hmq);
   }
   a.nd = notdone; a.counter = ws.sync;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = grid.x;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm2_fwd_wave_mma_kernel, grid, dim3(kStepThreads), args, smem, st);
-  TB_REQUIRE(e == cudaSuccess, "lstm2_fwd_wave_mma_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm2_fwd_wave_mma_kernel");
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = mma_hq(H); a.nctas = l.cfg.gridDim.x;
+  return launch(l, "lstm2_fwd_wave_mma_kernel", lstm2_fwd_wave_mma_kernel, a);
 }
 
 // slot 0 of the split recurrence's planes: hq = split(h0) (raw), hmq = split(h0 * nd_0); row padding zero
@@ -2354,60 +2414,31 @@ __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const
   hmq[i] = m; hmq[hmq_lo + i] = __float2bfloat16_rn(hm - __bfloat162float(m));
 }
 
-// The split kernels run as one cooperative grid of 2-CTA clusters: launch configuration with both attributes
-struct ClusterCoopLaunch {
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
-  ClusterCoopLaunch(dim3 grid, size_t smem, cudaStream_t st) {
-    cfg.gridDim = grid; cfg.blockDim = dim3(kSplitThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeCooperative; attr[1].val.cooperative = 1;
-    cfg.attrs = attr; cfg.numAttrs = 2;
-  }
-};
-// coop_fit for a grid of 2-CTA clusters: every cluster of the grid must be co-resident (the kernels spin on flags
-// written by other CTAs)
-template <typename Kernel>
-static int cluster_coop_fit(Kernel kernel, dim3 grid, size_t smem, size_t* attr_smem) {
-  int dev = 0, coop = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
-  cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-  if (!coop) return 0;
-  if (*attr_smem < smem) {
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) {
-      cudaGetLastError();
-      return 0;
-    }
-    *attr_smem = smem;
-  }
-  ClusterCoopLaunch l(grid, smem, nullptr);
-  int clusters = 0;
-  if (cudaOccupancyMaxActiveClusters(&clusters, kernel, &l.cfg) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  return int64_t(clusters) * 2 >= int64_t(grid.x);
+// The split kernels run as one cooperative grid of 2-CTA clusters.  Forward CTAs: kStepUnits units each, padded to whole
+// clusters; shared memory: tiles + partial sums + alignment slack
+static Launch wave_fwd_split_launch(int H, cudaStream_t st) {
+  return Launch(dim3(((H + kStepUnits - 1) / kStepUnits + 1) & ~1), kSplitThreads,
+                size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128, st, 2, true);
 }
-
-static size_t g_fwd_split_attr_dev[64] = {0};
-static size_t wave_fwd_split_smem() {   // tiles + partial sums + alignment slack
-  return size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128;
+// backward: kBwdCols columns per CTA and role, padded to whole clusters (a cluster never straddles the two roles); tile
+// rings + partial sums + prefetched pointwise operands + alignment slack
+static unsigned wave_bwd_split_role_ctas(int H) { return unsigned(((H + kBwdCols - 1) / kBwdCols + 1) & ~1); }
+static Launch wave_bwd_split_launch(int H, cudaStream_t st) {
+  return Launch(dim3(2 * wave_bwd_split_role_ctas(H)), kSplitThreads,
+                size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33 + sizeof(float) * 9 * 256 + 128,
+                st, 2, true);
 }
-// forward CTAs: kStepUnits units each, padded to whole clusters
-static dim3 wave_fwd_split_grid(int H) { return dim3(((H + kStepUnits - 1) / kStepUnits + 1) & ~1, 1); }
-// precision 2, two layers: the split-bf16 wavefront kernel (other shapes run the exact-fp32 recurrence kernels)
-static bool wave_fwd_split_applicable(int64_t B, int In, int H) {
+// both split kernels: the backward consumes the blocked saves only the split forward writes
+static bool wave_split_fits(int64_t B, int In, int H) {
   if (B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
-  const dim3 grid = wave_fwd_split_grid(H);
-  if (int(grid.x) > kSplitThreads || grid.x > 512) return false;
-  return cluster_coop_fit(lstm2_fwd_wave_split_kernel, grid, wave_fwd_split_smem(), per_device(g_fwd_split_attr_dev));
+  const Launch f = wave_fwd_split_launch(H, nullptr), b = wave_bwd_split_launch(H, nullptr);
+  if (int(f.cfg.gridDim.x) > kSplitThreads || f.cfg.gridDim.x > 512 || !fits<lstm2_fwd_wave_split_kernel>(f)) return false;
+  return int(b.cfg.gridDim.x / 2) + 1 <= kSplitThreads && b.cfg.gridDim.x <= 512 && fits<lstm2_bwd_wave_split_kernel>(b);
 }
 
 static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, const float* c0, float* hN,
                                 float* cN, int64_t T1, int64_t B, int H, cudaStream_t st) {
   const int Hq = mma_hq(H);
-  const dim3 grid = wave_fwd_split_grid(H);
   cudaError_t e = cudaMemsetAsync(ws.flags, 0, sizeof(unsigned) * 512 * kFlagStride, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   WaveFwdSplitArgs a;
@@ -2430,10 +2461,7 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
     const uint32_t box[4] = {kTileRowE, 16, 1, 2};
     tcd::make_map_nd(&maps[l], a.hq[l], 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
   }
-  ClusterCoopLaunch l(grid, wave_fwd_split_smem(), st);
-  e = cudaLaunchKernelEx(&l.cfg, lstm2_fwd_wave_split_kernel, maps[0], maps[1], a);
-  TB_REQUIRE(e == cudaSuccess, "lstm2_fwd_wave_split_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm2_fwd_wave_split_kernel");
+  return launch(wave_fwd_split_launch(H, st), "lstm2_fwd_wave_split_kernel", lstm2_fwd_wave_split_kernel, maps[0], maps[1], a);
 }
 
 // =========================================================================================
@@ -2598,40 +2626,17 @@ static size_t cluster_fwd_smem(int MT) {
   return 2 * (2 * R * kClHq * 2) + 8 * (R * 65 * 4) + 2 * R * kClU * 2;
 }
 
+// one 16-CTA cluster (non-portable size), no cooperative grid: the hardware places a cluster's CTAs together
+static Launch cluster_launch(size_t smem, cudaStream_t st) { return Launch(dim3(kClN), kClThreads, smem, st, kClN, false); }
+
 static int lstm_fwd_cluster(const LstmLayerWs& L, const float* w_hh, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
                             cudaStream_t st) {
-  if (H != kClH || B > 32 || B < 1) return -1;
-  static int attr_ok[64] = {0};   // per device: 0 unknown, 1 ok, -1 unavailable
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (attr_ok[dev & 63] == 0) {
-    cudaError_t e1 = cudaFuncSetAttribute(lstm_fwd_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    cudaError_t e2 = cudaFuncSetAttribute(lstm_fwd_cluster_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(lstm_fwd_cluster_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cluster_fwd_smem(1)));
-    if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(lstm_fwd_cluster_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cluster_fwd_smem(2)));
-    attr_ok[dev & 63] = (e1 == cudaSuccess && e2 == cudaSuccess) ? 1 : -1;
-    if (attr_ok[dev & 63] < 0) cudaGetLastError();
-  }
-  if (attr_ok[dev & 63] < 0) return -1;
   ClusterFwdArgs a;
   a.w_hh = w_hh; a.gates = L.gates; a.hs = hs; a.cs = L.cs; a.hm = L.hm; a.cm = L.cm; a.nd = notdone;
   a.T1 = int(T1); a.B = int(B); a.Hp = padded_h(H);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(kClN);
-  cfg.blockDim = dim3(kClThreads);
-  cfg.dynamicSmemBytes = cluster_fwd_smem(B <= 16 ? 1 : 2);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kClN; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = (B <= 16) ? cudaLaunchKernelEx(&cfg, lstm_fwd_cluster_kernel<1>, a) : cudaLaunchKernelEx(&cfg, lstm_fwd_cluster_kernel<2>, a);
-  if (e != cudaSuccess) {   // a 16-CTA cluster cannot be placed here: the cooperative kernel takes over
-    cudaGetLastError();
-    return -1;
-  }
-  return check_launch("lstm_fwd_cluster_kernel");
+  const Launch l = cluster_launch(cluster_fwd_smem(B <= 16 ? 1 : 2), st);
+  return B <= 16 ? launch(l, "lstm_fwd_cluster_kernel", lstm_fwd_cluster_kernel<1>, a)
+                 : launch(l, "lstm_fwd_cluster_kernel", lstm_fwd_cluster_kernel<2>, a);
 }
 
 // ---- backward on the same cluster ---------------------------------------------------------------------------------
@@ -2770,47 +2775,31 @@ static size_t cluster_bwd_smem(int MT) {
 }
 
 static int lstm_bwd_cluster(const LstmLayerWs& L, const float* w_hh, const float* dy, const float* notdone, int64_t T1, int64_t B,
-                            int H, cudaStream_t st) {
-  if (H != kClH || B > 32 || B < 1) return -1;
-  static int attr_ok[64] = {0};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (attr_ok[dev & 63] == 0) {
-    cudaError_t e1 = cudaFuncSetAttribute(lstm_bwd_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    cudaError_t e2 = cudaFuncSetAttribute(lstm_bwd_cluster_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(lstm_bwd_cluster_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cluster_bwd_smem(1)));
-    if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(lstm_bwd_cluster_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(cluster_bwd_smem(2)));
-    attr_ok[dev & 63] = (e1 == cudaSuccess && e2 == cudaSuccess) ? 1 : -1;
-    if (attr_ok[dev & 63] < 0) cudaGetLastError();
-  }
-  if (attr_ok[dev & 63] < 0) return -1;
+                            cudaStream_t st) {
   ClusterBwdArgs a;
   a.w_hh = w_hh; a.dy = dy; a.nd = notdone; a.gates = L.gates; a.cs = L.cs; a.cm = L.cm; a.dgates = L.dgates;
   a.T1 = int(T1); a.B = int(B);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(kClN);
-  cfg.blockDim = dim3(kClThreads);
-  cfg.dynamicSmemBytes = cluster_bwd_smem(B <= 16 ? 1 : 2);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kClN; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = (B <= 16) ? cudaLaunchKernelEx(&cfg, lstm_bwd_cluster_kernel<1>, a) : cudaLaunchKernelEx(&cfg, lstm_bwd_cluster_kernel<2>, a);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return -1;
-  }
-  return check_launch("lstm_bwd_cluster_kernel");
+  const Launch l = cluster_launch(cluster_bwd_smem(B <= 16 ? 1 : 2), st);
+  return B <= 16 ? launch(l, "lstm_bwd_cluster_kernel", lstm_bwd_cluster_kernel<1>, a)
+                 : launch(l, "lstm_bwd_cluster_kernel", lstm_bwd_cluster_kernel<2>, a);
+}
+
+// H = 256, B <= 32, and the cluster can be placed on this device
+static bool cluster_fwd_fits(int64_t B, int H) {
+  if (H != kClH || B > 32) return false;
+  return B <= 16 ? fits<lstm_fwd_cluster_kernel<1>>(cluster_launch(cluster_fwd_smem(1), nullptr))
+                 : fits<lstm_fwd_cluster_kernel<2>>(cluster_launch(cluster_fwd_smem(2), nullptr));
+}
+static bool cluster_bwd_fits(int64_t B, int H) {
+  if (H != kClH || B > 32) return false;
+  return B <= 16 ? fits<lstm_bwd_cluster_kernel<1>>(cluster_launch(cluster_bwd_smem(1), nullptr))
+                 : fits<lstm_bwd_cluster_kernel<2>>(cluster_launch(cluster_bwd_smem(2), nullptr));
 }
 
 static int lstm_bwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, const float* dy, const float* notdone,
                                    int64_t T1, int64_t B, int H, float* db, unsigned* counter, cudaStream_t st) {
   const int Hq = mma_hq(H);
-  const size_t smem = size_t(4) * 32 * Hq * 2;
-  dim3 grid((H + kBwdCols - 1) / kBwdCols, 1);
-  if (!coop_fit(lstm_bwd_persistent_mma_kernel, grid, smem, kStepThreads, per_device(g_bwd_mma_attr_dev))) return -1;
+  const Launch l = mma_bwd_launch(H, st);
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(L.dgq, 0, size_t(2) * 4 * B * Hq * 2, st);  // zero the row padding
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
@@ -2818,22 +2807,17 @@ static int lstm_bwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, cons
   a.w_hh = w_hh; a.dy = dy; a.nd = notdone; a.gates = L.gates; a.cs = L.cs; a.cm = L.cm;
   a.dgb = static_cast<__nv_bfloat16*>(L.dgb); a.lg = int(ld16(4 * H)); a.db = db;
   a.dgq = static_cast<__nv_bfloat16*>(L.dgq); a.counter = counter;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = grid.x;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm_bwd_persistent_mma_kernel, grid, dim3(kStepThreads), args, smem, st);
-  TB_REQUIRE(e == cudaSuccess, "lstm_bwd_persistent_mma_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm_bwd_persistent_mma_kernel");
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = l.cfg.gridDim.x;
+  return launch(l, "lstm_bwd_persistent_mma_kernel", lstm_bwd_persistent_mma_kernel, a);
 }
 
-static size_t g_bwd_wave_attr_dev[64] = {0};
-static size_t wave_bwd_smem(int H) {
+static Launch wave_bwd_launch(int H, cudaStream_t st) {
   const int kper = (4 * ((H + 15) / 16) + 15) / 16;
-  return size_t(4) * 32 * mma_hq(H) * 2 + size_t(16) * kper * 32 * 8;
+  return Launch(dim3(2 * ((H + kBwdCols - 1) / kBwdCols)), kStepThreads,
+                size_t(4) * 32 * mma_hq(H) * 2 + size_t(16) * kper * 32 * 8, st, 1, true);
 }
-static bool wave_bwd_applicable(int64_t B, int H) {
-  if (!mma_recurrence_applicable(B, H)) return false;
-  dim3 grid(2 * ((H + kBwdCols - 1) / kBwdCols), 1);
-  return coop_fit(lstm2_bwd_wave_mma_kernel, grid, wave_bwd_smem(H), kStepThreads, per_device(g_bwd_wave_attr_dev));
+static bool wave_bwd_fits(int64_t B, int H) {
+  return mma_fits(B, H) && fits<lstm2_bwd_wave_mma_kernel>(wave_bwd_launch(H, nullptr));
 }
 
 // both layers' backward recurrences in one launch; leaves dgb / bias gradients of both layers and
@@ -2859,24 +2843,7 @@ static int lstm2_bwd_wave(LstmWs& ws, const LstmParams& p, const LstmGrads& g, c
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq);
   a.dxm = ws.dx_mid; a.counter = counter;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc;
-  void* args[] = {&a};
-  e = cudaLaunchCooperativeKernel((const void*)lstm2_bwd_wave_mma_kernel, dim3(2 * nc), dim3(kStepThreads), args,
-                                  wave_bwd_smem(H), st);
-  TB_REQUIRE(e == cudaSuccess, "lstm2_bwd_wave_mma_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm2_bwd_wave_mma_kernel");
-}
-
-static size_t g_bwd_split_attr_dev[64] = {0};
-static size_t wave_bwd_split_smem() {   // tile rings + partial sums + prefetched pointwise operands + alignment slack
-  return size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33 + sizeof(float) * 9 * 256 + 128;
-}
-// CTAs per role: kBwdCols columns each, padded to whole clusters (a cluster never straddles the two roles)
-static unsigned wave_bwd_split_role_ctas(int H) { return unsigned(((H + kBwdCols - 1) / kBwdCols + 1) & ~1); }
-static bool wave_bwd_split_applicable(int64_t B, int In, int H) {
-  if (!wave_fwd_split_applicable(B, In, H)) return false;  // consumes the planes the split forward leaves behind
-  dim3 grid(2 * wave_bwd_split_role_ctas(H), 1);
-  if (int(grid.x / 2) + 1 > kSplitThreads || grid.x > 512) return false;
-  return cluster_coop_fit(lstm2_bwd_wave_split_kernel, grid, wave_bwd_split_smem(), per_device(g_bwd_split_attr_dev));
+  return launch(wave_bwd_launch(H, st), "lstm2_bwd_wave_mma_kernel", lstm2_bwd_wave_mma_kernel, a);
 }
 
 static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone,
@@ -2909,17 +2876,32 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
     const uint32_t box[5] = {kTileRowE, 16, 1, 1, 2};
     tcd::make_map_nd(&maps[r], r == 0 ? a.dgq_up : a.dgq_lo, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
   }
-  ClusterCoopLaunch l(dim3(2 * nc), wave_bwd_split_smem(), st);
-  e = cudaLaunchKernelEx(&l.cfg, lstm2_bwd_wave_split_kernel, maps[0], maps[1], a);
-  TB_REQUIRE(e == cudaSuccess, "lstm2_bwd_wave_split_kernel: %s", cudaGetErrorString(e));
-  return check_launch("lstm2_bwd_wave_split_kernel");
+  return launch(wave_bwd_split_launch(H, st), "lstm2_bwd_wave_split_kernel", lstm2_bwd_wave_split_kernel, maps[0], maps[1], a);
 }
 
 // Side stream for work that can run beside a recurrence kernel (which occupies only H/8 = 65 of the 132 SMs):
 // forked from / joined into the caller's stream with events, so it is captured into the learner's CUDA graph.
 struct SideStream {
   cudaStream_t stream = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
+  cudaEvent_t fork_ev = nullptr, join_ev = nullptr;
+  // what is enqueued on `stream` from here on runs after what is enqueued on `st` so far
+  int fork(cudaStream_t st) {
+    cudaError_t e = cudaEventRecord(fork_ev, st);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(stream, fork_ev, 0);
+    TB_REQUIRE(e == cudaSuccess, "lstm: side stream fork: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  // marks the end of the forked work; wait(st) orders what is enqueued on `st` afterwards behind it
+  int join() {
+    const cudaError_t e = cudaEventRecord(join_ev, stream);
+    TB_REQUIRE(e == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  int wait(cudaStream_t st) {
+    const cudaError_t e = cudaStreamWaitEvent(st, join_ev, 0);
+    TB_REQUIRE(e == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(e));
+    return 0;
+  }
 };
 // A caller-owned side stream (tb_set_aux_stream): data-parallel learners pass the stream they will enqueue the all-reduce of
 // the LSTM gradient slice on, so that it is ordered behind the weight-gradient GEMMs forked onto it.
@@ -2934,8 +2916,8 @@ static SideStream* side_stream() {
     static thread_local SideStream aux[64];
     SideStream& x = aux[dev];
     x.stream = g_aux_stream;
-    if (!x.fork && (cudaEventCreateWithFlags(&x.fork, cudaEventDisableTiming) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&x.join, cudaEventDisableTiming) != cudaSuccess)) {
+    if (!x.fork_ev && (cudaEventCreateWithFlags(&x.fork_ev, cudaEventDisableTiming) != cudaSuccess ||
+                       cudaEventCreateWithFlags(&x.join_ev, cudaEventDisableTiming) != cudaSuccess)) {
       cudaGetLastError();
       return nullptr;
     }
@@ -2943,8 +2925,8 @@ static SideStream* side_stream() {
   }
   if (!s.stream) {
     if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&s.fork_ev, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&s.join_ev, cudaEventDisableTiming) != cudaSuccess) {
       cudaGetLastError();
       s.stream = nullptr;
       return nullptr;
@@ -2953,21 +2935,83 @@ static SideStream* side_stream() {
   return &s;
 }
 
-#define TB_TRY(expr)        \
-  do {                      \
-    int _rc = (expr);       \
-    if (_rc) return _rc;    \
-  } while (0)
+// =========================================================================================
+// The plan: which recurrence each direction runs for a shape, and what the weight-gradient tail of the backward takes from
+// that choice.  lstm_plan is the only place that decides; lstm_forward and lstm_backward both follow its result, so the
+// backward always finds the buffers its forward wrote.
+// =========================================================================================
+enum LstmKind : int {  // numbered as TB_LSTM_* in torchbeast_b200.h
+  kLstmStep = TB_LSTM_STEP,                      // T+1 step kernels per layer (any shape)
+  kLstmPersistent = TB_LSTM_PERSISTENT,          // one cooperative fp32 kernel per layer
+  kLstmPersistentMma = TB_LSTM_PERSISTENT_MMA,   // one cooperative kernel per layer, bf16 mma.sync products
+  kLstmCluster = TB_LSTM_CLUSTER,                // one 16-CTA cluster per layer, split-bf16 products (H = 256)
+  kLstmWaveBf16 = TB_LSTM_WAVE_BF16,             // both layers in one cooperative wavefront kernel, bf16 products
+  kLstmWaveSplit = TB_LSTM_WAVE_SPLIT,           // both layers in one wavefront grid of 2-CTA clusters, split-bf16
+};
+
+// where the backward runs the weight-gradient GEMMs (and the bias-gradient copy)
+enum LstmWgrad : int {
+  kWgradCaller,  // on the caller's stream, with the caller's split-K scratch
+  kWgradTail,    // both layers' on the side stream after the wavefront kernel, with ws.wg_scratch; lstm_backward_join joins
+  kWgradSide,    // the upper layer's on the side stream beside the lower layer's recurrence, grid capped to the SMs that
+                 // recurrence leaves idle, with the caller's scratch: joined before the lower layer's GEMMs reuse it
+};
+
+struct LstmPlan {
+  LstmKind fwd = kLstmStep, bwd = kLstmStep;
+  // precision > 0: the operands of the weight-gradient GEMMs
+  bool hm_q = false;         // masked h: the bf16 hmq planes the forward recurrence wrote (else hm, converted into hmb)
+  bool hm_q_lo = false;      //   ... with their lo plane at hmq_lo
+  bool x1_hq = false;        // layer 1's input: slot t+1 of layer 0's hq planes, lo plane at hq_lo (else layer 1's xb)
+  bool dg_done = false;      // the backward recurrence wrote the gate gradients in bf16 (dgb) and summed the bias gradients
+  bool dx_mid_done = false;  // the backward recurrence wrote the upper layer's dx (ws.dx_mid)
+  LstmWgrad wgrad = kWgradCaller;
+};
+
+static LstmPlan lstm_plan(int64_t B, int In, int H, int layers, int precision) {
+  LstmPlan p;
+  if (precision == 2 && layers == 2 && wave_split_fits(B, In, H)) {
+    p.fwd = p.bwd = kLstmWaveSplit;
+  } else if (precision == 1 && mma_fits(B, H)) {
+    // the forward wavefront takes any input width, the backward one needs In <= H
+    p.fwd = layers == 2 && wave_fwd_fits(B, H) ? kLstmWaveBf16 : kLstmPersistentMma;
+    p.bwd = layers == 2 && In <= H && wave_bwd_fits(B, H) ? kLstmWaveBf16 : kLstmPersistentMma;
+  } else {
+    // fp32 recurrence kernels; at precision 2 the cluster kernels where they fit (backward: one layer only)
+    p.fwd = precision == 2 && cluster_fwd_fits(B, H) ? kLstmCluster : persistent_fwd_fits(B, H) ? kLstmPersistent : kLstmStep;
+    p.bwd = precision == 2 && layers == 1 && cluster_bwd_fits(B, H) ? kLstmCluster
+            : persistent_bwd_fits(B, H)                            ? kLstmPersistent
+                                                                   : kLstmStep;
+  }
+  p.hm_q = p.fwd == kLstmPersistentMma || p.fwd == kLstmWaveBf16 || p.fwd == kLstmWaveSplit;
+  p.hm_q_lo = p.x1_hq = p.fwd == kLstmWaveSplit;
+  p.dg_done = p.bwd == kLstmPersistentMma || p.bwd == kLstmWaveBf16 || p.bwd == kLstmWaveSplit;
+  p.dx_mid_done = p.bwd == kLstmWaveBf16 || p.bwd == kLstmWaveSplit;
+  p.wgrad = p.dx_mid_done ? kWgradTail : (p.bwd == kLstmPersistentMma && layers == 2) ? kWgradSide : kWgradCaller;
+  return p;
+}
+
+// hN / cN of layer l: the last step's h and c
+static int copy_state(float* hN, float* cN, int l, const float* hs, const float* cs, int64_t T1, int64_t B, int H,
+                      cudaStream_t st) {
+  cudaError_t e = cudaMemcpyAsync(hN + int64_t(l) * B * H, hs + (T1 - 1) * B * H, sizeof(float) * B * H,
+                                  cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess)
+    e = cudaMemcpyAsync(cN + int64_t(l) * B * H, cs + (T1 - 1) * B * H, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, st);
+  TB_REQUIRE(e == cudaSuccess, "lstm: state copy: %s", cudaGetErrorString(e));
+  return 0;
+}
 
 int lstm_forward(const float* x, const float* notdone, const float* h0, const float* c0, const LstmParams& p,
                  int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* y, float* hN, float* cN,
-                 float* splitk, int precision, cudaStream_t st) {
+                 int precision, cudaStream_t st) {
   TB_REQUIRE(layers >= 1 && layers <= kLstmMaxLayers, "lstm: 1..%d layers", kLstmMaxLayers);
+  const LstmPlan plan = lstm_plan(B, In, H, layers, precision);
   const int64_t N = T1 * B;
-  const float* xin = x;
-  int in_dim = In;
-  if (precision == 1 && layers == 2 && wave_fwd_applicable(B, H)) {
-    // both layers in one wavefront kernel: only layer 0's input projection is hoisted
+  if (plan.fwd == kLstmWaveBf16 || plan.fwd == kLstmWaveSplit) {
+    // both layers in one wavefront kernel: only layer 0's input projection is hoisted (one wgmma GEMM, split at precision
+    // 2, where every lo offset below is non-zero)
+    const bool split = plan.fwd == kLstmWaveSplit;
     const int Hq = mma_hq(H);
     for (int l = 0; l < 2; ++l) {
       LstmLayerWs& L = ws.layer[l];
@@ -2975,47 +3019,7 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
       const int64_t l16 = ld16(in_l);
       add2_kernel<<<(4 * H + 255) / 256, 256, 0, st>>>(p.b_ih[l], p.b_hh[l], L.bsum, 4 * H);
       TB_TRY(check_launch("add2_kernel"));
-      TB_TRY(pack_weights_bf16(p.w_ih[l], L.wihb, 4 * H, 1, in_l, l16, st));  // layer 1's is used by the backward
-      if (l == 0) {
-        TB_TRY(f32_to_bf16(x, L.xb, N, In, In, l16, st));
-        TcEpilogue te; te.C = L.gates; te.ldc = 4 * H; te.bias = L.bsum; te.tag = "lstm_xproj_fwd";
-        TB_TRY(gemm_tc_bf16(L.xb, L.wihb, N, 4 * H, In, l16, l16, te, st));
-      }
-      cudaError_t eq = cudaMemsetAsync(L.hmq, 0, size_t(N) * Hq * 2, st);
-      if (eq == cudaSuccess) eq = cudaMemsetAsync(L.hq, 0, size_t(N + B) * Hq * 2, st);
-      TB_REQUIRE(eq == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(eq));
-      lstm_init_state_q_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(
-          h0 + int64_t(l) * B * H, c0 + int64_t(l) * B * H, notdone, static_cast<__nv_bfloat16*>(L.hmq), L.cm, int(B), H,
-          Hq, static_cast<__nv_bfloat16*>(L.hq));
-      TB_TRY(check_launch("lstm_init_state_q_kernel"));
-    }
-    {
-      ProfScope prof("lstm_recurrence_fwd", st);
-      TB_TRY(lstm2_fwd_wave(ws, p, y, notdone, T1, B, H, st));
-    }
-    TB_TRY(f32_to_bf16(ws.layer[0].hs, ws.layer[1].xb, N, H, H, ld16(H), st));  // layer 1's input, for its dW_ih GEMM
-    for (int l = 0; l < 2; ++l) {
-      const float* hs = (l == 1) ? y : ws.layer[0].hs;
-      cudaError_t e = cudaMemcpyAsync(hN + int64_t(l) * B * H, hs + (T1 - 1) * B * H, sizeof(float) * B * H,
-                                      cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess)
-        e = cudaMemcpyAsync(cN + int64_t(l) * B * H, ws.layer[l].cs + (T1 - 1) * B * H, sizeof(float) * B * H,
-                            cudaMemcpyDeviceToDevice, st);
-      TB_REQUIRE(e == cudaSuccess, "lstm: state copy: %s", cudaGetErrorString(e));
-    }
-    return 0;
-  }
-  // (forward and backward are decided together: the split backward consumes the blocked saves only the split forward writes)
-  if (precision == 2 && layers == 2 && wave_bwd_split_applicable(B, In, H)) {
-    // split-bf16 wavefront: layer 0's input projection is one split wgmma GEMM, everything sequential is ONE kernel
-    const int Hq = mma_hq(H);
-    for (int l = 0; l < 2; ++l) {
-      LstmLayerWs& L = ws.layer[l];
-      const int in_l = (l == 0) ? In : H;
-      const int64_t l16 = ld16(in_l);
-      add2_kernel<<<(4 * H + 255) / 256, 256, 0, st>>>(p.b_ih[l], p.b_hh[l], L.bsum, 4 * H);
-      TB_TRY(check_launch("add2_kernel"));
-      TB_TRY(pack_weights_bf16(p.w_ih[l], L.wihb, 4 * H, 1, in_l, l16, st, L.wihb_lo));  // layer 1's: backward (dx)
+      TB_TRY(pack_weights_bf16(p.w_ih[l], L.wihb, 4 * H, 1, in_l, l16, st, L.wihb_lo));  // layer 1's is used by the backward
       if (l == 0) {
         TB_TRY(f32_to_bf16(x, L.xb, N, In, In, l16, st, L.xb_lo));
         TcEpilogue te; te.C = L.gates; te.ldc = 4 * H; te.bias = L.bsum; te.tag = "lstm_xproj_fwd";
@@ -3026,20 +3030,37 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
       cudaError_t eq = cudaMemsetAsync(L.hmq, 0, size_t(L.hmq_lo + N * Hq) * 2, st);
       if (eq == cudaSuccess) eq = cudaMemsetAsync(L.hq, 0, size_t(L.hq_lo + (N + B) * Hq) * 2, st);
       TB_REQUIRE(eq == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(eq));
-      lstm_init_state_split_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(
-          h0 + int64_t(l) * B * H, notdone, static_cast<__nv_bfloat16*>(L.hq), L.hq_lo, static_cast<__nv_bfloat16*>(L.hmq), L.hmq_lo,
-          int(B), H, Hq);
-      TB_TRY(check_launch("lstm_init_state_split_kernel"));
+      const float* h0l = h0 + int64_t(l) * B * H;
+      __nv_bfloat16* hq = static_cast<__nv_bfloat16*>(L.hq);
+      __nv_bfloat16* hmq = static_cast<__nv_bfloat16*>(L.hmq);
+      if (split) {
+        lstm_init_state_split_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(h0l, notdone, hq, L.hq_lo, hmq, L.hmq_lo,
+                                                                                      int(B), H, Hq);
+        TB_TRY(check_launch("lstm_init_state_split_kernel"));
+      } else {
+        lstm_init_state_q_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(h0l, c0 + int64_t(l) * B * H, notdone, hmq,
+                                                                                  L.cm, int(B), H, Hq, hq);
+        TB_TRY(check_launch("lstm_init_state_q_kernel"));
+      }
     }
     {
       ProfScope prof("lstm_recurrence_fwd", st);
-      TB_TRY(lstm2_fwd_wave_split(ws, p, y, notdone, c0, hN, cN, T1, B, H, st));  // writes hN / cN itself
+      TB_TRY(split ? lstm2_fwd_wave_split(ws, p, y, notdone, c0, hN, cN, T1, B, H, st)  // writes hN / cN itself
+                   : lstm2_fwd_wave(ws, p, y, notdone, T1, B, H, st));
     }
-    return 0;
+    if (split) return 0;
+    TB_TRY(f32_to_bf16(ws.layer[0].hs, ws.layer[1].xb, N, H, H, ld16(H), st));  // layer 1's input, for its dW_ih GEMM
+    TB_TRY(copy_state(hN, cN, 0, ws.layer[0].hs, ws.layer[0].cs, T1, B, H, st));
+    return copy_state(hN, cN, 1, y, ws.layer[1].cs, T1, B, H, st);
   }
+  const int Hp = padded_h(H);
+  const float* xin = x;
+  int in_dim = In;
   for (int l = 0; l < layers; ++l) {
     LstmLayerWs& L = ws.layer[l];
     float* hs = (l == layers - 1) ? y : L.hs;
+    const float* h0l = h0 + int64_t(l) * B * H;
+    const float* c0l = c0 + int64_t(l) * B * H;
     add2_kernel<<<(4 * H + 255) / 256, 256, 0, st>>>(p.b_ih[l], p.b_hh[l], L.bsum, 4 * H);
     TB_TRY(check_launch("add2_kernel"));
     if (precision) {
@@ -3054,205 +3075,121 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
       TB_TRY((gemm_simt<float, float, false, true>(xin, p.w_ih[l], L.gates, N, 4 * H, in_dim, in_dim, in_dim, 4 * H, ep, 1,
                                                     nullptr, st)));
     }
-    const int Hp = padded_h(H);
-    // precision 2 (split-bf16 GEMMs) keeps the recurrence itself in exact fp32 (lstm_*_persistent_kernel)
-    const bool use_mma = precision == 1 && mma_recurrence_applicable(B, H);
-    if (!use_mma) {  // operands of the fp32 recurrence kernels
+    if (plan.fwd != kLstmPersistentMma) {  // operands of the fp32-state kernels: padded W_hh, masked initial state
       const int64_t tot = int64_t(4 * H + 4) * Hp;
       lstm_pack_whh_kernel<<<(unsigned)((tot + 255) / 256 > 1184 ? 1184 : (tot + 255) / 256), 256, 0, st>>>(p.w_hh[l], L.wp, H, Hp);
       TB_TRY(check_launch("lstm_pack_whh_kernel"));
       cudaError_t em = cudaMemsetAsync(L.hm, 0, sizeof(float) * N * Hp, st);  // zero the row padding
       TB_REQUIRE(em == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(em));
-      lstm_init_state_kernel<<<(unsigned)((B * Hp + 255) / 256), 256, 0, st>>>(
-          h0 + int64_t(l) * B * H, c0 + int64_t(l) * B * H, notdone, L.hm, L.cm, int(B), H, Hp);
+      lstm_init_state_kernel<<<(unsigned)((B * Hp + 255) / 256), 256, 0, st>>>(h0l, c0l, notdone, L.hm, L.cm, int(B), H, Hp);
       TB_TRY(check_launch("lstm_init_state_kernel"));
     }
     ProfScope prof("lstm_recurrence_fwd", st);
-    int prc = -1;
-    if (use_mma) {
+    if (plan.fwd == kLstmPersistentMma) {
       const int Hq = mma_hq(H);
       cudaError_t eq = cudaMemsetAsync(L.hmq, 0, size_t(N) * Hq * 2, st);
       TB_REQUIRE(eq == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(eq));
       lstm_init_state_q_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(
-          h0 + int64_t(l) * B * H, c0 + int64_t(l) * B * H, notdone, static_cast<__nv_bfloat16*>(L.hmq), L.cm, int(B), H, Hq);
+          h0l, c0l, notdone, static_cast<__nv_bfloat16*>(L.hmq), L.cm, int(B), H, Hq);
       TB_TRY(check_launch("lstm_init_state_q_kernel"));
-      prc = lstm_fwd_persistent_mma(L, p.w_hh[l], hs, notdone, T1, B, H, ws.sync, st);
-      TB_REQUIRE(prc >= 0, "lstm: tensor-core recurrence kernel does not fit (B=%lld H=%d)", (long long)B, H);
+      TB_TRY(lstm_fwd_persistent_mma(L, p.w_hh[l], hs, notdone, T1, B, H, ws.sync, st));
+    } else if (plan.fwd == kLstmCluster) {
+      TB_TRY(lstm_fwd_cluster(L, p.w_hh[l], hs, notdone, T1, B, H, st));
+    } else if (plan.fwd == kLstmPersistent) {
+      TB_TRY(lstm_fwd_persistent(L, hs, notdone, T1, B, H, ws.sync, st));
+    } else {
+      TB_TRY(lstm_fwd_steps(L, hs, notdone, T1, B, H, st));
     }
-    if (prc < 0 && precision == 2) prc = lstm_fwd_cluster(L, p.w_hh[l], hs, notdone, T1, B, H, st);   // H = 256, B <= 32
-    if (prc < 0) prc = lstm_fwd_persistent(L, hs, notdone, T1, B, H, ws.sync, st);
-    if (prc > 0) return prc;
-    for (int64_t t = 0; prc < 0 && t < T1; ++t) {
-      StepArgs a;
-      a.hm = L.hm + t * B * Hp;
-      a.cm = L.cm + t * B * H;
-      const bool last = (t == T1 - 1);
-      a.nd_next = last ? nullptr : notdone + (t + 1) * B;
-      a.wp = L.wp;
-      a.gates = L.gates + t * B * 4 * H;
-      a.hs = hs + t * B * H; a.cs = L.cs + t * B * H;
-      a.hm_next = last ? nullptr : L.hm + (t + 1) * B * Hp;
-      a.cm_next = last ? nullptr : L.cm + (t + 1) * B * H;
-      a.B = int(B); a.H = H; a.Hp = Hp;
-      TB_TRY(launch_step_fwd(a, st));
-    }
-    cudaError_t e = cudaMemcpyAsync(hN + int64_t(l) * B * H, hs + (T1 - 1) * B * H, sizeof(float) * B * H,
-                                    cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess)
-      e = cudaMemcpyAsync(cN + int64_t(l) * B * H, L.cs + (T1 - 1) * B * H, sizeof(float) * B * H,
-                          cudaMemcpyDeviceToDevice, st);
-    TB_REQUIRE(e == cudaSuccess, "lstm: state copy: %s", cudaGetErrorString(e));
+    TB_TRY(copy_state(hN, cN, l, hs, L.cs, T1, B, H, st));
     xin = hs;
     in_dim = H;
   }
-  (void)splitk;
   return 0;
-}
-
-static int splits_for(int64_t M, int64_t N, int64_t K, int64_t scratch_floats) {
-  const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
-  const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
-  const int64_t ktiles = (K + kGemmBK - 1) / kGemmBK;
-  if (s > ktiles / 4) s = ktiles / 4;
-  if (s * M * N > scratch_floats) s = scratch_floats / (M * N);
-  if (s > 64) s = 64;
-  if (s < 1) s = 1;
-  return int(s);
 }
 
 static thread_local SideStream* g_pending_join = nullptr;
 
 int lstm_backward_join(cudaStream_t st) {
-  if (!g_pending_join) return 0;
-  cudaError_t e = cudaStreamWaitEvent(st, g_pending_join->join, 0);
+  SideStream* s = g_pending_join;
   g_pending_join = nullptr;
-  TB_REQUIRE(e == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(e));
-  return 0;
+  return s ? s->wait(st) : 0;
 }
 
 int lstm_backward(const float* dy, const float* x, const float* notdone, const LstmParams& p, const LstmGrads& g,
                   int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* dx, float* splitk,
                   float* colsum_scratch, int precision, cudaStream_t st) {
+  const LstmPlan plan = lstm_plan(B, In, H, layers, precision);
   const int64_t N = T1 * B;
-  const int64_t scratch = int64_t(8) << 20;  // == kSplitKScratchFloats (atarinet.cu)
-  const float* dyl = dy;
-  bool forked = false;
-  // two layers on the tensor-core backend: ONE wavefront kernel runs both recurrences (and the upper layer's
-  // input-gradient product); only the hoisted weight-gradient GEMMs and the lower layer's dx remain per layer
-  bool wave_done = false;
-  const bool split_fwd = precision == 2 && layers == 2 && wave_bwd_split_applicable(B, In, H);  // same predicate as the forward
-  bool split_bwd = false;  // the split wavefront kernel ran: gate gradients are already bf16 hi/lo planes, bias gradients summed
-  if (precision == 1 && layers == 2 && In <= H && wave_bwd_applicable(B, H)) {
+  const int Hp = padded_h(H);
+  const bool wave = plan.bwd == kLstmWaveBf16 || plan.bwd == kLstmWaveSplit;
+  if (wave) {
+    // both layers' recurrences (and the upper layer's input gradient) in one kernel; only the hoisted weight-gradient
+    // GEMMs and the lower layer's dx remain per layer.  (The 4 padding columns of the split kernel's [N, ld16(4H)] gate
+    // gradient planes are never read as data: the GEMMs' tensor maps end at column 4H.)
     ProfScope prof("lstm_recurrence_bwd", st);
-    TB_TRY(lstm2_bwd_wave(ws, p, g, dy, notdone, T1, B, H, st));
-    wave_done = true;
-  } else if (split_fwd) {
-    // (the 4 padding columns of the [N, ld16(4H)] gate-gradient planes are never read as data: the GEMMs' tensor maps
-    //  end at column 4H)
-    ProfScope prof("lstm_recurrence_bwd", st);
-    TB_TRY(lstm2_bwd_wave_split(ws, p, g, dy, notdone, T1, B, H, st));
-    wave_done = true;
-    split_bwd = true;
+    TB_TRY(plan.bwd == kLstmWaveSplit ? lstm2_bwd_wave_split(ws, p, g, dy, notdone, T1, B, H, st)
+                                      : lstm2_bwd_wave(ws, p, g, dy, notdone, T1, B, H, st));
   }
-  // After the wavefront kernel only the hoisted weight-gradient GEMMs of both layers (and the lower layer's dx) remain.
-  // The GEMMs feed nothing downstream in this backward pass: fork them onto the side stream (own split-K scratch); the
-  // caller joins with lstm_backward_join().
-  SideStream* tail = (wave_done && ws.wg_scratch) ? side_stream() : nullptr;
-  if (tail) {
+  // The weight-gradient GEMMs feed nothing downstream in this backward pass: see LstmWgrad for where they run.  Without a
+  // side stream they run on the caller's.
+  SideStream* side = plan.wgrad == kWgradCaller ? nullptr : side_stream();
+  if (side && plan.wgrad == kWgradTail) {
     TB_TRY(lstm_backward_join(st));  // a previous call's fork must be joined before its event is reused
-    cudaError_t ee = cudaEventRecord(tail->fork, st);
-    if (ee == cudaSuccess) ee = cudaStreamWaitEvent(tail->stream, tail->fork, 0);
-    TB_REQUIRE(ee == cudaSuccess, "lstm: side stream fork: %s", cudaGetErrorString(ee));
+    TB_TRY(side->fork(st));
   }
+  const float* dyl = dy;
   for (int l = layers - 1; l >= 0; --l) {
     LstmLayerWs& L = ws.layer[l];
     const float* xin = (l == 0) ? x : ws.layer[l - 1].hs;
     const int in_dim = (l == 0) ? In : H;
     float* dxl = (l == 0) ? dx : ws.dx_mid;
-    const int Hp = padded_h(H);
-    const bool use_mma = precision == 1 && mma_recurrence_applicable(B, H);
-    if (!use_mma && !split_bwd) {  // operands of the fp32 recurrence kernels
+    if (!plan.dg_done) {  // operands of the fp32-state kernels
       const int64_t tot = int64_t(H + 4) * 4 * Hp;
       lstm_pack_whh_t_kernel<<<(unsigned)((tot + 255) / 256 > 1184 ? 1184 : (tot + 255) / 256), 256, 0, st>>>(p.w_hh[l], L.w_hh_t, H, Hp);
       TB_TRY(check_launch("lstm_pack_whh_t_kernel"));
       cudaError_t em = cudaMemsetAsync(ws.dgp, 0, sizeof(float) * 4 * B * Hp, st);  // zero the row padding
       TB_REQUIRE(em == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(em));
     }
-    if (!wave_done) {
-    ProfScope prof("lstm_recurrence_bwd", st);
-    int prc = -1;
-    if (use_mma) {
-      prc = lstm_bwd_persistent_mma(L, p.w_hh[l], dyl, notdone, T1, B, H, g.b_ih[l], ws.sync + 16, st);
-      TB_REQUIRE(prc >= 0, "lstm: tensor-core recurrence kernel does not fit (B=%lld H=%d)", (long long)B, H);
-    }
-    if (prc < 0 && precision == 2 && layers == 1) prc = lstm_bwd_cluster(L, p.w_hh[l], dyl, notdone, T1, B, H, st);   // H = 256, B <= 32
-    if (prc < 0) prc = lstm_bwd_persistent(L, ws, dyl, notdone, T1, B, H, ws.sync + 16, st);
-    if (prc > 0) return prc;
-    for (int64_t t = T1 - 1; prc < 0 && t >= 0; --t) {
-      BwdPointArgs a;
-      a.dy = dyl + t * B * H;
-      a.first = (t == T1 - 1);
-      a.dh_raw = ws.dh; a.nd_next = a.first ? nullptr : notdone + (t + 1) * B;
-      a.nd = notdone + t * B;
-      a.gates = L.gates + t * B * 4 * H; a.cs = L.cs + t * B * H; a.cm = L.cm + t * B * H;
-      a.dc = ws.dc; a.dgates = L.dgates + t * B * 4 * H; a.B = int(B); a.H = H; a.dgp = ws.dgp; a.Hp = Hp;
-      const int64_t total = B * H;
-      lstm_step_bwd_point_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
-      TB_TRY(check_launch("lstm_step_bwd_point_kernel"));
-      if (t > 0) {
-        // dh_raw[B,H] = dgates_t[B,4H] . W_hh[4H,H]   (masked by notdone_t when consumed at t-1)
-        DhArgs d;
-        d.dgp = ws.dgp; d.wtp = L.w_hh_t; d.dh_raw = ws.dh; d.B = int(B); d.H = H; d.Hp = Hp;
-        TB_TRY(launch_step_bwd_dh(d, st));
-      }
-    }
+    if (!wave) {
+      ProfScope prof("lstm_recurrence_bwd", st);
+      if (plan.bwd == kLstmPersistentMma)
+        TB_TRY(lstm_bwd_persistent_mma(L, p.w_hh[l], dyl, notdone, T1, B, H, g.b_ih[l], ws.sync + 16, st));
+      else if (plan.bwd == kLstmCluster)
+        TB_TRY(lstm_bwd_cluster(L, p.w_hh[l], dyl, notdone, T1, B, st));
+      else if (plan.bwd == kLstmPersistent)
+        TB_TRY(lstm_bwd_persistent(L, ws, dyl, notdone, T1, B, H, ws.sync + 16, st));
+      else
+        TB_TRY(lstm_bwd_steps(L, ws, dyl, notdone, T1, B, H, st));
     }
     // parameter gradients over all steps at once
     if (precision) {
       const int64_t lg = ld16(4 * H), lh = ld16(H), li = ld16(in_dim);
-      if (forked) {  // the upper layer's side-stream GEMMs used the split-K scratch: join before reusing it
-        cudaError_t ej = cudaStreamWaitEvent(st, side_stream()->join, 0);
-        TB_REQUIRE(ej == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(ej));
-        forked = false;
-      }
-      // the tensor-core recurrence wrote the gate gradients in bf16 and summed the bias gradients itself
-      if (!use_mma && !split_bwd) TB_TRY(f32_to_bf16(L.dgates, L.dgb, N, 4 * H, 4 * H, lg, st, L.dgb_lo));
+      if (side && plan.wgrad == kWgradSide && l == 0) TB_TRY(side->wait(st));  // the upper layer's GEMMs used splitk
+      if (!plan.dg_done) TB_TRY(f32_to_bf16(L.dgates, L.dgb, N, 4 * H, 4 * H, lg, st, L.dgb_lo));
       const void* hm_b = L.hmb;
       int64_t hm_ld = lh, hm_lo = L.hmb_lo;
+      if (plan.hm_q) {
+        hm_b = L.hmq; hm_ld = mma_hq(H); hm_lo = plan.hm_q_lo ? L.hmq_lo : 0;
+      } else {
+        TB_TRY(f32_to_bf16(L.hm, L.hmb, N, H, Hp, lh, st, L.hmb_lo));
+      }
       const void* x_b = L.xb;
       int64_t x_ld = li, x_lo = L.xb_lo;
-      if (use_mma) {  // the tensor-core forward recurrence already left the masked h in bf16
-        hm_b = L.hmq; hm_ld = mma_hq(H); hm_lo = 0;
-      } else if (split_fwd) {
-        // the split wavefront forward left the masked h as hi / lo planes, and layer 1's input (= layer 0's raw h_t) is
-        // slot t+1 of layer 0's exchange planes
-        hm_b = L.hmq; hm_ld = mma_hq(H); hm_lo = L.hmq_lo;
-        if (l == 1) {
-          x_b = static_cast<const __nv_bfloat16*>(ws.layer[0].hq) + B * mma_hq(H); x_ld = mma_hq(H); x_lo = ws.layer[0].hq_lo;
-        }
-      } else {
-        TB_TRY(f32_to_bf16(L.hm, L.hmb, N, H, padded_h(H), lh, st, L.hmb_lo));
+      if (plan.x1_hq && l == 1) {
+        x_b = static_cast<const __nv_bfloat16*>(ws.layer[0].hq) + B * mma_hq(H); x_ld = mma_hq(H); x_lo = ws.layer[0].hq_lo;
       }
       const int64_t kb = (N + 63) / 64;
       int sp = int(kb / 8); if (sp < 1) sp = 1; if (sp > 4) sp = 4;
-      // The weight-gradient GEMMs of the UPPER layer do not feed the lower layer's recurrence (only dx does), and that
-      // recurrence occupies 65 SMs: run them on a side stream with a grid capped to the idle SMs and join before the
-      // split-K scratch is needed again.
-      SideStream* side = (use_mma && l == 1 && layers == 2 && !wave_done) ? side_stream() : nullptr;
       cudaStream_t gs = st;
       float* wscr = splitk;
       TcEpilogue te; te.tag = "lstm_wgrad";
-      if (tail) {
-        gs = tail->stream; wscr = ws.wg_scratch;
-      }
-      if (side) {
-        cudaError_t ee = cudaEventRecord(side->fork, st);
-        if (ee == cudaSuccess) ee = cudaStreamWaitEvent(side->stream, side->fork, 0);
-        TB_REQUIRE(ee == cudaSuccess, "lstm: side stream fork: %s", cudaGetErrorString(ee));
+      const bool fork = side && plan.wgrad == kWgradSide && l == 1;
+      if (side && plan.wgrad == kWgradTail) {
+        gs = side->stream; wscr = ws.wg_scratch;
+      } else if (fork) {
+        TB_TRY(side->fork(st));
         gs = side->stream;
         te.max_ctas = kNumSMs - int((H + kBwdCols - 1) / kBwdCols) - 2;
-        forked = true;
       }
       te.C = g.w_hh[l]; te.ldc = H;      // dW_hh[4H,H] = dgates^T . hm   (both operands stored [N, .]: MN-major)
       te.a_lo = L.dgb_lo; te.b_lo = hm_lo;
@@ -3260,41 +3197,36 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
       te.C = g.w_ih[l]; te.ldc = in_dim;  // dW_ih[4H,in] = dgates^T . x
       te.b_lo = x_lo;
       TB_TRY(gemm_tc_bf16_ex(L.dgb, x_b, 4 * H, in_dim, N, lg, x_ld, true, true, te, sp, wscr, gs));
-      if (!use_mma && !split_bwd) TB_TRY(colsum(L.dgates, g.b_ih[l], N, 4 * H, 4 * H, colsum_scratch, st));
+      if (!plan.dg_done) TB_TRY(colsum(L.dgates, g.b_ih[l], N, 4 * H, 4 * H, colsum_scratch, st));
       cudaError_t e = cudaMemcpyAsync(g.b_hh[l], g.b_ih[l], sizeof(float) * 4 * H, cudaMemcpyDeviceToDevice, gs);
       TB_REQUIRE(e == cudaSuccess, "lstm: bias grad copy: %s", cudaGetErrorString(e));
-      if (side) {
-        e = cudaEventRecord(side->join, side->stream);
-        TB_REQUIRE(e == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(e));
-      }
+      if (fork) TB_TRY(side->join());
       // dx[N,in] = dgates[N,4H] . W_ih[4H,in]   (W_ih as stored: reduction index is its row index)
-      if (!(wave_done && l == 1)) {  // the wavefront kernel already produced the upper layer's dx (= ws.dx_mid)
+      if (!(plan.dx_mid_done && l == 1)) {
         TcEpilogue td; td.tag = "lstm_xproj_dgrad"; td.C = dxl; td.ldc = in_dim;
         td.a_lo = L.dgb_lo; td.b_lo = L.wihb_lo;
         TB_TRY(gemm_tc_bf16_ex(L.dgb, L.wihb, N, in_dim, 4 * H, lg, li, false, true, td, 1, nullptr, st));
       }
     } else {
-    GemmEpilogue ep; ep.tag = "lstm_wgrad";
-    int s = splits_for(4 * H, H, N, scratch);
-    TB_TRY((gemm_simt<float, float, true, false>(L.dgates, L.hm, g.w_hh[l], 4 * H, H, N, 4 * H, padded_h(H), H, ep, s, splitk,
-                                                  st)));
-    s = splits_for(4 * H, in_dim, N, scratch);
-    TB_TRY((gemm_simt<float, float, true, false>(L.dgates, xin, g.w_ih[l], 4 * H, in_dim, N, 4 * H, in_dim, in_dim, ep, s,
-                                                  splitk, st)));
-    TB_TRY(colsum(L.dgates, g.b_ih[l], N, 4 * H, 4 * H, colsum_scratch, st));
-    cudaError_t e = cudaMemcpyAsync(g.b_hh[l], g.b_ih[l], sizeof(float) * 4 * H, cudaMemcpyDeviceToDevice, st);
-    TB_REQUIRE(e == cudaSuccess, "lstm: bias grad copy: %s", cudaGetErrorString(e));
-    // gradient w.r.t. this layer's input: dx[N,in] = dgates[N,4H] . W_ih[4H,in]
-    ep.tag = "lstm_xproj_dgrad";
-    TB_TRY((gemm_simt<float, float, false, false>(L.dgates, p.w_ih[l], dxl, N, in_dim, 4 * H, 4 * H, in_dim, in_dim, ep, 1,
-                                                   nullptr, st)));
+      GemmEpilogue ep; ep.tag = "lstm_wgrad";
+      int s = simt_splits(4 * H, H, N, kSplitKScratchFloats, 64);
+      TB_TRY((gemm_simt<float, float, true, false>(L.dgates, L.hm, g.w_hh[l], 4 * H, H, N, 4 * H, Hp, H, ep, s, splitk, st)));
+      s = simt_splits(4 * H, in_dim, N, kSplitKScratchFloats, 64);
+      TB_TRY((gemm_simt<float, float, true, false>(L.dgates, xin, g.w_ih[l], 4 * H, in_dim, N, 4 * H, in_dim, in_dim, ep, s,
+                                                    splitk, st)));
+      TB_TRY(colsum(L.dgates, g.b_ih[l], N, 4 * H, 4 * H, colsum_scratch, st));
+      cudaError_t e = cudaMemcpyAsync(g.b_hh[l], g.b_ih[l], sizeof(float) * 4 * H, cudaMemcpyDeviceToDevice, st);
+      TB_REQUIRE(e == cudaSuccess, "lstm: bias grad copy: %s", cudaGetErrorString(e));
+      // gradient w.r.t. this layer's input: dx[N,in] = dgates[N,4H] . W_ih[4H,in]
+      ep.tag = "lstm_xproj_dgrad";
+      TB_TRY((gemm_simt<float, float, false, false>(L.dgates, p.w_ih[l], dxl, N, in_dim, 4 * H, 4 * H, in_dim, in_dim, ep, 1,
+                                                     nullptr, st)));
     }
     dyl = dxl;
   }
-  if (tail) {
-    cudaError_t e = cudaEventRecord(tail->join, tail->stream);
-    TB_REQUIRE(e == cudaSuccess, "lstm: side stream join: %s", cudaGetErrorString(e));
-    g_pending_join = tail;
+  if (side && plan.wgrad == kWgradTail) {
+    TB_TRY(side->join());
+    g_pending_join = side;
   }
   return 0;
 }
@@ -3308,8 +3240,6 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
 using namespace tb;
 
 namespace {
-constexpr int64_t kLstmAbiSplitK = int64_t(8) << 20;  // floats, == kSplitKScratchFloats of the network entry points
-
 struct LstmAbiWs { LstmWs ws; float* splitk; float* colsum; size_t bytes; };
 
 LstmAbiWs lstm_abi_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int precision) {
@@ -3318,7 +3248,7 @@ LstmAbiWs lstm_abi_ws(void* base, int64_t T1, int64_t B, int In, int H, int laye
   size_t off = (lbytes + 255) & ~size_t(255);
   w.ws = lstm_ws(base, T1, B, In, H, layers, precision);
   w.splitk = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-  off += size_t(kLstmAbiSplitK) * sizeof(float);
+  off += size_t(kSplitKScratchFloats) * sizeof(float);
   w.colsum = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
   off += size_t(colsum_scratch_floats(4 * int64_t(H) > 512 ? 4 * int64_t(H) : 512)) * sizeof(float);
   w.bytes = off;
@@ -3329,7 +3259,6 @@ int lstm_abi_check(int64_t T1, int64_t B, int In, int H, int layers, int precisi
   TB_REQUIRE(T1 >= 1 && B >= 1 && In >= 1 && H >= 1, "tb_lstm: bad sizes T1=%lld B=%lld In=%d H=%d", (long long)T1, (long long)B, In, H);
   TB_REQUIRE(layers >= 1 && layers <= kLstmMaxLayers, "tb_lstm: 1..%d layers", kLstmMaxLayers);
   TB_REQUIRE(precision >= 0 && precision <= 2, "tb_lstm: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
-  TB_REQUIRE(precision == 0 || ((In % 1) == 0), "tb_lstm: bad precision");
   return 0;
 }
 }  // namespace
@@ -3346,6 +3275,16 @@ size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden
   return lstm_abi_ws(nullptr, T1, B, input_size, hidden_size, layers, precision).bytes;
 }
 
+int tb_lstm_plan(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kind_host,
+                 int* bwd_kind_host) {
+  if (lstm_abi_check(1, B, input_size, hidden_size, layers, precision)) return 1;
+  TB_REQUIRE(fwd_kind_host && bwd_kind_host, "tb_lstm_plan: null pointer");
+  const LstmPlan plan = lstm_plan(B, input_size, hidden_size, layers, precision);
+  *fwd_kind_host = plan.fwd;
+  *bwd_kind_host = plan.bwd;
+  return 0;
+}
+
 int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const float* c0, const float* const* params,
                     int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision, void* workspace,
                     float* y, float* hN, float* cN, void* stream) {
@@ -3357,7 +3296,7 @@ int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const
     TB_REQUIRE(p.w_ih[l] && p.w_hh[l] && p.b_ih[l] && p.b_hh[l], "tb_lstm_forward: null parameter pointer (layer %d)", l);
   }
   LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
-  return lstm_forward(x, notdone, h0, c0, p, T1, B, input_size, hidden_size, layers, w.ws, y, hN, cN, w.splitk, precision,
+  return lstm_forward(x, notdone, h0, c0, p, T1, B, input_size, hidden_size, layers, w.ws, y, hN, cN, precision,
                       (cudaStream_t)stream);
 }
 

@@ -6,6 +6,7 @@
 namespace tb {
 
 constexpr int kLstmMaxLayers = 2;
+constexpr int64_t kSplitKScratchFloats = int64_t(8) << 20;  // 32 MB: the split-K GEMM scratch the callers provide
 
 struct LstmParams {  // torch.nn.LSTM layout: weight_ih [4H, In], weight_hh [4H, H], gate order i,f,g,o
   const float* w_ih[kLstmMaxLayers]; const float* w_hh[kLstmMaxLayers];
@@ -58,16 +59,19 @@ struct LstmWs {
 size_t lstm_ws_bytes(int64_t T1, int64_t B, int In, int H, int layers, int precision);
 LstmWs lstm_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int precision);
 
-// precision: 0 = fp32 SIMT GEMMs; 1 = bf16 wgmma GEMMs for the hoisted projections and bf16 mma.sync operands in
-// the recurrence; 2 = split-bf16 (hi/lo planes, 3 MMAs) wgmma GEMMs with the recurrence in exact fp32.  State, gate
-// activations and accumulation are fp32 in every mode.
+// precision: 0 = fp32 SIMT GEMMs and the fp32 recurrence kernels; 1 = bf16 wgmma GEMMs for the hoisted projections and
+// bf16 mma.sync operands in the recurrence where it fits; 2 = split-bf16 (hi/lo planes, 3 MMAs) wgmma GEMMs, and a
+// split-bf16 recurrence where one fits (the two-layer wavefront, or the 16-CTA cluster kernels for H = 256), the fp32
+// recurrence kernels elsewhere.  lstm_plan (lstm.cu) picks the recurrence of each shape.  State, gate activations and
+// accumulation are fp32 in every mode.
 // x [T1*B, In] -> y [T1*B, H]; h0/c0/hN/cN [layers, B, H]; notdone [T1*B] (float, multiplies the state
-// before each step).  splitk: GEMM scratch (kSplitKScratchFloats).
+// before each step).
 int lstm_forward(const float* x, const float* notdone, const float* h0, const float* c0, const LstmParams& p,
                  int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* y, float* hN, float* cN,
-                 float* splitk, int precision, cudaStream_t stream);
+                 int precision, cudaStream_t stream);
 
-// dy [T1*B, H] -> dx [T1*B, In]; parameter gradients written (overwritten) into g.
+// dy [T1*B, H] -> dx [T1*B, In]; parameter gradients written (overwritten) into g.  splitk: GEMM scratch
+// (kSplitKScratchFloats).
 // Joins the side stream lstm_backward may have forked (weight-gradient GEMMs overlapping the caller's own backward):
 // call on the same stream after the work that may overlap, before anything consumes the LSTM parameter gradients.
 int lstm_backward_join(cudaStream_t stream);

@@ -178,22 +178,6 @@ ResWs<T> res_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int use_lst
   return w;
 }
 
-#define TB_TRY(expr)        \
-  do {                      \
-    int _rc = (expr);       \
-    if (_rc) return _rc;    \
-  } while (0)
-
-int splits_simt(int64_t M, int64_t N, int64_t K) {
-  const int64_t bm = (N <= 32) ? 128 : (M <= 64 ? 64 : 128), bn = (N <= 32) ? 32 : 64;
-  const int64_t tiles = ((M + bm - 1) / bm) * ((N + bn - 1) / bn);
-  int64_t s = (2 * kNumSMs + tiles - 1) / tiles;
-  const int64_t kt = (K + kGemmBK - 1) / kGemmBK;
-  if (s > kt / 4) s = kt / 4;
-  if (s * M * N > kScratchFloats) s = kScratchFloats / (M * N);
-  if (s > 128) s = 128;
-  return int(s < 1 ? 1 : s);
-}
 int splits_tc(int64_t M, int64_t N, int64_t K) {
   const int64_t bn = N <= 64 ? 64 : 128;
   const int64_t tiles = ((M + 127) / 128) * ((N + bn - 1) / bn);
@@ -239,7 +223,7 @@ int conv_dgrad(const __nv_bfloat16* dY, const __nv_bfloat16* W, __nv_bfloat16* d
 int conv_wgrad(const float* dY, const void* col, bool col_u8, float* dW, int64_t M, int cout, int64_t K, int64_t ldk, int permP,
                int permQ, float /*scale: the u8 operand is read as x/255*/, float* scratch, const char* tag, cudaStream_t st) {
   GemmEpilogue ep; ep.permP = permP; ep.permQ = permQ; ep.tag = tag;
-  const int s = splits_simt(cout, K, M);
+  const int s = simt_splits(cout, K, M, kScratchFloats, 128);
   if (col_u8)
     return gemm_simt<float, uint8_t, true, false>(dY, static_cast<const uint8_t*>(col), dW, cout, K, M, cout, ldk, K, ep, s, scratch, st);
   return gemm_simt<float, float, true, false>(dY, static_cast<const float*>(col), dW, cout, K, M, cout, ldk, K, ep, s, scratch, st);
@@ -317,8 +301,8 @@ struct Impl {
       LstmParams lp;
       lp.w_ih[0] = P + pp.lstm[0]; lp.w_hh[0] = P + pp.lstm[1]; lp.b_ih[0] = P + pp.lstm[2]; lp.b_hh[0] = P + pp.lstm[3];
       lp.w_ih[1] = lp.w_hh[1] = lp.b_ih[1] = lp.b_hh[1] = nullptr;
-      TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core_in, kLstmH, 1, w.lstm, w.core_out, hN, cN, w.splitk,
-                          kBf16 ? 1 : 0, st));
+      TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core_in, kLstmH, 1, w.lstm, w.core_out, hN, cN, kBf16 ? 1 : 0,
+                          st));
     }
     TB_TRY(heads_forward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N,
                          pp.core_out, A, policy_logits, baseline, st));
@@ -472,7 +456,7 @@ struct SplitImpl {
       LstmParams lp;
       lp.w_ih[0] = P + pp.lstm[0]; lp.w_hh[0] = P + pp.lstm[1]; lp.b_ih[0] = P + pp.lstm[2]; lp.b_hh[0] = P + pp.lstm[3];
       lp.w_ih[1] = lp.w_hh[1] = lp.b_ih[1] = lp.b_hh[1] = nullptr;
-      TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core_in, kLstmH, 1, w.lstm, w.core_out, hN, cN, w.splitk, 2, st));
+      TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core_in, kLstmH, 1, w.lstm, w.core_out, hN, cN, 2, st));
     }
     TB_TRY(heads_forward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N,
                          pp.core_out, A, policy_logits, baseline, st));

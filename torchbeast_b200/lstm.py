@@ -12,6 +12,8 @@ from torch import nn
 from torchbeast_b200 import _lib
 
 PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
+# recurrence kinds, numbered as TB_LSTM_* in include/torchbeast_b200.h
+KINDS = ("step", "persistent", "persistent_mma", "cluster", "wave_bf16", "wave_split")
 
 
 class LSTM(nn.Module):
@@ -38,6 +40,13 @@ class LSTM(nn.Module):
         if self._ws is None or self._ws.numel() < n or self._ws.device != self.weight_ih_l0.device:
             self._ws = torch.empty(n, dtype=torch.uint8, device=self.weight_ih_l0.device)
         return self._ws
+
+    def plan(self, B):
+        """(forward kind, backward kind): the recurrence implementations a batch of B runs on the current device."""
+        fwd, bwd = ctypes.c_int(), ctypes.c_int()
+        _lib.check(_lib.lib().tb_lstm_plan(B, self.input_size, self.hidden_size, self.num_layers, PRECISIONS[self.precision],
+                                           ctypes.byref(fwd), ctypes.byref(bwd)), "tb_lstm_plan")
+        return KINDS[fwd.value], KINDS[bwd.value]
 
     @staticmethod
     def _ptr_array(tensors):
