@@ -208,6 +208,16 @@ int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const
 int tb_lstm_backward(const float* dy, const float* x, const float* notdone, const float* const* params, float* const* grads,
                      int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision, void* workspace,
                      float* dx, void* stream);
+/* tb_lstm_backward with the gradients at both ends of the recurrence, each [layers, B, H] and each optional (NULL):
+ *   dhN, dcN (in):  dL/dhN and dL/dcN, the gradients arriving at the final state the forward returned (a loss on hN / cN,
+ *                   or the next unroll of a truncated-BPTT chain);
+ *   dh0, dc0 (out): dL/dh0 and dL/dc0 with respect to the h0 / c0 the forward was given.  Step 0 applies
+ *                   state *= notdone_0 first, so both include that mask: a column with notdone_0 = 0 gets exact zeros.
+ * dy stays read-only.  With all four NULL this is tb_lstm_backward: the same kernels and bit-identical outputs.       */
+int tb_lstm_backward_state(const float* dy, const float* x, const float* notdone, const float* const* params,
+                           float* const* grads, int64_t T1, int64_t B, int input_size, int hidden_size, int layers,
+                           int precision, void* workspace, float* dx, const float* dhN, const float* dcN, float* dh0,
+                           float* dc0, void* stream);
 
 /* ---- IMPALA ResNet (polybeast_learner.py:134-266 `Net`) forward / backward ------------------------- */
 

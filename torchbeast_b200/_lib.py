@@ -70,6 +70,7 @@ _SIGNATURES = {
     "tb_lstm_plan": ([_i64, _int, _int, _int, _int, _vp, _vp], _int),
     "tb_lstm_forward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 5, _int),
     "tb_lstm_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 3, _int),
+    "tb_lstm_backward_state": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
     "tb_atarinet_backward_phase": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _int, _vp], _int),
 }
 

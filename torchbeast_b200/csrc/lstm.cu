@@ -275,6 +275,18 @@ __global__ void lstm_init_state_kernel(const float* __restrict__ h0, const float
   }
 }
 
+// Layer l's [B, H] slices of the state-gradient ports (null where the port is null), for the per-layer backward recurrences:
+// dhN / dcN are added to dh / seed the cell carry at t = T1-1, dc0 receives the carry step 0 produces.
+struct LayerStatePorts {
+  const float* dhN = nullptr; const float* dcN = nullptr; float* dc0 = nullptr;
+  LayerStatePorts(const LstmStateGrads& sg, int l, int64_t B, int H) {
+    const int64_t o = int64_t(l) * B * H;
+    if (sg.dhN) dhN = sg.dhN + o;
+    if (sg.dcN) dcN = sg.dcN + o;
+    if (sg.dc0) dc0 = sg.dc0 + o;
+  }
+};
+
 // ---------------------------------------------------------------------------------------
 // backward step, pointwise part: dgates_t (pre-activation) and the cell-state carry.
 //   dh = dy_t + dh_raw * nd_next   (dh_raw = dgates_{t+1} . W_hh, masked by notdone_{t+1})
@@ -286,7 +298,8 @@ struct BwdPointArgs {
   float* dc;                                                   // [B,H] carry in/out (dL/dc_t in, dL/dc_{t-1} out)
   float* dgates;                                               // [B,4H]
   float* dgp; int Hp;                                          // [4,B,Hp] gate-major padded copy
-  int B, H; int first;                                         // first != 0: carries are zero (t = T1-1)
+  int B, H; int first;                                         // first != 0: t = T1-1, no carries from t+1
+  const float* dhN; const float* dcN;                          // [B,H] or null: what enters at t = T1-1 (read when first)
 };
 
 __global__ void lstm_step_bwd_point_kernel(BwdPointArgs a) {
@@ -301,6 +314,9 @@ __global__ void lstm_step_bwd_point_kernel(BwdPointArgs a) {
   if (!a.first) {
     dh += a.dh_raw[i] * a.nd_next[b];
     dc = a.dc[i];
+  } else {
+    if (a.dhN) dh += a.dhN[i];
+    if (a.dcN) dc = a.dcN[i];
   }
   const float tc = tanhf(a.cs[i]);
   const float d_o = dh * tc;
@@ -593,6 +609,7 @@ struct PersistBwdArgs {
   float* dgates; float* dgp;
   unsigned* counter;
   int T1, B, H, Hp; unsigned nctas;
+  const float* dhN; const float* dcN; float* dc0;  // [B,H] or null (LayerStatePorts)
 };
 
 __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_kernel(PersistBwdArgs a) {
@@ -638,6 +655,9 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_kernel(Persi
       if (it > 0) {
         dh += dh_s[q][lane] * a.nd[row0 + B + lane];
         dc = dc_s[q][lane];
+      } else {
+        if (a.dhN) dh += a.dhN[int64_t(lane) * H + j];
+        if (a.dcN) dc = a.dcN[int64_t(lane) * H + j];
       }
       const float tc = tanhf(a.cs[i]);
       const float d_o = dh * tc;
@@ -651,7 +671,10 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_kernel(Persi
       dc_s[q][lane] = dc * fg * a.nd[row0 + lane];
     }
     if (t == 0) {  // uniform: no earlier step needs dh
-      if (actA) { a.dgates[g0] = p_i; a.dgates[g0 + H] = p_f; a.dgates[g0 + 2 * H] = p_g; a.dgates[g0 + 3 * H] = p_o; }
+      if (actA) {
+        a.dgates[g0] = p_i; a.dgates[g0 + H] = p_f; a.dgates[g0 + 2 * H] = p_g; a.dgates[g0 + 3 * H] = p_o;
+        if (a.dc0) a.dc0[int64_t(lane) * H + k0 + q] = dc_s[q][lane];  // this thread's own carry
+      }
       break;
     }
     __syncthreads();
@@ -794,7 +817,7 @@ static int lstm_fwd_persistent(const LstmLayerWs& L, float* hs, const float* not
 }
 
 static int lstm_bwd_persistent(const LstmLayerWs& L, const LstmWs& ws, const float* dy, const float* notdone, int64_t T1,
-                               int64_t B, int H, unsigned* counter, cudaStream_t st) {
+                               int64_t B, int H, unsigned* counter, const LayerStatePorts& sp, cudaStream_t st) {
   const Launch l = persistent_bwd_launch(H, st);
   const int Hp = padded_h(H);
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
@@ -803,6 +826,7 @@ static int lstm_bwd_persistent(const LstmLayerWs& L, const LstmWs& ws, const flo
   PersistBwdArgs a;
   a.wtp = L.w_hh_t; a.dy = dy; a.nd = notdone; a.gates = L.gates; a.cs = L.cs; a.cm = L.cm; a.dgates = L.dgates;
   a.dgp = ws.dgp; a.counter = counter; a.T1 = int(T1); a.B = int(B); a.H = H; a.Hp = Hp; a.nctas = l.cfg.gridDim.x;
+  a.dhN = sp.dhN; a.dcN = sp.dcN; a.dc0 = sp.dc0;
   return launch(l, "lstm_bwd_persistent_kernel", lstm_bwd_persistent_kernel, a);
 }
 
@@ -828,12 +852,13 @@ static int lstm_fwd_steps(const LstmLayerWs& L, float* hs, const float* notdone,
 }
 
 static int lstm_bwd_steps(const LstmLayerWs& L, const LstmWs& ws, const float* dy, const float* notdone, int64_t T1,
-                          int64_t B, int H, cudaStream_t st) {
+                          int64_t B, int H, const LayerStatePorts& sp, cudaStream_t st) {
   const int Hp = padded_h(H);
   for (int64_t t = T1 - 1; t >= 0; --t) {
     BwdPointArgs a;
     a.dy = dy + t * B * H;
     a.first = (t == T1 - 1);
+    a.dhN = sp.dhN; a.dcN = sp.dcN;
     a.dh_raw = ws.dh; a.nd_next = a.first ? nullptr : notdone + (t + 1) * B;
     a.nd = notdone + t * B;
     a.gates = L.gates + t * B * 4 * H; a.cs = L.cs + t * B * H; a.cm = L.cm + t * B * H;
@@ -847,6 +872,10 @@ static int lstm_bwd_steps(const LstmLayerWs& L, const LstmWs& ws, const float* d
       d.dgp = ws.dgp; d.wtp = L.w_hh_t; d.dh_raw = ws.dh; d.B = int(B); d.H = H; d.Hp = Hp;
       TB_TRY(launch_step_bwd_dh(d, st));
     }
+  }
+  if (sp.dc0) {  // the carry step 0 left: notdone_0 * f_0 * dc_0
+    const cudaError_t e = cudaMemcpyAsync(sp.dc0, ws.dc, sizeof(float) * B * H, cudaMemcpyDeviceToDevice, st);
+    TB_REQUIRE(e == cudaSuccess, "lstm: dc0 copy: %s", cudaGetErrorString(e));
   }
   return 0;
 }
@@ -1218,6 +1247,7 @@ struct PersistBwdMmaArgs {
   __nv_bfloat16* dgq;                  // dgq: [2][4, B, Hq]
   unsigned* counter;
   int T1, B, H, Hq; unsigned nctas;
+  const float* dhN; const float* dcN; float* dc0;  // [B,H] or null (LayerStatePorts)
 };
 
 constexpr int kMaxKStepsBwd = 12;  // ceil(4*ceil(H/16) / 16) upper bound (H <= 768)
@@ -1298,6 +1328,9 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_mma_kernel(P
       if (it > 0) {
         dh += dh_s[q][lane] * n_ndn;
         dc = dc_s[q][lane];
+      } else {
+        if (a.dhN) dh += a.dhN[int64_t(lane) * H + k0 + q];
+        if (a.dcN) dc = a.dcN[int64_t(lane) * H + k0 + q];
       }
       const float tc = tanhf(n_cs);
       const float d_o = dh * tc;
@@ -1305,7 +1338,9 @@ __global__ void __launch_bounds__(kStepThreads) lstm_bwd_persistent_mma_kernel(P
       const float d_i = dc * gg, d_f = dc * n_cm, d_g = dc * ig;
       p_i = d_i * ig * (1.0f - ig); p_f = d_f * fg * (1.0f - fg);
       p_g = d_g * (1.0f - gg * gg); p_o = d_o * og * (1.0f - og);
-      dc_s[q][lane] = dc * fg * n_nd;
+      const float carry = dc * fg * n_nd;
+      dc_s[q][lane] = carry;
+      if (t == 0 && a.dc0) a.dc0[int64_t(lane) * H + k0 + q] = carry;
       bs_i += p_i; bs_f += p_f; bs_g += p_g; bs_o += p_o;
     }
     if (t == 0) {
@@ -1416,6 +1451,7 @@ struct WaveBwdArgs {
   float* dxm;                       // [T1*B, H] dL/d(lower output): written by the upper role, read by the lower
   unsigned* counter;
   int T1, B, H, Hq; unsigned nc;    // nc = CTAs per role
+  const float* dhN; const float* dcN; float* dc0;  // [2, B, H] or null: each role uses its layer's slice
 };
 
 __global__ void __launch_bounds__(kStepThreads) lstm2_bwd_wave_mma_kernel(WaveBwdArgs a) {
@@ -1511,9 +1547,13 @@ __global__ void __launch_bounds__(kStepThreads) lstm2_bwd_wave_mma_kernel(WaveBw
         const float ig = n_ig, fg = n_fg, gg = n_gg, og = n_og;
         float dh = n_dy;
         float dc = 0.0f;
+        const int64_t si = (upper ? int64_t(B) * H : 0) + int64_t(lane) * H + k0 + q;   // this role's layer in [2, B, H]
         if (it > 0) {
           dh += dh_s[q][lane] * n_ndn;
           dc = dc_s[q][lane];
+        } else {
+          if (a.dhN) dh += a.dhN[si];
+          if (a.dcN) dc = a.dcN[si];
         }
         const float tc = tanhf(n_cs);
         const float d_o = dh * tc;
@@ -1521,7 +1561,9 @@ __global__ void __launch_bounds__(kStepThreads) lstm2_bwd_wave_mma_kernel(WaveBw
         const float d_i = dc * gg, d_f = dc * n_cm, d_g = dc * ig;
         p_i = d_i * ig * (1.0f - ig); p_f = d_f * fg * (1.0f - fg);
         p_g = d_g * (1.0f - gg * gg); p_o = d_o * og * (1.0f - og);
-        dc_s[q][lane] = dc * fg * n_nd;
+        const float carry = dc * fg * n_nd;
+        dc_s[q][lane] = carry;
+        if (t == 0 && a.dc0) a.dc0[si] = carry;
         bs_i += p_i; bs_f += p_f; bs_g += p_g; bs_o += p_o;
       }
       // publish this CTA's 8 columns of the four gate-gradient tiles (16-byte stores staged through smem)
@@ -2062,6 +2104,7 @@ struct WaveBwdSplitArgs {
   int T1, B, H, Hq;
   unsigned nc;                      // CTAs per role, padded to whole clusters
   unsigned ncol;                    // CTAs per role that own columns < H (= ceil(H / 8))
+  const float* dhN; const float* dcN; float* dc0;  // [2, B, H] or null: each role uses its layer's slice
 };
 
 // dgq_map[role]: that role's exchange planes as a rank-5 map {Hq, B, gate, ping-pong buffer, plane}, box
@@ -2209,9 +2252,13 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         const float n_ndn = (t + 1 < a.T1) ? pre_s[1824 + lane] : 0.f;
         float dh = upper ? pre_s[1536 + lane * 8 + q] : n_dy;
         float dc = 0.0f;
+        const int64_t si = (upper ? int64_t(B) * H : 0) + int64_t(lane) * H + k0 + q;   // this role's layer in [2, B, H]
         if (it > 0) {
           dh += dh_s[q][lane] * n_ndn;
           dc = dc_s[q][lane];
+        } else {
+          if (a.dhN) dh += a.dhN[si];
+          if (a.dcN) dc = a.dcN[si];
         }
         const float tc = tanhf(n_cs);
         const float d_o = dh * tc;
@@ -2219,7 +2266,9 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         const float d_i = dc * gg, d_f = dc * n_cm, d_g = dc * ig;
         p_i = d_i * ig * (1.0f - ig); p_f = d_f * fg * (1.0f - fg);
         p_g = d_g * (1.0f - gg * gg); p_o = d_o * og * (1.0f - og);
-        dc_s[q][lane] = dc * fg * n_nd;
+        const float carry = dc * fg * n_nd;
+        dc_s[q][lane] = carry;
+        if (t == 0 && a.dc0) a.dc0[si] = carry;
         bs_i += p_i; bs_f += p_f; bs_g += p_g; bs_o += p_o;
       }
       // publish this CTA's 8 columns of the four gate-gradient tiles, hi and lo planes (16-byte stores staged through smem)
@@ -2649,6 +2698,7 @@ static int lstm_fwd_cluster(const LstmLayerWs& L, const float* w_hh, float* hs, 
 struct ClusterBwdArgs {
   const float* w_hh; const float* dy; const float* nd; const float* gates; const float* cs; const float* cm; float* dgates;
   int T1, B;
+  const float* dhN; const float* dcN; float* dc0;  // [B,H] or null (LayerStatePorts)
 };
 
 template <int MT>
@@ -2712,6 +2762,9 @@ __global__ void __launch_bounds__(kClThreads, 1) lstm_bwd_cluster_kernel(Cluster
         for (int sidx = 0; sidx < kClN; ++sidx) rec += recv[buf][sidx][r][u];   // fixed order
         dh += rec * in_ndn[q];
         dc = dc_carry[q];
+      } else if (r < B) {
+        if (a.dhN) dh += a.dhN[int64_t(r) * H + ug];
+        if (a.dcN) dc = a.dcN[int64_t(r) * H + ug];
       }
       const float ig = in_g[q][0], fg = in_g[q][1], gg = in_g[q][2], og = in_g[q][3];
       const float tc = tanhf(in_cs[q]);
@@ -2722,6 +2775,7 @@ __global__ void __launch_bounds__(kClThreads, 1) lstm_bwd_cluster_kernel(Cluster
       pv[0] = d_i * ig * (1.0f - ig); pv[1] = d_f * fg * (1.0f - fg);
       pv[2] = d_g * (1.0f - gg * gg); pv[3] = d_o * og * (1.0f - og);
       dc_carry[q] = dc * fg * in_nd[q];
+      if (t == 0 && a.dc0 && r < B) a.dc0[int64_t(r) * H + ug] = dc_carry[q];
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
         const __nv_bfloat16 hh = __float2bfloat16_rn(pv[g]);
@@ -2775,10 +2829,11 @@ static size_t cluster_bwd_smem(int MT) {
 }
 
 static int lstm_bwd_cluster(const LstmLayerWs& L, const float* w_hh, const float* dy, const float* notdone, int64_t T1, int64_t B,
-                            cudaStream_t st) {
+                            const LayerStatePorts& sp, cudaStream_t st) {
   ClusterBwdArgs a;
   a.w_hh = w_hh; a.dy = dy; a.nd = notdone; a.gates = L.gates; a.cs = L.cs; a.cm = L.cm; a.dgates = L.dgates;
   a.T1 = int(T1); a.B = int(B);
+  a.dhN = sp.dhN; a.dcN = sp.dcN; a.dc0 = sp.dc0;
   const Launch l = cluster_launch(cluster_bwd_smem(B <= 16 ? 1 : 2), st);
   return B <= 16 ? launch(l, "lstm_bwd_cluster_kernel", lstm_bwd_cluster_kernel<1>, a)
                  : launch(l, "lstm_bwd_cluster_kernel", lstm_bwd_cluster_kernel<2>, a);
@@ -2797,7 +2852,8 @@ static bool cluster_bwd_fits(int64_t B, int H) {
 }
 
 static int lstm_bwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, const float* dy, const float* notdone,
-                                   int64_t T1, int64_t B, int H, float* db, unsigned* counter, cudaStream_t st) {
+                                   int64_t T1, int64_t B, int H, float* db, unsigned* counter, const LayerStatePorts& sp,
+                                   cudaStream_t st) {
   const int Hq = mma_hq(H);
   const Launch l = mma_bwd_launch(H, st);
   cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(unsigned), st);
@@ -2808,6 +2864,7 @@ static int lstm_bwd_persistent_mma(const LstmLayerWs& L, const float* w_hh, cons
   a.dgb = static_cast<__nv_bfloat16*>(L.dgb); a.lg = int(ld16(4 * H)); a.db = db;
   a.dgq = static_cast<__nv_bfloat16*>(L.dgq); a.counter = counter;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = l.cfg.gridDim.x;
+  a.dhN = sp.dhN; a.dcN = sp.dcN; a.dc0 = sp.dc0;
   return launch(l, "lstm_bwd_persistent_mma_kernel", lstm_bwd_persistent_mma_kernel, a);
 }
 
@@ -2823,7 +2880,7 @@ static bool wave_bwd_fits(int64_t B, int H) {
 // both layers' backward recurrences in one launch; leaves dgb / bias gradients of both layers and
 // ws.dx_mid = dL/d(lower layer output)
 static int lstm2_bwd_wave(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone, int64_t T1,
-                          int64_t B, int H, cudaStream_t st) {
+                          int64_t B, int H, const LstmStateGrads& sg, cudaStream_t st) {
   const int Hq = mma_hq(H);
   const unsigned nc = unsigned((H + kBwdCols - 1) / kBwdCols);
   const LstmLayerWs& U = ws.layer[1];
@@ -2843,11 +2900,12 @@ static int lstm2_bwd_wave(LstmWs& ws, const LstmParams& p, const LstmGrads& g, c
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq);
   a.dxm = ws.dx_mid; a.counter = counter;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc;
+  a.dhN = sg.dhN; a.dcN = sg.dcN; a.dc0 = sg.dc0;
   return launch(wave_bwd_launch(H, st), "lstm2_bwd_wave_mma_kernel", lstm2_bwd_wave_mma_kernel, a);
 }
 
 static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone,
-                                int64_t T1, int64_t B, int H, cudaStream_t st) {
+                                int64_t T1, int64_t B, int H, const LstmStateGrads& sg, cudaStream_t st) {
   const int Hq = mma_hq(H);
   const unsigned nc = wave_bwd_split_role_ctas(H);
   const LstmLayerWs& U = ws.layer[1];
@@ -2869,6 +2927,7 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq); a.dgq_lo_off = U.dgq_lo;
   a.dxb = ws.dxb; a.flags = flags;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc; a.ncol = unsigned((H + kBwdCols - 1) / kBwdCols);
+  a.dhN = sg.dhN; a.dcN = sg.dcN; a.dc0 = sg.dc0;
   CUtensorMap maps[2];
   for (int r = 0; r < 2; ++r) {
     const uint64_t dims[5] = {uint64_t(Hq), uint64_t(B), 4, 2, 2};
@@ -2877,6 +2936,81 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
     tcd::make_map_nd(&maps[r], r == 0 ? a.dgq_up : a.dgq_lo, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
   }
   return launch(wave_bwd_split_launch(H, st), "lstm2_bwd_wave_split_kernel", lstm2_bwd_wave_split_kernel, maps[0], maps[1], a);
+}
+
+// ---- dL/dh0 of one layer, after its backward recurrence --------------------------------------------------------------
+// dh0[b, k] = notdone_0[b] * sum_r dgates_0[b, r] * W_hh[r, k]: the recurrent product the recurrences skip at t = 0, on the
+// step-0 rows of the gate gradients they leave for the weight-gradient GEMMs - fp32 (dg32), or bf16 (dgb, row stride lg)
+// plus, at split-bf16, its lo plane at dgb + dgb_lo (hi + lo are summed in fp32, so the product is fp32-grade).  A CTA owns
+// 32 columns x kDh0Rows batch rows; warp w takes the reduction indices [32w, 32w + 32) of every 256-wide chunk, and the
+// eight partial sums meet in shared memory in a fixed order.
+constexpr int kDh0Rows = 8, kDh0Chunk = 256;
+static_assert(kDh0Rows == 8, "the final sum maps one batch row to each of the 8 warps");
+
+struct Dh0Args {
+  const float* w_hh; const float* nd;
+  const float* dg32; const __nv_bfloat16* dgb; int64_t dgb_lo; int lg;
+  float* dh0;
+  int B, H;
+};
+
+__global__ void __launch_bounds__(256) lstm_dh0_kernel(Dh0Args a) {
+  __shared__ float dg_s[kDh0Rows][kDh0Chunk];
+  __shared__ float part_s[8][kDh0Rows][33];
+  const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
+  const int H = a.H, K = 4 * H;
+  const int k = blockIdx.x * 32 + lane, b0 = blockIdx.y * kDh0Rows;
+  float acc[kDh0Rows];
+#pragma unroll
+  for (int q = 0; q < kDh0Rows; ++q) acc[q] = 0.f;
+  for (int c0 = 0; c0 < K; c0 += kDh0Chunk) {
+    for (int i = tid; i < kDh0Rows * kDh0Chunk; i += 256) {
+      const int rr = i / kDh0Chunk, cc = i % kDh0Chunk, b = b0 + rr, r = c0 + cc;
+      float v = 0.f;
+      if (b < a.B && r < K) {
+        if (a.dg32) {
+          v = a.dg32[int64_t(b) * K + r];
+        } else {
+          const int64_t o = int64_t(b) * a.lg + r;
+          v = __bfloat162float(a.dgb[o]);
+          if (a.dgb_lo) v += __bfloat162float(a.dgb[a.dgb_lo + o]);
+        }
+      }
+      dg_s[rr][cc] = v;
+    }
+    __syncthreads();
+    if (k < H) {
+#pragma unroll 8
+      for (int cc = wrp * 32; cc < wrp * 32 + 32; ++cc) {
+        const int r = c0 + cc;
+        const float w = r < K ? __ldg(a.w_hh + int64_t(r) * H + k) : 0.f;
+#pragma unroll
+        for (int q = 0; q < kDh0Rows; ++q) acc[q] = fmaf(dg_s[q][cc], w, acc[q]);
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int q = 0; q < kDh0Rows; ++q) part_s[wrp][q][lane] = acc[q];
+  __syncthreads();
+  const int b = b0 + wrp;   // thread = (batch row b0 + wrp, column k)
+  if (k < H && b < a.B) {
+    float d = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) d += part_s[w][wrp][lane];
+    a.dh0[int64_t(b) * H + k] = d * a.nd[b];
+  }
+}
+
+static int lstm_dh0(const LstmLayerWs& L, const float* w_hh, const float* notdone, bool dg_done, int64_t B, int H, float* dh0,
+                    cudaStream_t st) {
+  Dh0Args a;
+  a.w_hh = w_hh; a.nd = notdone;
+  a.dg32 = dg_done ? nullptr : L.dgates;
+  a.dgb = static_cast<const __nv_bfloat16*>(L.dgb); a.dgb_lo = L.dgb_lo; a.lg = int(ld16(4 * H));
+  a.dh0 = dh0; a.B = int(B); a.H = H;
+  lstm_dh0_kernel<<<dim3((H + 31) / 32, unsigned((B + kDh0Rows - 1) / kDh0Rows)), 256, 0, st>>>(a);
+  return check_launch("lstm_dh0_kernel");
 }
 
 // Side stream for work that can run beside a recurrence kernel (which occupies only H/8 = 65 of the 132 SMs):
@@ -3117,7 +3251,7 @@ int lstm_backward_join(cudaStream_t st) {
 
 int lstm_backward(const float* dy, const float* x, const float* notdone, const LstmParams& p, const LstmGrads& g,
                   int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* dx, float* splitk,
-                  float* colsum_scratch, int precision, cudaStream_t st) {
+                  float* colsum_scratch, int precision, cudaStream_t st, const LstmStateGrads& sg) {
   const LstmPlan plan = lstm_plan(B, In, H, layers, precision);
   const int64_t N = T1 * B;
   const int Hp = padded_h(H);
@@ -3127,8 +3261,8 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
     // GEMMs and the lower layer's dx remain per layer.  (The 4 padding columns of the split kernel's [N, ld16(4H)] gate
     // gradient planes are never read as data: the GEMMs' tensor maps end at column 4H.)
     ProfScope prof("lstm_recurrence_bwd", st);
-    TB_TRY(plan.bwd == kLstmWaveSplit ? lstm2_bwd_wave_split(ws, p, g, dy, notdone, T1, B, H, st)
-                                      : lstm2_bwd_wave(ws, p, g, dy, notdone, T1, B, H, st));
+    TB_TRY(plan.bwd == kLstmWaveSplit ? lstm2_bwd_wave_split(ws, p, g, dy, notdone, T1, B, H, sg, st)
+                                      : lstm2_bwd_wave(ws, p, g, dy, notdone, T1, B, H, sg, st));
   }
   // The weight-gradient GEMMs feed nothing downstream in this backward pass: see LstmWgrad for where they run.  Without a
   // side stream they run on the caller's.
@@ -3152,14 +3286,15 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
     }
     if (!wave) {
       ProfScope prof("lstm_recurrence_bwd", st);
+      const LayerStatePorts sp(sg, l, B, H);
       if (plan.bwd == kLstmPersistentMma)
-        TB_TRY(lstm_bwd_persistent_mma(L, p.w_hh[l], dyl, notdone, T1, B, H, g.b_ih[l], ws.sync + 16, st));
+        TB_TRY(lstm_bwd_persistent_mma(L, p.w_hh[l], dyl, notdone, T1, B, H, g.b_ih[l], ws.sync + 16, sp, st));
       else if (plan.bwd == kLstmCluster)
-        TB_TRY(lstm_bwd_cluster(L, p.w_hh[l], dyl, notdone, T1, B, st));
+        TB_TRY(lstm_bwd_cluster(L, p.w_hh[l], dyl, notdone, T1, B, sp, st));
       else if (plan.bwd == kLstmPersistent)
-        TB_TRY(lstm_bwd_persistent(L, ws, dyl, notdone, T1, B, H, ws.sync + 16, st));
+        TB_TRY(lstm_bwd_persistent(L, ws, dyl, notdone, T1, B, H, ws.sync + 16, sp, st));
       else
-        TB_TRY(lstm_bwd_steps(L, ws, dyl, notdone, T1, B, H, st));
+        TB_TRY(lstm_bwd_steps(L, ws, dyl, notdone, T1, B, H, sp, st));
     }
     // parameter gradients over all steps at once
     if (precision) {
@@ -3223,6 +3358,10 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
                                                      nullptr, st)));
     }
     dyl = dxl;
+  }
+  if (sg.dh0) {
+    for (int l = 0; l < layers; ++l)
+      TB_TRY(lstm_dh0(ws.layer[l], p.w_hh[l], notdone, plan.dg_done, B, H, sg.dh0 + int64_t(l) * B * H, st));
   }
   if (side && plan.wgrad == kWgradTail) {
     TB_TRY(side->join());
@@ -3303,8 +3442,18 @@ int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const
 int tb_lstm_backward(const float* dy, const float* x, const float* notdone, const float* const* params, float* const* grads,
                      int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision, void* workspace,
                      float* dx, void* stream) {
+  return tb_lstm_backward_state(dy, x, notdone, params, grads, T1, B, input_size, hidden_size, layers, precision, workspace,
+                                dx, nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+int tb_lstm_backward_state(const float* dy, const float* x, const float* notdone, const float* const* params,
+                           float* const* grads, int64_t T1, int64_t B, int input_size, int hidden_size, int layers,
+                           int precision, void* workspace, float* dx, const float* dhN, const float* dcN, float* dh0,
+                           float* dc0, void* stream) {
   if (lstm_abi_check(T1, B, input_size, hidden_size, layers, precision)) return 1;
   TB_REQUIRE(dy && x && notdone && params && grads && workspace && dx, "tb_lstm_backward: null pointer");
+  LstmStateGrads sg;
+  sg.dhN = dhN; sg.dcN = dcN; sg.dh0 = dh0; sg.dc0 = dc0;
   LstmParams p; LstmGrads g;
   for (int l = 0; l < layers; ++l) {
     p.w_ih[l] = params[4 * l]; p.w_hh[l] = params[4 * l + 1]; p.b_ih[l] = params[4 * l + 2]; p.b_hh[l] = params[4 * l + 3];
@@ -3313,7 +3462,7 @@ int tb_lstm_backward(const float* dy, const float* x, const float* notdone, cons
   }
   LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
   int rc = lstm_backward(dy, x, notdone, p, g, T1, B, input_size, hidden_size, layers, w.ws, dx, w.splitk, w.colsum, precision,
-                         (cudaStream_t)stream);
+                         (cudaStream_t)stream, sg);
   if (rc) return rc;
   return lstm_backward_join((cudaStream_t)stream);
 }

@@ -70,6 +70,15 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
                  int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* y, float* hN, float* cN,
                  int precision, cudaStream_t stream);
 
+// Gradients at the two ends of the recurrence, each [layers, B, H] and each optional (null: not given / not wanted).
+// dhN / dcN arrive at the final state and enter every layer's backward recurrence at t = T1-1; dh0 / dc0 are the gradients
+// with respect to the h0 / c0 the forward was given, so they include the notdone_0 mask (a column that starts an episode at
+// t = 0 gets zeros).  All null: lstm_backward runs exactly the kernels, and computes exactly the values, it runs without them.
+struct LstmStateGrads {
+  const float* dhN = nullptr; const float* dcN = nullptr;
+  float* dh0 = nullptr; float* dc0 = nullptr;
+};
+
 // dy [T1*B, H] -> dx [T1*B, In]; parameter gradients written (overwritten) into g.  splitk: GEMM scratch
 // (kSplitKScratchFloats).
 // Joins the side stream lstm_backward may have forked (weight-gradient GEMMs overlapping the caller's own backward):
@@ -78,6 +87,6 @@ int lstm_backward_join(cudaStream_t stream);
 
 int lstm_backward(const float* dy, const float* x, const float* notdone, const LstmParams& p, const LstmGrads& g,
                   int64_t T1, int64_t B, int In, int H, int layers, LstmWs& ws, float* dx, float* splitk,
-                  float* colsum_scratch, int precision, cudaStream_t stream);
+                  float* colsum_scratch, int precision, cudaStream_t stream, const LstmStateGrads& sg = LstmStateGrads());
 
 }  // namespace tb

@@ -3,17 +3,62 @@
 The recurrence the reference spells as a Python loop of seq_len-1 `nn.LSTM` calls (monobeast.py:603-611,
 polybeast_learner.py:241-249), with hidden size / layers / batch / unroll as free parameters - BASELINE.json configs[4]
 stresses it at T=600, B=128, H=512.  `LSTM` keeps torch.nn.LSTM's parameter names and shapes, so
-`lstm.load_state_dict(torch_lstm.state_dict())` works."""
+`lstm.load_state_dict(torch_lstm.state_dict())` works, and `lstm(input, (h0, c0))` is an autograd forward with
+torch.nn.LSTM's sequence-first shapes plus an optional done-reset mask."""
 import ctypes
 
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
 
 from torchbeast_b200 import _lib
 
 PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 # recurrence kinds, numbered as TB_LSTM_* in include/torchbeast_b200.h
 KINDS = ("step", "persistent", "persistent_mma", "cluster", "wave_bf16", "wave_split")
+
+
+class _LSTMFunction(torch.autograd.Function):
+    """One unroll through tb_lstm_forward, backpropagated by tb_lstm_backward_state.  Each call allocates its own workspace
+    and keeps it, with its inputs and parameters, in ctx: forwards may be backpropagated in any order, and a chain of
+    unrolls whose states feed each other (truncated BPTT) backpropagates through all of them."""
+
+    @staticmethod
+    def forward(ctx, module, x, notdone, h0, c0, *params):
+        T1, B = x.shape[:2]
+        H, L, prec = module.hidden_size, module.num_layers, PRECISIONS[module.precision]
+        x, notdone = x.float().contiguous(), notdone.float().contiguous()
+        h0, c0 = h0.float().contiguous(), c0.float().contiguous()
+        params = [q.float().contiguous() for q in params]
+        ws = torch.empty(_lib.lib().tb_lstm_workspace_bytes(T1, B, module.input_size, H, L, prec), dtype=torch.uint8,
+                         device=x.device)
+        y = torch.empty(T1, B, H, device=x.device)
+        hN, cN = torch.empty(L, B, H, device=x.device), torch.empty(L, B, H, device=x.device)
+        p, arr = _lib.ptr, lambda ts: ctypes.cast(LSTM._ptr_array(ts), ctypes.c_void_p)
+        _lib.check(_lib.lib().tb_lstm_forward(p(x), p(notdone), p(h0), p(c0), arr(params), T1, B, module.input_size, H, L,
+                                              prec, p(ws), p(y), p(hN), p(cN), _lib.stream_ptr()), "tb_lstm_forward")
+        ctx.save_for_backward(x, notdone, ws, *params)
+        ctx.dims = (T1, B, module.input_size, H, L, prec)
+        ctx.set_materialize_grads(False)
+        return y, hN, cN
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy, dhN, dcN):
+        x, notdone, ws, *params = ctx.saved_tensors
+        T1, B, In, H, L, prec = ctx.dims
+        dy = torch.zeros(T1, B, H, device=x.device) if dy is None else dy.float().contiguous()
+        dhN = None if dhN is None else dhN.float().contiguous()
+        dcN = None if dcN is None else dcN.float().contiguous()
+        dx = torch.empty_like(x)
+        grads = [torch.empty_like(q) for q in params]
+        dh0 = torch.empty(L, B, H, device=x.device) if ctx.needs_input_grad[3] else None
+        dc0 = torch.empty(L, B, H, device=x.device) if ctx.needs_input_grad[4] else None
+        p, arr = _lib.ptr, lambda ts: ctypes.cast(LSTM._ptr_array(ts), ctypes.c_void_p)
+        _lib.check(_lib.lib().tb_lstm_backward_state(p(dy), p(x), p(notdone), arr(params), arr(grads), T1, B, In, H, L, prec,
+                                                     p(ws), p(dx), p(dhN), p(dcN), p(dh0), p(dc0), _lib.stream_ptr()),
+                   "tb_lstm_backward_state")
+        return (None, dx, None, dh0, dc0, *grads)
 
 
 class LSTM(nn.Module):
@@ -52,6 +97,26 @@ class LSTM(nn.Module):
     def _ptr_array(tensors):
         arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
         return arr
+
+    def forward(self, input, hx=None, notdone=None):
+        """input [T, B, In], hx = (h0, c0) each [layers, B, H] (None: zeros), notdone [T, B] (None: no reset) ->
+        output [T, B, H], (h_n, c_n) each [layers, B, H].  Step t first multiplies the state by notdone[t]; without
+        notdone this is torch.nn.LSTM.  Differentiable with respect to input, h0, c0 and every parameter (once)."""
+        if input.dim() != 3 or input.shape[2] != self.input_size:
+            raise _lib.TorchBeastB200Error("LSTM: input must be [T, B, %d], got %s" % (self.input_size, tuple(input.shape)))
+        T, B = input.shape[:2]
+        state_shape = (self.num_layers, B, self.hidden_size)
+        if hx is not None and (len(hx) != 2 or any(tuple(s.shape) != state_shape for s in hx)):
+            raise _lib.TorchBeastB200Error("LSTM: hx must be (h0, c0), each %s" % (state_shape,))
+        if notdone is not None and tuple(notdone.shape) != (T, B):
+            raise _lib.TorchBeastB200Error("LSTM: notdone must be [%d, %d], got %s" % (T, B, tuple(notdone.shape)))
+        _lib.require_cuda(input, notdone, *(hx or ()))
+        if hx is None:
+            hx = (torch.zeros(state_shape, device=input.device), torch.zeros(state_shape, device=input.device))
+        if notdone is None:
+            notdone = torch.ones(T, B, device=input.device)
+        y, hN, cN = _LSTMFunction.apply(self, input, notdone, hx[0], hx[1], *self._plist())
+        return y, (hN, cN)
 
     @torch.no_grad()
     def forward_unroll(self, x, notdone, state):
