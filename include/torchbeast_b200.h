@@ -186,14 +186,19 @@ int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_basel
  * Replaces the reference's loop of seq_len-1 nn.LSTM calls and its autograd graph (monobeast.py:603-611,
  * polybeast_learner.py:241-249):   for t: state *= notdone_t;  y_t, state = LSTM(x_t, state).
  * torch.nn.LSTM conventions: params[4*l + {0,1,2,3}] = weight_ih_l [4H, In|H], weight_hh_l [4H, H], bias_ih_l [4H],
- * bias_hh_l [4H] (gate order i, f, g, o); 1 or 2 layers; hidden size, input size, batch and unroll are free
+ * bias_hh_l [4H] (gate order i, f, g, o); any number of layers >= 1; hidden size, input size, batch and unroll are free
  * (BASELINE configs[4]: T = 600, B = 128, H = 512).  x [T1*B, In], notdone [T1*B] (float 0/1), h0/c0/hN/cN [layers, B, H],
  * y [T1*B, H].  precision 0 = fp32 everywhere (any shape); 1 / 2 = bf16 / split-bf16 tensor-core products for the hoisted
  * projections, and in the recurrence where a tensor-core recurrence fits the shape (tb_lstm_plan).  tb_lstm_backward must
- * follow tb_lstm_forward on the same workspace; grads[] mirrors params[] and is overwritten; dx [T1*B, In].             */
+ * follow tb_lstm_forward on the same workspace; grads[] mirrors params[] and is overwritten; dx [T1*B, In].
+ * A stack runs as a chain of segments of two layers (layers 2k and 2k+1; the top segment is one layer when the depth is
+ * odd), each planned as a stack of its own with input width In for the first segment and H above it, so every upper
+ * pair can take a two-layer wavefront.  Every notdone step resets all layers.  Above two layers the workspace also holds
+ * each segment's output but the top one's and two [T1*B, H] buffers for the gradient handed between segments.        */
 size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision);
 /* The recurrence kinds tb_lstm_forward (*fwd_kind_host) and tb_lstm_backward (*bwd_kind_host) run for this shape on the
- * current device; host query, runs no kernel.  The choice does not depend on the unroll length.                       */
+ * current device; host query, runs no kernel.  The choice does not depend on the unroll length.  1 or 2 layers
+ * (one segment); tb_lstm_plan_layers reports any depth.                                                               */
 #define TB_LSTM_STEP 0            /* one step kernel per time step (any shape) */
 #define TB_LSTM_PERSISTENT 1      /* one cooperative fp32 kernel per layer */
 #define TB_LSTM_PERSISTENT_MMA 2  /* one cooperative kernel per layer, bf16 tensor-core products (precision 1) */
@@ -202,6 +207,10 @@ size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden
 #define TB_LSTM_WAVE_SPLIT 5      /* both layers in one wavefront kernel, split-bf16 products (precision 2) */
 int tb_lstm_plan(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kind_host,
                  int* bwd_kind_host);
+/* Per layer, for any depth: fwd_kinds_host[l] / bwd_kinds_host[l] (each an array of `layers` ints) get the kinds of the
+ * segment that runs layer l; both layers of a wavefront segment report its kind.  Host query, runs no kernel.          */
+int tb_lstm_plan_layers(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kinds_host,
+                        int* bwd_kinds_host);
 int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const float* c0, const float* const* params,
                     int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision, void* workspace,
                     float* y, float* hN, float* cN, void* stream);

@@ -68,6 +68,7 @@ _SIGNATURES = {
     "tb_host_write_rollout_column": ([_vp, _vp, _vp, _int, _i64, _i64, _i64, _vp], _int),
     "tb_lstm_workspace_bytes": ([_i64, _i64, _int, _int, _int, _int], _c.c_size_t),
     "tb_lstm_plan": ([_i64, _int, _int, _int, _int, _vp, _vp], _int),
+    "tb_lstm_plan_layers": ([_i64, _int, _int, _int, _int, _vp, _vp], _int),
     "tb_lstm_forward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 5, _int),
     "tb_lstm_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 3, _int),
     "tb_lstm_backward_state": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),

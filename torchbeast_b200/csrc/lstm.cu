@@ -10,7 +10,9 @@
 // The recurrence has six implementations, and lstm_plan (near the end of this file) picks one per
 // shape and direction: T+1 fused step kernels (any shape), one persistent cooperative kernel per
 // layer in fp32 or with bf16 tensor-core products, one 16-CTA cluster per layer (H = 256), and
-// two-layer wavefront kernels (bf16 or split-bf16) that run both layers in one launch.
+// two-layer wavefront kernels (bf16 or split-bf16) that run both layers in one launch.  lstm_forward /
+// lstm_backward take one or two layers; the C ABI at the end of this file runs deeper stacks as a chain of
+// two-layer segments (LstmChain).
 // torch.nn.LSTM conventions: gate order i,f,g,o; weight_ih [4H,In], weight_hh [4H,H]; two biases.
 #include "lstm.cuh"
 
@@ -3379,24 +3381,83 @@ int lstm_backward(const float* dy, const float* x, const float* notdone, const L
 using namespace tb;
 
 namespace {
-struct LstmAbiWs { LstmWs ws; float* splitk; float* colsum; size_t bytes; };
+// A stack of any depth runs as a chain of segments of at most kLstmMaxLayers (= 2) layers: segment k holds layers 2k and
+// 2k+1, and the last one a single layer when the depth is odd.  Each segment is one lstm_forward / lstm_backward call with
+// its own LstmParams, LstmWs and lstm_plan, so every segment above the first, whose input width is H, can take a two-layer
+// wavefront.  A stack of one or two layers is one segment: a single lstm_forward / lstm_backward call on the caller's
+// buffers.
+struct LstmChain {
+  int In, H, layers;
+  int segments() const { return (layers + kLstmMaxLayers - 1) / kLstmMaxLayers; }
+  int first(int k) const { return k * kLstmMaxLayers; }  // segment k's lowest layer
+  int depth(int k) const { return layers - first(k) < kLstmMaxLayers ? layers - first(k) : kLstmMaxLayers; }
+  int in(int k) const { return k ? H : In; }
+};
+
+// ABI workspace, 256-byte aligned pieces:
+//   LstmWs of segment 0, 1, ..., S-1   lstm_ws_bytes of each segment's shape
+//   mid   (S-1) x [T1*B, H] fp32       segment k's y (k < S-1): segment k+1's input, kept for that segment's backward
+//   dmid  2 x [T1*B, H] fp32           the backward's ping-pong: segment k's dx is segment k-1's dy      (mid, dmid: S > 1)
+//   split-K scratch                    kSplitKScratchFloats fp32, shared by every segment's GEMMs (see tb_lstm_backward_state)
+//   column-sum scratch
+// With one segment this is the single-call layout [LstmWs][split-K][column sums].
+struct LstmAbiWs {
+  LstmChain c;
+  int64_t T1, B;
+  int precision;
+  char* base;
+  float* mid = nullptr;
+  float* dmid[2] = {nullptr, nullptr};
+  float* splitk;
+  float* colsum;
+  size_t bytes;
+  size_t seg_bytes(int k) const { return (lstm_ws_bytes(T1, B, c.in(k), c.H, c.depth(k), precision) + 255) & ~size_t(255); }
+  LstmWs seg(int k) const {
+    size_t off = 0;
+    for (int j = 0; j < k; ++j) off += seg_bytes(j);
+    return lstm_ws(base ? base + off : nullptr, T1, B, c.in(k), c.H, c.depth(k), precision);
+  }
+  float* y(int k) const { return mid + int64_t(k) * T1 * B * c.H; }
+};
 
 LstmAbiWs lstm_abi_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int precision) {
   LstmAbiWs w;
-  const size_t lbytes = lstm_ws_bytes(T1, B, In, H, layers, precision);
-  size_t off = (lbytes + 255) & ~size_t(255);
-  w.ws = lstm_ws(base, T1, B, In, H, layers, precision);
-  w.splitk = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-  off += size_t(kSplitKScratchFloats) * sizeof(float);
-  w.colsum = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+  w.c = LstmChain{In, H, layers};
+  w.T1 = T1; w.B = B; w.precision = precision; w.base = static_cast<char*>(base);
+  const int S = w.c.segments();
+  size_t off = 0;
+  for (int k = 0; k < S; ++k) off += w.seg_bytes(k);
+  auto take = [&](size_t n_floats) {
+    float* p = base ? reinterpret_cast<float*>(w.base + off) : nullptr;
+    off += (n_floats * sizeof(float) + 255) & ~size_t(255);
+    return p;
+  };
+  if (S > 1) {
+    const size_t act = size_t(T1 * B) * H;
+    w.mid = take(act * (S - 1));
+    w.dmid[0] = take(act); w.dmid[1] = take(act);
+  }
+  w.splitk = take(size_t(kSplitKScratchFloats));
+  w.colsum = base ? reinterpret_cast<float*>(w.base + off) : nullptr;
   off += size_t(colsum_scratch_floats(4 * int64_t(H) > 512 ? 4 * int64_t(H) : 512)) * sizeof(float);
   w.bytes = off;
   return w;
 }
 
+// layers [first, first + depth) of the caller's params[] / grads[] (4 pointers per layer, torch.nn.LSTM's order)
+template <typename P, typename Ptr>
+P layer_slice(Ptr const* a, int first, int depth) {
+  P p;
+  for (int j = 0; j < depth; ++j) {
+    Ptr const* l = a + 4 * (first + j);
+    p.w_ih[j] = l[0]; p.w_hh[j] = l[1]; p.b_ih[j] = l[2]; p.b_hh[j] = l[3];
+  }
+  return p;
+}
+
 int lstm_abi_check(int64_t T1, int64_t B, int In, int H, int layers, int precision) {
   TB_REQUIRE(T1 >= 1 && B >= 1 && In >= 1 && H >= 1, "tb_lstm: bad sizes T1=%lld B=%lld In=%d H=%d", (long long)T1, (long long)B, In, H);
-  TB_REQUIRE(layers >= 1 && layers <= kLstmMaxLayers, "tb_lstm: 1..%d layers", kLstmMaxLayers);
+  TB_REQUIRE(layers >= 1, "tb_lstm: at least 1 layer, got %d", layers);
   TB_REQUIRE(precision >= 0 && precision <= 2, "tb_lstm: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
   return 0;
 }
@@ -3410,17 +3471,33 @@ int tb_set_aux_stream(void* stream) {
 }
 
 size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision) {
-  if (T1 < 1 || B < 1 || input_size < 1 || hidden_size < 1 || layers < 1 || layers > kLstmMaxLayers) return 0;
+  if (T1 < 1 || B < 1 || input_size < 1 || hidden_size < 1 || layers < 1) return 0;
   return lstm_abi_ws(nullptr, T1, B, input_size, hidden_size, layers, precision).bytes;
 }
 
 int tb_lstm_plan(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kind_host,
                  int* bwd_kind_host) {
   if (lstm_abi_check(1, B, input_size, hidden_size, layers, precision)) return 1;
+  TB_REQUIRE(layers <= kLstmMaxLayers, "tb_lstm_plan: 1..%d layers (tb_lstm_plan_layers takes any depth)", kLstmMaxLayers);
   TB_REQUIRE(fwd_kind_host && bwd_kind_host, "tb_lstm_plan: null pointer");
   const LstmPlan plan = lstm_plan(B, input_size, hidden_size, layers, precision);
   *fwd_kind_host = plan.fwd;
   *bwd_kind_host = plan.bwd;
+  return 0;
+}
+
+int tb_lstm_plan_layers(int64_t B, int input_size, int hidden_size, int layers, int precision, int* fwd_kinds_host,
+                        int* bwd_kinds_host) {
+  if (lstm_abi_check(1, B, input_size, hidden_size, layers, precision)) return 1;
+  TB_REQUIRE(fwd_kinds_host && bwd_kinds_host, "tb_lstm_plan_layers: null pointer");
+  const LstmChain c{input_size, hidden_size, layers};
+  for (int k = 0; k < c.segments(); ++k) {
+    const LstmPlan plan = lstm_plan(B, c.in(k), hidden_size, c.depth(k), precision);
+    for (int j = 0; j < c.depth(k); ++j) {
+      fwd_kinds_host[c.first(k) + j] = plan.fwd;
+      bwd_kinds_host[c.first(k) + j] = plan.bwd;
+    }
+  }
   return 0;
 }
 
@@ -3429,14 +3506,23 @@ int tb_lstm_forward(const float* x, const float* notdone, const float* h0, const
                     float* y, float* hN, float* cN, void* stream) {
   if (lstm_abi_check(T1, B, input_size, hidden_size, layers, precision)) return 1;
   TB_REQUIRE(x && notdone && h0 && c0 && params && workspace && y && hN && cN, "tb_lstm_forward: null pointer");
-  LstmParams p;
   for (int l = 0; l < layers; ++l) {
-    p.w_ih[l] = params[4 * l]; p.w_hh[l] = params[4 * l + 1]; p.b_ih[l] = params[4 * l + 2]; p.b_hh[l] = params[4 * l + 3];
-    TB_REQUIRE(p.w_ih[l] && p.w_hh[l] && p.b_ih[l] && p.b_hh[l], "tb_lstm_forward: null parameter pointer (layer %d)", l);
+    const float* const* q = params + 4 * l;
+    TB_REQUIRE(q[0] && q[1] && q[2] && q[3], "tb_lstm_forward: null parameter pointer (layer %d)", l);
   }
-  LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
-  return lstm_forward(x, notdone, h0, c0, p, T1, B, input_size, hidden_size, layers, w.ws, y, hN, cN, precision,
-                      (cudaStream_t)stream);
+  const LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
+  const LstmChain& c = w.c;
+  const int S = c.segments();
+  // Bottom-up: segment k reads segment k-1's y and the slices [first, first + depth) of h0 / c0, writes the same slices of
+  // hN / cN, and gets the whole notdone (a reset clears every layer's state).  The top segment writes the caller's y.
+  for (int k = 0; k < S; ++k) {
+    const int64_t s = int64_t(c.first(k)) * B * hidden_size;
+    const LstmParams p = layer_slice<LstmParams>(params, c.first(k), c.depth(k));
+    LstmWs ws = w.seg(k);
+    TB_TRY(lstm_forward(k ? w.y(k - 1) : x, notdone, h0 + s, c0 + s, p, T1, B, c.in(k), hidden_size, c.depth(k), ws,
+                        k + 1 < S ? w.y(k) : y, hN + s, cN + s, precision, (cudaStream_t)stream));
+  }
+  return 0;
 }
 
 int tb_lstm_backward(const float* dy, const float* x, const float* notdone, const float* const* params, float* const* grads,
@@ -3452,19 +3538,38 @@ int tb_lstm_backward_state(const float* dy, const float* x, const float* notdone
                            float* dc0, void* stream) {
   if (lstm_abi_check(T1, B, input_size, hidden_size, layers, precision)) return 1;
   TB_REQUIRE(dy && x && notdone && params && grads && workspace && dx, "tb_lstm_backward: null pointer");
-  LstmStateGrads sg;
-  sg.dhN = dhN; sg.dcN = dcN; sg.dh0 = dh0; sg.dc0 = dc0;
-  LstmParams p; LstmGrads g;
   for (int l = 0; l < layers; ++l) {
-    p.w_ih[l] = params[4 * l]; p.w_hh[l] = params[4 * l + 1]; p.b_ih[l] = params[4 * l + 2]; p.b_hh[l] = params[4 * l + 3];
-    g.w_ih[l] = grads[4 * l]; g.w_hh[l] = grads[4 * l + 1]; g.b_ih[l] = grads[4 * l + 2]; g.b_hh[l] = grads[4 * l + 3];
-    TB_REQUIRE(p.w_ih[l] && p.w_hh[l] && g.w_ih[l] && g.w_hh[l] && g.b_ih[l] && g.b_hh[l], "tb_lstm_backward: null pointer (layer %d)", l);
+    const float* const* q = params + 4 * l;
+    float* const* r = grads + 4 * l;
+    TB_REQUIRE(q[0] && q[1] && r[0] && r[1] && r[2] && r[3], "tb_lstm_backward: null pointer (layer %d)", l);
   }
-  LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
-  int rc = lstm_backward(dy, x, notdone, p, g, T1, B, input_size, hidden_size, layers, w.ws, dx, w.splitk, w.colsum, precision,
-                         (cudaStream_t)stream, sg);
-  if (rc) return rc;
-  return lstm_backward_join((cudaStream_t)stream);
+  const LstmAbiWs w = lstm_abi_ws(workspace, T1, B, input_size, hidden_size, layers, precision);
+  const LstmChain& c = w.c;
+  const int S = c.segments();
+  const cudaStream_t st = (cudaStream_t)stream;
+  // Top-down: the top segment reads the caller's dy, each segment's dx is the dy of the segment below (through the dmid
+  // ping-pong), and segment 0 writes the caller's dx.  Each segment gets its slices of grads[] and of the state ports; a
+  // NULL port stays NULL.
+  //
+  // No join between segments.  A segment whose weight-gradient GEMMs run as a side-stream tail (kWgradTail) uses its own
+  // ws.wg_scratch and reads only its own LstmWs, so that tail overlaps the segments below: lstm_backward of the next
+  // segment down enqueues its wavefront recurrence first and joins the pending fork only before forking its own tail.
+  // A kWgradSide segment forks its upper layer's GEMMs with the split-K scratch it shares with every other segment; that is
+  // safe because the fork is ordered behind all earlier use of that scratch (on the side stream, which is in-order, behind
+  // the tails above, which never touch it; on the caller's stream, behind the fork point), and the same lstm_backward waits
+  // for the fork before its lower layer, or any later segment, uses the scratch again.
+  for (int k = S - 1; k >= 0; --k) {
+    const int64_t s = int64_t(c.first(k)) * B * hidden_size;
+    const LstmParams p = layer_slice<LstmParams>(params, c.first(k), c.depth(k));
+    const LstmGrads g = layer_slice<LstmGrads>(grads, c.first(k), c.depth(k));
+    LstmStateGrads sg;
+    sg.dhN = dhN ? dhN + s : nullptr; sg.dcN = dcN ? dcN + s : nullptr;
+    sg.dh0 = dh0 ? dh0 + s : nullptr; sg.dc0 = dc0 ? dc0 + s : nullptr;
+    LstmWs ws = w.seg(k);
+    TB_TRY(lstm_backward(k + 1 < S ? w.dmid[(k + 1) & 1] : dy, k ? w.y(k - 1) : x, notdone, p, g, T1, B, c.in(k),
+                         hidden_size, c.depth(k), ws, k ? w.dmid[k & 1] : dx, w.splitk, w.colsum, precision, st, sg));
+  }
+  return lstm_backward_join(st);
 }
 
 }  // extern "C"

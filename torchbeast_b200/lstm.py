@@ -64,8 +64,8 @@ class _LSTMFunction(torch.autograd.Function):
 class LSTM(nn.Module):
     def __init__(self, input_size, hidden_size, num_layers=1, device=None, precision="fp32"):
         super().__init__()
-        if num_layers not in (1, 2):
-            raise _lib.TorchBeastB200Error("torchbeast_b200.lstm.LSTM supports 1 or 2 layers")
+        if num_layers < 1:
+            raise _lib.TorchBeastB200Error("torchbeast_b200.lstm.LSTM: num_layers must be >= 1, got %r" % (num_layers,))
         self.input_size, self.hidden_size, self.num_layers = input_size, hidden_size, num_layers
         self.precision = precision
         dev = device or (torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else "cpu")
@@ -87,11 +87,22 @@ class LSTM(nn.Module):
         return self._ws
 
     def plan(self, B):
-        """(forward kind, backward kind): the recurrence implementations a batch of B runs on the current device."""
+        """(forward kind, backward kind): the recurrence implementations a batch of B runs on the current device (1 or 2
+        layers; plan_layers takes any depth)."""
         fwd, bwd = ctypes.c_int(), ctypes.c_int()
         _lib.check(_lib.lib().tb_lstm_plan(B, self.input_size, self.hidden_size, self.num_layers, PRECISIONS[self.precision],
                                            ctypes.byref(fwd), ctypes.byref(bwd)), "tb_lstm_plan")
         return KINDS[fwd.value], KINDS[bwd.value]
+
+    def plan_layers(self, B):
+        """[(forward kind, backward kind)] per layer.  The stack runs as segments of two layers (the top one alone when
+        num_layers is odd), each planned on its own; both layers of a wavefront segment report its kind."""
+        L = self.num_layers
+        fwd, bwd = (ctypes.c_int * L)(), (ctypes.c_int * L)()
+        _lib.check(_lib.lib().tb_lstm_plan_layers(B, self.input_size, self.hidden_size, L, PRECISIONS[self.precision],
+                                                  ctypes.cast(fwd, ctypes.c_void_p), ctypes.cast(bwd, ctypes.c_void_p)),
+                   "tb_lstm_plan_layers")
+        return [(KINDS[f], KINDS[b]) for f, b in zip(fwd, bwd)]
 
     @staticmethod
     def _ptr_array(tensors):
