@@ -268,6 +268,18 @@ int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const flo
  * frames and stacked_out 16-byte aligned.  One bandwidth-bound launch.                                               */
 int tb_restack_frames_u8(const uint8_t* frames, const uint8_t* done, int64_t T1, int64_t B, int64_t HW, uint8_t* stacked_out,
                          void* stream);
+/* Acting on newest frames: a device-resident frame history per actor stream builds rows 0..2 of the unstacked array.
+ * history u8 [S,3,HW] (caller-owned; a new one is all zeros) holds for stream s, oldest first, channels 1..3 of the
+ * stack of the last step this entry ran for s: channels 0..2 of its next stack unless that step starts an episode.
+ * frames u8 [T+3,B,HW] has the newest frames already in rows 3..T+2; done [T,B] (u8 or bool bytes, non-zero = the step
+ * starts an episode).  For each column b with s = stream_ids[b] in [0,S), rows 0..2 := history[s], then history[s] :=
+ * channels 1..3 of step T-1's stack (the rule above), so T = 1 with done set makes all three the new frame, as
+ * FrameStack.reset does.  A column whose id is < 0 or >= S gets zero rows 0..2, and no history is read or written for
+ * it (graph padding uses -1).  The ids of one call must be distinct: this is not checked, and two columns naming one
+ * stream race.  Calls that share a history must be ordered on one stream.  HW % 16 == 0; frames and history 16-byte
+ * aligned.  One launch; the output feeds tb_atarinet_forward_unstacked / tb_resnet_forward_unstacked with T1 = T.    */
+int tb_frame_history_fill_u8(uint8_t* frames, const uint8_t* done, const int64_t* stream_ids, int64_t T, int64_t B,
+                             int64_t HW, uint8_t* history, int64_t S, void* stream);
 /* Bytes of stacked_scratch the *_forward_unstacked entries need for net (0 = AtariNet, 1 = ResNet) at this precision:
  * 0 where the restack is fused into the backend's frame-image pass (AtariNet bf16 / bf16x3, ResNet bf16x3),
  * T1*B*4*84*84 where the backend reads stacked frames (AtariNet fp32, ResNet fp32 / bf16).  SIZE_MAX for an unknown net,

@@ -61,6 +61,7 @@ _SIGNATURES = {
     "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),
     "tb_restack_frames_u8": ([_vp, _vp, _i64, _i64, _i64, _vp, _vp], _int),
+    "tb_frame_history_fill_u8": ([_vp, _vp, _vp, _i64, _i64, _i64, _vp, _i64, _vp], _int),
     "tb_unstacked_scratch_bytes": ([_int, _i64, _i64, _int], _c.c_size_t),
     "tb_atarinet_forward_unstacked": ([_vp] * 8 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),
     "tb_resnet_forward_unstacked": ([_vp] * 7 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),

@@ -19,4 +19,9 @@ __device__ __forceinline__ int64_t unstacked_row(const uint8_t* __restrict__ don
 int restack_frames_u8(const uint8_t* frames, const uint8_t* done, int64_t T1, int64_t B, int64_t HW, uint8_t* stacked,
                       cudaStream_t stream);
 
+// rows 0..2 of frames [T+3, B, HW] from history [S, 3, HW] at stream_ids[b], then each history := channels 1..3 of
+// step T-1's stack; ids outside [0, S) get zero rows and leave the history alone (tb_frame_history_fill_u8)
+int frame_history_fill_u8(uint8_t* frames, const uint8_t* done, const int64_t* stream_ids, int64_t T, int64_t B,
+                          int64_t HW, uint8_t* history, int64_t S, cudaStream_t stream);
+
 }  // namespace tb

@@ -97,6 +97,21 @@ class FlatParamModule(nn.Module):
     # torchbeast_b200.sampling.ActionSampler used by training-mode forwards instead of torch.multinomial; None keeps the
     # reference's sampling.  Not part of the state_dict: checkpoint its `seed` and `step` alongside.
     action_sampler = None
+    # torchbeast_b200.acting.FrameHistory: with one attached, forward() also takes each stream's newest frame u8
+    # [T, B, 84, 84] and rebuilds the four-frame stacks on the device from that stream's history.  None: forward takes
+    # the stacked and unstacked frames only.  Not part of the state_dict.
+    frame_history = None
+
+    def _forward_frame(self, inputs):
+        """inputs["frame"], or, with a frame_history attached and newest frames [T, B, 84, 84] (T = reward's), the
+        unstacked rollout [T+3, B, 84, 84] the history builds from them (acting.FrameHistory.stack)."""
+        frame, reward = inputs["frame"], inputs["reward"]
+        if self.frame_history is None or frame.dim() != 4 or frame.shape[0] != reward.shape[0]:
+            return frame
+        if frame.shape[1] != reward.shape[1]:
+            raise _lib.TorchBeastB200Error("newest frames [T, B, 84, 84] must match reward's [T, B] = %r, got frame %r"
+                                           % (tuple(reward.shape[:2]), tuple(frame.shape)))
+        return self.frame_history.stack(frame, inputs.get("done"), inputs.get("stream_ids"), self._flat.device)
 
     def _sample(self, logits, inputs):
         """Training-mode action [T, B] of the reference-compatible forwards (monobeast.py:618-619).  With a sampler,
@@ -413,7 +428,7 @@ class AtariNet(FlatParamModule):
 
     # ---- reference-compatible forward ---------------------------------------------------------
     def forward(self, inputs, core_state=()):
-        frame, done = inputs["frame"], inputs.get("done")
+        frame, done = self._forward_frame(inputs), inputs.get("done")
         notdone = self._notdone(done) if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
         params = [v[0] for v in self._views]
@@ -600,7 +615,7 @@ class ResNet(FlatParamModule):
         return fg
 
     def forward(self, inputs, core_state=()):
-        frame, done = inputs["frame"], inputs.get("done")
+        frame, done = self._forward_frame(inputs), inputs.get("done")
         notdone = (~done).float().contiguous() if self.use_lstm else None
         h0, c0 = core_state if self.use_lstm else (None, None)
         params = [v[0] for v in self._views]
