@@ -97,6 +97,35 @@ int tb_impala_loss_fwd_bwd_f32(const float* behavior_logits, const float* target
                                float* target_alp, float* losses_out, float* grad_logits,
                                float* grad_values, int zero_tail, void* workspace, void* stream);
 
+/* ---- hyper-parameters read from device memory ------------------------------------------
+ * The scalar arguments of the loss and optimizer steps, as one block in device memory.  The *_hp entry points
+ * read their values from it when the kernel runs, so a captured CUDA graph follows changes the caller publishes
+ * between replays (annealed costs, population-based training).  Every value derived from them (1 - alpha,
+ * 1 - beta, the clip coefficient, the bias corrections) is computed in the kernel by the same expression as in
+ * the float-argument entry points, so both give bit-identical results for the same values.  Layout is fixed:
+ * tb_hparams_layout() reports it, so a binding can check its packing without a GPU.                       */
+typedef struct tb_hparams {
+  double beta1, beta2;         /* Adam / AdamW, in [0, 1); double as in tb_clip_adam_step_f32                  */
+  float discounting;           /* used where done is given; a `discounts` array is used as is                  */
+  float baseline_cost, entropy_cost;
+  float clip_rho, clip_pg_rho; /* negative or NaN: no clipping (Python None)                                   */
+  int32_t clip_rewards;        /* != 0: clamp rewards to [-1, 1]                                               */
+  float max_norm;              /* gradient-norm clip; negative: no clipping                                    */
+  float alpha, eps, momentum, weight_decay; /* RMSprop: alpha, eps, momentum, weight_decay; Adam: eps, weight_decay */
+} tb_hparams;
+/* Host only: out[0] = sizeof(tb_hparams), out[1..13] = offsetof of discounting, baseline_cost, entropy_cost,
+ * clip_rho, clip_pg_rho, clip_rewards, max_norm, alpha, eps, momentum, weight_decay, beta1, beta2.           */
+int tb_hparams_layout(int64_t* out_host);
+/* tb_impala_loss_fwd_bwd_f32 with discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho and
+ * clip_pg_rho read from hp (device pointer) when the kernel runs.                                          */
+int tb_impala_loss_fwd_bwd_hp_f32(const float* behavior_logits, const float* target_logits,
+                                  const int64_t* actions, const float* rewards, const uint8_t* done,
+                                  const float* discounts, const float* values, const float* bootstrap, int64_t T,
+                                  int64_t B, int64_t A, const tb_hparams* hp, float* vs, float* pg_adv,
+                                  float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                                  float* grad_logits, float* grad_values, int zero_tail, void* workspace,
+                                  void* stream);
+
 /* ---- seeded action sampling for the acting forward ------------------------------------ */
 
 /* monobeast.py:618-619 / polybeast_learner.py:256-257  torch.multinomial(F.softmax(policy_logits, dim=1), 1) as a
@@ -346,6 +375,19 @@ int tb_clip_rmsprop_ex_step_f32(float* params, float* grads, float* square_avg, 
                                 int64_t n, const float* sumsq, float max_norm, const float* lr_device, float lr,
                                 float alpha, float eps, float weight_decay, float momentum, float* grad_norm_out,
                                 void* stream);
+/* The three steps above with max_norm and the optimizer's values read from hp (device pointer, see tb_hparams)
+ * when the kernel runs; lr_device / lr as above.  The host cannot see hp's values, so the caller checks what the
+ * float-argument entry points check: momentum != 0 needs momentum_buf, betas in [0, 1).  momentum_buf != NULL
+ * selects the momentum update (pass NULL when momentum is 0, as the float-argument entry points do).          */
+int tb_clip_rmsprop_step_hp_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
+                                const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr,
+                                float* grad_norm_out, void* stream);
+int tb_clip_rmsprop_ex_step_hp_f32(float* params, float* grads, float* square_avg, float* grad_avg,
+                                   float* momentum_buf, int64_t n, const float* sumsq, const tb_hparams* hp,
+                                   const float* lr_device, float lr, float* grad_norm_out, void* stream);
+int tb_clip_adam_step_hp_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
+                             const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr, int decoupled,
+                             int64_t* step_device, float* grad_norm_out, void* stream);
 
 /* ---- bf16 tensor-core GEMM (wgmma + TMA), the throughput backend of the network -------- */
 

@@ -29,6 +29,8 @@ _SIGNATURES = {
     "tb_vtrace_from_importance_weights_f64": ([_vp] * 5 + [_i64, _i64, _f64, _f64, _vp, _vp, _vp], _int),
     "tb_impala_loss_fwd_bwd_f32": (
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 8 + [_int, _vp, _vp], _int),
+    "tb_hparams_layout": ([_vp], _int),
+    "tb_impala_loss_fwd_bwd_hp_f32": ([_vp] * 8 + [_i64, _i64, _i64] + [_vp] * 9 + [_int, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f32": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),
@@ -57,6 +59,9 @@ _SIGNATURES = {
     "tb_clip_adam_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f64, _f64, _f32, _f32, _int, _vp, _vp, _vp],
                               _int),
     "tb_clip_rmsprop_ex_step_f32": ([_vp] * 5 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _f32, _vp, _vp], _int),
+    "tb_clip_rmsprop_step_hp_f32": ([_vp] * 4 + [_i64, _vp, _vp, _vp, _f32, _vp, _vp], _int),
+    "tb_clip_rmsprop_ex_step_hp_f32": ([_vp] * 5 + [_i64, _vp, _vp, _vp, _f32, _vp, _vp], _int),
+    "tb_clip_adam_step_hp_f32": ([_vp] * 4 + [_i64, _vp, _vp, _vp, _f32, _int, _vp, _vp, _vp], _int),
     "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),

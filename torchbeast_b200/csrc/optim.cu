@@ -32,10 +32,13 @@ __global__ void grad_sumsq_kernel(const float* __restrict__ g, int64_t n, float*
 
 // coef = min(1, max_norm / (norm + 1e-6)); g *= coef; sq = alpha*sq + (1-alpha) g^2;
 // avg = sqrt(sq) + eps; momentum==0: p -= lr * g/avg; else buf = momentum*buf + g/avg; p -= lr*buf
+// hp (nullable) overrides max_norm, alpha, eps and momentum, as lr_dev overrides lr_host.
 __global__ void clip_rmsprop_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ sq,
                                     float* __restrict__ mom, int64_t n, const float* __restrict__ sumsq,
                                     float max_norm, const float* __restrict__ lr_dev, float lr_host, float alpha,
-                                    float eps, float momentum, float* __restrict__ norm_out) {
+                                    float eps, float momentum, const tb_hparams* __restrict__ hp,
+                                    float* __restrict__ norm_out) {
+  if (hp) { max_norm = hp->max_norm; alpha = hp->alpha; eps = hp->eps; momentum = hp->momentum; }
   const float norm = sqrtf(sumsq[0]);
   float coef = 1.0f;
   if (max_norm >= 0.0f) coef = fminf(max_norm / (norm + 1e-6f), 1.0f);
@@ -108,7 +111,8 @@ __global__ void clip_adam_kernel(float* __restrict__ p, float* __restrict__ g, f
                                  float* __restrict__ v, int64_t n, const float* __restrict__ sumsq, float max_norm,
                                  const float* __restrict__ lr_dev, float lr_host, double beta1, double beta2, float eps,
                                  float wd, int decoupled, const int64_t* __restrict__ step,
-                                 float* __restrict__ norm_out) {
+                                 const tb_hparams* __restrict__ hp, float* __restrict__ norm_out) {
+  if (hp) { max_norm = hp->max_norm; beta1 = hp->beta1; beta2 = hp->beta2; eps = hp->eps; wd = hp->weight_decay; }
   AdamArgs a;
   a.coef = clip_coef(sumsq, max_norm, norm_out);
   a.lr = lr_dev ? lr_dev[0] : lr_host;
@@ -172,7 +176,9 @@ __global__ void clip_rmsprop_ex_kernel(float* __restrict__ p, float* __restrict_
                                        float* __restrict__ ga, float* __restrict__ mom, int64_t n,
                                        const float* __restrict__ sumsq, float max_norm,
                                        const float* __restrict__ lr_dev, float lr_host, float alpha, float eps,
-                                       float wd, float momentum, float* __restrict__ norm_out) {
+                                       float wd, float momentum, const tb_hparams* __restrict__ hp,
+                                       float* __restrict__ norm_out) {
+  if (hp) { max_norm = hp->max_norm; alpha = hp->alpha; eps = hp->eps; wd = hp->weight_decay; momentum = hp->momentum; }
   RmsExArgs a;
   a.coef = clip_coef(sumsq, max_norm, norm_out);
   a.lr = lr_dev ? lr_dev[0] : lr_host;
@@ -232,7 +238,7 @@ int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, flo
   ProfScope prof("clip_rmsprop", (cudaStream_t)stream);
   clip_rmsprop_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       params, grads, square_avg, momentum != 0.0f ? momentum_buf : nullptr, n, sumsq, max_norm, lr_device, lr, alpha,
-      eps, momentum, grad_norm_out);
+      eps, momentum, nullptr, grad_norm_out);
   return check_launch("clip_rmsprop_kernel");
 }
 
@@ -248,7 +254,7 @@ int tb_clip_adam_step_f32(float* params, float* grads, float* exp_avg, float* ex
   ProfScope prof("clip_adam", (cudaStream_t)stream);
   clip_adam_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       params, grads, exp_avg, exp_avg_sq, n, sumsq, max_norm, lr_device, lr, beta1, beta2, eps, weight_decay,
-      decoupled, step_device, grad_norm_out);
+      decoupled, step_device, nullptr, grad_norm_out);
   if (int rc = check_launch("clip_adam_kernel")) return rc;
   adam_step_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_device);
   return check_launch("adam_step_advance_kernel");
@@ -267,7 +273,55 @@ int tb_clip_rmsprop_ex_step_f32(float* params, float* grads, float* square_avg, 
   ProfScope prof("clip_rmsprop_ex", (cudaStream_t)stream);
   clip_rmsprop_ex_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       params, grads, square_avg, grad_avg, momentum != 0.0f ? momentum_buf : nullptr, n, sumsq, max_norm, lr_device, lr,
-      alpha, eps, weight_decay, momentum, grad_norm_out);
+      alpha, eps, weight_decay, momentum, nullptr, grad_norm_out);
+  return check_launch("clip_rmsprop_ex_kernel");
+}
+
+// The _hp entry points launch the same kernels with the same grids and profile records; the kernels read the
+// scalars from hp.  momentum_buf is passed as given: the caller passes it exactly when momentum is non-zero.
+int tb_clip_rmsprop_step_hp_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
+                                const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr,
+                                float* grad_norm_out, void* stream) {
+  TB_REQUIRE(n >= 0 && sumsq && hp, "tb_clip_rmsprop_step_hp_f32: bad arguments");
+  if (n == 0) return 0;
+  TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_step_hp_f32: null buffer");
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  ProfScope prof("clip_rmsprop", (cudaStream_t)stream);
+  clip_rmsprop_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      params, grads, square_avg, momentum_buf, n, sumsq, 0.0f, lr_device, lr, 0.0f, 0.0f, 0.0f, hp, grad_norm_out);
+  return check_launch("clip_rmsprop_kernel");
+}
+
+int tb_clip_adam_step_hp_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
+                             const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr, int decoupled,
+                             int64_t* step_device, float* grad_norm_out, void* stream) {
+  TB_REQUIRE(n >= 0 && sumsq && hp && step_device, "tb_clip_adam_step_hp_f32: bad arguments");
+  TB_REQUIRE(n == 0 || (params && grads && exp_avg && exp_avg_sq), "tb_clip_adam_step_hp_f32: null buffer");
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  if (blocks < 1) blocks = 1;  // n == 0 still counts the step
+  ProfScope prof("clip_adam", (cudaStream_t)stream);
+  clip_adam_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      params, grads, exp_avg, exp_avg_sq, n, sumsq, 0.0f, lr_device, lr, 0.0, 0.0, 0.0f, 0.0f, decoupled, step_device,
+      hp, grad_norm_out);
+  if (int rc = check_launch("clip_adam_kernel")) return rc;
+  adam_step_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_device);
+  return check_launch("adam_step_advance_kernel");
+}
+
+int tb_clip_rmsprop_ex_step_hp_f32(float* params, float* grads, float* square_avg, float* grad_avg,
+                                   float* momentum_buf, int64_t n, const float* sumsq, const tb_hparams* hp,
+                                   const float* lr_device, float lr, float* grad_norm_out, void* stream) {
+  TB_REQUIRE(n >= 0 && sumsq && hp, "tb_clip_rmsprop_ex_step_hp_f32: bad arguments");
+  if (n == 0) return 0;
+  TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_ex_step_hp_f32: null buffer");
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  ProfScope prof("clip_rmsprop_ex", (cudaStream_t)stream);
+  clip_rmsprop_ex_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+      params, grads, square_avg, grad_avg, momentum_buf, n, sumsq, 0.0f, lr_device, lr, 0.0f, 0.0f, 0.0f, 0.0f, hp,
+      grad_norm_out);
   return check_launch("clip_rmsprop_ex_kernel");
 }
 

@@ -107,6 +107,21 @@ int tb_profile_collect(char* names_host, size_t names_cap, float* ms_host, int m
   return n;
 }
 
+// The layout of tb_hparams as compiled, for a binding's check of its packing (host only).
+int tb_hparams_layout(int64_t* out) {
+  TB_REQUIRE(out, "tb_hparams_layout: null pointer");
+  const int64_t layout[] = {
+      int64_t(sizeof(tb_hparams)),
+      int64_t(offsetof(tb_hparams, discounting)), int64_t(offsetof(tb_hparams, baseline_cost)),
+      int64_t(offsetof(tb_hparams, entropy_cost)), int64_t(offsetof(tb_hparams, clip_rho)),
+      int64_t(offsetof(tb_hparams, clip_pg_rho)), int64_t(offsetof(tb_hparams, clip_rewards)),
+      int64_t(offsetof(tb_hparams, max_norm)), int64_t(offsetof(tb_hparams, alpha)), int64_t(offsetof(tb_hparams, eps)),
+      int64_t(offsetof(tb_hparams, momentum)), int64_t(offsetof(tb_hparams, weight_decay)),
+      int64_t(offsetof(tb_hparams, beta1)), int64_t(offsetof(tb_hparams, beta2))};
+  memcpy(out, layout, sizeof(layout));
+  return 0;
+}
+
 // Host side of the learner-queue ingest (SURVEY 8(f) N1): one actor hands its [T1, ...] rollout over by writing it into
 // batch column b of a pinned [T1, B, ...] slot - what actorpool.cc:493-506 + the BatchingQueue's torch::cat (actorpool.cc:
 // 49-55) do with per-rollout tensors and a concatenation.  Plain memcpy per (leaf, time step): leaf l of the slot starts

@@ -431,7 +431,16 @@ struct LossArgs {
   float* grad_logits; float* grad_values; int zero_tail;
   void* workspace;
   int wide;  // see ScanArgs
+  const tb_hparams* hp;  // nullable: overrides the scalars above when the kernel runs
 };
+
+// The scalars of a tb_hparams block, with has_clip_* derived as the float-argument entry point derives them.
+__device__ __forceinline__ void load_hparams(LossArgs& p) {
+  const tb_hparams* h = p.hp;
+  p.discounting = h->discounting; p.baseline_cost = h->baseline_cost; p.entropy_cost = h->entropy_cost;
+  p.clip_rewards = h->clip_rewards; p.clip_rho = h->clip_rho; p.clip_pg = h->clip_pg_rho;
+  p.has_clip_rho = (p.clip_rho >= 0.0f); p.has_clip_pg = (p.clip_pg >= 0.0f);
+}
 
 __device__ __forceinline__ float reward_of(const LossArgs& p, int64_t i) {
   float r = p.rewards[i];
@@ -444,6 +453,7 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 
 template <int A>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
+  if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* sA = reinterpret_cast<float*>(smem_raw);
   float* sB = sA + blockDim.y * kWarp;
@@ -628,6 +638,56 @@ static int reduce_grid(int64_t N, int threads) {
   return int(blocks < 1 ? 1 : blocks);
 }
 
+// Both loss entry points: hp == nullptr takes the scalar arguments, else the kernel reads them from hp.
+static int launch_impala_loss(const float* blogits, const float* tlogits, const int64_t* actions,
+                              const float* rewards, const uint8_t* done, const float* discounts,
+                              const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
+                              float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
+                              float clip_rho, float clip_pg_rho, const tb_hparams* hp, float* vs, float* pg_adv,
+                              float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                              float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream) {
+  TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
+             (long long)B, (long long)A);
+  TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
+  if (T == 0 || B == 0) {
+    cudaError_t e = cudaMemsetAsync(losses_out, 0, 4 * sizeof(float), (cudaStream_t)stream);
+    TB_REQUIRE(e == cudaSuccess, "impala_loss: memset: %s", cudaGetErrorString(e));
+    if (B > 0 && zero_tail) {
+      if (grad_values) cudaMemsetAsync(grad_values, 0, B * sizeof(float), (cudaStream_t)stream);
+      if (grad_logits) cudaMemsetAsync(grad_logits, 0, B * A * sizeof(float), (cudaStream_t)stream);
+    }
+    return 0;
+  }
+  TB_REQUIRE(blogits && tlogits && actions && rewards && (done || discounts) && values && bootstrap,
+             "impala_loss: null input pointer");
+  TB_REQUIRE(vs && pg_adv && log_rhos && behavior_alp && target_alp, "impala_loss: null output pointer");
+  LossArgs p;
+  p.blogits = blogits; p.tlogits = tlogits; p.actions = actions; p.rewards = rewards; p.done = done;
+  p.discounts = discounts; p.values = values; p.bootstrap = bootstrap; p.T = T; p.B = B; p.A = A;
+  p.discounting = discounting; p.baseline_cost = baseline_cost; p.entropy_cost = entropy_cost;
+  p.clip_rewards = clip_rewards; p.clip_rho = clip_rho; p.clip_pg = clip_pg_rho;
+  p.has_clip_rho = (clip_rho >= 0.0f); p.has_clip_pg = (clip_pg_rho >= 0.0f);
+  p.vs = vs; p.pg_adv = pg_adv; p.log_rhos = log_rhos; p.balp = behavior_alp; p.talp = target_alp;
+  p.losses = losses_out; p.grad_logits = grad_logits; p.grad_values = grad_values; p.zero_tail = zero_tail;
+  p.workspace = workspace;
+  p.hp = hp;
+  const int64_t tiles = (B + kWarp - 1) / kWarp;
+  int W = pick_warps(T, tiles);
+  p.wide = (W == 1);
+  dim3 grid(pick_grid(tiles));
+  if (p.wide) {
+    W = kWideWarps;
+    int64_t g = (tiles + W - 1) / W;
+    if (g > kMaxPartialCtas) g = kMaxPartialCtas;  // per-CTA loss partials live in the workspace
+    grid = dim3((unsigned)(g < 1 ? 1 : g));
+  }
+  dim3 block(kWarp, W);
+  const size_t smem = size_t(2) * W * kWarp * sizeof(float);
+  ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
+  TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+  return check_launch("impala_loss_kernel");
+}
+
 }  // namespace tb
 
 // ========================================================================================
@@ -662,45 +722,22 @@ int tb_impala_loss_fwd_bwd_f32(const float* blogits, const float* tlogits, const
                                float clip_rho, float clip_pg_rho, float* vs, float* pg_adv, float* log_rhos,
                                float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
                                float* grad_values, int zero_tail, void* workspace, void* stream) {
-  TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
-             (long long)B, (long long)A);
-  TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
-  if (T == 0 || B == 0) {
-    cudaError_t e = cudaMemsetAsync(losses_out, 0, 4 * sizeof(float), (cudaStream_t)stream);
-    TB_REQUIRE(e == cudaSuccess, "impala_loss: memset: %s", cudaGetErrorString(e));
-    if (B > 0 && zero_tail) {
-      if (grad_values) cudaMemsetAsync(grad_values, 0, B * sizeof(float), (cudaStream_t)stream);
-      if (grad_logits) cudaMemsetAsync(grad_logits, 0, B * A * sizeof(float), (cudaStream_t)stream);
-    }
-    return 0;
-  }
-  TB_REQUIRE(blogits && tlogits && actions && rewards && (done || discounts) && values && bootstrap,
-             "impala_loss: null input pointer");
-  TB_REQUIRE(vs && pg_adv && log_rhos && behavior_alp && target_alp, "impala_loss: null output pointer");
-  LossArgs p;
-  p.blogits = blogits; p.tlogits = tlogits; p.actions = actions; p.rewards = rewards; p.done = done;
-  p.discounts = discounts; p.values = values; p.bootstrap = bootstrap; p.T = T; p.B = B; p.A = A;
-  p.discounting = discounting; p.baseline_cost = baseline_cost; p.entropy_cost = entropy_cost;
-  p.clip_rewards = clip_rewards; p.clip_rho = clip_rho; p.clip_pg = clip_pg_rho;
-  p.has_clip_rho = (clip_rho >= 0.0f); p.has_clip_pg = (clip_pg_rho >= 0.0f);
-  p.vs = vs; p.pg_adv = pg_adv; p.log_rhos = log_rhos; p.balp = behavior_alp; p.talp = target_alp;
-  p.losses = losses_out; p.grad_logits = grad_logits; p.grad_values = grad_values; p.zero_tail = zero_tail;
-  p.workspace = workspace;
-  const int64_t tiles = (B + kWarp - 1) / kWarp;
-  int W = pick_warps(T, tiles);
-  p.wide = (W == 1);
-  dim3 grid(pick_grid(tiles));
-  if (p.wide) {
-    W = kWideWarps;
-    int64_t g = (tiles + W - 1) / W;
-    if (g > kMaxPartialCtas) g = kMaxPartialCtas;  // per-CTA loss partials live in the workspace
-    grid = dim3((unsigned)(g < 1 ? 1 : g));
-  }
-  dim3 block(kWarp, W);
-  const size_t smem = size_t(2) * W * kWarp * sizeof(float);
-  ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
-  TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
-  return check_launch("impala_loss_kernel");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
+                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, nullptr,
+                            vs, pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
+                            zero_tail, workspace, stream);
+}
+
+int tb_impala_loss_fwd_bwd_hp_f32(const float* blogits, const float* tlogits, const int64_t* actions,
+                                  const float* rewards, const uint8_t* done, const float* discounts,
+                                  const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
+                                  const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
+                                  float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
+                                  float* grad_values, int zero_tail, void* workspace, void* stream) {
+  TB_REQUIRE(hp, "impala_loss: null hyper-parameter block");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A, 0.0f,
+                            0.0f, 0.0f, 0, -1.0f, -1.0f, hp, vs, pg_adv, log_rhos, behavior_alp, target_alp,
+                            losses_out, grad_logits, grad_values, zero_tail, workspace, stream);
 }
 
 #define TB_LOSS_ENTRY(NAME, F, KERNEL, ARGS_DECL, ARGS_CALL, NEXPR)                                     \

@@ -3,6 +3,7 @@ import collections
 import os
 import threading
 
+import numpy as np
 import torch
 
 from torchbeast_b200 import _lib
@@ -11,6 +12,52 @@ ImpalaLoss = collections.namedtuple(
     "ImpalaLoss",
     "vs pg_advantages log_rhos behavior_action_log_probs target_action_log_probs losses grad_logits grad_values",
 )
+
+# tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the *_hp entry points read from device memory.
+# tb_hparams_layout() reports the compiled layout; tests/test_graph_hparams_cpu.py checks this record against it.
+HPARAMS = np.dtype([
+    ("beta1", "<f8"), ("beta2", "<f8"), ("discounting", "<f4"), ("baseline_cost", "<f4"), ("entropy_cost", "<f4"),
+    ("clip_rho", "<f4"), ("clip_pg_rho", "<f4"), ("clip_rewards", "<i4"), ("max_norm", "<f4"), ("alpha", "<f4"),
+    ("eps", "<f4"), ("momentum", "<f4"), ("weight_decay", "<f4")], align=True)
+
+
+def _clip_rewards(reward_clipping):
+    if reward_clipping not in ("abs_one", "none"):
+        raise ValueError("reward_clipping must be 'abs_one' or 'none'")
+    return int(reward_clipping == "abs_one")
+
+
+def pack_hparams(flags, optimizer=None, clip_rho_threshold=1.0, clip_pg_rho_threshold=1.0):
+    """The tb_hparams record of one learn() step, as a 0-dim NumPy array of HPARAMS: the loss values and the gradient
+    clip from `flags`, the optimizer's from `optimizer.param_groups[0]` (a FusedOptimizer; fields it does not use stay
+    0).  Raises what the eager step would raise for the same values, so nothing is captured or replayed with them."""
+    rec = np.zeros((), HPARAMS)
+    rec["discounting"] = flags.discounting
+    rec["baseline_cost"] = flags.baseline_cost
+    rec["entropy_cost"] = flags.entropy_cost
+    rec["clip_rewards"] = _clip_rewards(flags.reward_clipping)
+    rec["clip_rho"] = _lib.clip_arg(clip_rho_threshold)
+    rec["clip_pg_rho"] = _lib.clip_arg(clip_pg_rho_threshold)
+    rec["max_norm"] = -1.0 if flags.grad_norm_clipping is None else float(flags.grad_norm_clipping)
+    if optimizer is not None:
+        for k, v in optimizer.hparams().items():
+            rec[k] = v
+    return rec
+
+
+def publish_hparams(rec, block):
+    """Enqueue the copy of record `rec` into the device block `block` (uint8 [HPARAMS.itemsize]) on the current stream.
+    The source is a fresh pinned buffer: the caching host allocator does not hand it out again until the copy is done."""
+    host = torch.empty(HPARAMS.itemsize, dtype=torch.uint8, pin_memory=True)
+    host.numpy()[:] = np.frombuffer(rec.tobytes(), dtype=np.uint8)
+    block.copy_(host, non_blocking=True)
+
+
+def hparams_field(block, name):
+    """Field `name` of a device tb_hparams block as a 0-dim tensor view (float32 / float64 / int32)."""
+    dt, off = HPARAMS.fields[name]
+    torch_dtype = {"<f4": torch.float32, "<f8": torch.float64, "<i4": torch.int32}[dt.str]
+    return block[off:off + dt.itemsize].view(torch_dtype).view(())
 
 
 @torch.no_grad()
@@ -29,6 +76,7 @@ def impala_loss_fwd_bwd(
     clip_rho_threshold=1.0,
     clip_pg_rho_threshold=1.0,
     with_grads=True,
+    hparams_dev=None,
 ):
     """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_fwd_bwd_f32).
 
@@ -37,11 +85,18 @@ def impala_loss_fwd_bwd(
     autograd graph behind them: returns vs / pg_advantages / log-rhos, losses =
     [pg, baseline_cost*baseline, entropy_cost*entropy, total] and d total / d(target logits,
     values) laid out as [T+1,B,...] with a zero bootstrap row, ready for the network backward.
+
+    With `hparams_dev` (a device tb_hparams block, see pack_hparams / publish_hparams) the kernel reads discounting,
+    the costs, the reward clip and the two V-trace clips from the block when it runs, and the corresponding arguments
+    are not used: a captured CUDA graph then follows what is published between replays.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
-    if reward_clipping not in ("abs_one", "none"):
-        raise ValueError("reward_clipping must be 'abs_one' or 'none'")
+    if hparams_dev is None:
+        clip_rewards = _clip_rewards(reward_clipping)
+    else:
+        _lib.require_cuda(hparams_dev)
+        discounting = hparams_field(hparams_dev, "discounting")  # uint8 done: the discounts below read the block
     T, B, A = target_policy_logits.shape
     dev = values.device
     f32 = torch.float32
@@ -63,11 +118,20 @@ def impala_loss_fwd_bwd(
     losses = torch.empty(4, dtype=f32, device=dev)
     gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
     gv = torch.empty((T + 1, B), dtype=f32, device=dev) if with_grads else None
+    if hparams_dev is not None:
+        _lib.check(
+            _lib.lib().tb_impala_loss_fwd_bwd_hp_f32(
+                _lib.ptr(bl), _lib.ptr(tl), _lib.ptr(ac), _lib.ptr(rw), _lib.ptr(dn), _lib.ptr(disc),
+                _lib.ptr(va), _lib.ptr(bs), T, B, A, _lib.ptr(hparams_dev),
+                *[_lib.ptr(o) for o in outs], _lib.ptr(losses), _lib.ptr(gl), _lib.ptr(gv), 1,
+                _lib.ptr(_lib.workspace()), _lib.stream_ptr()),
+            "tb_impala_loss_fwd_bwd_hp_f32")
+        return ImpalaLoss(*outs, losses, gl, gv)
     _lib.check(
         _lib.lib().tb_impala_loss_fwd_bwd_f32(
             _lib.ptr(bl), _lib.ptr(tl), _lib.ptr(ac), _lib.ptr(rw), _lib.ptr(dn), _lib.ptr(disc),
             _lib.ptr(va), _lib.ptr(bs), T, B, A, float(discounting), float(baseline_cost), float(entropy_cost),
-            int(reward_clipping == "abs_one"), _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold),
+            clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold),
             *[_lib.ptr(o) for o in outs], _lib.ptr(losses), _lib.ptr(gl), _lib.ptr(gv), 1,
             _lib.ptr(_lib.workspace()), _lib.stream_ptr()),
         "tb_impala_loss_fwd_bwd_f32")
@@ -141,11 +205,12 @@ def _backward_with_overlapped_all_reduce(model, grad_logits, grad_values):
     return fg
 
 
-def optimizer_step(model, optimizer, max_grad_norm):
+def optimizer_step(model, optimizer, max_grad_norm, hparams_dev=None):
     from torchbeast_b200 import optim as _optim
 
     if isinstance(optimizer, _optim.FusedOptimizer):
-        optimizer.step(max_grad_norm=max_grad_norm)  # fused clip + update on the flat buffers, 2-3 launches
+        # fused clip + update on the flat buffers, 2-3 launches
+        optimizer.step(max_grad_norm=max_grad_norm, hparams_dev=hparams_dev)
     else:
         # foreign optimizer object: gradients are already in .grad (views of the flat buffer)
         torch.nn.utils.clip_grad_norm_(model.parameters(), max_grad_norm)
@@ -153,12 +218,14 @@ def optimizer_step(model, optimizer, max_grad_norm):
 
 
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
-               behavior_logits=None, actions=None, stats_sync=True):
+               behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
       network forward -> fused V-trace + 3 losses + their gradients (1 launch) -> network
       backward into the flat gradient -> [NCCL all-reduce] -> fused clip + optimizer step -> actor copy.
+    With `hparams_dev` (GraphedLearner's device tb_hparams block) the loss and the optimizer read the values of
+    `flags` and of the optimizer's param group from the block, not from the host.
     """
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
@@ -167,9 +234,9 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
         out.baseline[:-1], out.baseline[-1],
         discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
-        reward_clipping=flags.reward_clipping)
+        reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
     _backward_with_overlapped_all_reduce(model, loss.grad_logits, loss.grad_values)
-    optimizer_step(model, optimizer, flags.grad_norm_clipping)
+    optimizer_step(model, optimizer, flags.grad_norm_clipping, hparams_dev=hparams_dev)
     if scheduler is not None:
         scheduler.step()
     if actor_model is not None and actor_model is not model:
@@ -243,13 +310,23 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
             batch = dict(batch, last_action=batch["action"])
         try:
             if _graph_enabled(flags):
+                _require_fused(optimizer)
+                hparams = pack_hparams(flags, optimizer)  # raises before anything is captured or replayed
+                structure = GraphedLearner.structure_of(optimizer, batch)
                 graphs = model.__dict__.setdefault("_tb_graphs", {})
                 gkey = (tuple((k, tuple(v.shape)) for k, v in batch.items() if k in GraphedLearner.KEYS), id(optimizer),
                         id(actor_model))
                 gl = graphs.get(gkey)
-                if gl is None:
-                    gl = graphs[gkey] = GraphedLearner(flags, model, actor_model, optimizer, batch, initial_agent_state)
-                gl.step(batch, initial_agent_state, scheduler)
+                if gl is None or gl.structure != structure:
+                    # a value that chooses a kernel or a buffer changed, so the eager step would switch too: replay the
+                    # graph of the new structure, captured now or kept from before; the current one stays cached
+                    if gl is not None:
+                        graphs[gkey + (gl.structure,)] = gl
+                    gl = graphs.pop(gkey + (structure,), None)
+                    if gl is None:
+                        gl = GraphedLearner(flags, model, actor_model, optimizer, batch, initial_agent_state)
+                    graphs[gkey] = gl
+                gl.step(batch, initial_agent_state, scheduler, hparams)
                 if stager is not None:
                     stager.release(slot)  # the inputs now live in the graph's static buffers
                     slot = None
@@ -289,6 +366,13 @@ def shard_rollout(batch, initial_agent_state, rank, world_size):
     return shard, state
 
 
+def _require_fused(optimizer):
+    from torchbeast_b200 import optim as _optim
+    if not isinstance(optimizer, _optim.FusedOptimizer):
+        raise _lib.TorchBeastB200Error(
+            "GraphedLearner needs a fused optimizer from torchbeast_b200.optim (RMSprop, Adam or AdamW)")
+
+
 class GraphedLearner:
     """The whole device side of learn() captured ONCE into a CUDA graph and replayed per step.
 
@@ -297,16 +381,27 @@ class GraphedLearner:
     become one cudaGraphLaunch, so a learner that reads its stats back every step (like the reference, monobeast.py:279-287) is no longer
     exposed to per-launch CPU latency.  Inputs are copied into static device buffers before each replay;
     the learning rate is read from a device scalar so LambdaLR keeps working; stats are computed from the
-    graph's static outputs after the replay."""
+    graph's static outputs after the replay.
+
+    The other values learn() reads (discounting, the two costs, reward clipping, the gradient clip, and the
+    optimizer's alpha / eps / momentum / weight_decay / betas) are read from a device tb_hparams block that step()
+    publishes before every replay, so they may change between steps without a new capture.  The values that choose a
+    kernel or a buffer (`structure`) are fixed per graph; learn() captures another graph when one of them changes."""
 
     KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return")
 
+    @staticmethod
+    def structure_of(optimizer, batch):
+        """What the captured launch sequence depends on besides shapes: the optimizer's kernel and buffer choices
+        (RMSprop centered / weight_decay != 0 / momentum != 0, Adam vs AdamW) and the dtype of `done`."""
+        return optimizer.structure() + (batch["done"].dtype,)
+
     def __init__(self, flags, model, actor_model, optimizer, example_batch, initial_agent_state=()):
-        from torchbeast_b200 import optim as _optim
-        if not isinstance(optimizer, _optim.FusedOptimizer):
-            raise _lib.TorchBeastB200Error(
-                "GraphedLearner needs a fused optimizer from torchbeast_b200.optim (RMSprop, Adam or AdamW)")
+        _require_fused(optimizer)
         self.flags, self.model, self.actor, self.opt = flags, model, actor_model, optimizer
+        self.structure = self.structure_of(optimizer, example_batch)
+        self.hparams = torch.zeros(HPARAMS.itemsize, dtype=torch.uint8, device=model.flat_params.device)
+        publish_hparams(pack_hparams(flags, optimizer), self.hparams)
         self.static = {k: torch.empty_like(v) for k, v in example_batch.items() if k in self.KEYS}
         self.static_state = tuple(torch.empty_like(s) for s in initial_agent_state)
         for k, v in self.static.items():
@@ -321,13 +416,14 @@ class GraphedLearner:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None, stats_sync=False)
+                learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None, stats_sync=False,
+                           hparams_dev=self.hparams)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.out = learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None,
-                                  stats_sync=False)
+                                  stats_sync=False, hparams_dev=self.hparams)
         # the graph writes into the model workspace it was captured with; the model replaces (and frees) that buffer when
         # it runs another shape, e.g. while the GraphedLearner of another batch shape is captured: keep it alive here
         self.workspace = getattr(model, "_ws", None)
@@ -342,12 +438,15 @@ class GraphedLearner:
         if actor_model is not None and hasattr(actor_model, "copy_params_from"):
             actor_model.copy_params_from(model)
 
-    def step(self, batch, initial_agent_state=(), scheduler=None):
+    def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
+        """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
+        flags this graph was captured with and the optimizer's current param group)."""
         for k, v in self.static.items():
             v.copy_(batch[k], non_blocking=True)
         for d, s in zip(self.static_state, initial_agent_state):
             d.copy_(s, non_blocking=True)
         self.opt.sync_lr_to_device()
+        publish_hparams(pack_hparams(self.flags, self.opt) if hparams is None else hparams, self.hparams)
         self.graph.replay()
         if scheduler is not None:
             scheduler.step()

@@ -7,6 +7,7 @@ same constructor arguments, `param_groups[0]["lr"]` is honoured so
 `torch.optim.lr_scheduler.LambdaLR` works unchanged, `state_dict()` carries the per-parameter
 state entries torch's optimizers write, and `load_state_dict()` accepts torch's.
 """
+import numpy as np
 import torch
 
 from torchbeast_b200 import _lib
@@ -19,7 +20,10 @@ class FusedOptimizer(torch.optim.Optimizer):
     * `flat_state()`: the device tensors a step updates besides the parameters (state buffers, device step counter);
       `snapshot()` / `restore(snapshot)` copy them (and any host-side counter) out and back;
     * `lr_from_device` / `sync_lr_to_device()`: read the learning rate from a device scalar, so a captured CUDA graph
-      sees scheduler updates.
+      sees scheduler updates;
+    * `step(..., hparams_dev=block)`: read max_norm and the other values of param_groups[0] from a device tb_hparams
+      block (learner.HPARAMS) instead, so a captured graph follows changes to them; `hparams()` gives those values,
+      checked as the host entry point checks them, and `structure()` the values that choose a kernel or a buffer.
 
     Subclasses name their flat buffers in `_buffers()` (per-parameter state key -> buffer or None), set the
     per-parameter "step" entry in `_set_step_entry` and launch their update in `_update`.
@@ -54,7 +58,13 @@ class FusedOptimizer(torch.optim.Optimizer):
     def _set_loaded_step(self, steps):
         raise NotImplementedError
 
-    def _update(self, flat, grad, max_norm, lr_device, stream):
+    def _update(self, flat, grad, max_norm, lr_device, stream, hparams_dev=None):
+        raise NotImplementedError
+
+    def hparams(self):
+        raise NotImplementedError
+
+    def structure(self):
         raise NotImplementedError
 
     def _validate_group(self, group):
@@ -113,8 +123,10 @@ class FusedOptimizer(torch.optim.Optimizer):
             self._point_state_at_flat()
 
     @torch.no_grad()
-    def step(self, closure=None, max_grad_norm=None):
-        """clip_grad_norm_(max_grad_norm) (skipped when None) + the update on the flat buffers."""
+    def step(self, closure=None, max_grad_norm=None, hparams_dev=None):
+        """clip_grad_norm_(max_grad_norm) (skipped when None) + the update on the flat buffers.  With `hparams_dev` (a
+        device tb_hparams block) the kernel reads max_norm and the optimizer's values from it when it runs; the
+        structural values (`structure()`) still come from param_groups[0]."""
         if closure is not None:
             raise _lib.TorchBeastB200Error("closure is not supported")
         flat, grad = self.model.flat_params, self.model.attach_grads()
@@ -122,7 +134,7 @@ class FusedOptimizer(torch.optim.Optimizer):
         _lib.check(_lib.lib().tb_grad_sumsq_f32(p(grad), grad.numel(), p(self._sumsq), p(_lib.workspace()), st),
                    "tb_grad_sumsq_f32")
         self._update(flat, grad, -1.0 if max_grad_norm is None else float(max_grad_norm),
-                     p(self._lr_dev) if self.lr_from_device else None, st)
+                     p(self._lr_dev) if self.lr_from_device else None, st, hparams_dev)
         return None
 
     def sync_lr_to_device(self):
@@ -167,10 +179,44 @@ class RMSprop(FusedOptimizer):
         super().restore(snapshot[0])
         self._steps = snapshot[1]
 
-    def _update(self, flat, grad, max_norm, lr_device, stream):
+    def _entry(self):
+        """The host entry point of the current configuration: the default kernel, or the one with the options."""
+        if self.grad_avg is None and self.param_groups[0]["weight_decay"] == 0:
+            return "tb_clip_rmsprop_step_f32"
+        return "tb_clip_rmsprop_ex_step_f32"
+
+    def _momentum_on(self):
+        # the host entry points compare the float argument: a momentum that rounds to 0.0f passes no buffer
+        return bool(np.float32(self.param_groups[0]["momentum"]) != 0)
+
+    def hparams(self):
+        group = self.param_groups[0]
+        if self._momentum_on() and self.momentum_buffer is None:
+            raise _lib.TorchBeastB200Error("%s failed (1): %s: momentum needs a buffer" % (self._entry(), self._entry()))
+        return dict(alpha=group["alpha"], eps=group["eps"], momentum=group["momentum"],
+                    weight_decay=group["weight_decay"])
+
+    def structure(self):
+        return ("rmsprop", self.grad_avg is not None, self.param_groups[0]["weight_decay"] != 0, self._momentum_on())
+
+    def _update(self, flat, grad, max_norm, lr_device, stream, hparams_dev=None):
         group = self.param_groups[0]
         lib, p = _lib.lib(), _lib.ptr
-        if self.grad_avg is None and group["weight_decay"] == 0:
+        if hparams_dev is not None:
+            mom = self.momentum_buffer if self._momentum_on() else None
+            if self._entry() == "tb_clip_rmsprop_step_f32":
+                _lib.check(
+                    lib.tb_clip_rmsprop_step_hp_f32(
+                        p(flat), p(grad), p(self.square_avg), p(mom), flat.numel(), p(self._sumsq), p(hparams_dev),
+                        lr_device, float(group["lr"]), p(self.grad_norm), stream),
+                    "tb_clip_rmsprop_step_hp_f32")
+            else:
+                _lib.check(
+                    lib.tb_clip_rmsprop_ex_step_hp_f32(
+                        p(flat), p(grad), p(self.square_avg), p(self.grad_avg), p(mom), flat.numel(), p(self._sumsq),
+                        p(hparams_dev), lr_device, float(group["lr"]), p(self.grad_norm), stream),
+                    "tb_clip_rmsprop_ex_step_hp_f32")
+        elif self.grad_avg is None and group["weight_decay"] == 0:
             _lib.check(
                 lib.tb_clip_rmsprop_step_f32(
                     p(flat), p(grad), p(self.square_avg), p(self.momentum_buffer), flat.numel(), p(self._sumsq),
@@ -243,10 +289,29 @@ class Adam(FusedOptimizer):
     def _set_loaded_step(self, steps):
         self.step_device.fill_(steps)
 
-    def _update(self, flat, grad, max_norm, lr_device, stream):
+    def hparams(self):
+        group = self.param_groups[0]
+        beta1, beta2 = (float(b) for b in group["betas"])
+        if not (0.0 <= beta1 < 1.0 and 0.0 <= beta2 < 1.0):
+            raise _lib.TorchBeastB200Error(
+                "tb_clip_adam_step_f32 failed (1): tb_clip_adam_step_f32: betas must be in [0, 1)")
+        return dict(beta1=beta1, beta2=beta2, eps=group["eps"], weight_decay=group["weight_decay"])
+
+    def structure(self):
+        return ("adam", bool(self.param_groups[0]["decoupled_weight_decay"]))
+
+    def _update(self, flat, grad, max_norm, lr_device, stream, hparams_dev=None):
         group = self.param_groups[0]
         beta1, beta2 = group["betas"]
         p = _lib.ptr
+        if hparams_dev is not None:
+            _lib.check(
+                _lib.lib().tb_clip_adam_step_hp_f32(
+                    p(flat), p(grad), p(self.exp_avg), p(self.exp_avg_sq), flat.numel(), p(self._sumsq),
+                    p(hparams_dev), lr_device, float(group["lr"]), int(bool(group["decoupled_weight_decay"])),
+                    p(self.step_device), p(self.grad_norm), stream),
+                "tb_clip_adam_step_hp_f32")
+            return
         _lib.check(
             _lib.lib().tb_clip_adam_step_f32(
                 p(flat), p(grad), p(self.exp_avg), p(self.exp_avg_sq), flat.numel(), p(self._sumsq), max_norm,
