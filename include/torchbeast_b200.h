@@ -126,6 +126,74 @@ int tb_impala_loss_fwd_bwd_hp_f32(const float* behavior_logits, const float* tar
                                   float* grad_logits, float* grad_values, int zero_tail, void* workspace,
                                   void* stream);
 
+/* ---- PopArt value normalisation (van Hasselt et al. 2016; Hessel et al. 2019) -----------
+ * Per task k, statistics mu[k], nu[k] (f64, device; start at 0 and 1) with
+ *   sigma_k = clamp(sqrt(max(nu_k - mu_k^2, 0)), 1e-4, 1e6).
+ * tb_impala_loss_popart_f32: the fused loss block of tb_impala_loss_fwd_bwd_f32 on a normalised value head.
+ *   values [T+1,B,K] f32 = normalised head outputs n, bootstrap row T included; task [T+1,B] i64, row (t,b) uses
+ *   k = task[t*B+b].  1. v = sigma_k * n[k] + mu_k (fp32, mu / sigma rounded once), the bootstrap with its own
+ *   task.  2. V-trace on v as in tb_impala_loss_fwd_bwd_f32: vs, pg_adv stay unnormalised.  3. policy gradient
+ *   -log pi(a) * pg_adv / sigma_k, entropy unchanged.  4. baseline loss baseline_cost * 1/2 ((vs - mu_k)/sigma_k -
+ *   n[k])^2; its gradient goes to column k of grad_values [T+1,B,K], every other column and row T get zero.
+ *   A row whose task id is outside [0, K) adds no loss and gets zero gradient rows (its v is 0 in the V-trace); ids
+ *   are not checked otherwise.  task_sums [3K] f64 out: count, sum vs and sum vs^2 of each task over rows t < T,
+ *   bit-identical from run to run (no atomics).  hp: NULL takes the scalar arguments, else they are read from hp.
+ *   1 <= K <= 64, T >= 1, B >= 1.  Two launches.
+ * tb_popart_update: for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
+ *   first), with beta read from device memory:
+ *     mu'_k = (1 - beta) mu_k + beta * sum vs / count,   nu'_k = (1 - beta) nu_k + beta * sum vs^2 / count
+ *   then rescales value-head row k so that its unnormalised outputs do not change:
+ *     weight[k, :] *= sigma_k / sigma'_k,   bias[k] = (sigma_k * bias[k] + mu_k - mu'_k) / sigma'_k
+ *   weight [K,F] and bias [K] f32 (e.g. inside a flat parameter buffer).  It runs after the optimizer step and does
+ *   not touch optimizer state.  One launch, no host sync; graph-capturable.                                    */
+int tb_impala_loss_popart_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                              const float* rewards, const uint8_t* done, const float* discounts,
+                              const float* values, const int64_t* task, const double* mu, const double* nu,
+                              int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
+                              float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                              const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
+                              float* target_alp, float* losses_out, float* grad_logits, float* grad_values,
+                              double* task_sums, void* workspace, void* stream);
+int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,
+                     float* bias, int64_t F, void* stream);
+/* Nets with num_values (1..64) value outputs, one per task: the tb_atarinet_* / tb_resnet_* entry points of the same
+ * name without _mt are their num_values = 1 case.  Parameter layout: baseline.weight [num_values, F] and
+ * baseline.bias [num_values] in place of [1, F] / [1] (still the last two tensors); baseline / grad_baseline are
+ * [T1, B, num_values].  Workspace sizes and tb_atarinet_grad_split do not depend on num_values.                */
+int64_t tb_atarinet_param_count_mt(int num_actions, int num_values, int use_lstm);
+int tb_atarinet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const int64_t* last_action,
+                           const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
+                           int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                           float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
+int tb_atarinet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                     const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                     int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                     void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                     float* hN, float* cN, void* stream);
+int tb_atarinet_backward_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                            const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                            int precision, void* workspace, float* grads, void* stream);
+int tb_atarinet_backward_phase_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                                  const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                  int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream);
+int64_t tb_resnet_param_count_mt(int num_actions, int num_values, int use_lstm);
+int tb_resnet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
+                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                         int precision, void* workspace, float* policy_logits, float* baseline, float* hN, float* cN,
+                         void* stream);
+int tb_resnet_backward_mt(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
+                          const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                          int precision, void* workspace, float* grads, void* stream);
+int tb_resnet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                   const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
+                                   int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                                   void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
+                                   void* stream);
+int tb_resnet_backward_unstacked_mt(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
+                                    const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
+                                    int num_values, int use_lstm, int precision, void* workspace, float* grads,
+                                    void* stream);
+
 /* ---- seeded action sampling for the acting forward ------------------------------------ */
 
 /* monobeast.py:618-619 / polybeast_learner.py:256-257  torch.multinomial(F.softmax(policy_logits, dim=1), 1) as a

@@ -31,6 +31,19 @@ _SIGNATURES = {
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 8 + [_int, _vp, _vp], _int),
     "tb_hparams_layout": ([_vp], _int),
     "tb_impala_loss_fwd_bwd_hp_f32": ([_vp] * 8 + [_i64, _i64, _i64] + [_vp] * 9 + [_int, _vp, _vp], _int),
+    "tb_impala_loss_popart_f32": (
+        [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 12, _int),
+    "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
+    "tb_atarinet_param_count_mt": ([_int, _int, _int], _i64),
+    "tb_atarinet_forward_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
+    "tb_atarinet_forward_unstacked_mt": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_atarinet_backward_mt": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_atarinet_backward_phase_mt": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
+    "tb_resnet_param_count_mt": ([_int, _int, _int], _i64),
+    "tb_resnet_forward_mt": ([_vp] * 6 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
+    "tb_resnet_backward_mt": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_resnet_forward_unstacked_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_resnet_backward_unstacked_mt": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f32": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),

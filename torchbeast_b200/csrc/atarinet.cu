@@ -54,7 +54,7 @@ struct AtariParams {  // offsets (in floats) into the flat parameter / gradient 
   int core;  // 512 + 1 + A
 };
 
-static AtariParams atari_params(int A, int use_lstm) {
+static AtariParams atari_params(int A, int use_lstm, int V = 1) {  // V: value outputs
   using G = AtariGeom;
   AtariParams p;
   int64_t o = 0;
@@ -74,7 +74,7 @@ static AtariParams atari_params(int A, int use_lstm) {
     }
   }
   p.policy_w = take(int64_t(A) * p.core); p.policy_b = take(A);
-  p.baseline_w = take(p.core); p.baseline_b = take(1);
+  p.baseline_w = take(int64_t(V) * p.core); p.baseline_b = take(V);
   p.total = o;
   return p;
 }
@@ -163,10 +163,10 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
 static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                             const int64_t* last_action, const float* h0, const float* c0, const float* P,
                             int64_t T1, int64_t B, int A, int use_lstm, int precision, void* workspace,
-                            float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st) {
+                            float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1) {
   using G = AtariGeom;
   const int64_t N = T1 * B;
-  const AtariParams pp = atari_params(A, use_lstm);
+  const AtariParams pp = atari_params(A, use_lstm, V);
   AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision);
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
@@ -236,7 +236,7 @@ static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const flo
   }
   // heads (fused skinny kernel: one pass over core_out for all A+1 outputs)
   TB_TRY(heads_forward(w.core_out, pp.core, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N, pp.core,
-                       A, policy_logits, baseline, st));
+                       A, policy_logits, baseline, st, V));
   return 0;
 }
 
@@ -329,19 +329,19 @@ static int atarinet_backward_trunk_bf16(const float* P, float* G_, const AtariPa
 // LSTM + heads slice (17 of 24 MB) while the trunk backward is still running (SURVEY 8(e) G1: bucket order = reverse of forward).
 static int atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
                              const float* P, int64_t T1, int64_t B, int A, int use_lstm, int precision,
-                             void* workspace, float* G_, cudaStream_t st, int phases = 3) {
+                             void* workspace, float* G_, cudaStream_t st, int phases = 3, int V = 1) {
   using G = AtariGeom;
   const int64_t N = T1 * B;
-  const AtariParams pp = atari_params(A, use_lstm);
+  const AtariParams pp = atari_params(A, use_lstm, V);
   AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision);
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
   if (phases & 1) {
   // heads: dcore_out = dlogits . Wp + dbaseline . Wb ; dWp, dbp, dWb, dbb
-  TB_REQUIRE(heads_scratch_floats(N, pp.core, A) <= kSplitKScratchFloats, "atarinet_backward: heads scratch too small");
+  TB_REQUIRE(heads_scratch_floats(N, pp.core, A, V) <= kSplitKScratchFloats, "atarinet_backward: heads scratch too small");
   TB_TRY(heads_backward(w.core_out, pp.core, P + pp.policy_w, P + pp.baseline_w, grad_logits, grad_baseline, N, pp.core, A,
                         w.dcore_out, pp.core, G_ + pp.policy_w, G_ + pp.policy_b, G_ + pp.baseline_w, G_ + pp.baseline_b, w.splitk,
-                        st));
+                        st, V));
   }
   if (use_lstm && (phases & 1)) {
     LstmParams lp; LstmGrads lg;
@@ -402,6 +402,10 @@ int64_t tb_atarinet_param_count(int num_actions, int use_lstm) {
   return atari_params(num_actions, use_lstm).total;
 }
 
+int64_t tb_atarinet_param_count_mt(int num_actions, int num_values, int use_lstm) {
+  return atari_params(num_actions, use_lstm, num_values).total;
+}
+
 int64_t tb_atarinet_grad_split(int num_actions, int use_lstm) {
   const AtariParams pp = atari_params(num_actions, use_lstm);
   return use_lstm ? pp.lstm[0][0] : pp.policy_w;  // first parameter after fc.bias
@@ -410,13 +414,21 @@ int64_t tb_atarinet_grad_split(int num_actions, int use_lstm) {
 int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_baseline, const float* notdone,
                                const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
                                void* workspace, float* grads, int phase, void* stream) {
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_backward_phase: bad sizes");
+  return tb_atarinet_backward_phase_mt(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm,
+                                       precision, workspace, grads, phase, stream);
+}
+
+int tb_atarinet_backward_phase_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                                  const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                  int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream) {
+  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1 && num_values >= 1 && num_values <= kHeadsMaxValues,
+             "atarinet_backward_phase: bad sizes");
   TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "atarinet_backward_phase: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "atarinet_backward_phase: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_backward_phase: precision must be 0, 1 or 2");
   TB_REQUIRE(phase == 1 || phase == 2, "atarinet_backward_phase: phase must be 1 (heads + LSTM) or 2 (conv/fc trunk)");
   return atarinet_backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, precision, workspace,
-                           grads, (cudaStream_t)stream, phase);
+                           grads, (cudaStream_t)stream, phase, num_values);
 }
 
 size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
@@ -427,6 +439,16 @@ int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* 
                         const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
                         int num_actions, int use_lstm, int precision, void* workspace, float* policy_logits,
                         float* baseline, float* hN, float* cN, void* stream) {
+  return tb_atarinet_forward_mt(frame, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, 1, use_lstm,
+                                precision, workspace, policy_logits, baseline, hN, cN, stream);
+}
+
+int tb_atarinet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const int64_t* last_action,
+                           const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
+                           int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                           float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward: num_values %d outside [1, %d]",
+             num_values, kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward: bad sizes T1=%lld B=%lld A=%d", (long long)T1,
              (long long)B, num_actions);
   TB_REQUIRE(frame && reward && last_action && params && workspace && policy_logits && baseline,
@@ -435,7 +457,7 @@ int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* 
   TB_REQUIRE(precision >= 0 && precision <= 2,
              "atarinet_forward: precision must be 0 (fp32 SIMT), 1 (bf16 tensor cores) or 2 (split-bf16 tensor cores)");
   return atarinet_forward(frame, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
-                          workspace, policy_logits, baseline, hN, cN, (cudaStream_t)stream);
+                          workspace, policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
 }
 
 int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
@@ -443,6 +465,18 @@ int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, co
                                   int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
                                   void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
                                   void* stream) {
+  return tb_atarinet_forward_unstacked_mt(frames, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, 1,
+                                          use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN, cN,
+                                          stream);
+}
+
+int tb_atarinet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                     const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                     int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                     void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                     float* hN, float* cN, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward_unstacked: num_values %d outside [1, %d]",
+             num_values, kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward_unstacked: bad sizes T1=%lld B=%lld A=%d",
              (long long)T1, (long long)B, num_actions);
   TB_REQUIRE(frames && done && reward && last_action && params && workspace && policy_logits && baseline,
@@ -452,24 +486,32 @@ int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, co
   cudaStream_t st = (cudaStream_t)stream;
   if (precision)  // fused: the frame-image pass reads the unstacked rows
     return atarinet_forward(frames, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
-                            precision, workspace, policy_logits, baseline, hN, cN, st);
+                            precision, workspace, policy_logits, baseline, hN, cN, st, num_values);
   TB_REQUIRE(stacked_scratch, "atarinet_forward_unstacked: the fp32 backend needs stacked_scratch "
                               "(tb_unstacked_scratch_bytes bytes)");
   uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
   TB_TRY(restack_frames_u8(frames, done, T1, B, int64_t(AtariGeom::H0) * AtariGeom::W0, stacked, st));
   return atarinet_forward(stacked, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
-                          precision, workspace, policy_logits, baseline, hN, cN, st);
+                          precision, workspace, policy_logits, baseline, hN, cN, st, num_values);
 }
 
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
                          const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
                          void* workspace, float* grads, void* stream) {
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_backward: bad sizes");
+  return tb_atarinet_backward_mt(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision,
+                                 workspace, grads, stream);
+}
+
+int tb_atarinet_backward_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                            const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                            int precision, void* workspace, float* grads, void* stream) {
+  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1 && num_values >= 1 && num_values <= kHeadsMaxValues,
+             "atarinet_backward: bad sizes");
   TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "atarinet_backward: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "atarinet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_backward: precision must be 0, 1 or 2");
   return atarinet_backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, precision, workspace,
-                           grads, (cudaStream_t)stream);
+                           grads, (cudaStream_t)stream, 3, num_values);
 }
 
 }  // extern "C"

@@ -41,7 +41,7 @@ struct ResParams {
   int core_in, core_out;
 };
 
-ResParams res_params(int A, int use_lstm) {
+ResParams res_params(int A, int use_lstm, int V = 1) {  // V: value outputs
   ResParams p;
   int64_t o = 0;
   auto take = [&](int64_t n) { int64_t r = o; o += n; return r; };
@@ -61,7 +61,7 @@ ResParams res_params(int A, int use_lstm) {
     p.lstm[2] = take(4 * kLstmH); p.lstm[3] = take(4 * kLstmH);
   }
   p.policy_w = take(int64_t(A) * p.core_out); p.policy_b = take(A);
-  p.baseline_w = take(p.core_out); p.baseline_b = take(1);
+  p.baseline_w = take(int64_t(V) * p.core_out); p.baseline_b = take(V);
   p.total = o;
   return p;
 }
@@ -254,9 +254,9 @@ struct Impl {
 
   static int forward(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
                      const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* policy_logits,
-                     float* baseline, float* hN, float* cN, cudaStream_t st) {
+                     float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1) {
     const int64_t N = T1 * B;
-    const ResParams pp = res_params(A, use_lstm);
+    const ResParams pp = res_params(A, use_lstm, V);
     ResWs<T> w = res_ws<T>(workspace, N, T1, B, A, use_lstm);
     // weight pack: [o, c, kh, kw] -> [o, (kh,kw), c]; first conv keeps (c,kh,kw); fc: [o, c, (h,w)] -> [o, (h,w), c]
     TB_TRY(pack_w(P + pp.feat[0].w, w.wfeat[0], kSecCh[0], 1, 36, ldk_of(4, kBf16), st));
@@ -305,7 +305,7 @@ struct Impl {
                           st));
     }
     TB_TRY(heads_forward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N,
-                         pp.core_out, A, policy_logits, baseline, st));
+                         pp.core_out, A, policy_logits, baseline, st, V));
     return 0;
   }
 
@@ -325,14 +325,16 @@ struct Impl {
   }
 
   static int backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                      const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st) {
+                      const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st,
+                      int V = 1) {
     const int64_t N = T1 * B;
-    const ResParams pp = res_params(A, use_lstm);
+    const ResParams pp = res_params(A, use_lstm, V);
     ResWs<T> w = res_ws<T>(workspace, N, T1, B, A, use_lstm);
     // heads
+    TB_REQUIRE(heads_scratch_floats(N, pp.core_out, A, V) <= w.splitk_floats, "resnet_backward: heads scratch too small");
     TB_TRY(heads_backward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.baseline_w, grad_logits, grad_baseline, N, pp.core_out,
                           A, w.dcore_out, pp.core_out, G + pp.policy_w, G + pp.policy_b, G + pp.baseline_w, G + pp.baseline_b,
-                          w.splitk, st));
+                          w.splitk, st, V));
     if (use_lstm) {
       LstmParams lp; LstmGrads lg;
       lp.w_ih[0] = P + pp.lstm[0]; lp.w_hh[0] = P + pp.lstm[1]; lp.b_ih[0] = P + pp.lstm[2]; lp.b_hh[0] = P + pp.lstm[3];
@@ -413,9 +415,9 @@ struct SplitImpl {
   // pass that writes the first conv's input image
   static int forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone, const float* h0,
                      const float* c0, const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace,
-                     float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st) {
+                     float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1) {
     const int64_t N = T1 * B;
-    const ResParams pp = res_params(A, use_lstm);
+    const ResParams pp = res_params(A, use_lstm, V);
     W w = res_ws<float>(workspace, N, T1, B, A, use_lstm, true);
     TB_TRY(pack_weights_bf16(P + pp.fc_w, w.wb_fc, kFcOut, 121, 32, kFcIn, st, w.wb_fc_lo));
     for (int i = 0; i < kSections; ++i) {
@@ -459,7 +461,7 @@ struct SplitImpl {
       TB_TRY(lstm_forward(w.core_in, notdone, h0, c0, lp, T1, B, pp.core_in, kLstmH, 1, w.lstm, w.core_out, hN, cN, 2, st));
     }
     TB_TRY(heads_forward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.policy_b, P + pp.baseline_w, P + pp.baseline_b, N,
-                         pp.core_out, A, policy_logits, baseline, st));
+                         pp.core_out, A, policy_logits, baseline, st, V));
     return 0;
   }
 
@@ -491,13 +493,14 @@ struct SplitImpl {
 
   // reads no frames: the first conv's weight gradient uses the input image the forward left in the workspace
   static int backward(const float* grad_logits, const float* grad_baseline, const float* notdone, const float* P, int64_t T1,
-                      int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st) {
+                      int64_t B, int A, int use_lstm, void* workspace, float* G, cudaStream_t st, int V = 1) {
     const int64_t N = T1 * B;
-    const ResParams pp = res_params(A, use_lstm);
+    const ResParams pp = res_params(A, use_lstm, V);
     W w = res_ws<float>(workspace, N, T1, B, A, use_lstm, true);
+    TB_REQUIRE(heads_scratch_floats(N, pp.core_out, A, V) <= w.splitk_floats, "resnet_backward: heads scratch too small");
     TB_TRY(heads_backward(w.core_out, pp.core_out, P + pp.policy_w, P + pp.baseline_w, grad_logits, grad_baseline, N, pp.core_out,
                           A, w.dcore_out, pp.core_out, G + pp.policy_w, G + pp.policy_b, G + pp.baseline_w, G + pp.baseline_b,
-                          w.splitk, st));
+                          w.splitk, st, V));
     if (use_lstm) {
       LstmParams lp; LstmGrads lg;
       lp.w_ih[0] = P + pp.lstm[0]; lp.w_hh[0] = P + pp.lstm[1]; lp.b_ih[0] = P + pp.lstm[2]; lp.b_hh[0] = P + pp.lstm[3];
@@ -566,50 +569,83 @@ extern "C" {
 
 int64_t tb_resnet_param_count(int num_actions, int use_lstm) { return res_params(num_actions, use_lstm).total; }
 
+
+int64_t tb_resnet_param_count_mt(int num_actions, int num_values, int use_lstm) {
+  return res_params(num_actions, use_lstm, num_values).total;
+}
+
 size_t tb_resnet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
   if (precision == 2) return res_ws<float>(nullptr, T1 * B, T1, B, num_actions, use_lstm, true).bytes;
   return precision ? res_ws<__nv_bfloat16>(nullptr, T1 * B, T1, B, num_actions, use_lstm).bytes
                    : res_ws<float>(nullptr, T1 * B, T1, B, num_actions, use_lstm).bytes;
 }
 
+
 int tb_resnet_forward(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
                       const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
                       float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
+  return tb_resnet_forward_mt(frame, reward, notdone, h0, c0, params, T1, B, num_actions, 1, use_lstm, precision, workspace, policy_logits, baseline, hN, cN, stream);
+}
+
+int tb_resnet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
+                      const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                      float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_forward: num_values %d outside [1, %d]", num_values,
+             kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward: bad sizes");
   TB_REQUIRE(frame && reward && params && workspace && policy_logits && baseline, "resnet_forward: null pointer");
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
   if (precision == 2)
     return SplitImpl::forward(frame, nullptr, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                              policy_logits, baseline, hN, cN, (cudaStream_t)stream);
+                              policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
   if (precision)
     return Impl<__nv_bfloat16>::forward(frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                                        policy_logits, baseline, hN, cN, (cudaStream_t)stream);
+                                        policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
   return Impl<float>::forward(frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace, policy_logits,
-                              baseline, hN, cN, (cudaStream_t)stream);
+                              baseline, hN, cN, (cudaStream_t)stream, num_values);
 }
+
 
 int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
                        const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
                        void* workspace, float* grads, void* stream) {
+  return tb_resnet_backward_mt(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision, workspace, grads, stream);
+}
+
+int tb_resnet_backward_mt(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
+                       const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                       void* workspace, float* grads, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_backward: num_values %d outside [1, %d]", num_values,
+             kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward: bad sizes");
   TB_REQUIRE(frame && grad_logits && grad_baseline && params && workspace && grads, "resnet_backward: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "resnet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward: precision must be 0, 1 or 2");
   if (precision == 2)
     return SplitImpl::backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads,
-                               (cudaStream_t)stream);
+                               (cudaStream_t)stream, num_values);
   if (precision)
     return Impl<__nv_bfloat16>::backward(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm,
-                                         workspace, grads, (cudaStream_t)stream);
+                                         workspace, grads, (cudaStream_t)stream, num_values);
   return Impl<float>::backward(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
-                               grads, (cudaStream_t)stream);
+                               grads, (cudaStream_t)stream, num_values);
 }
+
 
 int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
                                 const float* h0, const float* c0, const float* params, int64_t T1, int64_t B, int num_actions,
                                 int use_lstm, int precision, void* workspace, void* stacked_scratch, float* policy_logits,
                                 float* baseline, float* hN, float* cN, void* stream) {
+  return tb_resnet_forward_unstacked_mt(frames, done, reward, notdone, h0, c0, params, T1, B, num_actions, 1, use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN, cN, stream);
+}
+
+int tb_resnet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
+                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                int use_lstm, int precision, void* workspace, void* stacked_scratch, float* policy_logits,
+                                float* baseline, float* hN, float* cN, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_forward_unstacked: num_values %d outside [1, %d]", num_values,
+             kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward_unstacked: bad sizes");
   TB_REQUIRE(frames && done && reward && params && workspace && policy_logits && baseline,
              "resnet_forward_unstacked: null pointer");
@@ -618,36 +654,45 @@ int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, cons
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == 2)  // fused into the first conv's image pass
     return SplitImpl::forward(frames, done, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                              policy_logits, baseline, hN, cN, st);
+                              policy_logits, baseline, hN, cN, st, num_values);
   TB_REQUIRE(stacked_scratch, "resnet_forward_unstacked: the fp32 / bf16 backends need stacked_scratch "
                               "(tb_unstacked_scratch_bytes bytes)");
   uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
   TB_TRY(restack_frames_u8(frames, done, T1, B, 84 * 84, stacked, st));
   if (precision)
     return Impl<__nv_bfloat16>::forward(stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                                        policy_logits, baseline, hN, cN, st);
+                                        policy_logits, baseline, hN, cN, st, num_values);
   return Impl<float>::forward(stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace, policy_logits,
-                              baseline, hN, cN, st);
+                              baseline, hN, cN, st, num_values);
 }
+
 
 int tb_resnet_backward_unstacked(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
                                  const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
                                  int use_lstm, int precision, void* workspace, float* grads, void* stream) {
+  return tb_resnet_backward_unstacked_mt(stacked_scratch, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision, workspace, grads, stream);
+}
+
+int tb_resnet_backward_unstacked_mt(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
+                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                 int use_lstm, int precision, void* workspace, float* grads, void* stream) {
+  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_backward_unstacked: num_values %d outside [1, %d]", num_values,
+             kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward_unstacked: bad sizes");
   TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "resnet_backward_unstacked: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "resnet_backward_unstacked: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward_unstacked: precision must be 0, 1 or 2");
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == 2)
-    return SplitImpl::backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads, st);
+    return SplitImpl::backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads, st, num_values);
   TB_REQUIRE(stacked_scratch, "resnet_backward_unstacked: the fp32 / bf16 backends re-read the restacked frames from "
                               "stacked_scratch");
   const uint8_t* stacked = static_cast<const uint8_t*>(stacked_scratch);
   if (precision)
     return Impl<__nv_bfloat16>::backward(stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm,
-                                         workspace, grads, st);
+                                         workspace, grads, st, num_values);
   return Impl<float>::backward(stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
-                               grads, st);
+                               grads, st, num_values);
 }
 
 }  // extern "C"

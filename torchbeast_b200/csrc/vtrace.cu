@@ -432,7 +432,18 @@ struct LossArgs {
   void* workspace;
   int wide;  // see ScanArgs
   const tb_hparams* hp;  // nullable: overrides the scalars above when the kernel runs
+  // PopArt (impala_loss_kernel<A, true> only): `values` holds the normalised value head [T+1,B,K] (bootstrap row
+  // included, `bootstrap` unused), row (t,b) uses task[t*B+b]; grad_values is [T+1,B,K]
+  const int64_t* task; const double* pa_mu; const double* pa_nu; int K;
 };
+
+constexpr int kPopArtMaxTasks = 64;
+
+// PopArt sigma of one task from its first and second moments (include/torchbeast_b200.h)
+__host__ __device__ __forceinline__ double popart_sigma(double mu, double nu) {
+  const double s = sqrt(fmax(nu - mu * mu, 0.0));
+  return fmin(fmax(s, 1e-4), 1e6);
+}
 
 // The scalars of a tb_hparams block, with has_clip_* derived as the float-argument entry point derives them.
 __device__ __forceinline__ void load_hparams(LossArgs& p) {
@@ -451,12 +462,29 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
   return p.discounts ? p.discounts[i] : (p.done[i] ? 0.0f : p.discounting);
 }
 
-template <int A>
+// kPopArt: the value input is PopArt-normalised (LossArgs::task / pa_mu / pa_nu / K); the non-PopArt instantiations
+// compile none of that code.
+template <int A, bool kPopArt = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
   if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* sA = reinterpret_cast<float*>(smem_raw);
   float* sB = sA + blockDim.y * kWarp;
+  float* sMu = sB + blockDim.y * kWarp;  // PopArt: per-task mu and sigma in fp32, [K] each
+  float* sSig = sMu + kPopArtMaxTasks;
+  if constexpr (kPopArt) {
+    for (int k = threadIdx.x + threadIdx.y * blockDim.x; k < p.K; k += blockDim.x * blockDim.y) {
+      const double mu = p.pa_mu[k];
+      sMu[k] = float(mu);
+      sSig[k] = float(popart_sigma(mu, p.pa_nu[k]));
+    }
+    __syncthreads();
+  }
+  // PopArt: the unnormalised value of row t of column b (t == T: the bootstrap value); an out-of-range task id reads 0
+  auto pop_value = [&](int64_t t, int64_t b) -> float {
+    const int64_t k = p.task[t * p.B + b];
+    return (k >= 0 && k < p.K) ? sSig[k] * p.values[(t * p.B + b) * p.K + k] + sMu[k] : 0.0f;
+  };
   const int lane = threadIdx.x;
   const int w = p.wide ? 0 : threadIdx.y, W = p.wide ? 1 : blockDim.y;
   const int64_t T = p.T, B = p.B;
@@ -476,7 +504,7 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
     if (W > 1) {
       float a = 1.0f, bb = 0.0f;
       if (active && t1 > t0) {
-        float v_next = (t1 < T) ? p.values[t1 * B + b] : p.bootstrap[b];
+        float v_next = kPopArt ? pop_value(t1, b) : (t1 < T) ? p.values[t1 * B + b] : p.bootstrap[b];
         for (int64_t t = t1 - 1; t >= t0; --t) {
           const int64_t i = t * B + b;
           const int64_t act = p.actions[i];
@@ -485,7 +513,7 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
           const float lr = tlp - blp;
           p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
           const float rho = expf(lr);
-          const float g = discount_of(p, i), r = reward_of(p, i), v = p.values[i];
+          const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
           const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
           const float delta = rb * (r + g * v_next - v);
           const float dc = g * fminf(rho, 1.0f);
@@ -502,12 +530,18 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
     }
     if (!active) continue;
     if (p.zero_tail && w == 0) {  // bootstrap row of the learner outputs gets no gradient
-      if (p.grad_values) p.grad_values[T * B + b] = 0.0f;
+      if (p.grad_values) {
+        if constexpr (kPopArt) {
+          for (int j = 0; j < p.K; ++j) p.grad_values[(T * B + b) * p.K + j] = 0.0f;
+        } else {
+          p.grad_values[T * B + b] = 0.0f;
+        }
+      }
       if (p.grad_logits)
         for (int64_t j = 0; j < Ause; ++j) p.grad_logits[(T * B + b) * Ause + j] = 0.0f;
     }
     if (t1 <= t0) continue;
-    float v_next = (t1 < T) ? p.values[t1 * B + b] : p.bootstrap[b];
+    float v_next = kPopArt ? pop_value(t1, b) : (t1 < T) ? p.values[t1 * B + b] : p.bootstrap[b];
     float vs_next = (t1 < T) ? acc_in + v_next : v_next;
     float acc = acc_in;
     for (int64_t t = t1 - 1; t >= t0; --t) {
@@ -525,19 +559,35 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
       }
       const float rho = expf(lr);
-      const float g = discount_of(p, i), r = reward_of(p, i), v = p.values[i];
+      const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
       const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
       const float rp = p.has_clip_pg ? fminf(rho, p.clip_pg) : rho;
       const float delta = rb * (r + g * v_next - v);
       acc = delta + (g * fminf(rho, 1.0f)) * acc;
       const float vst = acc + v;
-      const float adv = rp * (r + g * vs_next - v);
+      float adv = rp * (r + g * vs_next - v);
       p.vs[i] = vst;
       p.pg_adv[i] = adv;
       vs_next = vst;
       v_next = v;
       // losses (monobeast.py:107-125) and closed-form backward (SURVEY 8(a) A4)
-      const float d = vst - v;
+      float d;
+      if constexpr (kPopArt) {
+        // normalised space: the policy gradient scales by 1/sigma_k, the baseline regresses n_k onto (vs - mu_k)/sigma_k;
+        // a row of an out-of-range task adds no loss and gets zero gradient rows
+        const int64_t k = p.task[i];
+        if (k < 0 || k >= p.K) {
+          if (p.grad_logits)
+            for (int64_t j = 0; j < Ause; ++j) p.grad_logits[i * Ause + j] = 0.0f;
+          if (p.grad_values)
+            for (int j = 0; j < p.K; ++j) p.grad_values[i * p.K + j] = 0.0f;
+          continue;
+        }
+        adv = adv / sSig[k];
+        d = (vst - sMu[k]) / sSig[k] - p.values[i * p.K + k];
+      } else {
+        d = vst - v;
+      }
       s_pg += double(-tlp * adv);
       s_bl += 0.5 * double(d * d);
       float ent_row = 0.0f;
@@ -567,7 +617,14 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         }
       }
       s_en += double(ent_row);
-      if (p.grad_values) p.grad_values[i] = -p.baseline_cost * d;
+      if (p.grad_values) {
+        if constexpr (kPopArt) {
+          const int64_t k = p.task[i];
+          for (int j = 0; j < p.K; ++j) p.grad_values[i * p.K + j] = (j == k) ? -p.baseline_cost * d : 0.0f;
+        } else {
+          p.grad_values[i] = -p.baseline_cost * d;
+        }
+      }
     }
   }
   double tot[3];
@@ -575,6 +632,62 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
     const double pg = tot[0], bl = double(p.baseline_cost) * tot[1], en = double(p.entropy_cost) * tot[2];
     p.losses[0] = float(pg); p.losses[1] = float(bl); p.losses[2] = float(en); p.losses[3] = float(pg + bl + en);
   }
+}
+
+// ----------------------------------------------------------------------------------------
+// PopArt statistics
+// ----------------------------------------------------------------------------------------
+// sums[k] = count, sums[K+k] = sum vs, sums[2K+k] = sum vs^2 over the rows t < T of task k.  CTA k owns task k and
+// walks every row in a fixed pattern (thread j takes rows j, j+256, ...; warps then CTA folded in index order), so the
+// sums are bit-identical from run to run without atomics.  The rows are the loss kernel's vs output, still in L2.
+constexpr int kPopArtStatsThreads = 256;
+__global__ void __launch_bounds__(kPopArtStatsThreads) popart_task_sums_kernel(const float* __restrict__ vs,
+                                                                                const int64_t* __restrict__ task,
+                                                                                int64_t N, int K, double* __restrict__ sums) {
+  __shared__ double sm[kPopArtStatsThreads / kWarp][3];
+  const int k = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double c = 0.0, s = 0.0, s2 = 0.0;
+  for (int64_t i = tid; i < N; i += kPopArtStatsThreads) {
+    if (__ldg(task + i) == k) {
+      const double x = double(__ldg(vs + i));
+      c += 1.0; s += x; s2 += x * x;
+    }
+  }
+  c = warp_sum(c); s = warp_sum(s); s2 = warp_sum(s2);
+  if (lane == 0) { sm[warp][0] = c; sm[warp][1] = s; sm[warp][2] = s2; }
+  __syncthreads();
+  if (tid == 0) {
+    double a = 0.0, b = 0.0, d = 0.0;
+    for (int w = 0; w < kPopArtStatsThreads / kWarp; ++w) { a += sm[w][0]; b += sm[w][1]; d += sm[w][2]; }
+    sums[k] = a; sums[K + k] = b; sums[2 * K + k] = d;
+  }
+}
+
+// Statistics update and output-preserving rescale of the value head, CTA k for task k.  A task without rows keeps
+// its statistics and its head row.
+__global__ void popart_update_kernel(const double* __restrict__ sums, const double* __restrict__ beta, double* mu,
+                                     double* nu, int K, float* __restrict__ weight, float* __restrict__ bias, int64_t F) {
+  __shared__ double s_scale, s_mu, s_mu_new, s_sig, s_sig_new;
+  __shared__ bool s_skip;
+  const int k = blockIdx.x;
+  if (threadIdx.x == 0) {
+    const double n = sums[k];
+    s_skip = !(n > 0.0);
+    if (!s_skip) {
+      const double b = *beta, m = mu[k], v = nu[k];
+      const double m2 = (1.0 - b) * m + b * (sums[K + k] / n);
+      const double v2 = (1.0 - b) * v + b * (sums[2 * K + k] / n);
+      s_mu = m; s_mu_new = m2;
+      s_sig = popart_sigma(m, v); s_sig_new = popart_sigma(m2, v2);
+      s_scale = s_sig / s_sig_new;
+      mu[k] = m2; nu[k] = v2;
+    }
+  }
+  __syncthreads();
+  if (s_skip) return;
+  float* row = weight + int64_t(k) * F;
+  for (int64_t f = threadIdx.x; f < F; f += blockDim.x) row[f] = float(double(row[f]) * s_scale);
+  if (threadIdx.x == 0) bias[k] = float((s_sig * double(bias[k]) + s_mu - s_mu_new) / s_sig_new);
 }
 
 // ----------------------------------------------------------------------------------------
@@ -645,7 +758,9 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
                               float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
                               float clip_rho, float clip_pg_rho, const tb_hparams* hp, float* vs, float* pg_adv,
                               float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
-                              float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream) {
+                              float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream,
+                              const int64_t* task = nullptr, const double* pa_mu = nullptr,
+                              const double* pa_nu = nullptr, int K = 0, double* task_sums = nullptr) {
   TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
              (long long)B, (long long)A);
   TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
@@ -671,6 +786,7 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   p.losses = losses_out; p.grad_logits = grad_logits; p.grad_values = grad_values; p.zero_tail = zero_tail;
   p.workspace = workspace;
   p.hp = hp;
+  p.task = task; p.pa_mu = pa_mu; p.pa_nu = pa_nu; p.K = K;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
   int W = pick_warps(T, tiles);
   p.wide = (W == 1);
@@ -683,6 +799,14 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   }
   dim3 block(kWarp, W);
   const size_t smem = size_t(2) * W * kWarp * sizeof(float);
+  if (task) {
+    ProfScope prof("impala_loss_popart", (cudaStream_t)stream);
+    const size_t pop_smem = smem + size_t(2) * kPopArtMaxTasks * sizeof(float);
+    TB_DISPATCH_A(A, (impala_loss_kernel<kA, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
+    TB_TRY(check_launch("impala_loss_kernel<popart>"));
+    popart_task_sums_kernel<<<K, kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, K, task_sums);
+    return check_launch("popart_task_sums_kernel");
+  }
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
   TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
   return check_launch("impala_loss_kernel");
@@ -738,6 +862,35 @@ int tb_impala_loss_fwd_bwd_hp_f32(const float* blogits, const float* tlogits, co
   return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A, 0.0f,
                             0.0f, 0.0f, 0, -1.0f, -1.0f, hp, vs, pg_adv, log_rhos, behavior_alp, target_alp,
                             losses_out, grad_logits, grad_values, zero_tail, workspace, stream);
+}
+
+int tb_impala_loss_popart_f32(const float* blogits, const float* tlogits, const int64_t* actions,
+                              const float* rewards, const uint8_t* done, const float* discounts,
+                              const float* values, const int64_t* task, const double* mu, const double* nu,
+                              int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
+                              float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                              const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
+                              float* target_alp, float* losses_out, float* grad_logits, float* grad_values,
+                              double* task_sums, void* workspace, void* stream) {
+  TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
+             (long long)B, (long long)A);
+  TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "impala_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
+             kPopArtMaxTasks);
+  TB_REQUIRE(values && task && mu && nu && task_sums, "impala_loss_popart: null PopArt pointer");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, values, T, B, A, discounting,
+                            baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs, pg_adv, log_rhos,
+                            behavior_alp, target_alp, losses_out, grad_logits, grad_values, 1, workspace, stream, task,
+                            mu, nu, int(K), task_sums);
+}
+
+int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,
+                     float* bias, int64_t F, void* stream) {
+  TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks && F >= 1, "popart_update: bad sizes K=%lld F=%lld", (long long)K,
+             (long long)F);
+  TB_REQUIRE(task_sums && beta && mu && nu && weight && bias, "popart_update: null pointer");
+  ProfScope prof("popart_update", (cudaStream_t)stream);
+  popart_update_kernel<<<unsigned(K), 128, 0, (cudaStream_t)stream>>>(task_sums, beta, mu, nu, int(K), weight, bias, F);
+  return check_launch("popart_update_kernel");
 }
 
 #define TB_LOSS_ENTRY(NAME, F, KERNEL, ARGS_DECL, ARGS_CALL, NEXPR)                                     \

@@ -139,6 +139,103 @@ def impala_loss_fwd_bwd(
     return ImpalaLoss(vs, pg, lr, blp, tlp, losses, gl, gv)
 
 
+@torch.no_grad()
+def impala_loss_popart(
+    behavior_policy_logits,
+    target_policy_logits,
+    actions,
+    rewards,
+    done,
+    values,
+    task,
+    mu,
+    nu,
+    discounting=0.99,
+    baseline_cost=0.5,
+    entropy_cost=0.0006,
+    reward_clipping="abs_one",
+    clip_rho_threshold=1.0,
+    clip_pg_rho_threshold=1.0,
+    hparams_dev=None,
+):
+    """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_popart_f32).
+
+    `values` is the normalised head output n [T+1, B, K] with its bootstrap row, `task` int64 [T+1, B] the task of each
+    of those rows, `mu` / `nu` float64 [K] the statistics.  The V-trace runs on sigma_k * n[k] + mu_k; vs and
+    pg_advantages are unnormalised, the losses and gradients are taken in normalised space, and grad_values is
+    [T+1, B, K].  A row with a task id outside [0, K) adds no loss and gets zero gradient rows.  Returns
+    (ImpalaLoss, task_sums): task_sums float64 [3, K] = per-task count, sum vs, sum vs^2 over rows t < T, the input
+    of popart_update (SUM all-reduce it first when data-parallel)."""
+    tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
+    _lib.require_cuda(*tensors)
+    T, B, A = target_policy_logits.shape
+    K = values.shape[-1]
+    if tuple(values.shape) != (T + 1, B, K) or tuple(task.shape) != (T + 1, B):
+        raise _lib.TorchBeastB200Error("PopArt values must be [T+1, B, K] and task [T+1, B] for T, B = %d, %d; got %r, %r"
+                                       % (T, B, tuple(values.shape), tuple(task.shape)))
+    if mu.dtype != torch.float64 or nu.dtype != torch.float64 or mu.numel() != K or nu.numel() != K:
+        raise _lib.TorchBeastB200Error("PopArt mu / nu must be float64 [%d]" % K)
+    if hparams_dev is None:
+        clip_rewards = _clip_rewards(reward_clipping)
+    else:
+        _lib.require_cuda(hparams_dev)
+        discounting = hparams_field(hparams_dev, "discounting")
+        clip_rewards = 0
+    dev = values.device
+    f32 = torch.float32
+    if done.dtype == torch.bool:
+        dn, disc = done.contiguous().view(torch.uint8), None
+    elif done.dtype == torch.uint8:
+        dn, disc = None, ((~done).to(f32) * discounting).contiguous()  # see impala_loss_fwd_bwd
+    else:
+        raise _lib.TorchBeastB200Error("done must be bool or uint8")
+    outs = [torch.empty((T, B), dtype=f32, device=dev) for _ in range(5)]
+    losses = torch.empty(4, dtype=f32, device=dev)
+    gl = torch.empty((T + 1, B, A), dtype=f32, device=dev)
+    gv = torch.empty((T + 1, B, K), dtype=f32, device=dev)
+    sums = torch.empty((3, K), dtype=torch.float64, device=dev)
+    p = _lib.ptr
+    _lib.check(
+        _lib.lib().tb_impala_loss_popart_f32(
+            p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
+            p(actions.to(torch.int64).contiguous()), p(rewards.to(f32).contiguous()), p(dn), p(disc),
+            p(values.detach().to(f32).contiguous()), p(task.to(torch.int64).contiguous()), p(mu.contiguous()),
+            p(nu.contiguous()), T, B, A, K, float(discounting) if hparams_dev is None else 0.0, float(baseline_cost),
+            float(entropy_cost), clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold),
+            p(hparams_dev), *[p(o) for o in outs], p(losses), p(gl), p(gv), p(sums), p(_lib.workspace()),
+            _lib.stream_ptr()),
+        "tb_impala_loss_popart_f32")
+    return ImpalaLoss(*outs, losses, gl, gv), sums
+
+
+@torch.no_grad()
+def popart_update(task_sums, beta, mu, nu, weight, bias):
+    """PopArt statistics update and output-preserving value-head rescale, in place (tb_popart_update): `beta` is a
+    float64 device scalar, `weight` [K, F] / `bias` [K] the value head (views of the flat parameter buffer)."""
+    _lib.require_cuda(task_sums, beta, mu, nu, weight, bias)
+    K, F = weight.shape
+    for t, dt in ((task_sums, torch.float64), (beta, torch.float64), (mu, torch.float64), (nu, torch.float64),
+                  (weight, torch.float32), (bias, torch.float32)):
+        if t.dtype != dt or not t.is_contiguous():
+            raise _lib.TorchBeastB200Error("popart_update: expected contiguous %s, got %s" % (dt, t.dtype))
+    if task_sums.numel() != 3 * K or mu.numel() != K or nu.numel() != K or bias.numel() != K or beta.numel() != 1:
+        raise _lib.TorchBeastB200Error("popart_update: sizes disagree with weight [%d, %d]" % (K, F))
+    p = _lib.ptr
+    _lib.check(_lib.lib().tb_popart_update(p(task_sums), p(beta), p(mu), p(nu), K, p(weight), p(bias), F,
+                                           _lib.stream_ptr()),
+               "tb_popart_update")
+
+
+def _popart_task(model, batch):
+    """batch["task"] as int64 [T+1, B]; optional (all zeros) for a single-task model."""
+    task = batch.get("task")
+    if task is None:
+        if model.popart.num_tasks > 1:
+            raise _lib.TorchBeastB200Error("a model with num_tasks > 1 needs batch['task']")
+        return torch.zeros(batch["reward"].shape[:2], dtype=torch.int64, device=batch["reward"].device)
+    return task.to(torch.int64)
+
+
 def _dp_world():
     import torch.distributed as dist
     if dist.is_available() and dist.is_initialized():
@@ -217,8 +314,21 @@ def optimizer_step(model, optimizer, max_grad_norm, hparams_dev=None):
         optimizer.step()
 
 
+DEFAULT_POPART_BETA = 3e-4
+
+
+def popart_beta(flags):
+    return float(getattr(flags, "popart_beta", DEFAULT_POPART_BETA))
+
+
+def _popart_stats(mu, nu):
+    """The stats-dict entries of a PopArt model from host copies of its statistics."""
+    sigma = [float(min(max(max(n - m * m, 0.0) ** 0.5, 1e-4), 1e6)) for m, n in zip(mu.tolist(), nu.tolist())]
+    return {"popart_mu": mu.tolist(), "popart_sigma": sigma}
+
+
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
-               behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None):
+               behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -226,17 +336,41 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
       backward into the flat gradient -> [NCCL all-reduce] -> fused clip + optimizer step -> actor copy.
     With `hparams_dev` (GraphedLearner's device tb_hparams block) the loss and the optimizer read the values of
     `flags` and of the optimizer's param group from the block, not from the host.
+
+    A model built with `num_tasks` (PopArt, model.popart) runs the PopArt loss instead (impala_loss_popart, one more
+    launch for the per-task sums), SUM all-reduces the sums when data-parallel, and after the optimizer step updates the
+    statistics and rescales the value head (popart_update) before the actor copy.  beta is `popart_beta_dev` (a float64
+    device scalar, GraphedLearner's) or flags.popart_beta.
     """
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
     acts = batch["action"] if actions is None else actions
-    loss = impala_loss_fwd_bwd(
-        blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
-        out.baseline[:-1], out.baseline[-1],
-        discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
-        reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
-    _backward_with_overlapped_all_reduce(model, loss.grad_logits, loss.grad_values)
+    pop = getattr(model, "popart", None)
+    if pop is None:
+        loss = impala_loss_fwd_bwd(
+            blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
+            out.baseline[:-1], out.baseline[-1],
+            discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
+            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
+        grad_values = loss.grad_values
+    else:
+        values = out.baseline.reshape(out.baseline.shape[:2] + (pop.num_tasks,))
+        loss, task_sums = impala_loss_popart(
+            blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:], values,
+            _popart_task(model, batch), pop.mu, pop.nu,
+            discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
+            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
+        grad_values = loss.grad_values.view(out.baseline.shape)
+    _backward_with_overlapped_all_reduce(model, loss.grad_logits, grad_values)
     optimizer_step(model, optimizer, flags.grad_norm_clipping, hparams_dev=hparams_dev)
+    if pop is not None:
+        if _dp_world() > 1:
+            import torch.distributed as dist
+            dist.all_reduce(task_sums, op=dist.ReduceOp.SUM)  # every rank applies the global batch's update
+        if popart_beta_dev is None:
+            popart_beta_dev = torch.full((1,), popart_beta(flags), dtype=torch.float64, device=task_sums.device)
+        weight, bias = model.value_head()
+        popart_update(task_sums, popart_beta_dev, pop.mu, pop.nu, weight, bias)
     if scheduler is not None:
         scheduler.step()
     if actor_model is not None and actor_model is not model:
@@ -250,7 +384,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     episode_returns = batch["episode_return"][1:][done.bool()]
     host = loss.losses.cpu()  # the step's one blocking read-back
     ep = episode_returns.cpu()
-    return {
+    stats = {
         "episode_returns": tuple(ep.numpy()),
         "mean_episode_return": torch.mean(ep).item(),
         "total_loss": host[3].item(),
@@ -258,6 +392,9 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         "baseline_loss": host[1].item(),
         "entropy_loss": host[2].item(),
     }
+    if pop is not None:
+        stats.update(_popart_stats(pop.mu.cpu(), pop.nu.cpu()))
+    return stats
 
 
 def _graph_enabled(flags):
@@ -388,7 +525,7 @@ class GraphedLearner:
     publishes before every replay, so they may change between steps without a new capture.  The values that choose a
     kernel or a buffer (`structure`) are fixed per graph; learn() captures another graph when one of them changes."""
 
-    KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return")
+    KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return", "task")
 
     @staticmethod
     def structure_of(optimizer, batch):
@@ -402,6 +539,12 @@ class GraphedLearner:
         self.structure = self.structure_of(optimizer, example_batch)
         self.hparams = torch.zeros(HPARAMS.itemsize, dtype=torch.uint8, device=model.flat_params.device)
         publish_hparams(pack_hparams(flags, optimizer), self.hparams)
+        # PopArt: beta is a device scalar published before every replay, like the tb_hparams block
+        self.popart = getattr(model, "popart", None)
+        self.popart_beta = None
+        if self.popart is not None:
+            self.popart_beta = torch.zeros(1, dtype=torch.float64, device=model.flat_params.device)
+            self._publish_beta(flags)
         self.static = {k: torch.empty_like(v) for k, v in example_batch.items() if k in self.KEYS}
         self.static_state = tuple(torch.empty_like(s) for s in initial_agent_state)
         for k, v in self.static.items():
@@ -411,19 +554,20 @@ class GraphedLearner:
         optimizer.lr_from_device = True
         optimizer.sync_lr_to_device()
         # warm up on a side stream (allocations, one-time attribute calls), then capture
-        snapshot = (model.flat_params.clone(), optimizer.snapshot())
+        snapshot = (model.flat_params.clone(), optimizer.snapshot(),
+                    None if self.popart is None else (self.popart.mu.clone(), self.popart.nu.clone()))
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
                 learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None, stats_sync=False,
-                           hparams_dev=self.hparams)
+                           hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.out = learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None,
-                                  stats_sync=False, hparams_dev=self.hparams)
+                                  stats_sync=False, hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
         # the graph writes into the model workspace it was captured with; the model replaces (and frees) that buffer when
         # it runs another shape, e.g. while the GraphedLearner of another batch shape is captured: keep it alive here
         self.workspace = getattr(model, "_ws", None)
@@ -435,6 +579,9 @@ class GraphedLearner:
         # undo the warm-up / capture-time updates so training starts from the caller's weights
         model.flat_params.copy_(snapshot[0])
         optimizer.restore(snapshot[1])  # state buffers and step count, the device step of Adam included
+        if self.popart is not None:
+            self.popart.mu.copy_(snapshot[2][0])
+            self.popart.nu.copy_(snapshot[2][1])
         if actor_model is not None and hasattr(actor_model, "copy_params_from"):
             actor_model.copy_params_from(model)
 
@@ -447,16 +594,27 @@ class GraphedLearner:
             d.copy_(s, non_blocking=True)
         self.opt.sync_lr_to_device()
         publish_hparams(pack_hparams(self.flags, self.opt) if hparams is None else hparams, self.hparams)
+        if self.popart is not None:
+            self._publish_beta(self.flags)
         self.graph.replay()
         if scheduler is not None:
             scheduler.step()
         return self.out
 
+    def _publish_beta(self, flags):
+        """Enqueue the copy of flags.popart_beta into the device scalar through a fresh pinned buffer (publish_hparams)."""
+        host = torch.full((1,), popart_beta(flags), dtype=torch.float64).pin_memory()
+        self.popart_beta.copy_(host, non_blocking=True)
+
     def snapshot(self):
-        """Device copies of what stats() reads (the step's losses and its done / episode_return rows), enqueued on the
-        current stream: lets the caller release the learner lock BEFORE the blocking read-back, so the next learner
-        thread's replay queues up behind this one instead of waiting for a host round trip."""
-        return (self.out["losses"].clone(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone())
+        """Device copies of what stats() reads (the step's losses and its done / episode_return rows, and a PopArt model's
+        statistics), enqueued on the current stream: lets the caller release the learner lock BEFORE the blocking
+        read-back, so the next learner thread's replay queues up behind this one instead of waiting for a host round
+        trip."""
+        snap = (self.out["losses"].clone(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone())
+        if self.popart is not None:
+            snap += (self.popart.mu.clone(), self.popart.nu.clone())
+        return snap
 
     _tls = threading.local()
 
@@ -465,7 +623,7 @@ class GraphedLearner:
         """Read the snapshot back on a per-thread READ-BACK stream that waits only for `event` (recorded right after the
         snapshot): a read-back on the compute stream would queue behind the NEXT step, which another learner thread has
         already enqueued there."""
-        losses, done, ep_ret = snap
+        losses, done, ep_ret = snap[:3]
         tls = GraphedLearner._tls
         dev = losses.device
         if getattr(tls, "stream", None) is None or tls.device != dev:
@@ -479,22 +637,29 @@ class GraphedLearner:
         with torch.cuda.stream(tls.stream):
             for dst, src in zip(bufs, (losses, done, ep_ret)):
                 dst.copy_(src, non_blocking=True)
+            popart = [s.to("cpu", non_blocking=True) for s in snap[3:]]
         tls.stream.synchronize()
         host, hdone, hret = bufs
         ep = hret[hdone.bool()].clone()
-        return {
+        stats = {
             "episode_returns": tuple(ep.numpy()), "mean_episode_return": torch.mean(ep).item(),
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
+        if popart:
+            stats.update(_popart_stats(*popart))
+        return stats
 
     def stats(self):
         """Same keys as monobeast.learn()'s return value; one blocking read-back."""
         done = self.static["done"][1:]
         ep = self.static["episode_return"][1:][done.bool()].cpu()
         host = self.out["losses"].cpu()
-        return {
+        stats = {
             "episode_returns": tuple(ep.numpy()), "mean_episode_return": torch.mean(ep).item(),
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
+        if self.popart is not None:
+            stats.update(_popart_stats(self.popart.mu.cpu(), self.popart.nu.cpu()))
+        return stats

@@ -21,7 +21,45 @@ class _ParamGroup(nn.Module):
     """Namespace module so parameters get the reference's dotted names (conv1.weight, ...)."""
 
 
-def atarinet_param_spec(num_actions, use_lstm, in_channels=4):
+class PopArt(nn.Module):
+    """PopArt value statistics of a net built with `num_tasks` = K (van Hasselt et al. 2016, Hessel et al. 2019):
+    buffers `mu` and `nu` (float64 [K], first and second moment of each task's V-trace targets; state_dict keys
+    popart.mu and popart.nu) start at 0 and 1.  The net's value head then has K normalised outputs, baseline [T, B, K]:
+    the value of task k is sigma_k * baseline[..., k] + mu_k with sigma_k = clamp(sqrt(nu_k - mu_k^2), 1e-4, 1e6).
+    learn() updates them."""
+
+    MAX_TASKS = 64
+
+    def __init__(self, num_tasks, device):
+        super().__init__()
+        num_tasks = int(num_tasks)
+        if not 1 <= num_tasks <= self.MAX_TASKS:
+            raise _lib.TorchBeastB200Error("num_tasks must be in [1, %d], got %d" % (self.MAX_TASKS, num_tasks))
+        self.num_tasks = num_tasks
+        self.register_buffer("mu", torch.zeros(num_tasks, dtype=torch.float64, device=device))
+        self.register_buffer("nu", torch.ones(num_tasks, dtype=torch.float64, device=device))
+
+    def _apply(self, fn, recurse=True):
+        # the statistics stay float64 through .float() and the like
+        super()._apply(fn, recurse)
+        for key, buf in list(self._buffers.items()):
+            self._buffers[key] = buf.to(torch.float64)
+        return self
+
+    def sigma(self):
+        return (self.nu - self.mu * self.mu).clamp_min(0).sqrt().clamp(1e-4, 1e6)
+
+    def unnormalize(self, baseline, task=None):
+        """The unnormalised value [T, B] (float32) of each row's own task from a normalised `baseline` [T, B, K]; `task`
+        int64 [T, B] (default: task 0; ids must be in [0, K))."""
+        if task is None:
+            task = torch.zeros(baseline.shape[:-1], dtype=torch.int64, device=baseline.device)
+        task = task.to(device=self.mu.device, dtype=torch.int64)
+        n = baseline.to(torch.float64).gather(-1, task.unsqueeze(-1).to(baseline.device)).squeeze(-1)
+        return (self.sigma()[task] * n + self.mu[task]).to(torch.float32)
+
+
+def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
     core = 512 + num_actions + 1
     spec = [
         ("conv1.weight", (32, in_channels, 8, 8)), ("conv1.bias", (32,)),
@@ -37,7 +75,7 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4):
             ]
     spec += [
         ("policy.weight", (num_actions, core)), ("policy.bias", (num_actions,)),
-        ("baseline.weight", (1, core)), ("baseline.bias", (1,)),
+        ("baseline.weight", (num_values, core)), ("baseline.bias", (num_values,)),
     ]
     return spec
 
@@ -102,6 +140,14 @@ class FlatParamModule(nn.Module):
     # the stacked and unstacked frames only.  Not part of the state_dict.
     frame_history = None
 
+    def _baseline_shape(self, T1, B):
+        """[T1, B], or [T1, B, K] for a net with K PopArt tasks."""
+        return (T1, B) if getattr(self, "popart", None) is None else (T1, B, self.num_values)
+
+    def value_head(self):
+        """(baseline.weight [K, F], baseline.bias [K]): the value head's views of the flat parameter buffer."""
+        return self.baseline.weight.data, self.baseline.bias.data
+
     def _forward_frame(self, inputs):
         """inputs["frame"], or, with a frame_history attached and newest frames [T, B, 84, 84] (T = reward's), the
         unstacked rollout [T+3, B, 84, 84] the history builds from them (acting.FrameHistory.stack)."""
@@ -157,6 +203,8 @@ class FlatParamModule(nn.Module):
         for key, buf in list(self._buffers.items()):
             if buf is not None:
                 self._buffers[key] = fn(buf)
+        if getattr(self, "popart", None) is not None:
+            self.popart._apply(fn)
         return self
 
     @property
@@ -184,8 +232,12 @@ class FlatParamModule(nn.Module):
         return fg
 
     def copy_params_from(self, other):
-        """actor_model.load_state_dict(model.state_dict()) as ONE device copy (monobeast.py:295)."""
+        """actor_model.load_state_dict(model.state_dict()) as ONE device copy (monobeast.py:295), plus the PopArt
+        statistics when both nets have them."""
         self._flat.copy_(other._flat, non_blocking=True)
+        if getattr(self, "popart", None) is not None and getattr(other, "popart", None) is not None:
+            self.popart.mu.copy_(other.popart.mu, non_blocking=True)
+            self.popart.nu.copy_(other.popart.nu, non_blocking=True)
 
     def _aliased_sibling(self, state_dict):
         """The FlatParamModule whose live flat buffer EVERY tensor of `state_dict` aliases at this module's own
@@ -211,9 +263,15 @@ class FlatParamModule(nn.Module):
         """Reference checkpoints / state_dicts load key by key; `actor.load_state_dict(model.state_dict())`
         (monobeast.py:295) is recognised by aliasing and becomes ONE device copy.  The dict itself carries nothing
         but tensors, so torch.save / torch.load(weights_only=True) / copy.deepcopy behave as for any nn.Module."""
-        src = self._aliased_sibling(state_dict)
+        stats = ("popart.mu", "popart.nu")
+        has_stats = getattr(self, "popart", None) is not None and all(k in state_dict for k in stats)
+        params = {k: v for k, v in state_dict.items() if k not in stats} if has_stats else state_dict
+        src = self._aliased_sibling(params)
         if src is not None:
             self.copy_params_from(src)
+            if has_stats:  # from any net with the same number of tasks (its statistics may be host tensors)
+                self.popart.mu.copy_(state_dict["popart.mu"])
+                self.popart.nu.copy_(state_dict["popart.nu"])
             return torch.nn.modules.module._IncompatibleKeys([], [])
         return super().load_state_dict(state_dict, strict=strict)
 
@@ -256,11 +314,11 @@ class _AtariNetFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_logits, g_baseline, _ghn, _gcn):
         module = ctx.module
-        T1, B = ctx.shape
+        T1, B = ctx.shape[:2]
         if g_logits is None:
             g_logits = torch.zeros(T1, B, module.num_actions, device=module._flat.device)
         if g_baseline is None:
-            g_baseline = torch.zeros(T1, B, device=module._flat.device)
+            g_baseline = torch.zeros(module._baseline_shape(T1, B), device=module._flat.device)
         grads = torch.empty_like(module._flat)
         module._launch_backward(g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
         outs = tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
@@ -280,7 +338,7 @@ class AtariNet(FlatParamModule):
     DEFAULT_PRECISION = "bf16x3"
     needs_last_action = True  # forward consumes inputs["last_action"] (monobeast.py:593-597); polybeast's Net does not
 
-    def __init__(self, observation_shape, num_actions, use_lstm=False, device=None, precision=None):
+    def __init__(self, observation_shape, num_actions, use_lstm=False, device=None, precision=None, num_tasks=None):
         super().__init__()
         if tuple(observation_shape) != (4, 84, 84):
             raise _lib.TorchBeastB200Error(
@@ -291,8 +349,12 @@ class AtariNet(FlatParamModule):
         self.core_size = 512 + num_actions + 1
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        self._build_flat(atarinet_param_spec(num_actions, use_lstm), device)
+        popart = None if num_tasks is None else PopArt(num_tasks, device)
+        self.num_values = 1 if popart is None else popart.num_tasks
+        self._build_flat(atarinet_param_spec(num_actions, use_lstm, num_values=self.num_values), device)
         self.reset_parameters_like_torch()
+        if popart is not None:
+            self.popart = popart  # registered after the parameters: its keys come last in the state_dict
         if use_lstm:
             self.core.num_layers = 2
             self.core.hidden_size = self.core_size
@@ -304,7 +366,7 @@ class AtariNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_atarinet_param_count(num_actions, int(use_lstm))
+        count = _lib.lib().tb_atarinet_param_count_mt(num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def initial_state(self, batch_size):
@@ -335,7 +397,7 @@ class AtariNet(FlatParamModule):
         reward = reward.to(torch.float32).contiguous()
         last_action = last_action.to(torch.int64).contiguous()
         logits = torch.empty(T1, B, self.num_actions, dtype=torch.float32, device=dev)
-        baseline = torch.empty(T1, B, dtype=torch.float32, device=dev)
+        baseline = torch.empty(self._baseline_shape(T1, B), dtype=torch.float32, device=dev)
         if self.use_lstm:
             hN = torch.empty(2, B, self.core_size, dtype=torch.float32, device=dev)
             cN = torch.empty_like(hN)
@@ -347,37 +409,37 @@ class AtariNet(FlatParamModule):
         p = _lib.ptr
         if unstacked:
             _lib.check(
-                _lib.lib().tb_atarinet_forward_unstacked(
+                _lib.lib().tb_atarinet_forward_unstacked_mt(
                     p(frame), p(done), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
-                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)),
+                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)),
                     p(logits), p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None,
                     _lib.stream_ptr()),
                 "tb_atarinet_forward_unstacked")
             return logits, baseline, hN, cN
         _lib.check(
-            _lib.lib().tb_atarinet_forward(
+            _lib.lib().tb_atarinet_forward_mt(
                 p(frame), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
-                self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(logits), p(baseline),
+                self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_atarinet_forward")
         return logits, baseline, hN, cN
 
     def _launch_backward(self, g_logits, g_baseline, notdone, grads_out, phase=None):
-        T1, B = g_baseline.shape
+        T1, B = g_baseline.shape[:2]
         ws = self._workspace(T1, B)
         p = _lib.ptr
         if phase is None:
             _lib.check(
-                _lib.lib().tb_atarinet_backward(
+                _lib.lib().tb_atarinet_backward_mt(
                     p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out),
+                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out),
                     _lib.stream_ptr()),
                 "tb_atarinet_backward")
         else:
             _lib.check(
-                _lib.lib().tb_atarinet_backward_phase(
+                _lib.lib().tb_atarinet_backward_phase_mt(
                     p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out), int(phase),
+                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out), int(phase),
                     _lib.stream_ptr()),
                 "tb_atarinet_backward_phase")
 
@@ -438,7 +500,7 @@ class AtariNet(FlatParamModule):
         else:
             logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"], h0, c0,
                                                             done)
-        T, B = baseline.shape
+        T, B = baseline.shape[:2]
         if self.training:
             action = self._sample(logits, inputs)
         else:
@@ -449,7 +511,7 @@ class AtariNet(FlatParamModule):
 
 
 
-def resnet_param_spec(num_actions, use_lstm):
+def resnet_param_spec(num_actions, use_lstm, num_values=1):
     """State_dict order/shapes of the reference's polybeast_learner.Net (pl:134-204, BASELINE.md section 5)."""
     spec = []
     cin = 4
@@ -467,7 +529,7 @@ def resnet_param_spec(num_actions, use_lstm):
                  ("core.bias_ih_l0", (1024,)), ("core.bias_hh_l0", (1024,))]
         head_in = 256
     spec += [("policy.weight", (num_actions, head_in)), ("policy.bias", (num_actions,)),
-             ("baseline.weight", (1, head_in)), ("baseline.bias", (1,))]
+             ("baseline.weight", (num_values, head_in)), ("baseline.bias", (num_values,))]
     return spec
 
 
@@ -482,12 +544,12 @@ class _ResNetFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_logits, g_baseline, _ghn, _gcn):
         module = ctx.module
-        T1, B = ctx.shape
+        T1, B = ctx.shape[:2]
         dev = module._flat.device
         if g_logits is None:
             g_logits = torch.zeros(T1, B, module.num_actions, device=dev)
         if g_baseline is None:
-            g_baseline = torch.zeros(T1, B, device=dev)
+            g_baseline = torch.zeros(module._baseline_shape(T1, B), device=dev)
         grads = torch.empty_like(module._flat)
         module._launch_backward(ctx.saved, g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
         return (None,) * 7 + tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
@@ -500,16 +562,20 @@ class ResNet(FlatParamModule):
 
     PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 
-    def __init__(self, num_actions, use_lstm=False, device=None, precision=None):
+    def __init__(self, num_actions, use_lstm=False, device=None, precision=None, num_tasks=None):
         super().__init__()
         import os
         self.num_actions = num_actions
         self.use_lstm = use_lstm
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        self._build_flat(resnet_param_spec(num_actions, use_lstm), device)
+        popart = None if num_tasks is None else PopArt(num_tasks, device)
+        self.num_values = 1 if popart is None else popart.num_tasks
+        self._build_flat(resnet_param_spec(num_actions, use_lstm, num_values=self.num_values), device)
         self._fix_module_names()
         self.reset_parameters_like_torch()
+        if popart is not None:
+            self.popart = popart  # registered after the parameters: its keys come last in the state_dict
         if use_lstm:
             self.core.num_layers, self.core.hidden_size, self.core.input_size = 1, 256, 257
         # patch-matrix GEMMs: "bf16x3" (default: split-bf16 tensor-core products over fp32 activations, parity-green),
@@ -520,7 +586,7 @@ class ResNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_resnet_param_count(num_actions, int(use_lstm))
+        count = _lib.lib().tb_resnet_param_count_mt(num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def _fix_module_names(self):
@@ -553,7 +619,7 @@ class ResNet(FlatParamModule):
         frame = frame.contiguous()
         reward = reward.to(torch.float32).contiguous()
         logits = torch.empty(T1, B, self.num_actions, dtype=torch.float32, device=dev)
-        baseline = torch.empty(T1, B, dtype=torch.float32, device=dev)
+        baseline = torch.empty(self._baseline_shape(T1, B), dtype=torch.float32, device=dev)
         if self.use_lstm:
             hN = torch.empty(1, B, 256, dtype=torch.float32, device=dev)
             cN = torch.empty_like(hN)
@@ -565,36 +631,37 @@ class ResNet(FlatParamModule):
         if unstacked:
             scratch = _scratch(self, 1, T1, B)
             _lib.check(
-                _lib.lib().tb_resnet_forward_unstacked(
+                _lib.lib().tb_resnet_forward_unstacked_mt(
                     p(frame), p(done), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions,
-                    int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(scratch), p(logits),
+                    self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(scratch), p(logits),
                     p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
                 "tb_resnet_forward_unstacked")
             return logits, baseline, hN, cN, ("unstacked", scratch)
         _lib.check(
-            _lib.lib().tb_resnet_forward(
-                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions, int(self.use_lstm),
+            _lib.lib().tb_resnet_forward_mt(
+                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions, self.num_values,
+                int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_resnet_forward")
         return logits, baseline, hN, cN, frame
 
     def _launch_backward(self, saved, g_logits, g_baseline, notdone, grads_out):
-        T1, B = g_baseline.shape
+        T1, B = g_baseline.shape[:2]
         p = _lib.ptr
         if isinstance(saved, tuple):  # ("unstacked", scratch): the backward reads the workspace (+ the restacked scratch)
             _lib.check(
-                _lib.lib().tb_resnet_backward_unstacked(
+                _lib.lib().tb_resnet_backward_unstacked_mt(
                     p(saved[1]), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
+                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
                     p(grads_out), _lib.stream_ptr()),
                 "tb_resnet_backward_unstacked")
             return
         frame = saved
         _lib.check(
-            _lib.lib().tb_resnet_backward(
+            _lib.lib().tb_resnet_backward_mt(
                 p(frame.contiguous()), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
-                T1, B, self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
+                T1, B, self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
                 p(grads_out), _lib.stream_ptr()),
             "tb_resnet_backward")
 
@@ -623,7 +690,7 @@ class ResNet(FlatParamModule):
             logits, baseline, hN, cN = _ResNetFunction.apply(self, frame, done, inputs["reward"], notdone, h0, c0, *params)
         else:
             logits, baseline, hN, cN, _ = self._launch_forward(frame, inputs["reward"], notdone, h0, c0, done)
-        T, B = baseline.shape
+        T, B = baseline.shape[:2]
         if self.training:
             action = self._sample(logits, inputs)
         else:
