@@ -194,6 +194,31 @@ int tb_resnet_backward_unstacked_mt(const void* stacked_scratch, const float* gr
                                     int num_values, int use_lstm, int precision, void* workspace, float* grads,
                                     void* stream);
 
+/* ---- IMPALA ResNet on other observation shapes ----------------------------------------------------------------------
+ * The tb_resnet_*_mt entry points with the observation u8 [C, H, W] as arguments: frame is u8 [T1, B, C, H, W] and the
+ * tb_resnet_*_mt entries are the (4, 84, 84) case of these.  Section i's feat conv runs at H_i x W_i (H_0 = H, W_0 = W),
+ * its max-pool (3, 2, 1) leaves ceil(H_i / 2) x ceil(W_i / 2) = H_{i+1} x W_{i+1}, and the parameter layout has
+ * feat_convs.0.0.weight (16, C, 3, 3) and fc.weight (256, 32 * H_3 * W_3); everything else is as for (4, 84, 84).
+ * Supported on every precision: 1 <= C <= 16, 17 <= H <= 126 and 33 <= W <= 126 (17 rows are the fewest that leave the
+ * last section 3 high, the smallest image of the split-bf16 conv kernels; 33 columns the fewest that leave it 5 wide, the
+ * narrowest row their weight gradient takes; 126 their widest padded row, 128 pixels).  tb_resnet_obs_range writes these
+ * bounds as {C min, C max, H min, H max, W min, W max}.  tb_resnet_obs_supported returns 1 for a supported shape and
+ * otherwise 0 with tb_last_error set; the other entries fail the same way (param count -1, workspace 0).  Unstacked
+ * rollouts stay (4, 84, 84) only.                                                                                     */
+int tb_resnet_obs_range(int* range);
+int tb_resnet_obs_supported(int C, int H, int W, int precision);
+int64_t tb_resnet_param_count_obs(int C, int H, int W, int num_actions, int num_values, int use_lstm);
+size_t tb_resnet_workspace_bytes_obs(int C, int H, int W, int64_t T1, int64_t B, int num_actions, int use_lstm,
+                                     int precision);
+int tb_resnet_forward_obs(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
+                          const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions,
+                          int num_values, int use_lstm, int precision, void* workspace, float* policy_logits,
+                          float* baseline, float* hN, float* cN, void* stream);
+int tb_resnet_backward_obs(const uint8_t* frame, const float* grad_logits, const float* grad_baseline,
+                           const float* notdone, const float* params, int C, int H, int W, int64_t T1, int64_t B,
+                           int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* grads,
+                           void* stream);
+
 /* ---- seeded action sampling for the acting forward ------------------------------------ */
 
 /* monobeast.py:618-619 / polybeast_learner.py:256-257  torch.multinomial(F.softmax(policy_logits, dim=1), 1) as a

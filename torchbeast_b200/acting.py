@@ -219,10 +219,14 @@ class GraphedActor:
     def __call__(self, inputs, core_state=()):
         model = self.model
         frame, history = inputs["frame"], model.frame_history
+        obs = tuple(getattr(model, "observation_shape", nets.ATARI_SHAPE))
         newest = history is not None and frame.dim() == 4
-        if frame.dim() != 5 and not newest:
-            raise _lib.TorchBeastB200Error("GraphedActor takes stacked frames [1, B, 4, 84, 84]; unstacked rollouts are a "
-                                           "learner input, got frame %r" % (tuple(inputs["frame"].shape),))
+        if (frame.dim() != 5 and not newest) or (frame.dim() == 5 and tuple(frame.shape[2:]) != obs):
+            raise _lib.TorchBeastB200Error("GraphedActor takes stacked frames [1, B, %d, %d, %d]; unstacked rollouts are a "
+                                           "learner input, got frame %r" % (obs + (tuple(inputs["frame"].shape),)))
+        if history is not None and obs != nets.ATARI_SHAPE:
+            raise _lib.TorchBeastB200Error("a frame_history rebuilds (4, 84, 84) stacks; this net takes stacked frames "
+                                           "[1, B, %d, %d, %d]: detach the history (model.frame_history = None)" % obs)
         if newest and (frame.dtype != torch.uint8 or tuple(frame.shape[2:]) != (84, 84)):
             raise _lib.TorchBeastB200Error("GraphedActor with a frame_history takes stacked frames or the newest frames "
                                            "uint8 [1, B, 84, 84], got %s %r" % (frame.dtype, tuple(frame.shape)))

@@ -278,10 +278,15 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a)
   }
 }
 
+// dynamic shared memory of the forward kernel: weights, kSwStages input windows of `pin` pixels, barriers, staging tiles
+inline size_t sw_fwd_smem(int pin, int CK, int NO) {
+  return 128 + 2 * size_t(9) * CK * NO * 2 + size_t(kSwStages) * 2 * (CK / 8) * pin * 16 + 8 * (2 * kSwStages + 2) +
+         2 * size_t(kTile) * (NO + 4) * sizeof(float) + 16;
+}
+
 template <int CK, int NO>
 int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
-  const size_t smem = 128 + 2 * size_t(9) * CK * NO * 2 + size_t(kSwStages) * 2 * (CK / 8) * a.g.pin * 16 + 8 * (2 * kSwStages + 2) +
-                      2 * size_t(kTile) * (NO + 4) * sizeof(float) + 16;
+  const size_t smem = sw_fwd_smem(a.g.pin, CK, NO);
   TB_REQUIRE(smem <= 227 * 1024, "sw_conv_fwd: shared memory");
   static size_t attr[64] = {0};
   int dev = 0;
@@ -312,6 +317,7 @@ int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
 // folded over the pixel groups through shared memory and written to partial[cta][o][tap*C + c] (folded in CTA order by
 // sw_wgrad_reduce_kernel: deterministic).
 constexpr int kWgStages = 3;
+constexpr int kWgMinW = 5;   // 2*(W + 2) + 2 >= 15: the zero run behind a frame's last pixel covers the last k16 step
 constexpr int kWgWarps = 9;
 constexpr int kWgThreads = (kWgWarps + 1) * 32;
 
@@ -401,7 +407,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) sw_conv_wgrad_kernel(SwWgradArg
     for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       const int n = w / a.g.tpf, p0 = (w - n * a.g.tpf) * kTile;
       // pixels past the frame's last output row alias the next chunk plane: stop at the 16-pixel step that covers the last
-      // valid pixel (the rest of that step falls into the >= 2*Wp + 2 zero pixels that follow in the dY image)
+      // valid pixel (the rest of that step, up to 15 pixels, falls into the 2*Wp + 2 zero pixels that follow in the dY image:
+      // the last row's right border, the bottom border, the next plane's top border and first left border - 15 or more
+      // only for W >= kWgMinW, which sw_conv_wgrad requires)
       int ksteps = (a.g.vend - p0 + 15) / 16;
       if (ksteps > kTile / 16) ksteps = kTile / 16;
       mbar_wait(full(stage), phase);
@@ -490,10 +498,14 @@ __global__ void __launch_bounds__(256) sw_wgrad_reduce_kernel(const float* __res
   }
 }
 
+// dynamic shared memory of the weight-gradient kernel: kWgStages (dY tile + input window) stages and the fold buffer
+inline size_t sw_wgrad_smem(int pin, int C, int O) {
+  return 384 + size_t(kWgStages) * (2 * size_t(O / 8) * kTile * 16 + 2 * size_t(C / 8) * pin * 16) + sizeof(float) * 9 * C * (O + 1);
+}
+
 template <int C, int O>
 int launch_sw_wgrad(const SwWgradArgs& a, int grid, cudaStream_t stream) {
-  const size_t smem = 384 + size_t(kWgStages) * (2 * size_t(O / 8) * kTile * 16 + 2 * size_t(C / 8) * a.g.pin * 16) +
-                      sizeof(float) * 9 * C * (O + 1);
+  const size_t smem = sw_wgrad_smem(a.g.pin, C, O);
   TB_REQUIRE(smem <= 227 * 1024, "sw_conv_wgrad: shared memory");
   static size_t attr[64] = {0};
   int dev = 0;
@@ -642,7 +654,8 @@ __global__ void __launch_bounds__(256) sw_pool_bwd_image_kernel(const uint8_t* _
   }
 }
 
-// uint8 NCHW frames -> 16-channel padded planar image: chunk 0 = the Cf frame channels (+ zeros), chunk 1 = zeros, lo = zeros
+// uint8 NCHW frames -> 16-channel padded planar image: chunk cv = frame channels 8*cv .. 8*cv + 7 (zeros from Cf on),
+// lo = zeros
 __global__ void sw_frames_u8_kernel(const uint8_t* __restrict__ frame, __nv_bfloat16* __restrict__ out, int64_t lo_off, int64_t Nf,
                                     int Cf, int H, int W, int slack_units) {
   const int Hp = H + 2, Wp = W + 2;
@@ -656,9 +669,10 @@ __global__ void sw_frames_u8_kernel(const uint8_t* __restrict__ frame, __nv_bflo
     const int cv = int(t & 1);
     const int64_t n = t >> 1;
     uint4 ph = make_uint4(0u, 0u, 0u, 0u);
-    if (cv == 0 && py >= 1 && py <= H && px >= 1 && px <= W) {
+    const int c0 = 8 * cv;
+    if (c0 < Cf && py >= 1 && py <= H && px >= 1 && px <= W) {
       float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      for (int c = 0; c < Cf; ++c) f[c] = float(__ldg(frame + ((n * Cf + c) * H + (py - 1)) * W + (px - 1)));
+      for (int c = c0; c < Cf && c < c0 + 8; ++c) f[c - c0] = float(__ldg(frame + ((n * Cf + c) * H + (py - 1)) * W + (px - 1)));
       __nv_bfloat162 p0 = __floats2bfloat162_rn(f[0], f[1]), p1 = __floats2bfloat162_rn(f[2], f[3]);
       __nv_bfloat162 p2 = __floats2bfloat162_rn(f[4], f[5]), p3 = __floats2bfloat162_rn(f[6], f[7]);
       ph.x = *reinterpret_cast<uint32_t*>(&p0); ph.y = *reinterpret_cast<uint32_t*>(&p1);
@@ -836,7 +850,7 @@ int sw_csum_reduce(float* csum, int64_t rows, int C, float* db, cudaStream_t str
 
 int sw_frames_u8(const uint8_t* frame, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int Cf, int H, int W, cudaStream_t stream) {
   ProfScope prof("frames_to_image", stream);
-  TB_REQUIRE(Cf >= 1 && Cf <= 8 && lo_off % 8 == 0, "sw_frames_u8: at most 8 frame channels");
+  TB_REQUIRE(Cf >= 1 && Cf <= 16 && lo_off % 8 == 0, "sw_frames_u8: 1 to 16 frame channels");
   const int64_t total = Nf * 2 * (H + 2) * (W + 2);
   if (total == 0) return 0;
   sw_frames_u8_kernel<<<sgrid(total, 256), 256, 0, stream>>>(frame, out, lo_off, Nf, Cf, H, W, sw_geom(H, W).pin + 8);
@@ -868,6 +882,18 @@ bool sw_conv_applicable(int H, int W, int CK, int NO) {
   return (CK == 16 || CK == 32) && (NO == 16 || NO == 32) && H >= 3 && W >= 3 && W <= 126;
 }
 
+bool sw_conv_trainable(int H, int W, int CK, int NO) {
+  if (!sw_conv_applicable(H, W, CK, NO) || W < kWgMinW) return false;
+  const int pin = sw_geom(H, W).pin;
+  const size_t limit = 227 * 1024;
+  return sw_fwd_smem(pin, CK, NO) <= limit && sw_fwd_smem(pin, NO, CK) <= limit && sw_wgrad_smem(pin, CK, NO) <= limit;
+}
+
+int64_t sw_colsum_scratch_floats(int64_t Nf, int H, int W, int C) {
+  const int ppb = 256 / (C / 8);
+  return (int64_t(((H + 2) * (W + 2) + ppb - 1) / ppb) * Nf + kColsumSlices) * C;
+}
+
 int sw_conv_fwd(const __nv_bfloat16* img, int64_t img_lo, const __nv_bfloat16* wk, float* out, int64_t Nf, int H, int W, int CK, int NO,
                 const SwEpilogue& ep, cudaStream_t stream) {
   TB_REQUIRE(img && wk && out && img_lo > 0, "sw_conv_fwd: null pointer");
@@ -895,6 +921,7 @@ int sw_conv_wgrad(const __nv_bfloat16* dyimg, int64_t dy_lo, const __nv_bfloat16
                   int c_real) {
   TB_REQUIRE(dyimg && ximg && dW && partial && dy_lo > 0 && x_lo > 0, "sw_conv_wgrad: null pointer");
   TB_REQUIRE(sw_conv_applicable(H, W, C, O), "sw_conv_wgrad: unsupported shape");
+  TB_REQUIRE(W >= kWgMinW, "sw_conv_wgrad: W = %d < %d: the last pixel step of a frame would read the next plane", W, kWgMinW);
   if (Nf == 0) return 0;
   ProfScope prof(tag, stream);
   SwWgradArgs a;

@@ -23,8 +23,12 @@ int sw_pad_split_colsum(const float* x, __nv_bfloat16* out, int64_t lo_off, int6
 int sw_pool_bwd_image_colsum(const uint8_t* argmax, const float* dy_pooled, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int H, int W,
                              int C, float* db, float* scratch, int64_t scratch_floats, cudaStream_t stream);
 
-// uint8 NCHW frames [Nf, Cf <= 8, H, W] -> padded planar image with 16 channels (channels >= Cf and the whole lo plane are
-// zero; pixel values 0..255 are exact in bf16): the first convolution of the net through the same kernels
+// scratch floats of sw_pad_split_colsum / sw_pool_bwd_image_colsum on an Nf x H x W image with C channels: one row of C
+// per 256-thread block plus the second-level slices
+int64_t sw_colsum_scratch_floats(int64_t Nf, int H, int W, int C);
+
+// uint8 NCHW frames [Nf, 1 <= Cf <= 16, H, W] -> padded planar image with 16 channels (channels >= Cf and the whole lo plane
+// are zero; pixel values 0..255 are exact in bf16): the first convolution of the net through the same kernels
 int sw_frames_u8(const uint8_t* frame, __nv_bfloat16* out, int64_t lo_off, int64_t Nf, int Cf, int H, int W, cudaStream_t stream);
 // the same image (Cf = 4, byte-identical) from an unstacked rollout: frames u8 [T1+3, B, H, W], done [T1, B] (restack.cuh)
 int sw_frames_u8_unstacked(const uint8_t* frames, const uint8_t* done, __nv_bfloat16* out, int64_t lo_off, int64_t T1, int64_t B,
@@ -57,6 +61,10 @@ int64_t sw_csum_rows(int64_t Nf, int H, int W);
 int sw_csum_reduce(float* csum, int64_t rows, int C, float* db, cudaStream_t stream);
 
 bool sw_conv_applicable(int H, int W, int CK, int NO);
+// a CK -> NO conv at H x W can be trained on these kernels: it is applicable, W >= 5 (the weight gradient's last pixel step
+// of a frame must end in the zero run behind it), and its forward, its input-gradient convolution (NO -> CK) and its weight
+// gradient fit the shared memory (the input window grows with W + 2)
+bool sw_conv_trainable(int H, int W, int CK, int NO);
 // out fp32 [Nf*H*W, NO] = epilogue(conv3x3(image) with the packed weights); CK = channels of the image (16 / 32),
 // NO = output channels (16 / 32)
 int sw_conv_fwd(const __nv_bfloat16* img, int64_t img_lo, const __nv_bfloat16* wk, float* out, int64_t Nf, int H, int W, int CK, int NO,

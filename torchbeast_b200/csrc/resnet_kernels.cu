@@ -105,15 +105,43 @@ __global__ void im2col3x3_u8_nchw_kernel(const uint8_t* __restrict__ frame, TOut
   }
 }
 
+// more than 4 channels (the kernel above keeps its patch row in 40 registers): one thread = the 9 taps of one (pixel,
+// channel) pair, k = c*9 + tap as above
+template <typename TOut>
+__global__ void im2col3x3_u8_nchw_wide_kernel(const uint8_t* __restrict__ frame, TOut* __restrict__ col, int64_t N, int C, int H,
+                                              int W, int64_t ldk) {
+  const int64_t total = N * H * W * C;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int c = int(i % C);
+    const int64_t pix = i / C;
+    const int ox = int(pix % W);
+    int64_t t = pix / W;
+    const int oy = int(t % H);
+    const int64_t n = t / H;
+    const uint8_t* src = frame + (n * C + c) * H * W;
+    TOut* dst = col + pix * ldk + c * 9;
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+      const int iy = oy + tap / 3 - 1, ix = ox + tap % 3 - 1;
+      dst[tap] = from_u8<TOut>((iy >= 0 && iy < H && ix >= 0 && ix < W) ? __ldg(src + iy * W + ix) : uint8_t(0));
+    }
+  }
+}
+
 template <typename TOut>
 int im2col3x3_u8_nchw(const uint8_t* frame, TOut* col, int64_t N, int C, int H, int W, int64_t ldk, cudaStream_t stream) {
   ProfScope prof("im2col3x3_u8", stream);
-  TB_REQUIRE(C <= 4, "im2col3x3_u8_nchw: at most 4 input channels");
+  TB_REQUIRE(C >= 1 && C <= 16 && ldk >= int64_t(C) * 9, "im2col3x3_u8_nchw: 1 to 16 input channels");
   const int64_t total = N * H * W;
   if (total == 0) return 0;
   if (ldk > int64_t(C) * 9 && !(sizeof(TOut) == 2 && ldk == 40)) {  // zero the k padding (the vector path writes it itself)
     cudaError_t e = cudaMemsetAsync(col, 0, size_t(N) * H * W * ldk * sizeof(TOut), stream);
     TB_REQUIRE(e == cudaSuccess, "im2col3x3_u8: memset: %s", cudaGetErrorString(e));
+  }
+  if (C > 4) {
+    im2col3x3_u8_nchw_wide_kernel<TOut><<<rgrid(total * C, 128), 128, 0, stream>>>(frame, col, N, C, H, W, ldk);
+    return check_launch("im2col3x3_u8_nchw_wide_kernel");
   }
   im2col3x3_u8_nchw_kernel<TOut><<<rgrid(total, 128), 128, 0, stream>>>(frame, col, N, C, H, W, ldk);
   return check_launch("im2col3x3_u8_nchw_kernel");

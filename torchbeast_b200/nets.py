@@ -7,6 +7,7 @@ gradients into one flat gradient buffer): that is what the C-ABI kernels, the fu
 clip+RMSprop step and the single NCCL all-reduce operate on.
 """
 import collections
+import ctypes
 import weakref
 
 import torch
@@ -80,16 +81,35 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
     return spec
 
 
-def frame_is_unstacked(frame, reward):
-    """False for a stacked frame u8 [T1, B, 4, 84, 84]; True for an unstacked rollout u8 [T1+3, B, 84, 84] with
-    T1 = reward.shape[0] (include/torchbeast_b200.h, "unstacked rollouts").  Anything else raises."""
+ATARI_SHAPE = (4, 84, 84)
+
+
+def resnet_obs_range():
+    """{"C": (min, max), "H": (min, max), "W": (min, max)}: the observations u8 [C, H, W] the ResNet takes on every
+    backend, as the C library states them (include/torchbeast_b200.h, tb_resnet_obs_range)."""
+    r = (ctypes.c_int * 6)()
+    _lib.check(_lib.lib().tb_resnet_obs_range(ctypes.cast(r, ctypes.c_void_p)), "tb_resnet_obs_range")
+    return {"C": (r[0], r[1]), "H": (r[2], r[3]), "W": (r[4], r[5])}
+
+
+def frame_is_unstacked(frame, reward, observation_shape=ATARI_SHAPE):
+    """False for a stacked frame u8 [T1, B, C, H, W] with [C, H, W] = observation_shape; True for an unstacked rollout
+    u8 [T1+3, B, 84, 84] with T1 = reward.shape[0] (include/torchbeast_b200.h, "unstacked rollouts"), which only a
+    (4, 84, 84) net takes.  Anything else raises."""
+    obs = tuple(observation_shape)
+    stacked = "[T,B,%d,%d,%d]" % obs
     if frame.dtype != torch.uint8 or frame.dim() not in (4, 5):
-        raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84] or unstacked [T+3,B,84,84], got %s %r"
-                                       % (frame.dtype, tuple(frame.shape)))
+        raise _lib.TorchBeastB200Error("frame must be uint8 %s%s, got %s %r"
+                                       % (stacked, " or unstacked [T+3,B,84,84]" if obs == ATARI_SHAPE else "",
+                                          frame.dtype, tuple(frame.shape)))
     if frame.dim() == 5:
-        if tuple(frame.shape[2:]) != (4, 84, 84):
-            raise _lib.TorchBeastB200Error("frame must be uint8 [T,B,4,84,84], got %s %r" % (frame.dtype, tuple(frame.shape)))
+        if tuple(frame.shape[2:]) != obs:
+            raise _lib.TorchBeastB200Error("frame must be uint8 %s, got %s %r" % (stacked, frame.dtype, tuple(frame.shape)))
         return False
+    if obs != ATARI_SHAPE:
+        raise _lib.TorchBeastB200Error(
+            "unstacked rollouts and newest frames rebuild (4, 84, 84) stacks; this net takes stacked frames uint8 %s, "
+            "got %r" % (stacked, tuple(frame.shape)))
     T1, B = reward.shape[:2]
     if tuple(frame.shape) != (T1 + 3, B, 84, 84):
         raise _lib.TorchBeastB200Error(
@@ -152,6 +172,10 @@ class FlatParamModule(nn.Module):
         """inputs["frame"], or, with a frame_history attached and newest frames [T, B, 84, 84] (T = reward's), the
         unstacked rollout [T+3, B, 84, 84] the history builds from them (acting.FrameHistory.stack)."""
         frame, reward = inputs["frame"], inputs["reward"]
+        obs = tuple(getattr(self, "observation_shape", ATARI_SHAPE))
+        if self.frame_history is not None and obs != ATARI_SHAPE:
+            raise _lib.TorchBeastB200Error("a frame_history rebuilds (4, 84, 84) stacks; this net takes stacked frames "
+                                           "uint8 [T,B,%d,%d,%d]: detach the history (model.frame_history = None)" % obs)
         if self.frame_history is None or frame.dim() != 4 or frame.shape[0] != reward.shape[0]:
             return frame
         if frame.shape[1] != reward.shape[1]:
@@ -511,10 +535,20 @@ class AtariNet(FlatParamModule):
 
 
 
-def resnet_param_spec(num_actions, use_lstm, num_values=1):
-    """State_dict order/shapes of the reference's polybeast_learner.Net (pl:134-204, BASELINE.md section 5)."""
+def resnet_fc_in(observation_shape=ATARI_SHAPE):
+    """Input features of the ResNet's fc layer: 32 x H_3 x W_3, each of the three max-pools (3, 2, 1) taking a side
+    s to ceil(s / 2) (84 -> 42 -> 21 -> 11: 3872)."""
+    _, h, w = observation_shape
+    for _ in range(3):
+        h, w = (h + 1) // 2, (w + 1) // 2
+    return 32 * h * w
+
+
+def resnet_param_spec(num_actions, use_lstm, num_values=1, observation_shape=ATARI_SHAPE):
+    """State_dict order/shapes of the reference's polybeast_learner.Net (pl:134-204, BASELINE.md section 5) for
+    observations u8 [C, H, W]: feat_convs.0.0.weight (16, C, 3, 3) and fc.weight (256, resnet_fc_in(...))."""
     spec = []
-    cin = 4
+    cin = observation_shape[0]
     for i, ch in enumerate([16, 32, 32]):
         spec += [("feat_convs.%d.0.weight" % i, (ch, cin, 3, 3)), ("feat_convs.%d.0.bias" % i, (ch,))]
         cin = ch
@@ -522,7 +556,7 @@ def resnet_param_spec(num_actions, use_lstm, num_values=1):
         for i, ch in enumerate([16, 32, 32]):
             for j in (1, 3):
                 spec += [("%s.%d.%d.weight" % (blk, i, j), (ch, ch, 3, 3)), ("%s.%d.%d.bias" % (blk, i, j), (ch,))]
-    spec += [("fc.weight", (256, 3872)), ("fc.bias", (256,))]
+    spec += [("fc.weight", (256, resnet_fc_in(observation_shape))), ("fc.bias", (256,))]
     head_in = 257
     if use_lstm:
         spec += [("core.weight_ih_l0", (1024, 257)), ("core.weight_hh_l0", (1024, 256)),
@@ -558,20 +592,33 @@ class _ResNetFunction(torch.autograd.Function):
 class ResNet(FlatParamModule):
     """CUDA IMPALA ResNet (reference polybeast_learner.py:134-266 `Net`): three sections of
     conv3x3 + maxpool3/2 + two residual blocks, fc 3872->256, cat[reward], optional LSTM(257->256), heads.
-    forward(inputs, core_state) returns ((action, policy_logits, baseline), core_state) like the reference."""
+    forward(inputs, core_state) returns ((action, policy_logits, baseline), core_state) like the reference.
+
+    observation_shape (keyword-only, default the Atari stack (4, 84, 84)): the u8 [C, H, W] of each frame, e.g.
+    (3, 64, 64) for Procgen or (3, 72, 96) for DMLab; C from 1 to 16, H from 17 and W from 33 to 126
+    (resnet_obs_range()), on every precision.  The fc then reads 32 x ceil(H/8) x ceil(W/8) features (resnet_fc_in).  Unstacked rollouts and a
+    frame_history are (4, 84, 84) only."""
 
     PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 
-    def __init__(self, num_actions, use_lstm=False, device=None, precision=None, num_tasks=None):
+    def __init__(self, num_actions, use_lstm=False, device=None, precision=None, num_tasks=None, *,
+                 observation_shape=ATARI_SHAPE):
         super().__init__()
         import os
         self.num_actions = num_actions
         self.use_lstm = use_lstm
+        obs = tuple(int(d) for d in observation_shape)
+        if len(obs) != 3 or not _lib.lib().tb_resnet_obs_supported(*obs, self.PRECISIONS["bf16x3"]):
+            rng = resnet_obs_range()
+            raise _lib.TorchBeastB200Error(
+                "ResNet observation_shape must be (C, H, W) with C in [%d, %d], H in [%d, %d] and W in [%d, %d], got %r"
+                % (sum((rng[k] for k in ("C", "H", "W")), ()) + (tuple(observation_shape),)))
+        self.observation_shape = obs
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
         popart = None if num_tasks is None else PopArt(num_tasks, device)
         self.num_values = 1 if popart is None else popart.num_tasks
-        self._build_flat(resnet_param_spec(num_actions, use_lstm, num_values=self.num_values), device)
+        self._build_flat(resnet_param_spec(num_actions, use_lstm, num_values=self.num_values, observation_shape=obs), device)
         self._fix_module_names()
         self.reset_parameters_like_torch()
         if popart is not None:
@@ -586,7 +633,7 @@ class ResNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_resnet_param_count_mt(num_actions, self.num_values, int(use_lstm))
+        count = _lib.lib().tb_resnet_param_count_obs(*obs, num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def _fix_module_names(self):
@@ -600,8 +647,10 @@ class ResNet(FlatParamModule):
     def _workspace(self, T1, B):
         key = (T1, B, self._flat.device, self.precision)
         if self._ws_key != key:
-            nbytes = _lib.lib().tb_resnet_workspace_bytes(T1, B, self.num_actions, int(self.use_lstm),
-                                                          self.PRECISIONS[self.precision])
+            nbytes = _lib.lib().tb_resnet_workspace_bytes_obs(*self.observation_shape, T1, B, self.num_actions,
+                                                              int(self.use_lstm), self.PRECISIONS[self.precision])
+            if nbytes == 0:
+                raise _lib.TorchBeastB200Error("tb_resnet_workspace_bytes_obs: %s" % _lib.lib().tb_last_error().decode())
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
             self._ws_key = key
         return self._ws
@@ -610,7 +659,7 @@ class ResNet(FlatParamModule):
         """Returns (logits, baseline, hN, cN, saved): `saved` is what _launch_backward re-reads - the stacked frame, or
         ("unstacked", stacked scratch or None).  `done` is read only with an unstacked frame, to rebuild the stacks."""
         _lib.require_cuda(frame, reward, self._flat)
-        unstacked = frame_is_unstacked(frame, reward)
+        unstacked = frame_is_unstacked(frame, reward, self.observation_shape)
         T1, B = reward.shape[:2] if unstacked else frame.shape[:2]
         if unstacked:
             _lib.require_cuda(done)
@@ -638,9 +687,9 @@ class ResNet(FlatParamModule):
                 "tb_resnet_forward_unstacked")
             return logits, baseline, hN, cN, ("unstacked", scratch)
         _lib.check(
-            _lib.lib().tb_resnet_forward_mt(
-                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions, self.num_values,
-                int(self.use_lstm),
+            _lib.lib().tb_resnet_forward_obs(
+                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), *self.observation_shape, T1, B, self.num_actions,
+                self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_resnet_forward")
@@ -659,10 +708,10 @@ class ResNet(FlatParamModule):
             return
         frame = saved
         _lib.check(
-            _lib.lib().tb_resnet_backward_mt(
+            _lib.lib().tb_resnet_backward_obs(
                 p(frame.contiguous()), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
-                T1, B, self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
-                p(grads_out), _lib.stream_ptr()),
+                *self.observation_shape, T1, B, self.num_actions, self.num_values, int(self.use_lstm),
+                self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(grads_out), _lib.stream_ptr()),
             "tb_resnet_backward")
 
     @torch.no_grad()

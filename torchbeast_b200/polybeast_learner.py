@@ -58,13 +58,14 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
     the host is enqueued before the lock is released."""
     device = torch.device(getattr(flags, "actor_device", None) or model.flat_params.device)
     graphed = inference_graph_enabled(flags)
+    obs = tuple(getattr(model, "observation_shape", (4, 84, 84)))
     with torch.no_grad():
         for batch in inference_batcher:
             batched_env_outputs, agent_state = batch.get_inputs()
             frame, reward, done, *rest = batched_env_outputs
-            if frame.dim() != 5:
-                raise _lib.TorchBeastB200Error("inference takes stacked frames [1, B, 4, 84, 84]; unstacked rollouts are a "
-                                               "learner input, got frame %r" % (tuple(frame.shape),))
+            if frame.dim() != 5 or tuple(frame.shape[2:]) != obs:
+                raise _lib.TorchBeastB200Error("inference takes stacked frames [1, B, %d, %d, %d]; unstacked rollouts are a "
+                                               "learner input, got frame %r" % (obs + (tuple(frame.shape),)))
             inputs = dict(frame=frame.to(device, non_blocking=True), reward=reward.to(device, non_blocking=True),
                           done=done.to(device, non_blocking=True))
             if getattr(model, "needs_last_action", False):
