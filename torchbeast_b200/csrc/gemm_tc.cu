@@ -2,7 +2,7 @@
 //
 //   C[M,N] = epilogue( sum_k A[m,k] * B[n,k] )     A [M,K], B [N,K] bf16, K contiguous ("K-major")
 //
-// One CTA computes a 128 x BLOCK_N tile.  Warp roles (160 threads):
+// gemm_tc_kernel (dense GEMMs): one CTA computes a 128 x BLOCK_N tile.  Warp roles (160 threads):
 //   warp 4     TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 64 bf16 = 128 B) into a
 //                             shared-memory ring, mbarrier expect_tx / complete_tx
 //   warps 0-3  consumer     : one warpgroup issues wgmma.m64nNk16 (N = BLOCK_N) for both 64-row halves of
@@ -20,6 +20,8 @@
 //   forward  act = col . W^T      : A K-major,  B K-major
 //   dgrad    dcol = dY . W        : A K-major,  B MN-major (W [n', k'] as stored)
 //   wgrad    dW   = dY^T . col    : A MN-major, B MN-major (no transposed copies), split-K over grid.z
+// The implicit-GEMM convolutions run on conv_tc_kernel (two consumer warpgroups, up to 256-row tiles) and
+// conv_wgrad_implicit_kernel, described where they are defined.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -39,39 +41,14 @@ namespace {
 // EPI: 0 = store the accumulator as is; 1 = scale / bias / ReLU; 2 = + ReLU-mask / residual loads.
 // (compile-time so the common epilogues carry no predicated per-element loads - ncu showed the generic
 //  epilogue, not the MMA pipe, bounding the K=64 dgrad products)
-// IMPL (implicit-GEMM convolution, forward): the A operand is not a matrix in memory but the NHWC activation
-// itself, addressed through a rank-4 tensor map {flat frame element, ox, oy, frame} whose dimensions overlap:
-// M tile t = the `rows` = OW*OH*fpt patches of frames [t*fpt, (t+1)*fpt), k-block kb = 64 consecutive
-// (kw, c) elements of kernel row kb / kbw starting at element e0 of the frame - one TMA box per stage lands
-// as [patch][64 k] rows in the canonical SWIZZLE_128B layout, so no patch matrix is ever written.
-//
-// The same machinery runs the INPUT gradient (mode 1/2) as a gather-form transposed convolution, so that
-// neither the [patches, KH*KW*C] gradient matrix nor a col2im pass exists:
-//   mode 1 (stride 1): dX[n,y,x,c] = sum_{kh,kw,o} dY[n,y-kh,x-kw,o] W[o,kh,kw,c]; the A tile of k-block (kh,kw) is
-//     the TMA box of dY at (x0,y0) = (-kw,-kh) - out-of-bounds rows/columns arrive as zeros (the "full" padding);
-//   mode 2 (stride 2, even kernel): output pixels split by parity (py,px) = (y&1, x&1): each class is a stride-1
-//     conv of dY with the (KH/2 x KW/2) sub-kernel W[o, py+2i, px+2j, c].  All classes read the SAME dY boxes, so
-//     they are the N dimension of one GEMM: B = [(py,px,c), (i,j,o)], and the epilogue scatters the 32-column
-//     chunk of class (py,px) to pixel (2u+py, 2v+px).
-struct ImplicitConv {
-  int rows = 0;       // valid rows per M tile (<= 128)
-  int fpt = 1;        // frames per tile
-  int kbw = 1;        // k-blocks per kernel row
-  int row_elems = 0;  // mode 0: W*C
-  int mode = 0;       // 0 forward, 1 input gradient stride 1, 2 input gradient stride 2 (parity classes)
-  int tw = 0;         // mode 2: tile width (v range) = ceil(W_in / 2)
-  int outH = 0, outW = 0;  // mode 2: input-gradient image size
-};
-
 // SPLIT (split-bf16, see TcEpilogue): a stage holds the hi AND lo plane tiles of both operands (tmAl / tmBl are the
 // lo planes' tensor maps) and every k-step issues three MMAs (lo.hi, hi.lo, hi.hi) into the same accumulator; the
 // epilogue can write its bf16 output as hi / lo planes.
-template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool IMPL = false, bool SPLIT = false>
+template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool SPLIT = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, TcEpilogue ep, int M,
-               int N, int K, float* partial, int tiles_m, int tiles_n, int splits, int ldp = 0,
-               ImplicitConv ic = ImplicitConv()) {
+               int N, int K, float* partial, int tiles_m, int tiles_n, int splits, int ldp) {
   constexpr uint32_t B_BYTES = BLOCK_N * kBlockK * 2;
   constexpr uint32_t A_STAGE = (SPLIT ? 2u : 1u) * kABytes, B_STAGE = (SPLIT ? 2u : 1u) * B_BYTES;  // [hi][lo]
   constexpr int LDS = BLOCK_N + 4;  // staging row pitch in floats (16-byte rows, conflict-free row reads)
@@ -116,20 +93,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int i = 0; i < num_kb; ++i) {
           const int kc = (kb0 + i) * kBlockK;
           mbar_wait(empty(stage), phase ^ 1);
-          mbar_expect_tx(full(stage), (SPLIT ? 2u : 1u) * ((IMPL ? uint32_t(ic.rows) * 128u : kABytes) + B_BYTES));
+          mbar_expect_tx(full(stage), (SPLIT ? 2u : 1u) * (kABytes + B_BYTES));
 #pragma unroll
           for (int pl = 0; pl < (SPLIT ? 2 : 1); ++pl) {  // plane 0 = hi, plane 1 = lo
             const CUtensorMap* mA = pl ? &tmAl : &tmA;
             const CUtensorMap* mB = pl ? &tmBl : &tmB;
             const uint32_t dA = sA + stage * A_STAGE + pl * kABytes, dB = sB + stage * B_STAGE + pl * B_BYTES;
-            if (IMPL) {
-              const int kb = kb0 + i;
-              if (ic.mode == 0)
-                tma_load_4d(dA, mA, full(stage), (kb / ic.kbw) * ic.row_elems + (kb % ic.kbw) * kBlockK, 0, 0,
-                            (m0 / kBlockM) * ic.fpt);
-              else
-                tma_load_4d(dA, mA, full(stage), 0, -(kb % ic.kbw), -(kb / ic.kbw), (m0 / kBlockM) * ic.fpt);
-            } else if (A_MN) {  // two 64(k) x 64(m) boxes
+            if (A_MN) {  // two 64(k) x 64(m) boxes
               tma_load_2d(dA, mA, full(stage), m0, kc);
               tma_load_2d(dA + 8192, mA, full(stage), m0 + 64, kc);
             } else {
@@ -153,30 +123,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int m0, n0, kb0, num_kb, z;
       decode(w, m0, n0, kb0, num_kb, z);
       const int rl = threadIdx.x;
-      const int64_t r = IMPL ? int64_t(m0 / kBlockM) * ic.rows + rl : int64_t(m0) + rl;
-      const bool rvalid = r < M && (!IMPL || rl < ic.rows);
-      // where this thread's 32 values of column chunk c0 live in memory: row pr, first column pc (== r, n0 + c0
-      // except for the parity-class scatter of the stride-2 input gradient); false = nothing to store
-      auto locate = [&](int c0, int64_t& pr, int& pc) -> bool {
-        pr = r; pc = n0 + c0;
-        if (IMPL && ic.mode == 2) {
-          const int cls = (n0 + c0) >> 5, u = rl / ic.tw, v2 = rl - u * ic.tw;
-          const int y = 2 * u + (cls >> 1), x = 2 * v2 + (cls & 1);
-          if (y >= ic.outH || x >= ic.outW) return false;
-          pr = (int64_t(m0 / kBlockM) * ic.outH + y) * ic.outW + x;
-          pc = 0;
-        }
-        return true;
-      };
+      const int64_t r = int64_t(m0) + rl;
+      const bool rvalid = r < M;
       // EPI 2: pull the ReLU-mask / residual rows of the WHOLE tile into L2 before waiting for the accumulator, so
-      // their DRAM latency hides behind the MMA main loop (fetching them chunk by chunk after the wait made the
-      // stride-2 input gradient - 4 chunks, 4 k-blocks - epilogue-latency bound)
+      // their DRAM latency hides behind the MMA main loop
       if constexpr (EPI >= 2) {
         if (rvalid) {
 #pragma unroll 1
           for (int c0 = 0; c0 < BLOCK_N && n0 + c0 < N; c0 += 32) {
-            int64_t pr; int pc;
-            if (!locate(c0, pr, pc)) continue;
+            const int64_t pr = r; const int pc = n0 + c0;
             if (ep.mask16) asm volatile("prefetch.global.L2 [%0];" ::"l"(ep.mask16 + pr * ep.ldmask + pc));
             if (ep.addend16) asm volatile("prefetch.global.L2 [%0];" ::"l"(ep.addend16 + pr * ep.ldadd + pc));
           }
@@ -260,8 +215,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         if (rvalid) {
           const int nbase = n0 + c0;
-          int64_t pr; int pc;
-          if (!locate(c0, pr, pc)) continue;
+          const int64_t pr = r; const int pc = nbase;
           float o[32];
           const bool full_cols = nbase + 32 <= N;
           // EPI 2: the ReLU mask / residual rows are read as four 16-byte vectors per 32 columns when aligned
@@ -433,6 +387,297 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// Implicit-GEMM convolution (conv_tc_kernel, forward = mode 0): the A operand is not a matrix in memory but the NHWC activation
+// itself, addressed through a rank-4 tensor map {flat frame element, ox, oy, frame} whose dimensions overlap:
+// M tile t = the `rows` = OW*OH*fpt (<= TM) patches of frames [t*fpt, (t+1)*fpt), k-block kb = 64 consecutive
+// (kw, c) elements of kernel row kb / kbw starting at element e0 of the frame - one TMA box per stage lands
+// as [patch][64 k] rows in the canonical SWIZZLE_128B layout, so no patch matrix is ever written.
+//
+// The same machinery runs the INPUT gradient (mode 1/2) as a gather-form transposed convolution, so that
+// neither the [patches, KH*KW*C] gradient matrix nor a col2im pass exists:
+//   mode 1 (stride 1): dX[n,y,x,c] = sum_{kh,kw,o} dY[n,y-kh,x-kw,o] W[o,kh,kw,c]; the A tile of k-block (kh,kw) is
+//     the TMA box of dY at (x0,y0) = (-kw,-kh) - out-of-bounds rows/columns arrive as zeros (the "full" padding);
+//   mode 2 (stride 2, even kernel): output pixels split by parity (py,px) = (y&1, x&1): each class is a stride-1
+//     conv of dY with the (KH/2 x KW/2) sub-kernel W[o, py+2i, px+2j, c].  All classes read the SAME dY boxes, so
+//     they are the N dimension of one GEMM: B = [(py,px,c), (i,j,o)], and the epilogue scatters the 32-column
+//     chunk of class (py,px) to pixel (2u+py, 2v+px).
+struct ImplicitConv {
+  int rows = 0;       // valid rows per M tile (<= TM)
+  int fpt = 1;        // frames per tile
+  int kbw = 1;        // k-blocks per kernel row
+  int row_elems = 0;  // mode 0: W*C
+  int mode = 0;       // 0 forward, 1 input gradient stride 1, 2 input gradient stride 2 (parity classes)
+  int tw = 0;         // mode 2: tile width (v range) = ceil(W_in / 2)
+  int outH = 0, outW = 0;  // mode 2: input-gradient image size
+};
+
+
+// Implicit-GEMM convolution kernel (forward, input gradient): the same operand layouts as gemm_tc_kernel with A read
+// through the rank-4 tensor map, but organised for the short-K, many-tile shape of the trunk convolutions (K = 256..576,
+// 4-9 k-blocks per tile, thousands of tiles), where a single consumer's epilogue is a large share of each tile:
+//   - a tile is TM x BLOCK_N with TM = 128 or 256 rows of whole frames (implicit_tile_rows): 256 rows hold 3 frames of
+//     81 patches or 5 of 49, so 243 / 245 of 256 MMA rows do useful work instead of 81 / 98 of 128;
+//   - 384 threads: warp 8 is the TMA producer filling ONE ring in the CTA's work order (its warpgroup gives its
+//     registers to the consumers with setmaxnreg: ptxas budgets a 288-thread CTA like a 384-thread one, 168 registers
+//     per thread, which would spill four 64-row accumulators plus the epilogue); warpgroups 0 and 1 are consumers taking
+//     alternate work items ("ping-pong"), so one runs its epilogue while the other issues wgmma.  Each stages its
+//     accumulators through its own 64-row shared-memory tile, one row group at a time; a thread finishes one row
+//     (half of its 32-column chunks) per pass.
+// Per output element the k-block order and the lo.hi, hi.lo, hi.hi order inside a k16 step are those of gemm_tc_kernel,
+// so the results are bit-identical to it.  EPI: 1 = scale / bias / ReLU; 2 = + bf16 ReLU mask (input gradient).
+constexpr int kConvThreads = 3 * kConsumers;
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;
+static_assert(kConsumers * (kProducerRegs + 2 * kConsumerRegs) <= 65536, "conv_tc_kernel: register split exceeds the SM");
+
+template <int TM, int BLOCK_N, int kStages, int EPI, bool SPLIT>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, TcEpilogue ep, int M,
+               int N, int K, int tiles_m, int tiles_n, ImplicitConv ic) {
+  static_assert(TM == kBlockM || TM == 2 * kBlockM, "conv_tc_kernel: 128- or 256-row tiles");
+  constexpr int RG = TM / 64;  // m64 row groups per tile
+  constexpr uint32_t A_BYTES = TM * kBlockK * 2;
+  constexpr uint32_t B_BYTES = BLOCK_N * kBlockK * 2;
+  constexpr uint32_t A_STAGE = (SPLIT ? 2u : 1u) * A_BYTES, B_STAGE = (SPLIT ? 2u : 1u) * B_BYTES;  // [hi][lo]
+  constexpr int LDS = BLOCK_N + 4;  // staging row pitch in floats (16-byte rows, conflict-free row reads)
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
+  const uint32_t sA = base, sB = base + kStages * A_STAGE;
+  const uint32_t bars = sB + kStages * B_STAGE;  // full[kStages], empty[kStages], then the two staging tiles
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (kStages + s); };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_kb = (K + kBlockK - 1) / kBlockK;
+  const int total_work = tiles_m * tiles_n;
+
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == 8 && lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int mt = w / tiles_n, n0 = (w % tiles_n) * BLOCK_N;  // n fastest: co-running CTAs share A boxes in L2
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty(stage), phase ^ 1);
+          mbar_expect_tx(full(stage), (SPLIT ? 2u : 1u) * (uint32_t(ic.rows) * 128u + B_BYTES));
+#pragma unroll
+          for (int pl = 0; pl < (SPLIT ? 2 : 1); ++pl) {  // plane 0 = hi, plane 1 = lo
+            const CUtensorMap* mA = pl ? &tmAl : &tmA;
+            const CUtensorMap* mB = pl ? &tmBl : &tmB;
+            const uint32_t dA = sA + stage * A_STAGE + pl * A_BYTES, dB = sB + stage * B_STAGE + pl * B_BYTES;
+            if (ic.mode == 0)
+              tma_load_4d(dA, mA, full(stage), (kb / ic.kbw) * ic.row_elems + (kb % ic.kbw) * kBlockK, 0, 0, mt * ic.fpt);
+            else
+              tma_load_4d(dA, mA, full(stage), 0, -(kb % ic.kbw), -(kb / ic.kbw), mt * ic.fpt);
+            tma_load_2d(dB, mB, full(stage), kb * kBlockK, n0);
+          }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int g = warp >> 2;  // consumer warpgroup: even (g = 0) or odd (g = 1) work items of this CTA
+    const int tid = threadIdx.x & 127;
+    // [64][LDS] fp32 per warpgroup: the epilogue reads whole rows, the wgmma fragments are scattered over row pairs
+    float* stg = reinterpret_cast<float*>(smem_raw + (bars + 16u * kStages - smem_addr(smem_raw))) + g * 64 * LDS;
+    float acc[RG][BLOCK_N / 2];  // row group h = rows [64h, 64h + 64) of the tile
+    // where the 32 values of column chunk c0 of tile row rl (global row r) live in memory: row pr, first column pc
+    // (== r, n0 + c0 except for the parity-class scatter of the stride-2 input gradient); false = nothing to store
+    auto locate = [&](int mt, int n0, int rl, int64_t r, int c0, int64_t& pr, int& pc) -> bool {
+      pr = r; pc = n0 + c0;
+      if (ic.mode == 2) {
+        const int cls = (n0 + c0) >> 5, u = rl / ic.tw, v2 = rl - u * ic.tw;
+        const int y = 2 * u + (cls >> 1), x = 2 * v2 + (cls & 1);
+        if (y >= ic.outH || x >= ic.outW) return false;
+        pr = (int64_t(mt) * ic.outH + y) * ic.outW + x;
+        pc = 0;
+      }
+      return true;
+    };
+    // the ring position of a work item: num_kb k-blocks per item, items in the CTA's order
+    for (int w = blockIdx.x + g * gridDim.x, it = g; w < total_work; w += 2 * gridDim.x, it += 2) {
+      const int mt = w / tiles_n, n0 = (w % tiles_n) * BLOCK_N;
+      const int pos = it * num_kb;
+      int stage = pos % kStages;
+      uint32_t phase = uint32_t(pos / kStages) & 1u;
+      // EPI 2: pull the ReLU-mask rows of the WHOLE tile into L2 before waiting for the accumulator, so their DRAM
+      // latency hides behind the MMA main loop
+      if (EPI >= 2 && ep.mask16) {
+#pragma unroll 1
+        for (int rl = tid; rl < ic.rows; rl += kConsumers) {
+          const int64_t r = int64_t(mt) * ic.rows + rl;
+          if (r >= M) break;
+#pragma unroll 1
+          for (int c0 = 0; c0 < BLOCK_N && n0 + c0 < N; c0 += 32) {
+            int64_t pr; int pc;
+            if (locate(mt, n0, rl, r, c0, pr, pc)) asm volatile("prefetch.global.L2 [%0];" ::"l"(ep.mask16 + pr * ep.ldmask + pc));
+          }
+        }
+      }
+      // Ordered hand-off: start waiting for this item's stages only once the other warpgroup has received all of the
+      // previous item's.  The ring slot of this item's first k-block has then been filled for the round before, so a
+      // parity wait cannot match a phase two rounds old (an item may span more k-blocks than the ring has stages), and
+      // the two warpgroups' main loops alternate instead of sharing the tensor cores.
+      if (it > 0) named_sync(3 + (g ^ 1), 2 * kConsumers);
+      // main loop: one k-block per stage; a stage is handed back once the wgmma group after it has been issued and
+      // its own group has completed (one group in flight)
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(full(stage), phase);
+        wgmma_fence();
+        const uint32_t aA = sA + stage * A_STAGE, aB = sB + stage * B_STAGE;
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          const uint64_t db = make_smem_desc(aB + k * 32);
+#pragma unroll
+          for (int h = 0; h < RG; ++h) {  // the 64-row groups of the tile, 8192 B apart
+            const uint32_t ah = aA + h * 8192;
+            const uint64_t da = make_smem_desc(ah + k * 32);
+            if constexpr (SPLIT) {  // small terms first: lo.hi, hi.lo, then hi.hi
+              wgmma_bf16<BLOCK_N, false, false>(acc[h], make_smem_desc(ah + A_BYTES + k * 32), db, (kb | k) != 0);
+              wgmma_bf16<BLOCK_N, false, false>(acc[h], da, make_smem_desc(aB + B_BYTES + k * 32), 1);
+              wgmma_bf16<BLOCK_N, false, false>(acc[h], da, db, 1);
+            } else {
+              wgmma_bf16<BLOCK_N, false, false>(acc[h], da, db, (kb | k) != 0);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty(prev)); }
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      if (w + gridDim.x < total_work) named_arrive(3 + g, 2 * kConsumers);  // the next item is the other warpgroup's
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(prev));
+      // epilogue, one row group at a time: thread tid finishes staged row tid % 64, column chunks 32 * (tid / 64) + 64 i
+      const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+      const int er = tid & 63, ec = (tid >> 6) * 32;
+#pragma unroll 1
+      for (int h = 0; h < RG; ++h) {
+        named_sync(1 + g, kConsumers);  // the previous pass has read the staging tile
+#pragma unroll
+        for (int q = 0; q < RG; ++q) {
+          if (q != h) continue;  // static register indices: acc[q] is never addressed with the runtime h
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            float* sp = stg + fr * LDS + 8 * j + fc;
+            *reinterpret_cast<float2*>(sp) = make_float2(acc[q][4 * j], acc[q][4 * j + 1]);
+            *reinterpret_cast<float2*>(sp + 8 * LDS) = make_float2(acc[q][4 * j + 2], acc[q][4 * j + 3]);
+          }
+        }
+        named_sync(1 + g, kConsumers);
+        const int rl = h * 64 + er;
+        const int64_t r = int64_t(mt) * ic.rows + rl;
+        if (rl >= ic.rows || r >= M) continue;
+#pragma unroll 1
+        for (int c0 = ec; c0 < BLOCK_N; c0 += 64) {
+          const int nbase = n0 + c0;
+          int64_t pr; int pc;
+          if (nbase >= N || !locate(mt, n0, rl, r, c0, pr, pc)) continue;
+          float o[32];
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 t = *reinterpret_cast<const float4*>(stg + er * LDS + c0 + j);
+            o[j] = t.x; o[j + 1] = t.y; o[j + 2] = t.z; o[j + 3] = t.w;
+          }
+          const bool full_cols = nbase + 32 <= N;
+          // uniform branches around whole 32-element passes (see gemm_tc_kernel)
+          if (ep.scale != 1.0f) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) o[j] *= ep.scale;
+          }
+          if (ep.bias) {
+            const float* bp = ep.bias + nbase;
+            if (full_cols && (reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
+#pragma unroll
+              for (int q = 0; q < 8; ++q) {
+                const float4 b4 = __ldg(reinterpret_cast<const float4*>(bp) + q);
+                o[4 * q] += b4.x; o[4 * q + 1] += b4.y; o[4 * q + 2] += b4.z; o[4 * q + 3] += b4.w;
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < 32; ++j)
+                if (nbase + j < N) o[j] += __ldg(bp + j);
+            }
+          }
+          if (ep.relu) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.0f);
+          }
+          if (EPI >= 2 && ep.mask16) {
+            const __nv_bfloat16* mp = ep.mask16 + pr * ep.ldmask + pc;
+            if (full_cols && (ep.ldmask & 7) == 0 && (reinterpret_cast<uintptr_t>(mp) & 15) == 0) {
+              // a bf16 is positive iff its bit pattern, read as a signed 16-bit integer, is > 0
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const uint4 t = __ldg(reinterpret_cast<const uint4*>(mp) + q);
+                const uint32_t m[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const int j = 8 * q + 2 * e;
+                  o[j] = (int(m[e] << 16) > 0) ? o[j] : 0.0f;
+                  o[j + 1] = (int(m[e] & 0xffff0000u) > 0) ? o[j + 1] : 0.0f;
+                }
+              }
+            } else {
+#pragma unroll
+              for (int j = 0; j < 32; ++j)
+                if (nbase + j < N) o[j] = (__bfloat162float(mp[j]) > 0.0f) ? o[j] : 0.0f;
+            }
+          }
+          if (ep.C) {
+            float* c = ep.C + pr * ep.ldc + pc;
+            const bool vec = (ep.ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(c) & 15) == 0;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              if (vec && nbase + j + 4 <= N) {
+                *reinterpret_cast<float4*>(c + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
+              } else {
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj)
+                  if (nbase + j + jj < N) c[j + jj] = o[j + jj];
+              }
+            }
+          }
+          if (ep.C16) {
+            __nv_bfloat16* c = ep.C16 + pr * ep.ldc16 + pc;
+            const bool wlo = SPLIT && ep.c16_lo != 0;  // also write the lo plane (c16_lo is a multiple of 8 elements)
+            const bool vec = (ep.ldc16 & 7) == 0 && (reinterpret_cast<uintptr_t>(c) & 15) == 0;
+#pragma unroll
+            for (int j = 0; j < 32; j += 8) {
+              if (vec && nbase + j + 8 <= N) {
+                uint4 ph, pl;
+                split_bf16x2(o[j], o[j + 1], ph.x, pl.x); split_bf16x2(o[j + 2], o[j + 3], ph.y, pl.y);
+                split_bf16x2(o[j + 4], o[j + 5], ph.z, pl.z); split_bf16x2(o[j + 6], o[j + 7], ph.w, pl.w);
+                *reinterpret_cast<uint4*>(c + j) = ph;
+                if (wlo) *reinterpret_cast<uint4*>(c + ep.c16_lo + j) = pl;
+              } else {
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj)
+                  if (nbase + j + jj < N) {
+                    const __nv_bfloat16 hb = __float2bfloat16_rn(o[j + jj]);
+                    c[j + jj] = hb;
+                    if (wlo) c[ep.c16_lo + j + jj] = bf16_lo_of(o[j + jj], hb);
+                  }
+              }
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
 struct TcMaps { CUtensorMap a, b, al, bl; };  // operand maps (+ lo planes in split mode; copies of a / b otherwise)
 
 // cudaFuncSetAttribute is per device: remember which devices have had it applied for this instantiation
@@ -445,37 +690,40 @@ static inline bool attr_done(uint64_t* mask) {
   return false;
 }
 
-// dynamic shared memory of gemm_tc_kernel: 1 KB alignment slack, the stage ring, the barriers, the accumulator staging tile
-constexpr size_t tc_smem(int block_n, int stages, bool split) {
-  return 1024 + size_t(stages) * (split ? 2 : 1) * (kABytes + size_t(block_n) * kBlockK * 2) + 16 * stages +
+// dynamic shared memory of gemm_tc_kernel / conv_tc_kernel with tm-row tiles: 1 KB alignment slack, the stage ring,
+// the barriers, the accumulator staging (one 128-row tile, or two 64-row tiles)
+constexpr size_t tc_smem(int tm, int block_n, int stages, bool split) {
+  return 1024 + size_t(stages) * (split ? 2 : 1) * (size_t(tm) * kBlockK * 2 + size_t(block_n) * kBlockK * 2) + 16 * stages +
          size_t(kBlockM) * (block_n + 4) * 4 + 16;
 }
-// the deepest ring of at most `want` stages that fits beside the staging tile
-constexpr int tc_stages(int block_n, int want, bool split) {
-  return (want <= 2 || tc_smem(block_n, want, split) <= 227 * 1024) ? want : tc_stages(block_n, want - 1, split);
+// the deepest ring of at most `want` stages that fits beside the staging tiles.  Depths of the convolutions: 128-row
+// tiles 4 stages (2 for the stride-2 input gradient: 4 k-blocks per tile), 256-row tiles (BLOCK_N <= 64) 4 single-plane,
+// 2 split (80 KB per stage)
+constexpr int tc_stages(int tm, int block_n, int want, bool split) {
+  return (want <= 2 || tc_smem(tm, block_n, want, split) <= 227 * 1024) ? want : tc_stages(tm, block_n, want - 1, split);
 }
 
 // CTAs of `kernel` resident per SM with `smem` bytes of dynamic shared memory: registers, not shared memory, are the
 // limit for most instantiations (a 128-column accumulator pair plus the epilogue needs > 204 registers per thread)
 template <typename Kernel>
-static int resident_per_sm(Kernel kernel, size_t smem) {
+static int resident_per_sm(Kernel kernel, int threads, size_t smem) {
   int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kThreads, smem) != cudaSuccess || n < 1) n = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, threads, smem) != cudaSuccess || n < 1) n = 1;
   return n;
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool SPLIT>
 int launch_e(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
              float* partial, cudaStream_t stream) {
-  constexpr size_t smem = tc_smem(BLOCK_N, kStages, SPLIT);
+  constexpr size_t smem = tc_smem(kBlockM, BLOCK_N, kStages, SPLIT);
   static_assert(smem <= 227 * 1024, "gemm_tc: stage ring exceeds shared memory");
   static uint64_t attr = 0;
   static int per_sm = 1;
   if (!attr_done(&attr)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT>,
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT>, smem);
+    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT>, kThreads, smem);
   }
   const int64_t tiles_m = (M + kBlockM - 1) / kBlockM, tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n * splits;
@@ -484,7 +732,7 @@ int launch_e(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64
   int64_t grid = int64_t(kNumSMs) * per_sm;
   if (ep.max_ctas > 0 && grid > ep.max_ctas) grid = ep.max_ctas;
   if (grid > total) grid = total;
-  gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, false, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
+  gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
       mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), partial, int(tiles_m), int(tiles_n), splits,
       int((N + 31) & ~int64_t(31)));
   return check_launch("gemm_tc_kernel");
@@ -511,10 +759,10 @@ int launch(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t
   const bool split = ep.a_lo != 0;
   if (split) {
     if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, true>(mp, ep, M, N, K, splits, partial, stream);
-    return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(BLOCK_N, 4, true), true>(mp, ep, M, N, K, splits, partial, stream);
+    return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(kBlockM, BLOCK_N, 4, true), true>(mp, ep, M, N, K, splits, partial, stream);
   }
   if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, false>(mp, ep, M, N, K, splits, partial, stream);
-  return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(BLOCK_N, 4, false), false>(mp, ep, M, N, K, splits, partial, stream);
+  return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(kBlockM, BLOCK_N, 4, false), false>(mp, ep, M, N, K, splits, partial, stream);
 }
 
 
@@ -635,34 +883,50 @@ conv_wgrad_implicit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid
   }
 }
 
-template <int BLOCK_N, int EPI, int kSt, bool SPLIT>
+template <int TM, int BLOCK_N, int EPI, int kSt, bool SPLIT>
 int launch_conv_fwd_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K,
                       int64_t tiles_m, const ImplicitConv& ic, cudaStream_t stream) {
-  constexpr size_t smem = tc_smem(BLOCK_N, kSt, SPLIT);
+  constexpr size_t smem = tc_smem(TM, BLOCK_N, kSt, SPLIT);
   static_assert(smem <= 227 * 1024, "gemm_tc: stage ring exceeds shared memory");
+  TB_REQUIRE(!ep.mask && !ep.addend16 && !ep.addend32 && (EPI >= 2 || !ep.mask16),
+             "conv_tc_kernel: the convolution epilogue takes scale / bias / ReLU (+ a bf16 ReLU mask in the input gradient)");
   static uint64_t attr = 0;
   static int per_sm = 1;
   if (!attr_done(&attr)) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT>,
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT>, smem);
+    per_sm = resident_per_sm(conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT>, kConvThreads, smem);
   }
   const int64_t tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n;
   int64_t grid = int64_t(kNumSMs) * per_sm;
   if (grid > total) grid = total;
-  gemm_tc_kernel<BLOCK_N, false, false, kSt, EPI, true, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
-      mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), nullptr, int(tiles_m), int(tiles_n), 1, 0, ic);
+  conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT><<<(unsigned)grid, kConvThreads, smem, stream>>>(
+      mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), int(tiles_m), int(tiles_n), ic);
   return check_launch("gemm_tc_kernel(implicit conv)");
 }
 
-template <int BLOCK_N, int EPI = 1, int kSt = 4>
+template <int TM, int BLOCK_N, int EPI = 1, int kSt = 4>
 int launch_conv_fwd(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int64_t tiles_m,
                     const ImplicitConv& ic, cudaStream_t stream) {
   if (ep.a_lo != 0)  // split: stages of twice the size
-    return launch_conv_fwd_s<BLOCK_N, EPI, tc_stages(BLOCK_N, kSt, true), true>(mp, ep, M, N, K, tiles_m, ic, stream);
-  return launch_conv_fwd_s<BLOCK_N, EPI, tc_stages(BLOCK_N, kSt, false), false>(mp, ep, M, N, K, tiles_m, ic, stream);
+    return launch_conv_fwd_s<TM, BLOCK_N, EPI, tc_stages(TM, BLOCK_N, kSt, true), true>(mp, ep, M, N, K, tiles_m, ic, stream);
+  return launch_conv_fwd_s<TM, BLOCK_N, EPI, tc_stages(TM, BLOCK_N, kSt, false), false>(mp, ep, M, N, K, tiles_m, ic, stream);
+}
+
+// Tile height of an implicit convolution with `pix` output pixels per frame and Nf frames: 256 rows (fpt = 256 / pix whole
+// frames) where that shortens the busiest CTA's MMA work, counted as waves of tiles x 64-row groups per tile.  At the
+// learner's 2592 frames: 81 pixels 7 x 4 instead of 20 x 2 (243 of 256 rows useful instead of 81 of 128), 49 pixels
+// 4 x 4 instead of 10 x 2; 100 pixels gain nothing (200/256 = 100/128).  Small batches (the acting forward) whose
+// 128-row tiles fill about one wave keep 128 rows: a 256-row tile there only adds row groups of padding.  BLOCK_N = 128
+// keeps 128 rows: four 64 x 128 accumulators do not fit in the registers.
+static int implicit_tile_rows(int pix, int bn, int64_t Nf) {
+  auto span = [&](int tm) {
+    const int64_t fpt = tm / pix, tiles = (Nf + fpt - 1) / fpt;
+    return ((tiles + kNumSMs - 1) / kNumSMs) * (tm / 64);
+  };
+  return (bn <= 64 && span(2 * kBlockM) < span(kBlockM)) ? 2 * kBlockM : kBlockM;
 }
 
 }  // namespace
@@ -681,9 +945,10 @@ int conv_tc_fwd_implicit(const void* act_nhwc_bf16, const void* w_packed_bf16, i
   if (Nf == 0) return 0;
   ProfScope prof(ep.tag, stream);
   const int OH = (H - KH) / S + 1, OW = (W - KW) / S + 1;
+  const int bn = (O <= 32) ? 32 : (O <= 64 ? 64 : 128);
+  const int tm = implicit_tile_rows(OW * OH, bn, Nf);
   ImplicitConv ic;
-  ic.fpt = kBlockM / (OW * OH);
-  if (ic.fpt > 256) ic.fpt = 256;
+  ic.fpt = tm / (OW * OH);  // <= 256: the frame dimension of the TMA box
   ic.rows = OW * OH * ic.fpt;
   ic.kbw = KW * C / kBlockK;
   ic.row_elems = W * C;
@@ -696,7 +961,6 @@ int conv_tc_fwd_implicit(const void* act_nhwc_bf16, const void* w_packed_bf16, i
   TcMaps mp;
   int rc = make_map_nd(&mp.a, act_nhwc_bf16, 4, dims, strides, box);
   if (rc) return rc;
-  const int bn = (O <= 32) ? 32 : (O <= 64 ? 64 : 128);
   rc = make_map(&mp.b, w_packed_bf16, O, K, K, bn);
   if (rc) return rc;
   mp.al = mp.a; mp.bl = mp.b;
@@ -706,9 +970,11 @@ int conv_tc_fwd_implicit(const void* act_nhwc_bf16, const void* w_packed_bf16, i
     rc = make_map(&mp.bl, static_cast<const __nv_bfloat16*>(w_packed_bf16) + ep.b_lo, O, K, K, bn);
     if (rc) return rc;
   }
-  if (bn == 32) return launch_conv_fwd<32>(mp, ep, M, O, K, tiles_m, ic, stream);
-  if (bn == 64) return launch_conv_fwd<64>(mp, ep, M, O, K, tiles_m, ic, stream);
-  return launch_conv_fwd<128>(mp, ep, M, O, K, tiles_m, ic, stream);
+  if (bn == 32) return tm == kBlockM ? launch_conv_fwd<kBlockM, 32>(mp, ep, M, O, K, tiles_m, ic, stream)
+                                     : launch_conv_fwd<2 * kBlockM, 32>(mp, ep, M, O, K, tiles_m, ic, stream);
+  if (bn == 64) return tm == kBlockM ? launch_conv_fwd<kBlockM, 64>(mp, ep, M, O, K, tiles_m, ic, stream)
+                                     : launch_conv_fwd<2 * kBlockM, 64>(mp, ep, M, O, K, tiles_m, ic, stream);
+  return launch_conv_fwd<kBlockM, 128>(mp, ep, M, O, K, tiles_m, ic, stream);
 }
 
 bool conv_tc_dgrad_implicit_applicable(int H, int W, int C, int KH, int KW, int S, int O) {
@@ -741,12 +1007,14 @@ int conv_tc_dgrad_implicit(const void* dy_nhwc_bf16, const void* wt_bf16, int64_
   const uint64_t strides[3] = {uint64_t(O) * 2, uint64_t(OW) * O * 2, uint64_t(OH) * OW * O * 2};
   int rc;
   if (S == 1) {
-    ic.mode = 1; ic.rows = H * W; ic.kbw = KW;
-    const uint32_t box[4] = {uint32_t(kBlockK), uint32_t(W), uint32_t(H), 1u};
+    const int bn = (C <= 32) ? 32 : (C <= 64 ? 64 : 128);
+    const int tm = implicit_tile_rows(H * W, bn, Nf);
+    ic.mode = 1; ic.fpt = tm / (H * W); ic.rows = H * W * ic.fpt; ic.kbw = KW;
+    const uint32_t box[4] = {uint32_t(kBlockK), uint32_t(W), uint32_t(H), uint32_t(ic.fpt)};
     rc = make_map_nd(&mp.a, dy_nhwc_bf16, 4, dims, strides, box);
     if (rc) return rc;
-    const int64_t K = int64_t(KH) * KW * O, M = Nf * ic.rows;
-    const int bn = (C <= 32) ? 32 : (C <= 64 ? 64 : 128);
+    const int64_t K = int64_t(KH) * KW * O, M = Nf * H * W;
+    const int64_t tiles_m = (Nf + ic.fpt - 1) / ic.fpt;
     rc = make_map(&mp.b, wt_bf16, C, K, K, bn);
     if (rc) return rc;
     mp.al = mp.a; mp.bl = mp.b;
@@ -756,10 +1024,13 @@ int conv_tc_dgrad_implicit(const void* dy_nhwc_bf16, const void* wt_bf16, int64_
       rc = make_map(&mp.bl, wt_lo, C, K, K, bn);
       if (rc) return rc;
     }
-    if (bn == 32) return launch_conv_fwd<32, 2>(mp, ep, M, C, K, Nf, ic, stream);
-    if (bn == 64) return launch_conv_fwd<64, 2>(mp, ep, M, C, K, Nf, ic, stream);
-    return launch_conv_fwd<128, 2>(mp, ep, M, C, K, Nf, ic, stream);
+    if (bn == 32) return tm == kBlockM ? launch_conv_fwd<kBlockM, 32, 2>(mp, ep, M, C, K, tiles_m, ic, stream)
+                                       : launch_conv_fwd<2 * kBlockM, 32, 2>(mp, ep, M, C, K, tiles_m, ic, stream);
+    if (bn == 64) return tm == kBlockM ? launch_conv_fwd<kBlockM, 64, 2>(mp, ep, M, C, K, tiles_m, ic, stream)
+                                       : launch_conv_fwd<2 * kBlockM, 64, 2>(mp, ep, M, C, K, tiles_m, ic, stream);
+    return launch_conv_fwd<kBlockM, 128, 2>(mp, ep, M, C, K, tiles_m, ic, stream);
   }
+  // the parity-class scatter assumes one frame per tile (100 pixels of conv2 gain nothing from 256 rows anyway)
   ic.mode = 2; ic.tw = W / 2; ic.rows = (H / 2) * (W / 2); ic.kbw = KW / 2; ic.outH = H; ic.outW = W;
   const uint32_t box[4] = {uint32_t(kBlockK), uint32_t(W / 2), uint32_t(H / 2), 1u};
   rc = make_map_nd(&mp.a, dy_nhwc_bf16, 4, dims, strides, box);
@@ -775,7 +1046,7 @@ int conv_tc_dgrad_implicit(const void* dy_nhwc_bf16, const void* wt_bf16, int64_
     if (rc) return rc;
   }
   // 4 k-blocks per tile: a 2-stage ring holds the next tile's operands while the epilogue runs
-  return launch_conv_fwd<128, 2, 2>(mp, ep, M, 4 * C, K, Nf, ic, stream);
+  return launch_conv_fwd<kBlockM, 128, 2, 2>(mp, ep, M, 4 * C, K, Nf, ic, stream);
 }
 
 template <int kSt, bool SPLIT>
