@@ -219,6 +219,31 @@ int tb_resnet_backward_obs(const uint8_t* frame, const float* grad_logits, const
                            int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* grads,
                            void* stream);
 
+/* ---- IMPALA ResNet with other section widths -------------------------------------------------------------------------
+ * The tb_resnet_*_obs entry points with the channel counts (c0, c1, c2) of the three sections after C, H, W; the _obs
+ * entries are the (16, 32, 32) case of these.  Each section takes 16, 32 or 64 channels, in any combination, over the
+ * whole observation range above, on every precision (tb_resnet_widths writes {16, 32, 64}); e.g. (32, 64, 64) is the
+ * "IMPALA x2" net.  Parameter layout (state_dict order, as for the default):
+ *   feat_convs.0.0.weight (c0, C, 3, 3), and for i >= 1 feat_convs.i.0.weight (c_i, c_{i-1}, 3, 3); feat_convs.i.0.bias (c_i)
+ *   resnet1.i.{1,3}.weight / resnet2.i.{1,3}.weight (c_i, c_i, 3, 3) and their biases (c_i)
+ *   fc.weight (256, c2 * H_3 * W_3), fc.bias (256), then the LSTM and the heads unchanged.
+ * tb_resnet_arch_supported returns 1 for a supported (shape, widths, precision) and otherwise 0 with tb_last_error set;
+ * the other entries fail the same way (param count -1, workspace 0).  Unstacked rollouts stay (4, 84, 84) x (16, 32, 32). */
+int tb_resnet_widths(int* widths);
+int tb_resnet_arch_supported(int C, int H, int W, int c0, int c1, int c2, int precision);
+int64_t tb_resnet_param_count_arch(int C, int H, int W, int c0, int c1, int c2, int num_actions, int num_values,
+                                   int use_lstm);
+size_t tb_resnet_workspace_bytes_arch(int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B,
+                                      int num_actions, int use_lstm, int precision);
+int tb_resnet_forward_arch(const uint8_t* frame, const float* reward, const float* notdone, const float* h0,
+                           const float* c0, const float* params, int C, int H, int W, int ch0, int ch1, int ch2,
+                           int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                           void* workspace, float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
+int tb_resnet_backward_arch(const uint8_t* frame, const float* grad_logits, const float* grad_baseline,
+                            const float* notdone, const float* params, int C, int H, int W, int c0, int c1, int c2,
+                            int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                            void* workspace, float* grads, void* stream);
+
 /* ---- seeded action sampling for the acting forward ------------------------------------ */
 
 /* monobeast.py:618-619 / polybeast_learner.py:256-257  torch.multinomial(F.softmax(policy_logits, dim=1), 1) as a

@@ -50,6 +50,12 @@ _SIGNATURES = {
     "tb_resnet_workspace_bytes_obs": ([_int] * 3 + [_i64, _i64, _int, _int, _int], _c.c_size_t),
     "tb_resnet_forward_obs": ([_vp] * 6 + [_int] * 3 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
     "tb_resnet_backward_obs": ([_vp] * 5 + [_int] * 3 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_resnet_widths": ([_vp], _int),
+    "tb_resnet_arch_supported": ([_int] * 7, _int),
+    "tb_resnet_param_count_arch": ([_int] * 9, _i64),
+    "tb_resnet_workspace_bytes_arch": ([_int] * 6 + [_i64, _i64, _int, _int, _int], _c.c_size_t),
+    "tb_resnet_forward_arch": ([_vp] * 6 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
+    "tb_resnet_backward_arch": ([_vp] * 5 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f32": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),

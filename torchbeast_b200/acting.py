@@ -227,6 +227,11 @@ class GraphedActor:
         if history is not None and obs != nets.ATARI_SHAPE:
             raise _lib.TorchBeastB200Error("a frame_history rebuilds (4, 84, 84) stacks; this net takes stacked frames "
                                            "[1, B, %d, %d, %d]: detach the history (model.frame_history = None)" % obs)
+        channels = tuple(getattr(model, "channels", nets.RESNET_CHANNELS))
+        if history is not None and channels != nets.RESNET_CHANNELS:
+            raise _lib.TorchBeastB200Error("a frame_history feeds the default widths %r; this net has channels=%r and "
+                                           "takes stacked frames: detach the history (model.frame_history = None)"
+                                           % (nets.RESNET_CHANNELS, channels))
         if newest and (frame.dtype != torch.uint8 or tuple(frame.shape[2:]) != (84, 84)):
             raise _lib.TorchBeastB200Error("GraphedActor with a frame_history takes stacked frames or the newest frames "
                                            "uint8 [1, B, 84, 84], got %s %r" % (frame.dtype, tuple(frame.shape)))

@@ -306,6 +306,256 @@ int launch_sw_fwd(const SwFwdArgs& a, cudaStream_t stream) {
   return check_launch("sw_conv_fwd_kernel");
 }
 
+// ---- forward with a 64-channel side (or a 32 -> 32 row too wide for the kernel above) -------------------------------
+// The kernel above keeps all weights resident and a whole tile's window (every chunk plane) per ring stage: at 64 -> 64
+// and W = 63 that is 144 KiB of weights + 4 x 66 KiB of windows.  This one (any pair with CK or NO = 64, and the 16 / 32
+// pairs the kernel above does not fit, e.g. 32 -> 32 at W = 63 in a 32-wide first section) changes two things and keeps
+// the image format, the tile, the split product and the epilogue:
+//   - output columns in blocks of NT = min(NO, 32): a CTA owns ONE block (blockIdx.x % NCB, the grid is a multiple of
+//     NCB) and keeps only that block's weights (<= 72 KiB); the CTAs of the NCB blocks of a tile read its window from L2;
+//   - the window is streamed one k16 step (2 chunk planes, hi + lo) per ring stage, KP = CK/16 stages per tile, accumulating
+//     into the same registers.  Each consumer group has its own 2-stage ring: a group then waits only on stages it released
+//     itself, so a parity wait cannot match a phase two rounds old however many stages a tile takes.
+// Shared memory at the widest rows the nets use: 64 -> 64 at W = 63: 72 KiB weights + 4 x 16.5 KiB stages + 2 x 18 KiB
+// staging + 33 KiB column-sum staging = 207 KiB; 16 -> 64 at W = 126: 18 + 4 x 24.5 + 36 + 33 = 185 KiB.
+constexpr int kWideGroupStages = 2;
+constexpr int kWideStages = 2 * kWideGroupStages;
+
+template <int CK, int NO>
+__global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_wide_kernel(SwFwdArgs a) {
+  constexpr int CH = CK / 8, KP = CK / 16;
+  constexpr int NT = NO < 32 ? NO : 32, NCB = NO / NT;
+  constexpr uint32_t W_BLOCK = 36u * CK * NT;       // bytes of one column block's [w_hi | w_lo] operand
+  constexpr int LDS = NT + 4;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_addr(smem_raw) + 127u) & ~127u;
+  const uint32_t chb = uint32_t(a.g.pin) * 16u;
+  const uint32_t stage_bytes = 4u * chb;            // [plane hi / lo][chunk 2*ks / 2*ks + 1][pixel][16 B]
+  const uint32_t sW = base;
+  const uint32_t sX = sW + W_BLOCK;
+  const uint32_t bars = sX + kWideStages * stage_bytes;
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (kWideStages + s); };
+  const uint32_t wbar = bars + 8u * (2 * kWideStages);
+  __shared__ float csum_s[8][32][NT + 1];
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int cb = blockIdx.x % NCB, G = gridDim.x / NCB, wb = blockIdx.x / NCB;
+  const int total_work = a.Nf * a.g.tpf;
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < kWideStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
+    mbar_init(wbar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      mbar_expect_tx(wbar, W_BLOCK);
+      bulk_g2s(sW, a.wk + int64_t(cb) * (W_BLOCK / 2), W_BLOCK, wbar);
+      int cnt0 = 0, cnt1 = 0;   // ring items issued per consumer group
+      for (int w = wb, it = 0; w < total_work; w += G, ++it) {
+        const int grp = it & 1;
+        const int n = w / a.g.tpf, p0 = (w - n * a.g.tpf) * kTile;
+#pragma unroll
+        for (int ks = 0; ks < KP; ++ks) {
+          const int item = grp ? cnt1++ : cnt0++;
+          const int stage = grp * kWideGroupStages + item % kWideGroupStages;
+          mbar_wait(empty(stage), (uint32_t(item / kWideGroupStages) & 1u) ^ 1u);
+          mbar_expect_tx(full(stage), stage_bytes);
+          const uint32_t st = sX + stage * stage_bytes;
+#pragma unroll
+          for (int pl = 0; pl < 2; ++pl)
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              const __nv_bfloat16* src =
+                  a.img + (pl ? a.img_lo : 0) + (int64_t(n) * CH + 2 * ks + j) * a.g.plane + int64_t(p0) * 8;
+              bulk_g2s(st + (pl * 2 + j) * chb, src, chb, full(stage));
+            }
+        }
+      }
+    }
+  } else {
+    const int quarter = warp & 3, ew = warp, grp = ew >> 2;
+    const int rl = quarter * 32 + lane;
+    float* stg = reinterpret_cast<float*>(smem_raw + (wbar + 16u - smem_addr(smem_raw))) + grp * kTile * LDS;
+    const int c0 = cb * NT;   // first output column of this CTA
+    mbar_wait(wbar, 0);
+    int item = 0;
+    for (int w = wb + grp * G; w < total_work; w += 2 * G) {
+      const int n = w / a.g.tpf, p = (w - n * a.g.tpf) * kTile + rl;
+      const int y = p / a.g.Wp, x = p - y * a.g.Wp;
+      const bool valid = x < a.g.W && y < a.g.H;
+      const int64_t r = (int64_t(n) * a.g.H + y) * a.g.W + x;
+      if (valid) {
+        if (a.mask) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.mask + r * NO + c0));
+        if (a.addend) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.addend + r * NO + c0));
+      }
+      float acc[2][NT];
+#pragma unroll
+      for (int ks = 0; ks < KP; ++ks, ++item) {
+        const int stage = grp * kWideGroupStages + item % kWideGroupStages;
+        mbar_wait(full(stage), uint32_t(item / kWideGroupStages) & 1u);
+        wgmma_fence();
+        const uint32_t st = sX + stage * stage_bytes;
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t shift = uint32_t((tap / 3) * a.g.Wp + (tap % 3)) * 16u;
+          const uint32_t wa = sW + uint32_t((tap * KP + ks) * 2 * 2 * NT) * 16u;
+          const uint64_t dbw = desc_k_noswz(wa, 2u * NT * 16u, 128u);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t xa = st + shift + h * 1024u;
+            const uint64_t dah = desc_k_noswz(xa, chb, 128u), dal = desc_k_noswz(xa + 2u * chb, chb, 128u);
+            wgmma_bf16<2 * NT>(acc[h], dah, dbw, (ks | tap) != 0);
+            wgmma_bf16<NT>(acc[h], dal, dbw, 1);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty(stage));
+      }
+      named_sync(1 + grp, 128);
+      {
+        const int fr = quarter * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < NT / 8; ++j) {
+            float* sp = stg + (h * 64 + fr) * LDS + 8 * j + fc;
+            *reinterpret_cast<float2*>(sp) = make_float2(acc[h][4 * j] + acc[h][4 * j + NT / 2], acc[h][4 * j + 1] + acc[h][4 * j + 1 + NT / 2]);
+            *reinterpret_cast<float2*>(sp + 8 * LDS) =
+                make_float2(acc[h][4 * j + 2] + acc[h][4 * j + 2 + NT / 2], acc[h][4 * j + 3] + acc[h][4 * j + 3 + NT / 2]);
+          }
+      }
+      named_sync(1 + grp, 128);
+      float o[NT];
+#pragma unroll
+      for (int j = 0; j < NT; ++j) o[j] = 0.f;
+      if (valid) {
+#pragma unroll
+        for (int j = 0; j < NT; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(stg + rl * LDS + j);
+          o[j] = t.x * a.scale; o[j + 1] = t.y * a.scale; o[j + 2] = t.z * a.scale; o[j + 3] = t.w * a.scale;
+        }
+        if (a.bias) {
+#pragma unroll
+          for (int q = 0; q < NT / 4; ++q) {
+            const float4 b4 = __ldg(reinterpret_cast<const float4*>(a.bias + c0) + q);
+            o[4 * q] += b4.x; o[4 * q + 1] += b4.y; o[4 * q + 2] += b4.z; o[4 * q + 3] += b4.w;
+          }
+        }
+        if (a.mask) {
+          const float4* mp = reinterpret_cast<const float4*>(a.mask + r * NO + c0);
+#pragma unroll
+          for (int q = 0; q < NT / 4; ++q) {
+            const float4 m4 = __ldg(mp + q);
+            o[4 * q] = m4.x > 0.f ? o[4 * q] : 0.f; o[4 * q + 1] = m4.y > 0.f ? o[4 * q + 1] : 0.f;
+            o[4 * q + 2] = m4.z > 0.f ? o[4 * q + 2] : 0.f; o[4 * q + 3] = m4.w > 0.f ? o[4 * q + 3] : 0.f;
+          }
+        }
+        if (a.addend) {
+          const float4* ap = reinterpret_cast<const float4*>(a.addend + r * NO + c0);
+#pragma unroll
+          for (int q = 0; q < NT / 4; ++q) {
+            const float4 a4 = __ldg(ap + q);
+            o[4 * q] += a4.x; o[4 * q + 1] += a4.y; o[4 * q + 2] += a4.z; o[4 * q + 3] += a4.w;
+          }
+        }
+        float4* op = reinterpret_cast<float4*>(a.out + r * NO + c0);
+#pragma unroll
+        for (int q = 0; q < NT / 4; ++q) op[q] = make_float4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
+      }
+      if (a.emit) {   // as in sw_conv_fwd_kernel, for this CTA's chunk planes c0/8 .. (c0 + NT)/8 - 1
+        const int hpwp = a.g.Hp * a.g.Wp, t = w - n * a.g.tpf;
+        const int64_t fbase = (int64_t(n) * (NO / 8) + c0 / 8) * hpwp;
+        auto put = [&](int q, int c, uint4 ph, uint4 pl) {
+          __nv_bfloat16* dst = a.emit + (fbase + int64_t(c) * hpwp + q) * 8;
+          *reinterpret_cast<uint4*>(dst) = ph;
+          *reinterpret_cast<uint4*>(dst + a.emit_lo) = pl;
+        };
+        const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+        const int q = p + a.g.Wp + 1;
+        if (q < hpwp) {
+#pragma unroll
+          for (int c = 0; c < NT / 8; ++c) {
+            uint4 ph, pl;
+            float e[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) e[j] = a.emit_relu ? fmaxf(o[8 * c + j], 0.f) : o[8 * c + j];
+            split_bf16x2(e[0], e[1], ph.x, pl.x); split_bf16x2(e[2], e[3], ph.y, pl.y);
+            split_bf16x2(e[4], e[5], ph.z, pl.z); split_bf16x2(e[6], e[7], ph.w, pl.w);
+            put(q, c, ph, pl);
+          }
+        }
+        if (t == 0 && rl < a.g.Wp + 1) {
+#pragma unroll
+          for (int c = 0; c < NT / 8; ++c) put(rl, c, z, z);
+        }
+        if (t == a.g.tpf - 1) {
+          const int q2 = a.g.tpf * kTile + a.g.Wp + 1 + rl;
+          if (q2 < hpwp) {
+#pragma unroll
+            for (int c = 0; c < NT / 8; ++c) put(q2, c, z, z);
+          }
+        }
+        if (w == 0 && cb == 0) {
+          const int64_t body = int64_t(a.Nf) * (NO / 8) * hpwp * 8;
+          for (int u = rl; u < a.g.pin + 8; u += 128) {
+            *reinterpret_cast<uint4*>(a.emit + body + int64_t(u) * 8) = z;
+            *reinterpret_cast<uint4*>(a.emit + a.emit_lo + body + int64_t(u) * 8) = z;
+          }
+        }
+      }
+      if (a.csum) {
+#pragma unroll
+        for (int j = 0; j < NT; ++j) csum_s[ew][lane][j] = o[j];
+        __syncwarp();
+        if (lane < NT) {
+          float sum = 0.f;
+#pragma unroll 8
+          for (int rr = 0; rr < 32; ++rr) sum += csum_s[ew][rr][lane];
+          a.csum[(int64_t(w) * 4 + quarter) * NO + c0 + lane] = sum;
+        }
+        __syncwarp();
+      }
+    }
+  }
+}
+
+// dynamic shared memory of the wide forward kernel (+ its static column-sum staging, which counts against the same 227 KiB)
+inline size_t sw_fwd_wide_smem(int pin, int CK, int NO) {
+  const int NT = NO < 32 ? NO : 32;
+  return 128 + size_t(36) * CK * NT + size_t(kWideStages) * 4 * pin * 16 + 8 * (2 * kWideStages + 2) +
+         2 * size_t(kTile) * (NT + 4) * sizeof(float) + 16;
+}
+inline size_t sw_fwd_wide_static(int NO) { return sizeof(float) * 8 * 32 * ((NO < 32 ? NO : 32) + 1); }
+
+template <int CK, int NO>
+int launch_sw_fwd_wide(const SwFwdArgs& a, cudaStream_t stream) {
+  constexpr int NCB = NO < 32 ? 1 : NO / 32;
+  const size_t smem = sw_fwd_wide_smem(a.g.pin, CK, NO);
+  TB_REQUIRE(smem + sw_fwd_wide_static(NO) <= 227 * 1024, "sw_conv_fwd: shared memory");
+  static size_t attr[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (attr[dev & 63] < smem) {
+    cudaError_t e = cudaFuncSetAttribute(sw_conv_fwd_wide_kernel<CK, NO>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    TB_REQUIRE(e == cudaSuccess, "sw_conv_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    attr[dev & 63] = smem;
+  }
+  int per_sm = int((224 * 1024) / (smem + sw_fwd_wide_static(NO) + 1024));
+  if (per_sm > 4) per_sm = 4;
+  if (per_sm < 1) per_sm = 1;
+  int64_t groups = int64_t(kNumSMs) * per_sm / NCB;   // CTAs per column block
+  const int64_t total = int64_t(a.Nf) * a.g.tpf;
+  if (groups > total) groups = total;
+  if (groups < 1) groups = 1;
+  sw_conv_fwd_wide_kernel<CK, NO><<<(unsigned)(groups * NCB), kSwThreads, smem, stream>>>(a);
+  return check_launch("sw_conv_fwd_wide_kernel");
+}
+
 // ---- weight gradient ------------------------------------------------------------------------------------------
 // dW[o, tap, c] = sum over pixels p of dY[p, o] * x[p + shift(tap), c]: M = O and N = C are 16..32 and the reduction runs
 // over pixels.  A wgmma atom is 64 rows, so three quarters of every MMA would be padding.  The
@@ -338,9 +588,15 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-template <int C, int O>
+// 64-channel sides: a CTA computes one (OT x CT) block of dW (OT, CT <= 32, block blockIdx.y of the O/OT x C/CT blocks),
+// loading only that block's dY and input chunk planes - the accumulators and the fold buffer are those of a 32 x 32 conv.
+// The blocks of a tile re-read its planes from L2 (each chunk plane is loaded by C/CT or O/OT blocks).
+template <int CF, int OF, int C = CF, int O = OF>
 __global__ void __launch_bounds__(kWgThreads, 1) sw_conv_wgrad_kernel(SwWgradArgs a) {
   constexpr int CC = C / 8, CO = O / 8, MT = O / 16, NP = C / 16;   // chunk planes; m16 tiles; pairs of n8 tiles
+  constexpr int CCF = CF / 8, COF = OF / 8, NBC = CF / C;           // chunk planes of the whole images; C blocks
+  const int blk = (NBC * (OF / O) > 1) ? int(blockIdx.y) : 0;
+  const int cc0 = (blk % NBC) * CC, co0 = (blk / NBC) * CO;         // first chunk plane of this block's x / dY
   constexpr uint32_t DY_CH = kTile * 16u;            // bytes of one dY chunk plane tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 127u) & ~127u;
@@ -372,12 +628,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) sw_conv_wgrad_kernel(SwWgradArg
         for (int pl = 0; pl < 2; ++pl) {
 #pragma unroll
           for (int c = 0; c < CO; ++c) {   // output pixel p is padded pixel p + Wp + 1 of the dY image
-            const __nv_bfloat16* src = a.dy + (pl ? a.dy_lo : 0) + (int64_t(n) * CO + c) * a.g.plane + int64_t(p0 + a.g.Wp + 1) * 8;
+            const __nv_bfloat16* src =
+                a.dy + (pl ? a.dy_lo : 0) + (int64_t(n) * COF + co0 + c) * a.g.plane + int64_t(p0 + a.g.Wp + 1) * 8;
             bulk_g2s(st + (pl * CO + c) * DY_CH, src, DY_CH, full(stage));
           }
 #pragma unroll
           for (int c = 0; c < CC; ++c) {
-            const __nv_bfloat16* src = a.x + (pl ? a.x_lo : 0) + (int64_t(n) * CC + c) * a.g.plane + int64_t(p0) * 8;
+            const __nv_bfloat16* src = a.x + (pl ? a.x_lo : 0) + (int64_t(n) * CCF + cc0 + c) * a.g.plane + int64_t(p0) * 8;
             bulk_g2s(st + dy_bytes + (pl * CC + c) * chb, src, chb, full(stage));
           }
         }
@@ -467,7 +724,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) sw_conv_wgrad_kernel(SwWgradArg
     }
     __syncthreads();
   }
-  float* dst = a.partial + int64_t(blockIdx.x) * O * (9 * C);
+  float* dst = a.partial + (int64_t(blk) * gridDim.x + blockIdx.x) * O * (9 * C);
   for (int i = threadIdx.x; i < O * 9 * C; i += kWgThreads) {
     const int o = i / (9 * C), col = i - o * (9 * C);
     dst[i] = red[col * LDR + o];
@@ -503,19 +760,23 @@ inline size_t sw_wgrad_smem(int pin, int C, int O) {
   return 384 + size_t(kWgStages) * (2 * size_t(O / 8) * kTile * 16 + 2 * size_t(C / 8) * pin * 16) + sizeof(float) * 9 * C * (O + 1);
 }
 
-template <int C, int O>
+// the (C, O) block a CTA of the weight gradient computes: the whole conv when both sides are 16 or 32, else 32-channel
+// blocks of the 64-channel sides
+inline int sw_wgrad_block(int n) { return n < 32 ? n : 32; }
+
+template <int C, int O, int CT = C, int OT = O>
 int launch_sw_wgrad(const SwWgradArgs& a, int grid, cudaStream_t stream) {
-  const size_t smem = sw_wgrad_smem(a.g.pin, C, O);
+  const size_t smem = sw_wgrad_smem(a.g.pin, CT, OT);
   TB_REQUIRE(smem <= 227 * 1024, "sw_conv_wgrad: shared memory");
   static size_t attr[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
   if (attr[dev & 63] < smem) {
-    cudaError_t e = cudaFuncSetAttribute(sw_conv_wgrad_kernel<C, O>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    cudaError_t e = cudaFuncSetAttribute(sw_conv_wgrad_kernel<C, O, CT, OT>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "sw_conv_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr[dev & 63] = smem;
   }
-  sw_conv_wgrad_kernel<C, O><<<grid, kWgThreads, smem, stream>>>(a);
+  sw_conv_wgrad_kernel<C, O, CT, OT><<<dim3(grid, (C / CT) * (O / OT)), kWgThreads, smem, stream>>>(a);
   return check_launch("sw_conv_wgrad_kernel");
 }
 
@@ -555,7 +816,7 @@ __global__ void __launch_bounds__(256) sw_pad_split_kernel(const float4* __restr
                                                            float* __restrict__ partial, int slack_units) {
   const int Hp = H + 2, Wp = W + 2;
   if (blockIdx.x == 0 && blockIdx.y == 0) zero_slack_units(out, lo_off, int64_t(gridDim.y) * C8 * Hp * Wp * 8, slack_units);
-  const int lc = (C8 == 4) ? 2 : (C8 == 2 ? 1 : 0);      // C8 is 1, 2 or 4
+  const int lc = (C8 == 8) ? 3 : (C8 == 4) ? 2 : (C8 == 2 ? 1 : 0);   // C8 is 1, 2, 4 or 8
   const int cv = threadIdx.x & (C8 - 1);
   const int p = blockIdx.x * (256 >> lc) + (threadIdx.x >> lc);
   const int64_t n = blockIdx.y;
@@ -602,7 +863,7 @@ __global__ void __launch_bounds__(256) sw_pool_bwd_image_kernel(const uint8_t* _
                                                                 int OW, int C8, float* __restrict__ partial, int slack_units) {
   const int Hp = H + 2, Wp = W + 2;
   if (blockIdx.x == 0 && blockIdx.y == 0) zero_slack_units(out, lo_off, int64_t(gridDim.y) * C8 * Hp * Wp * 8, slack_units);
-  const int lc = (C8 == 4) ? 2 : (C8 == 2 ? 1 : 0);
+  const int lc = (C8 == 8) ? 3 : (C8 == 4) ? 2 : (C8 == 2 ? 1 : 0);
   const int cv = threadIdx.x & (C8 - 1);
   const int p = blockIdx.x * (256 >> lc) + (threadIdx.x >> lc);
   const int64_t n = blockIdx.y;
@@ -748,27 +1009,31 @@ __global__ void __launch_bounds__(256) sw_colsum_l2_kernel(const float* __restri
 }
 
 __global__ void sw_pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ out, int O, int C, int transpose,
-                                       int c_real) {
+                                       int c_real, int RB) {
   const int R = transpose ? C : O, K = transpose ? O : C;   // operand rows, reduction channels
+  const int KP = K / 16, NB = 9 * KP * 2;
   const int64_t total = int64_t(9) * K * R;
   for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
-    // hi element index i = (((tap*KP + kp)*2 + j)*R + r)*8 + e; stored at row r (hi) and row R + r (lo) of a 2R-row block
+    // hi element index i = (((rb*9 + tap)*KP + kp)*2 + j)*RB + r_in)*8 + e for row r = rb*RB + r_in; stored at row r_in
+    // (hi) and row RB + r_in (lo) of a 2RB-row block: one complete operand per block of RB rows
     const int e = int(i & 7);
     int64_t t = i >> 3;
-    const int64_t blk = t / R;                     // ((tap*KP + kp)*2 + j)
-    const int r = int(t % R); t /= R;
-    const int j = int(t & 1); t >>= 1;
-    const int KP = K / 16;
-    const int kp = int(t % KP);
-    const int tap = int(t / KP);
+    const int r_in = int(t % RB); t /= RB;
+    const int64_t blk = t % NB;                    // ((tap*KP + kp)*2 + j)
+    const int rb = int(t / NB);
+    const int r = rb * RB + r_in;
+    const int j = int(blk & 1);
+    const int kp = int((blk >> 1) % KP);
+    const int tap = int((blk >> 1) / KP);
     const int k = kp * 16 + j * 8 + e;
     const int a = tap / 3, b = tap % 3;
     float v;
     if (transpose) v = w[((int64_t(k) * C + r) * 3 + (2 - a)) * 3 + (2 - b)];
     else v = k < c_real ? w[((int64_t(r) * c_real + k) * 3 + a) * 3 + b] : 0.0f;
     const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    out[(blk * 2 * R + r) * 8 + e] = h;
-    out[(blk * 2 * R + R + r) * 8 + e] = bf16_lo_of(v, h);
+    const int64_t ob = (int64_t(rb) * NB + blk) * 2 * RB;
+    out[(ob + r_in) * 8 + e] = h;
+    out[(ob + RB + r_in) * 8 + e] = bf16_lo_of(v, h);
   }
 }
 
@@ -874,19 +1139,37 @@ int sw_pack_weights(const float* w, __nv_bfloat16* out, int O, int C, int transp
   TB_REQUIRE(O % 16 == 0 && C % 16 == 0, "sw_pack_weights: channel counts must be multiples of 16");
   TB_REQUIRE(c_real == 0 || (!transpose && c_real <= C), "sw_pack_weights: c_real only for the forward operand");
   const int64_t total = int64_t(9) * O * C;
-  sw_pack_weights_kernel<<<sgrid(total, 256), 256, 0, stream>>>(w, out, O, C, transpose, c_real > 0 ? c_real : C);
+  const int R = transpose ? C : O;   // blocks of 32 operand rows: the wide forward kernel loads one block per CTA
+  sw_pack_weights_kernel<<<sgrid(total, 256), 256, 0, stream>>>(w, out, O, C, transpose, c_real > 0 ? c_real : C, R < 32 ? R : 32);
   return check_launch("sw_pack_weights_kernel");
 }
 
+namespace {
+bool sw_channels_ok(int c) { return c == 16 || c == 32 || c == 64; }
+// sw_conv_fwd_kernel (all weights and a whole window per stage) takes a 16 / 32-channel pair when it fits, static
+// column-sum staging included (32 -> 32 does not from W = 54 on); everything else runs on sw_conv_fwd_wide_kernel
+bool sw_fwd_resident(int pin, int CK, int NO) {
+  return CK <= 32 && NO <= 32 && sw_fwd_smem(pin, CK, NO) + sizeof(float) * 8 * 32 * (NO + 1) <= 227 * 1024;
+}
+// shared memory (dynamic + static) of the forward kernel that runs a CK -> NO conv at this window
+size_t sw_fwd_smem_any(int pin, int CK, int NO) {
+  return sw_fwd_resident(pin, CK, NO) ? sw_fwd_smem(pin, CK, NO) + sizeof(float) * 8 * 32 * (NO + 1)
+                                      : sw_fwd_wide_smem(pin, CK, NO) + sw_fwd_wide_static(NO);
+}
+}  // namespace
+
 bool sw_conv_applicable(int H, int W, int CK, int NO) {
-  return (CK == 16 || CK == 32) && (NO == 16 || NO == 32) && H >= 3 && W >= 3 && W <= 126;
+  if (!(sw_channels_ok(CK) && sw_channels_ok(NO) && H >= 3 && W >= 3 && W <= 126)) return false;
+  // a 64 -> 32 / 64 window fits up to W = 101
+  return sw_fwd_smem_any(sw_geom(H, W).pin, CK, NO) <= 227 * 1024;
 }
 
-bool sw_conv_trainable(int H, int W, int CK, int NO) {
-  if (!sw_conv_applicable(H, W, CK, NO) || W < kWgMinW) return false;
+bool sw_conv_trainable(int H, int W, int CK, int NO, bool input_grad) {
+  if (!sw_conv_applicable(H, W, CK, NO) || (input_grad && !sw_conv_applicable(H, W, NO, CK)) || W < kWgMinW) return false;
   const int pin = sw_geom(H, W).pin;
   const size_t limit = 227 * 1024;
-  return sw_fwd_smem(pin, CK, NO) <= limit && sw_fwd_smem(pin, NO, CK) <= limit && sw_wgrad_smem(pin, CK, NO) <= limit;
+  return sw_fwd_smem_any(pin, CK, NO) <= limit && (!input_grad || sw_fwd_smem_any(pin, NO, CK) <= limit) &&
+         sw_wgrad_smem(pin, sw_wgrad_block(CK), sw_wgrad_block(NO)) <= limit;
 }
 
 int64_t sw_colsum_scratch_floats(int64_t Nf, int H, int W, int C) {
@@ -910,10 +1193,21 @@ int sw_conv_fwd(const __nv_bfloat16* img, int64_t img_lo, const __nv_bfloat16* w
   a.emit = ep.emit; a.emit_lo = ep.emit_lo; a.emit_relu = ep.emit_relu; a.csum = ep.csum;
   TB_REQUIRE(!ep.emit || (ep.emit_lo > 0 && ep.emit_lo % 8 == 0 && (reinterpret_cast<uintptr_t>(ep.emit) & 15) == 0),
              "sw_conv_fwd: the emitted image needs a 16-byte aligned base and a lo plane");
-  if (CK == 16 && NO == 16) return launch_sw_fwd<16, 16>(a, stream);
-  if (CK == 16 && NO == 32) return launch_sw_fwd<16, 32>(a, stream);
-  if (CK == 32 && NO == 16) return launch_sw_fwd<32, 16>(a, stream);
-  return launch_sw_fwd<32, 32>(a, stream);
+  if (sw_fwd_resident(a.g.pin, CK, NO)) {
+    if (CK == 16 && NO == 16) return launch_sw_fwd<16, 16>(a, stream);
+    if (CK == 16 && NO == 32) return launch_sw_fwd<16, 32>(a, stream);
+    if (CK == 32 && NO == 16) return launch_sw_fwd<32, 16>(a, stream);
+    return launch_sw_fwd<32, 32>(a, stream);
+  }
+  if (CK == 16 && NO == 16) return launch_sw_fwd_wide<16, 16>(a, stream);
+  if (CK == 16 && NO == 32) return launch_sw_fwd_wide<16, 32>(a, stream);
+  if (CK == 32 && NO == 16) return launch_sw_fwd_wide<32, 16>(a, stream);
+  if (CK == 32 && NO == 32) return launch_sw_fwd_wide<32, 32>(a, stream);
+  if (CK == 16) return launch_sw_fwd_wide<16, 64>(a, stream);
+  if (CK == 32) return launch_sw_fwd_wide<32, 64>(a, stream);
+  if (NO == 16) return launch_sw_fwd_wide<64, 16>(a, stream);
+  if (NO == 32) return launch_sw_fwd_wide<64, 32>(a, stream);
+  return launch_sw_fwd_wide<64, 64>(a, stream);
 }
 
 int sw_conv_wgrad(const __nv_bfloat16* dyimg, int64_t dy_lo, const __nv_bfloat16* ximg, int64_t x_lo, float* dW, int64_t Nf, int H,
@@ -926,7 +1220,9 @@ int sw_conv_wgrad(const __nv_bfloat16* dyimg, int64_t dy_lo, const __nv_bfloat16
   ProfScope prof(tag, stream);
   SwWgradArgs a;
   a.dy = dyimg; a.dy_lo = dy_lo; a.x = ximg; a.x_lo = x_lo; a.partial = partial; a.Nf = int(Nf); a.g = sw_geom(H, W);
-  int64_t grid = kNumSMs;
+  // 64-channel sides run as NB blocks of CT x OT channels, kNumSMs / NB CTAs each (sw_conv_wgrad_kernel)
+  const int CT = sw_wgrad_block(C), OT = sw_wgrad_block(O), NBC = C / CT, NB = NBC * (O / OT);
+  int64_t grid = kNumSMs / NB;
   const int64_t total = Nf * a.g.tpf;
   if (grid > total) grid = total;
   TB_REQUIRE(grid * O * 9 * C <= partial_floats, "sw_conv_wgrad: partial buffer too small");
@@ -934,11 +1230,25 @@ int sw_conv_wgrad(const __nv_bfloat16* dyimg, int64_t dy_lo, const __nv_bfloat16
   if (C == 16 && O == 16) rc = launch_sw_wgrad<16, 16>(a, int(grid), stream);
   else if (C == 16 && O == 32) rc = launch_sw_wgrad<16, 32>(a, int(grid), stream);
   else if (C == 32 && O == 16) rc = launch_sw_wgrad<32, 16>(a, int(grid), stream);
-  else rc = launch_sw_wgrad<32, 32>(a, int(grid), stream);
+  else if (C == 32 && O == 32) rc = launch_sw_wgrad<32, 32>(a, int(grid), stream);
+  else if (C == 16) rc = launch_sw_wgrad<16, 64, 16, 32>(a, int(grid), stream);
+  else if (C == 32) rc = launch_sw_wgrad<32, 64, 32, 32>(a, int(grid), stream);
+  else if (O == 16) rc = launch_sw_wgrad<64, 16, 32, 16>(a, int(grid), stream);
+  else if (O == 32) rc = launch_sw_wgrad<64, 32, 32, 32>(a, int(grid), stream);
+  else rc = launch_sw_wgrad<64, 64, 32, 32>(a, int(grid), stream);
   if (rc) return rc;
   if (c_real <= 0 || c_real > C) c_real = C;
-  sw_wgrad_reduce_kernel<<<(O * 9 * C + 31) / 32, 256, 0, stream>>>(partial, dW, int(grid), O, C, c_real, scale);
-  return check_launch("sw_wgrad_reduce_kernel");
+  // one fixed-order reduce per block: block (ob, cb) holds rows ob*OT.. of dW and its columns cb*CT.. (c_real == C
+  // whenever C is split, so the row pitch c_real and the column bound hold for every block)
+  for (int b = 0; b < NB; ++b) {
+    const int ob = b / NBC, cb = b % NBC;
+    sw_wgrad_reduce_kernel<<<(OT * 9 * CT + 31) / 32, 256, 0, stream>>>(partial + int64_t(b) * grid * OT * 9 * CT,
+                                                                       dW + (int64_t(ob) * OT * c_real + cb * CT) * 9, int(grid),
+                                                                       OT, CT, c_real, scale);
+    rc = check_launch("sw_wgrad_reduce_kernel");
+    if (rc) return rc;
+  }
+  return 0;
 }
 
 }  // namespace tb

@@ -38,6 +38,8 @@ int sw_frames_u8_unstacked(const uint8_t* frames, const uint8_t* done, __nv_bflo
 // the hi rows of a block followed by its lo rows so that [w_hi | w_lo] is one 2R-row operand):
 //   transpose == 0 (forward):        R = O, K = C:  [tap][C/16][2][hi R rows | lo R rows][8]
 //   transpose == 1 (input gradient): R = C, K = O:  [tap][O/16][2][hi R rows | lo R rows][8] with flipped taps (W[o, c, 2-a, 2-b])
+// in blocks of RB = min(R, 32) rows, each block a complete operand of that layout with R = RB (one block when R <= 32;
+// R = 64: two, one per column block of the wide forward kernel)
 int64_t sw_weight_elems(int O, int C);
 // c_real > 0 (forward only): the weight tensor has c_real < C input channels, the rest of the operand is zero
 int sw_pack_weights(const float* w, __nv_bfloat16* out, int O, int C, int transpose, cudaStream_t stream, int c_real = 0);
@@ -63,10 +65,11 @@ int sw_csum_reduce(float* csum, int64_t rows, int C, float* db, cudaStream_t str
 bool sw_conv_applicable(int H, int W, int CK, int NO);
 // a CK -> NO conv at H x W can be trained on these kernels: it is applicable, W >= 5 (the weight gradient's last pixel step
 // of a frame must end in the zero run behind it), and its forward, its input-gradient convolution (NO -> CK) and its weight
-// gradient fit the shared memory (the input window grows with W + 2)
-bool sw_conv_trainable(int H, int W, int CK, int NO);
-// out fp32 [Nf*H*W, NO] = epilogue(conv3x3(image) with the packed weights); CK = channels of the image (16 / 32),
-// NO = output channels (16 / 32)
+// gradient fit the shared memory (the input window grows with W + 2); input_grad = false: a first conv, whose input
+// gradient is never formed
+bool sw_conv_trainable(int H, int W, int CK, int NO, bool input_grad = true);
+// out fp32 [Nf*H*W, NO] = epilogue(conv3x3(image) with the packed weights); CK = channels of the image (16 / 32 / 64),
+// NO = output channels (16 / 32 / 64; a pair with a 64-channel side runs on sw_conv_fwd_wide_kernel)
 int sw_conv_fwd(const __nv_bfloat16* img, int64_t img_lo, const __nv_bfloat16* wk, float* out, int64_t Nf, int H, int W, int CK, int NO,
                 const SwEpilogue& ep, cudaStream_t stream);
 

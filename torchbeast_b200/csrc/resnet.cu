@@ -26,7 +26,7 @@ namespace tb {
 namespace {
 
 constexpr int kSections = 3;
-constexpr int kSecCh[kSections] = {16, 32, 32};
+constexpr int kDefaultCh[kSections] = {16, 32, 32};   // the IMPALA paper's widths
 constexpr int kFcOut = 256;
 constexpr int kLstmH = 256;
 constexpr int64_t kScratchFloats = int64_t(8) << 20;
@@ -41,37 +41,47 @@ constexpr int kObsMinH = 17;
 constexpr int kObsMinW = 33;
 constexpr int kObsMaxHW = 126;
 
-// Observation geometry: section i's feat conv runs at H[i] x W[i] (H[0] x W[0] = the frame), its max-pool (3, 2, 1) leaves
-// ceil(H[i] / 2) x ceil(W[i] / 2) = H[i+1] x W[i+1]; the fc reads the last section's 32 x H[3] x W[3] output
+// Section widths (tb_resnet_arch_supported): each of 16, 32 or 64 channels, in any combination.  The shifted-window
+// kernels take 16 / 32 / 64 channels on either side of a conv; 64-channel convs run at W <= 63 (any 64-wide section after
+// the first, or the residual blocks of a 64-wide first section) or 16 -> 64 at W <= 126 (the first conv), which all fit.
+constexpr int kWidths[3] = {16, 32, 64};
+
+// Net geometry: section i has ch[i] channels; its feat conv runs at H[i] x W[i] (H[0] x W[0] = the frame), its max-pool
+// (3, 2, 1) leaves ceil(H[i] / 2) x ceil(W[i] / 2) = H[i+1] x W[i+1]; the fc reads the last section's ch[2] x H[3] x W[3]
+// output
 struct ResGeom {
-  int C, H[kSections + 1], W[kSections + 1];
-  int cin(int i) const { return i == 0 ? C : kSecCh[i - 1]; }
+  int C, H[kSections + 1], W[kSections + 1], ch[kSections];
+  int cin(int i) const { return i == 0 ? C : ch[i - 1]; }
   int fc_hw() const { return H[kSections] * W[kSections]; }
-  int fc_in() const { return kSecCh[kSections - 1] * fc_hw(); }
+  int fc_in() const { return ch[kSections - 1] * fc_hw(); }
 };
 
-ResGeom res_geom(int C, int H, int W) {
+ResGeom res_geom(int C, int H, int W, const int* ch = kDefaultCh) {
   ResGeom g;
   g.C = C; g.H[0] = H; g.W[0] = W;
-  for (int i = 0; i < kSections; ++i) { g.H[i + 1] = (g.H[i] + 1) / 2; g.W[i + 1] = (g.W[i] + 1) / 2; }
+  for (int i = 0; i < kSections; ++i) { g.H[i + 1] = (g.H[i] + 1) / 2; g.W[i + 1] = (g.W[i] + 1) / 2; g.ch[i] = ch[i]; }
   return g;
 }
 
 // the Atari stack u8 [4, 84, 84]: 84 -> 42 -> 21 -> 11, fc 3872 -> 256
 const ResGeom kAtariGeom = res_geom(4, 84, 84);
 
-// 0, or 1 with tb_last_error set: the range above, and on the split-bf16 backend every conv of the geometry on the
-// shifted-window kernels (the other backends' im2col / GEMM kernels take any size)
-int res_geom_check(int C, int H, int W, int precision, const char* who) {
+// 0, or 1 with tb_last_error set: the range above, the widths, and on the split-bf16 backend every conv of the geometry
+// on the shifted-window kernels (the other backends' im2col / GEMM kernels take any size)
+int res_geom_check(int C, int H, int W, const int* ch, int precision, const char* who) {
   TB_REQUIRE(C >= 1 && C <= kObsMaxC, "%s: observation channels %d outside [1, %d]", who, C, kObsMaxC);
   TB_REQUIRE(H >= kObsMinH && H <= kObsMaxHW && W >= kObsMinW && W <= kObsMaxHW,
              "%s: observation %d x %d outside [%d, %d] x [%d, %d]", who, H, W, kObsMinH, kObsMaxHW, kObsMinW, kObsMaxHW);
+  for (int i = 0; i < kSections; ++i)
+    TB_REQUIRE(ch[i] == kWidths[0] || ch[i] == kWidths[1] || ch[i] == kWidths[2],
+               "%s: section %d has %d channels; each section takes 16, 32 or 64", who, i, ch[i]);
   TB_REQUIRE(precision >= 0 && precision <= 2, "%s: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)", who);
   if (precision == 2) {
-    const ResGeom g = res_geom(C, H, W);
+    const ResGeom g = res_geom(C, H, W, ch);
     for (int i = 0; i < kSections; ++i) {
-      const int ch = kSecCh[i], cin = i == 0 ? 16 : g.cin(i);
-      TB_REQUIRE(sw_conv_trainable(g.H[i], g.W[i], cin, ch) && sw_conv_trainable(g.H[i + 1], g.W[i + 1], ch, ch),
+      const int c = g.ch[i], cin = i == 0 ? 16 : g.cin(i);
+      // (the first conv's input gradient is never formed)
+      TB_REQUIRE(sw_conv_trainable(g.H[i], g.W[i], cin, c, i > 0) && sw_conv_trainable(g.H[i + 1], g.W[i + 1], c, c),
                  "%s: section %d (%d x %d) does not fit the shifted-window conv kernels", who, i, g.H[i], g.W[i]);
     }
   }
@@ -89,12 +99,12 @@ ResParams res_params(const ResGeom& g, int A, int use_lstm, int V = 1) {  // V: 
   ResParams p;
   int64_t o = 0;
   auto take = [&](int64_t n) { int64_t r = o; o += n; return r; };
-  for (int i = 0; i < kSections; ++i) { p.feat[i].w = take(int64_t(kSecCh[i]) * g.cin(i) * 9); p.feat[i].b = take(kSecCh[i]); }
+  for (int i = 0; i < kSections; ++i) { p.feat[i].w = take(int64_t(g.ch[i]) * g.cin(i) * 9); p.feat[i].b = take(g.ch[i]); }
   for (int blk = 0; blk < 2; ++blk)     // resnet1.{0,1,2}.{1,3} then resnet2.{0,1,2}.{1,3}
     for (int i = 0; i < kSections; ++i)
       for (int j = 0; j < 2; ++j) {
-        p.blk[i][blk * 2 + j].w = take(int64_t(kSecCh[i]) * kSecCh[i] * 9);
-        p.blk[i][blk * 2 + j].b = take(kSecCh[i]);
+        p.blk[i][blk * 2 + j].w = take(int64_t(g.ch[i]) * g.ch[i] * 9);
+        p.blk[i][blk * 2 + j].b = take(g.ch[i]);
       }
   p.fc_w = take(int64_t(kFcOut) * g.fc_in()); p.fc_b = take(kFcOut);
   p.core_in = kFcOut + 1;
@@ -150,7 +160,7 @@ ResWs<T> res_ws(const ResGeom& g, void* base, int64_t N, int64_t T1, int64_t B, 
   const int64_t fc_in = g.fc_in();
   int64_t maxact = 0;
   for (int i = 0; i < kSections; ++i) {
-    const int64_t big = N * g.H[i] * g.W[i] * kSecCh[i], small = N * g.H[i + 1] * g.W[i + 1] * kSecCh[i];
+    const int64_t big = N * g.H[i] * g.W[i] * g.ch[i], small = N * g.H[i + 1] * g.W[i + 1] * g.ch[i];
     w.s[i].P = takeT(big); w.s[i].X0 = takeT(small); w.s[i].Y1 = takeT(small); w.s[i].X1 = takeT(small);
     w.s[i].Y2 = takeT(small); w.s[i].X2 = takeT(small);
     w.s[i].arg = static_cast<uint8_t*>(take(size_t(small)));
@@ -160,7 +170,7 @@ ResWs<T> res_ws(const ResGeom& g, void* base, int64_t N, int64_t T1, int64_t B, 
   for (int k = 0; k < 3; ++k) w.g[k] = takeT(maxact);
   int64_t maxcol = 0;
   for (int i = 0; i < kSections; ++i) {
-    const int64_t a = N * g.H[i] * g.W[i] * ldk_of(g.cin(i), kBf16), b = N * g.H[i + 1] * g.W[i + 1] * ldk_of(kSecCh[i], kBf16);
+    const int64_t a = N * g.H[i] * g.W[i] * ldk_of(g.cin(i), kBf16), b = N * g.H[i + 1] * g.W[i + 1] * ldk_of(g.ch[i], kBf16);
     if (a > maxcol) maxcol = a;
     if (b > maxcol) maxcol = b;
   }
@@ -175,31 +185,31 @@ ResWs<T> res_ws(const ResGeom& g, void* base, int64_t N, int64_t T1, int64_t B, 
     w.dfcb = takeh(N * kFcOut, w.dfcb_lo);
     w.wb_fc = takeh(int64_t(kFcOut) * fc_in, w.wb_fc_lo);
     for (int i = 0; i < kSections; ++i) {
-      if (i > 0) w.wd_feat[i] = takeh(int64_t(g.cin(i)) * 9 * kSecCh[i], w.wd_feat_lo[i]);
-      for (int j = 0; j < 4; ++j) w.wd_blk[i][j] = takeh(int64_t(kSecCh[i]) * 9 * kSecCh[i], w.wd_blk_lo[i][j]);
+      if (i > 0) w.wd_feat[i] = takeh(int64_t(g.cin(i)) * 9 * g.ch[i], w.wd_feat_lo[i]);
+      for (int j = 0; j < 4; ++j) w.wd_blk[i][j] = takeh(int64_t(g.ch[i]) * 9 * g.ch[i], w.wd_blk_lo[i][j]);
     }
     int64_t maxp = 0;
     for (int i = 0; i < kSections; ++i) {
       {   // (the frame channels of the first conv are padded to 16)
         const int cin16 = i == 0 ? 16 : g.cin(i);
         w.xp_feat[i] = takeh(sw_image_elems(N, g.H[i], g.W[i], cin16), w.xp_feat_lo[i]);
-        w.wi_feat[i] = takeh(sw_weight_elems(kSecCh[i], cin16) / 2, w.wi_feat_lo[i]);
-        const int64_t e = sw_image_elems(N, g.H[i], g.W[i], kSecCh[i]);
+        w.wi_feat[i] = takeh(sw_weight_elems(g.ch[i], cin16) / 2, w.wi_feat_lo[i]);
+        const int64_t e = sw_image_elems(N, g.H[i], g.W[i], g.ch[i]);
         if (e > maxp) maxp = e;
       }
       for (int j = 0; j < 4; ++j) {
-        w.xp_blk[i][j] = takeh(sw_image_elems(N, g.H[i + 1], g.W[i + 1], kSecCh[i]), w.xp_blk_lo[i][j]);
-        w.wi_blk[i][j] = takeh(sw_weight_elems(kSecCh[i], kSecCh[i]) / 2, w.wi_blk_lo[i][j]);
+        w.xp_blk[i][j] = takeh(sw_image_elems(N, g.H[i + 1], g.W[i + 1], g.ch[i]), w.xp_blk_lo[i][j]);
+        w.wi_blk[i][j] = takeh(sw_weight_elems(g.ch[i], g.ch[i]) / 2, w.wi_blk_lo[i][j]);
       }
-      const int64_t e = sw_image_elems(N, g.H[i + 1], g.W[i + 1], kSecCh[i]);
+      const int64_t e = sw_image_elems(N, g.H[i + 1], g.W[i + 1], g.ch[i]);
       if (e > maxp) maxp = e;
     }
     w.dyp = takeh(maxp, w.dyp_lo);     // dY images ping-pong: a conv's input-gradient epilogue writes the next conv's dY image
     w.dyp2 = takeh(maxp, w.dyp2_lo);
   }
   for (int i = 0; i < kSections; ++i) {
-    w.wfeat[i] = takeT(int64_t(kSecCh[i]) * ldk_of(g.cin(i), kBf16));
-    for (int j = 0; j < 4; ++j) w.wblk[i][j] = takeT(int64_t(kSecCh[i]) * ldk_of(kSecCh[i], kBf16));
+    w.wfeat[i] = takeT(int64_t(g.ch[i]) * ldk_of(g.cin(i), kBf16));
+    for (int j = 0; j < 4; ++j) w.wblk[i][j] = takeT(int64_t(g.ch[i]) * ldk_of(g.ch[i], kBf16));
   }
   w.wfc = takeT(int64_t(kFcOut) * fc_in);
   w.core_in = takef(N * pp.core_in);
@@ -215,11 +225,14 @@ ResWs<T> res_ws(const ResGeom& g, void* base, int64_t N, int64_t T1, int64_t B, 
   need(heads_scratch_floats(N, pp.core_out, A, kHeadsMaxValues));
   if (split) {
     for (int i = 0; i < kSections; ++i) {
-      const int ch = kSecCh[i];
+      const int ch = g.ch[i];
       need(sw_colsum_scratch_floats(N, g.H[i], g.W[i], ch));           // max-pool backward -> the feat conv's dY image
       need(sw_colsum_scratch_floats(N, g.H[i + 1], g.W[i + 1], ch));   // pad-split of a residual conv's dY
       need((sw_csum_rows(N, g.H[i + 1], g.W[i + 1]) + 128) * ch);      // residual dgrad emits the previous conv's dY
       if (i > 0) need((sw_csum_rows(N, g.H[i], g.W[i]) + 128) * g.cin(i));   // feat dgrad emits section i-1's last dY
+      // the weight gradients' per-CTA partials (at most kNumSMs CTAs, sw_conv_wgrad)
+      need(int64_t(kNumSMs) * ch * 9 * (i == 0 ? 16 : g.cin(i)));
+      need(int64_t(kNumSMs) * ch * 9 * ch);
     }
   }
   w.splitk = takef(w.splitk_floats);
@@ -318,15 +331,15 @@ struct Impl {
     ResWs<T> w = res_ws<T>(g, workspace, N, T1, B, A, use_lstm);
     const int64_t fc_in = g.fc_in(), k_first = int64_t(g.C) * 9;
     // weight pack: [o, c, kh, kw] -> [o, (kh,kw), c]; first conv keeps (c,kh,kw); fc: [o, c, (h,w)] -> [o, (h,w), c]
-    TB_TRY(pack_w(P + pp.feat[0].w, w.wfeat[0], kSecCh[0], 1, int(k_first), ldk_of(g.C, kBf16), st));
+    TB_TRY(pack_w(P + pp.feat[0].w, w.wfeat[0], g.ch[0], 1, int(k_first), ldk_of(g.C, kBf16), st));
     for (int i = 0; i < kSections; ++i) {
-      if (i > 0) TB_TRY(pack_w(P + pp.feat[i].w, w.wfeat[i], kSecCh[i], 9, g.cin(i), ldk_of(g.cin(i), kBf16), st));
-      for (int j = 0; j < 4; ++j) TB_TRY(pack_w(P + pp.blk[i][j].w, w.wblk[i][j], kSecCh[i], 9, kSecCh[i], ldk_of(kSecCh[i], kBf16), st));
+      if (i > 0) TB_TRY(pack_w(P + pp.feat[i].w, w.wfeat[i], g.ch[i], 9, g.cin(i), ldk_of(g.cin(i), kBf16), st));
+      for (int j = 0; j < 4; ++j) TB_TRY(pack_w(P + pp.blk[i][j].w, w.wblk[i][j], g.ch[i], 9, g.ch[i], ldk_of(g.ch[i], kBf16), st));
     }
-    TB_TRY(pack_w(P + pp.fc_w, w.wfc, kFcOut, g.fc_hw(), 32, fc_in, st));
+    TB_TRY(pack_w(P + pp.fc_w, w.wfc, kFcOut, g.fc_hw(), g.ch[kSections - 1], fc_in, st));
     const T* xin = nullptr;
     for (int i = 0; i < kSections; ++i) {
-      const int H = g.H[i], W = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = kSecCh[i], cin = g.cin(i);
+      const int H = g.H[i], W = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = g.ch[i], cin = g.cin(i);
       const int64_t M = N * H * W, Mo = N * Ho * Wo;
       const int64_t ldk_in = ldk_of(cin, kBf16), ldk = ldk_of(ch, kBf16);
       if (i == 0) {
@@ -409,12 +422,12 @@ struct Impl {
     TB_TRY(relu_mask_inplace(w.dcore_in, w.core_in, N, kFcOut, pp.core_in, pp.core_in, st));
     TB_TRY(colsum(w.dcore_in, G + pp.fc_b, N, kFcOut, pp.core_in, w.colsum_scratch, st));
     TB_TRY(convert_from_f32<T>(w.dcore_in, w.dfc, N, kFcOut, pp.core_in, kFcOut, st));
-    TB_TRY(conv_wgrad(w.dfc, w.fcin, false, G + pp.fc_w, N, kFcOut, fc_in, fc_in, g.fc_hw(), 32, 1.0f, w.splitk, "fc_wgrad", st));
+    TB_TRY(conv_wgrad(w.dfc, w.fcin, false, G + pp.fc_w, N, kFcOut, fc_in, fc_in, g.fc_hw(), g.ch[kSections - 1], 1.0f, w.splitk, "fc_wgrad", st));
     TB_TRY(conv_dgrad(w.dfc, w.wfc, w.dfcin, N, kFcOut, fc_in, fc_in, "fc_dgrad", st));
     T* g0 = w.g[0]; T* g1 = w.g[1]; T* g2 = w.g[2];
     TB_TRY(relu_bwd<T>(w.s[2].X2, w.dfcin, g0, N * fc_in, st));  // dL/dX2 of the last section
     for (int i = kSections - 1; i >= 0; --i) {
-      const int H = g.H[i], W = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = kSecCh[i], cin = g.cin(i);
+      const int H = g.H[i], W = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = g.ch[i], cin = g.cin(i);
       Sec<T>& s = w.s[i];
       // block 2: X2 = X1 + conv_b(relu(Y2)), Y2 = conv_a(relu(X1))
       TB_TRY(conv_bwd(s.Y2, true, g0, w.wblk[i][3], G + pp.blk[i][3].w, G + pp.blk[i][3].b, g1, nullptr, N, Ho, Wo, ch, ch, w, st));
@@ -482,9 +495,9 @@ struct SplitImpl {
     const ResParams pp = res_params(g, A, use_lstm, V);
     W w = res_ws<float>(g, workspace, N, T1, B, A, use_lstm, true);
     const int64_t fc_in = g.fc_in();
-    TB_TRY(pack_weights_bf16(P + pp.fc_w, w.wb_fc, kFcOut, g.fc_hw(), 32, fc_in, st, w.wb_fc_lo));
+    TB_TRY(pack_weights_bf16(P + pp.fc_w, w.wb_fc, kFcOut, g.fc_hw(), g.ch[kSections - 1], fc_in, st, w.wb_fc_lo));
     for (int i = 0; i < kSections; ++i) {
-      const int H = g.H[i], Wd = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = kSecCh[i], cin = g.cin(i);
+      const int H = g.H[i], Wd = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = g.ch[i], cin = g.cin(i);
       if (i == 0) {
         // the first conv through the same kernels: frame pixels (exact in bf16) as a 16-channel image, 1/255 in the epilogue
         TB_TRY(sw_pack_weights(P + pp.feat[0].w, w.wi_feat[0], ch, 16, 0, st, g.C));
@@ -578,7 +591,7 @@ struct SplitImpl {
     TB_TRY(colsum(w.dcore_in, G + pp.fc_b, N, kFcOut, pp.core_in, w.colsum_scratch, st));
     TB_TRY(f32_to_bf16(w.dcore_in, w.dfcb, N, kFcOut, pp.core_in, kFcOut, st, w.dfcb_lo));
     // (fcb still holds relu(X2) as hi / lo planes from the forward pass)
-    TB_TRY(gemm_wgrad(w.dfcb, w.dfcb_lo, w.fcb, w.fcb_lo, G + pp.fc_w, N, kFcOut, fc_in, fc_in, g.fc_hw(), 32, 1.0f, w.splitk,
+    TB_TRY(gemm_wgrad(w.dfcb, w.dfcb_lo, w.fcb, w.fcb_lo, G + pp.fc_w, N, kFcOut, fc_in, fc_in, g.fc_hw(), g.ch[kSections - 1], 1.0f, w.splitk,
                       "fc_wgrad", st));
     {
       TcEpilogue te; te.C = w.dfcin; te.ldc = fc_in; te.a_lo = w.dfcb_lo; te.b_lo = w.wb_fc_lo; te.tag = "fc_dgrad";
@@ -590,7 +603,7 @@ struct SplitImpl {
     const int64_t dyi_lo[2] = {w.dyp_lo, w.dyp2_lo};
     int dsel = 0;
     for (int i = kSections - 1; i >= 0; --i) {
-      const int H = g.H[i], Wd = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = kSecCh[i], cin = g.cin(i);
+      const int H = g.H[i], Wd = g.W[i], Ho = g.H[i + 1], Wo = g.W[i + 1], ch = g.ch[i], cin = g.cin(i);
       Sec<float>& s = w.s[i];
       const float* xs[4] = {s.X0, s.Y1, s.X1, s.Y2};
       const float* dys[4] = {g0, g2, g1, g0};       // dL/d(conv output) of r1a, r1b, r2a, r2b
@@ -685,32 +698,64 @@ int tb_resnet_obs_range(int* range) {
   return 0;
 }
 
+int tb_resnet_widths(int* widths) {
+  TB_REQUIRE(widths, "resnet_widths: null pointer");
+  for (int i = 0; i < 3; ++i) widths[i] = kWidths[i];
+  return 0;
+}
+
 int tb_resnet_obs_supported(int C, int H, int W, int precision) {
-  return res_geom_check(C, H, W, precision, "resnet_obs_supported") == 0 ? 1 : 0;
+  return res_geom_check(C, H, W, kDefaultCh, precision, "resnet_obs_supported") == 0 ? 1 : 0;
+}
+
+int tb_resnet_arch_supported(int C, int H, int W, int c0, int c1, int c2, int precision) {
+  const int ch[kSections] = {c0, c1, c2};
+  return res_geom_check(C, H, W, ch, precision, "resnet_arch_supported") == 0 ? 1 : 0;
 }
 
 int64_t tb_resnet_param_count_obs(int C, int H, int W, int num_actions, int num_values, int use_lstm) {
-  if (res_geom_check(C, H, W, 0, "resnet_param_count_obs")) return -1;
-  return res_params(res_geom(C, H, W), num_actions, use_lstm, num_values).total;
+  return tb_resnet_param_count_arch(C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], num_actions, num_values, use_lstm);
+}
+
+int64_t tb_resnet_param_count_arch(int C, int H, int W, int c0, int c1, int c2, int num_actions, int num_values, int use_lstm) {
+  const int ch[kSections] = {c0, c1, c2};
+  if (res_geom_check(C, H, W, ch, 0, "resnet_param_count")) return -1;
+  return res_params(res_geom(C, H, W, ch), num_actions, use_lstm, num_values).total;
 }
 
 size_t tb_resnet_workspace_bytes_obs(int C, int H, int W, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
-  if (res_geom_check(C, H, W, precision, "resnet_workspace_bytes_obs")) return 0;
-  return res_ws_bytes(res_geom(C, H, W), T1, B, num_actions, use_lstm, precision);
+  return tb_resnet_workspace_bytes_arch(C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], T1, B, num_actions, use_lstm,
+                                        precision);
+}
+
+size_t tb_resnet_workspace_bytes_arch(int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B, int num_actions,
+                                      int use_lstm, int precision) {
+  const int ch[kSections] = {c0, c1, c2};
+  if (res_geom_check(C, H, W, ch, precision, "resnet_workspace_bytes")) return 0;
+  return res_ws_bytes(res_geom(C, H, W, ch), T1, B, num_actions, use_lstm, precision);
 }
 
 int tb_resnet_forward_obs(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
                           const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions, int num_values,
                           int use_lstm, int precision, void* workspace, float* policy_logits, float* baseline, float* hN, float* cN,
                           void* stream) {
+  return tb_resnet_forward_arch(frame, reward, notdone, h0, c0, params, C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], T1,
+                                B, num_actions, num_values, use_lstm, precision, workspace, policy_logits, baseline, hN, cN, stream);
+}
+
+int tb_resnet_forward_arch(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
+                           const float* params, int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1, int64_t B,
+                           int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* policy_logits,
+                           float* baseline, float* hN, float* cN, void* stream) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_forward: num_values %d outside [1, %d]", num_values,
              kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward: bad sizes");
   TB_REQUIRE(frame && reward && params && workspace && policy_logits && baseline, "resnet_forward: null pointer");
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
-  TB_TRY(res_geom_check(C, H, W, precision, "resnet_forward"));
-  const ResGeom g = res_geom(C, H, W);
+  const int ch[kSections] = {ch0, ch1, ch2};
+  TB_TRY(res_geom_check(C, H, W, ch, precision, "resnet_forward"));
+  const ResGeom g = res_geom(C, H, W, ch);
   if (precision == 2)
     return SplitImpl::forward(g, frame, nullptr, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
                               policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
@@ -724,14 +769,22 @@ int tb_resnet_forward_obs(const uint8_t* frame, const float* reward, const float
 int tb_resnet_backward_obs(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
                            const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions, int num_values,
                            int use_lstm, int precision, void* workspace, float* grads, void* stream) {
+  return tb_resnet_backward_arch(frame, grad_logits, grad_baseline, notdone, params, C, H, W, kDefaultCh[0], kDefaultCh[1],
+                                 kDefaultCh[2], T1, B, num_actions, num_values, use_lstm, precision, workspace, grads, stream);
+}
+
+int tb_resnet_backward_arch(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
+                            const float* params, int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B, int num_actions,
+                            int num_values, int use_lstm, int precision, void* workspace, float* grads, void* stream) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_backward: num_values %d outside [1, %d]", num_values,
              kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward: bad sizes");
   TB_REQUIRE(frame && grad_logits && grad_baseline && params && workspace && grads, "resnet_backward: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "resnet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward: precision must be 0, 1 or 2");
-  TB_TRY(res_geom_check(C, H, W, precision, "resnet_backward"));
-  const ResGeom g = res_geom(C, H, W);
+  const int ch[kSections] = {c0, c1, c2};
+  TB_TRY(res_geom_check(C, H, W, ch, precision, "resnet_backward"));
+  const ResGeom g = res_geom(C, H, W, ch);
   if (precision == 2)
     return SplitImpl::backward(g, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads,
                                (cudaStream_t)stream, num_values);

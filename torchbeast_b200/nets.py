@@ -82,6 +82,7 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
 
 
 ATARI_SHAPE = (4, 84, 84)
+RESNET_CHANNELS = (16, 32, 32)   # the IMPALA paper's section widths
 
 
 def resnet_obs_range():
@@ -92,10 +93,17 @@ def resnet_obs_range():
     return {"C": (r[0], r[1]), "H": (r[2], r[3]), "W": (r[4], r[5])}
 
 
-def frame_is_unstacked(frame, reward, observation_shape=ATARI_SHAPE):
+def resnet_widths():
+    """The channel counts each ResNet section takes (16, 32, 64), as the C library states them (tb_resnet_widths)."""
+    r = (ctypes.c_int * 3)()
+    _lib.check(_lib.lib().tb_resnet_widths(ctypes.cast(r, ctypes.c_void_p)), "tb_resnet_widths")
+    return tuple(r)
+
+
+def frame_is_unstacked(frame, reward, observation_shape=ATARI_SHAPE, channels=RESNET_CHANNELS):
     """False for a stacked frame u8 [T1, B, C, H, W] with [C, H, W] = observation_shape; True for an unstacked rollout
     u8 [T1+3, B, 84, 84] with T1 = reward.shape[0] (include/torchbeast_b200.h, "unstacked rollouts"), which only a
-    (4, 84, 84) net takes.  Anything else raises."""
+    (4, 84, 84) net with the default section widths takes.  Anything else raises."""
     obs = tuple(observation_shape)
     stacked = "[T,B,%d,%d,%d]" % obs
     if frame.dtype != torch.uint8 or frame.dim() not in (4, 5):
@@ -110,6 +118,10 @@ def frame_is_unstacked(frame, reward, observation_shape=ATARI_SHAPE):
         raise _lib.TorchBeastB200Error(
             "unstacked rollouts and newest frames rebuild (4, 84, 84) stacks; this net takes stacked frames uint8 %s, "
             "got %r" % (stacked, tuple(frame.shape)))
+    if tuple(channels) != RESNET_CHANNELS:
+        raise _lib.TorchBeastB200Error(
+            "unstacked rollouts and newest frames run on the default widths %r; this net has channels=%r and takes "
+            "stacked frames uint8 %s, got %r" % (RESNET_CHANNELS, tuple(channels), stacked, tuple(frame.shape)))
     T1, B = reward.shape[:2]
     if tuple(frame.shape) != (T1 + 3, B, 84, 84):
         raise _lib.TorchBeastB200Error(
@@ -176,6 +188,11 @@ class FlatParamModule(nn.Module):
         if self.frame_history is not None and obs != ATARI_SHAPE:
             raise _lib.TorchBeastB200Error("a frame_history rebuilds (4, 84, 84) stacks; this net takes stacked frames "
                                            "uint8 [T,B,%d,%d,%d]: detach the history (model.frame_history = None)" % obs)
+        channels = tuple(getattr(self, "channels", RESNET_CHANNELS))
+        if self.frame_history is not None and channels != RESNET_CHANNELS:
+            raise _lib.TorchBeastB200Error("a frame_history feeds the default widths %r; this net has channels=%r and "
+                                           "takes stacked frames: detach the history (model.frame_history = None)"
+                                           % (RESNET_CHANNELS, channels))
         if self.frame_history is None or frame.dim() != 4 or frame.shape[0] != reward.shape[0]:
             return frame
         if frame.shape[1] != reward.shape[1]:
@@ -535,28 +552,29 @@ class AtariNet(FlatParamModule):
 
 
 
-def resnet_fc_in(observation_shape=ATARI_SHAPE):
-    """Input features of the ResNet's fc layer: 32 x H_3 x W_3, each of the three max-pools (3, 2, 1) taking a side
-    s to ceil(s / 2) (84 -> 42 -> 21 -> 11: 3872)."""
+def resnet_fc_in(observation_shape=ATARI_SHAPE, channels=RESNET_CHANNELS):
+    """Input features of the ResNet's fc layer: channels[2] x H_3 x W_3, each of the three max-pools (3, 2, 1) taking a
+    side s to ceil(s / 2) (84 -> 42 -> 21 -> 11: 32 x 121 = 3872)."""
     _, h, w = observation_shape
     for _ in range(3):
         h, w = (h + 1) // 2, (w + 1) // 2
-    return 32 * h * w
+    return channels[2] * h * w
 
 
-def resnet_param_spec(num_actions, use_lstm, num_values=1, observation_shape=ATARI_SHAPE):
+def resnet_param_spec(num_actions, use_lstm, num_values=1, observation_shape=ATARI_SHAPE, channels=RESNET_CHANNELS):
     """State_dict order/shapes of the reference's polybeast_learner.Net (pl:134-204, BASELINE.md section 5) for
-    observations u8 [C, H, W]: feat_convs.0.0.weight (16, C, 3, 3) and fc.weight (256, resnet_fc_in(...))."""
+    observations u8 [C, H, W] and section widths `channels`: feat_convs.i.0.weight (channels[i], C or channels[i-1],
+    3, 3), the residual convs (channels[i], channels[i], 3, 3) and fc.weight (256, resnet_fc_in(...))."""
     spec = []
     cin = observation_shape[0]
-    for i, ch in enumerate([16, 32, 32]):
+    for i, ch in enumerate(channels):
         spec += [("feat_convs.%d.0.weight" % i, (ch, cin, 3, 3)), ("feat_convs.%d.0.bias" % i, (ch,))]
         cin = ch
     for blk in ("resnet1", "resnet2"):
-        for i, ch in enumerate([16, 32, 32]):
+        for i, ch in enumerate(channels):
             for j in (1, 3):
                 spec += [("%s.%d.%d.weight" % (blk, i, j), (ch, ch, 3, 3)), ("%s.%d.%d.bias" % (blk, i, j), (ch,))]
-    spec += [("fc.weight", (256, resnet_fc_in(observation_shape))), ("fc.bias", (256,))]
+    spec += [("fc.weight", (256, resnet_fc_in(observation_shape, channels))), ("fc.bias", (256,))]
     head_in = 257
     if use_lstm:
         spec += [("core.weight_ih_l0", (1024, 257)), ("core.weight_hh_l0", (1024, 256)),
@@ -597,12 +615,16 @@ class ResNet(FlatParamModule):
     observation_shape (keyword-only, default the Atari stack (4, 84, 84)): the u8 [C, H, W] of each frame, e.g.
     (3, 64, 64) for Procgen or (3, 72, 96) for DMLab; C from 1 to 16, H from 17 and W from 33 to 126
     (resnet_obs_range()), on every precision.  The fc then reads 32 x ceil(H/8) x ceil(W/8) features (resnet_fc_in).  Unstacked rollouts and a
-    frame_history are (4, 84, 84) only."""
+    frame_history are (4, 84, 84) only.
+
+    channels (keyword-only, default (16, 32, 32)): the widths of the three sections, each 16, 32 or 64
+    (resnet_widths()), in any combination and at every supported observation shape, e.g. (32, 64, 64) for "IMPALA x2"
+    (Cobbe et al., 2020).  Unstacked rollouts and a frame_history take the default widths only."""
 
     PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 
     def __init__(self, num_actions, use_lstm=False, device=None, precision=None, num_tasks=None, *,
-                 observation_shape=ATARI_SHAPE):
+                 observation_shape=ATARI_SHAPE, channels=RESNET_CHANNELS):
         super().__init__()
         import os
         self.num_actions = num_actions
@@ -614,11 +636,20 @@ class ResNet(FlatParamModule):
                 "ResNet observation_shape must be (C, H, W) with C in [%d, %d], H in [%d, %d] and W in [%d, %d], got %r"
                 % (sum((rng[k] for k in ("C", "H", "W")), ()) + (tuple(observation_shape),)))
         self.observation_shape = obs
+        try:
+            ch = tuple(int(c) for c in channels)
+        except (TypeError, ValueError):
+            ch = ()
+        if len(ch) != 3 or not _lib.lib().tb_resnet_arch_supported(*obs, *ch, self.PRECISIONS["bf16x3"]):
+            raise _lib.TorchBeastB200Error(
+                "ResNet channels must be three section widths, each one of %r, got %r" % (resnet_widths(), channels))
+        self.channels = ch
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
         popart = None if num_tasks is None else PopArt(num_tasks, device)
         self.num_values = 1 if popart is None else popart.num_tasks
-        self._build_flat(resnet_param_spec(num_actions, use_lstm, num_values=self.num_values, observation_shape=obs), device)
+        self._build_flat(resnet_param_spec(num_actions, use_lstm, num_values=self.num_values, observation_shape=obs,
+                                           channels=ch), device)
         self._fix_module_names()
         self.reset_parameters_like_torch()
         if popart is not None:
@@ -633,7 +664,7 @@ class ResNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_resnet_param_count_obs(*obs, num_actions, self.num_values, int(use_lstm))
+        count = _lib.lib().tb_resnet_param_count_arch(*obs, *ch, num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def _fix_module_names(self):
@@ -647,10 +678,11 @@ class ResNet(FlatParamModule):
     def _workspace(self, T1, B):
         key = (T1, B, self._flat.device, self.precision)
         if self._ws_key != key:
-            nbytes = _lib.lib().tb_resnet_workspace_bytes_obs(*self.observation_shape, T1, B, self.num_actions,
-                                                              int(self.use_lstm), self.PRECISIONS[self.precision])
+            nbytes = _lib.lib().tb_resnet_workspace_bytes_arch(*self.observation_shape, *self.channels, T1, B,
+                                                               self.num_actions, int(self.use_lstm),
+                                                               self.PRECISIONS[self.precision])
             if nbytes == 0:
-                raise _lib.TorchBeastB200Error("tb_resnet_workspace_bytes_obs: %s" % _lib.lib().tb_last_error().decode())
+                raise _lib.TorchBeastB200Error("tb_resnet_workspace_bytes_arch: %s" % _lib.lib().tb_last_error().decode())
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
             self._ws_key = key
         return self._ws
@@ -659,7 +691,7 @@ class ResNet(FlatParamModule):
         """Returns (logits, baseline, hN, cN, saved): `saved` is what _launch_backward re-reads - the stacked frame, or
         ("unstacked", stacked scratch or None).  `done` is read only with an unstacked frame, to rebuild the stacks."""
         _lib.require_cuda(frame, reward, self._flat)
-        unstacked = frame_is_unstacked(frame, reward, self.observation_shape)
+        unstacked = frame_is_unstacked(frame, reward, self.observation_shape, self.channels)
         T1, B = reward.shape[:2] if unstacked else frame.shape[:2]
         if unstacked:
             _lib.require_cuda(done)
@@ -687,8 +719,9 @@ class ResNet(FlatParamModule):
                 "tb_resnet_forward_unstacked")
             return logits, baseline, hN, cN, ("unstacked", scratch)
         _lib.check(
-            _lib.lib().tb_resnet_forward_obs(
-                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), *self.observation_shape, T1, B, self.num_actions,
+            _lib.lib().tb_resnet_forward_arch(
+                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), *self.observation_shape, *self.channels, T1, B,
+                self.num_actions,
                 self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
@@ -708,9 +741,9 @@ class ResNet(FlatParamModule):
             return
         frame = saved
         _lib.check(
-            _lib.lib().tb_resnet_backward_obs(
+            _lib.lib().tb_resnet_backward_arch(
                 p(frame.contiguous()), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
-                *self.observation_shape, T1, B, self.num_actions, self.num_values, int(self.use_lstm),
+                *self.observation_shape, *self.channels, T1, B, self.num_actions, self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(grads_out), _lib.stream_ptr()),
             "tb_resnet_backward")
 
