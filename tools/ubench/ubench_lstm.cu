@@ -3,7 +3,8 @@
 //   2. all-gather cost: 130 CTAs each pulling the same 137 KB from L2 into shared memory (cp.async 16 B vs TMA 2D boxes)
 //   3. store -> remote-poll visibility latency through L2 (one CTA stores, another spins on ld.relaxed.gpu)
 //   0. (printed first) the split kernels' per-warp gather: cp.async vs TMA boxes vs 2-CTA multicast TMA, at 1 .. 132
-//      CTAs, and whether a cooperative launch with 2-CTA clusters is accepted and co-resident at their footprint
+//      CTAs, and whether a cooperative launch with 2-CTA clusters is accepted and co-resident at their footprint; then
+//      a reduce-scatter alternative to the backward gather (fp32 pair partials through an L2 ring, fence, flags, 1 KB chunk gather)
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o ubench_lstm ubench_lstm.cu -lcuda
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -231,6 +232,128 @@ __global__ void __launch_bounds__(kGWarps * 32, 1) coresident_probe_kernel(unsig
   asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// ---- reduce-scatter exchange (an alternative to the backward all-gather, see DESIGN.md) at H = 519, B = 32: 132 CTAs in 2-CTA
+// clusters, CTAs [0, 66) the upper-layer role and [66, 132) the lower-layer role, 33 pairs per role.  Per step every CTA
+// meets its peer at a cluster barrier (stand-in for the DSMEM pair reduction), writes its half of the pair's fp32 partial
+// products to a 2-slot ring blocked [pair][8-column block][32 rows][8] - upper role: dh and dL/dh_lower, 2 x 33 blocks =
+// 66 KB; lower role: dh, 33 KB - then bar.sync, fence.acq_rel.gpu, flag; it then waits for the flags of the CTAs that hold
+// its column block in every pair (lower role: of both roles) and sums 33 (66) one-KB chunks in pair order.  Before it
+// overwrites a dL/dh_lower slot the upper role waits until every lower pair has read it (lower flags of the step before).
+constexpr int kRsPairs = 33, kRsRole = 2 * kRsPairs, kRsFlag = 32;
+constexpr size_t kRsSlotF = size_t(kRsPairs) * kRsRole * 256;   // floats in one ring slot of one product
+__device__ __forceinline__ void rs_wait_flag(const unsigned* f, unsigned v) {
+  unsigned x;
+  do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(x) : "l"(f) : "memory"); } while (x < v);
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(x) : "l"(f) : "memory");
+}
+__global__ void __launch_bounds__(kGWarps * 32, 1) rs_exchange_kernel(float* rec, float* ih, unsigned* flags, int reps, long long* cycles,
+                                                                      long long* phase, float* sink) {
+  __shared__ float red_s[256];
+  const int tid = threadIdx.x;
+  const bool upper = blockIdx.x < kRsRole;
+  const int cidx = upper ? blockIdx.x : blockIdx.x - kRsRole, pair = cidx >> 1, rank = cidx & 1;
+  const int src_rank = cidx >= kRsPairs;   // the CTA rank that holds this CTA's column block in every pair
+  float* const rec_role = rec + (upper ? 0 : 2 * kRsSlotF);
+  const unsigned* const up_flags = flags;
+  const unsigned* const lo_flags = flags + kRsRole * kRsFlag;
+  const unsigned* const own_flags = upper ? up_flags : lo_flags;
+  float acc = 0.f;
+  long long ph[3] = {0, 0, 0};
+  g_cluster_sync();
+  const long long t0 = clock64();
+  for (int s = 0; s < reps; ++s) {
+    const long long p0 = clock64();
+    const size_t slot = size_t(s & 1) * kRsSlotF, mine = (size_t(pair) * kRsRole + size_t(rank) * kRsPairs) * 256;
+    g_cluster_sync();
+    if (upper && s >= 2 && tid < kRsPairs) rs_wait_flag(lo_flags + (2 * tid) * kRsFlag, unsigned(s));
+    __syncthreads();
+    float4* const dr = reinterpret_cast<float4*>(rec_role + slot + mine);
+    float4* const di = reinterpret_cast<float4*>(ih + slot + mine);
+    for (int i = tid; i < kRsPairs * 64; i += blockDim.x) {
+      const float4 v = make_float4(float(s), float(i), acc, 1.f);
+      dr[i] = v;
+      if (upper) di[i] = v;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      asm volatile("fence.acq_rel.gpu;" ::: "memory");
+      asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(flags + blockIdx.x * kRsFlag), "r"(unsigned(s + 1)) : "memory");
+    }
+    const long long p1 = clock64();
+    if (tid < kRsPairs) rs_wait_flag(own_flags + (2 * tid + src_rank) * kRsFlag, unsigned(s + 1));
+    else if (!upper && tid >= 64 && tid < 64 + kRsPairs) rs_wait_flag(up_flags + (2 * (tid - 64) + src_rank) * kRsFlag, unsigned(s + 1));
+    __syncthreads();
+    const long long p2 = clock64();
+    if (tid < 256) {
+      const float* g = rec_role + slot + size_t(cidx) * 256 + tid;
+      float v[kRsPairs];
+#pragma unroll
+      for (int p = 0; p < kRsPairs; ++p) v[p] = __ldcg(g + size_t(p) * kRsRole * 256);
+      float d = 0.f;
+#pragma unroll
+      for (int p = 0; p < kRsPairs; ++p) d += v[p];
+      if (!upper) {
+        const float* gi = ih + slot + size_t(cidx) * 256 + tid;
+#pragma unroll
+        for (int p = 0; p < kRsPairs; ++p) v[p] = __ldcg(gi + size_t(p) * kRsRole * 256);
+#pragma unroll
+        for (int p = 0; p < kRsPairs; ++p) d += v[p];
+      }
+      red_s[tid] = d;
+    }
+    __syncthreads();
+    acc += red_s[tid & 255] * 1e-9f;
+    const long long p3 = clock64();
+    ph[0] += p1 - p0; ph[1] += p2 - p1; ph[2] += p3 - p2;
+  }
+  const long long t1 = clock64();
+  g_cluster_sync();
+  if (tid == 0) {
+    cycles[blockIdx.x] = t1 - t0;
+    for (int i = 0; i < 3; ++i) phase[blockIdx.x * 3 + i] = ph[i];
+    sink[blockIdx.x] = acc;
+  }
+}
+
+static int rs_exchange() {
+  const int reps = 400, grid = 2 * kRsRole;
+  const size_t smem = 150 * 1024;   // one CTA per SM, as the wavefront kernels
+  float *rec, *ih, *sink; unsigned* flags; long long *cyc, *ph;
+  CK(cudaMalloc(&rec, 4 * kRsSlotF * sizeof(float))); CK(cudaMalloc(&ih, 2 * kRsSlotF * sizeof(float)));
+  CK(cudaMalloc(&flags, size_t(grid) * kRsFlag * 4)); CK(cudaMalloc(&cyc, grid * sizeof(long long)));
+  CK(cudaMalloc(&ph, 3 * grid * sizeof(long long))); CK(cudaMalloc(&sink, grid * sizeof(float)));
+  CK(cudaFuncSetAttribute(rs_exchange_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kGWarps * 32); cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute at[2];
+  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+  at[1].id = cudaLaunchAttributeCooperative; at[1].val.cooperative = 1;
+  cfg.attrs = at; cfg.numAttrs = 2;
+  int clusters = -1;
+  CK(cudaOccupancyMaxActiveClusters(&clusters, rs_exchange_kernel, &cfg));
+  if (clusters * 2 < grid) { printf("reduce-scatter exchange: not launched, %d co-resident 2-CTA clusters\n", clusters); return 0; }
+  std::vector<long long> h(grid), hp(3 * grid);
+  for (int run = 0; run < 2; ++run) {   // run 0 warms up
+    CK(cudaMemset(flags, 0, size_t(grid) * kRsFlag * 4));
+    CK(cudaLaunchKernelEx(&cfg, rs_exchange_kernel, rec, ih, flags, reps, cyc, ph, sink));
+    CK(cudaDeviceSynchronize());
+  }
+  CK(cudaMemcpy(h.data(), cyc, grid * sizeof(long long), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(hp.data(), ph, 3 * grid * sizeof(long long), cudaMemcpyDeviceToHost));
+  for (int role = 0; role < 2; ++role) {
+    long long mx = 0; double p[3] = {0, 0, 0};
+    for (int i = role * kRsRole; i < (role + 1) * kRsRole; ++i) {
+      mx = h[i] > mx ? h[i] : mx;
+      for (int k = 0; k < 3; ++k) p[k] += double(hp[3 * i + k]) / reps / kRsRole;
+    }
+    printf("reduce-scatter exchange, %s role (%d CTAs of %d): write %4.1f KB + read %4.1f KB per CTA per step: %6.0f cycles/step (max CTA); "
+           "mean split: cluster barrier + write + fence %5.0f, flag wait %5.0f, gather %5.0f\n",
+           role ? "lower" : "upper", kRsRole, grid, role ? 33.0 : 66.0, role ? 66.0 : 33.0, double(mx) / reps, p[0], p[1], p[2]);
+  }
+  CK(cudaFree(rec)); CK(cudaFree(ih)); CK(cudaFree(flags)); CK(cudaFree(cyc)); CK(cudaFree(ph)); CK(cudaFree(sink));
+  return 0;
+}
+
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                              const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
@@ -313,6 +436,7 @@ int main() {
     EncodeFn enc = nullptr; cudaDriverEntryPointQueryResult q;
     CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&enc, cudaEnableDefault, &q));
     if (split_gather(enc)) return 1;
+    if (rs_exchange()) return 1;
   }
   int clk = 0;
   cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);

@@ -37,6 +37,8 @@ static inline int64_t ld16(int64_t n) { return (n + 7) & ~int64_t(7); }
 // row length (bf16 elements) of the tensor-core recurrence's operand tiles: K padded to 16, +8 so that a
 // row is an odd number of 16-byte chunks (conflict-free ldmatrix)
 static inline int mma_hq(int H) { return ((H + 15) & ~15) + 8; }
+static unsigned wave_bwd_split_role_ctas(int H);
+static int wave_bwd_split_groups(int H);
 
 size_t lstm_ws_bytes(int64_t T1, int64_t B, int In, int H, int layers, int precision) {
   return lstm_ws(nullptr, T1, B, In, H, layers, precision).bytes;
@@ -88,7 +90,11 @@ LstmWs lstm_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int
   w.wg_scratch = (precision && layers == 2) ? takef(int64_t(4) * 4 * H * (((H > In ? H : In) + 31) & ~31)) : nullptr;
   w.dgp = takef(int64_t(2) * 4 * B * padded_h(H));
   w.sync = reinterpret_cast<unsigned*>(takef(64));
-  w.dxb = (precision == 2 && layers == 2) ? takef(T1 * int64_t((H + 7) / 8) * 256) : nullptr;
+  w.bwd_rec = w.bwd_dxr = nullptr;
+  if (precision == 2 && layers == 2) {   // lstm2_bwd_wave_split_kernel's rings: [2 slots][k-groups][column blocks][32][8] floats
+    const int64_t slot = int64_t(wave_bwd_split_groups(H)) * wave_bwd_split_role_ctas(H) * 256;
+    w.bwd_rec = takef(2 * 2 * slot); w.bwd_dxr = takef(2 * slot);
+  }
   w.flags = reinterpret_cast<unsigned*>(takef(2 * 512 * 32));  // 2 x 512 flags, 128 bytes apart (kFlagStride)
   w.Hp = padded_h(H);
   w.bytes = off;
@@ -1782,18 +1788,12 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 }
 // generic-proxy global writes (h / gate-gradient stores) vs the TMA reads of the same bytes
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-// one box of a rank-4 / rank-5 map into the same shared-memory offset of both CTAs of the pair; completes tx on the
+// one box of a rank-4 map into the same shared-memory offset of both CTAs of the pair; completes tx on the
 // mbarrier at `bar`'s offset in each of them
 __device__ __forceinline__ void tma_multicast_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(
           smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"((uint16_t)3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_multicast_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6, %7}], [%2], %8;" ::"r"(
-          smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "h"((uint16_t)3)
       : "memory");
 }
 // 128-byte aligned start of the dynamic shared memory (TMA destinations); the kernels request 128 bytes of slack
@@ -2083,15 +2083,20 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
 }
 
 // ---- split-precision backward wavefront (precision 2) ----------------------------------------------
-// lstm2_bwd_wave_mma_kernel's role split (CTAs [0, nc): upper layer recurrence + dL/dh_lower from the same tile;
-// CTAs [nc, 2nc): lower layer two wave steps behind; 8 hidden units per CTA) with hi/lo operand planes:
-//   * the four gate-gradient tiles of a step are 4 x (hi + lo) x 34 KB = 274 KB - more than shared memory - so they
-//     stream through a 2-deep ring by gate (the multicast TMA boxes of gate g+2 under the MMAs of gate g+1);
-//   * 11 MMA warps x 3 k16-steps cover one gate's K = 528 exactly; W_hh^T (and, upper role, W_ih_upper^T) as hi AND lo
-//     B fragments in registers (96 per thread);
-//   * per-CTA flags instead of the counter barrier (see lstm2_fwd_wave_split_kernel): a CTA waits for the CTAs of its
-//     own role (they produce the tile it pulls) and, lower role, for the upper CTA that owns the same 8 columns
-//     (it produces this CTA's dL/dh_lower).
+// Role split: CTAs [0, nc) run the upper layer's recurrence and produce dL/dh_lower; CTAs [nc, 2nc) run the lower layer
+// one wave step behind (it consumes dL/dh_lower[t] in the step after the upper role produced it).  8 hidden units
+// (kBwdCols) of the pointwise phase per CTA.
+// The recurrent product dh_{t-1} = dgates_t . W_hh (and, upper role, dL/dh_lower[t] = dgates_t . W_ih_upper) has K = 4H
+// and N = H.  It is split over K into k-groups of 48 units (all four gates of units [48w, 48w + 48)) and over N into n8
+// column tiles; ONE warp owns one (k-group, tile) item for all steps and accumulates it as one chain of mma3 over the
+// group's 12 k16 steps (gate-major), with that item's W fragments in registers (hi AND lo: 48 per matrix, 96 in the upper
+// role).  The CTAs of k-group w (gc of them, 11 tiles each) load only the gate gradients of the group's 6 producer CTAs
+// (24 KB with lo planes) instead of the whole 4H-wide tile (274 KB), and publish their per-tile partial products (1 KB per
+// tile and matrix) to an fp32 ring; the CTA owning a column block then sums the ngroups partials of its block in group
+// order.  Per step there are two hand-offs through per-CTA flags (stores, bar.sync, fence.acq_rel.gpu, flag = step + 1;
+// see lstm2_fwd_wave_split_kernel): A = gate gradients published, B = partial products published.
+// The chain of one item is exactly the chain one warp of the all-gather formulation ran (same operands, same MMA order),
+// and the partials are summed in the same order, so the results are those of that formulation bit for bit.
 struct WaveBwdSplitArgs {
   const float* w_hh_up; const float* w_hh_lo; const float* w_ih_up;
   const float* dy; const float* nd;
@@ -2101,75 +2106,71 @@ struct WaveBwdSplitArgs {
   __nv_bfloat16* dgb_up; __nv_bfloat16* dgb_lo; int lg; int64_t dgb_lo_off;   // gate gradients of all steps, hi plane (+ lo offset)
   float* db_up; float* db_lo;
   __nv_bfloat16* dgq_up; __nv_bfloat16* dgq_lo; int64_t dgq_lo_off;          // exchange planes: [2][4, B, Hq] (+ lo offset)
-  float* dxb;                       // dL/dh_lower, blocked [T1][ncol][32 rows][8 cols]: upper role -> lower role
-  unsigned* flags;                  // [2 * nc]
+  float* rec;                       // dh partials: [role][2 slots][ngroups][nc column blocks][32 rows][8 cols]
+  float* dxr;                       // dL/dh_lower partials, upper role -> lower role: [2 slots][ngroups][nc][32][8]
+  unsigned* flags;                  // A: [0, 2nc), B: [256, 256 + 2nc), kFlagStride apart
   int T1, B, H, Hq;
-  unsigned nc;                      // CTAs per role, padded to whole clusters
-  unsigned ncol;                    // CTAs per role that own columns < H (= ceil(H / 8))
+  unsigned nc;                      // CTAs per role (>= ncol, >= ngroups * gc)
+  unsigned ncol;                    // CTAs per role that own columns < H (= ceil(H / 8)) = n8 column tiles
+  int ngroups, gc;                  // k-groups (ceil(ceil(H/16) / 3)) and CTAs per k-group (ceil(ncol / 11))
   const float* dhN; const float* dcN; float* dc0;  // [2, B, H] or null: each role uses its layer's slice
 };
+constexpr int kBwdGroupCtas = kSplitK * 16 / kBwdCols;   // producer CTAs of one k-group's gate gradients (6)
+constexpr int kBwdGateE = 2 * kHalfE;                    // one gate's tile: [row half][hi, lo][16 rows][kTileRowE]
+constexpr int kBwdFlagsB = 256;                          // flag index of the B flags
+constexpr int kBwdMaxGroups = kSplitWarps;              // k-groups of ceil(H/16) <= 33 k16 steps, 3 per group
 
-// dgq_map[role]: that role's exchange planes as a rank-5 map {Hq, B, gate, ping-pong buffer, plane}, box
-// {kTileRowE, 16, 1, 1, 2}: rows >= B and columns >= Hq are zero-filled.  Launched as 2-CTA clusters, every pair within
-// one role; a role's padding CTA (index >= ncol, all columns past H) takes part in the loads and the flag protocol only.
-__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(const __grid_constant__ CUtensorMap dgq_map_up,
-                                                                               const __grid_constant__ CUtensorMap dgq_map_lo,
-                                                                               WaveBwdSplitArgs a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  unsigned char* const smem_b = smem_align128(smem_raw);
+__device__ __forceinline__ void wait_flag(const unsigned* f, unsigned v) {
+  while (ld_relaxed_u32(f) < v) {}
+  (void)ld_acquire_u32(f);
+}
+
+__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(WaveBwdSplitArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
   const int H = a.H, Hq = a.Hq, B = a.B;
-  // Every tile element is consumed by exactly one warp (K = (gate, unit) is split across the warps: this warp owns units
-  // [16*ks0, 16*ks0 + 48) of every gate), so the tiles stream through WARP-PRIVATE 2-slot rings - slot = one gate,
-  // [row half = CTA rank that loads it][hi, lo][16 rows][kTileRowE] - with no block barrier anywhere in the fetch / MMA
-  // phase.  The same warp of the peer CTA streams the same columns: each CTA loads one row half and multicasts it.
-  __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_b) + int64_t(wrp) * 4 * kHalfE;
-  typedef float PartT[2][kBwdCols][33];
-  PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes);  // [11 warps][product][col][row]
-  __shared__ float dh_s[kBwdCols][33];
-  __shared__ float dc_s[kBwdCols][33];
-  __shared__ __align__(16) __nv_bfloat16 stg_s[2][4][32][kBwdCols];       // [plane][gate][row][col]
-  // per warp and ring slot: full (this CTA's expect_tx, both CTAs' bytes), empty (this warp + the peer CTA's warp done)
-  __shared__ __align__(8) uint64_t full_s[kSplitWarps][2], empty_s[kSplitWarps][2];
-  const uint32_t rank = cluster_rank();
-  if (lane == 0) {
-    mbar_init(&full_s[wrp][0], 1); mbar_init(&full_s[wrp][1], 1);
-    mbar_init(&empty_s[wrp][0], 2); mbar_init(&empty_s[wrp][1], 2);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  const uint32_t peer_empty0 = peer_addr(&empty_s[wrp][0], rank ^ 1u), peer_empty1 = peer_addr(&empty_s[wrp][1], rank ^ 1u);
   const bool upper = blockIdx.x < a.nc;
-  const CUtensorMap* const dgq_map = upper ? &dgq_map_up : &dgq_map_lo;
+  const int role = upper ? 0 : 1;
   const int cidx = int(upper ? blockIdx.x : blockIdx.x - a.nc);
   const int k0 = cidx * kBwdCols;
   const int rows = B < 32 ? B : 32;
   const int kpg = (H + 15) / 16;           // k16 steps per gate (<= 33)
-  const int ks0 = wrp * kSplitK;           // this warp's k-steps inside every gate
-  const float* const w_hh = upper ? a.w_hh_up : a.w_hh_lo;
+  const bool idle = cidx >= int(a.ncol);   // pointwise: all units past H
+  // this CTA's products: k-group w, tiles (cidx % gc) * 11 + warp
+  const bool work = cidx < a.ngroups * a.gc;
+  const int w = work ? cidx / a.gc : 0, ks0 = w * kSplitK;
+  const int nt = (cidx % a.gc) * kSplitWarps + wrp;
+  const bool tile_ok = work && nt < int(a.ncol);
+  // the group's gate-gradient tiles [gate][row half][hi, lo][16 rows][kTileRowE]; rows >= B stay zero
+  __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_raw);
+  // The pointwise operands of the NEXT step (forward saves: 4 gates, c, masked c_prev, dy, 2 done masks) are prefetched
+  // into SHARED memory with 4-byte cp.async while this step's hand-offs and products run: held in registers they spilled
+  // to local memory (168-register cap with the 96 fragment registers) and their load latency landed on the critical path.
+  // layout: [0,1024) activated gates of the two forward CTAs whose units this CTA owns ([2][32 rows][16]); [1024,1280) c_t
+  // ([2][32][4]); [1280,1536) c_{t-1}; [1536,1792) dy ([32 rows][8 cols], upper role); [1792,1856) notdone_t, notdone_{t+1}
+  float* const pre_s = reinterpret_cast<float*>(smem_raw + size_t(4) * kBwdGateE * 2);
+  __shared__ float dh_s[kBwdCols][33];   // recurrent dh of the next step (before its done mask), gathered
+  __shared__ float dx_s[kBwdCols][33];   // lower role: dL/dh_lower of the next step, gathered
+  __shared__ float dc_s[kBwdCols][33];
+  __shared__ __align__(16) __nv_bfloat16 stg_s[2][4][32][kBwdCols];       // [plane][gate][row][col]
   const float* const gact = upper ? a.gact_up : a.gact_lo;
   const float* const csb = upper ? a.csb_up : a.csb_lo;
   __nv_bfloat16* const dgb = upper ? a.dgb_up : a.dgb_lo;
   __nv_bfloat16* const dgq = upper ? a.dgq_up : a.dgq_lo;
-  const bool idle = cidx >= int(a.ncol);
-  // B fragments: B[kk][n] = W[g*H + j][k0 + n] for kk = (gate g, j)
+  // B fragments of this warp's item: B[kk][n] = W[g*H + j][nt*8 + n] for kk = (gate g, unit j of the group)
   uint32_t bh[4][kSplitK][2], bl[4][kSplitK][2], ih[4][kSplitK][2], il[4][kSplitK][2];
-  // The pointwise operands of the NEXT step (forward saves: 4 gates, c, masked c_prev, dy, 2 done masks) are prefetched
-  // into SHARED memory with 4-byte cp.async while this step's hand-off and products run: held in registers they spilled
-  // to local memory (168-register cap with the 96 fragment registers) and their load latency landed on the critical path.
-  // layout: [0,1024) activated gates of the two forward CTAs whose units this CTA owns ([2][32 rows][16]); [1024,1280) c_t
-  // ([2][32][4]); [1280,1536) c_{t-1}; [1536,1792) dy ([32 rows][8 cols], upper role); [1792,1856) notdone_t, notdone_{t+1}
-  float* const pre_s = reinterpret_cast<float*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33);
   {
-    const int n = lane >> 2;
+    const float* const w_hh = upper ? a.w_hh_up : a.w_hh_lo;
+    const int n = nt * 8 + (lane >> 2);
 #pragma unroll
     for (int g = 0; g < 4; ++g)
 #pragma unroll
       for (int sk = 0; sk < kSplitK; ++sk) {
         const int j = (ks0 + sk) * 16 + (lane & 3) * 2;
         float v[4] = {0.f, 0.f, 0.f, 0.f}, u[4] = {0.f, 0.f, 0.f, 0.f};
-        if (ks0 + sk < kpg && k0 + n < H) {
-          const float* wc = w_hh + int64_t(g) * H * H + (k0 + n);
-          const float* ic = a.w_ih_up + int64_t(g) * H * H + (k0 + n);
+        if (tile_ok && ks0 + sk < kpg && n < H) {
+          const float* wc = w_hh + int64_t(g) * H * H + n;
+          const float* ic = a.w_ih_up + int64_t(g) * H * H + n;
           if (j < H) { v[0] = wc[int64_t(j) * H]; if (upper) u[0] = ic[int64_t(j) * H]; }
           if (j + 1 < H) { v[1] = wc[int64_t(j + 1) * H]; if (upper) u[1] = ic[int64_t(j + 1) * H]; }
           if (j + 8 < H) { v[2] = wc[int64_t(j + 8) * H]; if (upper) u[2] = ic[int64_t(j + 8) * H]; }
@@ -2181,16 +2182,18 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         split_pack(u[2], u[3], ih[g][sk][1], il[g][sk][1]);
       }
   }
-  if (wrp < kBwdCols) { dh_s[wrp][lane] = 0.0f; dc_s[wrp][lane] = 0.0f; }
-  cluster_sync_all();   // also: the peer's mbarriers are initialised before any multicast or remote arrive
+  for (int i = tid; i < 4 * kBwdGateE / 8; i += kSplitThreads) reinterpret_cast<uint4*>(X)[i] = make_uint4(0u, 0u, 0u, 0u);
+  if (wrp < kBwdCols) { dh_s[wrp][lane] = 0.0f; dx_s[wrp][lane] = 0.0f; dc_s[wrp][lane] = 0.0f; }
   const int64_t gs = int64_t(B) * Hq;      // one gate of one exchange buffer
   const int q = wrp;  // pointwise role: thread = (batch row lane, unit k0 + wrp), warps 0..7
   const bool actA = (wrp < kBwdCols && lane < rows && k0 + q < H);
-  auto time_of = [&](int s) { return upper ? a.T1 - 1 - s : a.T1 + 1 - s; };
-  float n_dy = 0.f;
+  auto time_of = [&](int s) { return upper ? a.T1 - 1 - s : a.T1 - s; };
   auto prefetch = [&](int t) {   // every thread commits one group; all copies are coalesced runs
     if (t >= 0 && t < a.T1) {
-      for (int idx = tid; idx < 384; idx += kSplitThreads) {
+#pragma unroll
+      for (int rep = 0; rep < 2; ++rep) {   // 384 copies: at most two per thread
+        const int idx = tid + rep * kSplitThreads;
+        if (idx >= 384) break;
         const float* src; float* dst;
         if (idx < 256) {          // activated gates: 2 forward-CTA blocks x 128 chunks
           const int blk = idx >> 7, fc = 2 * cidx + blk;
@@ -2217,10 +2220,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
-  auto fetch_dxm = [&](int t) {
-    if (upper || !actA || t < 0 || t >= a.T1) return;
-    n_dy = __ldcg(a.dxb + (int64_t(t) * a.ncol + cidx) * 256 + lane * 8 + q);
-  };
   // gate-gradient rows of all steps for the hoisted weight-gradient GEMMs ([N, lg] hi / lo planes): written from the staging
   // tile with 8 lanes per 16-byte run (4 cache lines per warp store; one 2-byte store per lane-row touched 32)
   auto store_dg = [&](int64_t row0s) {
@@ -2230,29 +2229,31 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         dgb[(pl ? a.dgb_lo_off : 0) + (row0s + r) * a.lg + int64_t(g) * H + k0 + e] = stg_s[pl][g][r][e];
     }
   };
-  if (upper) prefetch(a.T1 - 1); else asm volatile("cp.async.commit_group;" ::: "memory");
+  prefetch(time_of(0));
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   float bs_i = 0.f, bs_f = 0.f, bs_g = 0.f, bs_o = 0.f;
-  const int last_s = a.T1 + 1;
-  unsigned* const my_flag = a.flags + blockIdx.x * kFlagStride;
-  const unsigned* const role_flags = a.flags + (upper ? 0 : a.nc) * kFlagStride;
+  const int last_s = a.T1;
+  const int64_t slot_f = int64_t(a.ngroups) * a.nc * 256;   // floats in one ring slot
+  float* const rec = a.rec + (upper ? 0 : 2 * slot_f);
+  auto flag_a = [&](int r, int c) { return a.flags + (r * int(a.nc) + c) * kFlagStride; };
+  auto flag_b = [&](int r, int c) { return a.flags + (kBwdFlagsB + r * int(a.nc) + c) * kFlagStride; };
   int it = 0;  // this role's active-step counter
-  bool fetched = false;   // a tile fetch has run (the ring's empty barriers have completed phases)
   for (int s = 0; s <= last_s; ++s) {
     const int t = time_of(s);
     const bool active = (t >= 0 && t < a.T1);
     const int64_t row0 = int64_t(active ? t : 0) * B;
-    __nv_bfloat16* dgq_t = dgq + int64_t(it & 1) * 4 * gs;
+    const int slot = s & 1;
+    __nv_bfloat16* const dgq_t = dgq + int64_t(slot) * 4 * gs;
     float p_i = 0.f, p_f = 0.f, p_g = 0.f, p_o = 0.f;
     if (active) {
-      if (actA) {   // (the prefetched operands were waited for, and made visible by the barrier, at the end of the previous step)
+      if (actA) {   // (the prefetched and gathered operands were made visible by the barrier at the end of the previous step)
         const int gb = (q >> 2) * 512 + lane * 16 + (q & 3), cb = (q >> 2) * 128 + lane * 4 + (q & 3);
         const float ig = pre_s[gb], fg = pre_s[gb + 4], gg = pre_s[gb + 8], og = pre_s[gb + 12];
         const float n_nd = pre_s[1792 + lane];
         const float n_cs = pre_s[1024 + cb], n_cm = pre_s[1280 + cb] * n_nd;   // c_{t-1} * notdone_t
         const float n_ndn = (t + 1 < a.T1) ? pre_s[1824 + lane] : 0.f;
-        float dh = upper ? pre_s[1536 + lane * 8 + q] : n_dy;
+        float dh = upper ? pre_s[1536 + lane * 8 + q] : dx_s[q][lane];
         float dc = 0.0f;
         const int64_t si = (upper ? int64_t(B) * H : 0) + int64_t(lane) * H + k0 + q;   // this role's layer in [2, B, H]
         if (it > 0) {
@@ -2273,8 +2274,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         if (t == 0 && a.dc0) a.dc0[si] = carry;
         bs_i += p_i; bs_f += p_f; bs_g += p_g; bs_o += p_o;
       }
-      // publish this CTA's 8 columns of the four gate-gradient tiles, hi and lo planes (16-byte stores staged through smem)
-      if (wrp < kBwdCols) {
+      if (wrp < kBwdCols) {   // this CTA's 8 columns of the four gate-gradient tiles, hi and lo planes
         const float p[4] = {p_i, p_f, p_g, p_o};
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
@@ -2283,107 +2283,113 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
           stg_s[1][g][lane][q] = __float2bfloat16_rn(p[g] - __bfloat162float(h));
         }
       }
-      __syncthreads();
-      if (tid < 256 && (tid & 31) < rows && !idle) {
-        const int pl = tid >> 7, g = (tid >> 5) & 3, bb = tid & 31;
-        *reinterpret_cast<uint4*>(dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(bb) * Hq + k0) =
-            *reinterpret_cast<const uint4*>(&stg_s[pl][g][bb][0]);
-        fence_proxy_async_global();   // consumers read the tiles through TMA
-      }
     }
-    if (s == last_s) {
-      if (active) { __syncthreads(); store_dg(row0); }
-      break;
+    // Buffer `slot` held step s-2's gate gradients; its readers (the gc CTAs of this CTA's k-group) post flag B = s-1
+    // after their products of step s-2.
+    if (s >= 2 && active && !idle && tid < a.gc) wait_flag(flag_b(role, (k0 / (kSplitK * 16)) * a.gc + tid), unsigned(s - 1));
+    __syncthreads();
+    if (active && tid < 256 && (tid & 31) < rows && !idle) {   // publish (16-byte stores staged through smem)
+      const int pl = tid >> 7, g = (tid >> 5) & 3, bb = tid & 31;
+      *reinterpret_cast<uint4*>(dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(bb) * Hq + k0) =
+          *reinterpret_cast<const uint4*>(&stg_s[pl][g][bb][0]);
     }
     __syncthreads();
-    if (tid == 0) {  // this CTA's tile columns of wave step s (and, upper role, its dxm of step s-1) are out
+    if (tid == 0) {   // hand-off A: this CTA's gate gradients of wave step s are out
       asm volatile("fence.acq_rel.gpu;" ::: "memory");
-      st_relaxed_u32(my_flag, unsigned(s + 1));
+      st_relaxed_u32(flag_a(role, cidx), unsigned(s + 1));
     }
     if (active) store_dg(row0);
-    prefetch(time_of(s + 1));  // forward-pass operands only: overlaps the wait
-    // hand-off: this warp needs the tile columns of units [16*ks0, 16*ks0 + 48) -> the 6 CTAs of its own role that own
-    // them; the pointwise threads of the lower role additionally need the upper CTA with the same 8 columns (its dxm)
-    {
-      const int p0 = (ks0 * 16) / kBwdCols + lane;
-      const int pend = (min((ks0 + kSplitK) * 16, H) + kBwdCols - 1) / kBwdCols;
-      if (lane < 6 && p0 < pend && p0 < int(a.ncol)) {
-        while (ld_relaxed_u32(role_flags + p0 * kFlagStride) < unsigned(s + 1)) {}
-        (void)ld_acquire_u32(role_flags + p0 * kFlagStride);
-        fence_proxy_async_global();
-      } else if (!upper && lane == 8 && wrp < kBwdCols) {
-        while (ld_relaxed_u32(a.flags + cidx * kFlagStride) < unsigned(s + 1)) {}
-        (void)ld_acquire_u32(a.flags + cidx * kFlagStride);
+    const int tn = time_of(s + 1);
+    prefetch(tn);  // forward-pass operands only: overlaps the hand-offs
+    const bool need_rec = active && t > 0;   // dh_{t-1}; at t = 0 lstm_dh0_kernel forms it from the dgb rows
+    const bool need_dx = active && upper;    // dL/dh_lower[t]
+    if (work && (need_rec || need_dx)) {
+      if (tid < kBwdGroupCtas && w * kBwdGroupCtas + tid < int(a.nc))
+        wait_flag(flag_a(role, w * kBwdGroupCtas + tid), unsigned(s + 1));
+      __syncthreads();
+      // the group's 48 columns of the four gates, rows < B, both planes: 6 x 16-byte copies per (gate, plane, row)
+      for (int i = tid; i < 4 * 2 * rows * 6; i += kSplitThreads) {
+        const int c = i % 6, r = (i / 6) % rows, pl = (i / (6 * rows)) & 1, g = i / (12 * rows);
+        cp_async16(X + g * kBwdGateE + (r >> 4) * kHalfE + pl * 16 * kTileRowE + (r & 15) * kTileRowE + c * 8,
+                   dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(r) * Hq + ks0 * 16 + c * 8);
       }
-      __syncwarp();
-    }
-    fetch_dxm(time_of(s + 1));  // written by the upper role before it published wave step s
-    const bool need_rec = active && t > 0;
-    const bool need_dx = active && upper;
-    if (need_rec || need_dx) {
-      // Ring slot g & 1 holds gate g: its full and empty barriers complete twice per fetching step (gates g & 1 and
-      // (g & 1) + 2), so the phase parity of gate g is g >> 1 on the full barrier; before gate g is loaded, the empty
-      // barrier's previous phase (gate g - 2, or gate g + 2 of the previous fetching step) must have completed.
-      auto issue = [&](int g) {   // lane 0: this CTA's row half of this warp's columns of gate g, both planes
-        if (g >= 2 || fetched) mbar_wait_cluster(&empty_s[wrp][g & 1], g >= 2 ? 0u : 1u);
-        fence_proxy_async_global();
-        mbar_expect_tx(&full_s[wrp][g & 1], kSlotBytes);
-        tma_multicast_5d(X + ((g & 1) * 2 + rank) * kHalfE, dgq_map, &full_s[wrp][g & 1], ks0 * 16, 16 * int(rank), g, it & 1, 0);
-      };
-      float acc0[2][4], acc1[2][4];
+      asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+      __syncthreads();
+      if (tile_ok) {
+        float acc0[2][4], acc1[2][4];
 #pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
+        for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { acc0[mt][e] = 0.f; acc1[mt][e] = 0.f; }
-      if (lane == 0) { issue(0); issue(1); }
+          for (int e = 0; e < 4; ++e) { acc0[mt][e] = 0.f; acc1[mt][e] = 0.f; }
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        mbar_wait(&full_s[wrp][g & 1], uint32_t(g >> 1));
-        const __nv_bfloat16* Xg = X + (g & 1) * 2 * kHalfE;
+        for (int g = 0; g < 4; ++g)
 #pragma unroll
-        for (int sk = 0; sk < kSplitK; ++sk) {
-          if (ks0 + sk < kpg) {
+          for (int sk = 0; sk < kSplitK; ++sk) {
+            if (ks0 + sk < kpg) {
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = the row half CTA rank mt loaded
-              uint32_t ah[4], al[4];
-              const int off = mt * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
-              ldmatrix_x4(ah, Xg + off);
-              ldmatrix_x4(al, Xg + 16 * kTileRowE + off);
-              if (need_rec) mma3(acc0[mt], ah, al, bh[g][sk][0], bh[g][sk][1], bl[g][sk][0], bl[g][sk][1]);
-              if (need_dx) mma3(acc1[mt], ah, al, ih[g][sk][0], ih[g][sk][1], il[g][sk][0], il[g][sk][1]);
+              for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = batch rows [16 mt, 16 mt + 16)
+                uint32_t ah[4], al[4];
+                const int off = g * kBwdGateE + mt * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
+                ldmatrix_x4(ah, X + off);
+                ldmatrix_x4(al, X + 16 * kTileRowE + off);
+                if (need_rec) mma3(acc0[mt], ah, al, bh[g][sk][0], bh[g][sk][1], bl[g][sk][0], bl[g][sk][1]);
+                if (need_dx) mma3(acc1[mt], ah, al, ih[g][sk][0], ih[g][sk][1], il[g][sk][0], il[g][sk][1]);
+              }
             }
           }
+        // Ring slot `slot` held step s-2's partials; their readers (the CTA owning column block nt, in this role and, for
+        // dL/dh_lower, in the lower role) post flag A = s after their gather of step s-2.
+        if (s >= 2) {
+          if (lane == 0 && need_rec) wait_flag(flag_a(role, nt), unsigned(s));
+          if (lane == 1 && need_dx) wait_flag(flag_a(1, nt), unsigned(s));
         }
         __syncwarp();
-        if (lane == 0) {   // slot read: free it for both loaders
-          mbar_arrive_local(&empty_s[wrp][g & 1]);
-          mbar_arrive_remote((g & 1) ? peer_empty1 : peer_empty0);
-          if (g + 2 < 4) issue(g + 2);
+        const int e = (lane >> 2) * 8 + (lane & 3) * 2;   // [row][col] of this lane's first accumulator pair
+        const int64_t chunk = ((int64_t(slot) * a.ngroups + w) * a.nc + nt) * 256;
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) {
+          if (need_rec) {
+            *reinterpret_cast<float2*>(rec + chunk + mt * 128 + e) = make_float2(acc0[mt][0], acc0[mt][1]);
+            *reinterpret_cast<float2*>(rec + chunk + mt * 128 + 64 + e) = make_float2(acc0[mt][2], acc0[mt][3]);
+          }
+          if (need_dx) {
+            *reinterpret_cast<float2*>(a.dxr + chunk + mt * 128 + e) = make_float2(acc1[mt][0], acc1[mt][1]);
+            *reinterpret_cast<float2*>(a.dxr + chunk + mt * 128 + 64 + e) = make_float2(acc1[mt][2], acc1[mt][3]);
+          }
         }
       }
-      fetched = true;
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int r = mt * 16 + (lane >> 2), c = (lane & 3) * 2;
-        part[wrp][0][c][r] = acc0[mt][0]; part[wrp][0][c + 1][r] = acc0[mt][1];
-        part[wrp][0][c][r + 8] = acc0[mt][2]; part[wrp][0][c + 1][r + 8] = acc0[mt][3];
-        part[wrp][1][c][r] = acc1[mt][0]; part[wrp][1][c + 1][r] = acc1[mt][1];
-        part[wrp][1][c][r + 8] = acc1[mt][2]; part[wrp][1][c + 1][r + 8] = acc1[mt][3];
+    }
+    __syncthreads();
+    if (tid == 0) {   // hand-off B: this CTA's partial products of wave step s are out
+      asm volatile("fence.acq_rel.gpu;" ::: "memory");
+      st_relaxed_u32(flag_b(role, cidx), unsigned(s + 1));
+    }
+    if (s == last_s) break;
+    // gather for step s + 1: dh_{t-1} from every k-group of this role (written in this step), and, lower role,
+    // dL/dh_lower[tn] from every k-group of the upper role (written by the upper role in this wave step)
+    const bool want_dx = !upper && tn >= 0 && tn < a.T1;
+    if (!idle && (need_rec || want_dx)) {
+      const int owner = cidx / kSplitWarps;   // CTA of k-group g that holds column tile cidx: g * gc + owner
+      if (tid < a.ngroups) {
+        if (need_rec) wait_flag(flag_b(role, tid * a.gc + owner), unsigned(s + 1));
+      } else if (tid >= 64 && tid < 64 + a.ngroups) {
+        if (want_dx) wait_flag(flag_b(0, (tid - 64) * a.gc + owner), unsigned(s + 1));
       }
       __syncthreads();
-      if (wrp < kBwdCols) {            // warps 0..7: recurrent carry for time t-1 (fixed summation order)
-        if (need_rec) {
-          float d = 0.f;
+      if (tid < 256) {
+        const int64_t base = (int64_t(slot) * a.ngroups * a.nc + cidx) * 256 + tid, gstride = int64_t(a.nc) * 256;
+        float vr[kBwdMaxGroups], vx[kBwdMaxGroups];   // all loads in flight before the first add
 #pragma unroll
-          for (int w = 0; w < kSplitWarps; ++w) d += part[w][0][wrp][lane];
-          dh_s[wrp][lane] = d;
+        for (int g = 0; g < kBwdMaxGroups; ++g) {
+          vr[g] = (need_rec && g < a.ngroups) ? __ldcg(rec + base + g * gstride) : 0.f;
+          vx[g] = (want_dx && g < a.ngroups) ? __ldcg(a.dxr + base + g * gstride) : 0.f;
         }
-        if (need_dx) {                 // dL/dh_lower[t], this CTA's 8 columns
-          float d = 0.f;
+        float dr = 0.f, dx = 0.f;
 #pragma unroll
-          for (int w = 0; w < kSplitWarps; ++w) d += part[w][1][wrp][lane];
-          if (lane < rows && !idle) a.dxb[(int64_t(t) * a.ncol + cidx) * 256 + lane * 8 + wrp] = d;
-        }
+        for (int g = 0; g < kBwdMaxGroups; ++g)   // fixed group order: deterministic
+          if (g < a.ngroups) { dr += vr[g]; dx += vx[g]; }
+        if (need_rec) dh_s[tid & 7][tid >> 3] = dr;
+        if (want_dx) dx_s[tid & 7][tid >> 3] = dx;
       }
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");   // next step's prefetched pointwise operands (all threads' copies)
@@ -2397,7 +2403,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
       db[k0 + q] = bs_i; db[H + k0 + q] = bs_f; db[2 * H + k0 + q] = bs_g; db[3 * H + k0 + q] = bs_o;
     }
   }
-  cluster_sync_all();   // no CTA exits with multicast writes or remote arrives into it still in flight
 }
 
 static Launch mma_fwd_launch(int H, cudaStream_t st) {
@@ -2471,20 +2476,23 @@ static Launch wave_fwd_split_launch(int H, cudaStream_t st) {
   return Launch(dim3(((H + kStepUnits - 1) / kStepUnits + 1) & ~1), kSplitThreads,
                 size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128, st, 2, true);
 }
-// backward: kBwdCols columns per CTA and role, padded to whole clusters (a cluster never straddles the two roles); tile
-// rings + partial sums + prefetched pointwise operands + alignment slack
-static unsigned wave_bwd_split_role_ctas(int H) { return unsigned(((H + kBwdCols - 1) / kBwdCols + 1) & ~1); }
+// backward: per role, kBwdCols pointwise columns per CTA (padded to an even count), and at least the ngroups x gc CTAs that
+// run the products; shared memory: the k-group's gate-gradient tiles + prefetched pointwise operands
+static int wave_bwd_split_groups(int H) { return ((H + 15) / 16 + kSplitK - 1) / kSplitK; }
+static int wave_bwd_split_group_ctas(int H) { return ((H + kBwdCols - 1) / kBwdCols + kSplitWarps - 1) / kSplitWarps; }
+static unsigned wave_bwd_split_role_ctas(int H) {
+  const int ncol = (H + kBwdCols - 1) / kBwdCols, work = wave_bwd_split_groups(H) * wave_bwd_split_group_ctas(H);
+  return unsigned(std::max((ncol + 1) & ~1, work));
+}
 static Launch wave_bwd_split_launch(int H, cudaStream_t st) {
-  return Launch(dim3(2 * wave_bwd_split_role_ctas(H)), kSplitThreads,
-                size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * kBwdCols * 33 + sizeof(float) * 9 * 256 + 128,
-                st, 2, true);
+  return Launch(dim3(2 * wave_bwd_split_role_ctas(H)), kSplitThreads, size_t(4) * kBwdGateE * 2 + sizeof(float) * 9 * 256, st, 1, true);
 }
 // both split kernels: the backward consumes the blocked saves only the split forward writes
 static bool wave_split_fits(int64_t B, int In, int H) {
   if (B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
   const Launch f = wave_fwd_split_launch(H, nullptr), b = wave_bwd_split_launch(H, nullptr);
   if (int(f.cfg.gridDim.x) > kSplitThreads || f.cfg.gridDim.x > 512 || !fits<lstm2_fwd_wave_split_kernel>(f)) return false;
-  return int(b.cfg.gridDim.x / 2) + 1 <= kSplitThreads && b.cfg.gridDim.x <= 512 && fits<lstm2_bwd_wave_split_kernel>(b);
+  return b.cfg.gridDim.x <= 2 * (512 - kBwdFlagsB) && fits<lstm2_bwd_wave_split_kernel>(b);
 }
 
 static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const float* notdone, const float* c0, float* hN,
@@ -2914,7 +2922,7 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   const LstmLayerWs& L = ws.layer[0];
   unsigned* flags = ws.flags + 512 * kFlagStride;
   cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(unsigned) * 512 * kFlagStride, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(U.dgq, 0, size_t(U.dgq_lo + int64_t(2) * 4 * B * Hq) * 2, st);  // zero the row padding
+  if (e == cudaSuccess) e = cudaMemsetAsync(U.dgq, 0, size_t(U.dgq_lo + int64_t(2) * 4 * B * Hq) * 2, st);  // columns no CTA writes
   if (e == cudaSuccess) e = cudaMemsetAsync(L.dgq, 0, size_t(L.dgq_lo + int64_t(2) * 4 * B * Hq) * 2, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
   TB_REQUIRE(U.dgq_lo > 0 && U.dgq_lo == L.dgq_lo && U.dgb_lo > 0 && U.dgb_lo == L.dgb_lo, "lstm: split planes missing");
@@ -2922,22 +2930,16 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   a.w_hh_up = p.w_hh[1]; a.w_hh_lo = p.w_hh[0]; a.w_ih_up = p.w_ih[1];
   a.dy = dy; a.nd = notdone;
   a.gact_up = U.gact; a.csb_up = U.csb; a.gact_lo = L.gact; a.csb_lo = L.csb; a.nfwd = (H + kStepUnits - 1) / kStepUnits;
-  TB_REQUIRE(U.gact && U.csb && L.gact && L.csb && ws.dxb, "lstm: blocked save buffers missing");
+  TB_REQUIRE(U.gact && U.csb && L.gact && L.csb && ws.bwd_rec && ws.bwd_dxr, "lstm: blocked save buffers missing");
   a.dgb_up = static_cast<__nv_bfloat16*>(U.dgb); a.dgb_lo = static_cast<__nv_bfloat16*>(L.dgb); a.lg = int(ld16(4 * H));
   a.dgb_lo_off = U.dgb_lo;
   a.db_up = g.b_ih[1]; a.db_lo = g.b_ih[0];
   a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq); a.dgq_lo_off = U.dgq_lo;
-  a.dxb = ws.dxb; a.flags = flags;
+  a.rec = ws.bwd_rec; a.dxr = ws.bwd_dxr; a.flags = flags;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc; a.ncol = unsigned((H + kBwdCols - 1) / kBwdCols);
+  a.ngroups = wave_bwd_split_groups(H); a.gc = wave_bwd_split_group_ctas(H);
   a.dhN = sg.dhN; a.dcN = sg.dcN; a.dc0 = sg.dc0;
-  CUtensorMap maps[2];
-  for (int r = 0; r < 2; ++r) {
-    const uint64_t dims[5] = {uint64_t(Hq), uint64_t(B), 4, 2, 2};
-    const uint64_t strides[4] = {uint64_t(Hq) * 2, uint64_t(B) * Hq * 2, uint64_t(4) * B * Hq * 2, uint64_t(a.dgq_lo_off) * 2};
-    const uint32_t box[5] = {kTileRowE, 16, 1, 1, 2};
-    tcd::make_map_nd(&maps[r], r == 0 ? a.dgq_up : a.dgq_lo, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-  }
-  return launch(wave_bwd_split_launch(H, st), "lstm2_bwd_wave_split_kernel", lstm2_bwd_wave_split_kernel, maps[0], maps[1], a);
+  return launch(wave_bwd_split_launch(H, st), "lstm2_bwd_wave_split_kernel", lstm2_bwd_wave_split_kernel, a);
 }
 
 // ---- dL/dh0 of one layer, after its backward recurrence --------------------------------------------------------------

@@ -46,7 +46,8 @@ struct LstmWs {
   float* dc;      // [B, H] carry
   float* dx_mid;  // [T1*B, H] gradient w.r.t. the output of layer 0 (input of layer 1)
   unsigned* sync; // [64] grid-barrier counters of the persistent recurrence kernels (zeroed per launch)
-  float* dxb = nullptr;  // (precision 2) dL/dh_lower handed from the upper to the lower role, blocked [T1][ceil(H/8)][32][8]
+  float* bwd_rec = nullptr;  // (precision 2, two layers) the split backward's dh partials: [role][2 slots][k-groups][column blocks][32][8]
+  float* bwd_dxr = nullptr;  // (precision 2, two layers) its dL/dh_lower partials, upper -> lower role: [2][k-groups][column blocks][32][8]
   unsigned* flags; // [1024] per-CTA step flags of the split-precision recurrence kernels (forward [0,512), backward [512,1024))
   float* wg_scratch;  // split-K scratch private to the weight-gradient GEMMs (two layers, bf16 backend): lets them run on a
                       // side stream beside the caller's trunk backward, which uses the caller's scratch
