@@ -522,6 +522,16 @@ int tb_gemm_bf16_tn(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N
 int tb_gemm_bf16_ex(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N, int64_t K, int64_t lda,
                     int64_t ldb, int a_mn, int b_mn, float* C, int64_t ldc, int splits, float* partial,
                     void* stream);
+/* Split-bf16 ("bf16x3") form of tb_gemm_bf16_ex with the fused epilogue the network's products use: each operand holds
+ * its lo plane bf16(x - hi) a_lo / b_lo elements after its hi plane (same leading dimension), and every k-step issues
+ * lo.hi, hi.lo, hi.hi into one fp32 accumulator.  C = relu?(scale * acc + bias), then zeroed where mask_bf16 [M,N]
+ * (ldmask, nullable) is not positive; C_bf16 (nullable) gets the hi plane and, when c16_lo != 0, the lo plane c16_lo
+ * elements further.  splits > 1: fp32 C only, no mask.  A test and diagnostic entry point that reaches the learner's
+ * split-mode kernel configurations in isolation; the learner itself calls the kernel from C++, not through it.         */
+int tb_gemm_bf16x3_ex(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
+                      int a_mn, int b_mn, int64_t a_lo, int64_t b_lo, float* C, int64_t ldc, void* C_bf16, int64_t ldc16,
+                      int64_t c16_lo, const float* bias, float scale, int relu, const void* mask_bf16, int64_t ldmask,
+                      int splits, float* partial, void* stream);
 /* ---- implicit-GEMM convolutions (bf16 tensor-core backend) -------------------------------------------
  * The nn.Conv2d layers of AtariNet (monobeast.py:560-562: 8x8/4, 4x4/2, 3x3/1, no padding) as wgmma GEMMs whose
  * patch operand is read by TMA straight from the bf16 NHWC activation [Nf,H,W,C] (conv2/conv3) or gathered from a

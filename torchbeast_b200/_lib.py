@@ -66,6 +66,8 @@ _SIGNATURES = {
     "tb_pg_loss_f64": ([_vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_gemm_bf16_tn": ([_vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp, _i64, _vp, _i64, _vp, _f32, _int, _vp], _int),
     "tb_gemm_bf16_ex": ([_vp, _vp, _i64, _i64, _i64, _i64, _i64, _int, _int, _vp, _i64, _int, _vp, _vp], _int),
+    "tb_gemm_bf16x3_ex": ([_vp, _vp, _i64, _i64, _i64, _i64, _i64, _int, _int, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _vp,
+                           _f32, _int, _vp, _i64, _int, _vp, _vp], _int),
     "tb_conv_nhwc_bf16_fwd": ([_vp, _vp, _vp, _i64] + [_int] * 8 + [_vp, _vp, _vp], _int),
     "tb_conv_nhwc_bf16_dgrad": ([_vp, _vp, _vp, _i64] + [_int] * 7 + [_vp, _vp, _vp], _int),
     "tb_conv_nhwc_bf16_wgrad": ([_vp, _vp, _i64] + [_int] * 7 + [_vp, _vp, _i64, _vp], _int),

@@ -2,15 +2,16 @@
 //
 //   C[M,N] = epilogue( sum_k A[m,k] * B[n,k] )     A [M,K], B [N,K] bf16, K contiguous ("K-major")
 //
-// gemm_tc_kernel (dense GEMMs): one CTA computes a 128 x BLOCK_N tile.  Warp roles (160 threads):
-//   warp 4     TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 64 bf16 = 128 B) into a
-//                             shared-memory ring, mbarrier expect_tx / complete_tx
-//   warps 0-3  consumer     : one warpgroup issues wgmma.m64nNk16 (N = BLOCK_N) for both 64-row halves of
-//                             the tile, x4 per 64-wide k-block, keeping one wgmma group in flight; a ring slot
-//                             is handed back once the group that read it has completed.  The accumulator
-//                             fragments then go through a shared-memory staging tile so that each thread owns
-//                             one output row for the epilogue: scale / bias / ReLU / ReLU-mask, fp32 and/or
-//                             bf16 stores
+// gemm_tc_kernel (dense GEMMs): one CTA computes a 128 x BLOCK_N tile, BLOCK_N chosen per call (gemm_block_n).
+// Warp roles (384 threads, registers moved from the producer to the consumers with setmaxnreg):
+//   warp 8         TMA producer : cp.async.bulk.tensor.2d (SWIZZLE_128B boxes of 64 bf16 = 128 B) into a
+//                                 shared-memory ring of at least 3 stages, mbarrier expect_tx / complete_tx
+//   warps 0-3, 4-7 consumers    : two warpgroups on the SAME tile, warpgroup g owning rows [64g, 64g + 64): each
+//                                 issues its own wgmma.m64nNk16 chain (N = BLOCK_N), x4 per 64-wide k-block, one
+//                                 group in flight; a ring slot is handed back once both warpgroups' groups that read
+//                                 it have completed.  Each then runs the epilogue of its own 64 rows through its own
+//                                 64-column shared-memory staging tile, so that each thread owns one output row of
+//                                 a 32-column chunk: scale / bias / ReLU / ReLU-mask, fp32 and/or bf16 stores
 // M/N/K tails are handled by TMA out-of-bounds zero fill plus guarded stores.  Shared-memory
 // matrix descriptors: K-major, SWIZZLE_128B, SBO = 1024 B (8 rows x 128 B), advanced by 32 B per
 // K=16 step inside the swizzle atom (the CUTLASS/DeepGEMM canonical layout).
@@ -20,8 +21,8 @@
 //   forward  act = col . W^T      : A K-major,  B K-major
 //   dgrad    dcol = dY . W        : A K-major,  B MN-major (W [n', k'] as stored)
 //   wgrad    dW   = dY^T . col    : A MN-major, B MN-major (no transposed copies), split-K over grid.z
-// The implicit-GEMM convolutions run on conv_tc_kernel (two consumer warpgroups, up to 256-row tiles) and
-// conv_wgrad_implicit_kernel, described where they are defined.
+// The implicit-GEMM convolutions run on conv_tc_kernel (two consumer warpgroups taking alternate tiles, up to
+// 256-row tiles) and conv_wgrad_implicit_kernel, described where they are defined.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -44,22 +45,29 @@ namespace {
 // SPLIT (split-bf16, see TcEpilogue): a stage holds the hi AND lo plane tiles of both operands (tmAl / tmBl are the
 // lo planes' tensor maps) and every k-step issues three MMAs (lo.hi, hi.lo, hi.hi) into the same accumulator; the
 // epilogue can write its bf16 output as hi / lo planes.
+// Threads: warpgroups 0 and 1 are consumers, warp 8 of warpgroup 2 is the producer; the producer warpgroup gives its
+// registers to the consumers (ptxas budgets a 384-thread CTA at 168 registers per thread).
+constexpr int kTcThreads = 3 * kConsumers;
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;
+static_assert(kConsumers * (kProducerRegs + 2 * kConsumerRegs) <= 65536, "gemm_tc: register split exceeds the SM");
+
+// columns of one consumer warpgroup's staging tile: 64 rows x 64 columns, two 32-column chunks per row, one per thread
+constexpr int gemm_stage_cols(int block_n) { return block_n < 64 ? block_n : 64; }
+
 template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool SPLIT = false>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, TcEpilogue ep, int M,
                int N, int K, float* partial, int tiles_m, int tiles_n, int splits, int ldp) {
   constexpr uint32_t B_BYTES = BLOCK_N * kBlockK * 2;
   constexpr uint32_t A_STAGE = (SPLIT ? 2u : 1u) * kABytes, B_STAGE = (SPLIT ? 2u : 1u) * B_BYTES;  // [hi][lo]
-  constexpr int LDS = BLOCK_N + 4;  // staging row pitch in floats (16-byte rows, conflict-free row reads)
+  constexpr int SW = gemm_stage_cols(BLOCK_N);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024 B alignment
   const uint32_t sA = base, sB = base + kStages * A_STAGE;
-  const uint32_t bars = sB + kStages * B_STAGE;  // full[kStages], empty[kStages], then the accumulator staging tile
+  const uint32_t bars = sB + kStages * B_STAGE;  // full[kStages], empty[kStages], then the two staging tiles
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (kStages + s); };
-  // [128][LDS] fp32: the epilogue reads whole rows, the wgmma fragments are scattered over row pairs
-  float* stg = reinterpret_cast<float*>(smem_raw + (bars + 16u * kStages - smem_addr(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_kb = (K + kBlockK - 1) / kBlockK;
@@ -67,8 +75,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int tiles_mn = tiles_m * tiles_n;
   const int total_work = tiles_mn * splits;
 
-  if (warp == 4 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 4); }
+  if (warp == 8 && lane == 0) {  // a stage is free again once the 4 warps of BOTH consumer warpgroups have released it
+    for (int s = 0; s < kStages; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -84,8 +92,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     num_kb = kb1 > kb0 ? kb1 - kb0 : 0;
   };
 
-  if (warp == 4) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == 8 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
         int m0, n0, kb0, num_kb, z;
@@ -116,21 +125,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp < 4) {
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int g = warp >> 2;  // consumer warpgroup: rows [64g, 64g + 64) of every tile
+    const int tid = threadIdx.x & 127;
+    // [64][SW] fp32 per warpgroup, 16-byte chunk q of row rr stored at chunk q ^ (rr & 7): both the fragment writes
+    // (8 rows x 32 B per warp) and the row reads (32 rows x one chunk per warp) are free of bank conflicts
+    float* stg = reinterpret_cast<float*>(smem_raw + (bars + 16u * kStages - smem_addr(smem_raw))) + g * 64 * SW;
+    auto sidx = [](int rr, int col) { return rr * SW + ((((col >> 2) ^ (rr & 7))) << 2) + (col & 3); };
+    const int fr = (warp & 3) * 16 + (lane >> 2), fc = 2 * (lane & 3);  // fragment rows fr, fr + 8, columns 8j + fc
+    const int er = tid & 63, ec = (tid >> 6) * 32;                     // epilogue: staged row er, chunk ec
     int stage = 0; uint32_t phase = 0;
-    float acc[2][BLOCK_N / 2];  // rows [0, 64) and [64, 128) of the tile
+    float acc[BLOCK_N / 2];
     for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
       int m0, n0, kb0, num_kb, z;
       decode(w, m0, n0, kb0, num_kb, z);
-      const int rl = threadIdx.x;
-      const int64_t r = int64_t(m0) + rl;
+      const int64_t r = int64_t(m0) + g * 64 + er;
       const bool rvalid = r < M;
-      // EPI 2: pull the ReLU-mask / residual rows of the WHOLE tile into L2 before waiting for the accumulator, so
-      // their DRAM latency hides behind the MMA main loop
+      // EPI 2: pull this warpgroup's ReLU-mask / residual rows into L2 before waiting for the accumulator, so their
+      // DRAM latency hides behind the MMA main loop
       if constexpr (EPI >= 2) {
         if (rvalid) {
 #pragma unroll 1
-          for (int c0 = 0; c0 < BLOCK_N && n0 + c0 < N; c0 += 32) {
+          for (int c0 = ec; c0 < BLOCK_N && n0 + c0 < N; c0 += 64) {
             const int64_t pr = r; const int pc = n0 + c0;
             if (ep.mask16) asm volatile("prefetch.global.L2 [%0];" ::"l"(ep.mask16 + pr * ep.ldmask + pc));
             if (ep.addend16) asm volatile("prefetch.global.L2 [%0];" ::"l"(ep.addend16 + pr * ep.ldadd + pc));
@@ -143,23 +160,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(full(stage), phase);
         wgmma_fence();
-        const uint32_t aA = sA + stage * A_STAGE, aB = sB + stage * B_STAGE;
+        const uint32_t aA = sA + stage * A_STAGE + g * 8192, aB = sB + stage * B_STAGE;  // 64-row halves 8 KB apart
 #pragma unroll
         for (int k = 0; k < kBlockK / 16; ++k) {
           const uint64_t db = B_MN ? make_smem_desc_mn(aB + k * 2048) : make_smem_desc(aB + k * 32);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {  // the two 64-row halves of the tile (8192 B apart in both layouts)
-            const uint32_t ah = aA + h * 8192;
-            const uint64_t da = A_MN ? make_smem_desc_mn(ah + k * 2048) : make_smem_desc(ah + k * 32);
-            if constexpr (SPLIT) {  // small terms first: lo.hi, hi.lo, then hi.hi
-              const uint64_t dal = A_MN ? make_smem_desc_mn(ah + kABytes + k * 2048) : make_smem_desc(ah + kABytes + k * 32);
-              const uint64_t dbl = B_MN ? make_smem_desc_mn(aB + B_BYTES + k * 2048) : make_smem_desc(aB + B_BYTES + k * 32);
-              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], dal, db, (kb | k) != 0);
-              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, dbl, 1);
-              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, db, 1);
-            } else {
-              wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc[h], da, db, (kb | k) != 0);
-            }
+          const uint64_t da = A_MN ? make_smem_desc_mn(aA + k * 2048) : make_smem_desc(aA + k * 32);
+          if constexpr (SPLIT) {  // small terms first: lo.hi, hi.lo, then hi.hi
+            const uint64_t dal = A_MN ? make_smem_desc_mn(aA + kABytes + k * 2048) : make_smem_desc(aA + kABytes + k * 32);
+            const uint64_t dbl = B_MN ? make_smem_desc_mn(aB + B_BYTES + k * 2048) : make_smem_desc(aB + B_BYTES + k * 32);
+            wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc, dal, db, (kb | k) != 0);
+            wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc, da, dbl, 1);
+            wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc, da, db, 1);
+          } else {
+            wgmma_bf16<BLOCK_N, A_MN, B_MN>(acc, da, db, (kb | k) != 0);
           }
         }
         wgmma_commit();
@@ -172,27 +185,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty(prev)); }
       if (num_kb == 0) {  // nothing was accumulated (empty split)
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 2; ++j) { acc[0][j] = 0.0f; acc[1][j] = 0.0f; }
+        for (int j = 0; j < BLOCK_N / 2; ++j) acc[j] = 0.0f;
       }
-      named_sync(1, kConsumers);  // the previous tile's epilogue has read the staging tile
-      {
-        const int fr = warp * 16 + (lane >> 2), fc = 2 * (lane & 3);
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
-            float* sp = stg + (h * 64 + fr) * LDS + 8 * j + fc;
-            *reinterpret_cast<float2*>(sp) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
-            *reinterpret_cast<float2*>(sp + 8 * LDS) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
-          }
-      }
-      named_sync(1, kConsumers);
+      // epilogue in passes of SW columns: stage them, then thread (er, ec) finishes one 32-column chunk of row er
 #pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
+      for (int p = 0; p < BLOCK_N / SW; ++p) {
+        named_sync(1 + g, kConsumers);  // the previous pass has read the staging tile
+#pragma unroll
+        for (int q = 0; q < BLOCK_N / SW; ++q) {
+          if (q != p) continue;  // static register indices: acc is never addressed with the runtime p
+#pragma unroll
+          for (int j = 0; j < SW / 8; ++j) {
+            const int jj = q * (SW / 8) + j;
+            *reinterpret_cast<float2*>(stg + sidx(fr, 8 * j + fc)) = make_float2(acc[4 * jj], acc[4 * jj + 1]);
+            *reinterpret_cast<float2*>(stg + sidx(fr + 8, 8 * j + fc)) = make_float2(acc[4 * jj + 2], acc[4 * jj + 3]);
+          }
+        }
+        named_sync(1 + g, kConsumers);
+        if (ec >= SW) continue;  // 32-column tiles: one chunk per row, threads 64-127 idle
+        const int c0 = p * SW + ec;
         uint32_t v[32];
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
-          const float4 t = *reinterpret_cast<const float4*>(stg + rl * LDS + c0 + j);
+          const float4 t = *reinterpret_cast<const float4*>(stg + sidx(er, ec + j));
           v[j] = __float_as_uint(t.x); v[j + 1] = __float_as_uint(t.y); v[j + 2] = __float_as_uint(t.z); v[j + 3] = __float_as_uint(t.w);
         }
         if (partial) {  // split-K: raw partial tile [z][M][N]; splitk_reduce_kernel applies the epilogue
@@ -425,12 +440,8 @@ struct ImplicitConv {
 //     (half of its 32-column chunks) per pass.
 // Per output element the k-block order and the lo.hi, hi.lo, hi.hi order inside a k16 step are those of gemm_tc_kernel,
 // so the results are bit-identical to it.  EPI: 1 = scale / bias / ReLU; 2 = + bf16 ReLU mask (input gradient).
-constexpr int kConvThreads = 3 * kConsumers;
-constexpr int kProducerRegs = 24, kConsumerRegs = 240;
-static_assert(kConsumers * (kProducerRegs + 2 * kConsumerRegs) <= 65536, "conv_tc_kernel: register split exceeds the SM");
-
 template <int TM, int BLOCK_N, int kStages, int EPI, bool SPLIT>
-__global__ void __launch_bounds__(kConvThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmAl, const __grid_constant__ CUtensorMap tmBl, TcEpilogue ep, int M,
                int N, int K, int tiles_m, int tiles_n, ImplicitConv ic) {
@@ -690,8 +701,8 @@ static inline bool attr_done(uint64_t* mask) {
   return false;
 }
 
-// dynamic shared memory of gemm_tc_kernel / conv_tc_kernel with tm-row tiles: 1 KB alignment slack, the stage ring,
-// the barriers, the accumulator staging (one 128-row tile, or two 64-row tiles)
+// dynamic shared memory of conv_tc_kernel with tm-row tiles: 1 KB alignment slack, the stage ring, the barriers, the
+// accumulator staging (two 64-row tiles)
 constexpr size_t tc_smem(int tm, int block_n, int stages, bool split) {
   return 1024 + size_t(stages) * (split ? 2 : 1) * (size_t(tm) * kBlockK * 2 + size_t(block_n) * kBlockK * 2) + 16 * stages +
          size_t(kBlockM) * (block_n + 4) * 4 + 16;
@@ -703,8 +714,19 @@ constexpr int tc_stages(int tm, int block_n, int want, bool split) {
   return (want <= 2 || tc_smem(tm, block_n, want, split) <= 227 * 1024) ? want : tc_stages(tm, block_n, want - 1, split);
 }
 
-// CTAs of `kernel` resident per SM with `smem` bytes of dynamic shared memory: registers, not shared memory, are the
-// limit for most instantiations (a 128-column accumulator pair plus the epilogue needs > 204 registers per thread)
+// dynamic shared memory of gemm_tc_kernel: 1 KB alignment slack, the stage ring, the barriers, the two 64-row staging
+// tiles of gemm_stage_cols(block_n) columns
+constexpr size_t gemm_smem(int block_n, int stages, bool split) {
+  return 1024 + size_t(stages) * (split ? 2 : 1) * (size_t(kABytes) + size_t(block_n) * kBlockK * 2) + 16 * stages +
+         2 * 64 * size_t(gemm_stage_cols(block_n)) * 4;
+}
+// the deepest ring of at most 4 stages that fits: split mode 4 stages at BLOCK_N = 32 / 64 (40 / 48 KB per stage),
+// 3 at 128 (64 KB); single-plane 4 everywhere
+constexpr int gemm_stages(int block_n, bool split, int want = 4) {
+  return (want <= 1 || gemm_smem(block_n, want, split) <= 227 * 1024) ? want : gemm_stages(block_n, split, want - 1);
+}
+
+// CTAs of `kernel` resident per SM with `smem` bytes of dynamic shared memory
 template <typename Kernel>
 static int resident_per_sm(Kernel kernel, int threads, size_t smem) {
   int n = 0;
@@ -712,18 +734,19 @@ static int resident_per_sm(Kernel kernel, int threads, size_t smem) {
   return n;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, int EPI, bool SPLIT>
+template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool SPLIT>
 int launch_e(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
              float* partial, cudaStream_t stream) {
-  constexpr size_t smem = tc_smem(kBlockM, BLOCK_N, kStages, SPLIT);
-  static_assert(smem <= 227 * 1024, "gemm_tc: stage ring exceeds shared memory");
+  constexpr int kStages = gemm_stages(BLOCK_N, SPLIT);
+  constexpr size_t smem = gemm_smem(BLOCK_N, kStages, SPLIT);
+  static_assert(kStages >= 3 && smem <= 227 * 1024, "gemm_tc: fewer than 3 ring stages fit in shared memory");
   static uint64_t attr = 0;
   static int per_sm = 1;
   if (!attr_done(&attr)) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT>, kThreads, smem);
+    per_sm = resident_per_sm(gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT>, kTcThreads, smem);
   }
   const int64_t tiles_m = (M + kBlockM - 1) / kBlockM, tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n * splits;
@@ -732,37 +755,47 @@ int launch_e(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64
   int64_t grid = int64_t(kNumSMs) * per_sm;
   if (ep.max_ctas > 0 && grid > ep.max_ctas) grid = ep.max_ctas;
   if (grid > total) grid = total;
-  gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT><<<(unsigned)grid, kThreads, smem, stream>>>(
+  gemm_tc_kernel<BLOCK_N, A_MN, B_MN, kStages, EPI, SPLIT><<<(unsigned)grid, kTcThreads, smem, stream>>>(
       mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), partial, int(tiles_m), int(tiles_n), splits,
       int((N + 31) & ~int64_t(31)));
   return check_launch("gemm_tc_kernel");
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, int kStages, bool SPLIT>
-int launch_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
-             float* partial, cudaStream_t stream) {
-  const bool loads = ep.mask || ep.mask16 || ep.addend16 || ep.addend32;
-  const bool arith = ep.bias || ep.relu || ep.scale != 1.0f;
-  if (loads) return launch_e<BLOCK_N, A_MN, B_MN, kStages, 2, SPLIT>(mp, ep, M, N, K, splits, partial, stream);
-  if (arith && !partial) return launch_e<BLOCK_N, A_MN, B_MN, kStages, 1, SPLIT>(mp, ep, M, N, K, splits, partial, stream);
-  return launch_e<BLOCK_N, A_MN, B_MN, kStages, 0, SPLIT>(mp, ep, M, N, K, splits, partial, stream);
-}
-
-// Few k-blocks per CTA (dgrad: K = 64 channels): a deeper ring than 2 stages would only hold the next tile's data, so
-// the ring stays small.  Within a CTA the epilogue does not overlap the next tile's MMAs (the producer prefetches into
-// the ring meanwhile); overlap across CTAs happens only where registers allow two per SM.
-// Split mode doubles the stage (hi + lo planes); the ring is as deep as fits beside the accumulator staging tile.
 template <int BLOCK_N, bool A_MN, bool B_MN>
 int launch(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t N, int64_t K, int splits,
            float* partial, cudaStream_t stream) {
-  const int64_t kb_per_cta = ((K + kBlockK - 1) / kBlockK + splits - 1) / splits;
-  const bool split = ep.a_lo != 0;
-  if (split) {
-    if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, true>(mp, ep, M, N, K, splits, partial, stream);
-    return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(kBlockM, BLOCK_N, 4, true), true>(mp, ep, M, N, K, splits, partial, stream);
+  const bool loads = ep.mask || ep.mask16 || ep.addend16 || ep.addend32;
+  const bool arith = ep.bias || ep.relu || ep.scale != 1.0f;
+  const int epi = loads ? 2 : (arith && !partial ? 1 : 0);
+  if (ep.a_lo != 0) {  // split mode: stages of twice the size
+    if (epi == 2) return launch_e<BLOCK_N, A_MN, B_MN, 2, true>(mp, ep, M, N, K, splits, partial, stream);
+    if (epi == 1) return launch_e<BLOCK_N, A_MN, B_MN, 1, true>(mp, ep, M, N, K, splits, partial, stream);
+    return launch_e<BLOCK_N, A_MN, B_MN, 0, true>(mp, ep, M, N, K, splits, partial, stream);
   }
-  if (kb_per_cta <= 2) return launch_s<BLOCK_N, A_MN, B_MN, 2, false>(mp, ep, M, N, K, splits, partial, stream);
-  return launch_s<BLOCK_N, A_MN, B_MN, tc_stages(kBlockM, BLOCK_N, 4, false), false>(mp, ep, M, N, K, splits, partial, stream);
+  if (epi == 2) return launch_e<BLOCK_N, A_MN, B_MN, 2, false>(mp, ep, M, N, K, splits, partial, stream);
+  if (epi == 1) return launch_e<BLOCK_N, A_MN, B_MN, 1, false>(mp, ep, M, N, K, splits, partial, stream);
+  return launch_e<BLOCK_N, A_MN, B_MN, 0, false>(mp, ep, M, N, K, splits, partial, stream);
+}
+
+// BLOCK_N of a dense GEMM, chosen per call like implicit_tile_rows: the width that gives the busiest CTA the fewest MMA
+// columns, counted as waves of work items on the persistent grid x issued columns (padding included).  Every tile has two
+// 64-row groups and an item's k-blocks do not depend on the width, so those factors drop out; ties go to the wider tile
+// (fewer A-tile reloads).  At T=80, B=32 (N = 2592 rows) the weight gradients move to 64 columns: fc_wgrad 3 -> 5 waves
+// of 128 -> 64 columns, lstm_wgrad (N = 519: 5 x 128 = 640 issued columns vs 9 x 64 = 576) 3 -> 5 waves; the forward
+// and input-gradient products tie and keep 128.  32 columns only for N <= 32: a 32-wide split stage (40 KB of operands
+// per 768 MMA cycles) would ask more of L2 than it delivers to all SMs at once.
+static int gemm_block_n(int64_t M, int64_t N, int splits, bool b_mn, int max_ctas) {
+  const int64_t tiles_m = (M + kBlockM - 1) / kBlockM;
+  const int64_t grid = (max_ctas > 0 && max_ctas < kNumSMs) ? max_ctas : kNumSMs;
+  if (!b_mn && N <= 32) return 32;
+  int best = 0;
+  int64_t best_cost = 0;
+  for (int bn : {128, 64}) {
+    const int64_t items = tiles_m * ((N + bn - 1) / bn) * splits;
+    const int64_t cost = (items + grid - 1) / grid * bn;
+    if (!best || cost < best_cost) { best = bn; best_cost = cost; }
+  }
+  return best;
 }
 
 
@@ -896,13 +929,13 @@ int launch_conv_fwd_s(const TcMaps& mp, const TcEpilogue& ep, int64_t M, int64_t
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     TB_REQUIRE(e == cudaSuccess, "gemm_tc: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    per_sm = resident_per_sm(conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT>, kConvThreads, smem);
+    per_sm = resident_per_sm(conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT>, kTcThreads, smem);
   }
   const int64_t tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
   const int64_t total = tiles_m * tiles_n;
   int64_t grid = int64_t(kNumSMs) * per_sm;
   if (grid > total) grid = total;
-  conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT><<<(unsigned)grid, kConvThreads, smem, stream>>>(
+  conv_tc_kernel<TM, BLOCK_N, kSt, EPI, SPLIT><<<(unsigned)grid, kTcThreads, smem, stream>>>(
       mp.a, mp.b, mp.al, mp.bl, ep, int(M), int(N), int(K), int(tiles_m), int(tiles_n), ic);
   return check_launch("gemm_tc_kernel(implicit conv)");
 }
@@ -1142,8 +1175,7 @@ int gemm_tc_bf16_ex(const void* A, const void* B, int64_t M, int64_t N, int64_t 
   if (splits < 1) splits = 1;
   TB_REQUIRE(splits == 1 || partial, "gemm_tc: split-K needs a partial buffer");
   ProfScope prof(ep.tag, stream);
-  int bn = (N <= 32) ? 32 : (N <= 64 ? 64 : 128);
-  if (b_mn && bn < 64) bn = 64;  // MN-major tiles are built from 64-wide boxes
+  const int bn = gemm_block_n(M, N, splits, b_mn, ep.max_ctas);  // MN-major B: 64 or 128 (64-wide boxes)
   TB_REQUIRE((ep.a_lo != 0) == (ep.b_lo != 0), "gemm_tc: split mode needs the lo planes of both operands");
   TcMaps mp;
   // K-major operand [rows = mn, cols = k]: box {64 k, mn rows}.  MN-major operand [rows = k, cols = mn]: box {64 mn, 64 k}.
@@ -1226,6 +1258,19 @@ int tb_gemm_bf16_ex(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N
                     int a_mn, int b_mn, float* C, int64_t ldc, int splits, float* partial, void* stream) {
   TcEpilogue ep;
   ep.C = C; ep.ldc = ldc; ep.tag = "gemm_bf16_ex";
+  return gemm_tc_bf16_ex(A_bf16, B_bf16, M, N, K, lda, ldb, a_mn != 0, b_mn != 0, ep, splits, partial, (cudaStream_t)stream);
+}
+
+int tb_gemm_bf16x3_ex(const void* A_bf16, const void* B_bf16, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
+                      int a_mn, int b_mn, int64_t a_lo, int64_t b_lo, float* C, int64_t ldc, void* C_bf16, int64_t ldc16,
+                      int64_t c16_lo, const float* bias, float scale, int relu, const void* mask_bf16, int64_t ldmask,
+                      int splits, float* partial, void* stream) {
+  TB_REQUIRE(a_lo != 0 && b_lo != 0, "tb_gemm_bf16x3_ex: both operands need a lo plane");
+  TB_REQUIRE(splits <= 1 || (!C_bf16 && !mask_bf16), "tb_gemm_bf16x3_ex: split-K writes fp32 C only, without a mask");
+  TcEpilogue ep;
+  ep.C = C; ep.ldc = ldc; ep.C16 = static_cast<__nv_bfloat16*>(C_bf16); ep.ldc16 = ldc16; ep.c16_lo = c16_lo;
+  ep.a_lo = a_lo; ep.b_lo = b_lo; ep.bias = bias; ep.scale = scale; ep.relu = relu;
+  ep.mask16 = static_cast<const __nv_bfloat16*>(mask_bf16); ep.ldmask = ldmask; ep.tag = "gemm_bf16x3_ex";
   return gemm_tc_bf16_ex(A_bf16, B_bf16, M, N, K, lda, ldb, a_mn != 0, b_mn != 0, ep, splits, partial, (cudaStream_t)stream);
 }
 
