@@ -550,6 +550,68 @@ int tb_conv1_u8_fwd(const uint8_t* frame, const float* weight, const float* bias
                     void* out_bf16, void* image_bf16, void* pack_scratch_bf16, void* stream);
 int tb_conv1_u8_wgrad(const void* dy_bf16, const void* image_bf16, int64_t N, int H, int W, int S, float* dweight,
                       float* partial, int64_t partial_floats, void* stream);
+/* Split-bf16 ("bf16x3") forms of the five entries above: each bf16 operand / output is a hi plane followed, *_lo elements
+ * further, by its lo plane bf16(x - hi), and every k-step issues lo.hi, hi.lo, hi.hi.  The weights are packed as a hi
+ * plane of O*KH*KW*C elements with the lo plane right behind it: pack_scratch_bf16 >= 2*O*KH*KW*C bf16 (conv1: 2*32*256).
+ * The input gradient's ReLU mask reads the hi plane of act_bf16.  conv1's pixels are exact in bf16, so its image has no
+ * lo plane.  Test and diagnostic entry points: the learner calls the same internals from C++.                           */
+int tb_conv_nhwc_bf16x3_fwd(const void* act_bf16, int64_t act_lo, const float* weight, const float* bias, int64_t Nf, int H,
+                            int W, int C, int KH, int KW, int S, int O, int relu, void* out_bf16, int64_t out_lo,
+                            void* pack_scratch_bf16, void* stream);
+int tb_conv_nhwc_bf16x3_dgrad(const void* dy_bf16, int64_t dy_lo, const float* weight, const void* act_bf16, int64_t Nf,
+                              int H, int W, int C, int KH, int KW, int S, int O, void* dx_bf16, int64_t dx_lo,
+                              void* pack_scratch_bf16, void* stream);
+int tb_conv_nhwc_bf16x3_wgrad(const void* dy_bf16, int64_t dy_lo, const void* act_bf16, int64_t act_lo, int64_t Nf, int H,
+                              int W, int C, int KH, int KW, int S, int O, float* dweight, float* partial,
+                              int64_t partial_floats, void* stream);
+int tb_conv1_u8_bf16x3_fwd(const uint8_t* frame, const float* weight, const float* bias, int64_t N, int H, int W, int S,
+                           int relu, void* out_bf16, int64_t out_lo, void* image_bf16, void* pack_scratch_bf16,
+                           void* stream);
+int tb_conv1_u8_bf16x3_wgrad(const void* dy_bf16, int64_t dy_lo, const void* image_bf16, int64_t N, int H, int W, int S,
+                             float* dweight, float* partial, int64_t partial_floats, void* stream);
+
+/* ---- IMPALA ResNet 3x3 convolutions on shifted-window split-bf16 kernels -----------------------------------------------
+ * The building blocks of the precision 2 ResNet trunk, for tests and diagnostics (the learner calls them from C++).
+ * Padded planar image of an Nf x H x W x C tensor (C a multiple of 8): one plane of bf16 elements laid out as
+ *   [Nf][C/8][(H+2)*(W+2)][8]   (frame, 8-channel chunk, zero-padded pixel in row-major order, channel in chunk),
+ * followed by slack (zeros) that a frame's last tile may read past the last plane; tb_sw_image_elems() elements per plane
+ * slack included.  The hi plane is at the base, the lo plane lo_off elements further (lo_off > 0, a multiple of 8).
+ * Producers write every element of both planes, borders and slack included.                                            */
+int64_t tb_sw_image_elems(int64_t Nf, int H, int W, int C);
+/* fp32 NHWC x [Nf,H,W,C] (through ReLU if relu_in) -> padded planar hi / lo image.  db != NULL: also db[C] = column sums
+ * of x (no ReLU), with scratch of tb_sw_colsum_scratch_floats() floats.                                                  */
+int tb_sw_pad_split_f32(const float* x, void* out, int64_t lo_off, int64_t Nf, int H, int W, int C, int relu_in, float* db,
+                        float* scratch, int64_t scratch_floats, void* stream);
+int64_t tb_sw_colsum_scratch_floats(int64_t Nf, int H, int W, int C);
+/* uint8 NCHW frames [Nf, 1 <= Cf <= 16, H, W] -> 16-channel padded planar image (channels >= Cf and the lo plane zero) */
+int tb_sw_frames_u8(const uint8_t* frame, void* out, int64_t lo_off, int64_t Nf, int Cf, int H, int W, void* stream);
+/* weights fp32 [O,C,3,3] -> the packed hi / lo operand (tb_sw_weight_elems(O, C) bf16) of tb_sw_conv_fwd with CK = C,
+ * NO = O (transpose = 0), or of the input-gradient convolution with CK = O, NO = C and flipped taps (transpose = 1).
+ * c_real > 0 (forward only): the weights are [O,c_real,3,3] and input channels >= c_real get zeros.                    */
+int64_t tb_sw_weight_elems(int O, int C);
+int tb_sw_pack_weights(const float* weight, void* out, int O, int C, int transpose, int c_real, void* stream);
+/* out fp32 [Nf*H*W, NO] = 3x3 / stride 1 / pad 1 convolution of a CK-channel image (CK, NO in {16, 32, 64}), then the
+ * epilogue in this order: * scale, + bias[NO], zeroed where mask [Nf*H*W, NO] is not positive, + addend [Nf*H*W, NO]
+ * (each nullable).  emit != NULL: the result (through ReLU if emit_relu) is also written as the complete padded planar
+ * image of NO channels (lo plane at emit_lo).  csum != NULL: per (tile, warp) column sums of the result,
+ * [tb_sw_csum_rows(Nf, H, W)][NO] floats plus 128*NO floats of scratch behind them for tb_sw_csum_reduce, which folds
+ * them into db[C] in a fixed order.                                                                                      */
+int tb_sw_conv_fwd(const void* img, int64_t img_lo, const void* wk, float* out, int64_t Nf, int H, int W, int CK, int NO,
+                   float scale, const float* bias, const float* mask, const float* addend, void* emit, int64_t emit_lo,
+                   int emit_relu, float* csum, void* stream);
+int64_t tb_sw_csum_rows(int64_t Nf, int H, int W);
+int tb_sw_csum_reduce(float* csum, int64_t rows, int C, float* db, void* stream);
+/* dweight fp32 [O, c_real or C, 3, 3] = scale * sum over pixels of dY (x) input windows, from the dY image (O channels)
+ * and the input image (C channels); W >= 5; partial >= 132*O*9*C floats.                                              */
+int tb_sw_conv_wgrad(const void* dyimg, int64_t dy_lo, const void* ximg, int64_t x_lo, float* dweight, int64_t Nf, int H,
+                     int W, int C, int O, float scale, int c_real, float* partial, int64_t partial_floats, void* stream);
+/* nn.MaxPool2d(3, 2, 1) backward into an image: dy_pooled fp32 [Nf,OH,OW,C] and the argmax taps of
+ * tb_maxpool3x3s2_fwd_f32 -> padded planar image of dL/d(pool input) [Nf,H,W,C] and db[C] = its column sums.          */
+int tb_sw_pool_bwd_image_colsum(const uint8_t* argmax, const float* dy_pooled, void* out, int64_t lo_off, int64_t Nf, int H,
+                                int W, int C, float* db, float* scratch, int64_t scratch_floats, void* stream);
+/* nn.MaxPool2d(3, 2, 1) forward on fp32 NHWC [N,H,W,C] -> y [N,OH,OW,C] and argmax u8 [N,OH,OW,C]: the tap kh*3 + kw
+ * (0..8) of each window's first maximum in row-major tap order.                                                       */
+int tb_maxpool3x3s2_fwd_f32(const float* x, float* y, uint8_t* argmax, int64_t N, int H, int W, int C, void* stream);
 /* out_bf16[r, c] = bf16(in[r*ld + c]) for c < cols, 0 for cols <= c < ld16 (operand staging). */
 int tb_f32_to_bf16(const float* in, void* out_bf16, int64_t rows, int64_t cols, int64_t ld, int64_t ld16,
                    void* stream);

@@ -73,6 +73,24 @@ _SIGNATURES = {
     "tb_conv_nhwc_bf16_wgrad": ([_vp, _vp, _i64] + [_int] * 7 + [_vp, _vp, _i64, _vp], _int),
     "tb_conv1_u8_fwd": ([_vp, _vp, _vp, _i64, _int, _int, _int, _int, _vp, _vp, _vp, _vp], _int),
     "tb_conv1_u8_wgrad": ([_vp, _vp, _i64, _int, _int, _int, _vp, _vp, _i64, _vp], _int),
+    "tb_conv_nhwc_bf16x3_fwd": ([_vp, _i64, _vp, _vp, _i64] + [_int] * 8 + [_vp, _i64, _vp, _vp], _int),
+    "tb_conv_nhwc_bf16x3_dgrad": ([_vp, _i64, _vp, _vp, _i64] + [_int] * 7 + [_vp, _i64, _vp, _vp], _int),
+    "tb_conv_nhwc_bf16x3_wgrad": ([_vp, _i64, _vp, _i64, _i64] + [_int] * 7 + [_vp, _vp, _i64, _vp], _int),
+    "tb_conv1_u8_bf16x3_fwd": ([_vp, _vp, _vp, _i64, _int, _int, _int, _int, _vp, _i64, _vp, _vp, _vp], _int),
+    "tb_conv1_u8_bf16x3_wgrad": ([_vp, _i64, _vp, _i64, _int, _int, _int, _vp, _vp, _i64, _vp], _int),
+    "tb_sw_image_elems": ([_i64, _int, _int, _int], _i64),
+    "tb_sw_pad_split_f32": ([_vp, _vp, _i64, _i64, _int, _int, _int, _int, _vp, _vp, _i64, _vp], _int),
+    "tb_sw_colsum_scratch_floats": ([_i64, _int, _int, _int], _i64),
+    "tb_sw_frames_u8": ([_vp, _vp, _i64, _i64, _int, _int, _int, _vp], _int),
+    "tb_sw_weight_elems": ([_int, _int], _i64),
+    "tb_sw_pack_weights": ([_vp, _vp, _int, _int, _int, _int, _vp], _int),
+    "tb_sw_conv_fwd": ([_vp, _i64, _vp, _vp, _i64, _int, _int, _int, _int, _f32, _vp, _vp, _vp, _vp, _i64, _int, _vp, _vp],
+                       _int),
+    "tb_sw_csum_rows": ([_i64, _int, _int], _i64),
+    "tb_sw_csum_reduce": ([_vp, _i64, _int, _vp, _vp], _int),
+    "tb_sw_conv_wgrad": ([_vp, _i64, _vp, _i64, _vp, _i64, _int, _int, _int, _int, _f32, _int, _vp, _i64, _vp], _int),
+    "tb_sw_pool_bwd_image_colsum": ([_vp, _vp, _vp, _i64, _i64, _int, _int, _int, _vp, _vp, _i64, _vp], _int),
+    "tb_maxpool3x3s2_fwd_f32": ([_vp, _vp, _vp, _i64, _int, _int, _int, _vp], _int),
     "tb_f32_to_bf16": ([_vp, _vp, _i64, _i64, _i64, _i64, _vp], _int),
     "tb_atarinet_param_count": ([_int, _int], _i64),
     "tb_atarinet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),

@@ -243,9 +243,11 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_kernel(SwFwdArgs a)
             put(q, c, ph, pl);
           }
         }
-        if (t == 0 && rl < a.g.Wp + 1) {
+        // pixels [0, Wp + 1): the top border and the first left border - 129 of them at W = 126, one more than a tile
+        // has rows
+        for (int u = rl; t == 0 && u < a.g.Wp + 1; u += kTile) {
 #pragma unroll
-          for (int c = 0; c < NO / 8; ++c) put(rl, c, z, z);
+          for (int c = 0; c < NO / 8; ++c) put(u, c, z, z);
         }
         if (t == a.g.tpf - 1) {
           const int q2 = a.g.tpf * kTile + a.g.Wp + 1 + rl;
@@ -489,9 +491,9 @@ __global__ void __launch_bounds__(kSwThreads, 1) sw_conv_fwd_wide_kernel(SwFwdAr
             put(q, c, ph, pl);
           }
         }
-        if (t == 0 && rl < a.g.Wp + 1) {
+        for (int u = rl; t == 0 && u < a.g.Wp + 1; u += kTile) {   // as in sw_conv_fwd_kernel
 #pragma unroll
-          for (int c = 0; c < NT / 8; ++c) put(rl, c, z, z);
+          for (int c = 0; c < NT / 8; ++c) put(u, c, z, z);
         }
         if (t == a.g.tpf - 1) {
           const int q2 = a.g.tpf * kTile + a.g.Wp + 1 + rl;
