@@ -268,6 +268,46 @@ int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, 
 int tb_sample_actions_dev_f32(const float* logits, int64_t T, int64_t B, int64_t A, const uint64_t* seed_step,
                               const int64_t* stream_ids, int64_t* actions, void* stream);
 
+/* ---- experience replay: a device ring of earlier batch columns mixed into the learner batch --------------------------
+ * A replay buffer is a device ring of `capacity` batch columns.  A stored column holds every learner leaf of one rollout
+ * column (frame, stacked [T+1,...] or unstacked [T+4,...]; reward, done, policy_logits, action, and last_action,
+ * episode_return and task when present) and, for a net with an LSTM, its initial agent state (h, c: [layers, H] each).
+ * Each of these is one leaf of the table below: the fresh batch holds it as [outer, Bf, row], the ring as
+ * [capacity, outer, row] (one slot's rows contiguous), the mixed batch as [outer, Bf+R, row]; the agent state has
+ * outer = layers.  Device state: head_size = (head: the next slot to write, size: the number of valid slots) and
+ * seed_step = (seed, step); slot (head - 1 - k) mod capacity is the k-th newest column.
+ *
+ * One tb_replay_mix call with Bf fresh columns and R replayed columns, read against the device state when it runs:
+ *   1. n = min(size, capacity - Bf) survivors: the newest columns this call's insert leaves in place.  Replayed column
+ *      j in [0,R) takes x = word 0 of Philox4x32-10 with counter (lo32(step), hi32(step), j, stream_id) and key
+ *      (lo32(seed), hi32(seed)), k = (uint64(x) * n) >> 32, slot = (head - 1 - k) mod capacity.  Draws are with
+ *      replacement, and no slot drawn is one of the Bf slots this call writes, so the gather and the insert never race.
+ *      The caller guarantees n >= 1 when R > 0 (with n = 0 every draw names slot head - 1, whose contents are undefined).
+ *   2. out columns [0,Bf) = the fresh columns; columns [Bf,Bf+R) = the drawn slots, for every leaf whose out != NULL.
+ *   3. the fresh columns are written to slots head, head+1, ... (mod capacity).
+ *   4. slots_out[j] (int64 [R], nullable) = the slot of replayed column j.
+ * tb_replay_advance, the next launch on the stream, then sets head = (head + Bf) mod capacity,
+ * size = min(size + Bf, capacity), step = step + 1.  R = 0 inserts only.  Both read their state from device memory when
+ * they run, so a launch pair captured in a CUDA graph draws new slots on every replay.  Copies are exact byte copies.
+ * Sizes: 1 <= num_leaves <= TB_REPLAY_MAX_LEAVES, 0 <= R <= TB_REPLAY_MAX_R, Bf >= 1, capacity > Bf,
+ * 0 <= stream_id < 2^32, outer >= 1 and row_bytes >= 1 per leaf; fresh and ring must not be NULL.
+ * Algorithmic bytes of one call: sum over leaves of outer * row_bytes * (3*Bf + 2*R).                              */
+#define TB_REPLAY_MAX_LEAVES 16
+#define TB_REPLAY_MAX_R 4096
+typedef struct tb_replay_leaf {
+  const void* fresh; /* [outer, Bf, row_bytes] */
+  void* out;         /* [outer, Bf+R, row_bytes], or NULL: this leaf is inserted only */
+  void* ring;        /* [capacity, outer, row_bytes] */
+  int64_t outer;
+  int64_t row_bytes;
+} tb_replay_leaf;
+/* leaves_host: a host array of num_leaves entries, read before the call returns (the kernel gets it by value). */
+int tb_replay_mix(const tb_replay_leaf* leaves_host, int num_leaves, int64_t Bf, int64_t R, int64_t capacity,
+                  const uint64_t* seed_step, const int64_t* head_size, int64_t stream_id, int64_t* slots_out,
+                  void* stream);
+/* One-thread launch: the state advance of one tb_replay_mix call with Bf fresh columns. */
+int tb_replay_advance(int64_t* head_size, uint64_t* seed_step, int64_t Bf, int64_t capacity, void* stream);
+
 /* ---- the three loss functions on their own (API mirror; tests pass float64) ---------- */
 
 /* monobeast.py:107-108 compute_baseline_loss: out[0] = 0.5*sum(adv^2); grad (nullable) = adv. */

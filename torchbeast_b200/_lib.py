@@ -58,6 +58,8 @@ _SIGNATURES = {
     "tb_resnet_backward_arch": ([_vp] * 5 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
+    "tb_replay_mix": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp], _int),
+    "tb_replay_advance": ([_vp, _vp, _i64, _i64, _vp], _int),
     "tb_baseline_loss_f32": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f64": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_entropy_loss_f32": ([_vp, _i64, _i64, _vp, _vp, _vp, _vp], _int),

@@ -15,24 +15,6 @@
 
 namespace tb {
 
-// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011); only word 0 is used.
-__device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                                     uint32_t k1) {
-  constexpr uint32_t kM0 = 0xD2511F53u, kM1 = 0xCD9E8D57u, kW0 = 0x9E3779B9u, kW1 = 0xBB67AE85u;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(kM0, c0), lo0 = kM0 * c0;
-    const uint32_t hi1 = __umulhi(kM1, c2), lo1 = kM1 * c2;
-    c0 = hi1 ^ c1 ^ k0;
-    c1 = lo1;
-    c2 = hi0 ^ c3 ^ k1;
-    c3 = lo0;
-    k0 += kW0;
-    k1 += kW1;
-  }
-  return c0;
-}
-
 // kSeedStepOnDevice: seed and step are read from seed_step[0..1] when the kernel runs instead of the by-value
 // arguments, so a launch captured in a CUDA graph picks up whatever (seed, step) was written there before each replay.
 template <bool kSeedStepOnDevice>

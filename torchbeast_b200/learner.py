@@ -328,7 +328,8 @@ def _popart_stats(mu, nu):
 
 
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
-               behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None):
+               behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None,
+               fresh_columns=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -341,6 +342,9 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     launch for the per-task sums), SUM all-reduces the sums when data-parallel, and after the optimizer step updates the
     statistics and rescales the value head (popart_update) before the actor copy.  beta is `popart_beta_dev` (a float64
     device scalar, GraphedLearner's) or flags.popart_beta.
+
+    `fresh_columns` (a replay-mixed batch, see torchbeast_b200.replay): the stats' episode returns come from columns
+    [0, fresh_columns) only, so a replayed episode end is not counted twice; the losses cover the whole batch.
     """
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
@@ -380,8 +384,10 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             actor_model.load_state_dict(model.state_dict())
     if not stats_sync:
         return dict(losses=loss.losses, vtrace=loss)
-    done = batch["done"][1:]
-    episode_returns = batch["episode_return"][1:][done.bool()]
+    done, ep_ret = batch["done"][1:], batch["episode_return"][1:]
+    if fresh_columns is not None:
+        done, ep_ret = done[:, :fresh_columns], ep_ret[:, :fresh_columns]
+    episode_returns = ep_ret[done.bool()]
     host = loss.losses.cpu()  # the step's one blocking read-back
     ep = episode_returns.cpu()
     stats = {
@@ -421,6 +427,9 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       overlaps the other thread's step), then consumed under the lock.
     * with flags.cuda_graph (or TB_CUDA_GRAPH=1) the device side is ONE CUDA-graph replay (GraphedLearner, created on first
       use per batch shape); otherwise the eager launch sequence of learn_step.
+    * with a replay buffer attached as `model.replay` (torchbeast_b200.replay.ReplayBuffer), the staged batch and state
+      are mixed with replayed columns under the lock, inside the graph when graphed; the warm-up phase and the mixing
+      phase are two graphs, as their batch widths differ.
     Returns the reference's stats dict."""
     import contextlib
     from torchbeast_b200 import staging
@@ -453,6 +462,9 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
                 graphs = model.__dict__.setdefault("_tb_graphs", {})
                 gkey = (tuple((k, tuple(v.shape)) for k, v in batch.items() if k in GraphedLearner.KEYS), id(optimizer),
                         id(actor_model))
+                replay = getattr(model, "replay", None)
+                if replay is not None:
+                    gkey += (id(replay), replay.mixing(replay.prepare(batch, initial_agent_state)))
                 gl = graphs.get(gkey)
                 if gl is None or gl.structure != structure:
                     # a value that chooses a kernel or a buffer changed, so the eager step would switch too: replay the
@@ -473,7 +485,11 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
                 snap_event = torch.cuda.Event()
                 snap_event.record()
             else:
-                return learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler)
+                fresh = None
+                if getattr(model, "replay", None) is not None:
+                    batch, initial_agent_state, fresh = model.replay.mix(batch, initial_agent_state)
+                return learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
+                                  fresh_columns=fresh)
         finally:
             if stager is not None and slot is not None:
                 stager.release(slot)
@@ -553,6 +569,15 @@ class GraphedLearner:
             d.copy_(s)
         optimizer.lr_from_device = True
         optimizer.sync_lr_to_device()
+        # a replay buffer (model.replay): the mix runs inside the graph on the static fresh inputs, in the phase the buffer
+        # is in now; learn() keeps one graph per phase
+        self.replay = getattr(model, "replay", None)
+        self.mixing = False
+        replay_saved = None
+        if self.replay is not None:
+            self.fresh_columns = self.replay.prepare(self.static, self.static_state)
+            self.mixing = self.replay.mixing(self.fresh_columns)
+            replay_saved = self.replay.save(3)  # the two warm-up steps and the upload replay below each insert once
         # warm up on a side stream (allocations, one-time attribute calls), then capture
         snapshot = (model.flat_params.clone(), optimizer.snapshot(),
                     None if self.popart is None else (self.popart.mu.clone(), self.popart.nu.clone()))
@@ -560,14 +585,12 @@ class GraphedLearner:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for _ in range(2):
-                learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None, stats_sync=False,
-                           hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
+                self._learn_step()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.out = learn_step(flags, model, actor_model, self.static, self.static_state, optimizer, None,
-                                  stats_sync=False, hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
+            self.out = self._learn_step()
         # the graph writes into the model workspace it was captured with; the model replaces (and frees) that buffer when
         # it runs another shape, e.g. while the GraphedLearner of another batch shape is captured: keep it alive here
         self.workspace = getattr(model, "_ws", None)
@@ -584,6 +607,16 @@ class GraphedLearner:
             self.popart.nu.copy_(snapshot[2][1])
         if actor_model is not None and hasattr(actor_model, "copy_params_from"):
             actor_model.copy_params_from(model)
+        if replay_saved is not None:
+            self.replay.restore(replay_saved)  # ring slots, head, size, seed and step as the caller left them
+
+    def _learn_step(self):
+        """The captured launch sequence: [replay mix + advance], then learn_step without a host read."""
+        batch, state = self.static, self.static_state
+        if self.replay is not None:
+            batch, state = self.replay.launch(batch, state, self.mixing)
+        return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
+                          hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
 
     def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
         """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
@@ -596,7 +629,11 @@ class GraphedLearner:
         publish_hparams(pack_hparams(self.flags, self.opt) if hparams is None else hparams, self.hparams)
         if self.popart is not None:
             self._publish_beta(self.flags)
+        if self.replay is not None:
+            self.replay.prepare(self.static, self.static_state)  # publishes seed / step if the host changed them
         self.graph.replay()
+        if self.replay is not None:
+            self.replay.advance_host(self.fresh_columns)
         if scheduler is not None:
             scheduler.step()
         return self.out
