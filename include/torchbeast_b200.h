@@ -126,6 +126,20 @@ int tb_impala_loss_fwd_bwd_hp_f32(const float* behavior_logits, const float* tar
                                   float* grad_logits, float* grad_values, int zero_tail, void* workspace,
                                   void* stream);
 
+/* tb_impala_loss_fwd_bwd_f32 with importance weights: column_weights [B] f32 (device, not NULL).  The pg, baseline and
+ * entropy terms of every row (t, b) are multiplied by column_weights[b], in losses_out and in grad_logits / grad_values
+ * (after the unweighted term is formed, so weights of 1.0f give the bits of tb_impala_loss_fwd_bwd_f32 / _hp_f32; a
+ * weight of 0 gives zero gradient rows).  vs, pg_adv, log_rhos and the log-probabilities are not weighted.
+ * hp: NULL takes the scalar arguments, else they are read from hp when the kernel runs.                            */
+int tb_impala_loss_weighted_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                                const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                                const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                                float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
+                                float clip_pg_rho, const float* column_weights, const tb_hparams* hp, float* vs,
+                                float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
+                                float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
+                                void* workspace, void* stream);
+
 /* ---- PopArt value normalisation (van Hasselt et al. 2016; Hessel et al. 2019) -----------
  * Per task k, statistics mu[k], nu[k] (f64, device; start at 0 and 1) with
  *   sigma_k = clamp(sqrt(max(nu_k - mu_k^2, 0)), 1e-4, 1e6).
@@ -307,6 +321,46 @@ int tb_replay_mix(const tb_replay_leaf* leaves_host, int num_leaves, int64_t Bf,
                   void* stream);
 /* One-thread launch: the state advance of one tb_replay_mix call with Bf fresh columns. */
 int tb_replay_advance(int64_t* head_size, uint64_t* seed_step, int64_t Bf, int64_t capacity, void* stream);
+/* tb_replay_mix with the R replayed slots read from slots (int64 [R], device) instead of drawn: steps 2 and 3 above,
+ * with slot j = slots[j]; seed_step is not read.  The caller guarantees every slot is a survivor (tb_replay_sample_
+ * prioritized writes such slots).  Same sizes and validation as tb_replay_mix; stream id 0.                          */
+int tb_replay_mix_slots(const tb_replay_leaf* leaves_host, int num_leaves, int64_t Bf, int64_t R, int64_t capacity,
+                        const int64_t* slots, const int64_t* head_size, void* stream);
+
+/* ---- prioritised replay (Schaul et al. 2016; sequence priorities as in R2D2, Kapturowski et al. 2019) -----------------
+ * A prioritised buffer adds, on the device: priorities f32 [capacity], one value per slot (>= 0; never-written slots
+ * are never drawn), and prio f64 [4] = {alpha, beta, eta, eps} (alpha >= 0, 0 <= beta <= 1, 0 <= eta <= 1, eps > 0),
+ * read when the kernels run, so a captured graph follows the values published between replays.
+ *
+ * tb_replay_sample_prioritized, before tb_replay_mix_slots and tb_replay_advance, reads head_size, seed_step, prio and
+ * priorities and writes batch_slots (int64 [Bf+R]) and column_weights (f32 [Bf+R]):
+ *   Fresh column c: batch_slots[c] = (head + c) mod capacity, column_weights[c] = 1.  R = 0 writes these only.
+ *   Survivors as for tb_replay_mix: n = min(size, capacity - Bf), survivor k is slot (head - 1 - k) mod capacity; the
+ *   caller guarantees n >= 1 when R > 0.  q_k = pow((double)priorities[slot_k] + eps, alpha) in double.
+ *   Summation order (every + below a double add, rounded to nearest):
+ *     L = ceil(n / 1024); chunk i in [0, 1024) holds k in [i*L, min(i*L + L, n)) (possibly empty).
+ *     r_k = the running sum of q over chunk i up to k, in k order, from 0; T_i = its total (0 if empty).
+ *     Warp g in [0, 32) holds chunks 32g .. 32g+31.  P_i = the sum of T over the chunks of i's warp before i, in
+ *     order, from 0; G_g = the sum of all 32 T of warp g, in order, from 0; B_g = G_0 + ... + G_{g-1}, in order, from 0.
+ *     C_k = B_g + (P_i + r_k) for k in chunk i of warp g;  S = C_{n-1}.  C is non-decreasing.
+ *   Replayed column j in [0, R): (w0, w1) = words 0 and 1 of Philox4x32-10 with the counter and key of tb_replay_mix
+ *   (counter (lo32(step), hi32(step), j, stream_id), key (lo32(seed), hi32(seed))); u = ((w1 << 32 | w0) >> 11) * 2^-53;
+ *   k_j = the smallest k with C_k > u * S (the product rounded to double), or n - 1 if there is none.
+ *   batch_slots[Bf + j] = slot_{k_j}; column_weights[Bf + j] = (float)pow(q_min / q_{k_j}, beta) with q_min the
+ *   minimum of q over the survivors: (n P)^-beta normalised by its largest value over the buffer, in (0, 1].
+ *   Draws are with replacement and never name a slot the call overwrites.  One CTA; no atomics, so the results are
+ *   bit-identical from run to run.  Host validation as tb_replay_mix (null pointers, R, Bf, capacity, stream_id).
+ *
+ * tb_replay_update_priorities, after the loss, on the batch the loss used (vs, values [T, B] f32, B = Bf + R):
+ *   e_t = |(double)vs[t,c] - (double)values[t,c]|; p_c = eta * max_t e_t + (1 - eta) * (sum_t e_t / T), the sum in t
+ *   order, every operation rounded to double (no fused multiply-add); stored as (float)p_c, or 0 if that is not finite.
+ *   Column c writes priorities[batch_slots[c]] unless a later column c' > c names the same slot: of a slot drawn
+ *   more than once, the largest j wins.  Slots not in batch_slots are untouched.  One launch, deterministic.        */
+int tb_replay_sample_prioritized(const float* priorities, const double* prio, const int64_t* head_size,
+                                 const uint64_t* seed_step, int64_t Bf, int64_t R, int64_t capacity, int64_t stream_id,
+                                 int64_t* batch_slots, float* column_weights, void* stream);
+int tb_replay_update_priorities(const float* vs, const float* values, int64_t T, int64_t B, const int64_t* batch_slots,
+                                const double* prio, float* priorities, void* stream);
 
 /* ---- the three loss functions on their own (API mirror; tests pass float64) ---------- */
 

@@ -33,6 +33,8 @@ _SIGNATURES = {
     "tb_impala_loss_fwd_bwd_hp_f32": ([_vp] * 8 + [_i64, _i64, _i64] + [_vp] * 9 + [_int, _vp, _vp], _int),
     "tb_impala_loss_popart_f32": (
         [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 12, _int),
+    "tb_impala_loss_weighted_f32": (
+        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 10 + [_int, _vp, _vp], _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
     "tb_atarinet_param_count_mt": ([_int, _int, _int], _i64),
     "tb_atarinet_forward_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
@@ -60,6 +62,9 @@ _SIGNATURES = {
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_replay_mix": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp], _int),
     "tb_replay_advance": ([_vp, _vp, _i64, _i64, _vp], _int),
+    "tb_replay_mix_slots": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _vp], _int),
+    "tb_replay_sample_prioritized": ([_vp] * 4 + [_i64, _i64, _i64, _i64, _vp, _vp, _vp], _int),
+    "tb_replay_update_priorities": ([_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f32": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_baseline_loss_f64": ([_vp, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_entropy_loss_f32": ([_vp, _i64, _i64, _vp, _vp, _vp, _vp], _int),

@@ -56,10 +56,11 @@ template <> struct M<double> {
   static __device__ __forceinline__ double max(double a, double b) { return fmax(a, b); }
 };
 
-// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011); only word 0 is used.
-// Shared by the action sampler (sample.cu) and the replay slot draws (replay.cu).
-__device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                                     uint32_t k1) {
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): words 0 and 1 of the output.
+// Shared by the action sampler (sample.cu) and the replay slot draws (replay.cu); the uniform draws use word 0 only,
+// the prioritised draws both.
+__device__ __forceinline__ uint2 philox4x32_10_w01(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
+                                                   uint32_t k1) {
   constexpr uint32_t kM0 = 0xD2511F53u, kM1 = 0xCD9E8D57u, kW0 = 0x9E3779B9u, kW1 = 0xBB67AE85u;
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -72,7 +73,11 @@ __device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, u
     k0 += kW0;
     k1 += kW1;
   }
-  return c0;
+  return make_uint2(c0, c1);
+}
+__device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
+                                                     uint32_t k1) {
+  return philox4x32_10_w01(c0, c1, c2, c3, k0, k1).x;
 }
 
 __device__ __forceinline__ double warp_sum(double v) {

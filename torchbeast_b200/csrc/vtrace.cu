@@ -435,6 +435,9 @@ struct LossArgs {
   // PopArt (impala_loss_kernel<A, true> only): `values` holds the normalised value head [T+1,B,K] (bootstrap row
   // included, `bootstrap` unused), row (t,b) uses task[t*B+b]; grad_values is [T+1,B,K]
   const int64_t* task; const double* pa_mu; const double* pa_nu; int K;
+  // importance weights (impala_loss_kernel<A, false, true> only): column b's pg, baseline and entropy terms, in the
+  // losses and the gradients, are multiplied by column_weights[b]
+  const float* column_weights;
 };
 
 constexpr int kPopArtMaxTasks = 64;
@@ -463,8 +466,10 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 }
 
 // kPopArt: the value input is PopArt-normalised (LossArgs::task / pa_mu / pa_nu / K); the non-PopArt instantiations
-// compile none of that code.
-template <int A, bool kPopArt = false>
+// compile none of that code.  kWeighted: every term of column b is multiplied by LossArgs::column_weights[b], after the
+// unweighted term is formed, so a weight of 1.0f gives the unweighted bits; the other instantiations compile no weight
+// code.
+template <int A, bool kPopArt = false, bool kWeighted = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
   if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -588,8 +593,14 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
       } else {
         d = vst - v;
       }
-      s_pg += double(-tlp * adv);
-      s_bl += 0.5 * double(d * d);
+      if constexpr (kWeighted) {
+        const double wd = double(__ldg(p.column_weights + b));  // column b's weight, read where it is used (L1)
+        s_pg += double(-tlp * adv) * wd;
+        s_bl += 0.5 * double(d * d) * wd;
+      } else {
+        s_pg += double(-tlp * adv);
+        s_bl += 0.5 * double(d * d);
+      }
       float ent_row = 0.0f;
       if constexpr (A != 0) {
         float lp[A], pr[A];
@@ -601,8 +612,10 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         }
         if (p.grad_logits) {
 #pragma unroll
-          for (int j = 0; j < A; ++j)
-            p.grad_logits[i * A + j] = adv * (pr[j] - (act == j ? 1.0f : 0.0f)) + p.entropy_cost * pr[j] * (lp[j] - ent_row);
+          for (int j = 0; j < A; ++j) {
+            const float gl = adv * (pr[j] - (act == j ? 1.0f : 0.0f)) + p.entropy_cost * pr[j] * (lp[j] - ent_row);
+            if constexpr (kWeighted) p.grad_logits[i * A + j] = gl * __ldg(p.column_weights + b); else p.grad_logits[i * A + j] = gl;
+          }
         }
       } else {
         for (int64_t j = 0; j < Ause; ++j) {
@@ -612,15 +625,18 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         if (p.grad_logits) {
           for (int64_t j = 0; j < Ause; ++j) {
             const float lp = (trow[j] - m) - logs, pr = expf(lp);
-            p.grad_logits[i * Ause + j] = adv * (pr - (act == j ? 1.0f : 0.0f)) + p.entropy_cost * pr * (lp - ent_row);
+            const float gl = adv * (pr - (act == j ? 1.0f : 0.0f)) + p.entropy_cost * pr * (lp - ent_row);
+            if constexpr (kWeighted) p.grad_logits[i * Ause + j] = gl * __ldg(p.column_weights + b); else p.grad_logits[i * Ause + j] = gl;
           }
         }
       }
-      s_en += double(ent_row);
+      if constexpr (kWeighted) s_en += double(ent_row) * double(__ldg(p.column_weights + b)); else s_en += double(ent_row);
       if (p.grad_values) {
         if constexpr (kPopArt) {
           const int64_t k = p.task[i];
           for (int j = 0; j < p.K; ++j) p.grad_values[i * p.K + j] = (j == k) ? -p.baseline_cost * d : 0.0f;
+        } else if constexpr (kWeighted) {
+          p.grad_values[i] = (-p.baseline_cost * d) * __ldg(p.column_weights + b);
         } else {
           p.grad_values[i] = -p.baseline_cost * d;
         }
@@ -760,7 +776,8 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
                               float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
                               float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream,
                               const int64_t* task = nullptr, const double* pa_mu = nullptr,
-                              const double* pa_nu = nullptr, int K = 0, double* task_sums = nullptr) {
+                              const double* pa_nu = nullptr, int K = 0, double* task_sums = nullptr,
+                              const float* column_weights = nullptr) {
   TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
              (long long)B, (long long)A);
   TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
@@ -787,6 +804,7 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   p.workspace = workspace;
   p.hp = hp;
   p.task = task; p.pa_mu = pa_mu; p.pa_nu = pa_nu; p.K = K;
+  p.column_weights = column_weights;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
   int W = pick_warps(T, tiles);
   p.wide = (W == 1);
@@ -806,6 +824,11 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
     TB_TRY(check_launch("impala_loss_kernel<popart>"));
     popart_task_sums_kernel<<<K, kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, K, task_sums);
     return check_launch("popart_task_sums_kernel");
+  }
+  if (column_weights) {
+    ProfScope prof("impala_loss_weighted", (cudaStream_t)stream);
+    TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+    return check_launch("impala_loss_kernel<weighted>");
   }
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
   TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
@@ -881,6 +904,21 @@ int tb_impala_loss_popart_f32(const float* blogits, const float* tlogits, const 
                             baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs, pg_adv, log_rhos,
                             behavior_alp, target_alp, losses_out, grad_logits, grad_values, 1, workspace, stream, task,
                             mu, nu, int(K), task_sums);
+}
+
+int tb_impala_loss_weighted_f32(const float* blogits, const float* tlogits, const int64_t* actions,
+                                const float* rewards, const uint8_t* done, const float* discounts,
+                                const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
+                                float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
+                                float clip_rho, float clip_pg_rho, const float* column_weights, const tb_hparams* hp,
+                                float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
+                                float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
+                                void* workspace, void* stream) {
+  TB_REQUIRE(column_weights, "impala_loss_weighted: null column_weights");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
+                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs,
+                            pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
+                            zero_tail, workspace, stream, nullptr, nullptr, nullptr, 0, nullptr, column_weights);
 }
 
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,

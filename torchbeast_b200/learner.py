@@ -77,6 +77,7 @@ def impala_loss_fwd_bwd(
     clip_pg_rho_threshold=1.0,
     with_grads=True,
     hparams_dev=None,
+    column_weights=None,
 ):
     """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_fwd_bwd_f32).
 
@@ -89,9 +90,18 @@ def impala_loss_fwd_bwd(
     With `hparams_dev` (a device tb_hparams block, see pack_hparams / publish_hparams) the kernel reads discounting,
     the costs, the reward clip and the two V-trace clips from the block when it runs, and the corresponding arguments
     are not used: a captured CUDA graph then follows what is published between replays.
+
+    With `column_weights` (float32 [B], device) the pg, baseline and entropy terms of column b, in the losses and the
+    gradients, are multiplied by column_weights[b] (tb_impala_loss_weighted_f32, prioritised replay's importance
+    weights); weights of 1.0 give the unweighted bits.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
+    if column_weights is not None:
+        _lib.require_cuda(column_weights)
+        if column_weights.dtype != torch.float32 or column_weights.numel() != target_policy_logits.shape[1]:
+            raise _lib.TorchBeastB200Error("column_weights must be float32 [%d], got %s %r" % (
+                target_policy_logits.shape[1], column_weights.dtype, tuple(column_weights.shape)))
     if hparams_dev is None:
         clip_rewards = _clip_rewards(reward_clipping)
     else:
@@ -118,6 +128,17 @@ def impala_loss_fwd_bwd(
     losses = torch.empty(4, dtype=f32, device=dev)
     gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
     gv = torch.empty((T + 1, B), dtype=f32, device=dev) if with_grads else None
+    if column_weights is not None:
+        p = _lib.ptr
+        _lib.check(
+            _lib.lib().tb_impala_loss_weighted_f32(
+                p(bl), p(tl), p(ac), p(rw), p(dn), p(disc), p(va), p(bs), T, B, A,
+                0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
+                0 if hparams_dev is not None else clip_rewards, _lib.clip_arg(clip_rho_threshold),
+                _lib.clip_arg(clip_pg_rho_threshold), p(column_weights.contiguous()), p(hparams_dev),
+                *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(_lib.workspace()), _lib.stream_ptr()),
+            "tb_impala_loss_weighted_f32")
+        return ImpalaLoss(*outs, losses, gl, gv)
     if hparams_dev is not None:
         _lib.check(
             _lib.lib().tb_impala_loss_fwd_bwd_hp_f32(
@@ -327,9 +348,19 @@ def _popart_stats(mu, nu):
     return {"popart_mu": mu.tolist(), "popart_sigma": sigma}
 
 
+_POPART_PRIORITIZED = ("prioritised replay does not support PopArt (model.popart): weighted per-task statistics and "
+                       "normalised priorities are not defined; use a uniform ReplayBuffer (no priority_exponent)")
+
+
+def _check_replay(model):
+    replay = getattr(model, "replay", None)
+    if replay is not None and replay.prioritized and getattr(model, "popart", None) is not None:
+        raise _lib.TorchBeastB200Error(_POPART_PRIORITIZED)
+
+
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
                behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None,
-               fresh_columns=None):
+               fresh_columns=None, draw=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -345,18 +376,27 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
 
     `fresh_columns` (a replay-mixed batch, see torchbeast_b200.replay): the stats' episode returns come from columns
     [0, fresh_columns) only, so a replayed episode end is not counted twice; the losses cover the whole batch.
+
+    `draw` (a prioritised buffer's replay.Draw, or one built by hand): with `draw.weights` the loss is the importance-
+    weighted one (impala_loss_fwd_bwd with column_weights), so the stats' loss values are the weighted sums; with
+    `draw.buffer` its priorities are updated from the loss's vs and values at `draw.slots`, right after the loss.
     """
+    pop = getattr(model, "popart", None)
+    if draw is not None and pop is not None:
+        raise _lib.TorchBeastB200Error(_POPART_PRIORITIZED)
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
     acts = batch["action"] if actions is None else actions
-    pop = getattr(model, "popart", None)
     if pop is None:
         loss = impala_loss_fwd_bwd(
             blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
             out.baseline[:-1], out.baseline[-1],
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
-            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
+            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
+            column_weights=None if draw is None else draw.weights)
         grad_values = loss.grad_values
+        if draw is not None and draw.buffer is not None:
+            draw.buffer.update_priorities(loss.vs, out.baseline[:-1], draw.slots)
     else:
         values = out.baseline.reshape(out.baseline.shape[:2] + (pop.num_tasks,))
         loss, task_sums = impala_loss_popart(
@@ -429,7 +469,8 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       use per batch shape); otherwise the eager launch sequence of learn_step.
     * with a replay buffer attached as `model.replay` (torchbeast_b200.replay.ReplayBuffer), the staged batch and state
       are mixed with replayed columns under the lock, inside the graph when graphed; the warm-up phase and the mixing
-      phase are two graphs, as their batch widths differ.
+      phase are two graphs, as their batch widths differ.  A prioritised buffer adds its draw, the weighted loss and
+      the priority update to the same sequence (learn_step's `draw`); with PopArt it raises.
     Returns the reference's stats dict."""
     import contextlib
     from torchbeast_b200 import staging
@@ -455,6 +496,7 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
             # the polybeast nest has no separate last_action leaf: row t of `action` IS the action taken before frame t
             batch = dict(batch, last_action=batch["action"])
         try:
+            _check_replay(model)
             if _graph_enabled(flags):
                 _require_fused(optimizer)
                 hparams = pack_hparams(flags, optimizer)  # raises before anything is captured or replayed
@@ -485,11 +527,13 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
                 snap_event = torch.cuda.Event()
                 snap_event.record()
             else:
-                fresh = None
-                if getattr(model, "replay", None) is not None:
-                    batch, initial_agent_state, fresh = model.replay.mix(batch, initial_agent_state)
+                fresh = draw = None
+                replay = getattr(model, "replay", None)
+                if replay is not None:
+                    batch, initial_agent_state, fresh = replay.mix(batch, initial_agent_state)
+                    draw = replay.last_draw if replay.prioritized else None
                 return learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
-                                  fresh_columns=fresh)
+                                  fresh_columns=fresh, draw=draw)
         finally:
             if stager is not None and slot is not None:
                 stager.release(slot)
@@ -571,6 +615,7 @@ class GraphedLearner:
         optimizer.sync_lr_to_device()
         # a replay buffer (model.replay): the mix runs inside the graph on the static fresh inputs, in the phase the buffer
         # is in now; learn() keeps one graph per phase
+        _check_replay(model)
         self.replay = getattr(model, "replay", None)
         self.mixing = False
         replay_saved = None
@@ -613,10 +658,12 @@ class GraphedLearner:
     def _learn_step(self):
         """The captured launch sequence: [replay mix + advance], then learn_step without a host read."""
         batch, state = self.static, self.static_state
+        draw = None
         if self.replay is not None:
             batch, state = self.replay.launch(batch, state, self.mixing)
+            draw = self.replay.last_draw if self.replay.prioritized else None
         return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
-                          hparams_dev=self.hparams, popart_beta_dev=self.popart_beta)
+                          hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw)
 
     def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
         """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
