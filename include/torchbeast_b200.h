@@ -427,8 +427,10 @@ int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_basel
  * Replaces the reference's loop of seq_len-1 nn.LSTM calls and its autograd graph (monobeast.py:603-611,
  * polybeast_learner.py:241-249):   for t: state *= notdone_t;  y_t, state = LSTM(x_t, state).
  * torch.nn.LSTM conventions: params[4*l + {0,1,2,3}] = weight_ih_l [4H, In|H], weight_hh_l [4H, H], bias_ih_l [4H],
- * bias_hh_l [4H] (gate order i, f, g, o); any number of layers >= 1; hidden size, input size, batch and unroll are free
- * (BASELINE configs[4]: T = 600, B = 128, H = 512).  x [T1*B, In], notdone [T1*B] (float 0/1), h0/c0/hN/cN [layers, B, H],
+ * bias_hh_l [4H] (gate order i, f, g, o); any number of layers >= 1; input size, batch and unroll are free, hidden size is
+ * 1 .. TB_LSTM_MAX_HIDDEN (BASELINE configs[4]: T = 600, B = 128, H = 512).  Above that bound the backward's fp32 step kernel,
+ * which every precision falls back to, cannot hold a row of H in shared memory: every tb_lstm_* entry rejects such an H
+ * (tb_lstm_workspace_bytes returns 0).  x [T1*B, In], notdone [T1*B] (float 0/1), h0/c0/hN/cN [layers, B, H],
  * y [T1*B, H].  precision 0 = fp32 everywhere (any shape); 1 / 2 = bf16 / split-bf16 tensor-core products for the hoisted
  * projections, and in the recurrence where a tensor-core recurrence fits the shape (tb_lstm_plan).  tb_lstm_backward must
  * follow tb_lstm_forward on the same workspace; grads[] mirrors params[] and is overwritten; dx [T1*B, In].
@@ -436,6 +438,7 @@ int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_basel
  * odd), each planned as a stack of its own with input width In for the first segment and H above it, so every upper
  * pair can take a two-layer wavefront.  Every notdone step resets all layers.  Above two layers the workspace also holds
  * each segment's output but the top one's and two [T1*B, H] buffers for the gradient handed between segments.        */
+#define TB_LSTM_MAX_HIDDEN 700
 size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision);
 /* The recurrence kinds tb_lstm_forward (*fwd_kind_host) and tb_lstm_backward (*bwd_kind_host) run for this shape on the
  * current device; host query, runs no kernel.  The choice does not depend on the unroll length.  1 or 2 layers

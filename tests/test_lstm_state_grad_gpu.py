@@ -41,7 +41,7 @@ def problem(T1, B, In, H, layers, seed=1):
     nd[0, 0] = 0.0
     nd[0, 1:] = 1.0
     if T1 > 1:
-        nd[T1 - 1, 1] = 0.0
+        nd[T1 - 1, min(1, B - 1)] = 0.0   # column 0 when it is the only one
     return dict(x=d(rs.randn(T1, B, In) * 0.5), notdone=d(nd), h0=d(rs.randn(layers, B, H) * 0.1),
                 c0=d(rs.randn(layers, B, H) * 0.1), dy=d(rs.randn(T1, B, H) / T1 ** 0.5), dhN=d(rs.randn(layers, B, H)),
                 dcN=d(rs.randn(layers, B, H)))
@@ -99,9 +99,10 @@ def test_state_grads_vs_torch(T1, B, In, H, layers, precision, kind):
     assert torch.all(h0.grad[:, 1:].abs().sum(-1) > 0)
 
 
-def _abi_call(m, pb, ports):
+def _abi_call(m, pb, ports, fill=None):
     """tb_lstm_forward, then tb_lstm_backward (ports None) or tb_lstm_backward_state with the given ports; returns the
-    outputs and the number of kernel launches of the backward call."""
+    outputs ([dx] + parameter gradients + [y, hN, cN]) and the number of kernel launches of the backward call.  With
+    `fill` (a byte value) the workspace starts out filled with it instead of holding whatever torch.empty left."""
     from torchbeast_b200 import _lib
     from torchbeast_b200.lstm import PRECISIONS
     lib, p = _lib.lib(), _lib.ptr
@@ -111,6 +112,8 @@ def _abi_call(m, pb, ports):
     arr = lambda ts: ctypes.cast(m._ptr_array(ts), ctypes.c_void_p)
     params = [q.detach().contiguous() for q in m._plist()]
     ws = torch.empty(lib.tb_lstm_workspace_bytes(T1, B, In, H, L, prec), dtype=torch.uint8, device="cuda")
+    if fill is not None:
+        ws.fill_(fill)
     y, hN, cN = torch.empty(T1, B, H, device="cuda"), torch.empty(L, B, H, device="cuda"), torch.empty(L, B, H, device="cuda")
     _lib.check(lib.tb_lstm_forward(p(x), p(nd), p(h0), p(c0), arr(params), T1, B, In, H, L, prec, p(ws), p(y), p(hN), p(cN),
                                    _lib.stream_ptr()), "tb_lstm_forward")
@@ -126,7 +129,7 @@ def _abi_call(m, pb, ports):
     _lib.check(rc, "tb_lstm_backward")
     n = lib.tb_launch_count() - n0
     torch.cuda.synchronize()
-    return [dx] + grads, n
+    return [dx] + grads + [y, hN, cN], n
 
 
 @pytest.mark.parametrize("T1,B,In,H,layers,precision,kind", [c for c in KIND_CASES if c[0] == 9])

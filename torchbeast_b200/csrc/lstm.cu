@@ -27,11 +27,26 @@
 
 namespace tb {
 
-static inline int padded_h(int H) {
+static constexpr int padded_h(int H) {
   int hp = (H + 3) & ~3;
   if (((hp / 4) & 1) == 0) hp += 4;  // odd number of 16-byte groups per row: conflict-free LDS.128
   return hp;
 }
+
+// Dynamic shared memory of the fp32 step kernels, which hold whole padded rows of H: forward 16 rows of W_hh and a 32-row
+// h tile, backward 16 rows of W_hh^T and a 2-deep ring of 32-row gate-gradient tiles (+ mbarriers).  The persistent fp32
+// kernels stage the same tiles.  Every precision falls back to the step kernels above the other kinds' limits, so the
+// largest H whose backward step kernel fits is the largest hidden size the LSTM takes.
+constexpr size_t kStepFwdSmemMax = 200 * 1024, kStepBwdSmemMax = 220 * 1024;
+static constexpr size_t step_fwd_smem(int H) { return size_t(48) * padded_h(H) * sizeof(float) + 16; }
+static constexpr size_t step_bwd_smem(int H) { return size_t(80) * padded_h(H) * sizeof(float) + 32; }
+static constexpr int lstm_max_hidden() {
+  int H = 1;
+  while (step_bwd_smem(H + 1) <= kStepBwdSmemMax) ++H;
+  return H;
+}
+static_assert(lstm_max_hidden() == TB_LSTM_MAX_HIDDEN, "include/torchbeast_b200.h states the largest hidden size");
+static_assert(step_fwd_smem(TB_LSTM_MAX_HIDDEN) <= kStepFwdSmemMax, "the forward step kernel takes every H the backward takes");
 
 static inline int64_t ld16(int64_t n) { return (n + 7) & ~int64_t(7); }
 // row length (bf16 elements) of the tensor-core recurrence's operand tiles: K padded to 16, +8 so that a
@@ -423,13 +438,14 @@ __global__ void lstm_pack_whh_t_kernel(const float* __restrict__ w, float* __res
 
 static int launch_step_bwd_dh(const DhArgs& a, cudaStream_t st) {
   static bool attr_set = false;
-  const size_t smem = size_t(80) * a.Hp * sizeof(float) + 32;
+  const size_t smem = step_bwd_smem(a.H);
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(lstm_step_bwd_dh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(lstm_step_bwd_dh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kStepBwdSmemMax));
     TB_REQUIRE(e == cudaSuccess, "lstm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  TB_REQUIRE(smem <= 220 * 1024, "lstm: hidden size %d too large for the backward step kernel", a.H);
+  TB_REQUIRE(smem <= kStepBwdSmemMax, "lstm: hidden size %d too large for the backward step kernel (at most %d)", a.H,
+             lstm_max_hidden());
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((a.H + 3) / 4, (a.B + 31) / 32);
   cfg.blockDim = dim3(kStepThreads);
@@ -447,13 +463,13 @@ static int launch_step_bwd_dh(const DhArgs& a, cudaStream_t st) {
 
 static int launch_step_fwd(const StepArgs& a, cudaStream_t st) {
   static bool attr_set = false;
-  const size_t smem = size_t(48) * a.Hp * sizeof(float) + 16;
+  const size_t smem = step_fwd_smem(a.H);
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(lstm_step_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(lstm_step_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(kStepFwdSmemMax));
     TB_REQUIRE(e == cudaSuccess, "lstm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  TB_REQUIRE(smem <= 200 * 1024, "lstm: hidden size %d too large for the step kernel", a.H);
+  TB_REQUIRE(smem <= kStepFwdSmemMax, "lstm: hidden size %d too large for the step kernel", a.H);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((a.H + kStepUnits - 1) / kStepUnits, (a.B + 31) / 32);
   cfg.blockDim = dim3(kStepThreads);
@@ -798,19 +814,18 @@ static int launch(const Launch& l, const char* what, Kernel kernel, const Args&.
 }
 
 static Launch persistent_fwd_launch(int64_t B, int H, cudaStream_t st) {
-  return Launch(dim3((H + kStepUnits - 1) / kStepUnits, unsigned((B + 31) / 32)), kStepThreads,
-                size_t(48) * padded_h(H) * sizeof(float) + 16, st, 1, true);
+  return Launch(dim3((H + kStepUnits - 1) / kStepUnits, unsigned((B + 31) / 32)), kStepThreads, step_fwd_smem(H), st, 1, true);
 }
 static Launch persistent_bwd_launch(int H, cudaStream_t st) {
-  return Launch(dim3((H + 3) / 4), kStepThreads, size_t(80) * padded_h(H) * sizeof(float) + 32, st, 1, true);
+  return Launch(dim3((H + 3) / 4), kStepThreads, step_bwd_smem(H), st, 1, true);
 }
 static bool persistent_fwd_fits(int64_t B, int H) {
   const Launch l = persistent_fwd_launch(B, H, nullptr);
-  return B <= 64 && l.cfg.dynamicSmemBytes <= 200 * 1024 && fits<lstm_fwd_persistent_kernel>(l);
+  return B <= 64 && l.cfg.dynamicSmemBytes <= kStepFwdSmemMax && fits<lstm_fwd_persistent_kernel>(l);
 }
 static bool persistent_bwd_fits(int64_t B, int H) {
   const Launch l = persistent_bwd_launch(H, nullptr);
-  return B <= 32 && l.cfg.dynamicSmemBytes <= 220 * 1024 && fits<lstm_bwd_persistent_kernel>(l);
+  return B <= 32 && l.cfg.dynamicSmemBytes <= kStepBwdSmemMax && fits<lstm_bwd_persistent_kernel>(l);
 }
 
 static int lstm_fwd_persistent(const LstmLayerWs& L, float* hs, const float* notdone, int64_t T1, int64_t B, int H,
@@ -2518,7 +2533,7 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
     const uint64_t dims[4] = {uint64_t(Hq), uint64_t(B), uint64_t(T1 + 1), 2};
     const uint64_t strides[3] = {uint64_t(Hq) * 2, uint64_t(B) * Hq * 2, uint64_t(a.hq_lo) * 2};
     const uint32_t box[4] = {kTileRowE, 16, 1, 2};
-    tcd::make_map_nd(&maps[l], a.hq[l], 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+    TB_TRY(tcd::make_map_nd(&maps[l], a.hq[l], 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE));
   }
   return launch(wave_fwd_split_launch(H, st), "lstm2_fwd_wave_split_kernel", lstm2_fwd_wave_split_kernel, maps[0], maps[1], a);
 }
@@ -3459,6 +3474,8 @@ P layer_slice(Ptr const* a, int first, int depth) {
 
 int lstm_abi_check(int64_t T1, int64_t B, int In, int H, int layers, int precision) {
   TB_REQUIRE(T1 >= 1 && B >= 1 && In >= 1 && H >= 1, "tb_lstm: bad sizes T1=%lld B=%lld In=%d H=%d", (long long)T1, (long long)B, In, H);
+  TB_REQUIRE(H <= lstm_max_hidden(), "tb_lstm: hidden size %d above %d, the largest the backward step kernel takes", H,
+             lstm_max_hidden());
   TB_REQUIRE(layers >= 1, "tb_lstm: at least 1 layer, got %d", layers);
   TB_REQUIRE(precision >= 0 && precision <= 2, "tb_lstm: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
   return 0;
@@ -3473,7 +3490,7 @@ int tb_set_aux_stream(void* stream) {
 }
 
 size_t tb_lstm_workspace_bytes(int64_t T1, int64_t B, int input_size, int hidden_size, int layers, int precision) {
-  if (T1 < 1 || B < 1 || input_size < 1 || hidden_size < 1 || layers < 1) return 0;
+  if (lstm_abi_check(T1, B, input_size, hidden_size, layers, precision)) return 0;
   return lstm_abi_ws(nullptr, T1, B, input_size, hidden_size, layers, precision).bytes;
 }
 

@@ -1,8 +1,10 @@
 """Stacked LSTM over an unroll with per-step done-reset, on its own (C ABI tb_lstm_{forward,backward}).
 
 The recurrence the reference spells as a Python loop of seq_len-1 `nn.LSTM` calls (monobeast.py:603-611,
-polybeast_learner.py:241-249), with hidden size / layers / batch / unroll as free parameters - BASELINE.json configs[4]
-stresses it at T=600, B=128, H=512.  `LSTM` keeps torch.nn.LSTM's parameter names and shapes, so
+polybeast_learner.py:241-249), with layers / batch / unroll / input size as free parameters and any hidden size up to
+MAX_HIDDEN - BASELINE.json configs[4] stresses it at T=600, B=128, H=512.  Above MAX_HIDDEN (TB_LSTM_MAX_HIDDEN in
+include/torchbeast_b200.h) the backward's step kernel cannot hold a row of H in shared memory, so every call, the plan
+included, raises.  `LSTM` keeps torch.nn.LSTM's parameter names and shapes, so
 `lstm.load_state_dict(torch_lstm.state_dict())` works, and `lstm(input, (h0, c0))` is an autograd forward with
 torch.nn.LSTM's sequence-first shapes plus an optional done-reset mask."""
 import ctypes
@@ -16,6 +18,7 @@ from torchbeast_b200 import _lib
 PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
 # recurrence kinds, numbered as TB_LSTM_* in include/torchbeast_b200.h
 KINDS = ("step", "persistent", "persistent_mma", "cluster", "wave_bf16", "wave_split")
+MAX_HIDDEN = 700  # TB_LSTM_MAX_HIDDEN
 
 
 class _LSTMFunction(torch.autograd.Function):
