@@ -140,6 +140,44 @@ int tb_impala_loss_weighted_f32(const float* behavior_logits, const float* targe
                                 float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
                                 void* workspace, void* stream);
 
+/* ---- trust region for off-policy V-trace (Schmitt, Hessel & Simonyan, ICML 2020, "Off-Policy Actor-Critic with
+ * Shared Experience Replay": LASER's beta trust region) ---------------------------------------------------------------
+ * tb_impala_loss_trust_f32: the arguments of tb_impala_loss_weighted_f32 (column_weights may be NULL: unweighted; hp
+ * may be NULL: the scalar arguments) plus trust_beta (f32 [1], device, read when the kernel runs), kl_out [T,B] f32
+ * and trust_out [2] f32.  For every row (t, b) of the shifted inputs:
+ *   kl_t = sum_a pi_t(a) (log pi_t(a) - log mu_t(a)) in fp32, pi = softmax(target_logits), mu = softmax(behavior_logits),
+ *          both log-softmaxes from the max / log-sum-exp the action log-probabilities are formed with (behavior_alp and
+ *          target_alp keep their bits); written to kl_out.
+ *   m_t  = (kl_t <= beta), a comparison: a NaN kl_t is untrusted.
+ *   V-trace and the policy gradient use rho_t * m_t in place of rho_t: at an untrusted row the clipped rho, c_t and the
+ *   pg clip ratio are all 0, so its TD error adds nothing, the trace is cut there and its pg_adv is 0 (no pg loss, no
+ *   pg gradient).  The baseline and entropy terms are unchanged; where every later trace is cut, vs_t = V_t.  m is a
+ *   constant for the backward: no gradient flows through kl.
+ *   log_rhos, behavior_alp and target_alp are the true, unmasked values; vs and pg_adv are the masked ones.
+ * trust_out = {number of trusted rows, sum of kl_t over all T*B rows}: fp64 sums in a fixed order (no atomics), bit-
+ * identical from run to run, rounded to f32 once.  beta = +inf on finite inputs gives the bits of
+ * tb_impala_loss_fwd_bwd_f32 / _hp_f32 / tb_impala_loss_weighted_f32 in every output; identical behaviour and target
+ * logits give kl = 0 exactly, so beta = 0 trusts those rows.  One launch.
+ * tb_impala_loss_popart_trust_f32: tb_impala_loss_popart_f32 with the same rule and the same three arguments (the
+ * per-task sums come from the masked vs).  Two launches.                                                           */
+int tb_impala_loss_trust_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                             const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                             const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                             float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
+                             float clip_pg_rho, const float* column_weights, const tb_hparams* hp, float* vs,
+                             float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                             float* grad_logits, float* grad_values, int zero_tail, const float* trust_beta,
+                             float* kl_out, float* trust_out, void* workspace, void* stream);
+int tb_impala_loss_popart_trust_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                                    const float* rewards, const uint8_t* done, const float* discounts,
+                                    const float* values, const int64_t* task, const double* mu, const double* nu,
+                                    int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
+                                    float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                                    const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
+                                    float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
+                                    float* grad_values, double* task_sums, const float* trust_beta, float* kl_out,
+                                    float* trust_out, void* workspace, void* stream);
+
 /* ---- PopArt value normalisation (van Hasselt et al. 2016; Hessel et al. 2019) -----------
  * Per task k, statistics mu[k], nu[k] (f64, device; start at 0 and 1) with
  *   sigma_k = clamp(sqrt(max(nu_k - mu_k^2, 0)), 1e-4, 1e6).

@@ -35,6 +35,10 @@ _SIGNATURES = {
         [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 12, _int),
     "tb_impala_loss_weighted_f32": (
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 10 + [_int, _vp, _vp], _int),
+    "tb_impala_loss_trust_f32": (
+        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 10 + [_int] + [_vp] * 5, _int),
+    "tb_impala_loss_popart_trust_f32": (
+        [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 15, _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
     "tb_atarinet_param_count_mt": ([_int, _int, _int], _i64),
     "tb_atarinet_forward_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),

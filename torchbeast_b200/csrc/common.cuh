@@ -38,9 +38,11 @@ struct ProfScope {
 
 constexpr int kWarp = 32;
 constexpr int kNumSMs = 132;  // H100 SXM
-// workspace layout: [0] uint32 ticket counter (self-resetting), then kMaxPartialCtas x 4 doubles
+// workspace layout: [0] uint32 ticket counter (self-resetting), then kMaxPartialCtas per-CTA partials of up to
+// kMaxPartialSums doubles each (grid_sum3: stride 4, grid_sum<N>: stride N)
 constexpr int kMaxPartialCtas = 4096;
-constexpr size_t kWorkspaceBytes = 64 + size_t(kMaxPartialCtas) * 4 * sizeof(double);
+constexpr int kMaxPartialSums = 5;
+constexpr size_t kWorkspaceBytes = 64 + size_t(kMaxPartialCtas) * kMaxPartialSums * sizeof(double);
 
 template <typename F> struct M;
 template <> struct M<float> {
@@ -136,6 +138,82 @@ __device__ __forceinline__ bool grid_sum3(double s0, double s1, double s2, void*
       double a = 0, b = 0, c = 0;
       for (int w = 0; w < nwarps; ++w) { a += sm[w][0]; b += sm[w][1]; c += sm[w][2]; }
       tot[0] = a; tot[1] = b; tot[2] = c;
+      *counter = 0u;
+    }
+  }
+  __syncthreads();
+  return is_last && tid == 0;
+}
+
+// grid_sum3 for N doubles per thread (partials at stride N): the same summation order per value, so the first three
+// totals of grid_sum<5> are bit-identical to grid_sum3's for the same inputs and grid.
+template <int N>
+__device__ __forceinline__ bool grid_sum(double (&s)[N], void* ws, double* tot) {
+  static_assert(N >= 1 && N <= kMaxPartialSums, "grid_sum: partials do not fit the workspace");
+  __shared__ double sm[32][N];
+  __shared__ bool is_last;
+  const int tid = threadIdx.x + threadIdx.y * blockDim.x;
+  const int nthreads = blockDim.x * blockDim.y;
+  const int warp = tid >> 5, lane = tid & 31, nwarps = (nthreads + 31) >> 5;
+#pragma unroll
+  for (int k = 0; k < N; ++k) s[k] = warp_sum(s[k]);
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) sm[warp][k] = s[k];
+  }
+  __syncthreads();
+  const unsigned nblocks = gridDim.x * gridDim.y;
+  const unsigned bid = blockIdx.x + blockIdx.y * gridDim.x;
+  unsigned* counter = reinterpret_cast<unsigned*>(ws);
+  double* partials = reinterpret_cast<double*>(reinterpret_cast<char*>(ws) + 64);
+  if (tid == 0) {
+    double a[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) a[k] = 0;
+    for (int w = 0; w < nwarps; ++w) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) a[k] += sm[w][k];
+    }
+    if (nblocks == 1) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) tot[k] = a[k];
+      is_last = true;
+    } else {
+#pragma unroll
+      for (int k = 0; k < N; ++k) partials[bid * N + k] = a[k];
+      __threadfence();
+      unsigned ticket = atomicAdd(counter, 1u);
+      is_last = (ticket == nblocks - 1);
+    }
+  }
+  __syncthreads();
+  if (is_last && nblocks > 1) {  // fold as grid_sum3 does
+    __threadfence();
+    double x[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) x[k] = 0;
+    for (unsigned i = tid; i < nblocks; i += nthreads) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) x[k] += __ldcg(&partials[i * N + k]);
+    }
+#pragma unroll
+    for (int k = 0; k < N; ++k) x[k] = warp_sum(x[k]);
+    __syncthreads();
+    if (lane == 0) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) sm[warp][k] = x[k];
+    }
+    __syncthreads();
+    if (tid == 0) {
+      double a[N];
+#pragma unroll
+      for (int k = 0; k < N; ++k) a[k] = 0;
+      for (int w = 0; w < nwarps; ++w) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) a[k] += sm[w][k];
+      }
+#pragma unroll
+      for (int k = 0; k < N; ++k) tot[k] = a[k];
       *counter = 0u;
     }
   }

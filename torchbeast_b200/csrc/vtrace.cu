@@ -438,7 +438,81 @@ struct LossArgs {
   // importance weights (impala_loss_kernel<A, false, true> only): column b's pg, baseline and entropy terms, in the
   // losses and the gradients, are multiplied by column_weights[b]
   const float* column_weights;
+  // trust region (impala_loss_kernel<A, *, *, true> only): beta read from *trust_beta when the kernel runs, kl [T,B]
+  // out, trust_out [2] = {trusted rows, sum kl}
+  const float* trust_beta; float* kl; float* trust_out;
 };
+
+// ---- trust region (impala_loss_kernel<A, *, *, true>) ----------------------------------------------------------------
+// The kernel reaches the trust region only through the three helpers below, so the instantiations without it compile
+// to the same code as before the trust region existed.
+
+// KL(pi || mu) of row i in fp32.  Each row's max and log-sum-exp come from alp_row, the code that forms the action
+// log-probabilities, so both log-softmaxes are the ones behind target_alp / behavior_alp; identical rows give 0.
+template <int A>
+__device__ __forceinline__ float trust_kl(const LossArgs& p, int64_t i, int64_t Ause) {
+  const float* trow = p.tlogits + i * Ause;
+  const float* brow = p.blogits + i * Ause;
+  float mt, logst, mb, logsb;
+  alp_row<float, A>(trow, Ause, 0, &mt, &logst);
+  alp_row<float, A>(brow, Ause, 0, &mb, &logsb);
+  float kl = 0.0f;
+  if constexpr (A == 0) {
+    for (int64_t j = 0; j < Ause; ++j) {
+      const float lt = (trow[j] - mt) - logst, lb = (brow[j] - mb) - logsb;
+      kl += expf(lt) * (lt - lb);
+    }
+  } else {
+    float xt[A], xb[A];
+    RowOps<float, A>::load(trow, Ause, xt);
+    RowOps<float, A>::load(brow, Ause, xb);
+#pragma unroll
+    for (int j = 0; j < A; ++j) {
+      const float lt = (xt[j] - mt) - logst, lb = (xb[j] - mb) - logsb;
+      kl += expf(lt) * (lt - lb);
+    }
+  }
+  return kl;
+}
+
+// rho of row i under the trust region: expf(lr) where kl_i <= beta, else 0 (a NaN kl too).  kl_i is formed and written
+// to p.kl here, or, with `written`, read back from there (pass 1 of the split layout wrote it in this thread).
+template <int A>
+__device__ __forceinline__ float trust_rho(const LossArgs& p, int64_t i, int64_t Ause, float lr, bool written) {
+  float kl;
+  if (written) {
+    kl = p.kl[i];
+  } else {
+    kl = trust_kl<A>(p, i, Ause);
+    p.kl[i] = kl;
+  }
+  const float rho = expf(lr);
+  return kl <= *p.trust_beta ? rho : 0.0f;
+}
+
+// The end of the trust-region kernel: the trusted rows and the sum of kl over this thread's rows, read back from p.kl
+// in the order pass 3 walked them, then one five-value grid sum.  The loss values are those grid_sum3 would give.
+__device__ __forceinline__ void trust_finish(const LossArgs& p, double s_pg, double s_bl, double s_en, int64_t tile0,
+                                             int64_t tile_step, int64_t t0, int64_t t1) {
+  const int64_t tiles = (p.B + kWarp - 1) / kWarp;
+  const float beta = *p.trust_beta;
+  double rows = 0.0, kl_sum = 0.0;
+  for (int64_t tile = tile0; tile < tiles; tile += tile_step) {
+    const int64_t b = tile * kWarp + threadIdx.x;
+    if (b >= p.B) continue;
+    for (int64_t t = t1 - 1; t >= t0; --t) {
+      const float kl = p.kl[t * p.B + b];
+      rows += (kl <= beta) ? 1.0 : 0.0;
+      kl_sum += double(kl);
+    }
+  }
+  double s[5] = {s_pg, s_bl, s_en, rows, kl_sum}, tot[5];
+  if (grid_sum<5>(s, p.workspace, tot)) {
+    const double pg = tot[0], bl = double(p.baseline_cost) * tot[1], en = double(p.entropy_cost) * tot[2];
+    p.losses[0] = float(pg); p.losses[1] = float(bl); p.losses[2] = float(en); p.losses[3] = float(pg + bl + en);
+    p.trust_out[0] = float(tot[3]); p.trust_out[1] = float(tot[4]);
+  }
+}
 
 constexpr int kPopArtMaxTasks = 64;
 
@@ -468,8 +542,9 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 // kPopArt: the value input is PopArt-normalised (LossArgs::task / pa_mu / pa_nu / K); the non-PopArt instantiations
 // compile none of that code.  kWeighted: every term of column b is multiplied by LossArgs::column_weights[b], after the
 // unweighted term is formed, so a weight of 1.0f gives the unweighted bits; the other instantiations compile no weight
-// code.
-template <int A, bool kPopArt = false, bool kWeighted = false>
+// code.  kTrust: row (t, b) with kl_t = KL(pi_t || mu_t) > beta (or NaN) runs the V-trace and the policy gradient with
+// rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_trust_f32); the other instantiations compile no trust code.
+template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
   if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -517,7 +592,7 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
           const float blp = alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
           const float lr = tlp - blp;
           p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
-          const float rho = expf(lr);
+          const float rho = kTrust ? trust_rho<A>(p, i, Ause, lr, false) : expf(lr);  // kl read back in pass 3
           const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
           const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
           const float delta = rb * (r + g * v_next - v);
@@ -563,7 +638,7 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         lr = tlp - blp;
         p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
       }
-      const float rho = expf(lr);
+      const float rho = kTrust ? trust_rho<A>(p, i, Ause, lr, W > 1) : expf(lr);
       const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
       const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
       const float rp = p.has_clip_pg ? fminf(rho, p.clip_pg) : rho;
@@ -642,6 +717,10 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         }
       }
     }
+  }
+  if constexpr (kTrust) {
+    trust_finish(p, s_pg, s_bl, s_en, tile0, tile_step, t0, t1);
+    return;
   }
   double tot[3];
   if (grid_sum3(s_pg, s_bl, s_en, p.workspace, tot)) {
@@ -777,13 +856,19 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
                               float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream,
                               const int64_t* task = nullptr, const double* pa_mu = nullptr,
                               const double* pa_nu = nullptr, int K = 0, double* task_sums = nullptr,
-                              const float* column_weights = nullptr) {
+                              const float* column_weights = nullptr, const float* trust_beta = nullptr,
+                              float* kl_out = nullptr, float* trust_out = nullptr) {
   TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
              (long long)B, (long long)A);
   TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
+  TB_REQUIRE(!trust_beta || (kl_out && trust_out), "impala_loss_trust: kl_out/trust_out must not be null");
   if (T == 0 || B == 0) {
     cudaError_t e = cudaMemsetAsync(losses_out, 0, 4 * sizeof(float), (cudaStream_t)stream);
     TB_REQUIRE(e == cudaSuccess, "impala_loss: memset: %s", cudaGetErrorString(e));
+    if (trust_beta) {
+      e = cudaMemsetAsync(trust_out, 0, 2 * sizeof(float), (cudaStream_t)stream);
+      TB_REQUIRE(e == cudaSuccess, "impala_loss_trust: memset: %s", cudaGetErrorString(e));
+    }
     if (B > 0 && zero_tail) {
       if (grad_values) cudaMemsetAsync(grad_values, 0, B * sizeof(float), (cudaStream_t)stream);
       if (grad_logits) cudaMemsetAsync(grad_logits, 0, B * A * sizeof(float), (cudaStream_t)stream);
@@ -805,6 +890,7 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   p.hp = hp;
   p.task = task; p.pa_mu = pa_mu; p.pa_nu = pa_nu; p.K = K;
   p.column_weights = column_weights;
+  p.trust_beta = trust_beta; p.kl = kl_out; p.trust_out = trust_out;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
   int W = pick_warps(T, tiles);
   p.wide = (W == 1);
@@ -818,12 +904,26 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   dim3 block(kWarp, W);
   const size_t smem = size_t(2) * W * kWarp * sizeof(float);
   if (task) {
-    ProfScope prof("impala_loss_popart", (cudaStream_t)stream);
+    ProfScope prof(trust_beta ? "impala_loss_popart_trust" : "impala_loss_popart", (cudaStream_t)stream);
     const size_t pop_smem = smem + size_t(2) * kPopArtMaxTasks * sizeof(float);
-    TB_DISPATCH_A(A, (impala_loss_kernel<kA, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
-    TB_TRY(check_launch("impala_loss_kernel<popart>"));
+    if (trust_beta) {
+      TB_DISPATCH_A(A, (impala_loss_kernel<kA, true, false, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
+      TB_TRY(check_launch("impala_loss_kernel<popart, trust>"));
+    } else {
+      TB_DISPATCH_A(A, (impala_loss_kernel<kA, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
+      TB_TRY(check_launch("impala_loss_kernel<popart>"));
+    }
     popart_task_sums_kernel<<<K, kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, K, task_sums);
     return check_launch("popart_task_sums_kernel");
+  }
+  if (trust_beta) {
+    ProfScope prof("impala_loss_trust", (cudaStream_t)stream);
+    if (column_weights) {
+      TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, true, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+      return check_launch("impala_loss_kernel<weighted, trust>");
+    }
+    TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, false, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+    return check_launch("impala_loss_kernel<trust>");
   }
   if (column_weights) {
     ProfScope prof("impala_loss_weighted", (cudaStream_t)stream);
@@ -919,6 +1019,42 @@ int tb_impala_loss_weighted_f32(const float* blogits, const float* tlogits, cons
                             discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs,
                             pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
                             zero_tail, workspace, stream, nullptr, nullptr, nullptr, 0, nullptr, column_weights);
+}
+
+int tb_impala_loss_trust_f32(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
+                             const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
+                             int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
+                             int clip_rewards, float clip_rho, float clip_pg_rho, const float* column_weights,
+                             const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
+                             float* target_alp, float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
+                             const float* trust_beta, float* kl_out, float* trust_out, void* workspace, void* stream) {
+  TB_REQUIRE(trust_beta, "impala_loss_trust: null trust_beta");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
+                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs,
+                            pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
+                            zero_tail, workspace, stream, nullptr, nullptr, nullptr, 0, nullptr, column_weights,
+                            trust_beta, kl_out, trust_out);
+}
+
+int tb_impala_loss_popart_trust_f32(const float* blogits, const float* tlogits, const int64_t* actions,
+                                    const float* rewards, const uint8_t* done, const float* discounts,
+                                    const float* values, const int64_t* task, const double* mu, const double* nu,
+                                    int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
+                                    float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                                    const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
+                                    float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
+                                    float* grad_values, double* task_sums, const float* trust_beta, float* kl_out,
+                                    float* trust_out, void* workspace, void* stream) {
+  TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
+             (long long)B, (long long)A);
+  TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "impala_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
+             kPopArtMaxTasks);
+  TB_REQUIRE(values && task && mu && nu && task_sums, "impala_loss_popart: null PopArt pointer");
+  TB_REQUIRE(trust_beta, "impala_loss_popart_trust: null trust_beta");
+  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, values, T, B, A, discounting,
+                            baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs, pg_adv, log_rhos,
+                            behavior_alp, target_alp, losses_out, grad_logits, grad_values, 1, workspace, stream, task,
+                            mu, nu, int(K), task_sums, nullptr, trust_beta, kl_out, trust_out);
 }
 
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,

@@ -1,5 +1,6 @@
 """Fused pieces of the learner step shared by monobeast.learn and polybeast_learner.learn."""
 import collections
+import numbers
 import os
 import threading
 
@@ -12,6 +13,9 @@ ImpalaLoss = collections.namedtuple(
     "ImpalaLoss",
     "vs pg_advantages log_rhos behavior_action_log_probs target_action_log_probs losses grad_logits grad_values",
 )
+# What the trust-region loss returns next to its ImpalaLoss: kl float32 [T, B] = KL(pi_t || mu_t) of every row, sums
+# float32 [2] = {number of trusted rows, sum of kl over all rows}.
+TrustRegion = collections.namedtuple("TrustRegion", "kl sums")
 
 # tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the *_hp entry points read from device memory.
 # tb_hparams_layout() reports the compiled layout; tests/test_graph_hparams_cpu.py checks this record against it.
@@ -53,6 +57,35 @@ def publish_hparams(rec, block):
     block.copy_(host, non_blocking=True)
 
 
+def trust_region_kl(flags):
+    """flags.trust_region_kl as a float beta >= 0 (+inf allowed), or None when the flag is None or absent (no trust
+    region).  Raises ValueError for a negative, NaN or non-numeric value, before anything is launched."""
+    v = getattr(flags, "trust_region_kl", None)
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, numbers.Real):
+        raise ValueError("trust_region_kl must be None or a number >= 0, got %r" % (v,))
+    beta = float(v)
+    if not beta >= 0.0:  # NaN fails too
+        raise ValueError("trust_region_kl must be >= 0 (or None), got %r" % (v,))
+    return beta
+
+
+def _trust_beta_tensor(trust_region, device):
+    """The device float32 [1] beta the trust-region kernels read: `trust_region` itself when it is a tensor (a graph's
+    published scalar), else a new one holding float(trust_region)."""
+    if isinstance(trust_region, torch.Tensor):
+        _lib.require_cuda(trust_region)
+        if trust_region.dtype != torch.float32 or trust_region.numel() != 1:
+            raise _lib.TorchBeastB200Error("trust_region must be a float or a float32 device scalar, got %s %r" % (
+                trust_region.dtype, tuple(trust_region.shape)))
+        return trust_region
+    beta = float(trust_region)
+    if not beta >= 0.0:
+        raise ValueError("trust_region must be >= 0, got %r" % (trust_region,))
+    return torch.full((1,), beta, dtype=torch.float32, device=device)
+
+
 def hparams_field(block, name):
     """Field `name` of a device tb_hparams block as a 0-dim tensor view (float32 / float64 / int32)."""
     dt, off = HPARAMS.fields[name]
@@ -78,6 +111,7 @@ def impala_loss_fwd_bwd(
     with_grads=True,
     hparams_dev=None,
     column_weights=None,
+    trust_region=None,
 ):
     """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_fwd_bwd_f32).
 
@@ -94,6 +128,11 @@ def impala_loss_fwd_bwd(
     With `column_weights` (float32 [B], device) the pg, baseline and entropy terms of column b, in the losses and the
     gradients, are multiplied by column_weights[b] (tb_impala_loss_weighted_f32, prioritised replay's importance
     weights); weights of 1.0 give the unweighted bits.
+
+    With `trust_region` (beta: a float >= 0, or a float32 device scalar read when the kernel runs) a row whose
+    KL(pi || mu) exceeds beta gets rho = 0 in the V-trace and the policy gradient (tb_impala_loss_trust_f32; the rule
+    is stated in include/torchbeast_b200.h), and the call returns (ImpalaLoss, TrustRegion).  vs and pg_advantages
+    are the masked ones; log_rhos and the log-probabilities are not masked.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
@@ -128,6 +167,21 @@ def impala_loss_fwd_bwd(
     losses = torch.empty(4, dtype=f32, device=dev)
     gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
     gv = torch.empty((T + 1, B), dtype=f32, device=dev) if with_grads else None
+    if trust_region is not None:
+        p = _lib.ptr
+        beta = _trust_beta_tensor(trust_region, dev)
+        trust = TrustRegion(torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev))
+        cw = None if column_weights is None else column_weights.contiguous()
+        _lib.check(
+            _lib.lib().tb_impala_loss_trust_f32(
+                p(bl), p(tl), p(ac), p(rw), p(dn), p(disc), p(va), p(bs), T, B, A,
+                0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
+                0 if hparams_dev is not None else clip_rewards, _lib.clip_arg(clip_rho_threshold),
+                _lib.clip_arg(clip_pg_rho_threshold), p(cw), p(hparams_dev),
+                *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(beta), p(trust.kl), p(trust.sums),
+                p(_lib.workspace()), _lib.stream_ptr()),
+            "tb_impala_loss_trust_f32")
+        return ImpalaLoss(*outs, losses, gl, gv), trust
     if column_weights is not None:
         p = _lib.ptr
         _lib.check(
@@ -178,6 +232,7 @@ def impala_loss_popart(
     clip_rho_threshold=1.0,
     clip_pg_rho_threshold=1.0,
     hparams_dev=None,
+    trust_region=None,
 ):
     """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_popart_f32).
 
@@ -186,7 +241,8 @@ def impala_loss_popart(
     pg_advantages are unnormalised, the losses and gradients are taken in normalised space, and grad_values is
     [T+1, B, K].  A row with a task id outside [0, K) adds no loss and gets zero gradient rows.  Returns
     (ImpalaLoss, task_sums): task_sums float64 [3, K] = per-task count, sum vs, sum vs^2 over rows t < T, the input
-    of popart_update (SUM all-reduce it first when data-parallel)."""
+    of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd;
+    tb_impala_loss_popart_trust_f32) it returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs."""
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
     _lib.require_cuda(*tensors)
     T, B, A = target_policy_logits.shape
@@ -216,6 +272,20 @@ def impala_loss_popart(
     gv = torch.empty((T + 1, B, K), dtype=f32, device=dev)
     sums = torch.empty((3, K), dtype=torch.float64, device=dev)
     p = _lib.ptr
+    if trust_region is not None:
+        beta = _trust_beta_tensor(trust_region, dev)
+        trust = TrustRegion(torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev))
+        _lib.check(
+            _lib.lib().tb_impala_loss_popart_trust_f32(
+                p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
+                p(actions.to(torch.int64).contiguous()), p(rewards.to(f32).contiguous()), p(dn), p(disc),
+                p(values.detach().to(f32).contiguous()), p(task.to(torch.int64).contiguous()), p(mu.contiguous()),
+                p(nu.contiguous()), T, B, A, K, float(discounting) if hparams_dev is None else 0.0,
+                float(baseline_cost), float(entropy_cost), clip_rewards, _lib.clip_arg(clip_rho_threshold),
+                _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev), *[p(o) for o in outs], p(losses), p(gl), p(gv),
+                p(sums), p(beta), p(trust.kl), p(trust.sums), p(_lib.workspace()), _lib.stream_ptr()),
+            "tb_impala_loss_popart_trust_f32")
+        return ImpalaLoss(*outs, losses, gl, gv), sums, trust
     _lib.check(
         _lib.lib().tb_impala_loss_popart_f32(
             p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
@@ -360,7 +430,7 @@ def _check_replay(model):
 
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
                behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None,
-               fresh_columns=None, draw=None):
+               fresh_columns=None, draw=None, trust_beta_dev=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -380,10 +450,19 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     `draw` (a prioritised buffer's replay.Draw, or one built by hand): with `draw.weights` the loss is the importance-
     weighted one (impala_loss_fwd_bwd with column_weights), so the stats' loss values are the weighted sums; with
     `draw.buffer` its priorities are updated from the loss's vs and values at `draw.slots`, right after the loss.
+
+    flags.trust_region_kl (a float beta >= 0; None or absent: off) runs the trust-region loss: rows with
+    KL(pi || mu) > beta get rho = 0 in the V-trace and the policy gradient, on every column, fresh and replayed.  beta
+    is `trust_beta_dev` (a float32 device scalar, GraphedLearner's) or the flag.  The stats then carry
+    trust_fraction (trusted rows / T*B) and mean_policy_kl (sum KL / T*B), read back with the loss values; a prioritised
+    buffer's priorities come from the masked vs.
     """
     pop = getattr(model, "popart", None)
     if draw is not None and pop is not None:
         raise _lib.TorchBeastB200Error(_POPART_PRIORITIZED)
+    beta = trust_region_kl(flags)
+    trust_region = None if beta is None else (beta if trust_beta_dev is None else trust_beta_dev)
+    trust = None
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
     acts = batch["action"] if actions is None else actions
@@ -393,17 +472,22 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             out.baseline[:-1], out.baseline[-1],
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
-            column_weights=None if draw is None else draw.weights)
+            column_weights=None if draw is None else draw.weights, trust_region=trust_region)
+        if trust_region is not None:
+            loss, trust = loss
         grad_values = loss.grad_values
         if draw is not None and draw.buffer is not None:
             draw.buffer.update_priorities(loss.vs, out.baseline[:-1], draw.slots)
     else:
         values = out.baseline.reshape(out.baseline.shape[:2] + (pop.num_tasks,))
-        loss, task_sums = impala_loss_popart(
+        res = impala_loss_popart(
             blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:], values,
             _popart_task(model, batch), pop.mu, pop.nu,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
-            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev)
+            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region)
+        loss, task_sums = res[:2]
+        if trust_region is not None:
+            trust = res[2]
         grad_values = loss.grad_values.view(out.baseline.shape)
     _backward_with_overlapped_all_reduce(model, loss.grad_logits, grad_values)
     optimizer_step(model, optimizer, flags.grad_norm_clipping, hparams_dev=hparams_dev)
@@ -423,12 +507,13 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         else:
             actor_model.load_state_dict(model.state_dict())
     if not stats_sync:
-        return dict(losses=loss.losses, vtrace=loss)
+        return dict(losses=loss.losses, vtrace=loss, trust=trust)
     done, ep_ret = batch["done"][1:], batch["episode_return"][1:]
     if fresh_columns is not None:
         done, ep_ret = done[:, :fresh_columns], ep_ret[:, :fresh_columns]
     episode_returns = ep_ret[done.bool()]
-    host = loss.losses.cpu()  # the step's one blocking read-back
+    # the step's one blocking read-back: the loss values, and the trust-region sums behind them
+    host = (loss.losses if trust is None else torch.cat([loss.losses, trust.sums])).cpu()
     ep = episode_returns.cpu()
     stats = {
         "episode_returns": tuple(ep.numpy()),
@@ -438,9 +523,16 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         "baseline_loss": host[1].item(),
         "entropy_loss": host[2].item(),
     }
+    if trust is not None:
+        stats.update(_trust_stats(host[4:6], trust.kl.numel()))
     if pop is not None:
         stats.update(_popart_stats(pop.mu.cpu(), pop.nu.cpu()))
     return stats
+
+
+def _trust_stats(sums, rows):
+    """The stats-dict entries of the trust region from a host copy of its two sums over `rows` rows."""
+    return {"trust_fraction": sums[0].item() / rows, "mean_policy_kl": sums[1].item() / rows}
 
 
 def _graph_enabled(flags):
@@ -500,7 +592,7 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
             if _graph_enabled(flags):
                 _require_fused(optimizer)
                 hparams = pack_hparams(flags, optimizer)  # raises before anything is captured or replayed
-                structure = GraphedLearner.structure_of(optimizer, batch)
+                structure = GraphedLearner.structure_of(optimizer, batch, flags)
                 graphs = model.__dict__.setdefault("_tb_graphs", {})
                 gkey = (tuple((k, tuple(v.shape)) for k, v in batch.items() if k in GraphedLearner.KEYS), id(optimizer),
                         id(actor_model))
@@ -588,17 +680,24 @@ class GraphedLearner:
     KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return", "task")
 
     @staticmethod
-    def structure_of(optimizer, batch):
+    def structure_of(optimizer, batch, flags=None):
         """What the captured launch sequence depends on besides shapes: the optimizer's kernel and buffer choices
-        (RMSprop centered / weight_decay != 0 / momentum != 0, Adam vs AdamW) and the dtype of `done`."""
-        return optimizer.structure() + (batch["done"].dtype,)
+        (RMSprop centered / weight_decay != 0 / momentum != 0, Adam vs AdamW), the dtype of `done`, and whether
+        `flags` turn the trust region on (its beta is published per replay; on / off chooses the loss kernel)."""
+        trust = flags is not None and trust_region_kl(flags) is not None
+        return optimizer.structure() + (batch["done"].dtype,) + (("trust_region",) if trust else ())
 
     def __init__(self, flags, model, actor_model, optimizer, example_batch, initial_agent_state=()):
         _require_fused(optimizer)
         self.flags, self.model, self.actor, self.opt = flags, model, actor_model, optimizer
-        self.structure = self.structure_of(optimizer, example_batch)
+        self.structure = self.structure_of(optimizer, example_batch, flags)
         self.hparams = torch.zeros(HPARAMS.itemsize, dtype=torch.uint8, device=model.flat_params.device)
         publish_hparams(pack_hparams(flags, optimizer), self.hparams)
+        # trust region: beta is a float32 device scalar published before every replay, like PopArt's beta
+        self.trust_beta = None
+        if trust_region_kl(flags) is not None:
+            self.trust_beta = torch.zeros(1, dtype=torch.float32, device=model.flat_params.device)
+            self._publish_trust_beta(flags)
         # PopArt: beta is a device scalar published before every replay, like the tb_hparams block
         self.popart = getattr(model, "popart", None)
         self.popart_beta = None
@@ -663,7 +762,8 @@ class GraphedLearner:
             batch, state = self.replay.launch(batch, state, self.mixing)
             draw = self.replay.last_draw if self.replay.prioritized else None
         return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
-                          hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw)
+                          hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw,
+                          trust_beta_dev=self.trust_beta)
 
     def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
         """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
@@ -676,6 +776,8 @@ class GraphedLearner:
         publish_hparams(pack_hparams(self.flags, self.opt) if hparams is None else hparams, self.hparams)
         if self.popart is not None:
             self._publish_beta(self.flags)
+        if self.trust_beta is not None:
+            self._publish_trust_beta(self.flags)
         if self.replay is not None:
             self.replay.prepare(self.static, self.static_state)  # publishes seed / step if the host changed them
         self.graph.replay()
@@ -690,12 +792,27 @@ class GraphedLearner:
         host = torch.full((1,), popart_beta(flags), dtype=torch.float64).pin_memory()
         self.popart_beta.copy_(host, non_blocking=True)
 
+    def _publish_trust_beta(self, flags):
+        """Enqueue the copy of flags.trust_region_kl (validated; float32) into the device scalar, as _publish_beta."""
+        beta = trust_region_kl(flags)
+        if beta is None:
+            raise ValueError("this graph was captured with a trust region; trust_region_kl is now None")
+        host = torch.full((1,), beta, dtype=torch.float32).pin_memory()
+        self.trust_beta.copy_(host, non_blocking=True)
+
+    def _losses_out(self):
+        """The step's loss values, and with a trust region its two sums behind them: float32 [4] or [6]."""
+        trust = self.out["trust"]
+        return self.out["losses"] if trust is None else torch.cat([self.out["losses"], trust.sums])
+
     def snapshot(self):
-        """Device copies of what stats() reads (the step's losses and its done / episode_return rows, and a PopArt model's
-        statistics), enqueued on the current stream: lets the caller release the learner lock BEFORE the blocking
-        read-back, so the next learner thread's replay queues up behind this one instead of waiting for a host round
-        trip."""
-        snap = (self.out["losses"].clone(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone())
+        """Device copies of what stats() reads (the step's losses and its done / episode_return rows, a PopArt model's
+        statistics, the trust-region sums and row count), enqueued on the current stream: lets the caller release the
+        learner lock BEFORE the blocking read-back, so the next learner thread's replay queues up behind this one
+        instead of waiting for a host round trip."""
+        trust = self.out["trust"]
+        snap = (self._losses_out(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone(),
+                None if trust is None else trust.kl.numel())
         if self.popart is not None:
             snap += (self.popart.mu.clone(), self.popart.nu.clone())
         return snap
@@ -707,21 +824,22 @@ class GraphedLearner:
         """Read the snapshot back on a per-thread READ-BACK stream that waits only for `event` (recorded right after the
         snapshot): a read-back on the compute stream would queue behind the NEXT step, which another learner thread has
         already enqueued there."""
-        losses, done, ep_ret = snap[:3]
+        losses, done, ep_ret, trust_rows = snap[:4]
         tls = GraphedLearner._tls
         dev = losses.device
         if getattr(tls, "stream", None) is None or tls.device != dev:
             tls.stream, tls.device, tls.pinned = torch.cuda.Stream(device=dev), dev, {}
-        key = (tuple(done.shape), done.dtype)
+        key = (tuple(done.shape), done.dtype, losses.numel())
         bufs = tls.pinned.get(key)
         if bufs is None:
-            bufs = tls.pinned[key] = (torch.empty(4, dtype=torch.float32).pin_memory(), torch.empty(done.shape, dtype=done.dtype).pin_memory(),
+            bufs = tls.pinned[key] = (torch.empty(losses.numel(), dtype=torch.float32).pin_memory(),
+                                      torch.empty(done.shape, dtype=done.dtype).pin_memory(),
                                       torch.empty(ep_ret.shape, dtype=ep_ret.dtype).pin_memory())
         tls.stream.wait_event(event)
         with torch.cuda.stream(tls.stream):
             for dst, src in zip(bufs, (losses, done, ep_ret)):
                 dst.copy_(src, non_blocking=True)
-            popart = [s.to("cpu", non_blocking=True) for s in snap[3:]]
+            popart = [s.to("cpu", non_blocking=True) for s in snap[4:]]
         tls.stream.synchronize()
         host, hdone, hret = bufs
         ep = hret[hdone.bool()].clone()
@@ -730,6 +848,8 @@ class GraphedLearner:
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
+        if trust_rows is not None:
+            stats.update(_trust_stats(host[4:6], trust_rows))
         if popart:
             stats.update(_popart_stats(*popart))
         return stats
@@ -738,12 +858,14 @@ class GraphedLearner:
         """Same keys as monobeast.learn()'s return value; one blocking read-back."""
         done = self.static["done"][1:]
         ep = self.static["episode_return"][1:][done.bool()].cpu()
-        host = self.out["losses"].cpu()
+        host = self._losses_out().cpu()
         stats = {
             "episode_returns": tuple(ep.numpy()), "mean_episode_return": torch.mean(ep).item(),
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
+        if self.out["trust"] is not None:
+            stats.update(_trust_stats(host[4:6], self.out["trust"].kl.numel()))
         if self.popart is not None:
             stats.update(_popart_stats(self.popart.mu.cpu(), self.popart.nu.cpu()))
         return stats
