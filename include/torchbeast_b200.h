@@ -751,6 +751,71 @@ int tb_maxpool3x3s2_fwd_f32(const float* x, float* y, uint8_t* argmax, int64_t N
 int tb_f32_to_bf16(const float* in, void* out_bf16, int64_t rows, int64_t cols, int64_t ld, int64_t ld16,
                    void* stream);
 
+/* ---- fp32 network building blocks -----------------------------------------------------------------------------------
+ * The kernels of the fp32 backend, the ResNet patch-matrix path, the fused heads and the bias-gradient column sums, for
+ * tests and diagnostics (the learner calls the same internals from C++).  Every entry is a thin wrapper that adds no
+ * behaviour.
+ *
+ * fp32 SIMT GEMM: C[M,N] (+)= sum_k A(m,k) B(k,n), A(m,k) = ta ? A[k*lda + m] : A[m*lda + k], B(k,n) = tb ? B[n*ldb + k]
+ * : B[k*ldb + n]; a_u8 / b_u8: the operand is uint8, read as x/255.  The five (a_u8, b_u8, ta, tb) combinations the
+ * learner runs are (0,0,0,1) forward, (1,0,0,1) uint8 forward, (0,0,0,0) input gradient, (0,0,1,0) weight gradient and
+ * (0,1,1,0) uint8 weight gradient; any other is rejected.  splits (clamped to the K tiles of 16) > 1 or permP * permQ > 1
+ * takes the split-K path: raw partials [splits][M][N] in scratch, then a fixed-order reduce that applies C = scale * sum
+ * + bias, ReLU, and stores column n = p*permQ + q at q*permP + p (permP * permQ = N).  Otherwise the direct path applies
+ * C = acc + bias, ReLU, zeroed where mask [M, ldmask] is not positive, + addend [M, ldadd].  Either then stores C, or adds
+ * it to C when accumulate.  An epilogue field the chosen path does not apply (mask or addend on the split-K path, scale
+ * != 1 on the direct path) is rejected.  tb_gemm_f32_splits is the split count the learner picks for a weight gradient,
+ * with tb_splitk_scratch_floats() floats of partials.                                                                  */
+int tb_gemm_f32(const void* A, int a_u8, const void* B, int b_u8, int ta, int tb, int64_t M, int64_t N, int64_t K, int64_t lda,
+                int64_t ldb, float* C, int64_t ldc, const float* bias, int relu, const float* mask, int64_t ldmask,
+                const float* addend, int64_t ldadd, int accumulate, int permP, int permQ, float scale, int splits, float* scratch,
+                void* stream);
+int tb_gemm_f32_splits(int64_t M, int64_t N, int64_t K, int64_t scratch_floats, int64_t cap);
+int64_t tb_splitk_scratch_floats(void);
+/* AtariNet patch matrices: frames u8 NCHW [N,C,H,W] -> u8 [N*OH*OW, C*KH*KW] (k = (c*KH + kh)*KW + kw); act f32 NHWC
+ * [N,H,W,C] -> f32 [N*OH*OW, KH*KW*C] (k = (kh*KW + kw)*C + c, C % 4 == 0); col2im is the gather-form adjoint of the
+ * latter, times (act > 0) when act is not NULL.  No padding.                                                            */
+int tb_im2col_u8_nchw(const uint8_t* frame, uint8_t* col, int64_t N, int C, int H, int W, int KH, int KW, int S, void* stream);
+int tb_im2col_f32_nhwc(const float* act, float* col, int64_t N, int H, int W, int C, int KH, int KW, int S, void* stream);
+int tb_col2im_f32_nhwc(const float* dcol, const float* act, float* dact, int64_t N, int H, int W, int C, int KH, int KW, int S,
+                       void* stream);
+/* out[o, p*Q + q] = in[o, q*P + p] */
+int tb_permute_pq(const float* in, float* out, int64_t O, int P, int Q, void* stream);
+/* X[m, n] = 0 where !(Y[m, n] > 0), n < ncols */
+int tb_relu_mask_f32(float* X, const float* Y, int64_t M, int64_t ncols, int64_t ldx, int64_t ldy, void* stream);
+/* core[n, F] = clamp(reward[n], -1, 1), core[n, F+1+j] = (last_action[n] == j) for j < A */
+int tb_core_extras(float* core, int64_t ld, int64_t N, int F, const float* reward, const int64_t* last_action, int A,
+                   void* stream);
+/* ResNet patch-matrix path; dtype 0 = fp32, 1 = bf16 for every operand.  im2col3x3: x NHWC [N,H,W,C] (through ReLU if
+ * relu_in) -> col [N*H*W, ldk], k = (kh*3 + kw)*C + c, 3x3 / stride 1 / zero padding 1.  im2col3x3_u8: frames u8 NCHW
+ * [N,1..16,H,W] -> col [N*H*W, ldk] (dtype 0: uint8, 1: bf16), k = (c*3 + kh)*3 + kw.  col2im3x3: its adjoint, dx =
+ * gather(dcol) * (relu_src > 0 if relu_src) + addend (each nullable).  maxpool3x3s2: nn.MaxPool2d(3, 2, 1) on NHWC with the
+ * argmax taps of tb_maxpool3x3s2_fwd_f32; the backward gathers dy through them.  relu: y = max(x, 0), dx = dy * (x > 0). */
+int tb_im2col3x3(const void* x, void* col, int64_t N, int H, int W, int C, int64_t ldk, int relu_in, int dtype, void* stream);
+int tb_im2col3x3_u8(const uint8_t* frame, void* col, int64_t N, int C, int H, int W, int64_t ldk, int dtype, void* stream);
+int tb_col2im3x3(const void* dcol, const void* relu_src, const void* addend, void* dx, int64_t N, int H, int W, int C, int64_t ldk,
+                 int dtype, void* stream);
+int tb_maxpool3x3s2_fwd(const void* x, void* y, uint8_t* argmax, int64_t N, int H, int W, int C, int dtype, void* stream);
+int tb_maxpool3x3s2_bwd(const uint8_t* argmax, const void* dy, void* dx, int64_t N, int H, int W, int C, int dtype, void* stream);
+int tb_relu_fwd(const void* x, void* y, int64_t n, int dtype, void* stream);
+int tb_relu_bwd(const void* x, const void* dy, void* dx, int64_t n, int dtype, void* stream);
+/* Bias-gradient column sums out[n] = sum_m X[m*ld + n], n < ncols, fp32 accumulation in a fixed order.  bf16: plus the lo
+ * plane lo_off elements further when lo_off != 0.  scratch >= tb_colsum_scratch_floats(ncols) floats, and for bf16 at
+ * least tb_colsum_scratch_floats(512).                                                                                  */
+int64_t tb_colsum_scratch_floats(int64_t ncols);
+int tb_colsum_f32(const float* X, float* out, int64_t M, int64_t ncols, int64_t ld, float* scratch, void* stream);
+int tb_colsum_bf16(const void* X, float* out, int64_t M, int64_t ncols, int64_t ld, float* scratch, int64_t lo_off,
+                   void* stream);
+/* Fused policy / baseline heads: logits [N,A] = x Wp^T + bp, baseline [N,V] = x Wb^T + bb, x [N, ldx >= F]; 1 <= A <= 31,
+ * 1 <= V <= 64, F <= 12288.  The backward gives dx [N, lddx] and overwrites dWp, dbp, dWb, dbb, with
+ * tb_heads_scratch_floats(N, F, A, V) floats of scratch, at most 120 * (A + V) * (F + 1) whatever N.                  */
+int64_t tb_heads_scratch_floats(int64_t N, int F, int A, int V);
+int tb_heads_forward(const float* x, int64_t ldx, const float* Wp, const float* bp, const float* Wb, const float* bb, int64_t N,
+                     int F, int A, int V, float* logits, float* baseline, void* stream);
+int tb_heads_backward(const float* x, int64_t ldx, const float* Wp, const float* Wb, const float* dlogits, const float* dbaseline,
+                      int64_t N, int F, int A, int V, float* dx, int64_t lddx, float* dWp, float* dbp, float* dWb, float* dbb,
+                      float* scratch, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -103,6 +103,30 @@ _SIGNATURES = {
     "tb_sw_pool_bwd_image_colsum": ([_vp, _vp, _vp, _i64, _i64, _int, _int, _int, _vp, _vp, _i64, _vp], _int),
     "tb_maxpool3x3s2_fwd_f32": ([_vp, _vp, _vp, _i64, _int, _int, _int, _vp], _int),
     "tb_f32_to_bf16": ([_vp, _vp, _i64, _i64, _i64, _i64, _vp], _int),
+    "tb_gemm_f32": ([_vp, _int, _vp, _int, _int, _int] + [_i64] * 5 + [_vp, _i64, _vp, _int, _vp, _i64, _vp, _i64, _int, _int,
+                                                                        _int, _f32, _int, _vp, _vp], _int),
+    "tb_gemm_f32_splits": ([_i64] * 5, _int),
+    "tb_splitk_scratch_floats": ([], _i64),
+    "tb_im2col_u8_nchw": ([_vp, _vp, _i64] + [_int] * 6 + [_vp], _int),
+    "tb_im2col_f32_nhwc": ([_vp, _vp, _i64] + [_int] * 6 + [_vp], _int),
+    "tb_col2im_f32_nhwc": ([_vp, _vp, _vp, _i64] + [_int] * 6 + [_vp], _int),
+    "tb_permute_pq": ([_vp, _vp, _i64, _int, _int, _vp], _int),
+    "tb_relu_mask_f32": ([_vp, _vp, _i64, _i64, _i64, _i64, _vp], _int),
+    "tb_core_extras": ([_vp, _i64, _i64, _int, _vp, _vp, _int, _vp], _int),
+    "tb_im2col3x3": ([_vp, _vp, _i64, _int, _int, _int, _i64, _int, _int, _vp], _int),
+    "tb_im2col3x3_u8": ([_vp, _vp, _i64, _int, _int, _int, _i64, _int, _vp], _int),
+    "tb_col2im3x3": ([_vp, _vp, _vp, _vp, _i64, _int, _int, _int, _i64, _int, _vp], _int),
+    "tb_maxpool3x3s2_fwd": ([_vp, _vp, _vp, _i64, _int, _int, _int, _int, _vp], _int),
+    "tb_maxpool3x3s2_bwd": ([_vp, _vp, _vp, _i64, _int, _int, _int, _int, _vp], _int),
+    "tb_relu_fwd": ([_vp, _vp, _i64, _int, _vp], _int),
+    "tb_relu_bwd": ([_vp, _vp, _vp, _i64, _int, _vp], _int),
+    "tb_colsum_scratch_floats": ([_i64], _i64),
+    "tb_colsum_f32": ([_vp, _vp, _i64, _i64, _i64, _vp, _vp], _int),
+    "tb_colsum_bf16": ([_vp, _vp, _i64, _i64, _i64, _vp, _i64, _vp], _int),
+    "tb_heads_scratch_floats": ([_i64, _int, _int, _int], _i64),
+    "tb_heads_forward": ([_vp, _i64, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_heads_backward": ([_vp, _i64, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp],
+                          _int),
     "tb_atarinet_param_count": ([_int, _int], _i64),
     "tb_atarinet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
     "tb_atarinet_forward": ([_vp] * 7 + [_i64, _i64, _int, _int, _int] + [_vp] * 6, _int),

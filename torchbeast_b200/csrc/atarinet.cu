@@ -337,7 +337,10 @@ static int atarinet_backward(const float* grad_logits, const float* grad_baselin
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
   if (phases & 1) {
-  // heads: dcore_out = dlogits . Wp + dbaseline . Wb ; dWp, dbp, dWb, dbb
+  // heads: dcore_out = dlogits . Wp + dbaseline . Wb ; dWp, dbp, dWb, dbb.  The partials fit the split-K scratch at every
+  // batch size: their slab count is capped, and the largest heads (A = 31, V = 64, F = 544) fit at the cap.
+  static_assert(int64_t(kHeadsMaxSlabs) * (31 + kHeadsMaxValues) * (G::FC_OUT + 1 + 31 + 1) <= kSplitKScratchFloats,
+                "heads scratch");
   TB_REQUIRE(heads_scratch_floats(N, pp.core, A, V) <= kSplitKScratchFloats, "atarinet_backward: heads scratch too small");
   TB_TRY(heads_backward(w.core_out, pp.core, P + pp.policy_w, P + pp.baseline_w, grad_logits, grad_baseline, N, pp.core, A,
                         w.dcore_out, pp.core, G_ + pp.policy_w, G_ + pp.policy_b, G_ + pp.baseline_w, G_ + pp.baseline_b, w.splitk,

@@ -77,6 +77,10 @@ int gemm_simt(const AT* A, const BT* B, float* C, int64_t M, int64_t N, int64_t 
   if (splits > ktiles) splits = int(ktiles > 0 ? ktiles : 1);
   const bool via_scratch = splits > 1 || ep.permP > 1 || ep.permQ > 1;
   TB_REQUIRE(!via_scratch || splitk_scratch, "gemm: split-K / permuted output needs scratch");
+  // each path applies only part of the epilogue: reject what the chosen one would drop
+  TB_REQUIRE(via_scratch ? !ep.mask && !ep.addend : ep.scale == 1.0f,
+             "gemm: %s epilogue with %s", via_scratch ? "split-K / permuted" : "direct",
+             via_scratch ? "mask / addend (direct path only)" : "scale != 1 (split-K / permuted path only)");
   ProfScope prof(ep.tag, stream);
   GemmArgs g;
   g.A = A; g.B = B; g.C = C; g.M = M; g.N = N; g.K = K; g.lda = lda; g.ldb = ldb; g.ldc = ldc;

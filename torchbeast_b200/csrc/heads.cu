@@ -6,7 +6,7 @@ namespace tb {
 namespace {
 
 constexpr int kMaxOut = 32;   // A < kMaxOut actions
-constexpr int kSlabRows = 64; // rows per partial block of the weight-gradient reduction
+constexpr int kSlabRows = 64; // rows per partial block of the weight-gradient reduction, up to kHeadsMaxSlabs blocks
 constexpr int kFwdSmemFloats = 48 * 1024 / 4;  // the forward's weight stage
 
 // Block = 8 warps x kFwdRowsPerWarp rows each; the (A+V) x F weight matrix is staged in shared memory (the first version
@@ -58,12 +58,12 @@ __global__ void heads_fwd_kernel(const float* __restrict__ x, int64_t ldx, const
   }
 }
 
-// thread per (row, feature)
+// thread per (row, feature); rows on grid.x, which has no 65535 limit
 __global__ void heads_dgrad_kernel(const float* __restrict__ Wp, const float* __restrict__ Wb, const float* __restrict__ dl,
                                    const float* __restrict__ db, int64_t N, int F, int A, int V, float* __restrict__ dx,
                                    int64_t lddx) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t n = blockIdx.y;
+  const int f = blockIdx.y * blockDim.x + threadIdx.x;
+  const int64_t n = blockIdx.x;
   if (f >= F) return;
   float s = __ldg(db + n * V) * __ldg(Wb + f);
   for (int v = 1; v < V; ++v) s = fmaf(__ldg(db + n * V + v), __ldg(Wb + int64_t(v) * F + f), s);
@@ -72,14 +72,17 @@ __global__ void heads_dgrad_kernel(const float* __restrict__ Wp, const float* __
 }
 
 // block (32 x 8): 32 feature columns (column F is the implicit ones column -> bias gradients) x a slab of rows;
-// partial [slab][A+V][F+1]
+// partial [slab][A+V][F+1].  kLong: slabs of `long_rows` rows (N > 64 * kHeadsMaxSlabs), else of kSlabRows, a
+// compile-time bound the short form's loop is scheduled around.
+template <bool kLong>
 __global__ void heads_wgrad_partial_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ dl,
-                                           const float* __restrict__ db, int64_t N, int F, int A, int V,
+                                           const float* __restrict__ db, int64_t N, int F, int A, int V, int64_t long_rows,
                                            float* __restrict__ part) {
   __shared__ float sm[8][33];
+  const int64_t rows = kLong ? long_rows : kSlabRows;
   const int f = blockIdx.x * 32 + threadIdx.x;
-  const int64_t r0 = int64_t(blockIdx.y) * kSlabRows;
-  const int64_t r1 = (r0 + kSlabRows < N) ? r0 + kSlabRows : N;
+  const int64_t r0 = int64_t(blockIdx.y) * rows;
+  const int64_t r1 = (r0 + rows < N) ? r0 + rows : N;
   const int O = A + V, F1 = F + 1;
   for (int o0 = 0; o0 < O; o0 += 8) {
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -153,24 +156,40 @@ int heads_forward(const float* x, int64_t ldx, const float* Wp, const float* bp,
   return check_launch("heads_fwd_kernel");
 }
 
+// Rows per slab: kSlabRows while that takes at most kHeadsMaxSlabs slabs (the bits of every N <= 64 * kHeadsMaxSlabs do
+// not depend on the cap), else the fewest rows that keep the slab count at the cap.
+static int64_t heads_slab_rows(int64_t N) {
+  const int64_t slabs = (N + kSlabRows - 1) / kSlabRows;
+  return slabs <= kHeadsMaxSlabs ? kSlabRows : (N + kHeadsMaxSlabs - 1) / kHeadsMaxSlabs;
+}
+
+static int64_t heads_slabs(int64_t N) {
+  const int64_t rows = heads_slab_rows(N);
+  return (N + rows - 1) / rows;
+}
+
 int64_t heads_scratch_floats(int64_t N, int F, int A, int V) {
-  return ((N + kSlabRows - 1) / kSlabRows) * int64_t(A + V) * (F + 1);
+  return (N > 0 ? heads_slabs(N) : 0) * int64_t(A + V) * (F + 1);
 }
 
 int heads_backward(const float* x, int64_t ldx, const float* Wp, const float* Wb, const float* dlogits, const float* dbaseline,
                    int64_t N, int F, int A, float* dx, int64_t lddx, float* dWp, float* dbp, float* dWb, float* dbb, float* scratch,
                    cudaStream_t stream, int V) {
   TB_REQUIRE(x && Wp && Wb && dlogits && dbaseline && dx && dWp && dbp && dWb && dbb && scratch, "heads_backward: null pointer");
-  TB_REQUIRE(A >= 1 && A < kMaxOut && V >= 1 && V <= kHeadsMaxValues && F >= 1 && N >= 1 &&
-             N < 65536 * int64_t(kSlabRows), "heads_backward: bad sizes");
+  TB_REQUIRE(A >= 1 && A < kMaxOut && V >= 1 && V <= kHeadsMaxValues && F >= 1 && F <= 65535 * 128 && N >= 1 &&
+             N < (int64_t(1) << 31), "heads_backward: bad sizes A=%d V=%d F=%d N=%lld", A, V, F, (long long)N);
   ProfScope prof("heads_bwd", stream);
-  heads_dgrad_kernel<<<dim3((unsigned)((F + 127) / 128), (unsigned)N), 128, 0, stream>>>(Wp, Wb, dlogits, dbaseline, N, F, A, V,
+  heads_dgrad_kernel<<<dim3((unsigned)N, (unsigned)((F + 127) / 128)), 128, 0, stream>>>(Wp, Wb, dlogits, dbaseline, N, F, A, V,
                                                                                          dx, lddx);
   int rc = check_launch("heads_dgrad_kernel");
   if (rc) return rc;
-  const int slabs = int((N + kSlabRows - 1) / kSlabRows);
-  heads_wgrad_partial_kernel<<<dim3((unsigned)((F + 1 + 31) / 32), (unsigned)slabs), dim3(32, 8), 0, stream>>>(
-      x, ldx, dlogits, dbaseline, N, F, A, V, scratch);
+  const int slabs = int(heads_slabs(N));
+  const int64_t rows = heads_slab_rows(N);
+  const dim3 grid((unsigned)((F + 1 + 31) / 32), (unsigned)slabs);
+  if (rows == kSlabRows)
+    heads_wgrad_partial_kernel<false><<<grid, dim3(32, 8), 0, stream>>>(x, ldx, dlogits, dbaseline, N, F, A, V, rows, scratch);
+  else
+    heads_wgrad_partial_kernel<true><<<grid, dim3(32, 8), 0, stream>>>(x, ldx, dlogits, dbaseline, N, F, A, V, rows, scratch);
   rc = check_launch("heads_wgrad_partial_kernel");
   if (rc) return rc;
   const int total = (A + V) * (F + 1);
