@@ -2,9 +2,11 @@
 //   1. mma.sync.m16n8k16 bf16 issue rate per SM (8 / 16 warps, 12 independent accumulators)
 //   2. all-gather cost: 130 CTAs each pulling the same 137 KB from L2 into shared memory (cp.async 16 B vs TMA 2D boxes)
 //   3. store -> remote-poll visibility latency through L2 (one CTA stores, another spins on ld.relaxed.gpu)
-//   0. (printed first) the split kernels' per-warp gather: cp.async vs TMA boxes vs 2-CTA multicast TMA, at 1 .. 132
+//   0. (printed first) the split kernels' per-warp gather: cp.async vs TMA boxes vs 2-CTA multicast TMA vs 1-D bulk copies
+//      of a slice-blocked source (with and without multicast), at 1 .. 132
 //      CTAs, and whether a cooperative launch with 2-CTA clusters is accepted and co-resident at their footprint; then
-//      a reduce-scatter alternative to the backward gather (fp32 pair partials through an L2 ring, fence, flags, 1 KB chunk gather)
+//      a reduce-scatter alternative to the backward gather (fp32 pair partials through an L2 ring, fence, flags, 1 KB chunk gather),
+//      and the backward's k-group gate-gradient load (16-byte cp.async vs 1-D bulk copies of a blocked ring)
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o ubench_lstm ubench_lstm.cu -lcuda
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -131,6 +133,9 @@ __global__ void fence_kernel(uint32_t* buf, int reps, long long* cycles) {
 //   kMode 1: TMA boxes {56 cols, 16 rows, 1, 2 planes}, the CTA loads both row halves itself;
 //   kMode 2: 2-CTA clusters, CTA rank r loads rows [16r, 16r + 16) with .multicast::cluster into both CTAs; a "full"
 //            mbarrier per slot expects both halves, an "empty" one counts this warp and the peer's warp.
+//   kMode 3: as 2, but the source is slice-blocked ([group][warp][row half][plane][16 rows][56], the warp's shared-memory
+//            layout) and each half is ONE 1-D cp.async.bulk of a contiguous 3,584-byte block, multicast to the pair;
+//   kMode 4: the slice-blocked source, the CTA loads both halves itself with two 1-D bulk copies (no cluster).
 constexpr int kGWarps = 11, kGRowE = 56;
 constexpr uint32_t kGHalf = 2 * 16 * kGRowE * 2;     // one box: 2 planes x 16 rows x 112 B
 constexpr uint32_t kGSlot = 2 * kGHalf;              // both row halves
@@ -143,24 +148,26 @@ __device__ __forceinline__ void g_cluster_sync() {
 }
 template <int kMode>
 __global__ void __launch_bounds__(kGWarps * 32, 1) gather_split_kernel(const __grid_constant__ CUtensorMap tm, const __nv_bfloat16* __restrict__ src,
-                                                                       int hq, int groups, int reps, long long* cycles, uint32_t* sink) {
+                                                                       const uint8_t* __restrict__ blk, int hq, int groups, int reps,
+                                                                       long long* cycles, uint32_t* sink) {
+  constexpr bool kPair = kMode == 2 || kMode == 3;
   extern __shared__ __align__(128) uint8_t sm[];
   __shared__ __align__(8) uint64_t bars[kGWarps][4];   // full[2], empty[2]
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   uint32_t rank = 0;
-  if (kMode == 2) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+  if (kPair) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
   const uint32_t xs = (uint32_t)__cvta_generic_to_shared(sm) + w * 2 * kGSlot;
   const uint32_t full0 = (uint32_t)__cvta_generic_to_shared(&bars[w][0]), empty0 = full0 + 16;
   if (lane == 0) {
     for (int i = 0; i < 2; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(full0 + 8 * i) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty0 + 8 * i), "r"(kMode == 2 ? 2 : 1) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty0 + 8 * i), "r"(kPair ? 2 : 1) : "memory");
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (kMode == 2) g_cluster_sync(); else __syncthreads();
+  if (kPair) g_cluster_sync(); else __syncthreads();
   uint32_t peer_empty0 = 0;
-  if (kMode == 2) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer_empty0) : "r"(empty0), "r"(rank ^ 1u));
+  if (kPair) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer_empty0) : "r"(empty0), "r"(rank ^ 1u));
   const int total = reps * groups;
   auto issue = [&](int n) {   // group n of the stream -> slot n & 1
     const int slot = n & 1, g = n % groups;
@@ -180,8 +187,15 @@ __global__ void __launch_bounds__(kGWarps * 32, 1) gather_split_kernel(const __g
     if (n >= 2) g_wait(empty0 + 8 * slot, ((n >> 1) - 1) & 1);
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(full), "r"(kGSlot) : "memory");
     for (int h = 0; h < 2; ++h) {
-      if (kMode == 2 && h != int(rank)) continue;
-      if (kMode == 2)
+      if (kPair && h != int(rank)) continue;
+      const uint8_t* b = blk + (size_t(g) * kGWarps + w) * kGSlot + h * kGHalf;
+      if (kMode == 3)
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
+                     ::"r"(dst + h * kGHalf), "l"(b), "r"(kGHalf), "r"(full), "h"((uint16_t)3) : "memory");
+      else if (kMode == 4)
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     ::"r"(dst + h * kGHalf), "l"(b), "r"(kGHalf), "r"(full) : "memory");
+      else if (kMode == 2)
         asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
                      ::"r"(dst + h * kGHalf), "l"(reinterpret_cast<uint64_t>(&tm)), "r"(full), "r"(w * 48), "r"(16 * h), "r"(g), "r"(0), "h"((uint16_t)3)
                      : "memory");
@@ -208,13 +222,13 @@ __global__ void __launch_bounds__(kGWarps * 32, 1) gather_split_kernel(const __g
     __syncwarp();
     if (kMode != 0 && lane == 0) {
       asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(empty0 + 8 * slot) : "memory");
-      if (kMode == 2)
+      if (kPair)
         asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(peer_empty0 + 8 * slot) : "memory");
     }
     if (n + 2 < total) issue(n + 2);
   }
   long long t1 = clock64();
-  if (kMode == 2) g_cluster_sync();
+  if (kPair) g_cluster_sync();
   if (lane == 0) atomicMax(reinterpret_cast<unsigned long long*>(cycles + blockIdx.x), (unsigned long long)(t1 - t0));
   if (threadIdx.x == 0) sink[blockIdx.x] = acc;
 }
@@ -354,8 +368,89 @@ static int rs_exchange() {
   return 0;
 }
 
+// ---- the split backward's k-group gate-gradient load at H = 519, B = 32: 132 CTAs, the CTAs of k-group w = cta / 12 (11
+// groups) each load the group's 48 columns x 4 gates x 2 planes x 32 rows (24 KB of slice bytes) into the tile layout
+// [gate][row half][plane][16 rows][56] and wait for them, once per step.
+//   kMode 0: from [plane][gate][row][Hq] planes, 6 16-byte cp.async per (gate, plane, row): 1,536 copies;
+//   kMode 1: from a k-group-blocked ring already in the tile layout, one 1-D cp.async.bulk per gate (4 x 7 KB) on an mbarrier.
+constexpr int kBgHq = 528, kBgGateB = 4 * 16 * kGRowE * 2, kBgGroupB = 4 * kBgGateB;
+template <int kMode>
+__global__ void __launch_bounds__(kGWarps * 32, 1) bwd_group_load_kernel(const __nv_bfloat16* __restrict__ dgq, const uint8_t* __restrict__ blk,
+                                                                         int reps, long long* cycles, uint32_t* sink) {
+  extern __shared__ __align__(128) uint8_t sm[];
+  __shared__ __align__(8) uint64_t bar;
+  const int tid = threadIdx.x, w = blockIdx.x / 12, ks0 = 3 * w;
+  const uint32_t xs = (uint32_t)__cvta_generic_to_shared(sm), b = (uint32_t)__cvta_generic_to_shared(&bar);
+  if (tid == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(b) : "memory");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  uint32_t acc = 0;
+  const long long t0 = clock64();
+  for (int r = 0; r < reps; ++r) {
+    if (kMode == 0) {
+      const size_t gs = size_t(32) * kBgHq, lo = 4 * gs;
+      for (int i = tid; i < 4 * 2 * 32 * 6; i += blockDim.x) {
+        const int c = i % 6, row = (i / 6) % 32, pl = (i / (6 * 32)) & 1, g = i / (12 * 32);
+        const uint32_t d = xs + 2 * (g * 2 * 2 * 16 * kGRowE + (row >> 4) * 2 * 16 * kGRowE + pl * 16 * kGRowE + (row & 15) * kGRowE + c * 8);
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(dgq + (pl ? lo : 0) + g * gs + size_t(row) * kBgHq + ks0 * 16 + c * 8)
+                     : "memory");
+      }
+      asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+    } else {
+      if (tid == 0) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(uint32_t(kBgGroupB)) : "memory");
+        for (int g = 0; g < 4; ++g)
+          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                       ::"r"(xs + g * kBgGateB), "l"(blk + size_t(w) * kBgGroupB + g * kBgGateB), "r"(kBgGateB), "r"(b) : "memory");
+      }
+      g_wait(b, uint32_t(r & 1));
+    }
+    __syncthreads();
+    acc += reinterpret_cast<const uint32_t*>(sm)[tid];
+    __syncthreads();
+  }
+  const long long t1 = clock64();
+  if (tid == 0) { cycles[blockIdx.x] = t1 - t0; sink[blockIdx.x] = acc; }
+}
+
+static int bwd_group_load() {
+  const int reps = 400, grid = 132;
+  const size_t smem = size_t(kBgGroupB) + 9 * 1024;   // the group tiles + the kernel's other dynamic shared memory
+  __nv_bfloat16* dgq; uint8_t* blk; long long* cyc; uint32_t* sink;
+  CK(cudaMalloc(&dgq, size_t(2) * 4 * 32 * kBgHq * 2)); CK(cudaMemset(dgq, 0, size_t(2) * 4 * 32 * kBgHq * 2));
+  CK(cudaMalloc(&blk, size_t(11) * kBgGroupB)); CK(cudaMemset(blk, 0, size_t(11) * kBgGroupB));
+  CK(cudaMalloc(&cyc, grid * sizeof(long long))); CK(cudaMalloc(&sink, grid * 4));
+  CK(cudaFuncSetAttribute(bwd_group_load_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  CK(cudaFuncSetAttribute(bwd_group_load_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  std::vector<long long> h(grid);
+  for (int mode = 0; mode < 2; ++mode) {
+    for (int run = 0; run < 2; ++run) {   // run 0 warms up
+      if (mode == 0) bwd_group_load_kernel<0><<<grid, kGWarps * 32, smem>>>(dgq, blk, reps, cyc, sink);
+      else bwd_group_load_kernel<1><<<grid, kGWarps * 32, smem>>>(dgq, blk, reps, cyc, sink);
+      CK(cudaGetLastError());
+      CK(cudaDeviceSynchronize());
+    }
+    CK(cudaMemcpy(h.data(), cyc, grid * sizeof(long long), cudaMemcpyDeviceToHost));
+    long long mx = 0; for (int i = 0; i < grid; ++i) mx = h[i] > mx ? h[i] : mx;
+    printf("backward group load %-28s: %d CTAs, 24.0 KB slice bytes/CTA/step: %6.0f cycles/step (max CTA)\n",
+           mode == 0 ? "1536 x 16-byte cp.async" : "4 x 7 KB 1-D bulk (blocked)", grid, double(mx) / reps);
+  }
+  CK(cudaFree(dgq)); CK(cudaFree(blk)); CK(cudaFree(cyc)); CK(cudaFree(sink));
+  return 0;
+}
+
 typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                              const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+template <int kMode>
+static cudaError_t launch_split(cudaLaunchConfig_t& cfg, size_t smem, const CUtensorMap& tm, const __nv_bfloat16* src, const uint8_t* blk,
+                                int hq, int groups, int reps, long long* cyc, uint32_t* sink) {
+  cudaError_t e = cudaFuncSetAttribute(gather_split_kernel<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+  if (e == cudaSuccess) e = cudaLaunchKernelEx(&cfg, gather_split_kernel<kMode>, tm, src, blk, hq, groups, reps, cyc, sink);
+  return e;
+}
 
 static int split_gather(EncodeFn enc) {
   const int hq = 528, reps = 400;
@@ -363,7 +458,10 @@ static int split_gather(EncodeFn enc) {
   uint32_t* sink; CK(cudaMalloc(&sink, 4096));
   __nv_bfloat16* src; const size_t elems = size_t(2) * 4 * 32 * hq;   // [plane][group][row][hq]
   CK(cudaMalloc(&src, elems * 2)); CK(cudaMemset(src, 0, elems * 2));
+  uint8_t* blk; const size_t blk_bytes = size_t(4) * kGWarps * kGSlot;   // [group][warp][row half][plane][16][56]
+  CK(cudaMalloc(&blk, blk_bytes)); CK(cudaMemset(blk, 0, blk_bytes));
   std::vector<long long> h(256);
+  static const char* names[5] = {"cp.async", "TMA", "mc TMA", "mc bulk1D", "bulk1D"};
   for (int groups : {2, 4}) {
     CUtensorMap tm;
     cuuint64_t gd[4] = {cuuint64_t(hq), 32, cuuint64_t(groups), 2};
@@ -374,28 +472,31 @@ static int split_gather(EncodeFn enc) {
     if (r != CUDA_SUCCESS) { printf("encode failed %d\n", int(r)); return 1; }
     const size_t smem = size_t(kGWarps) * 2 * kGSlot;
     const double useful = double(groups) * 2 * 32 * kGWarps * 48 * 2;   // slice bytes per CTA per step
+    const double landed = useful * kGRowE / 48;                           // bytes written into each CTA's shared memory
     for (int ctas : {1, 65, 130, 132}) {
-      for (int mode = 0; mode < 3; ++mode) {
-        const int n = (mode == 2) ? (ctas + 1) & ~1 : ctas;
+      for (int mode = 0; mode < 5; ++mode) {
+        const bool pair = mode == 2 || mode == 3;
+        const int n = pair ? (ctas + 1) & ~1 : ctas;
         CK(cudaMemset(cyc, 0, 256 * sizeof(long long)));
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(n); cfg.blockDim = dim3(kGWarps * 32); cfg.dynamicSmemBytes = smem;
         cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2;
         at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = mode == 2 ? 1 : 0;
-        if (mode == 0) { CK(cudaFuncSetAttribute(gather_split_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-                         CK(cudaLaunchKernelEx(&cfg, gather_split_kernel<0>, tm, (const __nv_bfloat16*)src, hq, groups, reps, cyc, sink)); }
-        if (mode == 1) { CK(cudaFuncSetAttribute(gather_split_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-                         CK(cudaLaunchKernelEx(&cfg, gather_split_kernel<1>, tm, (const __nv_bfloat16*)src, hq, groups, reps, cyc, sink)); }
-        if (mode == 2) { CK(cudaFuncSetAttribute(gather_split_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-                         CK(cudaLaunchKernelEx(&cfg, gather_split_kernel<2>, tm, (const __nv_bfloat16*)src, hq, groups, reps, cyc, sink)); }
+        cfg.attrs = at; cfg.numAttrs = pair ? 1 : 0;
+        const __nv_bfloat16* sp = src;
+        if (mode == 0) CK(launch_split<0>(cfg, smem, tm, sp, blk, hq, groups, reps, cyc, sink));
+        if (mode == 1) CK(launch_split<1>(cfg, smem, tm, sp, blk, hq, groups, reps, cyc, sink));
+        if (mode == 2) CK(launch_split<2>(cfg, smem, tm, sp, blk, hq, groups, reps, cyc, sink));
+        if (mode == 3) CK(launch_split<3>(cfg, smem, tm, sp, blk, hq, groups, reps, cyc, sink));
+        if (mode == 4) CK(launch_split<4>(cfg, smem, tm, sp, blk, hq, groups, reps, cyc, sink));
         CK(cudaDeviceSynchronize());
         CK(cudaMemcpy(h.data(), cyc, n * sizeof(long long), cudaMemcpyDeviceToHost));
         long long mx = 0; for (int i = 0; i < n; ++i) mx = h[i] > mx ? h[i] : mx;
         const double cps = double(mx) / reps;
-        printf("split gather %-9s: %3d CTAs, %5.1f KB slice bytes/CTA/step: %7.0f cycles/step (max CTA), %5.1f B/clk/SM, chip %6.0f B/clk read from L2\n",
-               mode == 0 ? "cp.async" : mode == 1 ? "TMA" : "multicast", n, useful / 1024.0, cps, useful / cps,
-               n * (mode == 0 ? useful : mode == 1 ? useful * kGRowE / 48 : useful * kGRowE / 48 / 2) / cps);
+        printf("split gather %-9s: %3d CTAs, %5.1f KB slice bytes (%5.1f KB landed)/CTA/step: %7.0f cycles/step (max CTA), %5.1f B/clk/SM, "
+               "chip %6.0f B/clk read from L2\n",
+               names[mode], n, useful / 1024.0, landed / 1024.0, cps, useful / cps,
+               n * (mode == 0 ? useful : pair ? landed / 2 : landed) / cps);
       }
     }
   }
@@ -432,11 +533,11 @@ static int split_gather(EncodeFn enc) {
 int main() {
   {
     cudaDeviceProp prop; cudaGetDeviceProperties(&prop, 0);
-    printf("device %s, %d SMs\n", prop.name, prop.multiProcessorCount);
-    EncodeFn enc = nullptr; cudaDriverEntryPointQueryResult q;
+    printf("device %s, %d SMs\n", prop.name, prop.multiProcessorCount);    EncodeFn enc = nullptr; cudaDriverEntryPointQueryResult q;
     CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&enc, cudaEnableDefault, &q));
     if (split_gather(enc)) return 1;
     if (rs_exchange()) return 1;
+    if (bwd_group_load()) return 1;
   }
   int clk = 0;
   cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);

@@ -54,6 +54,9 @@ static inline int64_t ld16(int64_t n) { return (n + 7) & ~int64_t(7); }
 static inline int mma_hq(int H) { return ((H + 15) & ~15) + 8; }
 static unsigned wave_bwd_split_role_ctas(int H);
 static int wave_bwd_split_groups(int H);
+static bool wave_split_shape(int64_t B, int In, int H);
+static int64_t wave_split_hx_elems(int64_t T1);
+static int64_t wave_split_dgx_elems(int H);
 
 size_t lstm_ws_bytes(int64_t T1, int64_t B, int In, int H, int layers, int precision) {
   return lstm_ws(nullptr, T1, B, In, H, layers, precision).bytes;
@@ -78,6 +81,7 @@ LstmWs lstm_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int
       L.xb = L.wihb = L.dgb = L.hmb = L.hmq = L.dgq = L.hq = nullptr;
       L.xb_lo = L.wihb_lo = L.dgb_lo = L.hmb_lo = L.hq_lo = L.hmq_lo = L.dgq_lo = 0;
       L.gact = L.csb = nullptr;
+      L.hx = L.dgx = nullptr;
       if (precision) {  // bf16 operand copies (2 bytes per element: take half the float count, rounded up)
         const int64_t in_l = (l == 0) ? In : H;
         // precision 2 (split-bf16): every GEMM operand also has a lo plane right behind its hi plane
@@ -94,6 +98,10 @@ LstmWs lstm_ws(void* base, int64_t T1, int64_t B, int In, int H, int layers, int
         if (precision == 2) {
           const int64_t nC4 = (H + 3) / 4;
           L.gact = takef(T1 * nC4 * 512); L.csb = takef((T1 + 1) * nC4 * 128);
+          if (layers == 2 && wave_split_shape(B, In, H)) {
+            L.hx = takef((wave_split_hx_elems(T1) + 1) / 2);
+            L.dgx = takef((wave_split_dgx_elems(H) + 1) / 2);
+          }
         }
       }
     } else {
@@ -1721,9 +1729,9 @@ __global__ void lstm_init_state_q_kernel(const float* __restrict__ h0, const flo
 // measures the mma.sync, gather and hand-off rates this layout is built around):
 //   * 11 MMA warps x 3 k16-steps cover K = 528 exactly (33 k-steps): no padded k-steps, weights of all three
 //     matrices as hi AND lo B fragments in registers (72 per thread) for all steps;
-//   * h is exchanged as two bf16 planes (hq: raw h, slot t+1 = h_t) written with 8-byte stores (4 units x
-//     bf16 of one row and plane) and pulled per warp as TMA boxes of its 48 (+8) columns; the CTAs run as 2-CTA
-//     clusters and each CTA of a pair loads one 16-row half and multicasts it, so the pair reads each tile once;
+//   * h is exchanged as two bf16 planes (hx: raw h, slot t+1 = h_t) written with 8-byte stores (4 units x
+//     bf16 of one row and plane) into a slice-blocked layout, and pulled per warp as one 1-D bulk copy of its
+//     48 (+8) columns of all rows and both planes;
 //   * the cell state lives in a register of the thread that owns (layer, unit, row) for all steps;
 //   * the grid barrier is per-CTA FLAGS instead of one contended counter: producer = stores, bar.sync,
 //     fence.acq_rel.gpu, st flag[cta] = step; consumers = one thread per producer
@@ -1748,6 +1756,7 @@ struct WaveFwdSplitArgs {
   float* y;                 // layer-1 output [T1*B, H] (the heads' input)
   float* hN; float* cN;     // [2, B, H] final state
   __nv_bfloat16* hq[2];     // raw h planes [(T1+1)*B, Hq] (+ hq_lo): slot 0 = initial state, slot t+1 = h_t
+  __nv_bfloat16* hx[2];     // the same h, slice-blocked for the exchange: [T1+1][kXSlotE] (hx_index), zeroed before launch
   __nv_bfloat16* hmq[2];    // masked recurrent inputs [T1*B, Hq] (+ hmq_lo): operand of the weight-gradient GEMMs
   int64_t hq_lo, hmq_lo;
   const float* nd; unsigned* flags;
@@ -1761,57 +1770,35 @@ __device__ __forceinline__ void split_pack(float v0, float v1, uint32_t& hi, uin
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+// hi / lo bf16 of v in this lane and the next three (4 adjacent units of one row), packed for one 8-byte store per plane:
+// valid in the first lane of each group of 4; every lane of the warp must take part
+__device__ __forceinline__ void split_pack4(float v, uint32_t& ph, uint32_t& pl, uint32_t& ph2, uint32_t& pl2) {
+  const __nv_bfloat16 hh = __float2bfloat16_rn(v);
+  const __nv_bfloat16 hl = __float2bfloat16_rn(v - __bfloat162float(hh));
+  const uint32_t vh = uint32_t(__bfloat16_as_ushort(hh)), vl = uint32_t(__bfloat16_as_ushort(hl));
+  ph = vh | (__shfl_down_sync(0xffffffffu, vh, 1) << 16); pl = vl | (__shfl_down_sync(0xffffffffu, vl, 1) << 16);
+  ph2 = __shfl_down_sync(0xffffffffu, ph, 2); pl2 = __shfl_down_sync(0xffffffffu, pl, 2);
+}
 __device__ __forceinline__ void st_relaxed_u32(unsigned* p, unsigned v) {
   asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
-// ---- 2-CTA cluster tile exchange of the split kernels: each CTA of a pair loads one 16-row half of every tile box and
-// multicasts it into both CTAs' shared memory (halves the L2 -> SM traffic of the all-gather: tools/ubench/ubench_lstm.cu)
+// ---- tile exchange of the split kernels: each warp's tile of one step is [row half][hi, lo][16 rows][kTileRowE]
 constexpr int kTileRowE = kSplitK * 16 + 8;     // elements per tile row: a warp's 48 columns + 8 (112 B: conflict-free ldmatrix)
-constexpr int kHalfE = 2 * 16 * kTileRowE;      // one box: [hi, lo][16 rows][kTileRowE]
+constexpr int kHalfE = 2 * 16 * kTileRowE;      // one row half of a tile: [hi, lo][16 rows][kTileRowE]
 constexpr uint32_t kSlotBytes = 2 * kHalfE * 2; // both row halves of one tile slot
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// the peer CTA's copy of a local shared-memory mbarrier
-__device__ __forceinline__ uint32_t peer_addr(const void* p, uint32_t peer) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(peer));
-  return r;
+constexpr int kXSlotE = kSplitWarps * 2 * kHalfE; // one time slot of the h exchange buffer (see lstm2_fwd_wave_split_kernel)
+static int64_t wave_split_hx_elems(int64_t T1) { return (T1 + 1) * kXSlotE; }
+// element of (row r < 32, unit k < kSplitWarps * 48, plane) in one slot of the h exchange buffer
+__host__ __device__ __forceinline__ int hx_index(int r, int k, int plane) {
+  const int w = k / (kSplitK * 16);
+  return w * 2 * kHalfE + (r >> 4) * kHalfE + plane * 16 * kTileRowE + (r & 15) * kTileRowE + (k - w * kSplitK * 16);
 }
 __device__ __forceinline__ void mbar_arrive_local(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
-// wait on an mbarrier phase that the peer CTA's warp also arrives on (acquire at cluster scope)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "LAB_WAIT_%=:\n"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra LAB_DONE_%=;\n"
-      "bra LAB_WAIT_%=;\n"
-      "LAB_DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// generic-proxy global writes (h / gate-gradient stores) vs the TMA reads of the same bytes
+// generic-proxy global writes (h / gate-gradient stores) vs the bulk-copy / TMA reads of the same bytes
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-// one box of a rank-4 map into the same shared-memory offset of both CTAs of the pair; completes tx on the
-// mbarrier at `bar`'s offset in each of them
-__device__ __forceinline__ void tma_multicast_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(
-          smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"((uint16_t)3)
-      : "memory");
-}
-// 128-byte aligned start of the dynamic shared memory (TMA destinations); the kernels request 128 bytes of slack
+// 128-byte aligned start of the dynamic shared memory (bulk-copy destinations); the kernels request 128 bytes of slack
 __device__ __forceinline__ unsigned char* smem_align128(unsigned char* p) {
   return p + ((128u - (smem_u32(p) & 127u)) & 127u);
 }
@@ -1824,30 +1811,30 @@ __device__ __forceinline__ void mma3(float (&c)[4], const uint32_t (&ah)[4], con
   mma_bf16_16816(c, ah, bh0, bh1);
 }
 
-// hq_map[l]: the hq planes of layer l as a rank-4 map {Hq, B, T1 + 1, plane}, box {kTileRowE, 16, 1, 2}: rows >= B and
-// columns >= Hq are zero-filled.  Launched as 2-CTA clusters; a padding CTA (index >= a.nctas, all units past H) only
-// takes part in the loads.
-__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(const __grid_constant__ CUtensorMap hq_map0,
-                                                                               const __grid_constant__ CUtensorMap hq_map1,
-                                                                               WaveFwdSplitArgs a) {
+// The h exchange buffer hx[l] of layer l is slice-blocked: [slot t+1][warp slice w < kSplitWarps][row half][hi, lo]
+// [16 rows][kTileRowE] (hx_index), so that one warp's tile of one slot - its 48 columns (+ 8 never read) of all 32 rows,
+// both planes - is one contiguous, 128-byte aligned 7 KB block, byte for byte the warp's shared-memory tile, fetched with
+// ONE 1-D cp.async.bulk.  (The plain hq rows, boxed by TMA, cost 112-byte rows at a 1,072-byte pitch, most of them
+// straddling two lines; multicasting the halves to a CTA pair halved the L2 reads but the multicast copy itself runs at
+// ~25 B/clk/SM: tools/ubench/ubench_lstm.cu, DESIGN.md "LSTM recurrence".)  The buffer is zeroed before the launch, so
+// rows >= B and units past 4 * nctas - never written - are zero.
+__global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(WaveFwdSplitArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   unsigned char* const smem_b = smem_align128(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
   const int H = a.H, Hq = a.Hq, B = a.B;
-  const bool idle = blockIdx.x >= a.nctas;
-  // warp-private tiles [group: h0, h1][row half = CTA rank that loads it][hi, lo][16 rows][kTileRowE] of this warp's 48 columns
+  // warp-private tiles [group: h0, h1][row half][hi, lo][16 rows][kTileRowE] of this warp's 48 columns
   __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_b) + int64_t(wrp) * 4 * kHalfE;
   typedef float PartT[2][16][33];
   PartT* part = reinterpret_cast<PartT*>(smem_b + size_t(kSplitWarps) * 2 * kSlotBytes);  // [11 warps][set][col][row]
   __shared__ float act_s[2][4][kStepUnits][33];
-  // per warp: full[group] (this CTA's expect_tx, both CTAs' bytes), empty (this warp + the peer CTA's warp done reading)
+  // per warp: full[group] (the tile's bytes have landed), empty (this warp is done reading the step's tiles)
   __shared__ __align__(8) uint64_t full_s[kSplitWarps][2], empty_s[kSplitWarps];
-  const uint32_t rank = cluster_rank();
   if (lane == 0) {
-    mbar_init(&full_s[wrp][0], 1); mbar_init(&full_s[wrp][1], 1); mbar_init(&empty_s[wrp], 2);
+    mbar_init(&full_s[wrp][0], 1); mbar_init(&full_s[wrp][1], 1); mbar_init(&empty_s[wrp], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  const uint32_t peer_empty = peer_addr(&empty_s[wrp], rank ^ 1u);
+  __syncthreads();
   const int j0 = blockIdx.x * kStepUnits;
   const int rows = (B < 32) ? B : 32;
   const int ksteps = (H + 15) / 16;
@@ -1888,11 +1875,8 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
   const int ul = tid >> 7, ur = (tid & 127) >> 2, uu = tid & 3;
   const bool updrole = updthread && ur < rows && j0 + uu < H;
   float* const csb_u = ul ? a.csb[1] : a.csb[0];
-  __nv_bfloat16* const hq_u = ul ? a.hq[1] : a.hq[0];
-  __nv_bfloat16* const hmq_u = ul ? a.hmq[1] : a.hmq[0];
   float c_state = updrole ? a.c0[(int64_t(ul) * B + ur) * H + j0 + uu] : 0.f;  // c_{t-1} of this (layer, row, unit)
-  if (updthread && !idle) csb_u[int64_t(blockIdx.x) * 128 + (tid & 127)] = c_state;    // slot 0
-  cluster_sync_all();   // the peer's mbarriers are initialised before any multicast or remote arrive
+  if (updthread) csb_u[int64_t(blockIdx.x) * 128 + (tid & 127)] = c_state;    // slot 0
   for (int s = 0; s <= a.T1; ++s) {
     const bool act0 = (s < a.T1), act1 = (s >= 1);
     // inputs that do not depend on other CTAs: issued before the wait
@@ -1910,9 +1894,8 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
     }
     // Every tile element is consumed by exactly ONE warp (K is split across the warps), so each warp waits only for the
     // CTAs that produce ITS k-range (units [16*ks0, 16*ks0 + 48) -> 12 producer CTAs) and fetches its own columns of the
-    // four planes - no block-wide barrier between the hand-off and the products.  The same warp of the peer CTA needs the
-    // same columns: each loads one 16-row half and multicasts it to both.  (History: 130 threads per CTA polling 130
-    // flag words - 17 k pollers chip-wide on 5 cache lines - made the L2 slices of those lines the bottleneck: ncu
+    // four planes - no block-wide barrier between the hand-off and the products.  (History: 130 threads per CTA polling
+    // 130 flag words - 17 k pollers chip-wide on 5 cache lines - made the L2 slices of those lines the bottleneck: ncu
     // showed over a third of all samples in the spin.)
     if (s > 0) {
       const int p0 = (ks0 * 16) / kStepUnits + lane;                   // producer CTA of this lane
@@ -1927,12 +1910,13 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
     if (lane == 0) {
       // Two groups: the h0 planes first, so the layer-0 / input-projection MMAs start while the h1 planes land.  At s = 0
       // the h1 group (slot 0) is loaded but not used, which keeps one phase per step on every barrier.
-      if (s > 0) mbar_wait_cluster(&empty_s[wrp], (s - 1) & 1);   // both CTAs' warps have read step s-1's tiles
+      if (s > 0) mbar_wait(&empty_s[wrp], (s - 1) & 1);   // this warp has read step s-1's tiles
       fence_proxy_async_global();
+      const int64_t blk = int64_t(wrp) * 2 * kHalfE;
       mbar_expect_tx(&full_s[wrp][0], kSlotBytes);
-      tma_multicast_4d(X + rank * kHalfE, &hq_map0, &full_s[wrp][0], ks0 * 16, 16 * int(rank), s, 0);
+      bulk_g2s(X, a.hx[0] + int64_t(s) * kXSlotE + blk, kSlotBytes, &full_s[wrp][0]);
       mbar_expect_tx(&full_s[wrp][1], kSlotBytes);
-      tma_multicast_4d(X + (2 + rank) * kHalfE, &hq_map1, &full_s[wrp][1], ks0 * 16, 16 * int(rank), s > 0 ? s - 1 : 0, 0);
+      bulk_g2s(X + 2 * kHalfE, a.hx[1] + int64_t(s > 0 ? s - 1 : 0) * kXSlotE + blk, kSlotBytes, &full_s[wrp][1]);
     }
     float m0[2][2], m1[2][2];   // done masks of this thread's accumulator rows (layer 0 at t = s, layer 1 at t = s-1)
 #pragma unroll
@@ -1956,7 +1940,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       for (int sk = 0; sk < kSplitK; ++sk) {
         if (ks0 + sk < ksteps) {
 #pragma unroll
-          for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = the row half CTA rank mt loaded
+          for (int mt = 0; mt < 2; ++mt) {   // m16 tile mt = row half mt
             uint32_t ah[4], al[4];
             const int off = mt * kHalfE + (lane & 15) * kTileRowE + sk * 16 + (lane >> 4) * 8;
             ldmatrix_x4(ah, X + off);
@@ -1990,10 +1974,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
         }
       }
       __syncwarp();
-      if (lane == 0) {   // this warp's tiles are read: free them for both loaders of step s+1
-        mbar_arrive_local(&empty_s[wrp]);
-        mbar_arrive_remote(peer_empty);
-      }
+      if (lane == 0) mbar_arrive_local(&empty_s[wrp]);   // this warp's tiles are read: free them for step s+1's loads
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         const int r = mt * 16 + (lane >> 2);
@@ -2041,44 +2022,45 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
         h_new = og * tanhf(c_new);
         c_state = c_new;
       }
-      // publish raw h_t: the 4 units of a row sit in 4 adjacent lanes -> one 8-byte store per (row, plane)
-      const bool live = (ul ? act1 : act0);
-      const __nv_bfloat16 hh = __float2bfloat16_rn(h_new);
-      const __nv_bfloat16 hl = __float2bfloat16_rn(h_new - __bfloat162float(hh));
-      const uint32_t vh = uint32_t(__bfloat16_as_ushort(hh)), vl = uint32_t(__bfloat16_as_ushort(hl));
-      const uint32_t ph = vh | (__shfl_down_sync(0xffffffffu, vh, 1) << 16), pl = vl | (__shfl_down_sync(0xffffffffu, vl, 1) << 16);
-      const uint32_t ph2 = __shfl_down_sync(0xffffffffu, ph, 2), pl2 = __shfl_down_sync(0xffffffffu, pl, 2);
-      if (live && !idle && uu == 0 && ur < rows) {
-        __nv_bfloat16* d = hq_u + (int64_t(tu + 1) * B + ur) * Hq + j0;
+    }
+    // publish raw h_t into the exchange buffer: the 4 units of a row sit in 4 adjacent lanes -> one 8-byte store per
+    // (row, plane).  The plain hq rows, which only the GEMMs after the kernel read, are stored after the flag.
+    const bool live = (ul ? act1 : act0) && uu == 0 && ur < rows;
+    if (updthread) {
+      uint32_t ph, pl, ph2, pl2;
+      split_pack4(h_new, ph, pl, ph2, pl2);
+      if (live) {
+        __nv_bfloat16* d = (ul ? a.hx[1] : a.hx[0]) + int64_t(tu + 1) * kXSlotE + hx_index(ur, j0, 0);
         *reinterpret_cast<uint2*>(d) = make_uint2(ph, ph2);
-        *reinterpret_cast<uint2*>(d + a.hq_lo) = make_uint2(pl, pl2);
-        fence_proxy_async_global();   // consumers read h through TMA
+        *reinterpret_cast<uint2*>(d + 16 * kTileRowE) = make_uint2(pl, pl2);
+        fence_proxy_async_global();   // consumers read h through bulk copies
       }
     }
     __syncthreads();
-    if (tid == 0 && s < a.T1 && !idle) {
+    if (tid == 0 && s < a.T1) {
       asm volatile("fence.acq_rel.gpu;" ::: "memory");
       st_relaxed_u32(a.flags + blockIdx.x * kFlagStride, unsigned(s + 1));
     }
     // ---- everything below is consumed by this CTA or after the kernel: off the critical path ----
     // activated gates -> CTA-blocked [row][16] tiles, straight from act_s (rewritten only after the next step's barrier)
-    for (int idx = tid; idx < 1024 && !idle; idx += kSplitThreads) {
+    for (int idx = tid; idx < 1024; idx += kSplitThreads) {
       const int l = idx >> 9, e = idx & 511, row = e >> 4, c = e & 15;
       const int tl = s - l;
       if ((l ? act1 : act0) && row < rows)
         a.gact[l][(int64_t(tl) * a.nctas + blockIdx.x) * 512 + e] = act_s[l][c >> 2][c & 3][row];
     }
-    if (updthread && !idle) {
+    if (updthread) {
+      uint32_t ph, pl, ph2, pl2;
+      split_pack4(h_new, ph, pl, ph2, pl2);
+      if (live) {   // raw h_t rows: the weight-gradient GEMMs' operand and layer 1's input
+        __nv_bfloat16* d = (ul ? a.hq[1] : a.hq[0]) + (int64_t(tu + 1) * B + ur) * Hq + j0;
+        *reinterpret_cast<uint2*>(d) = make_uint2(ph, ph2);
+        *reinterpret_cast<uint2*>(d + a.hq_lo) = make_uint2(pl, pl2);
+      }
       // masked recurrent input of the NEXT step (h_t * notdone_{t+1}) for the weight-gradient GEMMs, as hi / lo planes
-      const float hm = h_new * nd_n;
-      const __nv_bfloat16 mh = __float2bfloat16_rn(hm);
-      const __nv_bfloat16 ml = __float2bfloat16_rn(hm - __bfloat162float(mh));
-      const uint32_t vh = uint32_t(__bfloat16_as_ushort(mh)), vl = uint32_t(__bfloat16_as_ushort(ml));
-      const uint32_t ph = vh | (__shfl_down_sync(0xffffffffu, vh, 1) << 16), pl = vl | (__shfl_down_sync(0xffffffffu, vl, 1) << 16);
-      const uint32_t ph2 = __shfl_down_sync(0xffffffffu, ph, 2), pl2 = __shfl_down_sync(0xffffffffu, pl, 2);
-      const bool live = (ul ? act1 : act0) && tu < a.T1 - 1;
-      if (live && uu == 0 && ur < rows) {
-        __nv_bfloat16* d = hmq_u + (int64_t(tu + 1) * B + ur) * Hq + j0;
+      split_pack4(h_new * nd_n, ph, pl, ph2, pl2);
+      if (live && tu < a.T1 - 1) {
+        __nv_bfloat16* d = (ul ? a.hmq[1] : a.hmq[0]) + (int64_t(tu + 1) * B + ur) * Hq + j0;
         *reinterpret_cast<uint2*>(d) = make_uint2(ph, ph2);
         *reinterpret_cast<uint2*>(d + a.hmq_lo) = make_uint2(pl, pl2);
       }
@@ -2094,7 +2076,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
       }
     }
   }
-  cluster_sync_all();   // no CTA exits with multicast writes or remote arrives into it still in flight
 }
 
 // ---- split-precision backward wavefront (precision 2) ----------------------------------------------
@@ -2106,7 +2087,9 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_fwd_wave_split_kernel(
 // column tiles; ONE warp owns one (k-group, tile) item for all steps and accumulates it as one chain of mma3 over the
 // group's 12 k16 steps (gate-major), with that item's W fragments in registers (hi AND lo: 48 per matrix, 96 in the upper
 // role).  The CTAs of k-group w (gc of them, 11 tiles each) load only the gate gradients of the group's 6 producer CTAs
-// (24 KB with lo planes) instead of the whole 4H-wide tile (274 KB), and publish their per-tile partial products (1 KB per
+// (24 KB with lo planes) instead of the whole 4H-wide tile (274 KB) - the producers store them into a k-group-blocked
+// ring laid out as the consumers' shared-memory tiles, so that the load is ONE 1-D bulk copy of 28 KB instead of 1,536
+// 16-byte cp.async of 96-byte row pieces (tools/ubench/ubench_lstm.cu) - and publish their per-tile partial products (1 KB per
 // tile and matrix) to an fp32 ring; the CTA owning a column block then sums the ngroups partials of its block in group
 // order.  Per step there are two hand-offs through per-CTA flags (stores, bar.sync, fence.acq_rel.gpu, flag = step + 1;
 // see lstm2_fwd_wave_split_kernel): A = gate gradients published, B = partial products published.
@@ -2120,11 +2103,11 @@ struct WaveBwdSplitArgs {
   int nfwd;
   __nv_bfloat16* dgb_up; __nv_bfloat16* dgb_lo; int lg; int64_t dgb_lo_off;   // gate gradients of all steps, hi plane (+ lo offset)
   float* db_up; float* db_lo;
-  __nv_bfloat16* dgq_up; __nv_bfloat16* dgq_lo; int64_t dgq_lo_off;          // exchange planes: [2][4, B, Hq] (+ lo offset)
+  __nv_bfloat16* dgx_up; __nv_bfloat16* dgx_lo;   // exchange rings, k-group-blocked: [2 slots][k-group][kBwdGroupE]
   float* rec;                       // dh partials: [role][2 slots][ngroups][nc column blocks][32 rows][8 cols]
   float* dxr;                       // dL/dh_lower partials, upper role -> lower role: [2 slots][ngroups][nc][32][8]
   unsigned* flags;                  // A: [0, 2nc), B: [256, 256 + 2nc), kFlagStride apart
-  int T1, B, H, Hq;
+  int T1, B, H;
   unsigned nc;                      // CTAs per role (>= ncol, >= ngroups * gc)
   unsigned ncol;                    // CTAs per role that own columns < H (= ceil(H / 8)) = n8 column tiles
   int ngroups, gc;                  // k-groups (ceil(ceil(H/16) / 3)) and CTAs per k-group (ceil(ncol / 11))
@@ -2132,6 +2115,8 @@ struct WaveBwdSplitArgs {
 };
 constexpr int kBwdGroupCtas = kSplitK * 16 / kBwdCols;   // producer CTAs of one k-group's gate gradients (6)
 constexpr int kBwdGateE = 2 * kHalfE;                    // one gate's tile: [row half][hi, lo][16 rows][kTileRowE]
+constexpr int kBwdGroupE = 4 * kBwdGateE;                // one k-group's tiles of the four gates, as the consumer holds them
+static int64_t wave_split_dgx_elems(int H) { return int64_t(2) * wave_bwd_split_groups(H) * kBwdGroupE; }
 constexpr int kBwdFlagsB = 256;                          // flag index of the B flags
 constexpr int kBwdMaxGroups = kSplitWarps;              // k-groups of ceil(H/16) <= 33 k16 steps, 3 per group
 
@@ -2143,7 +2128,7 @@ __device__ __forceinline__ void wait_flag(const unsigned* f, unsigned v) {
 __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(WaveBwdSplitArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, wrp = tid >> 5;
-  const int H = a.H, Hq = a.Hq, B = a.B;
+  const int H = a.H, B = a.B;
   const bool upper = blockIdx.x < a.nc;
   const int role = upper ? 0 : 1;
   const int cidx = int(upper ? blockIdx.x : blockIdx.x - a.nc);
@@ -2156,8 +2141,9 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   const int w = work ? cidx / a.gc : 0, ks0 = w * kSplitK;
   const int nt = (cidx % a.gc) * kSplitWarps + wrp;
   const bool tile_ok = work && nt < int(a.ncol);
-  // the group's gate-gradient tiles [gate][row half][hi, lo][16 rows][kTileRowE]; rows >= B stay zero
+  // the group's gate-gradient tiles [gate][row half][hi, lo][16 rows][kTileRowE], a copy of one block of the ring
   __nv_bfloat16* const X = reinterpret_cast<__nv_bfloat16*>(smem_raw);
+  __shared__ __align__(8) uint64_t x_full;   // the block's bytes have landed
   // The pointwise operands of the NEXT step (forward saves: 4 gates, c, masked c_prev, dy, 2 done masks) are prefetched
   // into SHARED memory with 4-byte cp.async while this step's hand-offs and products run: held in registers they spilled
   // to local memory (168-register cap with the 96 fragment registers) and their load latency landed on the critical path.
@@ -2171,7 +2157,6 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   const float* const gact = upper ? a.gact_up : a.gact_lo;
   const float* const csb = upper ? a.csb_up : a.csb_lo;
   __nv_bfloat16* const dgb = upper ? a.dgb_up : a.dgb_lo;
-  __nv_bfloat16* const dgq = upper ? a.dgq_up : a.dgq_lo;
   // B fragments of this warp's item: B[kk][n] = W[g*H + j][nt*8 + n] for kk = (gate g, unit j of the group)
   uint32_t bh[4][kSplitK][2], bl[4][kSplitK][2], ih[4][kSplitK][2], il[4][kSplitK][2];
   {
@@ -2197,9 +2182,11 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
         split_pack(u[2], u[3], ih[g][sk][1], il[g][sk][1]);
       }
   }
-  for (int i = tid; i < 4 * kBwdGateE / 8; i += kSplitThreads) reinterpret_cast<uint4*>(X)[i] = make_uint4(0u, 0u, 0u, 0u);
+  if (tid == 0) {
+    mbar_init(&x_full, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
   if (wrp < kBwdCols) { dh_s[wrp][lane] = 0.0f; dx_s[wrp][lane] = 0.0f; dc_s[wrp][lane] = 0.0f; }
-  const int64_t gs = int64_t(B) * Hq;      // one gate of one exchange buffer
   const int q = wrp;  // pointwise role: thread = (batch row lane, unit k0 + wrp), warps 0..7
   const bool actA = (wrp < kBwdCols && lane < rows && k0 + q < H);
   auto time_of = [&](int s) { return upper ? a.T1 - 1 - s : a.T1 - s; };
@@ -2253,13 +2240,14 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
   float* const rec = a.rec + (upper ? 0 : 2 * slot_f);
   auto flag_a = [&](int r, int c) { return a.flags + (r * int(a.nc) + c) * kFlagStride; };
   auto flag_b = [&](int r, int c) { return a.flags + (kBwdFlagsB + r * int(a.nc) + c) * kFlagStride; };
+  // block of k-group g in slot `slot` of this role's gate-gradient ring
+  auto ring = [&](int slot, int g) { return (upper ? a.dgx_up : a.dgx_lo) + (slot * a.ngroups + g) * kBwdGroupE; };
   int it = 0;  // this role's active-step counter
   for (int s = 0; s <= last_s; ++s) {
     const int t = time_of(s);
     const bool active = (t >= 0 && t < a.T1);
     const int64_t row0 = int64_t(active ? t : 0) * B;
     const int slot = s & 1;
-    __nv_bfloat16* const dgq_t = dgq + int64_t(slot) * 4 * gs;
     float p_i = 0.f, p_f = 0.f, p_g = 0.f, p_o = 0.f;
     if (active) {
       if (actA) {   // (the prefetched and gathered operands were made visible by the barrier at the end of the previous step)
@@ -2305,8 +2293,10 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     __syncthreads();
     if (active && tid < 256 && (tid & 31) < rows && !idle) {   // publish (16-byte stores staged through smem)
       const int pl = tid >> 7, g = (tid >> 5) & 3, bb = tid & 31;
-      *reinterpret_cast<uint4*>(dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(bb) * Hq + k0) =
-          *reinterpret_cast<const uint4*>(&stg_s[pl][g][bb][0]);
+      const int kg = k0 / (kSplitK * 16);   // this CTA's 8 columns in its k-group's block
+      *reinterpret_cast<uint4*>(ring(slot, kg) + (k0 - kg * kSplitK * 16) + g * kBwdGateE + (bb >> 4) * kHalfE + pl * 16 * kTileRowE +
+                                (bb & 15) * kTileRowE) = *reinterpret_cast<const uint4*>(&stg_s[pl][g][bb][0]);
+      fence_proxy_async_global();   // consumers read the ring through bulk copies
     }
     __syncthreads();
     if (tid == 0) {   // hand-off A: this CTA's gate gradients of wave step s are out
@@ -2319,17 +2309,18 @@ __global__ void __launch_bounds__(kSplitThreads, 1) lstm2_bwd_wave_split_kernel(
     const bool need_rec = active && t > 0;   // dh_{t-1}; at t = 0 lstm_dh0_kernel forms it from the dgb rows
     const bool need_dx = active && upper;    // dL/dh_lower[t]
     if (work && (need_rec || need_dx)) {
-      if (tid < kBwdGroupCtas && w * kBwdGroupCtas + tid < int(a.nc))
+      if (tid < kBwdGroupCtas && w * kBwdGroupCtas + tid < int(a.nc)) {
         wait_flag(flag_a(role, w * kBwdGroupCtas + tid), unsigned(s + 1));
-      __syncthreads();
-      // the group's 48 columns of the four gates, rows < B, both planes: 6 x 16-byte copies per (gate, plane, row)
-      for (int i = tid; i < 4 * 2 * rows * 6; i += kSplitThreads) {
-        const int c = i % 6, r = (i / 6) % rows, pl = (i / (6 * rows)) & 1, g = i / (12 * rows);
-        cp_async16(X + g * kBwdGateE + (r >> 4) * kHalfE + pl * 16 * kTileRowE + (r & 15) * kTileRowE + c * 8,
-                   dgq_t + (pl ? a.dgq_lo_off : 0) + int64_t(g) * gs + int64_t(r) * Hq + ks0 * 16 + c * 8);
+        fence_proxy_async_global();
       }
-      asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
       __syncthreads();
+      // the group's block: 48 (+8) columns of the four gates, both planes, all 32 rows (rows >= B and columns no CTA
+      // writes are zero in the ring)
+      if (tid == 0) {
+        mbar_expect_tx(&x_full, kBwdGroupE * 2);
+        bulk_g2s(X, ring(slot, w), kBwdGroupE * 2, &x_full);
+      }
+      mbar_wait(&x_full, uint32_t(it) & 1);   // every active step before this one loaded a block (t = 0 is the last)
       if (tile_ok) {
         float acc0[2][4], acc1[2][4];
 #pragma unroll
@@ -2470,10 +2461,11 @@ static int lstm2_fwd_wave(LstmWs& ws, const LstmParams& p, float* y, const float
   return launch(l, "lstm2_fwd_wave_mma_kernel", lstm2_fwd_wave_mma_kernel, a);
 }
 
-// slot 0 of the split recurrence's planes: hq = split(h0) (raw), hmq = split(h0 * nd_0); row padding zero
+// slot 0 of the split recurrence's planes: hq = split(h0) (raw), hmq = split(h0 * nd_0); row padding zero.  hx (the
+// slice-blocked exchange copy of hq) is zeroed beforehand: its columns past Hq stay zero.
 __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const float* __restrict__ nd,
                                              __nv_bfloat16* __restrict__ hq, int64_t hq_lo, __nv_bfloat16* __restrict__ hmq,
-                                             int64_t hmq_lo, int B, int H, int Hq) {
+                                             int64_t hmq_lo, __nv_bfloat16* __restrict__ hx, int B, int H, int Hq) {
   const int64_t total = int64_t(B) * Hq;
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -2483,13 +2475,14 @@ __global__ void lstm_init_state_split_kernel(const float* __restrict__ h0, const
   const __nv_bfloat16 a = __float2bfloat16_rn(h), m = __float2bfloat16_rn(hm);
   hq[i] = a; hq[hq_lo + i] = __float2bfloat16_rn(h - __bfloat162float(a));
   hmq[i] = m; hmq[hmq_lo + i] = __float2bfloat16_rn(hm - __bfloat162float(m));
+  if (k < kSplitWarps * kSplitK * 16) { hx[hx_index(b, k, 0)] = hq[i]; hx[hx_index(b, k, 1)] = hq[hq_lo + i]; }
 }
 
-// The split kernels run as one cooperative grid of 2-CTA clusters.  Forward CTAs: kStepUnits units each, padded to whole
-// clusters; shared memory: tiles + partial sums + alignment slack
+// The split kernels run as cooperative grids.  Forward CTAs: kStepUnits units each; shared memory: tiles + partial sums +
+// alignment slack
 static Launch wave_fwd_split_launch(int H, cudaStream_t st) {
-  return Launch(dim3(((H + kStepUnits - 1) / kStepUnits + 1) & ~1), kSplitThreads,
-                size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128, st, 2, true);
+  return Launch(dim3((H + kStepUnits - 1) / kStepUnits), kSplitThreads,
+                size_t(kSplitWarps) * 2 * kSlotBytes + sizeof(float) * kSplitWarps * 2 * 16 * 33 + 128, st, 1, true);
 }
 // backward: per role, kBwdCols pointwise columns per CTA (padded to an even count), and at least the ngroups x gc CTAs that
 // run the products; shared memory: the k-group's gate-gradient tiles + prefetched pointwise operands
@@ -2502,9 +2495,11 @@ static unsigned wave_bwd_split_role_ctas(int H) {
 static Launch wave_bwd_split_launch(int H, cudaStream_t st) {
   return Launch(dim3(2 * wave_bwd_split_role_ctas(H)), kSplitThreads, size_t(4) * kBwdGateE * 2 + sizeof(float) * 9 * 256, st, 1, true);
 }
+// the shapes the split kernels' layouts hold (lstm_ws sizes the exchange buffer for these)
+static bool wave_split_shape(int64_t B, int In, int H) { return B <= 32 && In == H && (H + 15) / 16 <= kSplitWarps * kSplitK; }
 // both split kernels: the backward consumes the blocked saves only the split forward writes
 static bool wave_split_fits(int64_t B, int In, int H) {
-  if (B > 32 || In != H || (H + 15) / 16 > kSplitWarps * kSplitK) return false;
+  if (!wave_split_shape(B, In, H)) return false;
   const Launch f = wave_fwd_split_launch(H, nullptr), b = wave_bwd_split_launch(H, nullptr);
   if (int(f.cfg.gridDim.x) > kSplitThreads || f.cfg.gridDim.x > 512 || !fits<lstm2_fwd_wave_split_kernel>(f)) return false;
   return b.cfg.gridDim.x <= 2 * (512 - kBwdFlagsB) && fits<lstm2_bwd_wave_split_kernel>(b);
@@ -2523,19 +2518,14 @@ static int lstm2_fwd_wave_split(LstmWs& ws, const LstmParams& p, float* y, const
     a.gact[l] = L.gact; a.csb[l] = L.csb;
     TB_REQUIRE(L.gact && L.csb, "lstm: blocked save buffers missing");
     a.hq[l] = static_cast<__nv_bfloat16*>(L.hq); a.hmq[l] = static_cast<__nv_bfloat16*>(L.hmq);
+    a.hx[l] = static_cast<__nv_bfloat16*>(L.hx);
+    TB_REQUIRE(L.hx, "lstm: h exchange buffer missing");
   }
   a.hq_lo = ws.layer[0].hq_lo; a.hmq_lo = ws.layer[0].hmq_lo;
   TB_REQUIRE(ws.layer[1].hq_lo == a.hq_lo && ws.layer[1].hmq_lo == a.hmq_lo && a.hq_lo > 0, "lstm: split planes missing");
   a.nd = notdone; a.flags = ws.flags;
   a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nctas = unsigned((H + kStepUnits - 1) / kStepUnits);
-  CUtensorMap maps[2];
-  for (int l = 0; l < 2; ++l) {
-    const uint64_t dims[4] = {uint64_t(Hq), uint64_t(B), uint64_t(T1 + 1), 2};
-    const uint64_t strides[3] = {uint64_t(Hq) * 2, uint64_t(B) * Hq * 2, uint64_t(a.hq_lo) * 2};
-    const uint32_t box[4] = {kTileRowE, 16, 1, 2};
-    TB_TRY(tcd::make_map_nd(&maps[l], a.hq[l], 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE));
-  }
-  return launch(wave_fwd_split_launch(H, st), "lstm2_fwd_wave_split_kernel", lstm2_fwd_wave_split_kernel, maps[0], maps[1], a);
+  return launch(wave_fwd_split_launch(H, st), "lstm2_fwd_wave_split_kernel", lstm2_fwd_wave_split_kernel, a);
 }
 
 // =========================================================================================
@@ -2931,16 +2921,15 @@ static int lstm2_bwd_wave(LstmWs& ws, const LstmParams& p, const LstmGrads& g, c
 
 static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads& g, const float* dy, const float* notdone,
                                 int64_t T1, int64_t B, int H, const LstmStateGrads& sg, cudaStream_t st) {
-  const int Hq = mma_hq(H);
   const unsigned nc = wave_bwd_split_role_ctas(H);
   const LstmLayerWs& U = ws.layer[1];
   const LstmLayerWs& L = ws.layer[0];
   unsigned* flags = ws.flags + 512 * kFlagStride;
   cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(unsigned) * 512 * kFlagStride, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(U.dgq, 0, size_t(U.dgq_lo + int64_t(2) * 4 * B * Hq) * 2, st);  // columns no CTA writes
-  if (e == cudaSuccess) e = cudaMemsetAsync(L.dgq, 0, size_t(L.dgq_lo + int64_t(2) * 4 * B * Hq) * 2, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(U.dgx, 0, size_t(wave_split_dgx_elems(H)) * 2, st);  // rows and columns no CTA writes
+  if (e == cudaSuccess) e = cudaMemsetAsync(L.dgx, 0, size_t(wave_split_dgx_elems(H)) * 2, st);
   TB_REQUIRE(e == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(e));
-  TB_REQUIRE(U.dgq_lo > 0 && U.dgq_lo == L.dgq_lo && U.dgb_lo > 0 && U.dgb_lo == L.dgb_lo, "lstm: split planes missing");
+  TB_REQUIRE(U.dgx && L.dgx && U.dgb_lo > 0 && U.dgb_lo == L.dgb_lo, "lstm: split planes missing");
   WaveBwdSplitArgs a;
   a.w_hh_up = p.w_hh[1]; a.w_hh_lo = p.w_hh[0]; a.w_ih_up = p.w_ih[1];
   a.dy = dy; a.nd = notdone;
@@ -2949,9 +2938,9 @@ static int lstm2_bwd_wave_split(LstmWs& ws, const LstmParams& p, const LstmGrads
   a.dgb_up = static_cast<__nv_bfloat16*>(U.dgb); a.dgb_lo = static_cast<__nv_bfloat16*>(L.dgb); a.lg = int(ld16(4 * H));
   a.dgb_lo_off = U.dgb_lo;
   a.db_up = g.b_ih[1]; a.db_lo = g.b_ih[0];
-  a.dgq_up = static_cast<__nv_bfloat16*>(U.dgq); a.dgq_lo = static_cast<__nv_bfloat16*>(L.dgq); a.dgq_lo_off = U.dgq_lo;
+  a.dgx_up = static_cast<__nv_bfloat16*>(U.dgx); a.dgx_lo = static_cast<__nv_bfloat16*>(L.dgx);
   a.rec = ws.bwd_rec; a.dxr = ws.bwd_dxr; a.flags = flags;
-  a.T1 = int(T1); a.B = int(B); a.H = H; a.Hq = Hq; a.nc = nc; a.ncol = unsigned((H + kBwdCols - 1) / kBwdCols);
+  a.T1 = int(T1); a.B = int(B); a.H = H; a.nc = nc; a.ncol = unsigned((H + kBwdCols - 1) / kBwdCols);
   a.ngroups = wave_bwd_split_groups(H); a.gc = wave_bwd_split_group_ctas(H);
   a.dhN = sg.dhN; a.dcN = sg.dcN; a.dc0 = sg.dc0;
   return launch(wave_bwd_split_launch(H, st), "lstm2_bwd_wave_split_kernel", lstm2_bwd_wave_split_kernel, a);
@@ -3187,8 +3176,10 @@ int lstm_forward(const float* x, const float* notdone, const float* h0, const fl
       __nv_bfloat16* hq = static_cast<__nv_bfloat16*>(L.hq);
       __nv_bfloat16* hmq = static_cast<__nv_bfloat16*>(L.hmq);
       if (split) {
+        eq = cudaMemsetAsync(L.hx, 0, size_t(wave_split_hx_elems(T1)) * 2, st);
+        TB_REQUIRE(eq == cudaSuccess, "lstm: memset: %s", cudaGetErrorString(eq));
         lstm_init_state_split_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(h0l, notdone, hq, L.hq_lo, hmq, L.hmq_lo,
-                                                                                      int(B), H, Hq);
+                                                                                      static_cast<__nv_bfloat16*>(L.hx), int(B), H, Hq);
         TB_TRY(check_launch("lstm_init_state_split_kernel"));
       } else {
         lstm_init_state_q_kernel<<<(unsigned)((B * Hq + 255) / 256), 256, 0, st>>>(h0l, c0 + int64_t(l) * B * H, notdone, hmq,

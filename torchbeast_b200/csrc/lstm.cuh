@@ -32,8 +32,12 @@ struct LstmLayerWs {
   float* gact = nullptr;  // (precision 2) activated gates, CTA-blocked [T1][ceil(H/4)][32][16] - see lstm2_fwd_wave_split_kernel
   float* csb = nullptr;   // (precision 2) cell state, CTA-blocked [T1+1][ceil(H/4)][32][4]: slot 0 = c0, slot t+1 = c_t
   void* hmq;      // bf16 [T1*B, Hq]         masked recurrent inputs written by the tensor-core recurrence (Hq = mma_hq(H))
-  void* hq;       // bf16 [(T1+1)*B, Hq]     raw h (slot 0 = initial state) exchanged by the two-layer wavefront kernel
+  void* hq;       // bf16 [(T1+1)*B, Hq]     raw h (slot 0 = initial state) written by the two-layer wavefront kernels
+  void* hx = nullptr;  // (precision 2, two layers) the same h as hi / lo planes, slice-blocked for the split wavefront's
+                       // exchange: [T1+1][kXSlotE] - see lstm2_fwd_wave_split_kernel
   void* dgq;      // bf16 [2][4, B, Hq]      this step's gate gradients for the tensor-core backward recurrence
+  void* dgx = nullptr;  // (precision 2, two layers) the split backward wavefront's gate-gradient exchange ring, hi / lo
+                        // planes blocked by k-group: [2 slots][k-group][kBwdGroupE] - see lstm2_bwd_wave_split_kernel
   float* wp;      // [4H+4, Hp]  W_hh with rows zero-padded to Hp floats (16-byte multiples for bulk copies)
   float* dgates;  // [T1*B, 4H]  backward: d pre-activations
   float* bsum;    // [4H]        b_ih + b_hh
