@@ -70,40 +70,14 @@ int tb_vtrace_from_importance_weights_f64(const double* log_rhos, const double* 
                                           double clip_rho, double clip_pg_rho, double* vs,
                                           double* pg_adv, void* stream);
 
-/* Fused learner loss block: torchbeast/core/vtrace.py:58-88 (from_logits) +
- * monobeast.py:107-125 / polybeast_learner.py:113-131 (three losses) +
- * monobeast.py:245-277 / polybeast_learner.py:332-361 (reward clip, discounts, weighting)
- * and their closed-form backward (SURVEY.md section 8(a) A4), ONE launch.
- *
- * inputs (already shifted: batch[1:], learner_outputs[:-1]):
- *   behavior_logits, target_logits [T,B,A] f32; actions [T,B] i64; rewards [T,B] f32 (raw);
- *   done [T,B] u8 (bool) if `discounts`==NULL, else discounts [T,B] f32 used as is;
- *   values [T,B] f32; bootstrap [B] f32.
- * flags: clip_rewards!=0 clamps rewards to [-1,1] (reward_clipping == "abs_one").
- * outputs:
- *   vs, pg_adv, log_rhos, behavior_alp, target_alp [T,B] f32 (all required);
- *   losses_out [4] f32 = {pg_loss, baseline_cost*baseline_loss, entropy_cost*entropy_loss, total};
- *   grad_logits [T(+1),B,A], grad_values [T(+1),B] f32 = d total / d target_logits, d values
- *   (may both be NULL: forward only).  If zero_tail!=0 they have T+1 rows and row T is
- *   zero-filled (the bootstrap row of the learner outputs gets no gradient, vtrace.py:91).
- * workspace: tb_workspace_bytes() zero-initialised bytes (see conventions).                */
-int tb_impala_loss_fwd_bwd_f32(const float* behavior_logits, const float* target_logits,
-                               const int64_t* actions, const float* rewards,
-                               const uint8_t* done, const float* discounts, const float* values,
-                               const float* bootstrap, int64_t T, int64_t B, int64_t A,
-                               float discounting, float baseline_cost, float entropy_cost,
-                               int clip_rewards, float clip_rho, float clip_pg_rho, float* vs,
-                               float* pg_adv, float* log_rhos, float* behavior_alp,
-                               float* target_alp, float* losses_out, float* grad_logits,
-                               float* grad_values, int zero_tail, void* workspace, void* stream);
-
 /* ---- hyper-parameters read from device memory ------------------------------------------
- * The scalar arguments of the loss and optimizer steps, as one block in device memory.  The *_hp entry points
- * read their values from it when the kernel runs, so a captured CUDA graph follows changes the caller publishes
- * between replays (annealed costs, population-based training).  Every value derived from them (1 - alpha,
- * 1 - beta, the clip coefficient, the bias corrections) is computed in the kernel by the same expression as in
- * the float-argument entry points, so both give bit-identical results for the same values.  Layout is fixed:
- * tb_hparams_layout() reports it, so a binding can check its packing without a GPU.                       */
+ * The scalar arguments of the loss and optimizer steps, as one block in device memory.  Given a non-NULL `hp`,
+ * tb_impala_loss_f32 and the tb_clip_*_step_f32 entry points read their values from it when the kernel runs, so a
+ * captured CUDA graph follows changes the caller publishes between replays (annealed costs, population-based
+ * training).  Every value derived from them (1 - alpha, 1 - beta, the clip coefficient, the bias corrections) is
+ * computed in the kernel by the same expression as from the float arguments, so both give bit-identical results for
+ * the same values.  Layout is fixed: tb_hparams_layout() reports it, so a binding can check its packing without a
+ * GPU.                                                                                                            */
 typedef struct tb_hparams {
   double beta1, beta2;         /* Adam / AdamW, in [0, 1); double as in tb_clip_adam_step_f32                  */
   float discounting;           /* used where done is given; a `discounts` array is used as is                  */
@@ -116,35 +90,38 @@ typedef struct tb_hparams {
 /* Host only: out[0] = sizeof(tb_hparams), out[1..13] = offsetof of discounting, baseline_cost, entropy_cost,
  * clip_rho, clip_pg_rho, clip_rewards, max_norm, alpha, eps, momentum, weight_decay, beta1, beta2.           */
 int tb_hparams_layout(int64_t* out_host);
-/* tb_impala_loss_fwd_bwd_f32 with discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho and
- * clip_pg_rho read from hp (device pointer) when the kernel runs.                                          */
-int tb_impala_loss_fwd_bwd_hp_f32(const float* behavior_logits, const float* target_logits,
-                                  const int64_t* actions, const float* rewards, const uint8_t* done,
-                                  const float* discounts, const float* values, const float* bootstrap, int64_t T,
-                                  int64_t B, int64_t A, const tb_hparams* hp, float* vs, float* pg_adv,
-                                  float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
-                                  float* grad_logits, float* grad_values, int zero_tail, void* workspace,
-                                  void* stream);
 
-/* tb_impala_loss_fwd_bwd_f32 with importance weights: column_weights [B] f32 (device, not NULL).  The pg, baseline and
- * entropy terms of every row (t, b) are multiplied by column_weights[b], in losses_out and in grad_logits / grad_values
- * (after the unweighted term is formed, so weights of 1.0f give the bits of tb_impala_loss_fwd_bwd_f32 / _hp_f32; a
- * weight of 0 gives zero gradient rows).  vs, pg_adv, log_rhos and the log-probabilities are not weighted.
- * hp: NULL takes the scalar arguments, else they are read from hp when the kernel runs.                            */
-int tb_impala_loss_weighted_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
-                                const float* rewards, const uint8_t* done, const float* discounts, const float* values,
-                                const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
-                                float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
-                                float clip_pg_rho, const float* column_weights, const tb_hparams* hp, float* vs,
-                                float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
-                                float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
-                                void* workspace, void* stream);
-
-/* ---- trust region for off-policy V-trace (Schmitt, Hessel & Simonyan, ICML 2020, "Off-Policy Actor-Critic with
- * Shared Experience Replay": LASER's beta trust region) ---------------------------------------------------------------
- * tb_impala_loss_trust_f32: the arguments of tb_impala_loss_weighted_f32 (column_weights may be NULL: unweighted; hp
- * may be NULL: the scalar arguments) plus trust_beta (f32 [1], device, read when the kernel runs), kl_out [T,B] f32
- * and trust_out [2] f32.  For every row (t, b) of the shifted inputs:
+/* Fused learner loss block: torchbeast/core/vtrace.py:58-88 (from_logits) +
+ * monobeast.py:107-125 / polybeast_learner.py:113-131 (three losses) +
+ * monobeast.py:245-277 / polybeast_learner.py:332-361 (reward clip, discounts, weighting)
+ * and their closed-form backward (SURVEY.md section 8(a) A4), ONE launch.  Each feature group below (hp, importance
+ * weights, PopArt, trust region) is off when its pointer is NULL; with all of them NULL this is the plain loss block.
+ *
+ * inputs (already shifted: batch[1:], learner_outputs[:-1]):
+ *   behavior_logits, target_logits [T,B,A] f32; actions [T,B] i64; rewards [T,B] f32 (raw);
+ *   done [T,B] u8 (bool) if `discounts`==NULL, else discounts [T,B] f32 used as is;
+ *   values [T,B] f32; bootstrap [B] f32.
+ * flags: clip_rewards!=0 clamps rewards to [-1,1] (reward_clipping == "abs_one").
+ * hp: NULL takes discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho and clip_pg_rho from the
+ *   arguments; else they are read from hp (device pointer, see tb_hparams) when the kernel runs, and the scalar
+ *   arguments are not read.
+ * outputs:
+ *   vs, pg_adv, log_rhos, behavior_alp, target_alp [T,B] f32 (all required);
+ *   losses_out [4] f32 = {pg_loss, baseline_cost*baseline_loss, entropy_cost*entropy_loss, total};
+ *   grad_logits [T(+1),B,A], grad_values [T(+1),B] f32 = d total / d target_logits, d values
+ *   (may both be NULL: forward only).  If zero_tail!=0 they have T+1 rows and row T is
+ *   zero-filled (the bootstrap row of the learner outputs gets no gradient, vtrace.py:91).
+ * workspace: tb_workspace_bytes() zero-initialised bytes (see conventions).
+ *
+ * ---- importance weights: column_weights [B] f32 (device; NULL: unweighted).  The pg, baseline and entropy terms of
+ * every row (t, b) are multiplied by column_weights[b], in losses_out and in grad_logits / grad_values (after the
+ * unweighted term is formed, so weights of 1.0f give the bits of column_weights = NULL; a weight of 0 gives zero
+ * gradient rows).  vs, pg_adv, log_rhos and the log-probabilities are not weighted.
+ *
+ * ---- trust region for off-policy V-trace (Schmitt, Hessel & Simonyan, ICML 2020, "Off-Policy Actor-Critic with
+ * Shared Experience Replay": LASER's beta trust region): trust_beta (f32 [1], device, read when the kernel runs; NULL:
+ * no trust region), kl_out [T,B] f32 and trust_out [2] f32 (both required with trust_beta).  For every row (t, b) of
+ * the shifted inputs:
  *   kl_t = sum_a pi_t(a) (log pi_t(a) - log mu_t(a)) in fp32, pi = softmax(target_logits), mu = softmax(behavior_logits),
  *          both log-softmaxes from the max / log-sum-exp the action log-probabilities are formed with (behavior_alp and
  *          target_alp keep their bits); written to kl_out.
@@ -155,57 +132,41 @@ int tb_impala_loss_weighted_f32(const float* behavior_logits, const float* targe
  *   constant for the backward: no gradient flows through kl.
  *   log_rhos, behavior_alp and target_alp are the true, unmasked values; vs and pg_adv are the masked ones.
  * trust_out = {number of trusted rows, sum of kl_t over all T*B rows}: fp64 sums in a fixed order (no atomics), bit-
- * identical from run to run, rounded to f32 once.  beta = +inf on finite inputs gives the bits of
- * tb_impala_loss_fwd_bwd_f32 / _hp_f32 / tb_impala_loss_weighted_f32 in every output; identical behaviour and target
- * logits give kl = 0 exactly, so beta = 0 trusts those rows.  One launch.
- * tb_impala_loss_popart_trust_f32: tb_impala_loss_popart_f32 with the same rule and the same three arguments (the
- * per-task sums come from the masked vs).  Two launches.                                                           */
-int tb_impala_loss_trust_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
-                             const float* rewards, const uint8_t* done, const float* discounts, const float* values,
-                             const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
-                             float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
-                             float clip_pg_rho, const float* column_weights, const tb_hparams* hp, float* vs,
-                             float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
-                             float* grad_logits, float* grad_values, int zero_tail, const float* trust_beta,
-                             float* kl_out, float* trust_out, void* workspace, void* stream);
-int tb_impala_loss_popart_trust_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
-                                    const float* rewards, const uint8_t* done, const float* discounts,
-                                    const float* values, const int64_t* task, const double* mu, const double* nu,
-                                    int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
-                                    float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
-                                    const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
-                                    float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
-                                    float* grad_values, double* task_sums, const float* trust_beta, float* kl_out,
-                                    float* trust_out, void* workspace, void* stream);
-
-/* ---- PopArt value normalisation (van Hasselt et al. 2016; Hessel et al. 2019) -----------
+ * identical from run to run, rounded to f32 once.  beta = +inf on finite inputs gives the bits of trust_beta = NULL
+ * (with the same hp, column_weights and PopArt arguments) in every output; identical behaviour and target logits give
+ * kl = 0 exactly, so beta = 0 trusts those rows.  With PopArt the per-task sums come from the masked vs.
+ *
+ * ---- PopArt value normalisation (van Hasselt et al. 2016; Hessel et al. 2019): task non-NULL.
  * Per task k, statistics mu[k], nu[k] (f64, device; start at 0 and 1) with
  *   sigma_k = clamp(sqrt(max(nu_k - mu_k^2, 0)), 1e-4, 1e6).
- * tb_impala_loss_popart_f32: the fused loss block of tb_impala_loss_fwd_bwd_f32 on a normalised value head.
- *   values [T+1,B,K] f32 = normalised head outputs n, bootstrap row T included; task [T+1,B] i64, row (t,b) uses
- *   k = task[t*B+b].  1. v = sigma_k * n[k] + mu_k (fp32, mu / sigma rounded once), the bootstrap with its own
- *   task.  2. V-trace on v as in tb_impala_loss_fwd_bwd_f32: vs, pg_adv stay unnormalised.  3. policy gradient
+ * The loss block then runs on a normalised value head:
+ *   values [T+1,B,K] f32 = normalised head outputs n, bootstrap row T included (bootstrap is not read); task [T+1,B]
+ *   i64, row (t,b) uses k = task[t*B+b].  1. v = sigma_k * n[k] + mu_k (fp32, mu / sigma rounded once), the bootstrap
+ *   with its own task.  2. V-trace on v as without PopArt: vs, pg_adv stay unnormalised.  3. policy gradient
  *   -log pi(a) * pg_adv / sigma_k, entropy unchanged.  4. baseline loss baseline_cost * 1/2 ((vs - mu_k)/sigma_k -
  *   n[k])^2; its gradient goes to column k of grad_values [T+1,B,K], every other column and row T get zero.
  *   A row whose task id is outside [0, K) adds no loss and gets zero gradient rows (its v is 0 in the V-trace); ids
  *   are not checked otherwise.  task_sums [3K] f64 out: count, sum vs and sum vs^2 of each task over rows t < T,
- *   bit-identical from run to run (no atomics).  hp: NULL takes the scalar arguments, else they are read from hp.
- *   1 <= K <= 64, T >= 1, B >= 1.  Two launches.
- * tb_popart_update: for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
- *   first), with beta read from device memory:
+ *   bit-identical from run to run (no atomics).
+ *   Requires 1 <= K <= 64, T >= 1, B >= 1, non-NULL mu, nu and task_sums, and zero_tail = 1; column_weights must be
+ *   NULL.  Two launches.  NULL task: K, mu, nu and task_sums are not read.                                       */
+int tb_impala_loss_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                       const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                       const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                       float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                       const tb_hparams* hp, const float* column_weights, const int64_t* task, const double* mu,
+                       const double* nu, int64_t K, double* task_sums, const float* trust_beta, float* kl_out,
+                       float* trust_out, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
+                       float* target_alp, float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
+                       void* workspace, void* stream);
+
+/* tb_popart_update: for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
+ *   first), with beta read from device memory and sigma_k as in tb_impala_loss_f32:
  *     mu'_k = (1 - beta) mu_k + beta * sum vs / count,   nu'_k = (1 - beta) nu_k + beta * sum vs^2 / count
  *   then rescales value-head row k so that its unnormalised outputs do not change:
  *     weight[k, :] *= sigma_k / sigma'_k,   bias[k] = (sigma_k * bias[k] + mu_k - mu'_k) / sigma'_k
  *   weight [K,F] and bias [K] f32 (e.g. inside a flat parameter buffer).  It runs after the optimizer step and does
  *   not touch optimizer state.  One launch, no host sync; graph-capturable.                                    */
-int tb_impala_loss_popart_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
-                              const float* rewards, const uint8_t* done, const float* discounts,
-                              const float* values, const int64_t* task, const double* mu, const double* nu,
-                              int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
-                              float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
-                              const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
-                              float* target_alp, float* losses_out, float* grad_logits, float* grad_values,
-                              double* task_sums, void* workspace, void* stream);
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,
                      float* bias, int64_t F, void* stream);
 /* Nets with num_values (1..64) value outputs, one per task: the tb_atarinet_* / tb_resnet_* entry points of the same
@@ -607,10 +568,15 @@ int tb_grad_sumsq_f32(const float* grads, int64_t n, float* out_sumsq, void* wor
  *   clipped in place like the reference); square_avg = alpha*square_avg + (1-alpha)*g^2;
  *   params -= lr * g/(sqrt(square_avg)+eps)   (momentum != 0: buf = momentum*buf + g/avg; params -= lr*buf).
  * lr_device (nullable) overrides `lr` with a device scalar; grad_norm_out (nullable) receives the
- * pre-clip norm.  No host synchronisation.                                                   */
+ * pre-clip norm.  No host synchronisation.
+ * hp, in this and the two steps below: NULL takes max_norm and the optimizer's values from the arguments.  Non-NULL:
+ * they are read from hp (device pointer, see tb_hparams) when the kernel runs, and the scalar arguments are not read;
+ * lr_device / lr as above.  The host cannot see hp's values, so the caller checks what the NULL case checks:
+ * momentum != 0 needs momentum_buf, betas in [0, 1).  With hp, momentum_buf != NULL selects the momentum update, so
+ * pass NULL when momentum is 0 (with hp NULL the buffer is ignored when momentum is 0).                          */
 int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
                              const float* sumsq, float max_norm, const float* lr_device, float lr, float alpha,
-                             float eps, float momentum, float* grad_norm_out, void* stream);
+                             float eps, float momentum, const tb_hparams* hp, float* grad_norm_out, void* stream);
 /* The same clip fused with one torch.optim.Adam (decoupled = 0, L2 weight decay) or AdamW (decoupled = 1) step,
  * non-amsgrad, in torch's op order:  g *= coef (written back);  Adam: g' = g + wd*p,  AdamW: p *= 1 - lr*wd;
  *   exp_avg = beta1*exp_avg + (1-beta1)*g';  exp_avg_sq = beta2*exp_avg_sq + (1-beta2)*g'^2;
@@ -620,27 +586,15 @@ int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, flo
  * captured into a CUDA graph and every replay takes the next t.  Bias corrections are computed in double.    */
 int tb_clip_adam_step_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, const float* sumsq,
                           float max_norm, const float* lr_device, float lr, double beta1, double beta2, float eps,
-                          float weight_decay, int decoupled, int64_t* step_device, float* grad_norm_out, void* stream);
+                          float weight_decay, int decoupled, int64_t* step_device, const tb_hparams* hp,
+                          float* grad_norm_out, void* stream);
 /* The same clip fused with torch.optim.RMSprop's remaining options: weight_decay (g' = g + wd*p after the clip) and
  * centered (grad_avg != NULL: grad_avg = alpha*grad_avg + (1-alpha)*g', avg = sqrt(square_avg - grad_avg^2) + eps),
  * combined with momentum as in tb_clip_rmsprop_step_f32.                                                         */
 int tb_clip_rmsprop_ex_step_f32(float* params, float* grads, float* square_avg, float* grad_avg, float* momentum_buf,
                                 int64_t n, const float* sumsq, float max_norm, const float* lr_device, float lr,
-                                float alpha, float eps, float weight_decay, float momentum, float* grad_norm_out,
-                                void* stream);
-/* The three steps above with max_norm and the optimizer's values read from hp (device pointer, see tb_hparams)
- * when the kernel runs; lr_device / lr as above.  The host cannot see hp's values, so the caller checks what the
- * float-argument entry points check: momentum != 0 needs momentum_buf, betas in [0, 1).  momentum_buf != NULL
- * selects the momentum update (pass NULL when momentum is 0, as the float-argument entry points do).          */
-int tb_clip_rmsprop_step_hp_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
-                                const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr,
+                                float alpha, float eps, float weight_decay, float momentum, const tb_hparams* hp,
                                 float* grad_norm_out, void* stream);
-int tb_clip_rmsprop_ex_step_hp_f32(float* params, float* grads, float* square_avg, float* grad_avg,
-                                   float* momentum_buf, int64_t n, const float* sumsq, const tb_hparams* hp,
-                                   const float* lr_device, float lr, float* grad_norm_out, void* stream);
-int tb_clip_adam_step_hp_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
-                             const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr, int decoupled,
-                             int64_t* step_device, float* grad_norm_out, void* stream);
 
 /* ---- bf16 tensor-core GEMM (wgmma + TMA), the throughput backend of the network -------- */
 

@@ -33,6 +33,33 @@ def test_library_exports_every_declared_symbol():
     assert _lib.lib().tb_workspace_bytes() > 64
 
 
+_CTYPES_OF = {"float": ctypes.c_float, "double": ctypes.c_double, "int": ctypes.c_int, "int64_t": ctypes.c_int64,
+              "uint64_t": ctypes.c_uint64, "size_t": ctypes.c_size_t}
+
+
+def _ctype_of(decl):
+    """The ctypes type a binding must use for one C parameter or return type (`decl` without its name)."""
+    if "*" in decl:
+        return (ctypes.c_char_p,) if decl.replace(" ", "") == "constchar*" else (ctypes.c_void_p, ctypes.c_char_p)
+    return (_CTYPES_OF[decl.strip()],)
+
+
+def test_binding_matches_every_header_signature():
+    # a ctypes call with a stale argument list passes whatever its arguments happen to be: check count and kind
+    from torchbeast_b200 import _lib
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "torchbeast_b200.h")).read(), flags=re.S)
+    decls = re.findall(r"([A-Za-z_][\w ]*?[\s*]+)(tb_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", text)
+    assert sorted(name for _, name, _ in decls) == header_symbols()
+    for ret, name, params in decls:
+        params = [p.strip() for p in params.split(",") if p.strip() not in ("", "void")]
+        argtypes, restype = _lib._SIGNATURES[name]
+        assert len(argtypes) == len(params), "%s: %d argtypes for %d parameters" % (name, len(argtypes), len(params))
+        for i, (param, argtype) in enumerate(zip(params, argtypes)):
+            kind = re.sub(r"\s*\b\w+$", "", param)  # drop the parameter name
+            assert argtype in _ctype_of(kind), "%s: parameter %d (%s) bound as %s" % (name, i, param, argtype.__name__)
+        assert restype in _ctype_of(ret), "%s: returns %s, bound as %s" % (name, ret.strip(), restype.__name__)
+
+
 def test_cpu_tensors_fail_loudly():
     from torchbeast_b200 import _lib
     from torchbeast_b200.core import vtrace

@@ -109,17 +109,17 @@ _P = ctypes.c_void_p(256)
 
 
 @pytest.mark.parametrize("centered,weight_decay", [(False, 0), (False, 1e-4), (True, 0)])
-def test_momentum_without_buffer_raises_the_entry_points_error(centered, weight_decay):
+def test_momentum_without_buffer_matches_the_null_hp_entry_point_error(centered, weight_decay):
     opt = optim.RMSprop(_net(), lr=4.8e-4, centered=centered, weight_decay=weight_decay)
     assert opt.momentum_buffer is None
     opt.param_groups[0]["momentum"] = 0.9
     lib = _lib.lib()
     if not centered and weight_decay == 0:
         want = _host_error(lib.tb_clip_rmsprop_step_f32, _P, _P, _P, None, 8, _P, 40.0, None, 1e-3, 0.99, 0.01, 0.9,
-                           None, None)
+                           None, None, None)
     else:
         want = _host_error(lib.tb_clip_rmsprop_ex_step_f32, _P, _P, _P, _P if centered else None, None, 8, _P, 40.0,
-                           None, 1e-3, 0.99, 0.01, weight_decay, 0.9, None, None)
+                           None, 1e-3, 0.99, 0.01, weight_decay, 0.9, None, None, None)
     assert "momentum needs a buffer" in want
     with pytest.raises(_lib.TorchBeastB200Error) as err:
         pack_hparams(_flags(), opt)
@@ -127,11 +127,11 @@ def test_momentum_without_buffer_raises_the_entry_points_error(centered, weight_
 
 
 @pytest.mark.parametrize("betas", [(1.0, 0.999), (0.9, 1.0), (-0.1, 0.999), (0.9, -1e-9)])
-def test_betas_outside_range_raise_the_entry_points_error(betas):
+def test_betas_outside_range_match_the_null_hp_entry_point_error(betas):
     opt = optim.Adam(_net(), lr=3e-4)
     opt.param_groups[0]["betas"] = betas
     want = _host_error(_lib.lib().tb_clip_adam_step_f32, None, None, None, None, 0, _P, 40.0, None, 3e-4,
-                       float(betas[0]), float(betas[1]), 1e-8, 0.0, 0, _P, None, None)
+                       float(betas[0]), float(betas[1]), 1e-8, 0.0, 0, _P, None, None, None)
     assert "betas must be in [0, 1)" in want
     with pytest.raises(_lib.TorchBeastB200Error) as err:
         pack_hparams(_flags(), opt)
@@ -179,15 +179,3 @@ def test_adam_structure():
     assert GraphedLearner.structure_of(adam, _batch(torch.uint8)) != key
     # an RMSprop is another launch sequence altogether
     assert GraphedLearner.structure_of(optim.RMSprop(_net()), batch) != key
-
-
-def test_hp_entry_points_need_a_block():
-    lib = _lib.lib()
-    assert "null hyper-parameter block" in _host_error(
-        lib.tb_impala_loss_fwd_bwd_hp_f32, *([_P] * 8), 4, 2, 6, None, *([_P] * 8), 1, _P, None)
-    assert "bad arguments" in _host_error(lib.tb_clip_rmsprop_step_hp_f32, _P, _P, _P, None, 8, _P, None, None, 1e-3,
-                                          None, None)
-    assert "bad arguments" in _host_error(lib.tb_clip_rmsprop_ex_step_hp_f32, _P, _P, _P, None, None, 8, _P, None,
-                                          None, 1e-3, None, None)
-    assert "bad arguments" in _host_error(lib.tb_clip_adam_step_hp_f32, _P, _P, _P, _P, 8, _P, None, None, 1e-3, 0, _P,
-                                          None, None)

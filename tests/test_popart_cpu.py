@@ -1,5 +1,7 @@
 """CPU: the PopArt restatement (tests/popart_oracle.py) reduces to the reference learn step with one task, identity
 statistics and beta = 0; the statistics update and the output-preserving rescale; the nets' PopArt state; the C ABI."""
+import ctypes
+
 import numpy as np
 import pytest
 import torch
@@ -147,17 +149,29 @@ def test_nets_popart_state(net):
             make(num_tasks=bad)
 
 
-def test_abi_declares_popart_entry_points():
+def test_popart_abi_and_host_side_checks():
     from tests.test_abi_cpu import header_symbols
     from torchbeast_b200 import _lib
-    for s in ("tb_impala_loss_popart_f32", "tb_popart_update", "tb_atarinet_forward_mt", "tb_atarinet_backward_phase_mt",
+    for s in ("tb_impala_loss_f32", "tb_popart_update", "tb_atarinet_forward_mt", "tb_atarinet_backward_phase_mt",
               "tb_resnet_backward_unstacked_mt"):
         assert s in header_symbols() and s in _lib.declared_symbols()
     h = _lib.lib()
     assert h.tb_popart_update(None, None, None, None, 65, None, None, 8, None) != 0
     assert b"bad sizes" in h.tb_last_error()
-    args = [None] * 10 + [4, 2, 6, 0, 0.99, 0.5, 0.0006, 1, 1.0, 1.0] + [None] * 12
-    assert h.tb_impala_loss_popart_f32(*args) != 0 and b"num_tasks" in h.tb_last_error()
+    P = ctypes.c_void_p(256)  # never dereferenced: every call below fails its host-side checks before a launch
+
+    def popart_error(T=4, K=3, mu=P, nu=P, task_sums=P, zero_tail=1):
+        args = ([None] * 6 + [P, None] + [T, 2, 6, 0.99, 0.5, 0.0006, 1, 1.0, 1.0, None, None, P, mu, nu, K, task_sums]
+                + [None] * 11 + [zero_tail, None, None])
+        assert h.tb_impala_loss_f32(*args) != 0
+        return h.tb_last_error()
+
+    assert b"num_tasks" in popart_error(K=0)
+    assert b"num_tasks" in popart_error(K=65)
+    for k in ("mu", "nu", "task_sums"):
+        assert b"null PopArt pointer" in popart_error(**{k: None})
+    assert b"bad sizes" in popart_error(T=0)
+    assert b"zero_tail" in popart_error(zero_tail=0)
     # the _mt layouts: num_values = 1 is the plain layout, each further value adds one head row
     for count in (h.tb_atarinet_param_count_mt, h.tb_resnet_param_count_mt):
         old = h.tb_atarinet_param_count if count == h.tb_atarinet_param_count_mt else h.tb_resnet_param_count

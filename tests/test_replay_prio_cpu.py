@@ -126,7 +126,7 @@ def test_constructor_validation():
     assert ReplayBuffer(100, 8, importance_exponent=7).importance_exponent == 7   # unused without priority_exponent
 
 
-def test_entry_points_validate_on_the_host():
+def test_replay_and_loss_entry_points_validate_on_the_host():
     from torchbeast_b200 import _lib
     from torchbeast_b200.replay import _Leaf
     h = _lib.lib()
@@ -167,5 +167,7 @@ def test_entry_points_validate_on_the_host():
     assert "capacity" in mix(cap=4)
     assert "null pointer in leaf 0" in mix(lv=(_Leaf * 1)(_Leaf(None, 512, 1024, 3, 16)))
 
-    args = [dev] * 8 + [4, 4, 6, 0.99, 0.5, 0.01, 1, 1.0, 1.0, None, None] + [dev] * 8 + [1, dev, None]
-    assert h.tb_impala_loss_weighted_f32(*args) != 0 and b"column_weights" in h.tb_last_error()
+    # PopArt (a task) with importance weights has no kernel
+    args = ([dev] * 8 + [4, 4, 6, 0.99, 0.5, 0.01, 1, 1.0, 1.0, None, dev, dev, dev, dev, 3, dev] + [None] * 3
+            + [dev] * 8 + [1, dev, None])
+    assert h.tb_impala_loss_f32(*args) != 0 and b"column_weights" in h.tb_last_error()

@@ -121,13 +121,18 @@ def test_flag_validation():
             trust_region_kl(_flags(bad))
 
 
-def test_entry_points_are_exported():
+def test_loss_entry_point_is_exported_and_checks_trust_outputs():
     from torchbeast_b200 import _lib
     h = ctypes.CDLL(_lib.LIB_PATH)
-    for name in ("tb_impala_loss_trust_f32", "tb_impala_loss_popart_trust_f32"):
-        assert hasattr(h, name)
-        assert name in _lib.declared_symbols()
-        getattr(_lib.lib(), name)
+    name = "tb_impala_loss_f32"
+    assert hasattr(h, name)
+    assert name in _lib.declared_symbols()
+    P = ctypes.c_void_p(256)  # never dereferenced: every call below fails its host-side checks before a launch
+    for kl, sums in ((None, P), (P, None)):
+        args = ([None] * 8 + [4, 2, A, 0.99, 0.5, 0.0006, 1, 1.0, 1.0] + [None] * 5 + [0, None, P, kl, sums]
+                + [None] * 5 + [P, None, None, 1, P, None])
+        assert getattr(_lib.lib(), name)(*args) != 0
+        assert b"kl_out/trust_out must not be null" in _lib.lib().tb_last_error()
 
 
 def test_trust_on_off_selects_another_graph():

@@ -1,4 +1,4 @@
-"""The trust region of tb_impala_loss_trust_f32 (include/torchbeast_b200.h) restated in float64 NumPy: the KL of every
+"""The trust region of tb_impala_loss_f32 (include/torchbeast_b200.h) restated in float64 NumPy: the KL of every
 row, the mask, V-trace with rho_t * m_t in place of rho_t, the three losses and their closed-form gradients."""
 import numpy as np
 

@@ -30,8 +30,8 @@ ac = torch.randint(0, A, (t, b2), device="cuda", generator=g); dn = (torch.rand(
 outs = [torch.empty(t, b2, device="cuda") for _ in range(5)]
 losses = torch.empty(4, device="cuda"); gl = torch.empty(t + 1, b2, A, device="cuda"); gv = torch.empty(t + 1, b2, device="cuda")
 for _ in range(2):
-    lib.tb_impala_loss_fwd_bwd_f32(p(bl), p(tl), p(ac), p(rw[:, :b2].contiguous()), p(dn), None, p(va[:, :b2].contiguous()), p(bs[:b2].contiguous()),
-                                   t, b2, A, 0.99, 0.5, 0.0006, 1, 1.0, 1.0, *[p(o) for o in outs], p(losses), p(gl), p(gv), 1,
-                                   p(_lib.workspace()), st)
+    lib.tb_impala_loss_f32(p(bl), p(tl), p(ac), p(rw[:, :b2].contiguous()), p(dn), None, p(va[:, :b2].contiguous()), p(bs[:b2].contiguous()),
+                           t, b2, A, 0.99, 0.5, 0.0006, 1, 1.0, 1.0, *[None] * 5, 0, *[None] * 4, *[p(o) for o in outs], p(losses),
+                           p(gl), p(gv), 1, p(_lib.workspace()), st)
 torch.cuda.synchronize()
 print("done", float(losses[3]))

@@ -92,8 +92,9 @@ def main():
         ws = _lib.workspace(); dnu = dn.view(torch.uint8)
 
         def fused():
-            lib.tb_impala_loss_fwd_bwd_f32(p(bl), p(tl), p(ac), p(rw), p(dnu), None, p(va), p(bs), T, B, A, 0.99, 0.5, 0.0006,
-                                           1, 1.0, 1.0, *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(ws), _lib.stream_ptr())
+            lib.tb_impala_loss_f32(p(bl), p(tl), p(ac), p(rw), p(dnu), None, p(va), p(bs), T, B, A, 0.99, 0.5, 0.0006,
+                                   1, 1.0, 1.0, *[None] * 5, 0, *[None] * 4, *[p(o) for o in outs], p(losses), p(gl), p(gv), 1,
+                                   p(ws), _lib.stream_ptr())
 
         med, best = time_kernel(fused, iters, flush)
         med_hot, _ = time_kernel(fused, iters, None)

@@ -27,18 +27,10 @@ _SIGNATURES = {
     "tb_action_log_probs_f64": ([_vp, _vp, _i64, _i64, _vp, _vp], _int),
     "tb_vtrace_from_importance_weights_f32": ([_vp] * 5 + [_i64, _i64, _f32, _f32, _vp, _vp, _vp], _int),
     "tb_vtrace_from_importance_weights_f64": ([_vp] * 5 + [_i64, _i64, _f64, _f64, _vp, _vp, _vp], _int),
-    "tb_impala_loss_fwd_bwd_f32": (
-        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 8 + [_int, _vp, _vp], _int),
     "tb_hparams_layout": ([_vp], _int),
-    "tb_impala_loss_fwd_bwd_hp_f32": ([_vp] * 8 + [_i64, _i64, _i64] + [_vp] * 9 + [_int, _vp, _vp], _int),
-    "tb_impala_loss_popart_f32": (
-        [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 12, _int),
-    "tb_impala_loss_weighted_f32": (
-        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 10 + [_int, _vp, _vp], _int),
-    "tb_impala_loss_trust_f32": (
-        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 10 + [_int] + [_vp] * 5, _int),
-    "tb_impala_loss_popart_trust_f32": (
-        [_vp] * 10 + [_i64] * 4 + [_f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 15, _int),
+    "tb_impala_loss_f32": (
+        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 5 + [_i64] + [_vp] * 12
+        + [_int, _vp, _vp], _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
     "tb_atarinet_param_count_mt": ([_int, _int, _int], _i64),
     "tb_atarinet_forward_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
@@ -135,13 +127,11 @@ _SIGNATURES = {
     "tb_resnet_forward": ([_vp] * 6 + [_i64, _i64, _int, _int, _int] + [_vp] * 6, _int),
     "tb_resnet_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_grad_sumsq_f32": ([_vp, _i64, _vp, _vp, _vp], _int),
-    "tb_clip_rmsprop_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _vp, _vp], _int),
-    "tb_clip_adam_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f64, _f64, _f32, _f32, _int, _vp, _vp, _vp],
-                              _int),
-    "tb_clip_rmsprop_ex_step_f32": ([_vp] * 5 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _f32, _vp, _vp], _int),
-    "tb_clip_rmsprop_step_hp_f32": ([_vp] * 4 + [_i64, _vp, _vp, _vp, _f32, _vp, _vp], _int),
-    "tb_clip_rmsprop_ex_step_hp_f32": ([_vp] * 5 + [_i64, _vp, _vp, _vp, _f32, _vp, _vp], _int),
-    "tb_clip_adam_step_hp_f32": ([_vp] * 4 + [_i64, _vp, _vp, _vp, _f32, _int, _vp, _vp, _vp], _int),
+    "tb_clip_rmsprop_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _vp, _vp, _vp], _int),
+    "tb_clip_adam_step_f32": (
+        [_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f64, _f64, _f32, _f32, _int, _vp, _vp, _vp, _vp], _int),
+    "tb_clip_rmsprop_ex_step_f32": (
+        [_vp] * 5 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp], _int),
     "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),

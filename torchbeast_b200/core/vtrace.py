@@ -107,13 +107,13 @@ def _fused_from_logits(blogits, tlogits, actions, discounts, rewards, values, bo
     outs = [torch.empty((T, B), dtype=torch.float32, device=dev) for _ in range(5)]
     losses = torch.empty(4, dtype=torch.float32, device=dev)
     _lib.check(
-        _lib.lib().tb_impala_loss_fwd_bwd_f32(
+        _lib.lib().tb_impala_loss_f32(
             _lib.ptr(blogits), _lib.ptr(tlogits), _lib.ptr(actions), _lib.ptr(rewards), None, _lib.ptr(discounts),
             _lib.ptr(values), _lib.ptr(bootstrap), T, B, A, 0.0, 0.0, 0.0, 0,
-            _lib.clip_arg(clip_rho), _lib.clip_arg(clip_pg),
+            _lib.clip_arg(clip_rho), _lib.clip_arg(clip_pg), None, None, None, None, None, 0, None, None, None, None,
             *[_lib.ptr(o) for o in outs], _lib.ptr(losses), None, None, 0,
             _lib.ptr(_lib.workspace()), _lib.stream_ptr()),
-        "tb_impala_loss_fwd_bwd_f32")
+        "tb_impala_loss_f32")
     vs, pg, lr, blp, tlp = outs
     return VTraceFromLogitsReturns(vs, pg, lr, blp, tlp)
 

@@ -226,35 +226,42 @@ int tb_grad_sumsq_f32(const float* grads, int64_t n, float* out_sumsq, void* wor
   return check_launch("grad_sumsq_kernel");
 }
 
+// hp == NULL takes the scalar arguments and checks them; else the kernels read the scalars from hp, and momentum_buf is
+// passed as given: the caller passes it exactly when momentum is non-zero.
 int tb_clip_rmsprop_step_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
                              const float* sumsq, float max_norm, const float* lr_device, float lr, float alpha,
-                             float eps, float momentum, float* grad_norm_out, void* stream) {
+                             float eps, float momentum, const tb_hparams* hp, float* grad_norm_out, void* stream) {
   TB_REQUIRE(n >= 0 && sumsq, "tb_clip_rmsprop_step_f32: bad arguments");
   if (n == 0) return 0;
   TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_step_f32: null buffer");
-  TB_REQUIRE(momentum == 0.0f || momentum_buf, "tb_clip_rmsprop_step_f32: momentum needs a buffer");
+  if (!hp) {
+    TB_REQUIRE(momentum == 0.0f || momentum_buf, "tb_clip_rmsprop_step_f32: momentum needs a buffer");
+    if (momentum == 0.0f) momentum_buf = nullptr;
+  }
   int64_t blocks = (n + 255) / 256;
   if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   ProfScope prof("clip_rmsprop", (cudaStream_t)stream);
   clip_rmsprop_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      params, grads, square_avg, momentum != 0.0f ? momentum_buf : nullptr, n, sumsq, max_norm, lr_device, lr, alpha,
-      eps, momentum, nullptr, grad_norm_out);
+      params, grads, square_avg, momentum_buf, n, sumsq, max_norm, lr_device, lr, alpha, eps, momentum, hp,
+      grad_norm_out);
   return check_launch("clip_rmsprop_kernel");
 }
 
 int tb_clip_adam_step_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, const float* sumsq,
                           float max_norm, const float* lr_device, float lr, double beta1, double beta2, float eps,
-                          float weight_decay, int decoupled, int64_t* step_device, float* grad_norm_out, void* stream) {
+                          float weight_decay, int decoupled, int64_t* step_device, const tb_hparams* hp,
+                          float* grad_norm_out, void* stream) {
   TB_REQUIRE(n >= 0 && sumsq && step_device, "tb_clip_adam_step_f32: bad arguments");
   TB_REQUIRE(n == 0 || (params && grads && exp_avg && exp_avg_sq), "tb_clip_adam_step_f32: null buffer");
-  TB_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "tb_clip_adam_step_f32: betas must be in [0, 1)");
+  TB_REQUIRE(hp || (beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0),
+             "tb_clip_adam_step_f32: betas must be in [0, 1)");
   int64_t blocks = (n + 255) / 256;
   if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   if (blocks < 1) blocks = 1;  // n == 0 still counts the step
   ProfScope prof("clip_adam", (cudaStream_t)stream);
   clip_adam_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       params, grads, exp_avg, exp_avg_sq, n, sumsq, max_norm, lr_device, lr, beta1, beta2, eps, weight_decay,
-      decoupled, step_device, nullptr, grad_norm_out);
+      decoupled, step_device, hp, grad_norm_out);
   if (int rc = check_launch("clip_adam_kernel")) return rc;
   adam_step_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_device);
   return check_launch("adam_step_advance_kernel");
@@ -262,66 +269,21 @@ int tb_clip_adam_step_f32(float* params, float* grads, float* exp_avg, float* ex
 
 int tb_clip_rmsprop_ex_step_f32(float* params, float* grads, float* square_avg, float* grad_avg, float* momentum_buf,
                                 int64_t n, const float* sumsq, float max_norm, const float* lr_device, float lr,
-                                float alpha, float eps, float weight_decay, float momentum, float* grad_norm_out,
-                                void* stream) {
+                                float alpha, float eps, float weight_decay, float momentum, const tb_hparams* hp,
+                                float* grad_norm_out, void* stream) {
   TB_REQUIRE(n >= 0 && sumsq, "tb_clip_rmsprop_ex_step_f32: bad arguments");
   if (n == 0) return 0;
   TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_ex_step_f32: null buffer");
-  TB_REQUIRE(momentum == 0.0f || momentum_buf, "tb_clip_rmsprop_ex_step_f32: momentum needs a buffer");
+  if (!hp) {
+    TB_REQUIRE(momentum == 0.0f || momentum_buf, "tb_clip_rmsprop_ex_step_f32: momentum needs a buffer");
+    if (momentum == 0.0f) momentum_buf = nullptr;
+  }
   int64_t blocks = (n + 255) / 256;
   if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   ProfScope prof("clip_rmsprop_ex", (cudaStream_t)stream);
   clip_rmsprop_ex_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      params, grads, square_avg, grad_avg, momentum != 0.0f ? momentum_buf : nullptr, n, sumsq, max_norm, lr_device, lr,
-      alpha, eps, weight_decay, momentum, nullptr, grad_norm_out);
-  return check_launch("clip_rmsprop_ex_kernel");
-}
-
-// The _hp entry points launch the same kernels with the same grids and profile records; the kernels read the
-// scalars from hp.  momentum_buf is passed as given: the caller passes it exactly when momentum is non-zero.
-int tb_clip_rmsprop_step_hp_f32(float* params, float* grads, float* square_avg, float* momentum_buf, int64_t n,
-                                const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr,
-                                float* grad_norm_out, void* stream) {
-  TB_REQUIRE(n >= 0 && sumsq && hp, "tb_clip_rmsprop_step_hp_f32: bad arguments");
-  if (n == 0) return 0;
-  TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_step_hp_f32: null buffer");
-  int64_t blocks = (n + 255) / 256;
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-  ProfScope prof("clip_rmsprop", (cudaStream_t)stream);
-  clip_rmsprop_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      params, grads, square_avg, momentum_buf, n, sumsq, 0.0f, lr_device, lr, 0.0f, 0.0f, 0.0f, hp, grad_norm_out);
-  return check_launch("clip_rmsprop_kernel");
-}
-
-int tb_clip_adam_step_hp_f32(float* params, float* grads, float* exp_avg, float* exp_avg_sq, int64_t n,
-                             const float* sumsq, const tb_hparams* hp, const float* lr_device, float lr, int decoupled,
-                             int64_t* step_device, float* grad_norm_out, void* stream) {
-  TB_REQUIRE(n >= 0 && sumsq && hp && step_device, "tb_clip_adam_step_hp_f32: bad arguments");
-  TB_REQUIRE(n == 0 || (params && grads && exp_avg && exp_avg_sq), "tb_clip_adam_step_hp_f32: null buffer");
-  int64_t blocks = (n + 255) / 256;
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-  if (blocks < 1) blocks = 1;  // n == 0 still counts the step
-  ProfScope prof("clip_adam", (cudaStream_t)stream);
-  clip_adam_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      params, grads, exp_avg, exp_avg_sq, n, sumsq, 0.0f, lr_device, lr, 0.0, 0.0, 0.0f, 0.0f, decoupled, step_device,
-      hp, grad_norm_out);
-  if (int rc = check_launch("clip_adam_kernel")) return rc;
-  adam_step_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(step_device);
-  return check_launch("adam_step_advance_kernel");
-}
-
-int tb_clip_rmsprop_ex_step_hp_f32(float* params, float* grads, float* square_avg, float* grad_avg,
-                                   float* momentum_buf, int64_t n, const float* sumsq, const tb_hparams* hp,
-                                   const float* lr_device, float lr, float* grad_norm_out, void* stream) {
-  TB_REQUIRE(n >= 0 && sumsq && hp, "tb_clip_rmsprop_ex_step_hp_f32: bad arguments");
-  if (n == 0) return 0;
-  TB_REQUIRE(params && grads && square_avg, "tb_clip_rmsprop_ex_step_hp_f32: null buffer");
-  int64_t blocks = (n + 255) / 256;
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-  ProfScope prof("clip_rmsprop_ex", (cudaStream_t)stream);
-  clip_rmsprop_ex_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      params, grads, square_avg, grad_avg, momentum_buf, n, sumsq, 0.0f, lr_device, lr, 0.0f, 0.0f, 0.0f, 0.0f, hp,
-      grad_norm_out);
+      params, grads, square_avg, grad_avg, momentum_buf, n, sumsq, max_norm, lr_device, lr, alpha, eps, weight_decay,
+      momentum, hp, grad_norm_out);
   return check_launch("clip_rmsprop_ex_kernel");
 }
 

@@ -543,7 +543,7 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 // compile none of that code.  kWeighted: every term of column b is multiplied by LossArgs::column_weights[b], after the
 // unweighted term is formed, so a weight of 1.0f gives the unweighted bits; the other instantiations compile no weight
 // code.  kTrust: row (t, b) with kl_t = KL(pi_t || mu_t) > beta (or NaN) runs the V-trace and the policy gradient with
-// rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_trust_f32); the other instantiations compile no trust code.
+// rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_f32); the other instantiations compile no trust code.
 template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
   if (p.hp) load_hparams(p);
@@ -846,18 +846,53 @@ static int reduce_grid(int64_t N, int threads) {
   return int(blocks < 1 ? 1 : blocks);
 }
 
-// Both loss entry points: hp == nullptr takes the scalar arguments, else the kernel reads them from hp.
-static int launch_impala_loss(const float* blogits, const float* tlogits, const int64_t* actions,
-                              const float* rewards, const uint8_t* done, const float* discounts,
-                              const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
-                              float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
-                              float clip_rho, float clip_pg_rho, const tb_hparams* hp, float* vs, float* pg_adv,
-                              float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
-                              float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream,
-                              const int64_t* task = nullptr, const double* pa_mu = nullptr,
-                              const double* pa_nu = nullptr, int K = 0, double* task_sums = nullptr,
-                              const float* column_weights = nullptr, const float* trust_beta = nullptr,
-                              float* kl_out = nullptr, float* trust_out = nullptr) {
+}  // namespace tb
+
+// ========================================================================================
+// C ABI
+// ========================================================================================
+using namespace tb;
+
+extern "C" {
+
+int tb_action_log_probs_f32(const float* l, const int64_t* a, int64_t N, int64_t A, float* o, void* s) {
+  return launch_alp<float>(l, a, N, A, o, s);
+}
+int tb_action_log_probs_f64(const double* l, const int64_t* a, int64_t N, int64_t A, double* o, void* s) {
+  return launch_alp<double>(l, a, N, A, o, s);
+}
+
+int tb_vtrace_from_importance_weights_f32(const float* lr, const float* d, const float* r, const float* v,
+                                          const float* bs, int64_t T, int64_t B, float c1, float c2,
+                                          float* vs, float* pg, void* s) {
+  return launch_scan<float>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
+}
+int tb_vtrace_from_importance_weights_f64(const double* lr, const double* d, const double* r, const double* v,
+                                          const double* bs, int64_t T, int64_t B, double c1, double c2,
+                                          double* vs, double* pg, void* s) {
+  return launch_scan<double>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
+}
+
+// The kernel instantiation follows from which of column_weights, task and trust_beta are non-NULL.
+int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
+                       const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
+                       int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
+                       int clip_rewards, float clip_rho, float clip_pg_rho, const tb_hparams* hp,
+                       const float* column_weights, const int64_t* task, const double* mu, const double* nu,
+                       int64_t K, double* task_sums, const float* trust_beta, float* kl_out, float* trust_out,
+                       float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
+                       float* losses_out, float* grad_logits, float* grad_values, int zero_tail, void* workspace,
+                       void* stream) {
+  if (task) {
+    TB_REQUIRE(!column_weights, "impala_loss_popart: column_weights are not supported with PopArt (task)");
+    TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
+               (long long)B, (long long)A);
+    TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "impala_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
+               kPopArtMaxTasks);
+    TB_REQUIRE(values && mu && nu && task_sums, "impala_loss_popart: null PopArt pointer");
+    TB_REQUIRE(zero_tail == 1, "impala_loss_popart: zero_tail must be 1");
+    bootstrap = values;  // not read: the bootstrap row is row T of values
+  }
   TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "impala_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
              (long long)B, (long long)A);
   TB_REQUIRE(losses_out && workspace, "impala_loss: losses_out/workspace must not be null");
@@ -888,7 +923,7 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   p.losses = losses_out; p.grad_logits = grad_logits; p.grad_values = grad_values; p.zero_tail = zero_tail;
   p.workspace = workspace;
   p.hp = hp;
-  p.task = task; p.pa_mu = pa_mu; p.pa_nu = pa_nu; p.K = K;
+  p.task = task; p.pa_mu = mu; p.pa_nu = nu; p.K = int(K);
   p.column_weights = column_weights;
   p.trust_beta = trust_beta; p.kl = kl_out; p.trust_out = trust_out;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
@@ -913,7 +948,8 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
       TB_DISPATCH_A(A, (impala_loss_kernel<kA, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
       TB_TRY(check_launch("impala_loss_kernel<popart>"));
     }
-    popart_task_sums_kernel<<<K, kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, K, task_sums);
+    popart_task_sums_kernel<<<unsigned(K), kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, int(K),
+                                                                                       task_sums);
     return check_launch("popart_task_sums_kernel");
   }
   if (trust_beta) {
@@ -933,128 +969,6 @@ static int launch_impala_loss(const float* blogits, const float* tlogits, const 
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
   TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
   return check_launch("impala_loss_kernel");
-}
-
-}  // namespace tb
-
-// ========================================================================================
-// C ABI
-// ========================================================================================
-using namespace tb;
-
-extern "C" {
-
-int tb_action_log_probs_f32(const float* l, const int64_t* a, int64_t N, int64_t A, float* o, void* s) {
-  return launch_alp<float>(l, a, N, A, o, s);
-}
-int tb_action_log_probs_f64(const double* l, const int64_t* a, int64_t N, int64_t A, double* o, void* s) {
-  return launch_alp<double>(l, a, N, A, o, s);
-}
-
-int tb_vtrace_from_importance_weights_f32(const float* lr, const float* d, const float* r, const float* v,
-                                          const float* bs, int64_t T, int64_t B, float c1, float c2,
-                                          float* vs, float* pg, void* s) {
-  return launch_scan<float>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
-}
-int tb_vtrace_from_importance_weights_f64(const double* lr, const double* d, const double* r, const double* v,
-                                          const double* bs, int64_t T, int64_t B, double c1, double c2,
-                                          double* vs, double* pg, void* s) {
-  return launch_scan<double>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
-}
-
-int tb_impala_loss_fwd_bwd_f32(const float* blogits, const float* tlogits, const int64_t* actions,
-                               const float* rewards, const uint8_t* done, const float* discounts,
-                               const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
-                               float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
-                               float clip_rho, float clip_pg_rho, float* vs, float* pg_adv, float* log_rhos,
-                               float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
-                               float* grad_values, int zero_tail, void* workspace, void* stream) {
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
-                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, nullptr,
-                            vs, pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
-                            zero_tail, workspace, stream);
-}
-
-int tb_impala_loss_fwd_bwd_hp_f32(const float* blogits, const float* tlogits, const int64_t* actions,
-                                  const float* rewards, const uint8_t* done, const float* discounts,
-                                  const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
-                                  const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
-                                  float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
-                                  float* grad_values, int zero_tail, void* workspace, void* stream) {
-  TB_REQUIRE(hp, "impala_loss: null hyper-parameter block");
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A, 0.0f,
-                            0.0f, 0.0f, 0, -1.0f, -1.0f, hp, vs, pg_adv, log_rhos, behavior_alp, target_alp,
-                            losses_out, grad_logits, grad_values, zero_tail, workspace, stream);
-}
-
-int tb_impala_loss_popart_f32(const float* blogits, const float* tlogits, const int64_t* actions,
-                              const float* rewards, const uint8_t* done, const float* discounts,
-                              const float* values, const int64_t* task, const double* mu, const double* nu,
-                              int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
-                              float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
-                              const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
-                              float* target_alp, float* losses_out, float* grad_logits, float* grad_values,
-                              double* task_sums, void* workspace, void* stream) {
-  TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
-             (long long)B, (long long)A);
-  TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "impala_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
-             kPopArtMaxTasks);
-  TB_REQUIRE(values && task && mu && nu && task_sums, "impala_loss_popart: null PopArt pointer");
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, values, T, B, A, discounting,
-                            baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs, pg_adv, log_rhos,
-                            behavior_alp, target_alp, losses_out, grad_logits, grad_values, 1, workspace, stream, task,
-                            mu, nu, int(K), task_sums);
-}
-
-int tb_impala_loss_weighted_f32(const float* blogits, const float* tlogits, const int64_t* actions,
-                                const float* rewards, const uint8_t* done, const float* discounts,
-                                const float* values, const float* bootstrap, int64_t T, int64_t B, int64_t A,
-                                float discounting, float baseline_cost, float entropy_cost, int clip_rewards,
-                                float clip_rho, float clip_pg_rho, const float* column_weights, const tb_hparams* hp,
-                                float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
-                                float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
-                                void* workspace, void* stream) {
-  TB_REQUIRE(column_weights, "impala_loss_weighted: null column_weights");
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
-                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs,
-                            pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
-                            zero_tail, workspace, stream, nullptr, nullptr, nullptr, 0, nullptr, column_weights);
-}
-
-int tb_impala_loss_trust_f32(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
-                             const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
-                             int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
-                             int clip_rewards, float clip_rho, float clip_pg_rho, const float* column_weights,
-                             const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
-                             float* target_alp, float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
-                             const float* trust_beta, float* kl_out, float* trust_out, void* workspace, void* stream) {
-  TB_REQUIRE(trust_beta, "impala_loss_trust: null trust_beta");
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A,
-                            discounting, baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs,
-                            pg_adv, log_rhos, behavior_alp, target_alp, losses_out, grad_logits, grad_values,
-                            zero_tail, workspace, stream, nullptr, nullptr, nullptr, 0, nullptr, column_weights,
-                            trust_beta, kl_out, trust_out);
-}
-
-int tb_impala_loss_popart_trust_f32(const float* blogits, const float* tlogits, const int64_t* actions,
-                                    const float* rewards, const uint8_t* done, const float* discounts,
-                                    const float* values, const int64_t* task, const double* mu, const double* nu,
-                                    int64_t T, int64_t B, int64_t A, int64_t K, float discounting, float baseline_cost,
-                                    float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
-                                    const tb_hparams* hp, float* vs, float* pg_adv, float* log_rhos,
-                                    float* behavior_alp, float* target_alp, float* losses_out, float* grad_logits,
-                                    float* grad_values, double* task_sums, const float* trust_beta, float* kl_out,
-                                    float* trust_out, void* workspace, void* stream) {
-  TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
-             (long long)B, (long long)A);
-  TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "impala_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
-             kPopArtMaxTasks);
-  TB_REQUIRE(values && task && mu && nu && task_sums, "impala_loss_popart: null PopArt pointer");
-  TB_REQUIRE(trust_beta, "impala_loss_popart_trust: null trust_beta");
-  return launch_impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, values, T, B, A, discounting,
-                            baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, vs, pg_adv, log_rhos,
-                            behavior_alp, target_alp, losses_out, grad_logits, grad_values, 1, workspace, stream, task,
-                            mu, nu, int(K), task_sums, nullptr, trust_beta, kl_out, trust_out);
 }
 
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,

@@ -17,7 +17,7 @@ ImpalaLoss = collections.namedtuple(
 # float32 [2] = {number of trusted rows, sum of kl over all rows}.
 TrustRegion = collections.namedtuple("TrustRegion", "kl sums")
 
-# tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the *_hp entry points read from device memory.
+# tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the entry points read from device memory.
 # tb_hparams_layout() reports the compiled layout; tests/test_graph_hparams_cpu.py checks this record against it.
 HPARAMS = np.dtype([
     ("beta1", "<f8"), ("beta2", "<f8"), ("discounting", "<f4"), ("baseline_cost", "<f4"), ("entropy_cost", "<f4"),
@@ -113,7 +113,7 @@ def impala_loss_fwd_bwd(
     column_weights=None,
     trust_region=None,
 ):
-    """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_fwd_bwd_f32).
+    """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_f32).
 
     Inputs are the shifted [T,B,...] slices (batch[1:], learner_outputs[:-1]); `done` is a
     bool/uint8 tensor.  Replaces monobeast.py:245-277 / polybeast_learner.py:332-361 and the
@@ -126,13 +126,13 @@ def impala_loss_fwd_bwd(
     are not used: a captured CUDA graph then follows what is published between replays.
 
     With `column_weights` (float32 [B], device) the pg, baseline and entropy terms of column b, in the losses and the
-    gradients, are multiplied by column_weights[b] (tb_impala_loss_weighted_f32, prioritised replay's importance
-    weights); weights of 1.0 give the unweighted bits.
+    gradients, are multiplied by column_weights[b] (prioritised replay's importance weights); weights of 1.0 give the
+    unweighted bits.
 
     With `trust_region` (beta: a float >= 0, or a float32 device scalar read when the kernel runs) a row whose
-    KL(pi || mu) exceeds beta gets rho = 0 in the V-trace and the policy gradient (tb_impala_loss_trust_f32; the rule
-    is stated in include/torchbeast_b200.h), and the call returns (ImpalaLoss, TrustRegion).  vs and pg_advantages
-    are the masked ones; log_rhos and the log-probabilities are not masked.
+    KL(pi || mu) exceeds beta gets rho = 0 in the V-trace and the policy gradient (the rule is stated with
+    tb_impala_loss_f32 in include/torchbeast_b200.h), and the call returns (ImpalaLoss, TrustRegion).  vs and
+    pg_advantages are the masked ones; log_rhos and the log-probabilities are not masked.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
@@ -141,77 +141,11 @@ def impala_loss_fwd_bwd(
         if column_weights.dtype != torch.float32 or column_weights.numel() != target_policy_logits.shape[1]:
             raise _lib.TorchBeastB200Error("column_weights must be float32 [%d], got %s %r" % (
                 target_policy_logits.shape[1], column_weights.dtype, tuple(column_weights.shape)))
-    if hparams_dev is None:
-        clip_rewards = _clip_rewards(reward_clipping)
-    else:
-        _lib.require_cuda(hparams_dev)
-        discounting = hparams_field(hparams_dev, "discounting")  # uint8 done: the discounts below read the block
-    T, B, A = target_policy_logits.shape
-    dev = values.device
-    f32 = torch.float32
-    bl = behavior_policy_logits.to(f32).contiguous()
-    tl = target_policy_logits.detach().to(f32).contiguous()
-    ac = actions.to(torch.int64).contiguous()
-    rw = rewards.to(f32).contiguous()
-    if done.dtype == torch.bool:
-        dn = done.contiguous().view(torch.uint8)
-        disc = None
-    elif done.dtype == torch.uint8:
-        # `~done` on uint8 is a bitwise NOT in the reference (SURVEY Appendix A): discount = (255-done)*gamma
-        dn, disc = None, ((~done).to(f32) * discounting).contiguous()
-    else:
-        raise _lib.TorchBeastB200Error("done must be bool or uint8")
-    va = values.detach().to(f32).contiguous()
-    bs = bootstrap_value.detach().to(f32).contiguous()
-    outs = [torch.empty((T, B), dtype=f32, device=dev) for _ in range(5)]
-    losses = torch.empty(4, dtype=f32, device=dev)
-    gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
-    gv = torch.empty((T + 1, B), dtype=f32, device=dev) if with_grads else None
-    if trust_region is not None:
-        p = _lib.ptr
-        beta = _trust_beta_tensor(trust_region, dev)
-        trust = TrustRegion(torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev))
-        cw = None if column_weights is None else column_weights.contiguous()
-        _lib.check(
-            _lib.lib().tb_impala_loss_trust_f32(
-                p(bl), p(tl), p(ac), p(rw), p(dn), p(disc), p(va), p(bs), T, B, A,
-                0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
-                0 if hparams_dev is not None else clip_rewards, _lib.clip_arg(clip_rho_threshold),
-                _lib.clip_arg(clip_pg_rho_threshold), p(cw), p(hparams_dev),
-                *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(beta), p(trust.kl), p(trust.sums),
-                p(_lib.workspace()), _lib.stream_ptr()),
-            "tb_impala_loss_trust_f32")
-        return ImpalaLoss(*outs, losses, gl, gv), trust
-    if column_weights is not None:
-        p = _lib.ptr
-        _lib.check(
-            _lib.lib().tb_impala_loss_weighted_f32(
-                p(bl), p(tl), p(ac), p(rw), p(dn), p(disc), p(va), p(bs), T, B, A,
-                0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
-                0 if hparams_dev is not None else clip_rewards, _lib.clip_arg(clip_rho_threshold),
-                _lib.clip_arg(clip_pg_rho_threshold), p(column_weights.contiguous()), p(hparams_dev),
-                *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(_lib.workspace()), _lib.stream_ptr()),
-            "tb_impala_loss_weighted_f32")
-        return ImpalaLoss(*outs, losses, gl, gv)
-    if hparams_dev is not None:
-        _lib.check(
-            _lib.lib().tb_impala_loss_fwd_bwd_hp_f32(
-                _lib.ptr(bl), _lib.ptr(tl), _lib.ptr(ac), _lib.ptr(rw), _lib.ptr(dn), _lib.ptr(disc),
-                _lib.ptr(va), _lib.ptr(bs), T, B, A, _lib.ptr(hparams_dev),
-                *[_lib.ptr(o) for o in outs], _lib.ptr(losses), _lib.ptr(gl), _lib.ptr(gv), 1,
-                _lib.ptr(_lib.workspace()), _lib.stream_ptr()),
-            "tb_impala_loss_fwd_bwd_hp_f32")
-        return ImpalaLoss(*outs, losses, gl, gv)
-    _lib.check(
-        _lib.lib().tb_impala_loss_fwd_bwd_f32(
-            _lib.ptr(bl), _lib.ptr(tl), _lib.ptr(ac), _lib.ptr(rw), _lib.ptr(dn), _lib.ptr(disc),
-            _lib.ptr(va), _lib.ptr(bs), T, B, A, float(discounting), float(baseline_cost), float(entropy_cost),
-            clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold),
-            *[_lib.ptr(o) for o in outs], _lib.ptr(losses), _lib.ptr(gl), _lib.ptr(gv), 1,
-            _lib.ptr(_lib.workspace()), _lib.stream_ptr()),
-        "tb_impala_loss_fwd_bwd_f32")
-    vs, pg, lr, blp, tlp = outs
-    return ImpalaLoss(vs, pg, lr, blp, tlp, losses, gl, gv)
+    loss, _, trust = _impala_loss(
+        behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value, discounting,
+        baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, with_grads,
+        hparams_dev, column_weights=column_weights, trust_region=trust_region)
+    return loss if trust is None else (loss, trust)
 
 
 @torch.no_grad()
@@ -234,15 +168,15 @@ def impala_loss_popart(
     hparams_dev=None,
     trust_region=None,
 ):
-    """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_popart_f32).
+    """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_f32 with a task).
 
     `values` is the normalised head output n [T+1, B, K] with its bootstrap row, `task` int64 [T+1, B] the task of each
     of those rows, `mu` / `nu` float64 [K] the statistics.  The V-trace runs on sigma_k * n[k] + mu_k; vs and
     pg_advantages are unnormalised, the losses and gradients are taken in normalised space, and grad_values is
     [T+1, B, K].  A row with a task id outside [0, K) adds no loss and gets zero gradient rows.  Returns
     (ImpalaLoss, task_sums): task_sums float64 [3, K] = per-task count, sum vs, sum vs^2 over rows t < T, the input
-    of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd;
-    tb_impala_loss_popart_trust_f32) it returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs."""
+    of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd) it
+    returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs."""
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
     _lib.require_cuda(*tensors)
     T, B, A = target_policy_logits.shape
@@ -252,51 +186,65 @@ def impala_loss_popart(
                                        % (T, B, tuple(values.shape), tuple(task.shape)))
     if mu.dtype != torch.float64 or nu.dtype != torch.float64 or mu.numel() != K or nu.numel() != K:
         raise _lib.TorchBeastB200Error("PopArt mu / nu must be float64 [%d]" % K)
+    loss, sums, trust = _impala_loss(
+        behavior_policy_logits, target_policy_logits, actions, rewards, done, values, None, discounting,
+        baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, True, hparams_dev,
+        popart=(task, mu, nu), trust_region=trust_region)
+    return (loss, sums) if trust is None else (loss, sums, trust)
+
+
+def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value,
+                 discounting, baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold,
+                 with_grads, hparams_dev, column_weights=None, popart=None, trust_region=None):
+    """The one tb_impala_loss_f32 call behind impala_loss_fwd_bwd and impala_loss_popart, on inputs they checked.
+    popart: None, or (task, mu, nu) with values [T+1, B, K].  Returns (ImpalaLoss, task_sums or None, TrustRegion or
+    None)."""
     if hparams_dev is None:
         clip_rewards = _clip_rewards(reward_clipping)
     else:
         _lib.require_cuda(hparams_dev)
-        discounting = hparams_field(hparams_dev, "discounting")
+        discounting = hparams_field(hparams_dev, "discounting")  # uint8 done: the discounts below read the block
         clip_rewards = 0
+    T, B, A = target_policy_logits.shape
     dev = values.device
     f32 = torch.float32
     if done.dtype == torch.bool:
         dn, disc = done.contiguous().view(torch.uint8), None
     elif done.dtype == torch.uint8:
-        dn, disc = None, ((~done).to(f32) * discounting).contiguous()  # see impala_loss_fwd_bwd
+        # `~done` on uint8 is a bitwise NOT in the reference (SURVEY Appendix A): discount = (255-done)*gamma
+        dn, disc = None, ((~done).to(f32) * discounting).contiguous()
     else:
         raise _lib.TorchBeastB200Error("done must be bool or uint8")
-    outs = [torch.empty((T, B), dtype=f32, device=dev) for _ in range(5)]
-    losses = torch.empty(4, dtype=f32, device=dev)
-    gl = torch.empty((T + 1, B, A), dtype=f32, device=dev)
-    gv = torch.empty((T + 1, B, K), dtype=f32, device=dev)
-    sums = torch.empty((3, K), dtype=torch.float64, device=dev)
-    p = _lib.ptr
+    task = mu = nu = sums = bs = None
+    K = 0
+    if popart is not None:
+        task, mu, nu = popart
+        K = values.shape[-1]
+        task, mu, nu = task.to(torch.int64).contiguous(), mu.contiguous(), nu.contiguous()
+        sums = torch.empty((3, K), dtype=torch.float64, device=dev)
+    else:
+        bs = bootstrap_value.detach().to(f32).contiguous()
+    beta = kl = kl_sums = None
     if trust_region is not None:
         beta = _trust_beta_tensor(trust_region, dev)
-        trust = TrustRegion(torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev))
-        _lib.check(
-            _lib.lib().tb_impala_loss_popart_trust_f32(
-                p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
-                p(actions.to(torch.int64).contiguous()), p(rewards.to(f32).contiguous()), p(dn), p(disc),
-                p(values.detach().to(f32).contiguous()), p(task.to(torch.int64).contiguous()), p(mu.contiguous()),
-                p(nu.contiguous()), T, B, A, K, float(discounting) if hparams_dev is None else 0.0,
-                float(baseline_cost), float(entropy_cost), clip_rewards, _lib.clip_arg(clip_rho_threshold),
-                _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev), *[p(o) for o in outs], p(losses), p(gl), p(gv),
-                p(sums), p(beta), p(trust.kl), p(trust.sums), p(_lib.workspace()), _lib.stream_ptr()),
-            "tb_impala_loss_popart_trust_f32")
-        return ImpalaLoss(*outs, losses, gl, gv), sums, trust
+        kl, kl_sums = torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev)
+    cw = None if column_weights is None else column_weights.contiguous()
+    outs = [torch.empty((T, B), dtype=f32, device=dev) for _ in range(5)]
+    losses = torch.empty(4, dtype=f32, device=dev)
+    gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
+    gv = torch.empty((T + 1, B) + ((K,) if popart is not None else ()), dtype=f32, device=dev) if with_grads else None
+    p = _lib.ptr
     _lib.check(
-        _lib.lib().tb_impala_loss_popart_f32(
+        _lib.lib().tb_impala_loss_f32(
             p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
             p(actions.to(torch.int64).contiguous()), p(rewards.to(f32).contiguous()), p(dn), p(disc),
-            p(values.detach().to(f32).contiguous()), p(task.to(torch.int64).contiguous()), p(mu.contiguous()),
-            p(nu.contiguous()), T, B, A, K, float(discounting) if hparams_dev is None else 0.0, float(baseline_cost),
-            float(entropy_cost), clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold),
-            p(hparams_dev), *[p(o) for o in outs], p(losses), p(gl), p(gv), p(sums), p(_lib.workspace()),
-            _lib.stream_ptr()),
-        "tb_impala_loss_popart_f32")
-    return ImpalaLoss(*outs, losses, gl, gv), sums
+            p(values.detach().to(f32).contiguous()), p(bs), T, B, A,
+            0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
+            clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev),
+            p(cw), p(task), p(mu), p(nu), K, p(sums), p(beta), p(kl), p(kl_sums),
+            *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(_lib.workspace()), _lib.stream_ptr()),
+        "tb_impala_loss_f32")
+    return ImpalaLoss(*outs, losses, gl, gv), sums, None if beta is None else TrustRegion(kl, kl_sums)
 
 
 @torch.no_grad()

@@ -5,7 +5,7 @@ Mirror of compute_baseline_loss / compute_entropy_loss / compute_policy_gradient
 names, sum reduction, float32 or float64 inputs, advantages receive no gradient.  Each
 forward is one launch that also emits the closed-form gradient (SURVEY.md 8(a) A4); the
 backward only scales it by the incoming scalar.  learn() does not use these - it calls the
-fully fused kernel (tb_impala_loss_fwd_bwd_f32) - they exist for API parity.
+fully fused kernel (tb_impala_loss_f32) - they exist for API parity.
 """
 import torch
 

@@ -202,34 +202,20 @@ class RMSprop(FusedOptimizer):
     def _update(self, flat, grad, max_norm, lr_device, stream, hparams_dev=None):
         group = self.param_groups[0]
         lib, p = _lib.lib(), _lib.ptr
-        if hparams_dev is not None:
-            mom = self.momentum_buffer if self._momentum_on() else None
-            if self._entry() == "tb_clip_rmsprop_step_f32":
-                _lib.check(
-                    lib.tb_clip_rmsprop_step_hp_f32(
-                        p(flat), p(grad), p(self.square_avg), p(mom), flat.numel(), p(self._sumsq), p(hparams_dev),
-                        lr_device, float(group["lr"]), p(self.grad_norm), stream),
-                    "tb_clip_rmsprop_step_hp_f32")
-            else:
-                _lib.check(
-                    lib.tb_clip_rmsprop_ex_step_hp_f32(
-                        p(flat), p(grad), p(self.square_avg), p(self.grad_avg), p(mom), flat.numel(), p(self._sumsq),
-                        p(hparams_dev), lr_device, float(group["lr"]), p(self.grad_norm), stream),
-                    "tb_clip_rmsprop_ex_step_hp_f32")
-        elif self.grad_avg is None and group["weight_decay"] == 0:
+        mom = self.momentum_buffer if self._momentum_on() else None
+        if self._entry() == "tb_clip_rmsprop_step_f32":
             _lib.check(
                 lib.tb_clip_rmsprop_step_f32(
-                    p(flat), p(grad), p(self.square_avg), p(self.momentum_buffer), flat.numel(), p(self._sumsq),
-                    max_norm, lr_device, float(group["lr"]), float(group["alpha"]), float(group["eps"]),
-                    float(group["momentum"]), p(self.grad_norm), stream),
+                    p(flat), p(grad), p(self.square_avg), p(mom), flat.numel(), p(self._sumsq), max_norm, lr_device,
+                    float(group["lr"]), float(group["alpha"]), float(group["eps"]), float(group["momentum"]),
+                    p(hparams_dev), p(self.grad_norm), stream),
                 "tb_clip_rmsprop_step_f32")
         else:
             _lib.check(
                 lib.tb_clip_rmsprop_ex_step_f32(
-                    p(flat), p(grad), p(self.square_avg), p(self.grad_avg), p(self.momentum_buffer), flat.numel(),
-                    p(self._sumsq), max_norm, lr_device, float(group["lr"]), float(group["alpha"]),
-                    float(group["eps"]), float(group["weight_decay"]), float(group["momentum"]), p(self.grad_norm),
-                    stream),
+                    p(flat), p(grad), p(self.square_avg), p(self.grad_avg), p(mom), flat.numel(), p(self._sumsq),
+                    max_norm, lr_device, float(group["lr"]), float(group["alpha"]), float(group["eps"]),
+                    float(group["weight_decay"]), float(group["momentum"]), p(hparams_dev), p(self.grad_norm), stream),
                 "tb_clip_rmsprop_ex_step_f32")
         self._steps += 1
 
@@ -304,20 +290,12 @@ class Adam(FusedOptimizer):
         group = self.param_groups[0]
         beta1, beta2 = group["betas"]
         p = _lib.ptr
-        if hparams_dev is not None:
-            _lib.check(
-                _lib.lib().tb_clip_adam_step_hp_f32(
-                    p(flat), p(grad), p(self.exp_avg), p(self.exp_avg_sq), flat.numel(), p(self._sumsq),
-                    p(hparams_dev), lr_device, float(group["lr"]), int(bool(group["decoupled_weight_decay"])),
-                    p(self.step_device), p(self.grad_norm), stream),
-                "tb_clip_adam_step_hp_f32")
-            return
         _lib.check(
             _lib.lib().tb_clip_adam_step_f32(
                 p(flat), p(grad), p(self.exp_avg), p(self.exp_avg_sq), flat.numel(), p(self._sumsq), max_norm,
                 lr_device, float(group["lr"]), float(beta1), float(beta2), float(group["eps"]),
                 float(group["weight_decay"]), int(bool(group["decoupled_weight_decay"])), p(self.step_device),
-                p(self.grad_norm), stream),
+                p(hparams_dev), p(self.grad_norm), stream),
             "tb_clip_adam_step_f32")
 
     def state_dict(self):
