@@ -169,93 +169,6 @@ int tb_impala_loss_f32(const float* behavior_logits, const float* target_logits,
  *   not touch optimizer state.  One launch, no host sync; graph-capturable.                                    */
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,
                      float* bias, int64_t F, void* stream);
-/* Nets with num_values (1..64) value outputs, one per task: the tb_atarinet_* / tb_resnet_* entry points of the same
- * name without _mt are their num_values = 1 case.  Parameter layout: baseline.weight [num_values, F] and
- * baseline.bias [num_values] in place of [1, F] / [1] (still the last two tensors); baseline / grad_baseline are
- * [T1, B, num_values].  Workspace sizes and tb_atarinet_grad_split do not depend on num_values.                */
-int64_t tb_atarinet_param_count_mt(int num_actions, int num_values, int use_lstm);
-int tb_atarinet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const int64_t* last_action,
-                           const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
-                           int num_actions, int num_values, int use_lstm, int precision, void* workspace,
-                           float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
-int tb_atarinet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                     const int64_t* last_action, const float* h0, const float* c0, const float* params,
-                                     int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
-                                     void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
-                                     float* hN, float* cN, void* stream);
-int tb_atarinet_backward_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                            const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
-                            int precision, void* workspace, float* grads, void* stream);
-int tb_atarinet_backward_phase_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                                  const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
-                                  int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream);
-int64_t tb_resnet_param_count_mt(int num_actions, int num_values, int use_lstm);
-int tb_resnet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
-                         int precision, void* workspace, float* policy_logits, float* baseline, float* hN, float* cN,
-                         void* stream);
-int tb_resnet_backward_mt(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                          const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
-                          int precision, void* workspace, float* grads, void* stream);
-int tb_resnet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                   const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
-                                   int num_actions, int num_values, int use_lstm, int precision, void* workspace,
-                                   void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
-                                   void* stream);
-int tb_resnet_backward_unstacked_mt(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
-                                    const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
-                                    int num_values, int use_lstm, int precision, void* workspace, float* grads,
-                                    void* stream);
-
-/* ---- IMPALA ResNet on other observation shapes ----------------------------------------------------------------------
- * The tb_resnet_*_mt entry points with the observation u8 [C, H, W] as arguments: frame is u8 [T1, B, C, H, W] and the
- * tb_resnet_*_mt entries are the (4, 84, 84) case of these.  Section i's feat conv runs at H_i x W_i (H_0 = H, W_0 = W),
- * its max-pool (3, 2, 1) leaves ceil(H_i / 2) x ceil(W_i / 2) = H_{i+1} x W_{i+1}, and the parameter layout has
- * feat_convs.0.0.weight (16, C, 3, 3) and fc.weight (256, 32 * H_3 * W_3); everything else is as for (4, 84, 84).
- * Supported on every precision: 1 <= C <= 16, 17 <= H <= 126 and 33 <= W <= 126 (17 rows are the fewest that leave the
- * last section 3 high, the smallest image of the split-bf16 conv kernels; 33 columns the fewest that leave it 5 wide, the
- * narrowest row their weight gradient takes; 126 their widest padded row, 128 pixels).  tb_resnet_obs_range writes these
- * bounds as {C min, C max, H min, H max, W min, W max}.  tb_resnet_obs_supported returns 1 for a supported shape and
- * otherwise 0 with tb_last_error set; the other entries fail the same way (param count -1, workspace 0).  Unstacked
- * rollouts stay (4, 84, 84) only.                                                                                     */
-int tb_resnet_obs_range(int* range);
-int tb_resnet_obs_supported(int C, int H, int W, int precision);
-int64_t tb_resnet_param_count_obs(int C, int H, int W, int num_actions, int num_values, int use_lstm);
-size_t tb_resnet_workspace_bytes_obs(int C, int H, int W, int64_t T1, int64_t B, int num_actions, int use_lstm,
-                                     int precision);
-int tb_resnet_forward_obs(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                          const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions,
-                          int num_values, int use_lstm, int precision, void* workspace, float* policy_logits,
-                          float* baseline, float* hN, float* cN, void* stream);
-int tb_resnet_backward_obs(const uint8_t* frame, const float* grad_logits, const float* grad_baseline,
-                           const float* notdone, const float* params, int C, int H, int W, int64_t T1, int64_t B,
-                           int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* grads,
-                           void* stream);
-
-/* ---- IMPALA ResNet with other section widths -------------------------------------------------------------------------
- * The tb_resnet_*_obs entry points with the channel counts (c0, c1, c2) of the three sections after C, H, W; the _obs
- * entries are the (16, 32, 32) case of these.  Each section takes 16, 32 or 64 channels, in any combination, over the
- * whole observation range above, on every precision (tb_resnet_widths writes {16, 32, 64}); e.g. (32, 64, 64) is the
- * "IMPALA x2" net.  Parameter layout (state_dict order, as for the default):
- *   feat_convs.0.0.weight (c0, C, 3, 3), and for i >= 1 feat_convs.i.0.weight (c_i, c_{i-1}, 3, 3); feat_convs.i.0.bias (c_i)
- *   resnet1.i.{1,3}.weight / resnet2.i.{1,3}.weight (c_i, c_i, 3, 3) and their biases (c_i)
- *   fc.weight (256, c2 * H_3 * W_3), fc.bias (256), then the LSTM and the heads unchanged.
- * tb_resnet_arch_supported returns 1 for a supported (shape, widths, precision) and otherwise 0 with tb_last_error set;
- * the other entries fail the same way (param count -1, workspace 0).  Unstacked rollouts stay (4, 84, 84) x (16, 32, 32). */
-int tb_resnet_widths(int* widths);
-int tb_resnet_arch_supported(int C, int H, int W, int c0, int c1, int c2, int precision);
-int64_t tb_resnet_param_count_arch(int C, int H, int W, int c0, int c1, int c2, int num_actions, int num_values,
-                                   int use_lstm);
-size_t tb_resnet_workspace_bytes_arch(int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B,
-                                      int num_actions, int use_lstm, int precision);
-int tb_resnet_forward_arch(const uint8_t* frame, const float* reward, const float* notdone, const float* h0,
-                           const float* c0, const float* params, int C, int H, int W, int ch0, int ch1, int ch2,
-                           int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
-                           void* workspace, float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
-int tb_resnet_backward_arch(const uint8_t* frame, const float* grad_logits, const float* grad_baseline,
-                            const float* notdone, const float* params, int C, int H, int W, int c0, int c1, int c2,
-                            int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
-                            void* workspace, float* grads, void* stream);
 
 /* ---- seeded action sampling for the acting forward ------------------------------------ */
 
@@ -376,51 +289,57 @@ int tb_pg_loss_f32(const float* logits, const int64_t* actions, const float* adv
 int tb_pg_loss_f64(const double* logits, const int64_t* actions, const double* adv, int64_t N, int64_t A,
                    double* out, double* grad, void* workspace, void* stream);
 
-/* ---- AtariNet (monobeast.py:545-635) forward / backward --------------------------------- */
-
-/* Parameters live in ONE flat f32 buffer in the reference's state_dict order and shapes
+/* ---- AtariNet (monobeast.py:545-635) forward / backward ---------------------------------
+ * Parameters live in ONE flat f32 buffer in the reference's state_dict order and shapes
  * (BASELINE.md section 5): conv1.weight (32,4,8,8), conv1.bias, conv2.weight (64,32,4,4), conv2.bias,
  * conv3.weight (64,64,3,3), conv3.bias, fc.weight (512,3136), fc.bias, [core.weight_ih_l0,
  * core.weight_hh_l0, core.bias_ih_l0, core.bias_hh_l0, ...l1 (2076 x 519 each)], policy.weight (A,519),
- * policy.bias, baseline.weight (1,519), baseline.bias.  Gradients use the same layout.       */
-int64_t tb_atarinet_param_count(int num_actions, int use_lstm);
-/* Bytes of caller-owned workspace for a [T1,B] rollout (T1 = unroll_length + 1): patch matrices,
- * activations kept for backward, packed weights, split-K scratch.                            */
-size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision);
-
-/* monobeast.py:582-632 AtariNet.forward (without the action sampling, which the learner never
- * uses - SURVEY.md K8).  frame u8 [T1,B,4,84,84]; reward f32 [T1,B]; last_action i64 [T1,B];
- * notdone f32 [T1,B] = (~done).float() (LSTM only; multiplies the state before each step,
- * monobeast.py:607-609); h0,c0 / hN,cN f32 [2,B,519] (LSTM only).
- * -> policy_logits f32 [T1,B,A], baseline f32 [T1,B].  Activations stay in `workspace`.
+ * policy.bias, baseline.weight (num_values,519), baseline.bias (num_values).  num_values (1..64) is the number of value
+ * outputs, one per PopArt task; 1 is the reference's net.  Gradients use the same layout.
+ * tb_atarinet_workspace_bytes: bytes of caller-owned workspace for a [T1,B] rollout (T1 = unroll_length + 1): patch
+ * matrices, activations kept for backward, packed weights, split-K scratch.  Neither it nor tb_atarinet_grad_split
+ * depends on num_values.
+ *
+ * tb_atarinet_forward: monobeast.py:582-632 AtariNet.forward (without the action sampling, which the learner never
+ * uses - SURVEY.md K8).  reward f32 [T1,B]; last_action i64 [T1,B]; notdone f32 [T1,B] = (~done).float() (LSTM only;
+ * multiplies the state before each step, monobeast.py:607-609); h0,c0 / hN,cN f32 [2,B,519] (LSTM only).
+ * -> policy_logits f32 [T1,B,A], baseline f32 [T1,B,num_values].  Activations stay in `workspace`.
+ *   done == NULL: frame is the stacked u8 [T1,B,4,84,84]; stacked_scratch is not read.
+ *   done != NULL: frame is an unstacked rollout u8 [T1+3,B,84,84] with done [T1,B] (see "unstacked rollouts" below),
+ *     and stacked_scratch is device memory of tb_unstacked_scratch_bytes(0, T1, B, precision) bytes (NULL allowed, and
+ *     not touched, when that is 0).  Outputs and workspace contents are bit-identical to the stacked forward on the
+ *     restacked frames.
  * precision: 0 = fp32 SIMT GEMMs (bit-comparable with the reference's fp32 CPU arithmetic);
  *            1 = bf16 operands with fp32 accumulation: conv/fc trunk (implicit-GEMM convolutions) and LSTM
  *                projections on wgmma tensor cores, LSTM recurrence products as bf16 mma.sync; LSTM state and
- *                gate math, heads, losses, optimizer, master weights and gradients stay fp32.             */
-int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* notdone,
-                        const int64_t* last_action, const float* h0, const float* c0,
-                        const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm,
-                        int precision, void* workspace, float* policy_logits, float* baseline, float* hN,
-                        float* cN, void* stream);
-/* Backward of the above (replaces the autograd graph of total_loss.backward(), monobeast.py:290):
- * grad_logits [T1,B,A], grad_baseline [T1,B] -> grads (flat, parameter layout, overwritten).
- * Must follow a tb_atarinet_forward on the same workspace and parameters.                    */
-int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                         const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm,
-                         int precision, void* workspace, float* grads, void* stream);
-
-/* The same backward in two calls, for data-parallel learners (the reference has a single learner device,
- * polybeast_learner.py:402-405; SURVEY 8(e) G1 "bucket order = reverse of forward"): phase 1 = policy/baseline heads +
- * LSTM, phase 2 = conv/fc trunk.  After phase 2 everything is final; after phase 1 the slice
- * [tb_atarinet_grad_split(), param_count) of `grads` (LSTM + heads: 17 of 24 MB) is final when the LSTM weight-gradient
- * GEMMs ran on the caller's stream; when they were forked onto the side stream (tensor-core backends), the slice is
- * final in STREAM ORDER on that side stream: pass your own with tb_set_aux_stream() (thread-local; NULL = library-owned)
- * before phase 1, make it wait for `stream`, and enqueue the slice's all-reduce on it - it then overlaps phase 2.      */
-int tb_set_aux_stream(void* stream);
+ *                gate math, heads, losses, optimizer, master weights and gradients stay fp32;
+ *            2 = split-bf16 (hi + lo planes) tensor-core products over fp32 activations.
+ *
+ * tb_atarinet_backward: the backward of the forward that last ran on `workspace` with the same parameters (replaces
+ * the autograd graph of total_loss.backward(), monobeast.py:290): grad_logits [T1,B,A], grad_baseline
+ * [T1,B,num_values] -> grads (flat, parameter layout, overwritten).  It reads only the workspace, never the frames.
+ *   phase 3: the whole backward.
+ *   phase 1, then phase 2: the same backward in two calls, for data-parallel learners (the reference has a single
+ *     learner device, polybeast_learner.py:402-405; SURVEY 8(e) G1 "bucket order = reverse of forward"): phase 1 =
+ *     policy/baseline heads + LSTM, phase 2 = conv/fc trunk.  After phase 2 everything is final; after phase 1 the slice
+ *     [tb_atarinet_grad_split(), param_count) of `grads` (LSTM + heads: 17 of 24 MB) is final when the LSTM
+ *     weight-gradient GEMMs ran on the caller's stream; when they were forked onto the side stream (tensor-core
+ *     backends), the slice is final in STREAM ORDER on that side stream: pass your own with tb_set_aux_stream()
+ *     (thread-local; NULL = library-owned) before phase 1, make it wait for `stream`, and enqueue the slice's
+ *     all-reduce on it - it then overlaps phase 2.
+ *   Any other phase is rejected.                                                                                      */
+int64_t tb_atarinet_param_count(int num_actions, int num_values, int use_lstm);
+size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision);
 int64_t tb_atarinet_grad_split(int num_actions, int use_lstm);
-int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                               const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm,
-                               int precision, void* workspace, float* grads, int phase, void* stream);
+int tb_set_aux_stream(void* stream);
+int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                        const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                        int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                        void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                        float* hN, float* cN, void* stream);
+int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                         int precision, void* workspace, float* grads, int phase, void* stream);
 
 /* ---- stacked LSTM over the unroll with per-step done-reset -------------------------------------------
  * Replaces the reference's loop of seq_len-1 nn.LSTM calls and its autograd graph (monobeast.py:603-611,
@@ -471,28 +390,59 @@ int tb_lstm_backward_state(const float* dy, const float* x, const float* notdone
                            int precision, void* workspace, float* dx, const float* dhN, const float* dcN, float* dh0,
                            float* dc0, void* stream);
 
-/* ---- IMPALA ResNet (polybeast_learner.py:134-266 `Net`) forward / backward ------------------------- */
-
-/* Flat parameter layout = the reference's state_dict order: feat_convs.{0,1,2}.0.{weight,bias}
- * ((16,4,3,3) (32,16,3,3) (32,32,3,3)), resnet1.{0,1,2}.{1,3}.{weight,bias}, resnet2.{0,1,2}.{1,3}.{weight,bias},
- * fc.{weight (256,3872), bias}, [core.weight_ih_l0 (1024,257), core.weight_hh_l0 (1024,256), core.bias_ih_l0,
- * core.bias_hh_l0], policy.{weight (A,257|256), bias}, baseline.{weight, bias}.                       */
-int64_t tb_resnet_param_count(int num_actions, int use_lstm);
-size_t tb_resnet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision);
-/* polybeast_learner.py:214-266 Net.forward without the action sampling: frame u8 [T1,B,4,84,84], reward f32
- * [T1,B], notdone f32 [T1,B] and h0,c0/hN,cN f32 [1,B,256] (LSTM only) -> policy_logits [T1,B,A], baseline [T1,B].
+/* ---- IMPALA ResNet (polybeast_learner.py:134-266 `Net`) forward / backward -------------------------
+ * Observations u8 [C, H, W] and section widths (ch0, ch1, ch2); the reference's net is (4, 84, 84) with (16, 32, 32).
+ * Section i (width ch_i) runs its feat conv at H_i x W_i (H_0 = H, W_0 = W); its max-pool (3, 2, 1) leaves
+ * ceil(H_i / 2) x ceil(W_i / 2) = H_{i+1} x W_{i+1}.  Flat parameter layout = the reference's state_dict order:
+ *   feat_convs.0.0.weight (ch0, C, 3, 3), feat_convs.{1,2}.0.weight (ch_i, ch_{i-1}, 3, 3), feat_convs.i.0.bias (ch_i),
+ *   resnet1.i.{1,3}.{weight (ch_i, ch_i, 3, 3), bias (ch_i)}, resnet2.i.{1,3}.{weight, bias},
+ *   fc.{weight (256, ch2 * H_3 * W_3), bias (256)}, [core.weight_ih_l0 (1024,257), core.weight_hh_l0 (1024,256),
+ *   core.bias_ih_l0, core.bias_hh_l0], policy.{weight (A,257|256), bias}, baseline.{weight (num_values,257|256),
+ *   bias (num_values)}.
+ * At (4, 84, 84) x (16, 32, 32): (16,4,3,3) (32,16,3,3) (32,32,3,3) and fc.weight (256,3872).  num_values (1..64) is
+ * the number of value outputs, one per PopArt task.  Gradients use the same layout.
+ * Supported on every precision: 1 <= C <= 16, 17 <= H <= 126 and 33 <= W <= 126 (17 rows are the fewest that leave the
+ * last section 3 high, the smallest image of the split-bf16 conv kernels; 33 columns the fewest that leave it 5 wide,
+ * the narrowest row their weight gradient takes; 126 their widest padded row, 128 pixels), each width 16, 32 or 64 in
+ * any combination (e.g. (32, 64, 64) is the "IMPALA x2" net).  tb_resnet_obs_range writes the shape bounds as
+ * {C min, C max, H min, H max, W min, W max}, tb_resnet_widths writes {16, 32, 64}.  tb_resnet_supported returns 1 for
+ * a supported (shape, widths, precision) and otherwise 0 with tb_last_error set; the other entries fail the same way
+ * (param count -1, workspace 0, forward / backward non-zero).
+ *
+ * tb_resnet_forward: polybeast_learner.py:214-266 Net.forward without the action sampling: reward f32 [T1,B], notdone
+ * f32 [T1,B] and h0,c0/hN,cN f32 [1,B,256] (LSTM only) -> policy_logits [T1,B,A], baseline [T1,B,num_values].
+ *   done == NULL: frame is the stacked u8 [T1,B,C,H,W]; stacked_scratch is not read.
+ *   done != NULL: frame is an unstacked rollout u8 [T1+3,B,84,84] with done [T1,B] (see "unstacked rollouts" below);
+ *     only (4, 84, 84) with widths (16, 32, 32).  stacked_scratch is device memory of
+ *     tb_unstacked_scratch_bytes(1, T1, B, precision) bytes (NULL allowed, and not touched, when that is 0); at
+ *     precision 0 / 1 the forward restacks the frames into it.  Outputs, workspace contents and gradients are
+ *     bit-identical to the stacked forward on the restacked frames.
  * precision: 0 = fp32 SIMT patch-matrix GEMMs; 1 = bf16 activations + patch-matrix wgmma GEMMs (not parity-grade);
  * 2 = split-bf16 (the Python default): fp32 activations, every 3x3 conv as a shifted-window implicit GEMM over padded
  * channel-chunk-planar hi/lo images (csrc/conv3x3_sw.cu), the H=256 LSTM on one thread-block cluster.  T1*B < 65536.
- * The same precision and workspace must be used for forward and backward.                                            */
-int tb_resnet_forward(const uint8_t* frame, const float* reward, const float* notdone, const float* h0,
-                      const float* c0, const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm,
-                      int precision, void* workspace, float* policy_logits, float* baseline, float* hN, float* cN,
-                      void* stream);
-/* Backward of the forward pass that last ran on `workspace` (it keeps the conv input images / activations it needs). */
+ * The same precision, shape, widths and workspace must be used for forward and backward.
+ *
+ * tb_resnet_backward: the backward of the forward pass that last ran on `workspace` (it keeps the conv input images /
+ * activations it needs).  grad_logits [T1,B,A], grad_baseline [T1,B,num_values] -> grads (flat, overwritten).  frame
+ * is what that forward's first conv read: the stacked frame after a stacked forward, stacked_scratch (still holding
+ * the restacked frames) after an unstacked one.  At precision 2 it is not read (the first conv's input image is in the
+ * workspace) and may be NULL.                                                                                         */
+int tb_resnet_obs_range(int* range);
+int tb_resnet_widths(int* widths);
+int tb_resnet_supported(int C, int H, int W, int ch0, int ch1, int ch2, int precision);
+int64_t tb_resnet_param_count(int C, int H, int W, int ch0, int ch1, int ch2, int num_actions, int num_values,
+                              int use_lstm);
+size_t tb_resnet_workspace_bytes(int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1, int64_t B,
+                                 int num_actions, int use_lstm, int precision);
+int tb_resnet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                      const float* h0, const float* c0, const float* params, int C, int H, int W, int ch0, int ch1,
+                      int ch2, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                      void* workspace, void* stacked_scratch, float* policy_logits, float* baseline, float* hN,
+                      float* cN, void* stream);
 int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline,
-                       const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
-                       int use_lstm, int precision, void* workspace, float* grads, void* stream);
+                       const float* notdone, const float* params, int C, int H, int W, int ch0, int ch1, int ch2,
+                       int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                       void* workspace, float* grads, void* stream);
 
 /* ---- unstacked rollouts: four-frame stacks rebuilt on the GPU ------------------------------------------------------
  * Each frame sits in four consecutive stacks, so a stacked `frame` leaf u8 [T1,B,4,84,84] is three quarters copies.  An
@@ -520,35 +470,14 @@ int tb_restack_frames_u8(const uint8_t* frames, const uint8_t* done, int64_t T1,
  * FrameStack.reset does.  A column whose id is < 0 or >= S gets zero rows 0..2, and no history is read or written for
  * it (graph padding uses -1).  The ids of one call must be distinct: this is not checked, and two columns naming one
  * stream race.  Calls that share a history must be ordered on one stream.  HW % 16 == 0; frames and history 16-byte
- * aligned.  One launch; the output feeds tb_atarinet_forward_unstacked / tb_resnet_forward_unstacked with T1 = T.    */
+ * aligned.  One launch; the output feeds tb_atarinet_forward / tb_resnet_forward (done != NULL) with T1 = T.          */
 int tb_frame_history_fill_u8(uint8_t* frames, const uint8_t* done, const int64_t* stream_ids, int64_t T, int64_t B,
                              int64_t HW, uint8_t* history, int64_t S, void* stream);
-/* Bytes of stacked_scratch the *_forward_unstacked entries need for net (0 = AtariNet, 1 = ResNet) at this precision:
+/* Bytes of stacked_scratch the forwards need with done != NULL, for net (0 = AtariNet, 1 = ResNet) at this precision:
  * 0 where the restack is fused into the backend's frame-image pass (AtariNet bf16 / bf16x3, ResNet bf16x3),
  * T1*B*4*84*84 where the backend reads stacked frames (AtariNet fp32, ResNet fp32 / bf16).  SIZE_MAX for an unknown net,
  * precision or a size < 1.                                                                                           */
 size_t tb_unstacked_scratch_bytes(int net, int64_t T1, int64_t B, int precision);
-/* tb_atarinet_forward / tb_resnet_forward on an unstacked rollout: the same arguments, with the stacked frame replaced
- * by frames u8 [T1+3,B,84,84] + done [T1,B], and stacked_scratch (device memory of tb_unstacked_scratch_bytes bytes;
- * NULL allowed, and not touched, when that is 0).  Logits, baseline, final state and the workspace contents are
- * bit-identical to the stacked entry on the restacked frames.  tb_atarinet_backward / _phase follow this forward
- * unchanged: they read only the workspace.                                                                          */
-int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                  const int64_t* last_action, const float* h0, const float* c0, const float* params,
-                                  int64_t T1, int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
-                                  void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
-                                  void* stream);
-int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
-                                int num_actions, int use_lstm, int precision, void* workspace, void* stacked_scratch,
-                                float* policy_logits, float* baseline, float* hN, float* cN, void* stream);
-/* Backward of tb_resnet_forward_unstacked (gradients bit-identical to tb_resnet_backward after the stacked forward).
- * It reads: the workspace, always; stacked_scratch only at precision 0 / 1, where it must still hold the frames that
- * forward restacked into it (precision 2 reads the first conv's input image from the workspace, and stacked_scratch may
- * be NULL).  No frames or done are read.                                                                            */
-int tb_resnet_backward_unstacked(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
-                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
-                                 int use_lstm, int precision, void* workspace, float* grads, void* stream);
 
 /* ---- learner-queue ingest, host side (SURVEY 8(f) N1) --------------------------------------------------
  * One actor writes its [T1, ...] rollout into batch column b of a pinned [T1, B, ...] slot (replaces the per-rollout

@@ -725,12 +725,12 @@ def test_heads_sizes():
 # the AtariNet backward at the batch sizes the heads used to refuse
 # ---------------------------------------------------------------------------------------------------------------------
 def atarinet_bias_grads(T1, B, A, V, precision):
-    """tb_atarinet_backward_mt on integer-valued cotangents: the policy / baseline bias gradients must be their float64
+    """tb_atarinet_backward on integer-valued cotangents: the policy / baseline bias gradients must be their float64
     column sums exactly.  They do not depend on the activations, so no forward is needed (the workspace is zeroed)."""
     h = lib()
     N = T1 * B
     core = 512 + 1 + A
-    nparam = h.tb_atarinet_param_count_mt(A, V, 0)
+    nparam = h.tb_atarinet_param_count(A, V, 0)
     wsb = h.tb_atarinet_workspace_bytes(T1, B, A, 0, precision)
     need = wsb + 4 * (2 * nparam + N * (A + V)) + (256 << 20)
     free = torch.cuda.mem_get_info()[0]
@@ -742,7 +742,7 @@ def atarinet_bias_grads(T1, B, A, V, precision):
     dl = ints((T1, B, A), -4, 4, g)
     db = ints((T1, B, V), -4, 4, g)
     grads = torch.full((nparam,), NAN, device="cuda")
-    call("tb_atarinet_backward_mt", P(dl), P(db), None, P(params), T1, B, A, V, 0, precision, P(ws), P(grads), stream())
+    call("tb_atarinet_backward", P(dl), P(db), None, P(params), T1, B, A, V, 0, precision, P(ws), P(grads), 3, stream())
     torch.cuda.synchronize()
     bb = grads[nparam - V:]
     bp = grads[nparam - V - V * core - A:nparam - V - V * core]
@@ -753,12 +753,12 @@ def atarinet_bias_grads(T1, B, A, V, precision):
     assert (grads[nparam - V - V * core:nparam - V] == 0).all()
 
 
-def test_atarinet_backward_multitask_many_columns():
+def test_atarinet_backward_heads_scratch_at_13770_rows():
     """A = 18, V = 57 at T1 * B = 13770: the heads' weight-gradient partials used to outgrow the split-K scratch
     ("heads scratch too small" from N > 13440)"""
     atarinet_bias_grads(81, 170, 18, 57, 2)
 
 
-def test_atarinet_backward_past_65535_rows():
+def test_atarinet_backward_heads_past_65535_rows():
     """T1 * B = 65610 >= 65536: the heads' input-gradient kernel put the rows on grid.y and failed to launch"""
     atarinet_bias_grads(81, 810, 6, 1, 2)

@@ -149,11 +149,11 @@ def test_nets_popart_state(net):
             make(num_tasks=bad)
 
 
-def test_popart_abi_and_host_side_checks():
+def test_popart_num_values_abi_and_host_side_checks():
     from tests.test_abi_cpu import header_symbols
     from torchbeast_b200 import _lib
-    for s in ("tb_impala_loss_f32", "tb_popart_update", "tb_atarinet_forward_mt", "tb_atarinet_backward_phase_mt",
-              "tb_resnet_backward_unstacked_mt"):
+    for s in ("tb_impala_loss_f32", "tb_popart_update", "tb_atarinet_param_count", "tb_atarinet_forward",
+              "tb_atarinet_backward", "tb_resnet_param_count", "tb_resnet_forward", "tb_resnet_backward"):
         assert s in header_symbols() and s in _lib.declared_symbols()
     h = _lib.lib()
     assert h.tb_popart_update(None, None, None, None, 65, None, None, 8, None) != 0
@@ -172,8 +172,11 @@ def test_popart_abi_and_host_side_checks():
         assert b"null PopArt pointer" in popart_error(**{k: None})
     assert b"bad sizes" in popart_error(T=0)
     assert b"zero_tail" in popart_error(zero_tail=0)
-    # the _mt layouts: num_values = 1 is the plain layout, each further value adds one head row
-    for count in (h.tb_atarinet_param_count_mt, h.tb_resnet_param_count_mt):
-        old = h.tb_atarinet_param_count if count == h.tb_atarinet_param_count_mt else h.tb_resnet_param_count
-        assert count(6, 1, 1) == old(6, 1)
-    assert h.tb_atarinet_param_count_mt(6, 57, 1) - h.tb_atarinet_param_count(6, 1) == 56 * (512 + 6 + 1 + 1)
+    # num_values = 1 is the plain layout (the parameter counts of the reference's nets), each further value adds one
+    # head row
+    assert h.tb_atarinet_param_count(6, 1, 1) == sum(int(np.prod(s)) for s in LT.atarinet_param_shapes(6, True).values())
+    assert h.tb_resnet_param_count(4, 84, 84, 16, 32, 32, 6, 1, 1) == sum(int(np.prod(s)) for s in
+                                                                        LT.resnet_param_shapes(6, True).values())
+    assert h.tb_atarinet_param_count(6, 57, 1) - h.tb_atarinet_param_count(6, 1, 1) == 56 * (512 + 6 + 1 + 1)
+    assert h.tb_resnet_param_count(4, 84, 84, 16, 32, 32, 6, 57, 1) - h.tb_resnet_param_count(4, 84, 84, 16, 32, 32, 6, 1, 1) \
+        == 56 * (256 + 1)

@@ -7,6 +7,7 @@ import torch
 from torchbeast_b200 import _lib
 from torchbeast_b200.nets import ResNet, resnet_fc_in, resnet_obs_range, resnet_param_spec
 
+DEFAULT_WIDTHS = (16, 32, 32)
 SHAPES = [(4, 84, 84), (3, 64, 64), (3, 72, 96), (12, 64, 64), (1, 84, 84), (3, 37, 53), (16, 17, 126), (5, 126, 33),
           (2, 17, 33)]
 
@@ -27,20 +28,20 @@ def _pooled(s):
 @pytest.mark.parametrize("obs", SHAPES)
 @pytest.mark.parametrize("use_lstm", [False, True])
 @pytest.mark.parametrize("num_values", [1, 4])
-def test_spec_agrees_with_abi(obs, use_lstm, num_values):
+def test_spec_agrees_with_resnet_param_count(obs, use_lstm, num_values):
     spec = dict(resnet_param_spec(7, use_lstm, num_values=num_values, observation_shape=obs))
     C, H, W = obs
     assert spec["feat_convs.0.0.weight"] == (16, C, 3, 3)
     assert spec["fc.weight"] == (256, 32 * _pooled(H) * _pooled(W)) and resnet_fc_in(obs) == 32 * _pooled(H) * _pooled(W)
     total = sum(_numel(s) for s in spec.values())
-    assert _lib.lib().tb_resnet_param_count_obs(C, H, W, 7, num_values, int(use_lstm)) == total
+    assert _lib.lib().tb_resnet_param_count(C, H, W, *DEFAULT_WIDTHS, 7, num_values, int(use_lstm)) == total
     for precision in range(3):
-        assert _lib.lib().tb_resnet_obs_supported(C, H, W, precision) == 1
-        assert _lib.lib().tb_resnet_workspace_bytes_obs(C, H, W, 5, 3, 7, int(use_lstm), precision) > 0
+        assert _lib.lib().tb_resnet_supported(C, H, W, *DEFAULT_WIDTHS, precision) == 1
+        assert _lib.lib().tb_resnet_workspace_bytes(C, H, W, *DEFAULT_WIDTHS, 5, 3, 7, int(use_lstm), precision) > 0
 
 
-# tb_resnet_param_count_mt(A, V, use_lstm) and tb_resnet_workspace_bytes(T1, B, 6, use_lstm, precision 0 / 1 / 2) as the
-# library reported them before it took an observation shape (the (4, 84, 84) constants): the default layout and
+# the (4, 84, 84) parameter count (A, use_lstm, V) and workspace bytes (T1, B, use_lstm; precision 0 / 1 / 2, A = 6) as
+# the library reported them before it took an observation shape (the (4, 84, 84) constants): the default layout and
 # workspace must not move
 PARAM_COUNTS = {(6, 0, 1): 1091038, (6, 0, 4): 1091812, (6, 1, 1): 1618391, (6, 1, 4): 1619162,
                 (18, 0, 1): 1094134, (18, 0, 4): 1094908, (18, 1, 1): 1621475, (18, 1, 4): 1622246}
@@ -53,16 +54,14 @@ WORKSPACE_BYTES = {
 }
 
 
-def test_default_layout_and_workspace_unchanged():
+def test_default_geometry_layout_and_workspace_unchanged():
     lib = _lib.lib()
     for (A, lstm, V), count in PARAM_COUNTS.items():
-        assert lib.tb_resnet_param_count_mt(A, V, lstm) == count
-        assert lib.tb_resnet_param_count_obs(4, 84, 84, A, V, lstm) == count
+        assert lib.tb_resnet_param_count(4, 84, 84, *DEFAULT_WIDTHS, A, V, lstm) == count
         assert sum(_numel(s) for _, s in resnet_param_spec(A, bool(lstm), num_values=V)) == count
     for (T1, B, lstm), sizes in WORKSPACE_BYTES.items():
         for precision, nbytes in enumerate(sizes):
-            assert lib.tb_resnet_workspace_bytes(T1, B, 6, lstm, precision) == nbytes
-            assert lib.tb_resnet_workspace_bytes_obs(4, 84, 84, T1, B, 6, lstm, precision) == nbytes
+            assert lib.tb_resnet_workspace_bytes(4, 84, 84, *DEFAULT_WIDTHS, T1, B, 6, lstm, precision) == nbytes
     d = dict(resnet_param_spec(6, True))
     assert d["feat_convs.0.0.weight"] == (16, 4, 3, 3) and d["fc.weight"] == (256, 3872)
 
@@ -76,8 +75,8 @@ def test_model_layout_at_new_shape():
     assert ResNet(5, device=torch.device("cpu")).observation_shape == (4, 84, 84)
 
 
-def test_range_is_the_libraries_and_exactly_what_is_supported():
-    """The documented range, read from the C library, is the set tb_resnet_obs_supported accepts on every backend, and
+def test_range_is_the_libraries_and_exactly_what_resnet_supported_accepts():
+    """The documented range, read from the C library, is the set tb_resnet_supported accepts on every backend, and
     its lower bounds are the smallest sides whose last section is 3 high and 5 wide (the smallest image of the
     shifted-window kernels; the narrowest row their weight gradient takes)."""
     rng = resnet_obs_range()
@@ -89,9 +88,9 @@ def test_range_is_the_libraries_and_exactly_what_is_supported():
         for H in range(1, 131):
             for W in range(1, 131):
                 want = rng["H"][0] <= H <= rng["H"][1] and rng["W"][0] <= W <= rng["W"][1]
-                assert lib.tb_resnet_obs_supported(3, H, W, precision) == int(want), (H, W, precision)
+                assert lib.tb_resnet_supported(3, H, W, *DEFAULT_WIDTHS, precision) == int(want), (H, W, precision)
         for C in range(0, 18):
-            assert lib.tb_resnet_obs_supported(C, 64, 64, precision) == int(rng["C"][0] <= C <= rng["C"][1])
+            assert lib.tb_resnet_supported(C, 64, 64, *DEFAULT_WIDTHS, precision) == int(rng["C"][0] <= C <= rng["C"][1])
 
 
 # (3, 32, 17) .. (3, 32, 32): last section 3 or 4 wide, narrower than the weight-gradient kernel's last pixel step allows
@@ -100,7 +99,7 @@ BAD = [(0, 84, 84), (17, 84, 84), (3, 16, 64), (3, 64, 16), (3, 32, 17), (3, 64,
 
 
 @pytest.mark.parametrize("obs", BAD)
-def test_out_of_range_raises_at_construction(obs):
+def test_out_of_range_shape_raises_and_every_entry_refuses_it(obs):
     rng = resnet_obs_range()
     with pytest.raises(_lib.TorchBeastB200Error, match=r"observation_shape must be \(C, H, W\) with C in \[%d, %d\], H in "
                                                       r"\[%d, %d\] and W in \[%d, %d\]" % (rng["C"] + rng["H"] + rng["W"])):
@@ -108,10 +107,10 @@ def test_out_of_range_raises_at_construction(obs):
     if len(obs) == 3:
         lib = _lib.lib()
         for precision in range(3):
-            assert lib.tb_resnet_obs_supported(*obs, precision) == 0
-            assert lib.tb_last_error().decode().startswith("resnet_obs_supported: observation")
-        assert lib.tb_resnet_param_count_obs(*obs, 6, 1, 0) == -1
-        assert lib.tb_resnet_workspace_bytes_obs(*obs, 2, 2, 6, 0, 2) == 0
+            assert lib.tb_resnet_supported(*obs, *DEFAULT_WIDTHS, precision) == 0
+            assert lib.tb_last_error().decode().startswith("resnet_supported: observation")
+        assert lib.tb_resnet_param_count(*obs, *DEFAULT_WIDTHS, 6, 1, 0) == -1
+        assert lib.tb_resnet_workspace_bytes(*obs, *DEFAULT_WIDTHS, 2, 2, 6, 0, 2) == 0
 
 
 def test_range_edges_are_supported():

@@ -3,7 +3,6 @@ single-channel Atari (1, 84, 84), an odd non-square (3, 37, 53) and the edges of
 oracle/learner_torch.resnet_forward (which reads its sizes from the frame and the parameters), plus the learner, the
 graphed paths, PopArt, the acting paths, and the (4, 84, 84) path against the bits it had before the library took an
 observation shape."""
-import ctypes
 import functools
 import gc
 import types
@@ -125,75 +124,25 @@ def test_forward_backward_vs_float64_oracle(obs, use_lstm, precision):
     assert not bad, (bad, report)
 
 
-def _abi_run(lib, frame, params, T1, B, use_lstm, precision, ws, obs=None):
-    """One forward + backward through the _mt entries (obs None) or the _obs entries at obs."""
-    p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    rs = np.random.RandomState(3)
-    reward = torch.from_numpy(rs.randn(T1, B).astype(np.float32)).cuda()
-    notdone = torch.ones(T1, B, device="cuda") if use_lstm else None
-    h0 = torch.from_numpy(rs.randn(1, B, 256).astype(np.float32) * 0.1).cuda() if use_lstm else None
-    c0 = h0.clone() if use_lstm else None
-    hN = torch.empty(1, B, 256, device="cuda") if use_lstm else None
-    cN = torch.empty(1, B, 256, device="cuda") if use_lstm else None
-    logits = torch.empty(T1, B, A, device="cuda")
-    baseline = torch.empty(T1, B, device="cuda")
-    gl = torch.from_numpy(rs.randn(T1, B, A).astype(np.float32)).cuda()
-    gb = torch.from_numpy(rs.randn(T1, B).astype(np.float32)).cuda()
-    grads = torch.empty_like(params)
-    torch.cuda.synchronize()
-    before = lib.tb_launch_count()
-    if obs is None:
-        rc = lib.tb_resnet_forward_mt(p(frame), p(reward), p(notdone), p(h0), p(c0), p(params), T1, B, A, 1, int(use_lstm),
-                                      precision, p(ws), p(logits), p(baseline), p(hN), p(cN), st)
-        assert rc == 0, lib.tb_last_error()
-        rc = lib.tb_resnet_backward_mt(p(frame), p(gl), p(gb), p(notdone), p(params), T1, B, A, 1, int(use_lstm), precision,
-                                       p(ws), p(grads), st)
-    else:
-        rc = lib.tb_resnet_forward_obs(p(frame), p(reward), p(notdone), p(h0), p(c0), p(params), *obs, T1, B, A, 1,
-                                       int(use_lstm), precision, p(ws), p(logits), p(baseline), p(hN), p(cN), st)
-        assert rc == 0, lib.tb_last_error()
-        rc = lib.tb_resnet_backward_obs(p(frame), p(gl), p(gb), p(notdone), p(params), *obs, T1, B, A, 1, int(use_lstm),
-                                        precision, p(ws), p(grads), st)
-    assert rc == 0, lib.tb_last_error()
-    torch.cuda.synchronize()
-    return logits, baseline, hN, grads, lib.tb_launch_count() - before
-
-
-@pytest.mark.parametrize("precision", [0, 1, 2])
-@pytest.mark.parametrize("use_lstm", [False, True])
-def test_obs_entries_at_atari_shape_are_the_existing_entries(precision, use_lstm):
-    from torchbeast_b200 import _lib
-    lib = _lib.lib()
-    T1, B = 5, 3
-    params = torch.cat([v.flatten() for v in LT.random_params(obs_param_shapes((4, 84, 84), A, use_lstm), seed=2).values()]).cuda()
-    assert params.numel() == lib.tb_resnet_param_count(A, int(use_lstm))
-    frame = torch.from_numpy(np.random.RandomState(4).randint(0, 256, size=(T1, B, 4, 84, 84)).astype(np.uint8)).cuda()
-    nbytes = lib.tb_resnet_workspace_bytes(T1, B, A, int(use_lstm), precision)
-    assert nbytes == lib.tb_resnet_workspace_bytes_obs(4, 84, 84, T1, B, A, int(use_lstm), precision)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
-    a = _abi_run(lib, frame, params, T1, B, use_lstm, precision, ws)
-    b = _abi_run(lib, frame, params, T1, B, use_lstm, precision, ws, obs=(4, 84, 84))
-    for x, y in zip(a[:4], b[:4]):
-        assert (x is None and y is None) or torch.equal(x, y)
-    assert a[4] == b[4] > 0
-
-
 def test_default_path_reproduces_the_fixed_geometry_bits():
-    """The (4, 84, 84) path through the tb_resnet_*_mt entries (which run the tb_resnet_*_obs code) gives the bits the
-    library gave before it took an observation shape (tests/golden/resnet_obs_default_bits.npz, written by
-    tools/make_resnet_default_golden.py with that build): logits, baseline, hN and sampled gradients on every backend."""
+    """The (4, 84, 84) path with the default widths gives the bits the library gave before it took an observation shape
+    (tests/golden/resnet_obs_default_bits.npz, written by tools/make_resnet_default_golden.py with that build): logits,
+    baseline, hN and sampled gradients on every backend, from library launches."""
     import importlib.util
     import os
     from tests.common import golden
+    from torchbeast_b200 import _lib
     path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools", "make_resnet_default_golden.py")
     spec = importlib.util.spec_from_file_location("make_resnet_default_golden", path)
     tool = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(tool)
     g = golden("resnet_obs_default_bits.npz")
+    lib = _lib.lib()
     for use_lstm in (False, True):
         for precision in (0, 1, 2):
+            before = lib.tb_launch_count()
             got = tool.default_case(use_lstm, precision)
+            assert lib.tb_launch_count() > before, (use_lstm, precision)
             for k, v in got.items():
                 assert np.array_equal(v, g["%s/lstm%d/p%d" % (k, use_lstm, precision)]), (k, use_lstm, precision)
 

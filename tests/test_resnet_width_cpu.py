@@ -1,6 +1,5 @@
-"""IMPALA ResNet section widths without a GPU: the Python parameter spec against the C ABI, the fc width, the _arch
-entries at the default widths against the _obs entries, the supported set the library reports, construction errors,
-and the oracle's default shapes."""
+"""IMPALA ResNet section widths without a GPU: the Python parameter spec against the C ABI, the fc width, the supported
+set the library reports, construction errors, and the oracle's default shapes."""
 import itertools
 import math
 
@@ -24,7 +23,7 @@ def test_library_states_the_widths():
 
 @pytest.mark.parametrize("obs", SHAPES)
 @pytest.mark.parametrize("channels", [(16, 32, 32), (32, 64, 64), (64, 64, 64), (16, 64, 32), (64, 16, 32)])
-def test_spec_matches_the_abi_parameter_count(obs, channels):
+def test_spec_matches_resnet_param_count_at_every_width(obs, channels):
     for use_lstm, num_values in ((False, 1), (True, 1), (True, 4)):
         spec = nets.resnet_param_spec(A, use_lstm, num_values, observation_shape=obs, channels=channels)
         d = dict(spec)
@@ -35,7 +34,7 @@ def test_spec_matches_the_abi_parameter_count(obs, channels):
             assert d["resnet1.%d.1.weight" % i] == d["resnet2.%d.3.weight" % i] == (channels[i], channels[i], 3, 3)
         assert d["fc.weight"] == (256, nets.resnet_fc_in(obs, channels))
         total = sum(math.prod(s) for _, s in spec)
-        assert lib().tb_resnet_param_count_arch(*obs, *channels, A, num_values, int(use_lstm)) == total
+        assert lib().tb_resnet_param_count(*obs, *channels, A, num_values, int(use_lstm)) == total
 
 
 def test_fc_in():
@@ -46,39 +45,27 @@ def test_fc_in():
     assert nets.resnet_fc_in((2, 17, 33), (64, 64, 64)) == 64 * 3 * 5
 
 
-@pytest.mark.parametrize("obs", SHAPES)
-def test_arch_entries_at_default_widths_are_the_obs_entries(obs):
-    L = lib()
-    for use_lstm in (0, 1):
-        assert L.tb_resnet_param_count_arch(*obs, 16, 32, 32, A, 1, use_lstm) == L.tb_resnet_param_count_obs(*obs, A, 1, use_lstm)
-        for precision in (0, 1, 2):
-            assert L.tb_resnet_arch_supported(*obs, 16, 32, 32, precision) == L.tb_resnet_obs_supported(*obs, precision) == 1
-            for T1, B in ((1, 1), (81, 8), (81, 32)):
-                a = L.tb_resnet_workspace_bytes_arch(*obs, 16, 32, 32, T1, B, A, use_lstm, precision)
-                assert a > 0 and a == L.tb_resnet_workspace_bytes_obs(*obs, T1, B, A, use_lstm, precision)
-
-
 @pytest.mark.parametrize("obs", SHAPES + [(1, 17, 126), (5, 126, 33)])
-def test_every_width_tuple_is_supported_on_every_backend(obs):
+def test_every_width_tuple_is_supported_at_every_shape_and_backend(obs):
     """The library's supported set: each section 16, 32 or 64, in all 27 combinations, at every shape of the range."""
     L = lib()
     for ch in ALL:
         for precision in (0, 1, 2):
-            assert L.tb_resnet_arch_supported(*obs, *ch, precision) == 1, (ch, precision, L.tb_last_error())
-            assert L.tb_resnet_workspace_bytes_arch(*obs, *ch, 5, 3, A, 1, precision) > 0
+            assert L.tb_resnet_supported(*obs, *ch, precision) == 1, (ch, precision, L.tb_last_error())
+            assert L.tb_resnet_workspace_bytes(*obs, *ch, 5, 3, A, 1, precision) > 0
 
 
 @pytest.mark.parametrize("bad", [8, 48, 128, 0, -16, 24])
-def test_other_widths_are_refused(bad):
+def test_other_widths_are_refused_by_every_entry(bad):
     L = lib()
     for pos in range(3):
         ch = [16, 32, 32]
         ch[pos] = bad
         for precision in (0, 1, 2):
-            assert L.tb_resnet_arch_supported(4, 84, 84, *ch, precision) == 0
-            assert L.tb_last_error().decode().startswith("resnet_arch_supported: section %d has %d channels" % (pos, bad))
-        assert L.tb_resnet_param_count_arch(4, 84, 84, *ch, A, 1, 1) == -1
-        assert L.tb_resnet_workspace_bytes_arch(4, 84, 84, *ch, 5, 3, A, 1, 2) == 0
+            assert L.tb_resnet_supported(4, 84, 84, *ch, precision) == 0
+            assert L.tb_last_error().decode().startswith("resnet_supported: section %d has %d channels" % (pos, bad))
+        assert L.tb_resnet_param_count(4, 84, 84, *ch, A, 1, 1) == -1
+        assert L.tb_resnet_workspace_bytes(4, 84, 84, *ch, 5, 3, A, 1, 2) == 0
 
 
 def test_construction_errors_quote_the_supported_set():

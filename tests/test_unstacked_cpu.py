@@ -137,11 +137,11 @@ def test_acting_paths_reject_unstacked_frames():
         polybeast_learner.inference(types.SimpleNamespace(actor_device="cpu"), [Batch()], model)
 
 
-def test_unstacked_abi_host_side():
+def test_unstacked_frames_host_side_checks():
     from torchbeast_b200 import _lib
     h = _lib.lib()
-    for name in ("tb_restack_frames_u8", "tb_unstacked_scratch_bytes", "tb_atarinet_forward_unstacked",
-                 "tb_resnet_forward_unstacked", "tb_resnet_backward_unstacked"):
+    for name in ("tb_restack_frames_u8", "tb_unstacked_scratch_bytes", "tb_atarinet_forward", "tb_resnet_forward",
+                 "tb_resnet_backward"):
         assert name in _lib.declared_symbols() and hasattr(ctypes.CDLL(_lib.LIB_PATH), name)
     stacked = 81 * 32 * 4 * 7056
     # the restack is fused into AtariNet bf16 / bf16x3 and ResNet bf16x3; the other backends get a stacked scratch
@@ -151,12 +151,32 @@ def test_unstacked_abi_host_side():
     assert h.tb_unstacked_scratch_bytes(0, 81, 32, 3) == ctypes.c_size_t(-1).value
     assert h.tb_restack_frames_u8(None, None, 4, 2, 7056, None, None) != 0 and b"null pointer" in h.tb_last_error()
     assert h.tb_restack_frames_u8(None, None, 4, 2, 7055, None, None) != 0 and b"bad sizes" in h.tb_last_error()
-    args = [None] * 8 + [4, 2, 6, 0, 0] + [None] * 7
-    assert h.tb_atarinet_forward_unstacked(*args) != 0 and b"null pointer" in h.tb_last_error()
-    args = [None] * 7 + [4, 2, 6, 0, 0] + [None] * 7
-    assert h.tb_resnet_forward_unstacked(*args) != 0 and b"null pointer" in h.tb_last_error()
-    args = [None] * 5 + [4, 2, 6, 0, 0, None, None, None]
-    assert h.tb_resnet_backward_unstacked(*args) != 0 and b"null pointer" in h.tb_last_error()
+    P = ctypes.c_void_p(256)  # never dereferenced: every call below fails its host-side checks before a launch
+    args = [None, P] + [None] * 6 + [4, 2, 6, 1, 0, 0] + [None] * 7
+    assert h.tb_atarinet_forward(*args) != 0 and b"null pointer" in h.tb_last_error()
+    default = [4, 84, 84, 16, 32, 32]
+    args = [None, P] + [None] * 5 + default + [4, 2, 6, 1, 0, 0] + [None] * 7
+    assert h.tb_resnet_forward(*args) != 0 and b"null pointer" in h.tb_last_error()
+    args = [None] * 5 + default + [4, 2, 6, 1, 0, 0] + [None] * 3
+    assert h.tb_resnet_backward(*args) != 0 and b"null pointer" in h.tb_last_error()
+    # unstacked frames (done != NULL) rebuild (4, 84, 84) stacks for the default widths only
+    for geometry in ([3, 64, 64, 16, 32, 32], [4, 84, 84, 32, 64, 64], [4, 84, 84, 16, 32, 64]):
+        for precision in (0, 1, 2):
+            args = [P] * 7 + geometry + [4, 2, 6, 1, 0, precision] + [P] * 7
+            assert h.tb_resnet_forward(*args) != 0
+            assert h.tb_last_error().decode().startswith("resnet_forward: unstacked frames (done != NULL) need the "
+                                                         "(4, 84, 84) observation and the default widths (16, 32, 32)")
+    # the backward re-reads the frame the first conv read, except at precision 2: a NULL frame then gets as far as the
+    # geometry check (an unsupported shape stops it there)
+    for precision in (0, 1, 2):
+        args = [None] + [P] * 4 + [4, 16, 16, 16, 32, 32] + [4, 2, 6, 1, 0, precision] + [P] * 3
+        assert h.tb_resnet_backward(*args) != 0
+        want = b"resnet_backward: observation 16 x 16" if precision == 2 else b"resnet_backward: null pointer"
+        assert h.tb_last_error().startswith(want), (precision, h.tb_last_error())
+    # phase 3 is the whole backward, 1 and 2 its two halves; nothing else
+    for phase in (0, 4, -1):
+        args = [P] * 4 + [4, 2, 6, 1, 0, 0, P, P, phase, P]
+        assert h.tb_atarinet_backward(*args) != 0 and b"atarinet_backward: phase must be" in h.tb_last_error()
 
 
 def test_shard_rollout_keeps_the_unstacked_format():

@@ -1,5 +1,5 @@
-"""Write tests/golden/resnet_obs_default_bits.npz: the exact float32 results of the ResNet's (4, 84, 84) path through the
-tb_resnet_forward_mt / tb_resnet_backward_mt entry points on each backend, ±LSTM, at T1=3, B=2 (policy logits, baseline,
+"""Write tests/golden/resnet_obs_default_bits.npz: the exact float32 results of the ResNet's (4, 84, 84) path with the
+default widths through tb_resnet_forward / tb_resnet_backward on each backend, ±LSTM, at T1=3, B=2 (policy logits, baseline,
 hN and 4096 strided samples of the parameter gradients).  The committed file was written by the build that had no
 observation geometry (fixed 84 x 84 constants); tests/test_resnet_obs_gpu.py checks that the current build reproduces it
 bit for bit on an H100.
@@ -40,12 +40,15 @@ def default_case(use_lstm, precision):
     gl = torch.from_numpy(rs.randn(T1, B, A).astype(np.float32)).cuda()
     gb = torch.from_numpy(rs.randn(T1, B).astype(np.float32)).cuda()
     grads = torch.empty_like(params)
-    ws = torch.empty(lib.tb_resnet_workspace_bytes(T1, B, A, int(use_lstm), precision), dtype=torch.uint8, device="cuda")
+    geometry = (4, 84, 84, 16, 32, 32)
+    ws = torch.empty(lib.tb_resnet_workspace_bytes(*geometry, T1, B, A, int(use_lstm), precision), dtype=torch.uint8,
+                     device="cuda")
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _lib.check(lib.tb_resnet_forward_mt(p(frame), p(reward), p(notdone), p(h0), p(c0), p(params), T1, B, A, 1, int(use_lstm),
-                                        precision, p(ws), p(logits), p(baseline), p(hN), p(cN), st), "tb_resnet_forward_mt")
-    _lib.check(lib.tb_resnet_backward_mt(p(frame), p(gl), p(gb), p(notdone), p(params), T1, B, A, 1, int(use_lstm), precision,
-                                         p(ws), p(grads), st), "tb_resnet_backward_mt")
+    _lib.check(lib.tb_resnet_forward(p(frame), None, p(reward), p(notdone), p(h0), p(c0), p(params), *geometry, T1, B, A, 1,
+                                     int(use_lstm), precision, p(ws), None, p(logits), p(baseline), p(hN), p(cN), st),
+               "tb_resnet_forward")
+    _lib.check(lib.tb_resnet_backward(p(frame), p(gl), p(gb), p(notdone), p(params), *geometry, T1, B, A, 1, int(use_lstm),
+                                      precision, p(ws), p(grads), st), "tb_resnet_backward")
     idx = torch.linspace(0, params.numel() - 1, SAMPLES).long().cuda()
     return {"logits": logits.cpu().numpy(), "baseline": baseline.cpu().numpy(),
             "hN": hN.cpu().numpy() if use_lstm else np.zeros(0, np.float32), "grads": grads[idx].cpu().numpy()}

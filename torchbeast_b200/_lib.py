@@ -32,28 +32,18 @@ _SIGNATURES = {
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 5 + [_i64] + [_vp] * 12
         + [_int, _vp, _vp], _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
-    "tb_atarinet_param_count_mt": ([_int, _int, _int], _i64),
-    "tb_atarinet_forward_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_atarinet_forward_unstacked_mt": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
-    "tb_atarinet_backward_mt": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
-    "tb_atarinet_backward_phase_mt": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
-    "tb_resnet_param_count_mt": ([_int, _int, _int], _i64),
-    "tb_resnet_forward_mt": ([_vp] * 6 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_resnet_backward_mt": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
-    "tb_resnet_forward_unstacked_mt": ([_vp] * 7 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
-    "tb_resnet_backward_unstacked_mt": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_atarinet_param_count": ([_int, _int, _int], _i64),
+    "tb_atarinet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
+    "tb_atarinet_grad_split": ([_int, _int], _i64),
+    "tb_atarinet_forward": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
     "tb_resnet_obs_range": ([_vp], _int),
-    "tb_resnet_obs_supported": ([_int] * 4, _int),
-    "tb_resnet_param_count_obs": ([_int] * 6, _i64),
-    "tb_resnet_workspace_bytes_obs": ([_int] * 3 + [_i64, _i64, _int, _int, _int], _c.c_size_t),
-    "tb_resnet_forward_obs": ([_vp] * 6 + [_int] * 3 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_resnet_backward_obs": ([_vp] * 5 + [_int] * 3 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_resnet_widths": ([_vp], _int),
-    "tb_resnet_arch_supported": ([_int] * 7, _int),
-    "tb_resnet_param_count_arch": ([_int] * 9, _i64),
-    "tb_resnet_workspace_bytes_arch": ([_int] * 6 + [_i64, _i64, _int, _int, _int], _c.c_size_t),
-    "tb_resnet_forward_arch": ([_vp] * 6 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_resnet_backward_arch": ([_vp] * 5 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
+    "tb_resnet_supported": ([_int] * 7, _int),
+    "tb_resnet_param_count": ([_int] * 9, _i64),
+    "tb_resnet_workspace_bytes": ([_int] * 6 + [_i64, _i64, _int, _int, _int], _c.c_size_t),
+    "tb_resnet_forward": ([_vp] * 7 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_resnet_backward": ([_vp] * 5 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_replay_mix": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp], _int),
@@ -119,28 +109,16 @@ _SIGNATURES = {
     "tb_heads_forward": ([_vp, _i64, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_heads_backward": ([_vp, _i64, _vp, _vp, _vp, _vp, _i64, _int, _int, _int, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp],
                           _int),
-    "tb_atarinet_param_count": ([_int, _int], _i64),
-    "tb_atarinet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
-    "tb_atarinet_forward": ([_vp] * 7 + [_i64, _i64, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_resnet_param_count": ([_int, _int], _i64),
-    "tb_resnet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
-    "tb_resnet_forward": ([_vp] * 6 + [_i64, _i64, _int, _int, _int] + [_vp] * 6, _int),
-    "tb_resnet_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_grad_sumsq_f32": ([_vp, _i64, _vp, _vp, _vp], _int),
     "tb_clip_rmsprop_step_f32": ([_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _vp, _vp, _vp], _int),
     "tb_clip_adam_step_f32": (
         [_vp] * 4 + [_i64, _vp, _f32, _vp, _f32, _f64, _f64, _f32, _f32, _int, _vp, _vp, _vp, _vp], _int),
     "tb_clip_rmsprop_ex_step_f32": (
         [_vp] * 5 + [_i64, _vp, _f32, _vp, _f32, _f32, _f32, _f32, _f32, _vp, _vp, _vp], _int),
-    "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
-    "tb_atarinet_grad_split": ([_int, _int], _i64),
     "tb_set_aux_stream": ([_vp], _int),
     "tb_restack_frames_u8": ([_vp, _vp, _i64, _i64, _i64, _vp, _vp], _int),
     "tb_frame_history_fill_u8": ([_vp, _vp, _vp, _i64, _i64, _i64, _vp, _i64, _vp], _int),
     "tb_unstacked_scratch_bytes": ([_int, _i64, _i64, _int], _c.c_size_t),
-    "tb_atarinet_forward_unstacked": ([_vp] * 8 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),
-    "tb_resnet_forward_unstacked": ([_vp] * 7 + [_i64, _i64, _int, _int, _int] + [_vp] * 7, _int),
-    "tb_resnet_backward_unstacked": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_host_write_rollout_column": ([_vp, _vp, _vp, _int, _i64, _i64, _i64, _vp], _int),
     "tb_lstm_workspace_bytes": ([_i64, _i64, _int, _int, _int, _int], _c.c_size_t),
     "tb_lstm_plan": ([_i64, _int, _int, _int, _int, _vp, _vp], _int),
@@ -148,7 +126,6 @@ _SIGNATURES = {
     "tb_lstm_forward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 5, _int),
     "tb_lstm_backward": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 3, _int),
     "tb_lstm_backward_state": ([_vp] * 5 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
-    "tb_atarinet_backward_phase": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _vp, _vp, _int, _vp], _int),
 }
 
 _lib = None

@@ -401,11 +401,7 @@ using namespace tb;
 
 extern "C" {
 
-int64_t tb_atarinet_param_count(int num_actions, int use_lstm) {
-  return atari_params(num_actions, use_lstm).total;
-}
-
-int64_t tb_atarinet_param_count_mt(int num_actions, int num_values, int use_lstm) {
+int64_t tb_atarinet_param_count(int num_actions, int num_values, int use_lstm) {
   return atari_params(num_actions, use_lstm, num_values).total;
 }
 
@@ -414,42 +410,15 @@ int64_t tb_atarinet_grad_split(int num_actions, int use_lstm) {
   return use_lstm ? pp.lstm[0][0] : pp.policy_w;  // first parameter after fc.bias
 }
 
-int tb_atarinet_backward_phase(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                               const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
-                               void* workspace, float* grads, int phase, void* stream) {
-  return tb_atarinet_backward_phase_mt(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm,
-                                       precision, workspace, grads, phase, stream);
-}
-
-int tb_atarinet_backward_phase_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                                  const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
-                                  int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream) {
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1 && num_values >= 1 && num_values <= kHeadsMaxValues,
-             "atarinet_backward_phase: bad sizes");
-  TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "atarinet_backward_phase: null pointer");
-  TB_REQUIRE(!use_lstm || notdone, "atarinet_backward_phase: LSTM needs notdone");
-  TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_backward_phase: precision must be 0, 1 or 2");
-  TB_REQUIRE(phase == 1 || phase == 2, "atarinet_backward_phase: phase must be 1 (heads + LSTM) or 2 (conv/fc trunk)");
-  return atarinet_backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, precision, workspace,
-                           grads, (cudaStream_t)stream, phase, num_values);
-}
-
 size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
   return atari_ws(nullptr, T1 * B, T1, B, num_actions, use_lstm, precision).bytes;
 }
 
-int tb_atarinet_forward(const uint8_t* frame, const float* reward, const float* notdone, const int64_t* last_action,
-                        const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
-                        int num_actions, int use_lstm, int precision, void* workspace, float* policy_logits,
-                        float* baseline, float* hN, float* cN, void* stream) {
-  return tb_atarinet_forward_mt(frame, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, 1, use_lstm,
-                                precision, workspace, policy_logits, baseline, hN, cN, stream);
-}
-
-int tb_atarinet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const int64_t* last_action,
-                           const float* h0, const float* c0, const float* params, int64_t T1, int64_t B,
-                           int num_actions, int num_values, int use_lstm, int precision, void* workspace,
-                           float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
+int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                        const int64_t* last_action, const float* h0, const float* c0, const float* params, int64_t T1,
+                        int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                        void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
+                        void* stream) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward: num_values %d outside [1, %d]",
              num_values, kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward: bad sizes T1=%lld B=%lld A=%d", (long long)T1,
@@ -459,62 +428,32 @@ int tb_atarinet_forward_mt(const uint8_t* frame, const float* reward, const floa
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "atarinet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2,
              "atarinet_forward: precision must be 0 (fp32 SIMT), 1 (bf16 tensor cores) or 2 (split-bf16 tensor cores)");
-  return atarinet_forward(frame, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
-                          workspace, policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
-}
-
-int tb_atarinet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                  const int64_t* last_action, const float* h0, const float* c0, const float* params, int64_t T1,
-                                  int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
-                                  void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
-                                  void* stream) {
-  return tb_atarinet_forward_unstacked_mt(frames, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, 1,
-                                          use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN, cN,
-                                          stream);
-}
-
-int tb_atarinet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                     const int64_t* last_action, const float* h0, const float* c0, const float* params,
-                                     int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
-                                     void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
-                                     float* hN, float* cN, void* stream) {
-  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward_unstacked: num_values %d outside [1, %d]",
-             num_values, kHeadsMaxValues);
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward_unstacked: bad sizes T1=%lld B=%lld A=%d",
-             (long long)T1, (long long)B, num_actions);
-  TB_REQUIRE(frames && done && reward && last_action && params && workspace && policy_logits && baseline,
-             "atarinet_forward_unstacked: null pointer");
-  TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "atarinet_forward_unstacked: LSTM needs notdone/h0/c0/hN/cN");
-  TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_forward_unstacked: precision must be 0, 1 or 2");
   cudaStream_t st = (cudaStream_t)stream;
-  if (precision)  // fused: the frame-image pass reads the unstacked rows
-    return atarinet_forward(frames, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
-                            precision, workspace, policy_logits, baseline, hN, cN, st, num_values);
-  TB_REQUIRE(stacked_scratch, "atarinet_forward_unstacked: the fp32 backend needs stacked_scratch "
-                              "(tb_unstacked_scratch_bytes bytes)");
-  uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
-  TB_TRY(restack_frames_u8(frames, done, T1, B, int64_t(AtariGeom::H0) * AtariGeom::W0, stacked, st));
-  return atarinet_forward(stacked, nullptr, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm,
-                          precision, workspace, policy_logits, baseline, hN, cN, st, num_values);
+  // unstacked frames: the tensor-core backends' frame-image pass reads them directly; the fp32 one restacks them first
+  if (done && !precision) {
+    TB_REQUIRE(stacked_scratch, "atarinet_forward: the fp32 backend needs stacked_scratch "
+                                "(tb_unstacked_scratch_bytes bytes)");
+    uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
+    TB_TRY(restack_frames_u8(frame, done, T1, B, int64_t(AtariGeom::H0) * AtariGeom::W0, stacked, st));
+    frame = stacked;
+    done = nullptr;
+  }
+  return atarinet_forward(frame, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
+                          workspace, policy_logits, baseline, hN, cN, st, num_values);
 }
 
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                         const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
-                         void* workspace, float* grads, void* stream) {
-  return tb_atarinet_backward_mt(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision,
-                                 workspace, grads, stream);
-}
-
-int tb_atarinet_backward_mt(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                            const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
-                            int precision, void* workspace, float* grads, void* stream) {
+                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                         int precision, void* workspace, float* grads, int phase, void* stream) {
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1 && num_values >= 1 && num_values <= kHeadsMaxValues,
              "atarinet_backward: bad sizes");
   TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "atarinet_backward: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "atarinet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "atarinet_backward: precision must be 0, 1 or 2");
+  TB_REQUIRE(phase >= 1 && phase <= 3,
+             "atarinet_backward: phase must be 1 (heads + LSTM), 2 (conv/fc trunk) or 3 (the whole backward)");
   return atarinet_backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, precision, workspace,
-                           grads, (cudaStream_t)stream, 3, num_values);
+                           grads, (cudaStream_t)stream, phase, num_values);
 }
 
 }  // extern "C"

@@ -3,7 +3,7 @@
 // Replaces /root/reference/torchbeast/polybeast_learner.py:214-266 (Net.forward) and its autograd graph:
 //   for ch in (16, 32, 32):  x = maxpool3x3/2(conv3x3(x));  x += conv(relu(conv(relu(x))));  x += conv(relu(conv(relu(x))))
 //   x = relu(x) -> fc 3872->256 -> relu -> cat[x, clip(reward)] -> [LSTM(257->256)] -> policy / baseline
-// (3872 = 32 * 11 * 11 for u8 [4, 84, 84] frames; the _obs entry points take other observation shapes, see ResGeom)
+// (3872 = 32 * 11 * 11 for u8 [4, 84, 84] frames; the entry points take other observation shapes, see ResGeom)
 // Same construction as atarinet.cu: NHWC activations, every conv a patch-matrix GEMM through the shared
 // GEMM backends (fp32 SIMT for parity, bf16 wgmma for throughput - the activation element type T
 // follows the backend), residual adds fused into the GEMM epilogue, ReLU-on-read fused into the patch
@@ -41,7 +41,7 @@ constexpr int kObsMinH = 17;
 constexpr int kObsMinW = 33;
 constexpr int kObsMaxHW = 126;
 
-// Section widths (tb_resnet_arch_supported): each of 16, 32 or 64 channels, in any combination.  The shifted-window
+// Section widths (tb_resnet_supported): each of 16, 32 or 64 channels, in any combination.  The shifted-window
 // kernels take 16 / 32 / 64 channels on either side of a conv; 64-channel convs run at W <= 63 (any 64-wide section after
 // the first, or the residual blocks of a 64-wide first section) or 16 -> 64 at W <= 126 (the first conv), which all fit.
 constexpr int kWidths[3] = {16, 32, 64};
@@ -56,15 +56,12 @@ struct ResGeom {
   int fc_in() const { return ch[kSections - 1] * fc_hw(); }
 };
 
-ResGeom res_geom(int C, int H, int W, const int* ch = kDefaultCh) {
+ResGeom res_geom(int C, int H, int W, const int* ch) {
   ResGeom g;
   g.C = C; g.H[0] = H; g.W[0] = W;
   for (int i = 0; i < kSections; ++i) { g.H[i + 1] = (g.H[i] + 1) / 2; g.W[i + 1] = (g.W[i] + 1) / 2; g.ch[i] = ch[i]; }
   return g;
 }
-
-// the Atari stack u8 [4, 84, 84]: 84 -> 42 -> 21 -> 11, fc 3872 -> 256
-const ResGeom kAtariGeom = res_geom(4, 84, 84);
 
 // 0, or 1 with tb_last_error set: the range above, the widths, and on the split-bf16 backend every conv of the geometry
 // on the shifted-window kernels (the other backends' im2col / GEMM kernels take any size)
@@ -486,7 +483,7 @@ struct SplitImpl {
     return sw_conv_fwd(xp, xp_lo, wi, out, N, H, Wd, cin, cout, ep, st);
   }
 
-  // done == nullptr: frame is stacked u8 [T1,B,C,H,W]; otherwise an unstacked rollout u8 [T1+3,B,84,84] (g = kAtariGeom),
+  // done == nullptr: frame is stacked u8 [T1,B,C,H,W]; otherwise an unstacked rollout u8 [T1+3,B,84,84] (g = (4, 84, 84)),
   // restacked by the pass that writes the first conv's input image
   static int forward(const ResGeom& g, const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                      const float* h0, const float* c0, const float* P, int64_t T1, int64_t B, int A, int use_lstm, void* workspace,
@@ -651,46 +648,6 @@ using namespace tb;
 
 extern "C" {
 
-int64_t tb_resnet_param_count(int num_actions, int use_lstm) { return res_params(kAtariGeom, num_actions, use_lstm).total; }
-
-
-int64_t tb_resnet_param_count_mt(int num_actions, int num_values, int use_lstm) {
-  return res_params(kAtariGeom, num_actions, use_lstm, num_values).total;
-}
-
-size_t tb_resnet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
-  return res_ws_bytes(kAtariGeom, T1, B, num_actions, use_lstm, precision);
-}
-
-
-int tb_resnet_forward(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                      const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision, void* workspace,
-                      float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
-  return tb_resnet_forward_mt(frame, reward, notdone, h0, c0, params, T1, B, num_actions, 1, use_lstm, precision, workspace, policy_logits, baseline, hN, cN, stream);
-}
-
-int tb_resnet_forward_mt(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                      const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
-                      float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
-  return tb_resnet_forward_obs(frame, reward, notdone, h0, c0, params, 4, 84, 84, T1, B, num_actions, num_values, use_lstm, precision,
-                               workspace, policy_logits, baseline, hN, cN, stream);
-}
-
-
-int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                       const float* params, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision,
-                       void* workspace, float* grads, void* stream) {
-  return tb_resnet_backward_mt(frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision, workspace, grads, stream);
-}
-
-int tb_resnet_backward_mt(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                       const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
-                       void* workspace, float* grads, void* stream) {
-  return tb_resnet_backward_obs(frame, grad_logits, grad_baseline, notdone, params, 4, 84, 84, T1, B, num_actions, num_values,
-                                use_lstm, precision, workspace, grads, stream);
-}
-
-
 int tb_resnet_obs_range(int* range) {
   TB_REQUIRE(range, "resnet_obs_range: null pointer");
   const int r[6] = {1, kObsMaxC, kObsMinH, kObsMaxHW, kObsMinW, kObsMaxHW};
@@ -704,85 +661,71 @@ int tb_resnet_widths(int* widths) {
   return 0;
 }
 
-int tb_resnet_obs_supported(int C, int H, int W, int precision) {
-  return res_geom_check(C, H, W, kDefaultCh, precision, "resnet_obs_supported") == 0 ? 1 : 0;
+int tb_resnet_supported(int C, int H, int W, int ch0, int ch1, int ch2, int precision) {
+  const int ch[kSections] = {ch0, ch1, ch2};
+  return res_geom_check(C, H, W, ch, precision, "resnet_supported") == 0 ? 1 : 0;
 }
 
-int tb_resnet_arch_supported(int C, int H, int W, int c0, int c1, int c2, int precision) {
-  const int ch[kSections] = {c0, c1, c2};
-  return res_geom_check(C, H, W, ch, precision, "resnet_arch_supported") == 0 ? 1 : 0;
-}
-
-int64_t tb_resnet_param_count_obs(int C, int H, int W, int num_actions, int num_values, int use_lstm) {
-  return tb_resnet_param_count_arch(C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], num_actions, num_values, use_lstm);
-}
-
-int64_t tb_resnet_param_count_arch(int C, int H, int W, int c0, int c1, int c2, int num_actions, int num_values, int use_lstm) {
-  const int ch[kSections] = {c0, c1, c2};
+int64_t tb_resnet_param_count(int C, int H, int W, int ch0, int ch1, int ch2, int num_actions, int num_values, int use_lstm) {
+  const int ch[kSections] = {ch0, ch1, ch2};
   if (res_geom_check(C, H, W, ch, 0, "resnet_param_count")) return -1;
   return res_params(res_geom(C, H, W, ch), num_actions, use_lstm, num_values).total;
 }
 
-size_t tb_resnet_workspace_bytes_obs(int C, int H, int W, int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
-  return tb_resnet_workspace_bytes_arch(C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], T1, B, num_actions, use_lstm,
-                                        precision);
-}
-
-size_t tb_resnet_workspace_bytes_arch(int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B, int num_actions,
-                                      int use_lstm, int precision) {
-  const int ch[kSections] = {c0, c1, c2};
+size_t tb_resnet_workspace_bytes(int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1, int64_t B, int num_actions,
+                                 int use_lstm, int precision) {
+  const int ch[kSections] = {ch0, ch1, ch2};
   if (res_geom_check(C, H, W, ch, precision, "resnet_workspace_bytes")) return 0;
   return res_ws_bytes(res_geom(C, H, W, ch), T1, B, num_actions, use_lstm, precision);
 }
 
-int tb_resnet_forward_obs(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                          const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions, int num_values,
-                          int use_lstm, int precision, void* workspace, float* policy_logits, float* baseline, float* hN, float* cN,
-                          void* stream) {
-  return tb_resnet_forward_arch(frame, reward, notdone, h0, c0, params, C, H, W, kDefaultCh[0], kDefaultCh[1], kDefaultCh[2], T1,
-                                B, num_actions, num_values, use_lstm, precision, workspace, policy_logits, baseline, hN, cN, stream);
-}
-
-int tb_resnet_forward_arch(const uint8_t* frame, const float* reward, const float* notdone, const float* h0, const float* c0,
-                           const float* params, int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1, int64_t B,
-                           int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* policy_logits,
-                           float* baseline, float* hN, float* cN, void* stream) {
+int tb_resnet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone, const float* h0,
+                      const float* c0, const float* params, int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1,
+                      int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                      void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN, void* stream) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_forward: num_values %d outside [1, %d]", num_values,
              kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward: bad sizes");
   TB_REQUIRE(frame && reward && params && workspace && policy_logits && baseline, "resnet_forward: null pointer");
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward: precision must be 0 (fp32), 1 (bf16) or 2 (split-bf16)");
+  TB_REQUIRE(!done || (C == 4 && H == 84 && W == 84 && ch0 == kDefaultCh[0] && ch1 == kDefaultCh[1] && ch2 == kDefaultCh[2]),
+             "resnet_forward: unstacked frames (done != NULL) need the (4, 84, 84) observation and the default widths "
+             "(16, 32, 32), got (%d, %d, %d) and (%d, %d, %d)", C, H, W, ch0, ch1, ch2);
   const int ch[kSections] = {ch0, ch1, ch2};
   TB_TRY(res_geom_check(C, H, W, ch, precision, "resnet_forward"));
   const ResGeom g = res_geom(C, H, W, ch);
-  if (precision == 2)
-    return SplitImpl::forward(g, frame, nullptr, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                              policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision == 2)  // unstacked frames: the restack is fused into the first conv's image pass
+    return SplitImpl::forward(g, frame, done, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
+                              policy_logits, baseline, hN, cN, st, num_values);
+  if (done) {
+    TB_REQUIRE(stacked_scratch, "resnet_forward: the fp32 / bf16 backends need stacked_scratch "
+                                "(tb_unstacked_scratch_bytes bytes)");
+    uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
+    TB_TRY(restack_frames_u8(frame, done, T1, B, 84 * 84, stacked, st));
+    frame = stacked;
+  }
   if (precision)
     return Impl<__nv_bfloat16>::forward(g, frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                                        policy_logits, baseline, hN, cN, (cudaStream_t)stream, num_values);
+                                        policy_logits, baseline, hN, cN, st, num_values);
   return Impl<float>::forward(g, frame, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace, policy_logits,
-                              baseline, hN, cN, (cudaStream_t)stream, num_values);
+                              baseline, hN, cN, st, num_values);
 }
 
-int tb_resnet_backward_obs(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                           const float* params, int C, int H, int W, int64_t T1, int64_t B, int num_actions, int num_values,
-                           int use_lstm, int precision, void* workspace, float* grads, void* stream) {
-  return tb_resnet_backward_arch(frame, grad_logits, grad_baseline, notdone, params, C, H, W, kDefaultCh[0], kDefaultCh[1],
-                                 kDefaultCh[2], T1, B, num_actions, num_values, use_lstm, precision, workspace, grads, stream);
-}
-
-int tb_resnet_backward_arch(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
-                            const float* params, int C, int H, int W, int c0, int c1, int c2, int64_t T1, int64_t B, int num_actions,
-                            int num_values, int use_lstm, int precision, void* workspace, float* grads, void* stream) {
+int tb_resnet_backward(const uint8_t* frame, const float* grad_logits, const float* grad_baseline, const float* notdone,
+                       const float* params, int C, int H, int W, int ch0, int ch1, int ch2, int64_t T1, int64_t B,
+                       int num_actions, int num_values, int use_lstm, int precision, void* workspace, float* grads,
+                       void* stream) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_backward: num_values %d outside [1, %d]", num_values,
              kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward: bad sizes");
-  TB_REQUIRE(frame && grad_logits && grad_baseline && params && workspace && grads, "resnet_backward: null pointer");
+  // the split-bf16 backend reads the first conv's input image from the workspace, the others re-read the frame
+  TB_REQUIRE((frame || precision == 2) && grad_logits && grad_baseline && params && workspace && grads,
+             "resnet_backward: null pointer");
   TB_REQUIRE(!use_lstm || notdone, "resnet_backward: LSTM needs notdone");
   TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward: precision must be 0, 1 or 2");
-  const int ch[kSections] = {c0, c1, c2};
+  const int ch[kSections] = {ch0, ch1, ch2};
   TB_TRY(res_geom_check(C, H, W, ch, precision, "resnet_backward"));
   const ResGeom g = res_geom(C, H, W, ch);
   if (precision == 2)
@@ -793,70 +736,6 @@ int tb_resnet_backward_arch(const uint8_t* frame, const float* grad_logits, cons
                                          workspace, grads, (cudaStream_t)stream, num_values);
   return Impl<float>::backward(g, frame, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace,
                                grads, (cudaStream_t)stream, num_values);
-}
-
-
-int tb_resnet_forward_unstacked(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B, int num_actions,
-                                int use_lstm, int precision, void* workspace, void* stacked_scratch, float* policy_logits,
-                                float* baseline, float* hN, float* cN, void* stream) {
-  return tb_resnet_forward_unstacked_mt(frames, done, reward, notdone, h0, c0, params, T1, B, num_actions, 1, use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN, cN, stream);
-}
-
-int tb_resnet_forward_unstacked_mt(const uint8_t* frames, const uint8_t* done, const float* reward, const float* notdone,
-                                const float* h0, const float* c0, const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
-                                int use_lstm, int precision, void* workspace, void* stacked_scratch, float* policy_logits,
-                                float* baseline, float* hN, float* cN, void* stream) {
-  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_forward_unstacked: num_values %d outside [1, %d]", num_values,
-             kHeadsMaxValues);
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_forward_unstacked: bad sizes");
-  TB_REQUIRE(frames && done && reward && params && workspace && policy_logits && baseline,
-             "resnet_forward_unstacked: null pointer");
-  TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "resnet_forward_unstacked: LSTM needs notdone/h0/c0/hN/cN");
-  TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_forward_unstacked: precision must be 0, 1 or 2");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (precision == 2)  // fused into the first conv's image pass
-    return SplitImpl::forward(kAtariGeom, frames, done, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                              policy_logits, baseline, hN, cN, st, num_values);
-  TB_REQUIRE(stacked_scratch, "resnet_forward_unstacked: the fp32 / bf16 backends need stacked_scratch "
-                              "(tb_unstacked_scratch_bytes bytes)");
-  uint8_t* stacked = static_cast<uint8_t*>(stacked_scratch);
-  TB_TRY(restack_frames_u8(frames, done, T1, B, 84 * 84, stacked, st));
-  if (precision)
-    return Impl<__nv_bfloat16>::forward(kAtariGeom, stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                                        policy_logits, baseline, hN, cN, st, num_values);
-  return Impl<float>::forward(kAtariGeom, stacked, reward, notdone, h0, c0, params, T1, B, num_actions, use_lstm, workspace,
-                              policy_logits, baseline, hN, cN, st, num_values);
-}
-
-
-int tb_resnet_backward_unstacked(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
-                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions,
-                                 int use_lstm, int precision, void* workspace, float* grads, void* stream) {
-  return tb_resnet_backward_unstacked_mt(stacked_scratch, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, 1, use_lstm, precision, workspace, grads, stream);
-}
-
-int tb_resnet_backward_unstacked_mt(const void* stacked_scratch, const float* grad_logits, const float* grad_baseline,
-                                 const float* notdone, const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
-                                 int use_lstm, int precision, void* workspace, float* grads, void* stream) {
-  TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "resnet_backward_unstacked: num_values %d outside [1, %d]", num_values,
-             kHeadsMaxValues);
-  TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "resnet_backward_unstacked: bad sizes");
-  TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "resnet_backward_unstacked: null pointer");
-  TB_REQUIRE(!use_lstm || notdone, "resnet_backward_unstacked: LSTM needs notdone");
-  TB_REQUIRE(precision >= 0 && precision <= 2, "resnet_backward_unstacked: precision must be 0, 1 or 2");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (precision == 2)
-    return SplitImpl::backward(kAtariGeom, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, workspace, grads,
-                               st, num_values);
-  TB_REQUIRE(stacked_scratch, "resnet_backward_unstacked: the fp32 / bf16 backends re-read the restacked frames from "
-                              "stacked_scratch");
-  const uint8_t* stacked = static_cast<const uint8_t*>(stacked_scratch);
-  if (precision)
-    return Impl<__nv_bfloat16>::backward(kAtariGeom, stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions,
-                                         use_lstm, workspace, grads, st, num_values);
-  return Impl<float>::backward(kAtariGeom, stacked, grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm,
-                               workspace, grads, st, num_values);
 }
 
 }  // extern "C"

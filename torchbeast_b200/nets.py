@@ -407,7 +407,7 @@ class AtariNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_atarinet_param_count_mt(num_actions, self.num_values, int(use_lstm))
+        count = _lib.lib().tb_atarinet_param_count(num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def initial_state(self, batch_size):
@@ -448,41 +448,26 @@ class AtariNet(FlatParamModule):
             h0 = c0 = notdone = None
         ws = self._workspace(T1, B)
         p = _lib.ptr
-        if unstacked:
-            _lib.check(
-                _lib.lib().tb_atarinet_forward_unstacked_mt(
-                    p(frame), p(done), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
-                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)),
-                    p(logits), p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None,
-                    _lib.stream_ptr()),
-                "tb_atarinet_forward_unstacked")
-            return logits, baseline, hN, cN
         _lib.check(
-            _lib.lib().tb_atarinet_forward_mt(
-                p(frame), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), T1, B,
-                self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(logits), p(baseline),
-                p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
+            _lib.lib().tb_atarinet_forward(
+                p(frame), p(done) if unstacked else None, p(reward), p(notdone), p(last_action), p(h0), p(c0),
+                p(self._flat), T1, B, self.num_actions, self.num_values, int(self.use_lstm),
+                self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)) if unstacked else None, p(logits),
+                p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_atarinet_forward")
         return logits, baseline, hN, cN
 
-    def _launch_backward(self, g_logits, g_baseline, notdone, grads_out, phase=None):
+    def _launch_backward(self, g_logits, g_baseline, notdone, grads_out, phase=3):
+        """phase 3: the whole backward; 1 then 2: heads + LSTM, then the conv/fc trunk."""
         T1, B = g_baseline.shape[:2]
         ws = self._workspace(T1, B)
         p = _lib.ptr
-        if phase is None:
-            _lib.check(
-                _lib.lib().tb_atarinet_backward_mt(
-                    p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out),
-                    _lib.stream_ptr()),
-                "tb_atarinet_backward")
-        else:
-            _lib.check(
-                _lib.lib().tb_atarinet_backward_phase_mt(
-                    p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws), p(grads_out), int(phase),
-                    _lib.stream_ptr()),
-                "tb_atarinet_backward_phase")
+        _lib.check(
+            _lib.lib().tb_atarinet_backward(
+                p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
+                self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws),
+                p(grads_out), int(phase), _lib.stream_ptr()),
+            "tb_atarinet_backward")
 
     def grad_split(self):
         """Flat-gradient offset where the LSTM + heads slice starts (final after backward phase 1 for precision
@@ -630,7 +615,7 @@ class ResNet(FlatParamModule):
         self.num_actions = num_actions
         self.use_lstm = use_lstm
         obs = tuple(int(d) for d in observation_shape)
-        if len(obs) != 3 or not _lib.lib().tb_resnet_obs_supported(*obs, self.PRECISIONS["bf16x3"]):
+        if len(obs) != 3 or not _lib.lib().tb_resnet_supported(*obs, *RESNET_CHANNELS, self.PRECISIONS["bf16x3"]):
             rng = resnet_obs_range()
             raise _lib.TorchBeastB200Error(
                 "ResNet observation_shape must be (C, H, W) with C in [%d, %d], H in [%d, %d] and W in [%d, %d], got %r"
@@ -640,7 +625,7 @@ class ResNet(FlatParamModule):
             ch = tuple(int(c) for c in channels)
         except (TypeError, ValueError):
             ch = ()
-        if len(ch) != 3 or not _lib.lib().tb_resnet_arch_supported(*obs, *ch, self.PRECISIONS["bf16x3"]):
+        if len(ch) != 3 or not _lib.lib().tb_resnet_supported(*obs, *ch, self.PRECISIONS["bf16x3"]):
             raise _lib.TorchBeastB200Error(
                 "ResNet channels must be three section widths, each one of %r, got %r" % (resnet_widths(), channels))
         self.channels = ch
@@ -664,7 +649,7 @@ class ResNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_resnet_param_count_arch(*obs, *ch, num_actions, self.num_values, int(use_lstm))
+        count = _lib.lib().tb_resnet_param_count(*obs, *ch, num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def _fix_module_names(self):
@@ -678,18 +663,19 @@ class ResNet(FlatParamModule):
     def _workspace(self, T1, B):
         key = (T1, B, self._flat.device, self.precision)
         if self._ws_key != key:
-            nbytes = _lib.lib().tb_resnet_workspace_bytes_arch(*self.observation_shape, *self.channels, T1, B,
-                                                               self.num_actions, int(self.use_lstm),
-                                                               self.PRECISIONS[self.precision])
+            nbytes = _lib.lib().tb_resnet_workspace_bytes(*self.observation_shape, *self.channels, T1, B,
+                                                          self.num_actions, int(self.use_lstm),
+                                                          self.PRECISIONS[self.precision])
             if nbytes == 0:
-                raise _lib.TorchBeastB200Error("tb_resnet_workspace_bytes_arch: %s" % _lib.lib().tb_last_error().decode())
+                raise _lib.TorchBeastB200Error("tb_resnet_workspace_bytes: %s" % _lib.lib().tb_last_error().decode())
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
             self._ws_key = key
         return self._ws
 
     def _launch_forward(self, frame, reward, notdone, h0, c0, done=None):
-        """Returns (logits, baseline, hN, cN, saved): `saved` is what _launch_backward re-reads - the stacked frame, or
-        ("unstacked", stacked scratch or None).  `done` is read only with an unstacked frame, to rebuild the stacks."""
+        """Returns (logits, baseline, hN, cN, saved): `saved` is the frame _launch_backward re-reads - the stacked frame,
+        or with an unstacked one the stacked scratch it was rebuilt into (None where the backend needs none).  `done` is
+        read only with an unstacked frame, to rebuild the stacks."""
         _lib.require_cuda(frame, reward, self._flat)
         unstacked = frame_is_unstacked(frame, reward, self.observation_shape, self.channels)
         T1, B = reward.shape[:2] if unstacked else frame.shape[:2]
@@ -709,40 +695,23 @@ class ResNet(FlatParamModule):
             hN = cN = torch.empty(0, device=dev)
             h0 = c0 = notdone = None
         p = _lib.ptr
-        if unstacked:
-            scratch = _scratch(self, 1, T1, B)
-            _lib.check(
-                _lib.lib().tb_resnet_forward_unstacked_mt(
-                    p(frame), p(done), p(reward), p(notdone), p(h0), p(c0), p(self._flat), T1, B, self.num_actions,
-                    self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(scratch), p(logits),
-                    p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
-                "tb_resnet_forward_unstacked")
-            return logits, baseline, hN, cN, ("unstacked", scratch)
+        scratch = _scratch(self, 1, T1, B) if unstacked else None
         _lib.check(
-            _lib.lib().tb_resnet_forward_arch(
-                p(frame), p(reward), p(notdone), p(h0), p(c0), p(self._flat), *self.observation_shape, *self.channels, T1, B,
-                self.num_actions,
-                self.num_values, int(self.use_lstm),
-                self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits), p(baseline),
+            _lib.lib().tb_resnet_forward(
+                p(frame), p(done) if unstacked else None, p(reward), p(notdone), p(h0), p(c0), p(self._flat),
+                *self.observation_shape, *self.channels, T1, B, self.num_actions, self.num_values, int(self.use_lstm),
+                self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(scratch), p(logits), p(baseline),
                 p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
             "tb_resnet_forward")
-        return logits, baseline, hN, cN, frame
+        return logits, baseline, hN, cN, scratch if unstacked else frame
 
-    def _launch_backward(self, saved, g_logits, g_baseline, notdone, grads_out):
+    def _launch_backward(self, frame, g_logits, g_baseline, notdone, grads_out):
+        """`frame`: the `saved` of the forward."""
         T1, B = g_baseline.shape[:2]
         p = _lib.ptr
-        if isinstance(saved, tuple):  # ("unstacked", scratch): the backward reads the workspace (+ the restacked scratch)
-            _lib.check(
-                _lib.lib().tb_resnet_backward_unstacked_mt(
-                    p(saved[1]), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
-                    self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(self._workspace(T1, B)),
-                    p(grads_out), _lib.stream_ptr()),
-                "tb_resnet_backward_unstacked")
-            return
-        frame = saved
         _lib.check(
-            _lib.lib().tb_resnet_backward_arch(
-                p(frame.contiguous()), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
+            _lib.lib().tb_resnet_backward(
+                p(frame), p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat),
                 *self.observation_shape, *self.channels, T1, B, self.num_actions, self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(grads_out), _lib.stream_ptr()),
             "tb_resnet_backward")
