@@ -493,8 +493,8 @@ int tb_host_write_rollout_column(uint8_t* slot_base, const int64_t* leaf_offset,
  * nn.utils.clip_grad_norm_ (monobeast.py:291); grads must be 16-byte aligned.                */
 int tb_grad_sumsq_f32(const float* grads, int64_t n, float* out_sumsq, void* workspace, void* stream);
 /* Second half of clip_grad_norm_ fused with torch.optim.RMSprop.step() (monobeast.py:292,388-394):
- *   coef = min(1, max_norm/(sqrt(sumsq)+1e-6)) (max_norm < 0: no clipping); grads *= coef (left
- *   clipped in place like the reference); square_avg = alpha*square_avg + (1-alpha)*g^2;
+ *   coef = min(1, max_norm/(sqrt(sumsq)+1e-6)), NaN when sumsq is NaN as torch.clamp gives it (max_norm < 0: no
+ *   clipping); grads *= coef (left clipped in place like the reference); square_avg = alpha*square_avg + (1-alpha)*g^2;
  *   params -= lr * g/(sqrt(square_avg)+eps)   (momentum != 0: buf = momentum*buf + g/avg; params -= lr*buf).
  * lr_device (nullable) overrides `lr` with a device scalar; grad_norm_out (nullable) receives the
  * pre-clip norm.  No host synchronisation.

@@ -30,7 +30,17 @@ __global__ void grad_sumsq_kernel(const float* __restrict__ g, int64_t n, float*
   if (grid_sum3(s, 0.0, 0.0, ws, tot)) out[0] = float(tot[0]);
 }
 
-// coef = min(1, max_norm / (norm + 1e-6)); g *= coef; sq = alpha*sq + (1-alpha) g^2;
+// clip_grad_norm_'s coefficient: min(max_norm / (norm + 1e-6), 1), NaN when the norm is NaN (torch clamps with
+// torch.clamp, which propagates NaN, so one NaN gradient element turns the whole step into NaN); max_norm < 0: 1, no
+// clipping.  Thread 0 of block 0 reports the pre-clip norm.
+__device__ __forceinline__ float clip_coef(const float* sumsq, float max_norm, float* norm_out) {
+  const float norm = sqrtf(sumsq[0]);
+  if (norm_out && blockIdx.x == 0 && threadIdx.x == 0) norm_out[0] = norm;
+  const float coef = max_norm / (norm + 1e-6f);
+  return max_norm >= 0.0f ? (coef > 1.0f ? 1.0f : coef) : 1.0f;  // not fminf: fminf(NaN, 1) is 1
+}
+
+// coef = clip_coef(...); g *= coef; sq = alpha*sq + (1-alpha) g^2;
 // avg = sqrt(sq) + eps; momentum==0: p -= lr * g/avg; else buf = momentum*buf + g/avg; p -= lr*buf
 // hp (nullable) overrides max_norm, alpha, eps and momentum, as lr_dev overrides lr_host.
 __global__ void clip_rmsprop_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ sq,
@@ -39,11 +49,8 @@ __global__ void clip_rmsprop_kernel(float* __restrict__ p, float* __restrict__ g
                                     float eps, float momentum, const tb_hparams* __restrict__ hp,
                                     float* __restrict__ norm_out) {
   if (hp) { max_norm = hp->max_norm; alpha = hp->alpha; eps = hp->eps; momentum = hp->momentum; }
-  const float norm = sqrtf(sumsq[0]);
-  float coef = 1.0f;
-  if (max_norm >= 0.0f) coef = fminf(max_norm / (norm + 1e-6f), 1.0f);
+  const float coef = clip_coef(sumsq, max_norm, norm_out);
   const float lr = lr_dev ? lr_dev[0] : lr_host;
-  if (norm_out && blockIdx.x == 0 && threadIdx.x == 0) norm_out[0] = norm;
   const int64_t stride = int64_t(gridDim.x) * blockDim.x;
   int64_t done = 0;
   if (!mom && ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(sq)) & 15) == 0) {
@@ -76,12 +83,6 @@ __global__ void clip_rmsprop_kernel(float* __restrict__ p, float* __restrict__ g
       p[i] -= lr * (gi / avg);
     }
   }
-}
-
-__device__ __forceinline__ float clip_coef(const float* sumsq, float max_norm, float* norm_out) {
-  const float norm = sqrtf(sumsq[0]);
-  if (norm_out && blockIdx.x == 0 && threadIdx.x == 0) norm_out[0] = norm;
-  return max_norm >= 0.0f ? fminf(max_norm / (norm + 1e-6f), 1.0f) : 1.0f;
 }
 
 __device__ __forceinline__ bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
