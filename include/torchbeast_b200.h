@@ -160,7 +160,40 @@ int tb_impala_loss_f32(const float* behavior_logits, const float* target_logits,
                        float* target_alp, float* losses_out, float* grad_logits, float* grad_values, int zero_tail,
                        void* workspace, void* stream);
 
-/* tb_popart_update: for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
+/* UPGO, the upgoing policy gradient (Vinyals et al. 2019, "Grandmaster level in StarCraft II", Nature 575): a second
+ * launch enqueued right after tb_impala_loss_f32 on the same stream.  It reads that launch's log_rhos and, with a
+ * trust region, its kl_out, so rho and the mask have the same bits.  The other inputs are the loss call's own: target
+ * logits, actions, rewards, done or discounts, values and bootstrap (or the PopArt values, task, mu, nu and K),
+ * column_weights, hp (discounting, clip_rewards and clip_pg_rho are read from it when non-NULL, else from the
+ * arguments) and trust_beta.  In the loss block's row notation (rows t = 0..T-1 of column b, shifted inputs):
+ *   r_t    reward after the reward clip; g_t the discount, from done or discounts as the loss builds it;
+ *   V_t    the value, V_T the bootstrap (PopArt: V_t = sigma_k n_t[k] + mu_k, 0 for a task out of range);
+ *   rho_t  = exp(log_rhos_t).
+ *   Trace switch, t = 0..T-2: lambda_{t+1} = 1 when r_{t+1} + g_{t+1} V_{t+2} >= V_{t+1}, else 0 (a comparison: NaN
+ *     gives 0).
+ *   Return: G_{T-1} = r_{T-1} + g_{T-1} V_T;  G_t = r_t + g_t (lambda_{t+1} G_{t+1} + (1 - lambda_{t+1}) V_{t+1}).
+ *     A lambda-return whose lambda is 0 or 1 at each step; the split-T layout composes it as the loss composes V-trace.
+ *   Advantage: A_t = rhobar_t (G_t - V_t), rhobar_t = min(rho_t m_t, clip_pg_rho) (unclipped when clip_pg_rho is
+ *     negative or NaN, as in the V-trace policy gradient); m_t = (kl_t <= beta) with trust_beta, else 1.  PopArt: A_t
+ *     is divided by sigma_k; a row whose task is out of range gets A_t = 0 and adds nothing.
+ *   Loss: upgo_cost * sum_{t,b} w_b (-log pi_t(a_t)) A_t, with A constant; w_b = column_weights[b], or 1.
+ *     Gradient: upgo_cost * w_b * A_t * (pi_t - onehot(a_t)), ADDED into grad_logits (NULL: forward only); row T and
+ *     the values get nothing.
+ * upgo_cost f32 [1] (device, read when the kernel runs).  outputs: upgo_adv [T,B] f32 = A; upgo_out [1] f32 = the
+ * loss; losses_out[3] (the loss launch's total) becomes float(double(total) + double(upgo_out)).  When *upgo_cost == 0
+ * grad_logits and losses_out are not written, so a zero cost leaves the loss launch's bits.  The sum is fp64 in a fixed
+ * order (no atomics): bit-identical from run to run.  workspace: the one the loss launch used (or any other).  PopArt
+ * requires T >= 1, B >= 1, 1 <= K <= 64, non-NULL mu and nu, and NULL column_weights; trust_beta requires kl.  One
+ * launch.                                                                                                          */
+int tb_upgo_loss_f32(const float* target_logits, const int64_t* actions, const float* rewards, const uint8_t* done,
+                     const float* discounts, const float* values, const float* bootstrap, int64_t T, int64_t B,
+                     int64_t A, float discounting, int clip_rewards, float clip_pg_rho, const tb_hparams* hp,
+                     const float* column_weights, const int64_t* task, const double* mu, const double* nu, int64_t K,
+                     const float* log_rhos, const float* trust_beta, const float* kl, const float* upgo_cost,
+                     float* upgo_adv, float* upgo_out, float* losses_out, float* grad_logits, void* workspace,
+                     void* stream);
+
+/* tb_popart_update:for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
  *   first), with beta read from device memory and sigma_k as in tb_impala_loss_f32:
  *     mu'_k = (1 - beta) mu_k + beta * sum vs / count,   nu'_k = (1 - beta) nu_k + beta * sum vs^2 / count
  *   then rescales value-head row k so that its unnormalised outputs do not change:

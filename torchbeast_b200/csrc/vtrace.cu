@@ -730,6 +730,137 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
 }
 
 // ----------------------------------------------------------------------------------------
+// UPGO: upgoing policy gradient (tb_upgo_loss_f32), a second launch after impala_loss_kernel
+// ----------------------------------------------------------------------------------------
+// The loss's arguments (so reward_of, discount_of and load_hparams apply unchanged) plus UPGO's own.  log_rhos and kl are
+// the loss launch's outputs, read here.
+struct UpgoArgs : LossArgs {
+  const float* upgo_cost;  // f32 [1], read when the kernel runs; 0: grad_logits and losses are not written
+  float* upgo_adv;         // [T,B] out
+  float* upgo_out;         // [1] out: the weighted loss
+};
+
+// The return is carried backwards as X_t = lambda_t ? G_t : V_t, X_T = V_T, so G_t = r_t + g_t X_{t+1}.  A chunk of rows
+// is the affine map X_t0 = a X_t1 + bb, which is the select above when composed row by row (a = 0 after a lambda of 0),
+// so the split-T layout composes it across warps as the loss kernel composes its V-trace maps.
+// __maxnreg__(128) is the register ceiling of a 512-thread block, as __launch_bounds__(512) would give; under the
+// latter ptxas settled on 64 registers and spilled in some instantiations.
+template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false>
+__global__ void __maxnreg__(128) upgo_loss_kernel(UpgoArgs p) {
+  if (p.hp) load_hparams(p);
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float* sA = reinterpret_cast<float*>(smem_raw);
+  float* sB = sA + blockDim.y * kWarp;
+  float* sMu = sB + blockDim.y * kWarp;
+  float* sSig = sMu + kPopArtMaxTasks;
+  if constexpr (kPopArt) {
+    for (int k = threadIdx.x + threadIdx.y * blockDim.x; k < p.K; k += blockDim.x * blockDim.y) {
+      const double mu = p.pa_mu[k];
+      sMu[k] = float(mu);
+      sSig[k] = float(popart_sigma(mu, p.pa_nu[k]));
+    }
+    __syncthreads();
+  }
+  const int64_t T = p.T, B = p.B;
+  // V_t of column b, t == T: the bootstrap value (PopArt: unnormalised as in impala_loss_kernel's pop_value)
+  auto value_of = [&](int64_t t, int64_t b) -> float {
+    if constexpr (kPopArt) {
+      const int64_t k = p.task[t * B + b];
+      return (k >= 0 && k < p.K) ? sSig[k] * p.values[(t * B + b) * p.K + k] + sMu[k] : 0.0f;
+    } else {
+      return t < T ? p.values[t * B + b] : p.bootstrap[b];
+    }
+  };
+  const float cost = *p.upgo_cost;
+  const int lane = threadIdx.x;
+  const int w = p.wide ? 0 : threadIdx.y, W = p.wide ? 1 : blockDim.y;
+  const int64_t Ause = A ? A : p.A;
+  const int64_t tiles = (B + kWarp - 1) / kWarp;
+  const int64_t chunk = (T + W - 1) / W;
+  const int64_t t0 = (int64_t(w) * chunk < T) ? int64_t(w) * chunk : T;
+  const int64_t t1 = (t0 + chunk < T) ? t0 + chunk : T;
+  const int64_t tile0 = p.wide ? int64_t(blockIdx.x) * blockDim.y + threadIdx.y : blockIdx.x;
+  const int64_t tile_step = p.wide ? int64_t(gridDim.x) * blockDim.y : gridDim.x;
+  double s_up = 0.0;
+
+  for (int64_t tile = tile0; tile < tiles; tile += tile_step) {
+    const int64_t b = tile * kWarp + lane;
+    const bool active = b < B;
+    float x_in = active ? value_of(T, b) : 0.0f;  // X_T = V_T
+    if (W > 1) {
+      float a = 1.0f, bb = 0.0f;
+      if (active && t1 > t0) {
+        float v_next = value_of(t1, b);
+        for (int64_t t = t1 - 1; t >= t0; --t) {
+          const int64_t i = t * B + b;
+          const float g = discount_of(p, i), r = reward_of(p, i), v = value_of(t, b);
+          if (r + g * v_next >= v) {  // lambda_t = 1
+            bb = r + g * bb;
+            a = g * a;
+          } else {
+            bb = v;
+            a = 0.0f;
+          }
+          v_next = v;
+        }
+      }
+      __syncthreads();
+      sA[w * kWarp + lane] = a;
+      sB[w * kWarp + lane] = bb;
+      __syncthreads();
+      for (int w2 = W - 1; w2 > w; --w2) x_in = sB[w2 * kWarp + lane] + sA[w2 * kWarp + lane] * x_in;
+    }
+    if (!active || t1 <= t0) continue;
+    float v_next = value_of(t1, b);
+    float x = x_in;  // X_{t+1}
+    for (int64_t t = t1 - 1; t >= t0; --t) {
+      const int64_t i = t * B + b;
+      const float g = discount_of(p, i), r = reward_of(p, i), v = value_of(t, b);
+      const float G = r + g * x;
+      x = (r + g * v_next >= v) ? G : v;
+      v_next = v;
+      float rho = expf(p.log_rhos[i]);
+      if constexpr (kTrust) rho = p.kl[i] <= *p.trust_beta ? rho : 0.0f;
+      const float rp = p.has_clip_pg ? fminf(rho, p.clip_pg) : rho;
+      float adv = rp * (G - v);
+      if constexpr (kPopArt) {
+        const int64_t k = p.task[i];
+        if (k < 0 || k >= p.K) {  // adds nothing
+          p.upgo_adv[i] = 0.0f;
+          continue;
+        }
+        adv = adv / sSig[k];
+      }
+      p.upgo_adv[i] = adv;
+      const int64_t act = p.actions[i];
+      const float* trow = p.tlogits + i * Ause;
+      float m, logs;
+      const float tlp = alp_row<float, A>(trow, Ause, act, &m, &logs);
+      float scale = cost * adv;  // d loss / d logits = cost * w_b * adv * (pi - onehot)
+      if constexpr (kWeighted) {
+        const float wb = __ldg(p.column_weights + b);
+        s_up += double(-tlp * adv) * double(wb);
+        scale *= wb;
+      } else {
+        s_up += double(-tlp * adv);
+      }
+      if (p.grad_logits && cost != 0.0f) {
+        // the row is re-read (L1) rather than kept in registers from alp_row
+        float* grow = p.grad_logits + i * Ause;
+#pragma unroll
+        for (int64_t j = 0; j < Ause; ++j) grow[j] += scale * (expf((trow[j] - m) - logs) - (act == j ? 1.0f : 0.0f));
+      }
+    }
+  }
+  double tot[3];
+  if (grid_sum3(s_up, 0.0, 0.0, p.workspace, tot)) {
+    const float up = float(double(cost) * tot[0]);
+    p.upgo_out[0] = up;
+    if (cost != 0.0f) p.losses[3] = float(double(p.losses[3]) + double(up));
+  }
+}
+
+// ----------------------------------------------------------------------------------------
 // PopArt statistics
 // ----------------------------------------------------------------------------------------
 // sums[k] = count, sums[K+k] = sum vs, sums[2K+k] = sum vs^2 over the rows t < T of task k.  CTA k owns task k and
@@ -969,6 +1100,88 @@ int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
   TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
   return check_launch("impala_loss_kernel");
+}
+
+// The kernel instantiation follows from which of column_weights, task and trust_beta are non-NULL, as in the loss.
+int tb_upgo_loss_f32(const float* tlogits, const int64_t* actions, const float* rewards, const uint8_t* done,
+                     const float* discounts, const float* values, const float* bootstrap, int64_t T, int64_t B,
+                     int64_t A, float discounting, int clip_rewards, float clip_pg_rho, const tb_hparams* hp,
+                     const float* column_weights, const int64_t* task, const double* mu, const double* nu, int64_t K,
+                     const float* log_rhos, const float* trust_beta, const float* kl, const float* upgo_cost,
+                     float* upgo_adv, float* upgo_out, float* losses_out, float* grad_logits, void* workspace,
+                     void* stream) {
+  if (task) {
+    TB_REQUIRE(!column_weights, "upgo_loss_popart: column_weights are not supported with PopArt (task)");
+    TB_REQUIRE(T >= 1 && B >= 1, "upgo_loss_popart: bad sizes T=%lld B=%lld", (long long)T, (long long)B);
+    TB_REQUIRE(K >= 1 && K <= kPopArtMaxTasks, "upgo_loss_popart: num_tasks %lld outside [1, %d]", (long long)K,
+               kPopArtMaxTasks);
+    TB_REQUIRE(values && mu && nu, "upgo_loss_popart: null PopArt pointer");
+    bootstrap = values;  // not read: the bootstrap row is row T of values
+  }
+  TB_REQUIRE(T >= 0 && B >= 0 && A >= 1, "upgo_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T, (long long)B,
+             (long long)A);
+  TB_REQUIRE(upgo_cost && upgo_out && losses_out && workspace,
+             "upgo_loss: upgo_cost/upgo_out/losses_out/workspace must not be null");
+  TB_REQUIRE(!trust_beta || kl, "upgo_loss_trust: kl must not be null");
+  if (T == 0 || B == 0) {
+    cudaError_t e = cudaMemsetAsync(upgo_out, 0, sizeof(float), (cudaStream_t)stream);
+    TB_REQUIRE(e == cudaSuccess, "upgo_loss: memset: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  TB_REQUIRE(tlogits && actions && rewards && (done || discounts) && values && bootstrap && log_rhos,
+             "upgo_loss: null input pointer");
+  TB_REQUIRE(upgo_adv, "upgo_loss: upgo_adv must not be null");
+  UpgoArgs p = {};
+  p.tlogits = tlogits; p.actions = actions; p.rewards = rewards; p.done = done; p.discounts = discounts;
+  p.values = values; p.bootstrap = bootstrap; p.T = T; p.B = B; p.A = A;
+  p.discounting = discounting; p.clip_rewards = clip_rewards; p.clip_pg = clip_pg_rho;
+  p.has_clip_pg = (clip_pg_rho >= 0.0f);
+  p.log_rhos = const_cast<float*>(log_rhos);  // read only
+  p.losses = losses_out; p.grad_logits = grad_logits; p.workspace = workspace; p.hp = hp;
+  p.task = task; p.pa_mu = mu; p.pa_nu = nu; p.K = int(K);
+  p.column_weights = column_weights;
+  p.trust_beta = trust_beta; p.kl = const_cast<float*>(kl);  // read only
+  p.upgo_cost = upgo_cost; p.upgo_adv = upgo_adv; p.upgo_out = upgo_out;
+  const int64_t tiles = (B + kWarp - 1) / kWarp;
+  int W = pick_warps(T, tiles);
+  p.wide = (W == 1);
+  dim3 grid(pick_grid(tiles));
+  if (p.wide) {
+    W = kWideWarps;
+    int64_t g = (tiles + W - 1) / W;
+    if (g > kMaxPartialCtas) g = kMaxPartialCtas;
+    grid = dim3((unsigned)(g < 1 ? 1 : g));
+  }
+  dim3 block(kWarp, W);
+  const size_t smem = size_t(2) * W * kWarp * sizeof(float);
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (task) {
+    ProfScope prof(trust_beta ? "upgo_loss_popart_trust" : "upgo_loss_popart", s);
+    const size_t pop_smem = smem + size_t(2) * kPopArtMaxTasks * sizeof(float);
+    if (trust_beta) {
+      TB_DISPATCH_A(A, (upgo_loss_kernel<kA, true, false, true><<<grid, block, pop_smem, s>>>(p)));
+      return check_launch("upgo_loss_kernel<popart, trust>");
+    }
+    TB_DISPATCH_A(A, (upgo_loss_kernel<kA, true><<<grid, block, pop_smem, s>>>(p)));
+    return check_launch("upgo_loss_kernel<popart>");
+  }
+  if (trust_beta) {
+    ProfScope prof("upgo_loss_trust", s);
+    if (column_weights) {
+      TB_DISPATCH_A(A, (upgo_loss_kernel<kA, false, true, true><<<grid, block, smem, s>>>(p)));
+      return check_launch("upgo_loss_kernel<weighted, trust>");
+    }
+    TB_DISPATCH_A(A, (upgo_loss_kernel<kA, false, false, true><<<grid, block, smem, s>>>(p)));
+    return check_launch("upgo_loss_kernel<trust>");
+  }
+  if (column_weights) {
+    ProfScope prof("upgo_loss_weighted", s);
+    TB_DISPATCH_A(A, (upgo_loss_kernel<kA, false, true><<<grid, block, smem, s>>>(p)));
+    return check_launch("upgo_loss_kernel<weighted>");
+  }
+  ProfScope prof("upgo_loss", s);
+  TB_DISPATCH_A(A, (upgo_loss_kernel<kA><<<grid, block, smem, s>>>(p)));
+  return check_launch("upgo_loss_kernel");
 }
 
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,

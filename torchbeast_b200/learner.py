@@ -16,6 +16,9 @@ ImpalaLoss = collections.namedtuple(
 # What the trust-region loss returns next to its ImpalaLoss: kl float32 [T, B] = KL(pi_t || mu_t) of every row, sums
 # float32 [2] = {number of trusted rows, sum of kl over all rows}.
 TrustRegion = collections.namedtuple("TrustRegion", "kl sums")
+# What the loss returns last when given upgo_cost: adv float32 [T, B] = the UPGO advantage of every row, loss float32
+# [1] = upgo_cost * sum w_b * (-log pi(a)) * adv (already included in losses[3]).
+Upgo = collections.namedtuple("Upgo", "adv loss")
 
 # tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the entry points read from device memory.
 # tb_hparams_layout() reports the compiled layout; tests/test_graph_hparams_cpu.py checks this record against it.
@@ -71,19 +74,33 @@ def trust_region_kl(flags):
     return beta
 
 
-def _trust_beta_tensor(trust_region, device):
-    """The device float32 [1] beta the trust-region kernels read: `trust_region` itself when it is a tensor (a graph's
-    published scalar), else a new one holding float(trust_region)."""
-    if isinstance(trust_region, torch.Tensor):
-        _lib.require_cuda(trust_region)
-        if trust_region.dtype != torch.float32 or trust_region.numel() != 1:
-            raise _lib.TorchBeastB200Error("trust_region must be a float or a float32 device scalar, got %s %r" % (
-                trust_region.dtype, tuple(trust_region.shape)))
-        return trust_region
-    beta = float(trust_region)
-    if not beta >= 0.0:
-        raise ValueError("trust_region must be >= 0, got %r" % (trust_region,))
-    return torch.full((1,), beta, dtype=torch.float32, device=device)
+def upgo_cost(flags):
+    """flags.upgo_cost as a finite float >= 0, or None when the flag is None or absent (no UPGO).  Raises ValueError for
+    a negative, NaN, infinite, boolean or non-numeric value, before anything is launched."""
+    v = getattr(flags, "upgo_cost", None)
+    if v is None:
+        return None
+    if isinstance(v, bool) or not isinstance(v, numbers.Real):
+        raise ValueError("upgo_cost must be None or a finite number >= 0, got %r" % (v,))
+    cost = float(v)
+    if not 0.0 <= cost < float("inf"):  # NaN fails too
+        raise ValueError("upgo_cost must be finite and >= 0 (or None), got %r" % (v,))
+    return cost
+
+
+def _device_scalar(value, name, device, finite=False):
+    """The device float32 [1] a kernel reads when it runs: `value` itself when it is a tensor (a graph's published
+    scalar), else a new one holding float(value), which must be >= 0 (and finite with `finite`)."""
+    if isinstance(value, torch.Tensor):
+        _lib.require_cuda(value)
+        if value.dtype != torch.float32 or value.numel() != 1:
+            raise _lib.TorchBeastB200Error("%s must be a float or a float32 device scalar, got %s %r" % (
+                name, value.dtype, tuple(value.shape)))
+        return value
+    x = float(value)
+    if not (0.0 <= x < float("inf") if finite else x >= 0.0):
+        raise ValueError("%s must be >= 0%s, got %r" % (name, " and finite" if finite else "", value))
+    return torch.full((1,), x, dtype=torch.float32, device=device)
 
 
 def hparams_field(block, name):
@@ -112,8 +129,9 @@ def impala_loss_fwd_bwd(
     hparams_dev=None,
     column_weights=None,
     trust_region=None,
+    upgo_cost=None,
 ):
-    """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_f32).
+    """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_f32), two with UPGO.
 
     Inputs are the shifted [T,B,...] slices (batch[1:], learner_outputs[:-1]); `done` is a
     bool/uint8 tensor.  Replaces monobeast.py:245-277 / polybeast_learner.py:332-361 and the
@@ -133,6 +151,11 @@ def impala_loss_fwd_bwd(
     KL(pi || mu) exceeds beta gets rho = 0 in the V-trace and the policy gradient (the rule is stated with
     tb_impala_loss_f32 in include/torchbeast_b200.h), and the call returns (ImpalaLoss, TrustRegion).  vs and
     pg_advantages are the masked ones; log_rhos and the log-probabilities are not masked.
+
+    With `upgo_cost` (a finite float >= 0, or a float32 device scalar read when the kernel runs) the upgoing policy
+    gradient (tb_upgo_loss_f32, a second launch; the rule is stated in include/torchbeast_b200.h) adds
+    upgo_cost * sum w_b * (-log pi(a)) * A_upgo to losses[3] and its gradient to grad_logits, and an Upgo(adv, loss)
+    is appended last to what the call returns.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
@@ -141,11 +164,12 @@ def impala_loss_fwd_bwd(
         if column_weights.dtype != torch.float32 or column_weights.numel() != target_policy_logits.shape[1]:
             raise _lib.TorchBeastB200Error("column_weights must be float32 [%d], got %s %r" % (
                 target_policy_logits.shape[1], column_weights.dtype, tuple(column_weights.shape)))
-    loss, _, trust = _impala_loss(
+    loss, _, trust, upgo = _impala_loss(
         behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value, discounting,
         baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, with_grads,
-        hparams_dev, column_weights=column_weights, trust_region=trust_region)
-    return loss if trust is None else (loss, trust)
+        hparams_dev, column_weights=column_weights, trust_region=trust_region, upgo_cost=upgo_cost)
+    out = (loss,) + tuple(x for x in (trust, upgo) if x is not None)
+    return out[0] if len(out) == 1 else out
 
 
 @torch.no_grad()
@@ -167,6 +191,7 @@ def impala_loss_popart(
     clip_pg_rho_threshold=1.0,
     hparams_dev=None,
     trust_region=None,
+    upgo_cost=None,
 ):
     """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_f32 with a task).
 
@@ -176,7 +201,8 @@ def impala_loss_popart(
     [T+1, B, K].  A row with a task id outside [0, K) adds no loss and gets zero gradient rows.  Returns
     (ImpalaLoss, task_sums): task_sums float64 [3, K] = per-task count, sum vs, sum vs^2 over rows t < T, the input
     of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd) it
-    returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs."""
+    returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs.  With `upgo_cost` (see
+    impala_loss_fwd_bwd; its advantage is divided by sigma_k) an Upgo is appended last."""
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
     _lib.require_cuda(*tensors)
     T, B, A = target_policy_logits.shape
@@ -186,19 +212,19 @@ def impala_loss_popart(
                                        % (T, B, tuple(values.shape), tuple(task.shape)))
     if mu.dtype != torch.float64 or nu.dtype != torch.float64 or mu.numel() != K or nu.numel() != K:
         raise _lib.TorchBeastB200Error("PopArt mu / nu must be float64 [%d]" % K)
-    loss, sums, trust = _impala_loss(
+    loss, sums, trust, upgo = _impala_loss(
         behavior_policy_logits, target_policy_logits, actions, rewards, done, values, None, discounting,
         baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, True, hparams_dev,
-        popart=(task, mu, nu), trust_region=trust_region)
-    return (loss, sums) if trust is None else (loss, sums, trust)
+        popart=(task, mu, nu), trust_region=trust_region, upgo_cost=upgo_cost)
+    return (loss, sums) + tuple(x for x in (trust, upgo) if x is not None)
 
 
 def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value,
                  discounting, baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold,
-                 with_grads, hparams_dev, column_weights=None, popart=None, trust_region=None):
-    """The one tb_impala_loss_f32 call behind impala_loss_fwd_bwd and impala_loss_popart, on inputs they checked.
-    popart: None, or (task, mu, nu) with values [T+1, B, K].  Returns (ImpalaLoss, task_sums or None, TrustRegion or
-    None)."""
+                 with_grads, hparams_dev, column_weights=None, popart=None, trust_region=None, upgo_cost=None):
+    """The tb_impala_loss_f32 call behind impala_loss_fwd_bwd and impala_loss_popart, on inputs they checked, and with
+    `upgo_cost` the tb_upgo_loss_f32 call right behind it on the same inputs.  popart: None, or (task, mu, nu) with
+    values [T+1, B, K].  Returns (ImpalaLoss, task_sums or None, TrustRegion or None, Upgo or None)."""
     if hparams_dev is None:
         clip_rewards = _clip_rewards(reward_clipping)
     else:
@@ -226,25 +252,37 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
         bs = bootstrap_value.detach().to(f32).contiguous()
     beta = kl = kl_sums = None
     if trust_region is not None:
-        beta = _trust_beta_tensor(trust_region, dev)
+        beta = _device_scalar(trust_region, "trust_region", dev)
         kl, kl_sums = torch.empty((T, B), dtype=f32, device=dev), torch.empty(2, dtype=f32, device=dev)
+    cost = None if upgo_cost is None else _device_scalar(upgo_cost, "upgo_cost", dev, finite=True)
     cw = None if column_weights is None else column_weights.contiguous()
     outs = [torch.empty((T, B), dtype=f32, device=dev) for _ in range(5)]
     losses = torch.empty(4, dtype=f32, device=dev)
     gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
     gv = torch.empty((T + 1, B) + ((K,) if popart is not None else ()), dtype=f32, device=dev) if with_grads else None
+    tl, act = target_policy_logits.detach().to(f32).contiguous(), actions.to(torch.int64).contiguous()
+    rw, vals = rewards.to(f32).contiguous(), values.detach().to(f32).contiguous()
+    disc_arg = 0.0 if hparams_dev is not None else float(discounting)
     p = _lib.ptr
+    ws = _lib.workspace()
     _lib.check(
         _lib.lib().tb_impala_loss_f32(
-            p(behavior_policy_logits.to(f32).contiguous()), p(target_policy_logits.detach().to(f32).contiguous()),
-            p(actions.to(torch.int64).contiguous()), p(rewards.to(f32).contiguous()), p(dn), p(disc),
-            p(values.detach().to(f32).contiguous()), p(bs), T, B, A,
-            0.0 if hparams_dev is not None else float(discounting), float(baseline_cost), float(entropy_cost),
+            p(behavior_policy_logits.to(f32).contiguous()), p(tl), p(act), p(rw), p(dn), p(disc), p(vals), p(bs),
+            T, B, A, disc_arg, float(baseline_cost), float(entropy_cost),
             clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev),
             p(cw), p(task), p(mu), p(nu), K, p(sums), p(beta), p(kl), p(kl_sums),
-            *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(_lib.workspace()), _lib.stream_ptr()),
+            *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(ws), _lib.stream_ptr()),
         "tb_impala_loss_f32")
-    return ImpalaLoss(*outs, losses, gl, gv), sums, None if beta is None else TrustRegion(kl, kl_sums)
+    upgo = None
+    if cost is not None:
+        upgo = Upgo(torch.empty((T, B), dtype=f32, device=dev), torch.empty(1, dtype=f32, device=dev))
+        _lib.check(
+            _lib.lib().tb_upgo_loss_f32(
+                p(tl), p(act), p(rw), p(dn), p(disc), p(vals), p(bs), T, B, A, disc_arg, clip_rewards,
+                _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev), p(cw), p(task), p(mu), p(nu), K, p(outs[2]),
+                p(beta), p(kl), p(cost), p(upgo.adv), p(upgo.loss), p(losses), p(gl), p(ws), _lib.stream_ptr()),
+            "tb_upgo_loss_f32")
+    return ImpalaLoss(*outs, losses, gl, gv), sums, None if beta is None else TrustRegion(kl, kl_sums), upgo
 
 
 @torch.no_grad()
@@ -378,7 +416,7 @@ def _check_replay(model):
 
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
                behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None,
-               fresh_columns=None, draw=None, trust_beta_dev=None):
+               fresh_columns=None, draw=None, trust_beta_dev=None, upgo_cost_dev=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -404,13 +442,19 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     is `trust_beta_dev` (a float32 device scalar, GraphedLearner's) or the flag.  The stats then carry
     trust_fraction (trusted rows / T*B) and mean_policy_kl (sum KL / T*B), read back with the loss values; a prioritised
     buffer's priorities come from the masked vs.
+
+    flags.upgo_cost (a finite float >= 0; None or absent: off) adds the upgoing policy gradient (tb_upgo_loss_f32, one
+    more launch right after the loss) on every path above.  The cost is `upgo_cost_dev` (a float32 device scalar,
+    GraphedLearner's) or the flag.  The stats then carry upgo_loss, which total_loss includes.
     """
     pop = getattr(model, "popart", None)
     if draw is not None and pop is not None:
         raise _lib.TorchBeastB200Error(_POPART_PRIORITIZED)
     beta = trust_region_kl(flags)
     trust_region = None if beta is None else (beta if trust_beta_dev is None else trust_beta_dev)
-    trust = None
+    cost = upgo_cost(flags)
+    upgo_arg = None if cost is None else (cost if upgo_cost_dev is None else upgo_cost_dev)
+    trust = upgo = None
     out = model.learner_forward(batch, initial_agent_state)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
     acts = batch["action"] if actions is None else actions
@@ -420,9 +464,11 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             out.baseline[:-1], out.baseline[-1],
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
-            column_weights=None if draw is None else draw.weights, trust_region=trust_region)
-        if trust_region is not None:
-            loss, trust = loss
+            column_weights=None if draw is None else draw.weights, trust_region=trust_region, upgo_cost=upgo_arg)
+        if trust_region is not None or upgo_arg is not None:
+            loss, *rest = loss
+            trust = rest.pop(0) if trust_region is not None else None
+            upgo = rest.pop(0) if upgo_arg is not None else None
         grad_values = loss.grad_values
         if draw is not None and draw.buffer is not None:
             draw.buffer.update_priorities(loss.vs, out.baseline[:-1], draw.slots)
@@ -432,10 +478,11 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:], values,
             _popart_task(model, batch), pop.mu, pop.nu,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
-            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region)
-        loss, task_sums = res[:2]
-        if trust_region is not None:
-            trust = res[2]
+            reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region,
+            upgo_cost=upgo_arg)
+        loss, task_sums, *rest = res
+        trust = rest.pop(0) if trust_region is not None else None
+        upgo = rest.pop(0) if upgo_arg is not None else None
         grad_values = loss.grad_values.view(out.baseline.shape)
     _backward_with_overlapped_all_reduce(model, loss.grad_logits, grad_values)
     optimizer_step(model, optimizer, flags.grad_norm_clipping, hparams_dev=hparams_dev)
@@ -455,13 +502,13 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         else:
             actor_model.load_state_dict(model.state_dict())
     if not stats_sync:
-        return dict(losses=loss.losses, vtrace=loss, trust=trust)
+        return dict(losses=loss.losses, vtrace=loss, trust=trust, upgo=upgo)
     done, ep_ret = batch["done"][1:], batch["episode_return"][1:]
     if fresh_columns is not None:
         done, ep_ret = done[:, :fresh_columns], ep_ret[:, :fresh_columns]
     episode_returns = ep_ret[done.bool()]
-    # the step's one blocking read-back: the loss values, and the trust-region sums behind them
-    host = (loss.losses if trust is None else torch.cat([loss.losses, trust.sums])).cpu()
+    # the step's one blocking read-back: the loss values, and the trust-region sums and UPGO loss behind them
+    host = _loss_values(loss.losses, trust, upgo).cpu()
     ep = episode_returns.cpu()
     stats = {
         "episode_returns": tuple(ep.numpy()),
@@ -471,10 +518,26 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         "baseline_loss": host[1].item(),
         "entropy_loss": host[2].item(),
     }
-    if trust is not None:
-        stats.update(_trust_stats(host[4:6], trust.kl.numel()))
+    stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), upgo is not None))
     if pop is not None:
         stats.update(_popart_stats(pop.mu.cpu(), pop.nu.cpu()))
+    return stats
+
+
+def _loss_values(losses, trust, upgo):
+    """The device values the stats read back at once: losses [4], then the trust-region sums [2] and the UPGO loss [1]
+    when they are on."""
+    parts = [losses] + ([] if trust is None else [trust.sums]) + ([] if upgo is None else [upgo.loss])
+    return parts[0] if len(parts) == 1 else torch.cat(parts)
+
+
+def _extra_stats(host, trust_rows, has_upgo):
+    """The trust-region and UPGO stats entries from a host copy of _loss_values; trust_rows None: no trust region."""
+    stats = {}
+    if has_upgo:
+        stats["upgo_loss"] = host[-1].item()
+    if trust_rows is not None:
+        stats.update(_trust_stats(host[4:6], trust_rows))
     return stats
 
 
@@ -631,9 +694,12 @@ class GraphedLearner:
     def structure_of(optimizer, batch, flags=None):
         """What the captured launch sequence depends on besides shapes: the optimizer's kernel and buffer choices
         (RMSprop centered / weight_decay != 0 / momentum != 0, Adam vs AdamW), the dtype of `done`, and whether
-        `flags` turn the trust region on (its beta is published per replay; on / off chooses the loss kernel)."""
+        `flags` turn the trust region and UPGO on (beta and the UPGO cost are published per replay; on / off chooses the
+        loss kernel, and UPGO adds a launch)."""
         trust = flags is not None and trust_region_kl(flags) is not None
-        return optimizer.structure() + (batch["done"].dtype,) + (("trust_region",) if trust else ())
+        upgo = flags is not None and upgo_cost(flags) is not None
+        return (optimizer.structure() + (batch["done"].dtype,) + (("trust_region",) if trust else ())
+                + (("upgo",) if upgo else ()))
 
     def __init__(self, flags, model, actor_model, optimizer, example_batch, initial_agent_state=()):
         _require_fused(optimizer)
@@ -646,6 +712,11 @@ class GraphedLearner:
         if trust_region_kl(flags) is not None:
             self.trust_beta = torch.zeros(1, dtype=torch.float32, device=model.flat_params.device)
             self._publish_trust_beta(flags)
+        # UPGO: its cost is a float32 device scalar published before every replay, like the trust region's beta
+        self.upgo_cost = None
+        if upgo_cost(flags) is not None:
+            self.upgo_cost = torch.zeros(1, dtype=torch.float32, device=model.flat_params.device)
+            self._publish_upgo_cost(flags)
         # PopArt: beta is a device scalar published before every replay, like the tb_hparams block
         self.popart = getattr(model, "popart", None)
         self.popart_beta = None
@@ -711,7 +782,7 @@ class GraphedLearner:
             draw = self.replay.last_draw if self.replay.prioritized else None
         return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
                           hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw,
-                          trust_beta_dev=self.trust_beta)
+                          trust_beta_dev=self.trust_beta, upgo_cost_dev=self.upgo_cost)
 
     def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
         """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
@@ -726,6 +797,8 @@ class GraphedLearner:
             self._publish_beta(self.flags)
         if self.trust_beta is not None:
             self._publish_trust_beta(self.flags)
+        if self.upgo_cost is not None:
+            self._publish_upgo_cost(self.flags)
         if self.replay is not None:
             self.replay.prepare(self.static, self.static_state)  # publishes seed / step if the host changed them
         self.graph.replay()
@@ -748,19 +821,26 @@ class GraphedLearner:
         host = torch.full((1,), beta, dtype=torch.float32).pin_memory()
         self.trust_beta.copy_(host, non_blocking=True)
 
+    def _publish_upgo_cost(self, flags):
+        """Enqueue the copy of flags.upgo_cost (validated; float32) into the device scalar, as _publish_trust_beta."""
+        cost = upgo_cost(flags)
+        if cost is None:
+            raise ValueError("this graph was captured with UPGO; upgo_cost is now None")
+        host = torch.full((1,), cost, dtype=torch.float32).pin_memory()
+        self.upgo_cost.copy_(host, non_blocking=True)
+
     def _losses_out(self):
-        """The step's loss values, and with a trust region its two sums behind them: float32 [4] or [6]."""
-        trust = self.out["trust"]
-        return self.out["losses"] if trust is None else torch.cat([self.out["losses"], trust.sums])
+        """The step's loss values, then the trust-region sums and the UPGO loss when on: float32 [4] to [7]."""
+        return _loss_values(self.out["losses"], self.out["trust"], self.out["upgo"])
 
     def snapshot(self):
         """Device copies of what stats() reads (the step's losses and its done / episode_return rows, a PopArt model's
-        statistics, the trust-region sums and row count), enqueued on the current stream: lets the caller release the
-        learner lock BEFORE the blocking read-back, so the next learner thread's replay queues up behind this one
-        instead of waiting for a host round trip."""
+        statistics, the trust-region sums and row count, the UPGO loss), enqueued on the current stream: lets the caller
+        release the learner lock BEFORE the blocking read-back, so the next learner thread's replay queues up behind
+        this one instead of waiting for a host round trip."""
         trust = self.out["trust"]
         snap = (self._losses_out(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone(),
-                None if trust is None else trust.kl.numel())
+                None if trust is None else trust.kl.numel(), self.out["upgo"] is not None)
         if self.popart is not None:
             snap += (self.popart.mu.clone(), self.popart.nu.clone())
         return snap
@@ -772,7 +852,7 @@ class GraphedLearner:
         """Read the snapshot back on a per-thread READ-BACK stream that waits only for `event` (recorded right after the
         snapshot): a read-back on the compute stream would queue behind the NEXT step, which another learner thread has
         already enqueued there."""
-        losses, done, ep_ret, trust_rows = snap[:4]
+        losses, done, ep_ret, trust_rows, has_upgo = snap[:5]
         tls = GraphedLearner._tls
         dev = losses.device
         if getattr(tls, "stream", None) is None or tls.device != dev:
@@ -787,7 +867,7 @@ class GraphedLearner:
         with torch.cuda.stream(tls.stream):
             for dst, src in zip(bufs, (losses, done, ep_ret)):
                 dst.copy_(src, non_blocking=True)
-            popart = [s.to("cpu", non_blocking=True) for s in snap[4:]]
+            popart = [s.to("cpu", non_blocking=True) for s in snap[5:]]
         tls.stream.synchronize()
         host, hdone, hret = bufs
         ep = hret[hdone.bool()].clone()
@@ -796,8 +876,7 @@ class GraphedLearner:
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
-        if trust_rows is not None:
-            stats.update(_trust_stats(host[4:6], trust_rows))
+        stats.update(_extra_stats(host, trust_rows, has_upgo))
         if popart:
             stats.update(_popart_stats(*popart))
         return stats
@@ -812,8 +891,8 @@ class GraphedLearner:
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
-        if self.out["trust"] is not None:
-            stats.update(_trust_stats(host[4:6], self.out["trust"].kl.numel()))
+        trust = self.out["trust"]
+        stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), self.out["upgo"] is not None))
         if self.popart is not None:
             stats.update(_popart_stats(self.popart.mu.cpu(), self.popart.nu.cpu()))
         return stats
