@@ -193,6 +193,25 @@ int tb_upgo_loss_f32(const float* target_logits, const int64_t* actions, const f
                      float* upgo_adv, float* upgo_out, float* losses_out, float* grad_logits, void* workspace,
                      void* stream);
 
+/* Kickstarting (Schmitt et al. 2018, "Kickstarting Deep Reinforcement Learning", arXiv:1803.03835): distils a frozen
+ * teacher policy into the learner.  A launch enqueued after tb_impala_loss_f32 (and tb_upgo_loss_f32) on the same
+ * stream, before the network backward.  teacher_logits and target_logits are [T,B,A]: the [:-1] prefixes of the
+ * teacher's and the learner's [T+1,B,A] forward outputs.  In the loss block's row notation (rows t = 0..T-1 of column b):
+ *   log p_T, log p_S  the row log-softmaxes of the two, by the max / log-sum-exp code the loss uses;
+ *   KL_t = sum_a p_T(a) (log p_T(a) - log p_S(a)) in fp32; a term with p_T(a) == 0 adds exactly 0, so a teacher that
+ *     masks actions with -inf logits gives no NaN.  Identical rows give KL_t = 0 and a gradient of +-0.
+ *   Loss: kickstart_cost * sum_{t,b} w_b KL_t; w_b = column_weights[b], or 1.  Gradient: kickstart_cost * w_b *
+ *     (p_S - p_T), ADDED into grad_logits rows t < T (NULL: forward only); row T, the values and the teacher get
+ *     nothing.  The trust region's mask and PopArt do not apply.
+ * kickstart_cost f32 [1] (device, read when the kernel runs).  outputs: kickstart_out [2] f32 = {the loss, sum_{t,b}
+ * KL_t unweighted}, always written; losses_out[3] (the loss launch's total) becomes float(double(total) +
+ * double(kickstart_out[0])).  When *kickstart_cost == 0 grad_logits and losses_out are not written, so a zero cost
+ * leaves the loss launch's bits.  The sums are fp64 in a fixed order (no atomics): bit-identical from run to run.
+ * workspace: the one the loss launch used (or any other).  Requires T, B, A >= 1.  One launch.                    */
+int tb_kickstart_loss_f32(const float* teacher_logits, const float* target_logits, int64_t T, int64_t B, int64_t A,
+                          const float* column_weights, const float* kickstart_cost, float* kickstart_out,
+                          float* losses_out, float* grad_logits, void* workspace, void* stream);
+
 /* tb_popart_update:for each task k with task_sums count > 0 (data-parallel callers SUM all-reduce task_sums
  *   first), with beta read from device memory and sigma_k as in tb_impala_loss_f32:
  *     mu'_k = (1 - beta) mu_k + beta * sum vs / count,   nu'_k = (1 - beta) nu_k + beta * sum vs^2 / count

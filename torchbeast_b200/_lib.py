@@ -32,6 +32,7 @@ _SIGNATURES = {
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 5 + [_i64] + [_vp] * 12
         + [_int, _vp, _vp], _int),
     "tb_upgo_loss_f32": ([_vp] * 7 + [_i64, _i64, _i64, _f32, _int, _f32] + [_vp] * 5 + [_i64] + [_vp] * 10, _int),
+    "tb_kickstart_loss_f32": ([_vp, _vp, _i64, _i64, _i64] + [_vp] * 7, _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
     "tb_atarinet_param_count": ([_int, _int, _int], _i64),
     "tb_atarinet_workspace_bytes": ([_i64, _i64, _int, _int, _int], _c.c_size_t),

@@ -861,6 +861,78 @@ __global__ void __maxnreg__(128) upgo_loss_kernel(UpgoArgs p) {
 }
 
 // ----------------------------------------------------------------------------------------
+// Kickstarting: KL(teacher || learner) per row (tb_kickstart_loss_f32), a launch after the loss (and UPGO)
+// ----------------------------------------------------------------------------------------
+struct KickstartArgs {
+  const float* teacher; const float* target;  // [T,B,A] each
+  int64_t T, B, A;
+  const float* column_weights;                // [B] or NULL (kickstart_loss_kernel<A, true> only)
+  const float* cost;                          // f32 [1], read when the kernel runs; 0: grad and losses not written
+  float* out;                                 // [2] out: {cost * sum w_b KL_t, sum KL_t}
+  float* losses;                              // [4]: losses[3] += out[0]
+  float* grad;                                // [T(+1),B,A] or NULL: rows t < T += cost w_b (p_S - p_T)
+  void* workspace;
+};
+
+// KL_t = sum_a p_T(a) (log p_T(a) - log p_S(a)) of one row in fp32, with both log-softmaxes from the max / log-sum-exp
+// the loss uses; a term with p_T(a) == 0 adds exactly 0 (a -inf teacher logit), a NaN one propagates.  With `grow` the
+// gradient scale * (p_S - p_T) is added into it.
+template <int A>
+__device__ __forceinline__ float kickstart_row(const float* __restrict__ trow, const float* __restrict__ srow,
+                                               int64_t Ause, float* __restrict__ grow, float scale) {
+  float kl = 0.0f;
+  if constexpr (A == 0) {
+    float mt, logst, ms, logss;
+    alp_dyn<float>(trow, Ause, 0, &mt, &logst);
+    alp_dyn<float>(srow, Ause, 0, &ms, &logss);
+    for (int64_t j = 0; j < Ause; ++j) {
+      const float lt = (trow[j] - mt) - logst, ls = (srow[j] - ms) - logss, pt = expf(lt);
+      kl += pt == 0.0f ? 0.0f : pt * (lt - ls);
+      if (grow) grow[j] += scale * (expf(ls) - pt);
+    }
+  } else {
+    float xt[A], xs[A], mt, logst, ms, logss;
+    RowOps<float, A>::load(trow, Ause, xt);
+    RowOps<float, A>::load(srow, Ause, xs);
+    RowOps<float, A>::lse(xt, mt, logst);
+    RowOps<float, A>::lse(xs, ms, logss);
+#pragma unroll
+    for (int j = 0; j < A; ++j) {
+      const float lt = (xt[j] - mt) - logst, ls = (xs[j] - ms) - logss, pt = expf(lt);
+      kl += pt == 0.0f ? 0.0f : pt * (lt - ls);
+      if (grow) grow[j] += scale * (expf(ls) - pt);
+    }
+  }
+  return kl;
+}
+
+// Rows are independent: a grid-stride loop over the T*B rows, then one grid_sum3 of {sum w_b KL_t, sum KL_t}.
+// kWeighted: row (t, b)'s loss and gradient are multiplied by column_weights[b]; the other instantiations compile none.
+template <int A, bool kWeighted>
+__global__ void __launch_bounds__(256) kickstart_loss_kernel(KickstartArgs p) {
+  const float cost = *p.cost;
+  const int64_t Ause = A ? A : p.A;
+  const int64_t N = p.T * p.B;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  double s_w = 0.0, s_kl = 0.0;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < N; i += stride) {
+    float scale = cost;
+    if constexpr (kWeighted) scale *= __ldg(p.column_weights + i % p.B);
+    float* grow = (p.grad && cost != 0.0f) ? p.grad + i * Ause : nullptr;
+    const float kl = kickstart_row<A>(p.teacher + i * Ause, p.target + i * Ause, Ause, grow, scale);
+    s_kl += double(kl);
+    if constexpr (kWeighted) s_w += double(kl) * double(__ldg(p.column_weights + i % p.B)); else s_w += double(kl);
+  }
+  double tot[3];
+  if (grid_sum3(s_w, s_kl, 0.0, p.workspace, tot)) {
+    const float ks = float(double(cost) * tot[0]);
+    p.out[0] = ks;
+    p.out[1] = float(tot[1]);
+    if (cost != 0.0f) p.losses[3] = float(double(p.losses[3]) + double(ks));
+  }
+}
+
+// ----------------------------------------------------------------------------------------
 // PopArt statistics
 // ----------------------------------------------------------------------------------------
 // sums[k] = count, sums[K+k] = sum vs, sums[2K+k] = sum vs^2 over the rows t < T of task k.  CTA k owns task k and
@@ -1182,6 +1254,34 @@ int tb_upgo_loss_f32(const float* tlogits, const int64_t* actions, const float* 
   ProfScope prof("upgo_loss", s);
   TB_DISPATCH_A(A, (upgo_loss_kernel<kA><<<grid, block, smem, s>>>(p)));
   return check_launch("upgo_loss_kernel");
+}
+
+// The kernel instantiation follows from whether column_weights is non-NULL.
+int tb_kickstart_loss_f32(const float* teacher_logits, const float* target_logits, int64_t T, int64_t B, int64_t A,
+                          const float* column_weights, const float* kickstart_cost, float* kickstart_out,
+                          float* losses_out, float* grad_logits, void* workspace, void* stream) {
+  TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "kickstart_loss: bad sizes T=%lld B=%lld A=%lld", (long long)T,
+             (long long)B, (long long)A);
+  TB_REQUIRE(teacher_logits && target_logits, "kickstart_loss: null input pointer");
+  TB_REQUIRE(kickstart_cost && kickstart_out && losses_out && workspace,
+             "kickstart_loss: kickstart_cost/kickstart_out/losses_out/workspace must not be null");
+  KickstartArgs p;
+  p.teacher = teacher_logits; p.target = target_logits; p.T = T; p.B = B; p.A = A;
+  p.column_weights = column_weights; p.cost = kickstart_cost; p.out = kickstart_out; p.losses = losses_out;
+  p.grad = grad_logits; p.workspace = workspace;
+  const int threads = 256;
+  int64_t blocks = (T * B + threads - 1) / threads;
+  const int64_t cap = int64_t(sm_count()) * 8 < kMaxPartialCtas ? int64_t(sm_count()) * 8 : kMaxPartialCtas;
+  if (blocks > cap) blocks = cap;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (column_weights) {
+    ProfScope prof("kickstart_loss_weighted", s);
+    TB_DISPATCH_A(A, (kickstart_loss_kernel<kA, true><<<unsigned(blocks), threads, 0, s>>>(p)));
+    return check_launch("kickstart_loss_kernel<weighted>");
+  }
+  ProfScope prof("kickstart_loss", s);
+  TB_DISPATCH_A(A, (kickstart_loss_kernel<kA, false><<<unsigned(blocks), threads, 0, s>>>(p)));
+  return check_launch("kickstart_loss_kernel");
 }
 
 int tb_popart_update(const double* task_sums, const double* beta, double* mu, double* nu, int64_t K, float* weight,

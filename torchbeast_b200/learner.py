@@ -8,6 +8,7 @@ import numpy as np
 import torch
 
 from torchbeast_b200 import _lib
+from torchbeast_b200.kickstart import kickstart_cost, teacher_of
 
 ImpalaLoss = collections.namedtuple(
     "ImpalaLoss",
@@ -19,6 +20,9 @@ TrustRegion = collections.namedtuple("TrustRegion", "kl sums")
 # What the loss returns last when given upgo_cost: adv float32 [T, B] = the UPGO advantage of every row, loss float32
 # [1] = upgo_cost * sum w_b * (-log pi(a)) * adv (already included in losses[3]).
 Upgo = collections.namedtuple("Upgo", "adv loss")
+# What kickstart_loss returns: loss float32 [1] = cost * sum w_b * KL_t (already included in losses[3]), kl_sum float32
+# [1] = sum KL_t over all T*B rows, unweighted.
+Kickstart = collections.namedtuple("Kickstart", "loss kl_sum")
 
 # tb_hparams (include/torchbeast_b200.h): the loss and optimizer values the entry points read from device memory.
 # tb_hparams_layout() reports the compiled layout; tests/test_graph_hparams_cpu.py checks this record against it.
@@ -286,6 +290,47 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
 
 
 @torch.no_grad()
+def kickstart_loss(teacher_logits, target_logits, losses, grad_logits, cost, column_weights=None):
+    """The kickstarting term (tb_kickstart_loss_f32, one launch; the rule is stated in include/torchbeast_b200.h):
+    cost * sum_{t,b} w_b KL(p_teacher,t || p_learner,t) over the [T, B, A] logits (the [:-1] rows of the two forward
+    outputs), ADDED into `losses[3]` (float32 [4], the loss's) and, unless `grad_logits` is None, its gradient
+    cost * w_b * (p_learner - p_teacher) ADDED into rows t < T of `grad_logits` (float32 [T or T+1, B, A]).  A zero
+    cost writes neither.  `cost`: a finite float >= 0, or a float32 device scalar read when the kernel runs.
+    `column_weights`: float32 [B] (w_b), or None for 1.  Returns Kickstart(loss, kl_sum)."""
+    _lib.require_cuda(teacher_logits, target_logits, losses)
+    T, B, A = target_logits.shape
+    f32 = torch.float32
+    if tuple(teacher_logits.shape) != (T, B, A):
+        raise _lib.TorchBeastB200Error("teacher logits %r do not match the learner's %r"
+                                       % (tuple(teacher_logits.shape), (T, B, A)))
+    if losses.dtype != f32 or losses.numel() != 4 or not losses.is_contiguous():
+        raise _lib.TorchBeastB200Error("losses must be contiguous float32 [4], got %s %r"
+                                       % (losses.dtype, tuple(losses.shape)))
+    if grad_logits is not None:
+        _lib.require_cuda(grad_logits)
+        if grad_logits.dtype != f32 or not grad_logits.is_contiguous() or tuple(grad_logits.shape) not in (
+                (T, B, A), (T + 1, B, A)):
+            raise _lib.TorchBeastB200Error("grad_logits must be contiguous float32 [T(+1), B, A] for %r, got %s %r"
+                                           % ((T, B, A), grad_logits.dtype, tuple(grad_logits.shape)))
+    if column_weights is not None:
+        _lib.require_cuda(column_weights)
+        if column_weights.dtype != f32 or column_weights.numel() != B:
+            raise _lib.TorchBeastB200Error("column_weights must be float32 [%d], got %s %r" % (
+                B, column_weights.dtype, tuple(column_weights.shape)))
+        column_weights = column_weights.contiguous()
+    dev = target_logits.device
+    c = _device_scalar(cost, "kickstart_cost", dev, finite=True)
+    out = torch.empty(2, dtype=f32, device=dev)
+    p = _lib.ptr
+    _lib.check(
+        _lib.lib().tb_kickstart_loss_f32(
+            p(teacher_logits.detach().to(f32).contiguous()), p(target_logits.detach().to(f32).contiguous()), T, B, A,
+            p(column_weights), p(c), p(out), p(losses), p(grad_logits), p(_lib.workspace()), _lib.stream_ptr()),
+        "tb_kickstart_loss_f32")
+    return Kickstart(out[:1], out[1:])
+
+
+@torch.no_grad()
 def popart_update(task_sums, beta, mu, nu, weight, bias):
     """PopArt statistics update and output-preserving value-head rescale, in place (tb_popart_update): `beta` is a
     float64 device scalar, `weight` [K, F] / `bias` [K] the value head (views of the flat parameter buffer)."""
@@ -416,7 +461,7 @@ def _check_replay(model):
 
 def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer, scheduler,
                behavior_logits=None, actions=None, stats_sync=True, hparams_dev=None, popart_beta_dev=None,
-               fresh_columns=None, draw=None, trust_beta_dev=None, upgo_cost_dev=None):
+               fresh_columns=None, draw=None, trust_beta_dev=None, upgo_cost_dev=None, kickstart_cost_dev=None):
     """One optimisation step on a [T+1, B, ...] rollout batch (dict of CUDA tensors).
 
     Launch sequence (no autograd graph, no host sync until the stats read-back):
@@ -446,6 +491,12 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     flags.upgo_cost (a finite float >= 0; None or absent: off) adds the upgoing policy gradient (tb_upgo_loss_f32, one
     more launch right after the loss) on every path above.  The cost is `upgo_cost_dev` (a float32 device scalar,
     GraphedLearner's) or the flag.  The stats then carry upgo_loss, which total_loss includes.
+
+    flags.kickstart_cost (a finite float >= 0; None or absent: off) distils the teacher attached as model.teacher (a
+    torchbeast_b200.kickstart.Teacher) into the learner on every path above: the teacher's forward runs on the same
+    batch right after the learner's, and kickstart_loss (one launch after the loss and UPGO) adds its term to the total
+    and to grad_logits.  The cost is `kickstart_cost_dev` (a float32 device scalar, GraphedLearner's) or the flag.  The
+    stats then carry kickstart_loss, which total_loss includes, and teacher_kl (sum KL / T*B, unweighted).
     """
     pop = getattr(model, "popart", None)
     if draw is not None and pop is not None:
@@ -454,8 +505,12 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     trust_region = None if beta is None else (beta if trust_beta_dev is None else trust_beta_dev)
     cost = upgo_cost(flags)
     upgo_arg = None if cost is None else (cost if upgo_cost_dev is None else upgo_cost_dev)
-    trust = upgo = None
+    ks_cost = kickstart_cost(flags)
+    teacher = _teacher_for(model, actor_model, ks_cost)
+    ks_arg = None if ks_cost is None else (ks_cost if kickstart_cost_dev is None else kickstart_cost_dev)
+    trust = upgo = ks = None
     out = model.learner_forward(batch, initial_agent_state)
+    teacher_logits = None if teacher is None else teacher.logits(batch)
     blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
     acts = batch["action"] if actions is None else actions
     if pop is None:
@@ -484,6 +539,9 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         trust = rest.pop(0) if trust_region is not None else None
         upgo = rest.pop(0) if upgo_arg is not None else None
         grad_values = loss.grad_values.view(out.baseline.shape)
+    if teacher is not None:
+        ks = kickstart_loss(teacher_logits[:-1], out.policy_logits[:-1], loss.losses, loss.grad_logits, ks_arg,
+                            column_weights=None if draw is None else draw.weights)
     _backward_with_overlapped_all_reduce(model, loss.grad_logits, grad_values)
     optimizer_step(model, optimizer, flags.grad_norm_clipping, hparams_dev=hparams_dev)
     if pop is not None:
@@ -502,13 +560,14 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         else:
             actor_model.load_state_dict(model.state_dict())
     if not stats_sync:
-        return dict(losses=loss.losses, vtrace=loss, trust=trust, upgo=upgo)
+        return dict(losses=loss.losses, vtrace=loss, trust=trust, upgo=upgo, kickstart=ks)
     done, ep_ret = batch["done"][1:], batch["episode_return"][1:]
     if fresh_columns is not None:
         done, ep_ret = done[:, :fresh_columns], ep_ret[:, :fresh_columns]
     episode_returns = ep_ret[done.bool()]
-    # the step's one blocking read-back: the loss values, and the trust-region sums and UPGO loss behind them
-    host = _loss_values(loss.losses, trust, upgo).cpu()
+    # the step's one blocking read-back: the loss values, and the trust-region sums, UPGO and kickstarting values behind
+    # them
+    host = _loss_values(loss.losses, trust, upgo, ks).cpu()
     ep = episode_returns.cpu()
     stats = {
         "episode_returns": tuple(ep.numpy()),
@@ -518,24 +577,51 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
         "baseline_loss": host[1].item(),
         "entropy_loss": host[2].item(),
     }
-    stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), upgo is not None))
+    stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), upgo is not None,
+                              _kickstart_rows(ks, loss)))
     if pop is not None:
         stats.update(_popart_stats(pop.mu.cpu(), pop.nu.cpu()))
     return stats
 
 
-def _loss_values(losses, trust, upgo):
-    """The device values the stats read back at once: losses [4], then the trust-region sums [2] and the UPGO loss [1]
-    when they are on."""
-    parts = [losses] + ([] if trust is None else [trust.sums]) + ([] if upgo is None else [upgo.loss])
+def _teacher_for(model, actor_model, cost):
+    """The Teacher the step runs (model.teacher, checked against the learner), or None when kickstarting is off
+    (`cost` None).  Raises before anything is launched: for a bare nn.Module as model.teacher whatever the cost, and
+    for a cost without a teacher or a teacher that cannot run beside the learner (kickstart.Teacher.check)."""
+    teacher = teacher_of(model)
+    if cost is None:
+        return None
+    if teacher is None:
+        raise _lib.TorchBeastB200Error("flags.kickstart_cost is set but the learner has no teacher: attach one as "
+                                       "model.teacher = torchbeast_b200.kickstart.Teacher(net), or set the cost to None")
+    teacher.check(model, actor_model)
+    return teacher
+
+
+def _kickstart_rows(ks, loss):
+    """T*B, the rows teacher_kl averages over, or None without kickstarting."""
+    return None if ks is None else loss.vs.numel()
+
+
+def _loss_values(losses, trust, upgo, ks=None):
+    """The device values the stats read back at once: losses [4], then the trust-region sums [2], the UPGO loss [1]
+    and the kickstarting loss and KL sum [2] when they are on."""
+    parts = [losses] + ([] if trust is None else [trust.sums]) + ([] if upgo is None else [upgo.loss]) + (
+        [] if ks is None else [ks.loss, ks.kl_sum])
     return parts[0] if len(parts) == 1 else torch.cat(parts)
 
 
-def _extra_stats(host, trust_rows, has_upgo):
-    """The trust-region and UPGO stats entries from a host copy of _loss_values; trust_rows None: no trust region."""
+def _extra_stats(host, trust_rows, has_upgo, kickstart_rows=None):
+    """The trust-region, UPGO and kickstarting stats entries from a host copy of _loss_values; trust_rows None: no
+    trust region; kickstart_rows (T*B) None: no kickstarting."""
     stats = {}
+    i = 4 if trust_rows is None else 6
     if has_upgo:
-        stats["upgo_loss"] = host[-1].item()
+        stats["upgo_loss"] = host[i].item()
+        i += 1
+    if kickstart_rows is not None:
+        stats["kickstart_loss"] = host[i].item()
+        stats["teacher_kl"] = host[i + 1].item() / kickstart_rows
     if trust_rows is not None:
         stats.update(_trust_stats(host[4:6], trust_rows))
     return stats
@@ -574,9 +660,15 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       are mixed with replayed columns under the lock, inside the graph when graphed; the warm-up phase and the mixing
       phase are two graphs, as their batch widths differ.  A prioritised buffer adds its draw, the weighted loss and
       the priority update to the same sequence (learn_step's `draw`); with PopArt it raises.
+    * with flags.kickstart_cost, the teacher attached as model.teacher (torchbeast_b200.kickstart.Teacher) runs on the
+      same (mixed) batch and its KL term joins the loss (learn_step); the teacher is part of the graph's structure.
     Returns the reference's stats dict."""
     import contextlib
     from torchbeast_b200 import staging
+    # raises before anything is staged or launched: an invalid cost, a cost without a usable teacher, a bare net
+    teacher = _teacher_for(model, actor_model, kickstart_cost(flags))
+    needs_last_action = getattr(model, "needs_last_action", False) or (
+        teacher is not None and getattr(teacher.net, "needs_last_action", False))
     slot = None
     stager = None
     if _is_host(batch):
@@ -595,7 +687,7 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
                 if slot in stager._submitted:
                     stager._submitted.remove(slot)
             batch = stager.dev[slot]
-        if "last_action" not in batch and getattr(model, "needs_last_action", False):
+        if "last_action" not in batch and needs_last_action:
             # the polybeast nest has no separate last_action leaf: row t of `action` IS the action taken before frame t
             batch = dict(batch, last_action=batch["action"])
         try:
@@ -603,7 +695,7 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
             if _graph_enabled(flags):
                 _require_fused(optimizer)
                 hparams = pack_hparams(flags, optimizer)  # raises before anything is captured or replayed
-                structure = GraphedLearner.structure_of(optimizer, batch, flags)
+                structure = GraphedLearner.structure_of(optimizer, batch, flags, model)
                 graphs = model.__dict__.setdefault("_tb_graphs", {})
                 gkey = (tuple((k, tuple(v.shape)) for k, v in batch.items() if k in GraphedLearner.KEYS), id(optimizer),
                         id(actor_model))
@@ -691,20 +783,25 @@ class GraphedLearner:
     KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return", "task")
 
     @staticmethod
-    def structure_of(optimizer, batch, flags=None):
+    def structure_of(optimizer, batch, flags=None, model=None):
         """What the captured launch sequence depends on besides shapes: the optimizer's kernel and buffer choices
         (RMSprop centered / weight_decay != 0 / momentum != 0, Adam vs AdamW), the dtype of `done`, and whether
-        `flags` turn the trust region and UPGO on (beta and the UPGO cost are published per replay; on / off chooses the
-        loss kernel, and UPGO adds a launch)."""
+        `flags` turn the trust region, UPGO and kickstarting on (beta and the two costs are published per replay; on /
+        off chooses the loss kernel, and UPGO and kickstarting add launches).  With kickstarting, the identity of
+        `model`'s teacher net is part of it too: another teacher replays another graph."""
         trust = flags is not None and trust_region_kl(flags) is not None
         upgo = flags is not None and upgo_cost(flags) is not None
+        ks = ()
+        if flags is not None and kickstart_cost(flags) is not None:
+            teacher = None if model is None else teacher_of(model)
+            ks = ("kickstart", None if teacher is None else id(teacher.net))
         return (optimizer.structure() + (batch["done"].dtype,) + (("trust_region",) if trust else ())
-                + (("upgo",) if upgo else ()))
+                + (("upgo",) if upgo else ()) + ks)
 
     def __init__(self, flags, model, actor_model, optimizer, example_batch, initial_agent_state=()):
         _require_fused(optimizer)
         self.flags, self.model, self.actor, self.opt = flags, model, actor_model, optimizer
-        self.structure = self.structure_of(optimizer, example_batch, flags)
+        self.structure = self.structure_of(optimizer, example_batch, flags, model)
         self.hparams = torch.zeros(HPARAMS.itemsize, dtype=torch.uint8, device=model.flat_params.device)
         publish_hparams(pack_hparams(flags, optimizer), self.hparams)
         # trust region: beta is a float32 device scalar published before every replay, like PopArt's beta
@@ -717,6 +814,13 @@ class GraphedLearner:
         if upgo_cost(flags) is not None:
             self.upgo_cost = torch.zeros(1, dtype=torch.float32, device=model.flat_params.device)
             self._publish_upgo_cost(flags)
+        # kickstarting: the cost is a device scalar published before every replay; the teacher is held so that its net
+        # (whose identity keys this graph) and its zero states stay alive
+        self.teacher = _teacher_for(model, actor_model, kickstart_cost(flags))
+        self.kickstart_cost = None
+        if self.teacher is not None:
+            self.kickstart_cost = torch.zeros(1, dtype=torch.float32, device=model.flat_params.device)
+            self._publish_kickstart_cost(flags)
         # PopArt: beta is a device scalar published before every replay, like the tb_hparams block
         self.popart = getattr(model, "popart", None)
         self.popart_beta = None
@@ -760,6 +864,11 @@ class GraphedLearner:
         # the same holds for the stacked scratch an unstacked rollout is restacked into (AtariNet fp32, ResNet fp32 / bf16):
         # the graph writes it, its forward reads it, and the ResNet backward reads it again
         self.scratch = getattr(model, "_scratch_buf", None)
+        # and for the teacher's workspace and restack scratch, which its forward in the graph writes
+        self.teacher_workspace = self.teacher_scratch = None
+        if self.teacher is not None:
+            self.teacher_workspace = getattr(self.teacher.net, "_ws", None)
+            self.teacher_scratch = getattr(self.teacher.net, "_scratch_buf", None)
         self.graph.replay()  # first replay uploads the graph to the device; keep that out of the training loop
         torch.cuda.synchronize()
         # undo the warm-up / capture-time updates so training starts from the caller's weights
@@ -782,7 +891,8 @@ class GraphedLearner:
             draw = self.replay.last_draw if self.replay.prioritized else None
         return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
                           hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw,
-                          trust_beta_dev=self.trust_beta, upgo_cost_dev=self.upgo_cost)
+                          trust_beta_dev=self.trust_beta, upgo_cost_dev=self.upgo_cost,
+                          kickstart_cost_dev=self.kickstart_cost)
 
     def step(self, batch, initial_agent_state=(), scheduler=None, hparams=None):
         """One replay on `batch`.  `hparams`: the record of pack_hparams() to publish (default: packed from the
@@ -799,6 +909,8 @@ class GraphedLearner:
             self._publish_trust_beta(self.flags)
         if self.upgo_cost is not None:
             self._publish_upgo_cost(self.flags)
+        if self.kickstart_cost is not None:
+            self._publish_kickstart_cost(self.flags)
         if self.replay is not None:
             self.replay.prepare(self.static, self.static_state)  # publishes seed / step if the host changed them
         self.graph.replay()
@@ -829,18 +941,30 @@ class GraphedLearner:
         host = torch.full((1,), cost, dtype=torch.float32).pin_memory()
         self.upgo_cost.copy_(host, non_blocking=True)
 
+    def _publish_kickstart_cost(self, flags):
+        """Enqueue the copy of flags.kickstart_cost (validated; float32) into the device scalar, as _publish_upgo_cost."""
+        cost = kickstart_cost(flags)
+        if cost is None:
+            raise ValueError("this graph was captured with kickstarting; kickstart_cost is now None")
+        host = torch.full((1,), cost, dtype=torch.float32).pin_memory()
+        self.kickstart_cost.copy_(host, non_blocking=True)
+
     def _losses_out(self):
-        """The step's loss values, then the trust-region sums and the UPGO loss when on: float32 [4] to [7]."""
-        return _loss_values(self.out["losses"], self.out["trust"], self.out["upgo"])
+        """The step's loss values, then the trust-region sums, the UPGO loss and the kickstarting loss and KL sum when
+        on: float32 [4] to [9]."""
+        return _loss_values(self.out["losses"], self.out["trust"], self.out["upgo"], self.out["kickstart"])
+
+    def _kickstart_rows(self):
+        return _kickstart_rows(self.out["kickstart"], self.out["vtrace"])
 
     def snapshot(self):
         """Device copies of what stats() reads (the step's losses and its done / episode_return rows, a PopArt model's
-        statistics, the trust-region sums and row count, the UPGO loss), enqueued on the current stream: lets the caller
+        statistics, the trust-region sums and row count, the UPGO loss, the kickstarting values), enqueued on the current stream: lets the caller
         release the learner lock BEFORE the blocking read-back, so the next learner thread's replay queues up behind
         this one instead of waiting for a host round trip."""
         trust = self.out["trust"]
         snap = (self._losses_out(), self.static["done"][1:].clone(), self.static["episode_return"][1:].clone(),
-                None if trust is None else trust.kl.numel(), self.out["upgo"] is not None)
+                None if trust is None else trust.kl.numel(), self.out["upgo"] is not None, self._kickstart_rows())
         if self.popart is not None:
             snap += (self.popart.mu.clone(), self.popart.nu.clone())
         return snap
@@ -852,7 +976,7 @@ class GraphedLearner:
         """Read the snapshot back on a per-thread READ-BACK stream that waits only for `event` (recorded right after the
         snapshot): a read-back on the compute stream would queue behind the NEXT step, which another learner thread has
         already enqueued there."""
-        losses, done, ep_ret, trust_rows, has_upgo = snap[:5]
+        losses, done, ep_ret, trust_rows, has_upgo, kickstart_rows = snap[:6]
         tls = GraphedLearner._tls
         dev = losses.device
         if getattr(tls, "stream", None) is None or tls.device != dev:
@@ -867,7 +991,7 @@ class GraphedLearner:
         with torch.cuda.stream(tls.stream):
             for dst, src in zip(bufs, (losses, done, ep_ret)):
                 dst.copy_(src, non_blocking=True)
-            popart = [s.to("cpu", non_blocking=True) for s in snap[5:]]
+            popart = [s.to("cpu", non_blocking=True) for s in snap[6:]]
         tls.stream.synchronize()
         host, hdone, hret = bufs
         ep = hret[hdone.bool()].clone()
@@ -876,7 +1000,7 @@ class GraphedLearner:
             "total_loss": host[3].item(), "pg_loss": host[0].item(), "baseline_loss": host[1].item(),
             "entropy_loss": host[2].item(),
         }
-        stats.update(_extra_stats(host, trust_rows, has_upgo))
+        stats.update(_extra_stats(host, trust_rows, has_upgo, kickstart_rows))
         if popart:
             stats.update(_popart_stats(*popart))
         return stats
@@ -892,7 +1016,8 @@ class GraphedLearner:
             "entropy_loss": host[2].item(),
         }
         trust = self.out["trust"]
-        stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), self.out["upgo"] is not None))
+        stats.update(_extra_stats(host, None if trust is None else trust.kl.numel(), self.out["upgo"] is not None,
+                                  self._kickstart_rows()))
         if self.popart is not None:
             stats.update(_popart_stats(self.popart.mu.cpu(), self.popart.nu.cpu()))
         return stats

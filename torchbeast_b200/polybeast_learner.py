@@ -150,6 +150,9 @@ def learn(
             stats["mean_episode_step"] = mean_step
             for k in ("total_loss", "pg_loss", "baseline_loss", "entropy_loss"):
                 stats[k] = out[k]
+            for k in ("kickstart_loss", "teacher_kl"):   # with a teacher (torchbeast_b200.kickstart)
+                if k in out:
+                    stats[k] = out[k]
             stats["learner_queue_size"] = learner_queue.size()
             plogger.log(stats)
             if not len(out["episode_returns"]):
