@@ -246,10 +246,36 @@ int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, 
 int tb_sample_actions_dev_f32(const float* logits, int64_t T, int64_t B, int64_t A, const uint64_t* seed_step,
                               const int64_t* stream_ids, int64_t* actions, void* stream);
 
+/* ---- legal-action masks ("invalid action masking": the policy renormalised over each step's legal actions) ---------
+ * A rollout may carry a leaf legal_actions bool / uint8 [T+1,B,A], nonzero = legal, indexed like frame: row t holds the
+ * actions legal at frame t (an env output, stored beside the frame it came with).  Behaviour logits row t+1 and action
+ * row t+1 were formed at frame t, so:
+ *   - the learner's forward output row t is masked by legal_actions row t;
+ *   - the behaviour logits policy_logits[1:] are masked by legal_actions[:-1];
+ *   - action[1:] is checked against legal_actions[:-1].
+ * An illegal logit becomes TB_MASKED_LOGIT = -FLT_MAX (torch.finfo(torch.float32).min), finite on purpose: expf of it
+ * minus any realistic row maximum is exactly 0, so the loss, UPGO, kickstarting, trust-region and sampling kernels
+ * above give p = 0, p * log p = -0 and a logit gradient of +-0 at an illegal entry, and the legal entries' sums keep
+ * their bits (adding +0 changes no float sum).  What they compute is the softmax over the legal set.  -inf would make
+ * 0 * (-inf) = NaN in the entropy, its gradient and the trust region's KL.                                         */
+#define TB_MASKED_LOGIT (-3.40282346638528859812e+38F)
+/* in, out [N,A] f32 (out == in allowed: in place); legal [N,A] u8, nonzero = legal; actions [N] i64 or NULL.  For each
+ * row i:
+ *   - no legal entry (some environments send an empty mask on terminal frames): out[i,:] = in[i,:], unmasked;
+ *   - else, with actions given and 0 <= actions[i] < A and legal[i, actions[i]] == 0 (an illegal taken action, a
+ *     caller bug the kernel cannot raise): out[i,:] = NaN.  On the target logits this makes the step's losses NaN, as
+ *     an out-of-range action does in tb_impala_loss_f32 (on the behaviour logits alone it does not: the rho clips
+ *     drop a NaN log-rho); an out-of-range action is left to the loss;
+ *   - else out[i,a] = legal[i,a] ? in[i,a] : fill, bit for bit.
+ * fill: TB_MASKED_LOGIT for logits; 0 for the gradient of the mask (d out / d in = legal on a masked row).  Sizes:
+ * N >= 0 (0: a no-op success), A >= 1.  One launch, no host sync, no atomics; graph-capturable.                    */
+int tb_mask_logits_f32(const float* in, float* out, const uint8_t* legal, const int64_t* actions, int64_t N, int64_t A,
+                       float fill, void* stream);
+
 /* ---- experience replay: a device ring of earlier batch columns mixed into the learner batch --------------------------
  * A replay buffer is a device ring of `capacity` batch columns.  A stored column holds every learner leaf of one rollout
  * column (frame, stacked [T+1,...] or unstacked [T+4,...]; reward, done, policy_logits, action, and last_action,
- * episode_return and task when present) and, for a net with an LSTM, its initial agent state (h, c: [layers, H] each).
+ * episode_return, task and legal_actions when present) and, for a net with an LSTM, its initial agent state (h, c: [layers, H] each).
  * Each of these is one leaf of the table below: the fresh batch holds it as [outer, Bf, row], the ring as
  * [capacity, outer, row] (one slot's rows contiguous), the mixed batch as [outer, Bf+R, row]; the agent state has
  * outer = layers.  Device state: head_size = (head: the next slot to write, size: the number of valid slots) and

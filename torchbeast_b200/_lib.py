@@ -48,6 +48,7 @@ _SIGNATURES = {
     "tb_resnet_backward": ([_vp] * 5 + [_int] * 6 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _vp], _int),
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
+    "tb_mask_logits_f32": ([_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp], _int),
     "tb_replay_mix": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp], _int),
     "tb_replay_advance": ([_vp, _vp, _i64, _i64, _vp], _int),
     "tb_replay_mix_slots": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _vp], _int),

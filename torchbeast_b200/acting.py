@@ -21,6 +21,9 @@ every kernel of the network; a replay pays one graph launch plus the copies into
   show up in the next replay.  If the buffer moves (.to(), .cuda()), the graphs are dropped and captured again.
 * Outputs are views of the graph's static buffers, valid until the next call on the same GraphedActor; calls must be
   serialised by the caller (polybeast_learner.inference holds its lock around the call).
+* With inputs["legal_actions"] (bool or uint8 [1, B, A], torchbeast_b200.legal_actions) the mask is one more static
+  input, and its presence is part of the graph key: the forward masks its logits, so the sampled and greedy actions
+  are legal.  Padding columns hold an all-zero row, which leaves their logits unmasked.
 * With a FrameHistory attached as `model.frame_history`, a call may pass each stream's newest frame u8 [1, B, 84, 84]
   instead of its stack, with inputs["stream_ids"] naming the streams (default: the column indices).  The graph's static
   frame is then the unstacked array [4, Bk, 84, 84]: the call's frames go to row 3 and the captured history fill writes
@@ -212,9 +215,10 @@ class GraphedActor:
         self._flat_ptr = model.flat_params.data_ptr()
         self.captures = 0  # graphs captured so far (a recapture after the weights moved counts again)
 
-    def _input_names(self):
-        return ("frame", "reward", "done", "last_action") if getattr(self.model, "needs_last_action", False) \
+    def _input_names(self, inputs):
+        names = ("frame", "reward", "done", "last_action") if getattr(self.model, "needs_last_action", False) \
             else ("frame", "reward", "done")
+        return names + (("legal_actions",) if inputs.get("legal_actions") is not None else ())
 
     def __call__(self, inputs, core_state=()):
         model = self.model
@@ -243,8 +247,8 @@ class GraphedActor:
         if model.flat_params.data_ptr() != self._flat_ptr:  # the weights moved: every graph reads the old address
             self._graphs.clear()
             self._flat_ptr = model.flat_params.data_ptr()
-        names = self._input_names()
-        key = (bucket_size(B), model.training, model.precision, tuple(inputs[k].dtype for k in names),
+        names = self._input_names(inputs)
+        key = (bucket_size(B), model.training, model.precision, tuple((k, inputs[k].dtype) for k in names),
                "newest" if newest else "stacked",
                (history.buffer.data_ptr(), history.num_streams) if newest else None)
         ids = inputs.get("stream_ids")

@@ -9,6 +9,7 @@ import torch
 
 from torchbeast_b200 import _lib
 from torchbeast_b200.kickstart import kickstart_cost, teacher_of
+from torchbeast_b200.legal_actions import LEAF as _LEGAL, check_leaf as _check_legal, mask_logits
 
 ImpalaLoss = collections.namedtuple(
     "ImpalaLoss",
@@ -497,6 +498,12 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     batch right after the learner's, and kickstart_loss (one launch after the loss and UPGO) adds its term to the total
     and to grad_logits.  The cost is `kickstart_cost_dev` (a float32 device scalar, GraphedLearner's) or the flag.  The
     stats then carry kickstart_loss, which total_loss includes, and teacher_kl (sum KL / T*B, unweighted).
+
+    A batch with a legal_actions leaf (bool or uint8 [T+1, B, A], torchbeast_b200.legal_actions) learns over each
+    step's legal actions on every path above: the learner's and the teacher's forwards mask their own logits, and one
+    launch writes a masked copy of the behaviour logits (policy_logits[1:] or `behavior_logits`) under
+    legal_actions[:-1], checking action[1:] against it; one more checks it in place on the learner's rows [:-1] (an
+    illegal taken action makes the losses NaN).  The loss, the trust region, UPGO and kickstarting read that copy.
     """
     pop = getattr(model, "popart", None)
     if draw is not None and pop is not None:
@@ -511,11 +518,18 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     trust = upgo = ks = None
     out = model.learner_forward(batch, initial_agent_state)
     teacher_logits = None if teacher is None else teacher.logits(batch)
-    blogits = batch["policy_logits"] if behavior_logits is None else behavior_logits
+    blogits = (batch["policy_logits"] if behavior_logits is None else behavior_logits)[1:]
     acts = batch["action"] if actions is None else actions
+    legal = batch.get(_LEGAL)
+    if legal is not None:
+        # the behaviour logits row t+1 and action row t+1 were formed at frame t, whose legal set is row t
+        blogits = mask_logits(blogits.detach().to(torch.float32), legal[:-1], actions=acts[1:])
+        # the same check on the learner's own rows (already masked by its forward, so only a NaN row can change): a NaN
+        # behaviour row alone would not reach the losses, as the rho clips (fminf) drop a NaN log-rho
+        mask_logits(out.policy_logits[:-1], legal[:-1], actions=acts[1:], out=out.policy_logits[:-1])
     if pop is None:
         loss = impala_loss_fwd_bwd(
-            blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
+            blogits, out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:],
             out.baseline[:-1], out.baseline[-1],
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
@@ -530,7 +544,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     else:
         values = out.baseline.reshape(out.baseline.shape[:2] + (pop.num_tasks,))
         res = impala_loss_popart(
-            blogits[1:], out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:], values,
+            blogits, out.policy_logits[:-1], acts[1:], batch["reward"][1:], batch["done"][1:], values,
             _popart_task(model, batch), pop.mu, pop.nu,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region,
@@ -660,12 +674,16 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       are mixed with replayed columns under the lock, inside the graph when graphed; the warm-up phase and the mixing
       phase are two graphs, as their batch widths differ.  A prioritised buffer adds its draw, the weighted loss and
       the priority update to the same sequence (learn_step's `draw`); with PopArt it raises.
+    * a legal_actions leaf (torchbeast_b200.legal_actions) is checked first, then staged, graphed and replayed like
+      any other leaf; learn_step learns over each step's legal actions.
     * with flags.kickstart_cost, the teacher attached as model.teacher (torchbeast_b200.kickstart.Teacher) runs on the
       same (mixed) batch and its KL term joins the loss (learn_step); the teacher is part of the graph's structure.
     Returns the reference's stats dict."""
     import contextlib
     from torchbeast_b200 import staging
-    # raises before anything is staged or launched: an invalid cost, a cost without a usable teacher, a bare net
+    # raises before anything is staged or launched: an invalid legal_actions leaf, an invalid cost, a cost without a
+    # usable teacher, a bare net
+    _check_legal(batch)
     teacher = _teacher_for(model, actor_model, kickstart_cost(flags))
     needs_last_action = getattr(model, "needs_last_action", False) or (
         teacher is not None and getattr(teacher.net, "needs_last_action", False))
@@ -780,7 +798,8 @@ class GraphedLearner:
     publishes before every replay, so they may change between steps without a new capture.  The values that choose a
     kernel or a buffer (`structure`) are fixed per graph; learn() captures another graph when one of them changes."""
 
-    KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return", "task")
+    KEYS = ("frame", "reward", "done", "policy_logits", "action", "last_action", "episode_return", "task",
+            "legal_actions")
 
     @staticmethod
     def structure_of(optimizer, batch, flags=None, model=None):

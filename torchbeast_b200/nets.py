@@ -14,6 +14,7 @@ import torch
 from torch import nn
 
 from torchbeast_b200 import _lib
+from torchbeast_b200.legal_actions import mask_policy
 
 LearnerOutputs = collections.namedtuple("LearnerOutputs", "policy_logits baseline core_state")
 
@@ -487,7 +488,7 @@ class AtariNet(FlatParamModule):
         logits, baseline, hN, cN = self._launch_forward(
             inputs["frame"], inputs["reward"], notdone, inputs["last_action"], h0, c0, inputs.get("done"))
         self._saved_notdone = notdone
-        return LearnerOutputs(logits, baseline, (hN, cN) if self.use_lstm else tuple())
+        return LearnerOutputs(mask_policy(logits, inputs), baseline, (hN, cN) if self.use_lstm else tuple())
 
     @torch.no_grad()
     def learner_backward(self, grad_logits, grad_baseline, between=None, aux_stream=None):
@@ -526,6 +527,7 @@ class AtariNet(FlatParamModule):
         else:
             logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"], h0, c0,
                                                             done)
+        logits = mask_policy(logits, inputs)  # with inputs["legal_actions"]: the sampler and argmax pick legal actions
         T, B = baseline.shape[:2]
         if self.training:
             action = self._sample(logits, inputs)
@@ -723,7 +725,7 @@ class ResNet(FlatParamModule):
         logits, baseline, hN, cN, saved = self._launch_forward(inputs["frame"], inputs["reward"], notdone, h0, c0,
                                                                inputs.get("done"))
         self._saved = (saved, notdone)
-        return LearnerOutputs(logits, baseline, (hN, cN) if self.use_lstm else tuple())
+        return LearnerOutputs(mask_policy(logits, inputs), baseline, (hN, cN) if self.use_lstm else tuple())
 
     @torch.no_grad()
     def learner_backward(self, grad_logits, grad_baseline):
@@ -741,6 +743,7 @@ class ResNet(FlatParamModule):
             logits, baseline, hN, cN = _ResNetFunction.apply(self, frame, done, inputs["reward"], notdone, h0, c0, *params)
         else:
             logits, baseline, hN, cN, _ = self._launch_forward(frame, inputs["reward"], notdone, h0, c0, done)
+        logits = mask_policy(logits, inputs)  # with inputs["legal_actions"]: the sampler and argmax pick legal actions
         T, B = baseline.shape[:2]
         if self.training:
             action = self._sample(logits, inputs)
