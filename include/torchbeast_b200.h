@@ -246,6 +246,55 @@ int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, 
 int tb_sample_actions_dev_f32(const float* logits, int64_t T, int64_t B, int64_t A, const uint64_t* seed_step,
                               const int64_t* stream_ids, int64_t* actions, void* stream);
 
+/* ---- multi-discrete (factored) action spaces ------------------------------------------------------------------------
+ * An action is a tuple (a_1 .. a_D) of D independent choices, component k taking one of A_k values (gym's MultiDiscrete).
+ * The policy is a product of D categoricals, pi(a) = prod_k pi_k(a_k), each pi_k a softmax over a segment of the row:
+ *   logits [.., A], A = A_1 + ... + A_D: component k owns columns [off_k, off_k + A_k), off_k = A_1 + ... + A_{k-1}
+ *     (off_1 = 0; components are counted from 0 below, so off_0 = 0);
+ *   actions and last_action int64 [.., D]: column k is a_k, in [0, A_k).
+ * The space reaches the library as a host tb_action_space, read before the call returns.  1 <= num_components <=
+ * TB_MAX_ACTION_COMPONENTS, dims[k] >= 1 for k < num_components (later entries are not read), and sum dims = A; an entry
+ * given anything else fails with tb_last_error set.  Per row, every segment quantity below is formed by the code the flat
+ * contract uses for its whole row, on the segment alone:
+ *   log pi_k(a_k) = (l[off_k + a_k] - m_k) - logs_k, with m_k and logs_k the segment's max and log-sum-exp formed as
+ *     tb_action_log_probs_f32 forms them; an a_k outside [0, A_k) gives NaN, which poisons the row as in the flat loss;
+ *   log pi(a) = the fp32 sum over k in index order, from log pi_0(a_0) (no leading 0 is added);
+ *   entropy term: ent_k = sum_{j in k} p_j lp_j in index order, ent = the sum of ent_k over k in index order;
+ *   trust-region KL: KL_k = sum_{j in k} pi_j (lp_j - lmu_j) in index order, KL = the sum of KL_k over k in index order;
+ *   gradient of segment k: adv * (p - onehot(a_k)) + entropy_cost * p * (lp - ent_k), weighted as in the flat loss.
+ * Two properties follow: a component with A_k = 1 contributes exactly 0 to log pi, the entropy and the KL, and a
+ * gradient of +-0; and a space whose components all have size 1 but one gives the flat contract's bits on that one.   */
+#define TB_MAX_ACTION_COMPONENTS 16
+typedef struct tb_action_space {
+  int32_t num_components;                  /* D */
+  int32_t dims[TB_MAX_ACTION_COMPONENTS];  /* A_k */
+} tb_action_space;
+/* Host only: out[0] = sizeof(tb_action_space), out[1] = offsetof num_components, out[2] = offsetof dims. */
+int tb_action_space_layout(int64_t* out_host);
+/* tb_impala_loss_f32 on a factored policy: the same arguments and outputs (hp block, column_weights, PopArt, trust
+ * region; A = sum dims), with actions [T,B,D] and the per-segment rules above in place of the flat row's.  V-trace runs
+ * on log rho = log pi(a) - log mu(a) of the whole tuple; the pg loss is -log pi(a) * pg_adv; target_alp / behavior_alp
+ * are the summed log-probabilities.  With D = 1 it gives tb_impala_loss_f32's bits.  tb_upgo_loss_f32 and
+ * tb_kickstart_loss_f32 take flat rows only.                                                                        */
+int tb_impala_loss_factored_f32(const float* behavior_logits, const float* target_logits, const int64_t* actions,
+                                const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                                const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                                float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
+                                float clip_pg_rho, const tb_hparams* hp, const float* column_weights,
+                                const int64_t* task, const double* mu, const double* nu, int64_t K, double* task_sums,
+                                const float* trust_beta, float* kl_out, float* trust_out, float* vs, float* pg_adv,
+                                float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                                float* grad_logits, float* grad_values, int zero_tail, const tb_action_space* space,
+                                void* workspace, void* stream);
+/* Seeded sampling of a factored policy: logits [T,B,A] -> actions [T,B,D].  Component k of row (t,b) takes x = word
+ * (k mod 4) of Philox4x32-10 with tb_sample_actions_f32's counter and key (lo32(seed), hi32(seed) + k/4) (mod 2^32),
+ * then steps 2-5 of that contract on its segment (a segment with a NaN, all -inf or a +inf logit gets -1).  So D = 1
+ * gives tb_sample_actions_f32's actions.  seed_step (device, nullable) wins over (seed, step), as in
+ * tb_sample_actions_dev_f32, so one entry serves eager and graphed acting.  Sizes as tb_sample_actions_f32.          */
+int tb_sample_actions_factored_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
+                                   const uint64_t* seed_step, const int64_t* stream_ids, const tb_action_space* space,
+                                   int64_t* actions, void* stream);
+
 /* ---- legal-action masks ("invalid action masking": the policy renormalised over each step's legal actions) ---------
  * A rollout may carry a leaf legal_actions bool / uint8 [T+1,B,A], nonzero = legal, indexed like frame: row t holds the
  * actions legal at frame t (an env output, stored beside the frame it came with).  Behaviour logits row t+1 and action
@@ -415,6 +464,15 @@ int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* 
                         int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
                         void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
                         float* hN, float* cN, void* stream);
+/* tb_atarinet_forward of a net with a factored action space (num_actions = sum dims, see "multi-discrete (factored)
+ * action spaces"): last_action is int64 [T1,B,D], and the core input takes a K-hot, core[n, 512+1+off_k+a_k] = 1 for
+ * each k (a component outside [0, A_k) sets nothing), in place of the one-hot.  Everything else is tb_atarinet_forward;
+ * the K-hot gets no gradient, so tb_atarinet_backward is its backward.                                             */
+int tb_atarinet_forward_factored(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                                 const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                 int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                 void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                 float* hN, float* cN, const tb_action_space* space, void* stream);
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
                          const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
                          int precision, void* workspace, float* grads, int phase, void* stream);

@@ -34,7 +34,7 @@ every kernel of the network; a replay pays one graph launch plus the copies into
 """
 import torch
 
-from torchbeast_b200 import _lib, nets
+from torchbeast_b200 import _lib, nets, sampling
 
 
 def bucket_size(B):
@@ -179,11 +179,13 @@ class _DeviceStepSampler:
     def __init__(self, seed_step):
         self.seed_step = seed_step
 
-    def sample(self, logits, stream_ids=None):
+    def sample(self, logits, stream_ids=None, action_dims=None):
         T, B, A = logits.shape
         logits = logits.detach().contiguous()
         if stream_ids is not None:
             stream_ids = stream_ids.to(device=logits.device, dtype=torch.int64).contiguous()
+        if action_dims is not None:  # a factored policy: one entry reads seed_step the same way
+            return sampling.sample_factored(logits, action_dims, stream_ids, seed_step=self.seed_step)
         actions = torch.empty(T, B, dtype=torch.int64, device=logits.device)
         _lib.check(
             _lib.lib().tb_sample_actions_dev_f32(_lib.ptr(logits), T, B, A, _lib.ptr(self.seed_step),

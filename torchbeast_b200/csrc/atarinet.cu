@@ -159,11 +159,13 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
 // forward
 // ---------------------------------------------------------------------------------------
 // done == nullptr: frame is stacked u8 [T1,B,4,84,84]; otherwise frame is an unstacked rollout u8 [T1+3,B,84,84] whose stacks
-// the tensor-core backends rebuild in their frame-image pass (the fp32 backend is handed restacked frames by its caller)
+// the tensor-core backends rebuild in their frame-image pass (the fp32 backend is handed restacked frames by its caller).
+// seg non-NULL: a factored action space, last_action [T1,B,D] enters the core as a K-hot (core_extras).
 static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                             const int64_t* last_action, const float* h0, const float* c0, const float* P,
                             int64_t T1, int64_t B, int A, int use_lstm, int precision, void* workspace,
-                            float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1) {
+                            float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1,
+                            const ActionSegments* seg = nullptr) {
   using G = AtariGeom;
   const int64_t N = T1 * B;
   const AtariParams pp = atari_params(A, use_lstm, V);
@@ -224,7 +226,7 @@ static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const flo
   TB_TRY((gemm_simt<float, float, false, true>(w.act3, w.wfcp, w.core_in, N, G::FC_OUT, G::FC_IN, G::FC_IN, G::FC_IN,
                                                 pp.core, ep, 1, nullptr, st)));
   }
-  TB_TRY(core_extras(w.core_in, pp.core, N, G::FC_OUT, reward, last_action, A, st));
+  TB_TRY(core_extras(w.core_in, pp.core, N, G::FC_OUT, reward, last_action, A, st, seg));
   if (use_lstm) {
     LstmParams lp;
     for (int l = 0; l < 2; ++l) {
@@ -414,11 +416,12 @@ size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int u
   return atari_ws(nullptr, T1 * B, T1, B, num_actions, use_lstm, precision).bytes;
 }
 
-int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
-                        const int64_t* last_action, const float* h0, const float* c0, const float* params, int64_t T1,
-                        int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
-                        void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
-                        void* stream) {
+// tb_atarinet_forward and, with seg non-NULL, tb_atarinet_forward_factored
+static int atarinet_forward_entry(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                                  const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                  int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                  void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                  float* hN, float* cN, void* stream, const ActionSegments* seg) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward: num_values %d outside [1, %d]",
              num_values, kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward: bad sizes T1=%lld B=%lld A=%d", (long long)T1,
@@ -439,7 +442,29 @@ int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* 
     done = nullptr;
   }
   return atarinet_forward(frame, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
-                          workspace, policy_logits, baseline, hN, cN, st, num_values);
+                          workspace, policy_logits, baseline, hN, cN, st, num_values, seg);
+}
+
+int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                        const int64_t* last_action, const float* h0, const float* c0, const float* params, int64_t T1,
+                        int64_t B, int num_actions, int num_values, int use_lstm, int precision, void* workspace,
+                        void* stacked_scratch, float* policy_logits, float* baseline, float* hN, float* cN,
+                        void* stream) {
+  return atarinet_forward_entry(frame, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions,
+                                num_values, use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN,
+                                cN, stream, nullptr);
+}
+
+int tb_atarinet_forward_factored(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                                 const int64_t* last_action, const float* h0, const float* c0, const float* params,
+                                 int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                 void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                 float* hN, float* cN, const tb_action_space* space, void* stream) {
+  ActionSegments seg;
+  TB_TRY(action_segments(space, num_actions, "atarinet_forward_factored", &seg));
+  return atarinet_forward_entry(frame, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions,
+                                num_values, use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN,
+                                cN, stream, &seg);
 }
 
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,

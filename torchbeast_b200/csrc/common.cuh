@@ -38,6 +38,16 @@ struct ProfScope {
 
 constexpr int kWarp = 32;
 constexpr int kNumSMs = 132;  // H100 SXM
+
+// A factored action space (include/torchbeast_b200.h, tb_action_space) as the kernels take it, by value: component k
+// owns logit columns [off[k], off[k+1]) and column k of the [.., D] actions.
+struct ActionSegments {
+  int D;
+  int off[TB_MAX_ACTION_COMPONENTS + 1];
+};
+// Checks `space` against a row of A logits (non-NULL, 1 <= D <= 16, every dim >= 1, sum == A) and fills `out`; sets the
+// error and returns non-zero otherwise.  `who` prefixes the message.
+int action_segments(const tb_action_space* space, int64_t A, const char* who, ActionSegments* out);
 // workspace layout: [0] uint32 ticket counter (self-resetting), then kMaxPartialCtas per-CTA partials of up to
 // kMaxPartialSums doubles each (grid_sum3: stride 4, grid_sum<N>: stride N)
 constexpr int kMaxPartialCtas = 4096;
@@ -61,8 +71,9 @@ template <> struct M<double> {
 // Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): words 0 and 1 of the output.
 // Shared by the action sampler (sample.cu) and the replay slot draws (replay.cu); the uniform draws use word 0 only,
 // the prioritised draws both.
-__device__ __forceinline__ uint2 philox4x32_10_w01(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                                   uint32_t k1) {
+// The factored action sampler (sample.cu) uses all four words.
+__device__ __forceinline__ uint4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
+                                              uint32_t k1) {
   constexpr uint32_t kM0 = 0xD2511F53u, kM1 = 0xCD9E8D57u, kW0 = 0x9E3779B9u, kW1 = 0xBB67AE85u;
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -75,7 +86,12 @@ __device__ __forceinline__ uint2 philox4x32_10_w01(uint32_t c0, uint32_t c1, uin
     k0 += kW0;
     k1 += kW1;
   }
-  return make_uint2(c0, c1);
+  return make_uint4(c0, c1, c2, c3);
+}
+__device__ __forceinline__ uint2 philox4x32_10_w01(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
+                                                   uint32_t k1) {
+  const uint4 r = philox4x32_10(c0, c1, c2, c3, k0, k1);
+  return make_uint2(r.x, r.y);
 }
 __device__ __forceinline__ uint32_t philox4x32_10_w0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
                                                      uint32_t k1) {

@@ -237,10 +237,37 @@ __global__ void core_extras_kernel(float* __restrict__ core, int64_t ld, int64_t
   }
 }
 
+// The factored form: core[n, F+1+c] = 1 where column c is off_k + last_action[n, k] of its segment k (a K-hot).
+__global__ void core_extras_factored_kernel(float* __restrict__ core, int64_t ld, int64_t N, int F,
+                                            const float* __restrict__ reward, const int64_t* __restrict__ last_action,
+                                            ActionSegments seg) {
+  const int A = seg.off[seg.D];
+  const int64_t total = N * (A + 1);
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int64_t n = i / (A + 1);
+    const int j = int(i % (A + 1));
+    float v;
+    if (j == 0) {
+      v = fminf(fmaxf(reward[n], -1.0f), 1.0f);
+    } else {
+      int k = 0;
+      while (seg.off[k + 1] <= j - 1) ++k;
+      v = (last_action[n * seg.D + k] == int64_t(j - 1 - seg.off[k])) ? 1.0f : 0.0f;
+    }
+    core[n * ld + F + j] = v;
+  }
+}
+
 int core_extras(float* core, int64_t ld, int64_t N, int F, const float* reward, const int64_t* last_action, int A,
-                cudaStream_t stream) {
+                cudaStream_t stream, const ActionSegments* seg) {
   ProfScope prof("core_extras", stream);
   if (N == 0) return 0;
+  if (seg) {
+    core_extras_factored_kernel<<<grid_for(N * (A + 1), 256), 256, 0, stream>>>(core, ld, N, F, reward, last_action,
+                                                                                *seg);
+    return check_launch("core_extras_factored_kernel");
+  }
   // A == 0: reward column only (polybeast Net has no last-action one-hot)
   core_extras_kernel<<<grid_for(N * (A + 1), 256), 256, 0, stream>>>(core, ld, N, F, reward, last_action, A);
   return check_launch("core_extras_kernel");

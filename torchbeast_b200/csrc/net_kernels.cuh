@@ -30,8 +30,10 @@ int64_t colsum_scratch_floats(int64_t ncols);
 int colsum(const float* X, float* out, int64_t M, int64_t ncols, int64_t ld, float* scratch, cudaStream_t stream);
 
 // core[n, F] = clamp(reward[n], -1, 1); core[n, F+1+j] = (last_action[n] == j)   (monobeast.py:593-597)
+// seg non-NULL (a factored action space, A = its width): last_action is [N, D] and the one-hot becomes a K-hot,
+// core[n, F+1+off_k+last_action[n, k]] = 1 for each component k
 int core_extras(float* core, int64_t ld, int64_t N, int F, const float* reward, const int64_t* last_action, int A,
-                cudaStream_t stream);
+                cudaStream_t stream, const ActionSegments* seg = nullptr);
 
 // X[m, n] *= (Y[m, n] > 0) for n < ncols (ReLU backward in place on a strided view)
 int relu_mask_inplace(float* X, const float* Y, int64_t M, int64_t ncols, int64_t ldx, int64_t ldy,

@@ -441,7 +441,73 @@ struct LossArgs {
   // trust region (impala_loss_kernel<A, *, *, true> only): beta read from *trust_beta when the kernel runs, kl [T,B]
   // out, trust_out [2] = {trusted rows, sum kl}
   const float* trust_beta; float* kl; float* trust_out;
+  // factored action space (impala_loss_kernel<0, *, *, *, true> only): actions are [T,B,D], row segments as in seg
+  ActionSegments seg;
 };
+
+// ---- factored action spaces (impala_loss_kernel<0, *, *, *, true>) -----------------------------------------------------
+// Each segment is a row of its own for alp_dyn, the code the flat rows use; the sums over segments run in index order from
+// segment 0 (include/torchbeast_b200.h, "multi-discrete (factored) action spaces").
+
+// log pi(a) = sum_k log pi_k(a_k) of the row at `row`, actions act[0..D)
+__device__ __forceinline__ float alp_factored(const ActionSegments& seg, const float* __restrict__ row,
+                                              const int64_t* __restrict__ act) {
+  float lp = alp_dyn<float>(row, seg.off[1], act[0], nullptr, nullptr);
+  for (int k = 1; k < seg.D; ++k)
+    lp += alp_dyn<float>(row + seg.off[k], seg.off[k + 1] - seg.off[k], act[k], nullptr, nullptr);
+  return lp;
+}
+
+// sum_k KL(pi_k || mu_k) of row i in fp32, each segment as trust_kl forms a whole row
+__device__ __forceinline__ float trust_kl_factored(const LossArgs& p, int64_t i) {
+  const float* trow = p.tlogits + i * p.A;
+  const float* brow = p.blogits + i * p.A;
+  float kl = 0.0f;
+  for (int k = 0; k < p.seg.D; ++k) {
+    const int o = p.seg.off[k], Ak = p.seg.off[k + 1] - o;
+    float mt, logst, mb, logsb;
+    alp_dyn<float>(trow + o, Ak, 0, &mt, &logst);
+    alp_dyn<float>(brow + o, Ak, 0, &mb, &logsb);
+    float klk = 0.0f;
+    for (int j = o; j < o + Ak; ++j) {
+      const float lt = (trow[j] - mt) - logst, lb = (brow[j] - mb) - logsb;
+      klk += expf(lt) * (lt - lb);
+    }
+    kl = k == 0 ? klk : kl + klk;
+  }
+  return kl;
+}
+
+// The entropy term sum_k ent_k of row i, and with grad_logits its gradient row: segment k gets
+// adv * (p - onehot(a_k)) + entropy_cost * p * (lp - ent_k), times column_weights[b] when kWeighted.
+template <bool kWeighted>
+__device__ __forceinline__ float factored_entropy_grad(const LossArgs& p, int64_t i, int64_t b, float adv) {
+  const float* trow = p.tlogits + i * p.A;
+  const int64_t* act = p.actions + i * p.seg.D;
+  float ent_row = 0.0f;
+  for (int k = 0; k < p.seg.D; ++k) {
+    const int o = p.seg.off[k], Ak = p.seg.off[k + 1] - o;
+    const float* srow = trow + o;
+    const int64_t ak = act[k];
+    float m, logs;
+    alp_dyn<float>(srow, Ak, 0, &m, &logs);
+    float ent = 0.0f;
+    for (int j = 0; j < Ak; ++j) {
+      const float lp = (srow[j] - m) - logs;
+      ent += expf(lp) * lp;
+    }
+    if (p.grad_logits) {
+      float* g = p.grad_logits + i * p.A + o;
+      for (int j = 0; j < Ak; ++j) {
+        const float lp = (srow[j] - m) - logs, pr = expf(lp);
+        const float gl = adv * (pr - (ak == j ? 1.0f : 0.0f)) + p.entropy_cost * pr * (lp - ent);
+        if constexpr (kWeighted) g[j] = gl * __ldg(p.column_weights + b); else g[j] = gl;
+      }
+    }
+    ent_row = k == 0 ? ent : ent_row + ent;
+  }
+  return ent_row;
+}
 
 // ---- trust region (impala_loss_kernel<A, *, *, true>) ----------------------------------------------------------------
 // The kernel reaches the trust region only through the three helpers below, so the instantiations without it compile
@@ -477,13 +543,13 @@ __device__ __forceinline__ float trust_kl(const LossArgs& p, int64_t i, int64_t 
 
 // rho of row i under the trust region: expf(lr) where kl_i <= beta, else 0 (a NaN kl too).  kl_i is formed and written
 // to p.kl here, or, with `written`, read back from there (pass 1 of the split layout wrote it in this thread).
-template <int A>
+template <int A, bool kFactored = false>
 __device__ __forceinline__ float trust_rho(const LossArgs& p, int64_t i, int64_t Ause, float lr, bool written) {
   float kl;
   if (written) {
     kl = p.kl[i];
   } else {
-    kl = trust_kl<A>(p, i, Ause);
+    if constexpr (kFactored) kl = trust_kl_factored(p, i); else kl = trust_kl<A>(p, i, Ause);
     p.kl[i] = kl;
   }
   const float rho = expf(lr);
@@ -543,9 +609,12 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 // compile none of that code.  kWeighted: every term of column b is multiplied by LossArgs::column_weights[b], after the
 // unweighted term is formed, so a weight of 1.0f gives the unweighted bits; the other instantiations compile no weight
 // code.  kTrust: row (t, b) with kl_t = KL(pi_t || mu_t) > beta (or NaN) runs the V-trace and the policy gradient with
-// rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_f32); the other instantiations compile no trust code.
-template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false>
+// rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_f32); the other instantiations compile no trust code.  kFactored
+// (with A = 0 only): actions are [T,B,D] and every row quantity is formed per segment (LossArgs::seg); the other
+// instantiations compile none of that code.
+template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false, bool kFactored = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
+  static_assert(!kFactored || A == 0, "factored rows take the dynamic-A path");
   if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* sA = reinterpret_cast<float*>(smem_raw);
@@ -587,12 +656,18 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         float v_next = kPopArt ? pop_value(t1, b) : (t1 < T) ? p.values[t1 * B + b] : p.bootstrap[b];
         for (int64_t t = t1 - 1; t >= t0; --t) {
           const int64_t i = t * B + b;
-          const int64_t act = p.actions[i];
-          const float tlp = alp_row<float, A>(p.tlogits + i * Ause, Ause, act, nullptr, nullptr);
-          const float blp = alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
+          float tlp, blp;
+          if constexpr (kFactored) {
+            tlp = alp_factored(p.seg, p.tlogits + i * Ause, p.actions + i * p.seg.D);
+            blp = alp_factored(p.seg, p.blogits + i * Ause, p.actions + i * p.seg.D);
+          } else {
+            const int64_t act = p.actions[i];
+            tlp = alp_row<float, A>(p.tlogits + i * Ause, Ause, act, nullptr, nullptr);
+            blp = alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
+          }
           const float lr = tlp - blp;
           p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
-          const float rho = kTrust ? trust_rho<A>(p, i, Ause, lr, false) : expf(lr);  // kl read back in pass 3
+          const float rho = kTrust ? trust_rho<A, kFactored>(p, i, Ause, lr, false) : expf(lr);  // kl read back in pass 3
           const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
           const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
           const float delta = rb * (r + g * v_next - v);
@@ -626,19 +701,21 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
     float acc = acc_in;
     for (int64_t t = t1 - 1; t >= t0; --t) {
       const int64_t i = t * B + b;
-      const int64_t act = p.actions[i];
+      const int64_t act = kFactored ? 0 : p.actions[i];
       const float* trow = p.tlogits + i * Ause;
       float m, logs;
-      const float tlp = alp_row<float, A>(trow, Ause, act, &m, &logs);
+      const float tlp = kFactored ? alp_factored(p.seg, trow, p.actions + i * p.seg.D)
+                                  : alp_row<float, A>(trow, Ause, act, &m, &logs);
       float lr;
       if (W > 1) {
         lr = p.log_rhos[i];  // written by this same thread in pass 1
       } else {
-        const float blp = alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
+        const float blp = kFactored ? alp_factored(p.seg, p.blogits + i * Ause, p.actions + i * p.seg.D)
+                                    : alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
         lr = tlp - blp;
         p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
       }
-      const float rho = kTrust ? trust_rho<A>(p, i, Ause, lr, W > 1) : expf(lr);
+      const float rho = kTrust ? trust_rho<A, kFactored>(p, i, Ause, lr, W > 1) : expf(lr);
       const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
       const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
       const float rp = p.has_clip_pg ? fminf(rho, p.clip_pg) : rho;
@@ -677,7 +754,9 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         s_bl += 0.5 * double(d * d);
       }
       float ent_row = 0.0f;
-      if constexpr (A != 0) {
+      if constexpr (kFactored) {
+        ent_row = factored_entropy_grad<kWeighted>(p, i, b, adv);
+      } else if constexpr (A != 0) {
         float lp[A], pr[A];
 #pragma unroll
         for (int j = 0; j < A; ++j) {
@@ -1041,43 +1120,19 @@ __global__ void pg_loss_kernel(const F* __restrict__ logits, const int64_t* __re
   if (grid_sum3(s, 0.0, 0.0, ws, tot)) out[0] = F(tot[0]);
 }
 
-static int reduce_grid(int64_t N, int threads) {
-  int64_t blocks = (N + threads - 1) / threads;
-  const int64_t cap = int64_t(sm_count()) * 4;
-  if (blocks > cap) blocks = cap;
-  if (blocks > kMaxPartialCtas) blocks = kMaxPartialCtas;
-  return int(blocks < 1 ? 1 : blocks);
+// One fused-loss launch: the flat kernel of the row width p.A (TB_DISPATCH_A), or with `factored` the dynamic-A kernel
+// that reads p.seg.
+template <bool kPopArt, bool kWeighted, bool kTrust>
+static void launch_loss_kernel(const LossArgs& p, bool factored, dim3 grid, dim3 block, size_t smem, cudaStream_t st) {
+  if (factored)
+    impala_loss_kernel<0, kPopArt, kWeighted, kTrust, true><<<grid, block, smem, st>>>(p);
+  else
+    TB_DISPATCH_A(p.A, (impala_loss_kernel<kA, kPopArt, kWeighted, kTrust><<<grid, block, smem, st>>>(p)));
 }
 
-}  // namespace tb
-
-// ========================================================================================
-// C ABI
-// ========================================================================================
-using namespace tb;
-
-extern "C" {
-
-int tb_action_log_probs_f32(const float* l, const int64_t* a, int64_t N, int64_t A, float* o, void* s) {
-  return launch_alp<float>(l, a, N, A, o, s);
-}
-int tb_action_log_probs_f64(const double* l, const int64_t* a, int64_t N, int64_t A, double* o, void* s) {
-  return launch_alp<double>(l, a, N, A, o, s);
-}
-
-int tb_vtrace_from_importance_weights_f32(const float* lr, const float* d, const float* r, const float* v,
-                                          const float* bs, int64_t T, int64_t B, float c1, float c2,
-                                          float* vs, float* pg, void* s) {
-  return launch_scan<float>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
-}
-int tb_vtrace_from_importance_weights_f64(const double* lr, const double* d, const double* r, const double* v,
-                                          const double* bs, int64_t T, int64_t B, double c1, double c2,
-                                          double* vs, double* pg, void* s) {
-  return launch_scan<double>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
-}
-
-// The kernel instantiation follows from which of column_weights, task and trust_beta are non-NULL.
-int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
+// tb_impala_loss_f32 and, with seg non-NULL, tb_impala_loss_factored_f32.  The kernel instantiation follows from which
+// of column_weights, task and trust_beta are non-NULL.
+static int impala_loss(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
                        const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
                        int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
                        int clip_rewards, float clip_rho, float clip_pg_rho, const tb_hparams* hp,
@@ -1085,7 +1140,8 @@ int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t
                        int64_t K, double* task_sums, const float* trust_beta, float* kl_out, float* trust_out,
                        float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
                        float* losses_out, float* grad_logits, float* grad_values, int zero_tail, void* workspace,
-                       void* stream) {
+                       void* stream, const ActionSegments* seg) {
+
   if (task) {
     TB_REQUIRE(!column_weights, "impala_loss_popart: column_weights are not supported with PopArt (task)");
     TB_REQUIRE(T >= 1 && B >= 1 && A >= 1, "impala_loss_popart: bad sizes T=%lld B=%lld A=%lld", (long long)T,
@@ -1129,6 +1185,7 @@ int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t
   p.task = task; p.pa_mu = mu; p.pa_nu = nu; p.K = int(K);
   p.column_weights = column_weights;
   p.trust_beta = trust_beta; p.kl = kl_out; p.trust_out = trust_out;
+  if (seg) p.seg = *seg;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
   int W = pick_warps(T, tiles);
   p.wide = (W == 1);
@@ -1145,10 +1202,10 @@ int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t
     ProfScope prof(trust_beta ? "impala_loss_popart_trust" : "impala_loss_popart", (cudaStream_t)stream);
     const size_t pop_smem = smem + size_t(2) * kPopArtMaxTasks * sizeof(float);
     if (trust_beta) {
-      TB_DISPATCH_A(A, (impala_loss_kernel<kA, true, false, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
+      launch_loss_kernel<true, false, true>(p, seg, grid, block, pop_smem, (cudaStream_t)stream);
       TB_TRY(check_launch("impala_loss_kernel<popart, trust>"));
     } else {
-      TB_DISPATCH_A(A, (impala_loss_kernel<kA, true><<<grid, block, pop_smem, (cudaStream_t)stream>>>(p)));
+      launch_loss_kernel<true, false, false>(p, seg, grid, block, pop_smem, (cudaStream_t)stream);
       TB_TRY(check_launch("impala_loss_kernel<popart>"));
     }
     popart_task_sums_kernel<<<unsigned(K), kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, int(K),
@@ -1158,20 +1215,88 @@ int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t
   if (trust_beta) {
     ProfScope prof("impala_loss_trust", (cudaStream_t)stream);
     if (column_weights) {
-      TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, true, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+      launch_loss_kernel<false, true, true>(p, seg, grid, block, smem, (cudaStream_t)stream);
       return check_launch("impala_loss_kernel<weighted, trust>");
     }
-    TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, false, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+    launch_loss_kernel<false, false, true>(p, seg, grid, block, smem, (cudaStream_t)stream);
     return check_launch("impala_loss_kernel<trust>");
   }
   if (column_weights) {
     ProfScope prof("impala_loss_weighted", (cudaStream_t)stream);
-    TB_DISPATCH_A(A, (impala_loss_kernel<kA, false, true><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+    launch_loss_kernel<false, true, false>(p, seg, grid, block, smem, (cudaStream_t)stream);
     return check_launch("impala_loss_kernel<weighted>");
   }
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
-  TB_DISPATCH_A(A, (impala_loss_kernel<kA><<<grid, block, smem, (cudaStream_t)stream>>>(p)));
+  launch_loss_kernel<false, false, false>(p, seg, grid, block, smem, (cudaStream_t)stream);
   return check_launch("impala_loss_kernel");
+}
+
+static int reduce_grid(int64_t N, int threads) {
+  int64_t blocks = (N + threads - 1) / threads;
+  const int64_t cap = int64_t(sm_count()) * 4;
+  if (blocks > cap) blocks = cap;
+  if (blocks > kMaxPartialCtas) blocks = kMaxPartialCtas;
+  return int(blocks < 1 ? 1 : blocks);
+}
+
+}  // namespace tb
+
+// ========================================================================================
+// C ABI
+// ========================================================================================
+using namespace tb;
+
+extern "C" {
+
+int tb_action_log_probs_f32(const float* l, const int64_t* a, int64_t N, int64_t A, float* o, void* s) {
+  return launch_alp<float>(l, a, N, A, o, s);
+}
+int tb_action_log_probs_f64(const double* l, const int64_t* a, int64_t N, int64_t A, double* o, void* s) {
+  return launch_alp<double>(l, a, N, A, o, s);
+}
+
+int tb_vtrace_from_importance_weights_f32(const float* lr, const float* d, const float* r, const float* v,
+                                          const float* bs, int64_t T, int64_t B, float c1, float c2,
+                                          float* vs, float* pg, void* s) {
+  return launch_scan<float>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
+}
+int tb_vtrace_from_importance_weights_f64(const double* lr, const double* d, const double* r, const double* v,
+                                          const double* bs, int64_t T, int64_t B, double c1, double c2,
+                                          double* vs, double* pg, void* s) {
+  return launch_scan<double>(lr, d, r, v, bs, T, B, c1, c2, vs, pg, s);
+}
+
+int tb_impala_loss_f32(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
+                       const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
+                       int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
+                       int clip_rewards, float clip_rho, float clip_pg_rho, const tb_hparams* hp,
+                       const float* column_weights, const int64_t* task, const double* mu, const double* nu,
+                       int64_t K, double* task_sums, const float* trust_beta, float* kl_out, float* trust_out,
+                       float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
+                       float* losses_out, float* grad_logits, float* grad_values, int zero_tail, void* workspace,
+                       void* stream) {
+  return impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A, discounting,
+                     baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, column_weights, task, mu, nu,
+                     K, task_sums, trust_beta, kl_out, trust_out, vs, pg_adv, log_rhos, behavior_alp, target_alp,
+                     losses_out, grad_logits, grad_values, zero_tail, workspace, stream, nullptr);
+}
+
+int tb_impala_loss_factored_f32(const float* blogits, const float* tlogits, const int64_t* actions,
+                                const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                                const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                                float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
+                                float clip_pg_rho, const tb_hparams* hp, const float* column_weights,
+                                const int64_t* task, const double* mu, const double* nu, int64_t K, double* task_sums,
+                                const float* trust_beta, float* kl_out, float* trust_out, float* vs, float* pg_adv,
+                                float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                                float* grad_logits, float* grad_values, int zero_tail, const tb_action_space* space,
+                                void* workspace, void* stream) {
+  ActionSegments seg;
+  TB_TRY(action_segments(space, A, "impala_loss_factored", &seg));
+  return impala_loss(blogits, tlogits, actions, rewards, done, discounts, values, bootstrap, T, B, A, discounting,
+                     baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, column_weights, task, mu, nu,
+                     K, task_sums, trust_beta, kl_out, trust_out, vs, pg_adv, log_rhos, behavior_alp, target_alp,
+                     losses_out, grad_logits, grad_values, zero_tail, workspace, stream, &seg);
 }
 
 // The kernel instantiation follows from which of column_weights, task and trust_beta are non-NULL, as in the loss.

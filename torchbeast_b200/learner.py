@@ -1,5 +1,6 @@
 """Fused pieces of the learner step shared by monobeast.learn and polybeast_learner.learn."""
 import collections
+import ctypes
 import numbers
 import os
 import threading
@@ -8,6 +9,7 @@ import numpy as np
 import torch
 
 from torchbeast_b200 import _lib
+from torchbeast_b200 import action_space as _action_space
 from torchbeast_b200.kickstart import kickstart_cost, teacher_of
 from torchbeast_b200.legal_actions import LEAF as _LEGAL, check_leaf as _check_legal, mask_logits
 
@@ -135,6 +137,7 @@ def impala_loss_fwd_bwd(
     column_weights=None,
     trust_region=None,
     upgo_cost=None,
+    action_space=None,
 ):
     """The whole loss block of learn() in ONE kernel launch (tb_impala_loss_f32), two with UPGO.
 
@@ -161,6 +164,10 @@ def impala_loss_fwd_bwd(
     gradient (tb_upgo_loss_f32, a second launch; the rule is stated in include/torchbeast_b200.h) adds
     upgo_cost * sum w_b * (-log pi(a)) * A_upgo to losses[3] and its gradient to grad_logits, and an Upgo(adv, loss)
     is appended last to what the call returns.
+
+    With `action_space` (component sizes (A_1, ..., A_D) summing to A; torchbeast_b200.action_space) the policy is
+    factored: `actions` are int64 [T, B, D] and tb_impala_loss_factored_f32 forms every row quantity per component
+    (the rules are stated in include/torchbeast_b200.h).  UPGO takes flat rows only.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
@@ -172,7 +179,8 @@ def impala_loss_fwd_bwd(
     loss, _, trust, upgo = _impala_loss(
         behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value, discounting,
         baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, with_grads,
-        hparams_dev, column_weights=column_weights, trust_region=trust_region, upgo_cost=upgo_cost)
+        hparams_dev, column_weights=column_weights, trust_region=trust_region, upgo_cost=upgo_cost,
+        action_space=action_space)
     out = (loss,) + tuple(x for x in (trust, upgo) if x is not None)
     return out[0] if len(out) == 1 else out
 
@@ -197,6 +205,7 @@ def impala_loss_popart(
     hparams_dev=None,
     trust_region=None,
     upgo_cost=None,
+    action_space=None,
 ):
     """impala_loss_fwd_bwd on a PopArt-normalised value head (tb_impala_loss_f32 with a task).
 
@@ -207,7 +216,8 @@ def impala_loss_popart(
     (ImpalaLoss, task_sums): task_sums float64 [3, K] = per-task count, sum vs, sum vs^2 over rows t < T, the input
     of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd) it
     returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs.  With `upgo_cost` (see
-    impala_loss_fwd_bwd; its advantage is divided by sigma_k) an Upgo is appended last."""
+    impala_loss_fwd_bwd; its advantage is divided by sigma_k) an Upgo is appended last.  `action_space`: a factored
+    policy, as in impala_loss_fwd_bwd."""
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
     _lib.require_cuda(*tensors)
     T, B, A = target_policy_logits.shape
@@ -220,16 +230,26 @@ def impala_loss_popart(
     loss, sums, trust, upgo = _impala_loss(
         behavior_policy_logits, target_policy_logits, actions, rewards, done, values, None, discounting,
         baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold, True, hparams_dev,
-        popart=(task, mu, nu), trust_region=trust_region, upgo_cost=upgo_cost)
+        popart=(task, mu, nu), trust_region=trust_region, upgo_cost=upgo_cost, action_space=action_space)
     return (loss, sums) + tuple(x for x in (trust, upgo) if x is not None)
 
 
 def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value,
                  discounting, baseline_cost, entropy_cost, reward_clipping, clip_rho_threshold, clip_pg_rho_threshold,
-                 with_grads, hparams_dev, column_weights=None, popart=None, trust_region=None, upgo_cost=None):
+                 with_grads, hparams_dev, column_weights=None, popart=None, trust_region=None, upgo_cost=None,
+                 action_space=None):
     """The tb_impala_loss_f32 call behind impala_loss_fwd_bwd and impala_loss_popart, on inputs they checked, and with
     `upgo_cost` the tb_upgo_loss_f32 call right behind it on the same inputs.  popart: None, or (task, mu, nu) with
-    values [T+1, B, K].  Returns (ImpalaLoss, task_sums or None, TrustRegion or None, Upgo or None)."""
+    values [T+1, B, K].  action_space: component sizes, for tb_impala_loss_factored_f32.  Returns (ImpalaLoss,
+    task_sums or None, TrustRegion or None, Upgo or None)."""
+    dims = _action_space.dims_of(None if action_space is None else tuple(action_space))
+    if dims is not None:
+        if upgo_cost is not None:
+            raise _lib.TorchBeastB200Error("UPGO (upgo_cost) is not built for a factored action space %r" % (dims,))
+        T, B = target_policy_logits.shape[:2]
+        if tuple(actions.shape) != (T, B, len(dims)):
+            raise _lib.TorchBeastB200Error("a factored action space %r takes actions [T, B, D] = %r, got %r"
+                                           % (dims, (T, B, len(dims)), tuple(actions.shape)))
     if hparams_dev is None:
         clip_rewards = _clip_rewards(reward_clipping)
     else:
@@ -270,14 +290,17 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
     disc_arg = 0.0 if hparams_dev is not None else float(discounting)
     p = _lib.ptr
     ws = _lib.workspace()
-    _lib.check(
-        _lib.lib().tb_impala_loss_f32(
-            p(behavior_policy_logits.to(f32).contiguous()), p(tl), p(act), p(rw), p(dn), p(disc), p(vals), p(bs),
+    args = (p(behavior_policy_logits.to(f32).contiguous()), p(tl), p(act), p(rw), p(dn), p(disc), p(vals), p(bs),
             T, B, A, disc_arg, float(baseline_cost), float(entropy_cost),
             clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev),
             p(cw), p(task), p(mu), p(nu), K, p(sums), p(beta), p(kl), p(kl_sums),
-            *[p(o) for o in outs], p(losses), p(gl), p(gv), 1, p(ws), _lib.stream_ptr()),
-        "tb_impala_loss_f32")
+            *[p(o) for o in outs], p(losses), p(gl), p(gv), 1)
+    if dims is None:
+        _lib.check(_lib.lib().tb_impala_loss_f32(*args, p(ws), _lib.stream_ptr()), "tb_impala_loss_f32")
+    else:
+        _lib.check(_lib.lib().tb_impala_loss_factored_f32(*args, ctypes.byref(_action_space.c_space(dims)), p(ws),
+                                                          _lib.stream_ptr()),
+                   "tb_impala_loss_factored_f32")
     upgo = None
     if cost is not None:
         upgo = Upgo(torch.empty((T, B), dtype=f32, device=dev), torch.empty(1, dtype=f32, device=dev))
@@ -499,6 +522,9 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     and to grad_logits.  The cost is `kickstart_cost_dev` (a float32 device scalar, GraphedLearner's) or the flag.  The
     stats then carry kickstart_loss, which total_loss includes, and teacher_kl (sum KL / T*B, unweighted).
 
+    A model with a factored action space (model.action_dims, torchbeast_b200.action_space) takes action [T+1, B, D] and
+    runs the factored loss (tb_impala_loss_factored_f32) on every path above but UPGO and kickstarting.
+
     A batch with a legal_actions leaf (bool or uint8 [T+1, B, A], torchbeast_b200.legal_actions) learns over each
     step's legal actions on every path above: the learner's and the teacher's forwards mask their own logits, and one
     launch writes a masked copy of the behaviour logits (policy_logits[1:] or `behavior_logits`) under
@@ -533,7 +559,8 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             out.baseline[:-1], out.baseline[-1],
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
-            column_weights=None if draw is None else draw.weights, trust_region=trust_region, upgo_cost=upgo_arg)
+            column_weights=None if draw is None else draw.weights, trust_region=trust_region, upgo_cost=upgo_arg,
+            action_space=_action_space.dims_of_model(model))
         if trust_region is not None or upgo_arg is not None:
             loss, *rest = loss
             trust = rest.pop(0) if trust_region is not None else None
@@ -548,7 +575,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             _popart_task(model, batch), pop.mu, pop.nu,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region,
-            upgo_cost=upgo_arg)
+            upgo_cost=upgo_arg, action_space=_action_space.dims_of_model(model))
         loss, task_sums, *rest = res
         trust = rest.pop(0) if trust_region is not None else None
         upgo = rest.pop(0) if upgo_arg is not None else None
@@ -676,6 +703,8 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       the priority update to the same sequence (learn_step's `draw`); with PopArt it raises.
     * a legal_actions leaf (torchbeast_b200.legal_actions) is checked first, then staged, graphed and replayed like
       any other leaf; learn_step learns over each step's legal actions.
+    * a model with a factored action space (torchbeast_b200.action_space) learns on action [T+1, B, D] on every path
+      above; UPGO, kickstarting, a legal_actions leaf or a teacher with another space raise before anything is staged.
     * with flags.kickstart_cost, the teacher attached as model.teacher (torchbeast_b200.kickstart.Teacher) runs on the
       same (mixed) batch and its KL term joins the loss (learn_step); the teacher is part of the graph's structure.
     Returns the reference's stats dict."""
@@ -685,6 +714,7 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
     # usable teacher, a bare net
     _check_legal(batch)
     teacher = _teacher_for(model, actor_model, kickstart_cost(flags))
+    _action_space.check_learner(model, flags, batch, teacher_of(model))
     needs_last_action = getattr(model, "needs_last_action", False) or (
         teacher is not None and getattr(teacher.net, "needs_last_action", False))
     slot = None

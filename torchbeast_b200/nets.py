@@ -13,7 +13,7 @@ import weakref
 import torch
 from torch import nn
 
-from torchbeast_b200 import _lib
+from torchbeast_b200 import _lib, action_space
 from torchbeast_b200.legal_actions import mask_policy
 
 LearnerOutputs = collections.namedtuple("LearnerOutputs", "policy_logits baseline core_state")
@@ -83,6 +83,7 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
 
 
 ATARI_SHAPE = (4, 84, 84)
+LSTM_MAX_HIDDEN = 700  # TB_LSTM_MAX_HIDDEN
 RESNET_CHANNELS = (16, 32, 32)   # the IMPALA paper's section widths
 
 
@@ -201,13 +202,34 @@ class FlatParamModule(nn.Module):
                                            % (tuple(reward.shape[:2]), tuple(frame.shape)))
         return self.frame_history.stack(frame, inputs.get("done"), inputs.get("stream_ids"), self._flat.device)
 
+    # component sizes (A_1, ..., A_D) of a factored action space (torchbeast_b200.action_space), or None: one categorical
+    # over num_actions choices.  num_actions is the policy-logit width either way.
+    action_dims = None
+
+    def _set_action_space(self, num_actions):
+        """num_actions: an int, or a tuple of component sizes (a factored space); sets num_actions to the logit width."""
+        self.action_dims = action_space.dims_of(num_actions)
+        self.num_actions = action_space.width(num_actions)
+
     def _sample(self, logits, inputs):
-        """Training-mode action [T, B] of the reference-compatible forwards (monobeast.py:618-619).  With a sampler,
-        an optional inputs["stream_ids"] (int64 [B], e.g. actor indices) names each column's random stream."""
+        """Training-mode action [T, B] (factored: [T, B, D]) of the reference-compatible forwards
+        (monobeast.py:618-619).  With a sampler, an optional inputs["stream_ids"] (int64 [B], e.g. actor indices) names
+        each column's random stream."""
         T, B, A = logits.shape
         if self.action_sampler is not None:
+            if self.action_dims is not None:
+                return self.action_sampler.sample(logits, inputs.get("stream_ids"), action_dims=self.action_dims)
             return self.action_sampler.sample(logits, inputs.get("stream_ids"))
+        if self.action_dims is not None:
+            return action_space.multinomial(logits, self.action_dims)
         return torch.multinomial(torch.softmax(logits.detach().view(T * B, A), dim=1), num_samples=1).view(T, B)
+
+    def _greedy(self, logits):
+        """Eval-mode action: argmax over the row, or per segment of a factored space."""
+        T, B = logits.shape[:2]
+        if self.action_dims is not None:
+            return action_space.greedy(logits, self.action_dims)
+        return torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
 
     def _build_flat(self, spec, device):
         self._spec = list(spec)
@@ -386,9 +408,14 @@ class AtariNet(FlatParamModule):
             raise _lib.TorchBeastB200Error(
                 "torchbeast_b200.AtariNet is specialised for (4, 84, 84) uint8 frames, got %r" % (tuple(observation_shape),))
         self.observation_shape = tuple(observation_shape)
-        self.num_actions = num_actions
+        self._set_action_space(num_actions)
+        num_actions = self.num_actions
         self.use_lstm = use_lstm
         self.core_size = 512 + num_actions + 1
+        if self.action_dims is not None and use_lstm and self.core_size > LSTM_MAX_HIDDEN:
+            raise _lib.TorchBeastB200Error(
+                "AtariNet with an LSTM needs 512 + sum(num_actions) + 1 <= %d, got %d for num_actions=%r"
+                % (LSTM_MAX_HIDDEN, self.core_size, self.action_dims))
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
         popart = None if num_tasks is None else PopArt(num_tasks, device)
@@ -449,13 +476,20 @@ class AtariNet(FlatParamModule):
             h0 = c0 = notdone = None
         ws = self._workspace(T1, B)
         p = _lib.ptr
-        _lib.check(
-            _lib.lib().tb_atarinet_forward(
-                p(frame), p(done) if unstacked else None, p(reward), p(notdone), p(last_action), p(h0), p(c0),
+        args = (p(frame), p(done) if unstacked else None, p(reward), p(notdone), p(last_action), p(h0), p(c0),
                 p(self._flat), T1, B, self.num_actions, self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)) if unstacked else None, p(logits),
-                p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
-            "tb_atarinet_forward")
+                p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None)
+        if self.action_dims is None:
+            _lib.check(_lib.lib().tb_atarinet_forward(*args, _lib.stream_ptr()), "tb_atarinet_forward")
+        else:
+            D = len(self.action_dims)
+            if tuple(last_action.shape) != (T1, B, D):
+                raise _lib.TorchBeastB200Error("last_action must be int64 [T, B, D] = %r for num_actions=%r, got %r"
+                                               % ((T1, B, D), self.action_dims, tuple(last_action.shape)))
+            _lib.check(_lib.lib().tb_atarinet_forward_factored(*args, ctypes.byref(action_space.c_space(self.action_dims)),
+                                                               _lib.stream_ptr()),
+                       "tb_atarinet_forward_factored")
         return logits, baseline, hN, cN
 
     def _launch_backward(self, g_logits, g_baseline, notdone, grads_out, phase=3):
@@ -529,11 +563,8 @@ class AtariNet(FlatParamModule):
                                                             done)
         logits = mask_policy(logits, inputs)  # with inputs["legal_actions"]: the sampler and argmax pick legal actions
         T, B = baseline.shape[:2]
-        if self.training:
-            action = self._sample(logits, inputs)
-        else:
-            action = torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
-        out = dict(policy_logits=logits, baseline=baseline, action=action.view(T, B))
+        action = self._sample(logits, inputs) if self.training else self._greedy(logits)
+        out = dict(policy_logits=logits, baseline=baseline, action=action.view((T, B) + action.shape[2:]))
         return out, ((hN, cN) if self.use_lstm else tuple())
 
 
@@ -614,7 +645,8 @@ class ResNet(FlatParamModule):
                  observation_shape=ATARI_SHAPE, channels=RESNET_CHANNELS):
         super().__init__()
         import os
-        self.num_actions = num_actions
+        self._set_action_space(num_actions)
+        num_actions = self.num_actions
         self.use_lstm = use_lstm
         obs = tuple(int(d) for d in observation_shape)
         if len(obs) != 3 or not _lib.lib().tb_resnet_supported(*obs, *RESNET_CHANNELS, self.PRECISIONS["bf16x3"]):
@@ -745,11 +777,8 @@ class ResNet(FlatParamModule):
             logits, baseline, hN, cN, _ = self._launch_forward(frame, inputs["reward"], notdone, h0, c0, done)
         logits = mask_policy(logits, inputs)  # with inputs["legal_actions"]: the sampler and argmax pick legal actions
         T, B = baseline.shape[:2]
-        if self.training:
-            action = self._sample(logits, inputs)
-        else:
-            action = torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
-        return (action.view(T, B), logits, baseline), ((hN, cN) if self.use_lstm else tuple())
+        action = self._sample(logits, inputs) if self.training else self._greedy(logits)
+        return (action.view((T, B) + action.shape[2:]), logits, baseline), ((hN, cN) if self.use_lstm else tuple())
 
 
 Net = AtariNet

@@ -12,9 +12,11 @@ Attach a sampler to a network to use it in training-mode forwards (the eval path
 The forward then passes `inputs["stream_ids"]` (int64 [B]) to the sampler when the inputs carry it, and otherwise
 uses each row's batch column as its stream id.
 """
+import ctypes
+
 import torch
 
-from torchbeast_b200 import _lib
+from torchbeast_b200 import _lib, action_space
 
 
 class ActionSampler:
@@ -32,11 +34,15 @@ class ActionSampler:
         self.seed = int(seed)
         self.step = int(step)
 
-    def sample(self, logits, stream_ids=None):
+    def sample(self, logits, stream_ids=None, action_dims=None):
         """logits: [T, B, A] float32 CUDA tensor -> int64 [T, B] actions; advances `step` by T.
 
         Row (t, b) uses counter step + t and stream id `stream_ids[b]` (int64 [B], any device; default: the column
-        index b).  A row containing NaN, with every logit -inf, or with a +inf logit gets action -1."""
+        index b).  A row containing NaN, with every logit -inf, or with a +inf logit gets action -1.
+
+        action_dims (A_1, ..., A_D), summing to A: a factored policy (torchbeast_b200.action_space), sampled by
+        tb_sample_actions_factored_f32 into int64 [T, B, D]; component k draws from its own segment of the row, and a
+        segment with no distribution gets -1."""
         _lib.require_cuda(logits)
         if logits.dim() != 3 or logits.dtype != torch.float32:
             raise _lib.TorchBeastB200Error("logits must be float32 [T, B, A], got %s %r" % (logits.dtype, tuple(logits.shape)))
@@ -46,6 +52,10 @@ class ActionSampler:
             if tuple(stream_ids.shape) != (B,):
                 raise _lib.TorchBeastB200Error("stream_ids must have shape [B] = [%d], got %r" % (B, tuple(stream_ids.shape)))
             stream_ids = stream_ids.to(device=logits.device, dtype=torch.int64).contiguous()
+        if action_dims is not None:
+            actions = sample_factored(logits, action_dims, stream_ids, seed=self.seed, step=self.step)
+            self.step += T
+            return actions
         actions = torch.empty(T, B, dtype=torch.int64, device=logits.device)
         _lib.check(
             _lib.lib().tb_sample_actions_f32(_lib.ptr(logits), T, B, A, self.seed % 2 ** 64, self.step % 2 ** 64,
@@ -56,3 +66,18 @@ class ActionSampler:
 
     def __repr__(self):
         return "ActionSampler(seed=%d, step=%d)" % (self.seed, self.step)
+
+
+def sample_factored(logits, action_dims, stream_ids=None, seed=0, step=0, seed_step=None):
+    """tb_sample_actions_factored_f32 on contiguous float32 logits [T, B, sum(action_dims)] -> int64 [T, B, D].  The
+    (seed, step) it samples at is `seed_step` (int64 [2] on the device, read when the kernel runs: graph-capturable)
+    when given, else the host ints `seed` and `step`.  stream_ids: int64 [B] on the logits' device, or None."""
+    T, B, A = logits.shape
+    dims = action_space.dims_of(tuple(action_dims))
+    actions = torch.empty(T, B, len(dims), dtype=torch.int64, device=logits.device)
+    _lib.check(
+        _lib.lib().tb_sample_actions_factored_f32(
+            _lib.ptr(logits), T, B, A, seed % 2 ** 64, step % 2 ** 64, _lib.ptr(seed_step), _lib.ptr(stream_ids),
+            ctypes.byref(action_space.c_space(dims)), _lib.ptr(actions), _lib.stream_ptr()),
+        "tb_sample_actions_factored_f32")
+    return actions

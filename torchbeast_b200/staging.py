@@ -24,7 +24,7 @@ import threading
 
 import torch
 
-from torchbeast_b200 import _lib
+from torchbeast_b200 import _lib, action_space
 
 LEAF_ORDER = ("frame", "reward", "done", "episode_return", "episode_step", "policy_logits", "baseline", "action", "last_action")
 
@@ -35,7 +35,12 @@ FRAME_FORMATS = ("stacked", "unstacked")
 def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), extra=(), frame_format="stacked"):
     """Leaf name -> (shape, dtype) of one [T+1, B, ...] rollout batch (monobeast.py:299-316 buffers / the B2 nest).
     frame_format="unstacked": the frame leaf is [T+4, B, H, W], one newest frame per step after step 0's first three
-    channels; the learner rebuilds the stacks on the GPU (include/torchbeast_b200.h, "unstacked rollouts")."""
+    channels; the learner rebuilds the stacks on the GPU (include/torchbeast_b200.h, "unstacked rollouts").
+    num_actions a tuple (A_1, ..., A_D): a factored action space (torchbeast_b200.action_space), whose policy_logits
+    are [T+1, B, sum A_k] and whose action and last_action are [T+1, B, D]."""
+    dims = action_space.dims_of(num_actions)
+    act = (T + 1, B) if dims is None else (T + 1, B, len(dims))
+    num_actions = action_space.width(num_actions)
     if frame_format not in FRAME_FORMATS:
         raise ValueError("frame_format must be one of %s, got %r" % (FRAME_FORMATS, frame_format))
     T1 = T + 1
@@ -48,10 +53,10 @@ def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), e
         episode_step=((T1, B), torch.int32),
         policy_logits=((T1, B, num_actions), torch.float32),
         baseline=((T1, B), torch.float32),
-        action=((T1, B), torch.int64),
+        action=(act, torch.int64),
     )
     if use_last_action:
-        spec["last_action"] = ((T1, B), torch.int64)
+        spec["last_action"] = (act, torch.int64)
     for name, shape, dtype in extra:
         spec[name] = (tuple(shape), dtype)
     return spec
