@@ -131,15 +131,23 @@ def rms(x):
     return float(x.double().pow(2).mean().sqrt())
 
 
-def tolerance(K, scale, ref, rtol=2.0 ** -20, extra=None):
+def tolerance(K, scale, ref, rtol=2.0 ** -20, extra=None, lolo=True):
     """Bound on |split-bf16 result - float64 reference on the hi + lo operands| for sums of K products of RMS size
     `scale` (epilogue scale factor included).  Operands are exact as hi + lo, so the error has two sources:
       - the lo.lo product the kernels never issue: |x_lo w_lo| <= u^2 |x| |w| with u = 2^-8 per product;
       - fp32 accumulation, at most 2^-24 of the running sum per addition, taken over a chain of all K terms.
     Both add K terms of independent sign, so their spread is sqrt(K) * scale * (u^2 + 2^-24 sqrt(K)); the bound allows six
     times that, plus rtol of the magnitude of the result (and of `extra`, e.g. a residual addend) for the epilogue's
-    fp32 roundings.  An operand whose lo plane is dropped moves a result by about 2^-9 sqrt(K) scale, far outside it."""
-    tol = 6.0 * scale * K ** 0.5 * (U_BF16 ** 2 + U_F32 * K ** 0.5) + rtol * ref.abs()
+    fp32 roundings.  An operand whose lo plane is dropped moves a result by about 2^-9 sqrt(K) scale, far outside it.
+    lolo=False: single-plane bf16 operands against the float64 product of those same bf16 values.  No lo.lo term exists
+    and fp32 accumulation is the only source, so it is charged as the tensor cores do it: they add each group of 16
+    products to the running sum with truncation, not rounding (Fasi et al., "Numerical behavior of NVIDIA tensor
+    cores", PeerJ CS 2021), so each of the K/16 additions loses about 2^-24 of the sum in the same direction and the
+    losses add up instead of cancelling: (K/16) 2^-24 sqrt(K) scale, where that exceeds the rounding term (K > 256).
+    On an H100 (700 W) the rounding term alone was exceeded 1.87 times at K = 20000.  A 64-term k-block left out moves
+    a result by about 8 scale, far outside it."""
+    acc = U_F32 * (K ** 0.5 if lolo else max(K ** 0.5, K / 16.0))
+    tol = 6.0 * scale * K ** 0.5 * ((U_BF16 ** 2 if lolo else 0.0) + acc) + rtol * ref.abs()
     return tol if extra is None else tol + rtol * extra.abs()
 
 

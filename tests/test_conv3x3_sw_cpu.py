@@ -98,3 +98,16 @@ def test_tolerance_admits_split_fp32_and_rejects_a_lost_lo_product(C, O, W):
     tol = S.tolerance(9 * C, S.rms(S.value(xh, xl)) * S.rms(S.value(wh, wl)), ref)
     assert S.excess(split32, ref, tol) <= 1.0
     assert S.excess(ref - S.conv3x3(xl, wh), ref, tol) >= 10.0
+
+
+@pytest.mark.parametrize("M,N,K", [(64, 48, 64), (128, 96, 520), (32, 64, 3136), (32, 256, 20000)])
+def test_single_plane_tolerance_admits_fp32_sums_and_rejects_a_lost_k_block(M, N, K):
+    """lolo=False: bf16 operands multiplied exactly and summed in fp32 stay inside the bound; the float64 reference
+    without the products of one 64-term k-block is at least ten times outside it."""
+    g = torch.Generator().manual_seed(M + K)
+    a = torch.randn(M, K, generator=g).to(torch.bfloat16).double()
+    b = (torch.randn(N, K, generator=g) * 0.1).to(torch.bfloat16).double()
+    ref = a @ b.t()
+    tol = S.tolerance(K, S.rms(a) * S.rms(b), ref, lolo=False)
+    assert S.excess(a.float() @ b.float().t(), ref, tol) <= 1.0
+    assert S.excess(ref - a[:, :64] @ b[:, :64].t(), ref, tol) >= 10.0

@@ -69,6 +69,19 @@ def check(got, ref, ref_drop, K, scale, rtol=2.0 ** -20, extra=None):
 # the hi + lo planes of a bf16 output carry the fp32 value to 2^-16 of itself
 OUT_RTOL = 2.0 ** -16 + 2.0 ** -20
 
+# bf16 bit patterns of ReLU-mask values the input gradient must zero (NaN of either sign and a signalling one, +0, -0, a
+# negative subnormal) or keep (the smallest positive subnormal)
+MASK_EDGES = [0x7FC0, 0xFFC0, 0x7F81, 0x0000, 0x8000, 0x0001, 0x8001]
+
+
+def plant_mask_edges(act):
+    """every 6th element of the hi plane act[0] replaced by the MASK_EDGES values in turn; returns the plane in float64"""
+    edges = torch.tensor([b - (1 << 16) if b >= 1 << 15 else b for b in MASK_EDGES], dtype=torch.int16)
+    hi = act[0]
+    n = hi[::6].numel()
+    hi[::6] = edges.view(torch.bfloat16).to(hi.device).repeat(-(-n // len(MASK_EDGES)))[:n]
+    return hi.double()
+
 
 @pytest.mark.parametrize("H,W,C,K,S_,O", CONVS)
 @pytest.mark.parametrize("N", FRAMES)
@@ -95,11 +108,13 @@ def test_forward(H, W, C, K, S_, O, N):
 @pytest.mark.parametrize("H,W,C,K,S_,O", CONVS)
 @pytest.mark.parametrize("N", FRAMES)
 def test_input_gradient(H, W, C, K, S_, O, N):
-    """Stride 2 (conv2) runs the parity-class path, stride 1 (conv3) the plain one; the ReLU mask is the act hi plane."""
+    """Stride 2 (conv2) runs the parity-class path, stride 1 (conv3) the plain one; the ReLU mask is the act hi plane,
+    which holds NaN of both signs, +-0 and subnormals (MASK_EDGES): an element is kept exactly where the mask is > 0."""
     L, p = _lib(), _lib().ptr
     g = torch.Generator(device="cuda").manual_seed(5 * N + H)
     OH = (H - K) // S_ + 1
-    act, a_lo, _, ah, _ = planes(torch.randn(N, H, W, C, device="cuda", generator=g))
+    act, a_lo, _, _, _ = planes(torch.randn(N, H, W, C, device="cuda", generator=g))
+    ah = plant_mask_edges(act)
     dy, d_lo, dv, dh, dl = planes(torch.randn(N, OH, OH, O, device="cuda", generator=g))
     w = torch.randn(O, C, K, K, device="cuda", generator=g) * 0.1
     dx = nan(2 * N * H * W * C, torch.bfloat16).view(2, -1)

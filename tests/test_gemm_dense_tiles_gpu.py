@@ -2,16 +2,19 @@
 
 Each case below makes gemm_block_n pick the BLOCK_N given with it (restated in `block_n`, checked first so that a
 change of the rule shows up here rather than as a silently lost case).  Products are checked against float64 torch on the
-hi + lo operand values; the tolerance, 2e-4 * sqrt(K), is ten times below what single-plane bf16 operands reach, so it
-also tells whether the lo planes took part.  Tile widths must not change any sum: rows computed inside a 2592-row call
+hi + lo operand values within tests/sw_image.py's tolerance, and the reference without the lo(A) . hi(B) product must lie
+at least ten times outside it, so the bound also tells whether the lo planes took part.  Tile widths must not change any sum: rows computed inside a 2592-row call
 are compared bit for bit with the same rows computed by a short call that picks another width.  Last, the standalone
 split-bf16 LSTM at AtariNet's shape (B = 32, H = 519, 81 steps: its projections and weight gradients are the 2592-row
 GEMMs of the learner step) against float64 torch.nn.LSTM."""
 import ctypes
+from collections import namedtuple
 
 import numpy as np
 import pytest
 import torch
+
+from tests import sw_image as S
 
 pytestmark = pytest.mark.gpu
 
@@ -28,13 +31,16 @@ def block_n(M, N, splits, b_mn):
 
 
 def planes(x, ld):
-    """fp32 [rows, cols] -> bf16 [2, rows, ld] (hi plane, lo plane, zero columns past cols), lo offset, fp64 value."""
+    """fp32 [rows, cols] -> bf16 [2, rows, ld] (hi plane, lo plane, zero columns past cols), lo offset, fp64 hi, fp64 lo."""
     rows, cols = x.shape
     buf = torch.zeros(2, rows, ld, dtype=torch.bfloat16, device="cuda")
-    hi = x.to(torch.bfloat16)
-    lo = (x - hi.float()).to(torch.bfloat16)
+    hi, lo = S.split(x)
     buf[0, :, :cols], buf[1, :, :cols] = hi, lo
-    return buf, rows * ld, hi.double() + lo.double()
+    return buf, rows * ld, hi.double(), lo.double()
+
+
+# float64 result, the same without the lo(A) . hi(B) product, the RMS product size and the bias (sw_image.tolerance)
+Ref = namedtuple("Ref", "value dropped_lo scale extra")
 
 
 def rup8(n):
@@ -54,18 +60,24 @@ def gemm(M, N, K, layout, splits, epi, seed=0, gen_m=None):
     Ax = (Ax[:, :M] if a_mn else Ax[:M]).contiguous()
     Bx = torch.randn((K, N) if b_mn else (N, K), device="cuda", generator=g)
     lda, ldb = rup8(Ax.shape[1]), rup8(Bx.shape[1])
-    Ab, a_lo, A64 = planes(Ax, lda)
-    Bb, b_lo, B64 = planes(Bx, ldb)
-    ref = (A64.t() if a_mn else A64) @ (B64 if b_mn else B64.t())
+    Ab, a_lo, Ah, Al = planes(Ax, lda)
+    Bb, b_lo, Bh, Bl = planes(Bx, ldb)
+    mat = lambda a, b: (a.t() if a_mn else a) @ (b if b_mn else b.t())
+    acc, acc_drop = mat(Ah + Al, Bh + Bl), mat(Ah, Bh + Bl) + mat(Al, Bl)
     scale, bias, relu, mask = 1.0, None, 0, None
     if epi >= 1:
         scale, relu = 0.75, 1
         bias = torch.randn(N, device="cuda", generator=g)
-        ref = torch.relu(ref * scale + bias.double())
     if epi == 2:
         mask = torch.zeros(M, rup8(N), dtype=torch.bfloat16, device="cuda")
         mask[:, :N] = torch.randn(gm, N, device="cuda", generator=g)[:M].to(torch.bfloat16)
-        ref = torch.where(mask[:, :N].double() > 0, ref, torch.zeros_like(ref))
+
+    def epilogue(x):
+        if epi >= 1:
+            x = torch.relu(x * scale + bias.double())
+        return torch.where(mask[:, :N].double() > 0, x, torch.zeros_like(x)) if epi == 2 else x
+    ref = Ref(epilogue(acc), epilogue(acc_drop), S.rms(Ah + Al) * S.rms(Bh + Bl) * scale,
+              bias.double() if bias is not None else None)
     C = torch.full((M, N), float("nan"), device="cuda")
     C16 = torch.zeros(2, M, rup8(N), dtype=torch.bfloat16, device="cuda") if epi >= 1 and splits == 1 else None
     part = torch.empty(splits * M * ((N + 31) // 32 * 32), device="cuda") if splits > 1 else None
@@ -98,11 +110,15 @@ CASES = [
 def test_split_gemm_every_tile_vs_fp64(M, N, K, layout, splits, epi, bn):
     assert block_n(M, N, splits, layout != "kk") == bn
     C, C16, ref = gemm(M, N, K, layout, splits, epi)
-    tol = 2e-4 * np.sqrt(K)
+    tol = S.tolerance(K, ref.scale, ref.value, extra=ref.extra)
     assert torch.isfinite(C).all()
-    torch.testing.assert_close(C.double(), ref, rtol=1e-5, atol=tol)
-    if C16 is not None:  # hi + lo planes of the bf16 output carry the fp32 value to ~2^-17
-        torch.testing.assert_close(C16[0, :, :N].double() + C16[1, :, :N].double(), ref, rtol=1e-5, atol=tol)
+    err, miss = S.excess(C, ref.value, tol), S.excess(ref.dropped_lo, ref.value, tol)
+    assert err <= 1.0, "max |err| / tol = %.3g" % err
+    assert miss >= 10.0, "the reference without a lo product is only %.3g x the tolerance" % miss
+    if C16 is not None:  # hi + lo planes of the bf16 output carry the fp32 value to 2^-16 of itself
+        tol16 = S.tolerance(K, ref.scale, ref.value, rtol=2.0 ** -16 + 2.0 ** -20, extra=ref.extra)
+        err16 = S.excess(S.value(C16[0, :, :N], C16[1, :, :N]), ref.value, tol16)
+        assert err16 <= 1.0, "bf16 planes: max |err| / tol = %.3g" % err16
 
 
 @pytest.mark.parametrize("N,K,layout,epi", [(519, 520, "kk", 1), (519, 2076, "km", 2), (512, 3136, "kk", 0)])

@@ -1,9 +1,10 @@
-"""GPU: the wgmma/TMA bf16 GEMM against a plain PyTorch fp32 reference of the same op
-(inputs rounded to bf16 first, so products are exact and only the fp32 accumulation order differs:
-tolerance rtol 1e-4 / atol 1e-4 x sqrt(K))."""
-import numpy as np
+"""GPU: the wgmma/TMA bf16 GEMM against float64 on the same bf16 operand values.  Products of bf16 values are exact, so
+fp32 accumulation is the only source of error: tests/sw_image.py's tolerance with lolo=False bounds it, and every case
+checks that the reference with one 64-term k-block left out lies at least ten times outside that bound."""
 import pytest
 import torch
+
+from tests import sw_image as S
 
 pytestmark = pytest.mark.gpu
 
@@ -25,29 +26,39 @@ def run(M, N, K, bias, relu, scale, want16):
     rc = _lib.lib().tb_gemm_bf16_tn(p(A), p(B), M, N, K, K, K, p(C), N, p(C16), N, p(bvec), scale, int(relu), _lib.stream_ptr())
     _lib.check(rc, "tb_gemm_bf16_tn")
     torch.cuda.synchronize()
-    ref = (A.float() @ B.float().t()) * scale
-    if bias:
-        ref = ref + bvec
-    if relu:
-        ref = ref.clamp(min=0)
-    return C, C16, ref
+    check(C, A.double(), B.double(), scale, bvec, relu)
+    return C, C16
+
+
+def check(C, A64, B64, scale=1.0, bias=None, relu=False):
+    """C against float64 A64 [M, K] . B64 [N, K]^T through the epilogue, within the single-plane bound; the reference
+    without the first k-block's 64 products is at least ten times outside it"""
+    def epilogue(acc):
+        out = acc * scale + (bias.double() if bias is not None else 0.0)
+        return out.clamp(min=0) if relu else out
+    K = A64.shape[1]
+    ref = epilogue(A64 @ B64.t())
+    tol = S.tolerance(K, S.rms(A64) * S.rms(B64) * scale, ref, extra=bias.double() if bias is not None else None,
+                      lolo=False)
+    assert torch.isfinite(C).all()
+    err = S.excess(C, ref, tol)
+    assert err <= 1.0, "max |err| / tol = %.3g" % err
+    miss = S.excess(epilogue(A64 @ B64.t() - A64[:, :64] @ B64[:, :64].t()), ref, tol)
+    assert miss >= 10.0, "the reference without a k-block is only %.3g x the tolerance" % miss
 
 
 @pytest.mark.parametrize("M,N,K", SHAPES)
 def test_gemm_tc_matches_fp32_reference(M, N, K):
     if K % 8:
         pytest.skip("ld must be a multiple of 8")
-    C, _, ref = run(M, N, K, bias=False, relu=False, scale=1.0, want16=False)
-    tol = 1e-4 * np.sqrt(K)
-    assert torch.isfinite(C).all()
-    torch.testing.assert_close(C, ref, rtol=1e-4, atol=tol)
+    run(M, N, K, bias=False, relu=False, scale=1.0, want16=False)
 
 
 @pytest.mark.parametrize("M,N,K", [(300, 64, 512), (2592, 512, 3136), (1000, 32, 256)])
 def test_gemm_tc_epilogue(M, N, K):
-    C, C16, ref = run(M, N, K, bias=True, relu=True, scale=1.0 / 255.0, want16=True)
-    torch.testing.assert_close(C, ref, rtol=1e-4, atol=1e-4 * np.sqrt(K))
-    torch.testing.assert_close(C16.float(), ref, rtol=1e-2, atol=1e-2)
+    """the bf16 output is the round-to-nearest-even of the fp32 one, bit for bit"""
+    C, C16 = run(M, N, K, bias=True, relu=True, scale=1.0 / 255.0, want16=True)
+    assert torch.equal(C16.view(torch.int16), C.to(torch.bfloat16).view(torch.int16))
 
 
 def test_f32_to_bf16_padding():
@@ -80,5 +91,4 @@ def test_gemm_tc_mn_major_operands(M, N, K, mode):
     rc = _lib.lib().tb_gemm_bf16_ex(p(A), p(B), M, N, K, A.shape[1], N, int(a_mn), 1, p(C), N, splits, p(part), _lib.stream_ptr())
     _lib.check(rc, "tb_gemm_bf16_ex")
     torch.cuda.synchronize()
-    ref = (A.float().t() if a_mn else A.float()) @ B.float()
-    torch.testing.assert_close(C, ref, rtol=1e-4, atol=1e-4 * np.sqrt(K))
+    check(C, A.double().t() if a_mn else A.double(), B.double().t())

@@ -306,12 +306,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 }
               }
             }
-            if (vm) {  // a bf16 is positive iff its bit pattern, read as a signed 16-bit integer, is > 0
+            if (vm) {  // a bf16 is > 0 iff its bit pattern is in (0, 0x7f80]: +subnormal .. +inf, no NaN
 #pragma unroll
               for (int j = 0; j < 32; j += 2) {
                 const uint32_t m = m16[j >> 1];
-                o[j] = (int(m << 16) > 0) ? o[j] : 0.0f;
-                o[j + 1] = (int(m & 0xffff0000u) > 0) ? o[j + 1] : 0.0f;
+                o[j] = ((m & 0xffffu) - 1u < 0x7f80u) ? o[j] : 0.0f;
+                o[j + 1] = ((m >> 16) - 1u < 0x7f80u) ? o[j + 1] : 0.0f;
               }
             } else if (ep.mask16) {
 #pragma unroll
@@ -628,7 +628,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (EPI >= 2 && ep.mask16) {
             const __nv_bfloat16* mp = ep.mask16 + pr * ep.ldmask + pc;
             if (full_cols && (ep.ldmask & 7) == 0 && (reinterpret_cast<uintptr_t>(mp) & 15) == 0) {
-              // a bf16 is positive iff its bit pattern, read as a signed 16-bit integer, is > 0
+              // a bf16 is > 0 iff its bit pattern is in (0, 0x7f80]: +subnormal .. +inf, no NaN
 #pragma unroll
               for (int q = 0; q < 4; ++q) {
                 const uint4 t = __ldg(reinterpret_cast<const uint4*>(mp) + q);
@@ -636,8 +636,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                   const int j = 8 * q + 2 * e;
-                  o[j] = (int(m[e] << 16) > 0) ? o[j] : 0.0f;
-                  o[j + 1] = (int(m[e] & 0xffff0000u) > 0) ? o[j + 1] : 0.0f;
+                  o[j] = ((m[e] & 0xffffu) - 1u < 0x7f80u) ? o[j] : 0.0f;
+                  o[j + 1] = ((m[e] >> 16) - 1u < 0x7f80u) ? o[j + 1] : 0.0f;
                 }
               }
             } else {
