@@ -295,6 +295,49 @@ int tb_sample_actions_factored_f32(const float* logits, int64_t T, int64_t B, in
                                    const uint64_t* seed_step, const int64_t* stream_ids, const tb_action_space* space,
                                    int64_t* actions, void* stream);
 
+/* ---- continuous (diagonal-Gaussian) action spaces -------------------------------------------------------------------
+ * An action is a real vector a of D dimensions, 1 <= D <= TB_MAX_CONTINUOUS_DIM, drawn from a diagonal Gaussian:
+ *   policy row [.., A], A = 2D: columns [0, D) are the mean mu, columns [D, 2D) the log standard deviation l, taken as
+ *     the head outputs it (no clamp, no squash), sigma = exp(l).  A Gaussian head is a policy layer of width 2D.
+ *   rollout leaves: policy_logits keeps its name and holds the actor's (mu, l) rows [T+1,B,2D]; action and last_action
+ *     are float32 [.., D].  The action is the unclipped sample: an actor clips it to the environment's bounds itself,
+ *     before stepping the environment, and stores the unclipped value.
+ * Per row, with z_k = (a_k - mu_k) * exp(-l_k) and c = TB_GAUSSIAN_HALF_LOG_2PI (0.5 log 2 pi, one fp32 constant),
+ * each quantity is an fp32 sum over k in index order that starts from the k = 0 term:
+ *   log pi(a) = sum_k (-0.5 z_k^2 - l_k - c);
+ *   entropy term (the sign the flat loss uses for sum p log p): ent = sum_k -(l_k + 0.5 + c);
+ *   trust-region KL(pi || mu_b) = sum_k ((lb_k - l_k) + 0.5 (exp(2 (l_k - lb_k)) + ((mu_k - mub_k) exp(-lb_k))^2) - 0.5);
+ *   gradient of mu_k: -adv * z_k * exp(-l_k); gradient of l_k: adv * (1 - z_k^2) - entropy_cost; both multiplied by
+ *     the column weight where the flat loss applies one.
+ * A NaN or +-inf mu, l or action entry gives NaN for its row: log pi(a), the entropy term and the whole gradient row of a
+ * row with one, and the KL of a pair of rows with one (the flat loss's "poison the row" convention).                */
+#define TB_MAX_CONTINUOUS_DIM 64
+#define TB_GAUSSIAN_HALF_LOG_2PI 0.918938533204672742f
+/* tb_impala_loss_f32 on a Gaussian policy: the same arguments and outputs (hp block, column_weights, PopArt, trust
+ * region, single-launch and split-T layouts), with actions float32 [T,B,D] and the rules above in place of the flat
+ * row's.  A must be 2D with 1 <= D <= TB_MAX_CONTINUOUS_DIM (an odd A is rejected).  V-trace runs on
+ * log rho = log pi(a) - log mu(a); the pg loss is -log pi(a) * pg_adv; target_alp / behavior_alp are the Gaussian
+ * log-densities.  tb_upgo_loss_f32 and tb_kickstart_loss_f32 take categorical rows only.                            */
+int tb_impala_loss_gaussian_f32(const float* behavior_logits, const float* target_logits, const float* actions,
+                                const float* rewards, const uint8_t* done, const float* discounts, const float* values,
+                                const float* bootstrap, int64_t T, int64_t B, int64_t A, float discounting,
+                                float baseline_cost, float entropy_cost, int clip_rewards, float clip_rho,
+                                float clip_pg_rho, const tb_hparams* hp, const float* column_weights,
+                                const int64_t* task, const double* mu, const double* nu, int64_t K, double* task_sums,
+                                const float* trust_beta, float* kl_out, float* trust_out, float* vs, float* pg_adv,
+                                float* log_rhos, float* behavior_alp, float* target_alp, float* losses_out,
+                                float* grad_logits, float* grad_values, int zero_tail, void* workspace, void* stream);
+/* Seeded sampling of a Gaussian policy: rows [T,B,A = 2D] -> actions float32 [T,B,D].  Component k of row (t,b) takes
+ * the Philox4x32-10 block with tb_sample_actions_f32's counter (step + t, stream id) and key (lo32(seed),
+ * hi32(seed) + k/2) (mod 2^32), and its words x0, x1 = words 2 (k mod 2) and 2 (k mod 2) + 1.  Then
+ *   u1 = ((x0 >> 8) + 1) * 2^-24 in (0, 1], u2 = (x1 >> 8) * 2^-24;
+ *   z = sqrtf(-2 logf(u1)) * cospif(2 u2);  a_k = mu_k + expf(l_k) * z;
+ * a non-finite mu_k or l_k gives NaN for a_k.  The greedy (eval-mode) action is mu.  seed_step (device, nullable) wins
+ * over (seed, step), as in tb_sample_actions_factored_f32, so one entry serves eager and graphed acting.  Sizes:
+ * T, B >= 0 (T*B == 0 is a no-op success), A = 2D as in the loss.                                                  */
+int tb_sample_gaussian_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
+                           const uint64_t* seed_step, const int64_t* stream_ids, float* actions, void* stream);
+
 /* ---- legal-action masks ("invalid action masking": the policy renormalised over each step's legal actions) ---------
  * A rollout may carry a leaf legal_actions bool / uint8 [T+1,B,A], nonzero = legal, indexed like frame: row t holds the
  * actions legal at frame t (an env output, stored beside the frame it came with).  Behaviour logits row t+1 and action
@@ -476,6 +519,23 @@ int tb_atarinet_forward_factored(const uint8_t* frame, const uint8_t* done, cons
 int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
                          const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
                          int precision, void* workspace, float* grads, int phase, void* stream);
+/* AtariNet with a continuous action space (see "continuous (diagonal-Gaussian) action spaces"): num_actions = 2D is the
+ * policy layer's width, and the core input is 512 + D + 1 wide, F = 512 + D + 1 in place of 519 above: column 512 holds
+ * the clipped reward and columns 513 .. 512 + D hold last_action[n, k] (float32 [T1,B,D]) as it is.  The parameters are
+ * the layout above with that F (the LSTM 4F x F, policy.weight (2D, F)), counted by tb_atarinet_param_count_continuous;
+ * the workspace is tb_atarinet_workspace_bytes_continuous bytes; tb_atarinet_grad_split holds unchanged.  The forward
+ * and the backward are tb_atarinet_forward / tb_atarinet_backward on that layout; last_action gets no gradient.  An odd
+ * num_actions, or D > TB_MAX_CONTINUOUS_DIM, is rejected; the heads take at most 31 outputs, so D <= 15 here.        */
+int64_t tb_atarinet_param_count_continuous(int num_actions, int num_values, int use_lstm);
+size_t tb_atarinet_workspace_bytes_continuous(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision);
+int tb_atarinet_forward_continuous(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                                   const float* last_action, const float* h0, const float* c0, const float* params,
+                                   int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                   void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                   float* hN, float* cN, void* stream);
+int tb_atarinet_backward_continuous(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                                    const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                    int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream);
 
 /* ---- stacked LSTM over the unroll with per-step done-reset -------------------------------------------
  * Replaces the reference's loop of seq_len-1 nn.LSTM calls and its autograd graph (monobeast.py:603-611,

@@ -35,6 +35,9 @@ _SIGNATURES = {
         [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 5 + [_i64] + [_vp] * 12
         + [_int, _vp, _vp, _vp], _int),
     "tb_action_space_layout": ([_vp], _int),
+    "tb_impala_loss_gaussian_f32": (
+        [_vp] * 8 + [_i64, _i64, _i64, _f32, _f32, _f32, _int, _f32, _f32] + [_vp] * 5 + [_i64] + [_vp] * 12
+        + [_int, _vp, _vp], _int),
     "tb_upgo_loss_f32": ([_vp] * 7 + [_i64, _i64, _i64, _f32, _int, _f32] + [_vp] * 5 + [_i64] + [_vp] * 10, _int),
     "tb_kickstart_loss_f32": ([_vp, _vp, _i64, _i64, _i64] + [_vp] * 7, _int),
     "tb_popart_update": ([_vp] * 4 + [_i64, _vp, _vp, _i64, _vp], _int),
@@ -44,6 +47,10 @@ _SIGNATURES = {
     "tb_atarinet_forward": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
     "tb_atarinet_forward_factored": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 8, _int),
     "tb_atarinet_backward": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
+    "tb_atarinet_param_count_continuous": ([_int, _int, _int], _i64),
+    "tb_atarinet_workspace_bytes_continuous": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
+    "tb_atarinet_forward_continuous": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
+    "tb_atarinet_backward_continuous": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
     "tb_resnet_obs_range": ([_vp], _int),
     "tb_resnet_widths": ([_vp], _int),
     "tb_resnet_supported": ([_int] * 7, _int),
@@ -54,6 +61,7 @@ _SIGNATURES = {
     "tb_sample_actions_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64, _vp, _vp, _vp], _int),
     "tb_sample_actions_dev_f32": ([_vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp], _int),
     "tb_sample_actions_factored_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64] + [_vp] * 5, _int),
+    "tb_sample_gaussian_f32": ([_vp, _i64, _i64, _i64, _c.c_uint64, _c.c_uint64] + [_vp] * 4, _int),
     "tb_mask_logits_f32": ([_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp], _int),
     "tb_replay_mix": ([_vp, _int, _i64, _i64, _i64, _vp, _vp, _i64, _vp, _vp], _int),
     "tb_replay_advance": ([_vp, _vp, _i64, _i64, _vp], _int),

@@ -179,13 +179,15 @@ class _DeviceStepSampler:
     def __init__(self, seed_step):
         self.seed_step = seed_step
 
-    def sample(self, logits, stream_ids=None, action_dims=None):
+    def sample(self, logits, stream_ids=None, action_dims=None, continuous_dim=None):
         T, B, A = logits.shape
         logits = logits.detach().contiguous()
         if stream_ids is not None:
             stream_ids = stream_ids.to(device=logits.device, dtype=torch.int64).contiguous()
         if action_dims is not None:  # a factored policy: one entry reads seed_step the same way
             return sampling.sample_factored(logits, action_dims, stream_ids, seed_step=self.seed_step)
+        if continuous_dim is not None:  # a Gaussian policy: likewise
+            return sampling.sample_gaussian(logits, continuous_dim, stream_ids, seed_step=self.seed_step)
         actions = torch.empty(T, B, dtype=torch.int64, device=logits.device)
         _lib.check(
             _lib.lib().tb_sample_actions_dev_f32(_lib.ptr(logits), T, B, A, _lib.ptr(self.seed_step),

@@ -51,15 +51,17 @@ struct AtariParams {  // offsets (in floats) into the flat parameter / gradient 
   int64_t conv1_w, conv1_b, conv2_w, conv2_b, conv3_w, conv3_b, fc_w, fc_b;
   int64_t lstm[2][4];  // per layer: w_ih, w_hh, b_ih, b_hh
   int64_t policy_w, policy_b, baseline_w, baseline_b, total;
-  int core;  // 512 + 1 + A
+  int core;  // 512 + 1 + A (a continuous space: 512 + 1 + D)
 };
 
-static AtariParams atari_params(int A, int use_lstm, int V = 1) {  // V: value outputs
+// V: value outputs.  Dc > 0: a continuous action space of Dc dimensions, whose core takes Dc last-action columns while
+// the policy layer stays A = 2 Dc wide; 0: the core takes A columns.
+static AtariParams atari_params(int A, int use_lstm, int V = 1, int Dc = 0) {
   using G = AtariGeom;
   AtariParams p;
   int64_t o = 0;
   auto take = [&](int64_t n) { int64_t r = o; o += n; return r; };
-  p.core = G::FC_OUT + 1 + A;
+  p.core = G::FC_OUT + 1 + (Dc ? Dc : A);
   p.conv1_w = take(int64_t(G::C1) * G::KD1); p.conv1_b = take(G::C1);
   p.conv2_w = take(int64_t(G::C2) * G::KD2); p.conv2_b = take(G::C2);
   p.conv3_w = take(int64_t(G::C3) * G::KD3); p.conv3_b = take(G::C3);
@@ -98,7 +100,7 @@ struct AtariWs {  // bump-carved view of the caller's workspace
   size_t bytes;
 };
 
-static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int use_lstm, int precision) {
+static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int use_lstm, int precision, int Dc = 0) {
   using G = AtariGeom;
   AtariWs w;
   size_t off = 0;
@@ -107,7 +109,7 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
     off += (nbytes + 255) & ~size_t(255);
     return p;
   };
-  const AtariParams pp = atari_params(A, use_lstm);
+  const AtariParams pp = atari_params(A, use_lstm, 1, Dc);
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   auto takef = [&](int64_t n) { return static_cast<float*>(take(size_t(n) * sizeof(float))); };
   const bool split = precision == 2;
@@ -161,15 +163,18 @@ static AtariWs atari_ws(void* base, int64_t N, int64_t T1, int64_t B, int A, int
 // done == nullptr: frame is stacked u8 [T1,B,4,84,84]; otherwise frame is an unstacked rollout u8 [T1+3,B,84,84] whose stacks
 // the tensor-core backends rebuild in their frame-image pass (the fp32 backend is handed restacked frames by its caller).
 // seg non-NULL: a factored action space, last_action [T1,B,D] enters the core as a K-hot (core_extras).
+// clast_action non-NULL (last_action then NULL): a continuous space of A / 2 dimensions, whose float32 [T1,B,A/2] last
+// actions enter the core as they are (core_extras_continuous).
 static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                             const int64_t* last_action, const float* h0, const float* c0, const float* P,
                             int64_t T1, int64_t B, int A, int use_lstm, int precision, void* workspace,
                             float* policy_logits, float* baseline, float* hN, float* cN, cudaStream_t st, int V = 1,
-                            const ActionSegments* seg = nullptr) {
+                            const ActionSegments* seg = nullptr, const float* clast_action = nullptr) {
   using G = AtariGeom;
   const int64_t N = T1 * B;
-  const AtariParams pp = atari_params(A, use_lstm, V);
-  AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision);
+  const int Dc = clast_action ? A / 2 : 0;
+  const AtariParams pp = atari_params(A, use_lstm, V, Dc);
+  AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision, Dc);
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
   if (precision) {
@@ -226,7 +231,10 @@ static int atarinet_forward(const uint8_t* frame, const uint8_t* done, const flo
   TB_TRY((gemm_simt<float, float, false, true>(w.act3, w.wfcp, w.core_in, N, G::FC_OUT, G::FC_IN, G::FC_IN, G::FC_IN,
                                                 pp.core, ep, 1, nullptr, st)));
   }
-  TB_TRY(core_extras(w.core_in, pp.core, N, G::FC_OUT, reward, last_action, A, st, seg));
+  if (clast_action)
+    TB_TRY(core_extras_continuous(w.core_in, pp.core, N, G::FC_OUT, reward, clast_action, Dc, st));
+  else
+    TB_TRY(core_extras(w.core_in, pp.core, N, G::FC_OUT, reward, last_action, A, st, seg));
   if (use_lstm) {
     LstmParams lp;
     for (int l = 0; l < 2; ++l) {
@@ -331,11 +339,11 @@ static int atarinet_backward_trunk_bf16(const float* P, float* G_, const AtariPa
 // LSTM + heads slice (17 of 24 MB) while the trunk backward is still running (SURVEY 8(e) G1: bucket order = reverse of forward).
 static int atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
                              const float* P, int64_t T1, int64_t B, int A, int use_lstm, int precision,
-                             void* workspace, float* G_, cudaStream_t st, int phases = 3, int V = 1) {
+                             void* workspace, float* G_, cudaStream_t st, int phases = 3, int V = 1, int Dc = 0) {
   using G = AtariGeom;
   const int64_t N = T1 * B;
-  const AtariParams pp = atari_params(A, use_lstm, V);
-  AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision);
+  const AtariParams pp = atari_params(A, use_lstm, V, Dc);
+  AtariWs w = atari_ws(workspace, N, T1, B, A, use_lstm, precision, Dc);
   const int64_t M1 = N * G::H1 * G::W1, M2 = N * G::H2 * G::W2, M3 = N * G::H3 * G::W3;
   GemmEpilogue ep;
   if (phases & 1) {
@@ -416,17 +424,26 @@ size_t tb_atarinet_workspace_bytes(int64_t T1, int64_t B, int num_actions, int u
   return atari_ws(nullptr, T1 * B, T1, B, num_actions, use_lstm, precision).bytes;
 }
 
-// tb_atarinet_forward and, with seg non-NULL, tb_atarinet_forward_factored
+// num_actions = 2D with 1 <= D <= TB_MAX_CONTINUOUS_DIM: the width of a continuous space's policy layer
+static int continuous_width_ok(int num_actions, const char* who) {
+  TB_REQUIRE(num_actions >= 2 && num_actions % 2 == 0 && num_actions / 2 <= TB_MAX_CONTINUOUS_DIM,
+             "%s: num_actions = %d must be 2D with 1 <= D <= %d", who, num_actions, TB_MAX_CONTINUOUS_DIM);
+  return 0;
+}
+
+// tb_atarinet_forward, with seg non-NULL tb_atarinet_forward_factored, and with clast_action non-NULL (last_action then
+// NULL) tb_atarinet_forward_continuous
 static int atarinet_forward_entry(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
                                   const int64_t* last_action, const float* h0, const float* c0, const float* params,
                                   int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
                                   void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
-                                  float* hN, float* cN, void* stream, const ActionSegments* seg) {
+                                  float* hN, float* cN, void* stream, const ActionSegments* seg,
+                                  const float* clast_action = nullptr) {
   TB_REQUIRE(num_values >= 1 && num_values <= kHeadsMaxValues, "atarinet_forward: num_values %d outside [1, %d]",
              num_values, kHeadsMaxValues);
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1, "atarinet_forward: bad sizes T1=%lld B=%lld A=%d", (long long)T1,
              (long long)B, num_actions);
-  TB_REQUIRE(frame && reward && last_action && params && workspace && policy_logits && baseline,
+  TB_REQUIRE(frame && reward && (last_action || clast_action) && params && workspace && policy_logits && baseline,
              "atarinet_forward: null pointer");
   TB_REQUIRE(!use_lstm || (notdone && h0 && c0 && hN && cN), "atarinet_forward: LSTM needs notdone/h0/c0/hN/cN");
   TB_REQUIRE(precision >= 0 && precision <= 2,
@@ -442,7 +459,7 @@ static int atarinet_forward_entry(const uint8_t* frame, const uint8_t* done, con
     done = nullptr;
   }
   return atarinet_forward(frame, done, reward, notdone, last_action, h0, c0, params, T1, B, num_actions, use_lstm, precision,
-                          workspace, policy_logits, baseline, hN, cN, st, num_values, seg);
+                          workspace, policy_logits, baseline, hN, cN, st, num_values, seg, clast_action);
 }
 
 int tb_atarinet_forward(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
@@ -467,9 +484,11 @@ int tb_atarinet_forward_factored(const uint8_t* frame, const uint8_t* done, cons
                                 cN, stream, &seg);
 }
 
-int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
-                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
-                         int precision, void* workspace, float* grads, int phase, void* stream) {
+// tb_atarinet_backward and, with Dc > 0, tb_atarinet_backward_continuous
+static int atarinet_backward_entry(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                                   const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                   int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream,
+                                   int Dc) {
   TB_REQUIRE(T1 >= 1 && B >= 1 && num_actions >= 1 && num_values >= 1 && num_values <= kHeadsMaxValues,
              "atarinet_backward: bad sizes");
   TB_REQUIRE(grad_logits && grad_baseline && params && workspace && grads, "atarinet_backward: null pointer");
@@ -478,7 +497,44 @@ int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, c
   TB_REQUIRE(phase >= 1 && phase <= 3,
              "atarinet_backward: phase must be 1 (heads + LSTM), 2 (conv/fc trunk) or 3 (the whole backward)");
   return atarinet_backward(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, use_lstm, precision, workspace,
-                           grads, (cudaStream_t)stream, phase, num_values);
+                           grads, (cudaStream_t)stream, phase, num_values, Dc);
+}
+
+int tb_atarinet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                         const float* params, int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm,
+                         int precision, void* workspace, float* grads, int phase, void* stream) {
+  return atarinet_backward_entry(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, num_values, use_lstm,
+                                 precision, workspace, grads, phase, stream, 0);
+}
+
+int64_t tb_atarinet_param_count_continuous(int num_actions, int num_values, int use_lstm) {
+  if (continuous_width_ok(num_actions, "atarinet_param_count_continuous")) return -1;
+  return atari_params(num_actions, use_lstm, num_values, num_actions / 2).total;
+}
+
+size_t tb_atarinet_workspace_bytes_continuous(int64_t T1, int64_t B, int num_actions, int use_lstm, int precision) {
+  if (continuous_width_ok(num_actions, "atarinet_workspace_bytes_continuous")) return 0;
+  return atari_ws(nullptr, T1 * B, T1, B, num_actions, use_lstm, precision, num_actions / 2).bytes;
+}
+
+int tb_atarinet_forward_continuous(const uint8_t* frame, const uint8_t* done, const float* reward, const float* notdone,
+                                   const float* last_action, const float* h0, const float* c0, const float* params,
+                                   int64_t T1, int64_t B, int num_actions, int num_values, int use_lstm, int precision,
+                                   void* workspace, void* stacked_scratch, float* policy_logits, float* baseline,
+                                   float* hN, float* cN, void* stream) {
+  TB_TRY(continuous_width_ok(num_actions, "atarinet_forward_continuous"));
+  TB_REQUIRE(last_action, "atarinet_forward_continuous: null last_action");
+  return atarinet_forward_entry(frame, done, reward, notdone, nullptr, h0, c0, params, T1, B, num_actions, num_values,
+                                use_lstm, precision, workspace, stacked_scratch, policy_logits, baseline, hN, cN, stream,
+                                nullptr, last_action);
+}
+
+int tb_atarinet_backward_continuous(const float* grad_logits, const float* grad_baseline, const float* notdone,
+                                    const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
+                                    int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream) {
+  TB_TRY(continuous_width_ok(num_actions, "atarinet_backward_continuous"));
+  return atarinet_backward_entry(grad_logits, grad_baseline, notdone, params, T1, B, num_actions, num_values, use_lstm,
+                                 precision, workspace, grads, phase, stream, num_actions / 2);
 }
 
 }  // extern "C"

@@ -259,6 +259,27 @@ __global__ void core_extras_factored_kernel(float* __restrict__ core, int64_t ld
   }
 }
 
+// The continuous form: core[n, F] = clamp(reward[n], -1, 1), core[n, F+1+k] = last_action[n, k] as it is.
+__global__ void core_extras_continuous_kernel(float* __restrict__ core, int64_t ld, int64_t N, int F,
+                                              const float* __restrict__ reward, const float* __restrict__ last_action,
+                                              int D) {
+  const int64_t total = N * (D + 1);
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int64_t n = i / (D + 1);
+    const int j = int(i % (D + 1));
+    core[n * ld + F + j] = j == 0 ? fminf(fmaxf(reward[n], -1.0f), 1.0f) : last_action[n * D + j - 1];
+  }
+}
+
+int core_extras_continuous(float* core, int64_t ld, int64_t N, int F, const float* reward, const float* last_action,
+                           int D, cudaStream_t stream) {
+  ProfScope prof("core_extras_continuous", stream);
+  if (N == 0) return 0;
+  core_extras_continuous_kernel<<<grid_for(N * (D + 1), 256), 256, 0, stream>>>(core, ld, N, F, reward, last_action, D);
+  return check_launch("core_extras_continuous_kernel");
+}
+
 int core_extras(float* core, int64_t ld, int64_t N, int F, const float* reward, const int64_t* last_action, int A,
                 cudaStream_t stream, const ActionSegments* seg) {
   ProfScope prof("core_extras", stream);

@@ -34,6 +34,10 @@ int colsum(const float* X, float* out, int64_t M, int64_t ncols, int64_t ld, flo
 // core[n, F+1+off_k+last_action[n, k]] = 1 for each component k
 int core_extras(float* core, int64_t ld, int64_t N, int F, const float* reward, const int64_t* last_action, int A,
                 cudaStream_t stream, const ActionSegments* seg = nullptr);
+// A continuous action space of D dimensions: core[n, F] = clamp(reward[n], -1, 1); core[n, F+1+k] = last_action[n, k]
+// (float32 [N, D]) as it is
+int core_extras_continuous(float* core, int64_t ld, int64_t N, int F, const float* reward, const float* last_action,
+                           int D, cudaStream_t stream);
 
 // X[m, n] *= (Y[m, n] > 0) for n < ncols (ReLU backward in place on a strided view)
 int relu_mask_inplace(float* X, const float* Y, int64_t M, int64_t ncols, int64_t ldx, int64_t ldy,

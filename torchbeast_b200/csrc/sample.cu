@@ -166,9 +166,62 @@ static int sample_actions(const float* logits, int64_t T, int64_t B, int64_t A, 
   return check_launch("sample_actions_kernel");
 }
 
+// The Gaussian form (include/torchbeast_b200.h, tb_sample_gaussian_f32): a row is (mu, log sigma) of width 2D, and the
+// components 2j and 2j + 1 share the Philox block keyed (lo32(seed), hi32(seed) + j), words (0, 1) and (2, 3), each pair
+// turned into one standard normal by Box-Muller.  seed_step non-NULL: read when the kernel runs.
+__global__ void __launch_bounds__(256) sample_gaussian_kernel(const float* __restrict__ logits, int64_t N, int64_t B,
+                                                              int D, uint64_t seed, uint64_t step,
+                                                              const uint64_t* __restrict__ seed_step,
+                                                              const int64_t* __restrict__ stream_ids,
+                                                              float* __restrict__ actions) {
+  if (seed_step) {
+    seed = seed_step[0];
+    step = seed_step[1];
+  }
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < N; i += stride) {
+    const int64_t t = i / B, b = i - t * B;
+    const uint64_t ctr = step + uint64_t(t);
+    const uint64_t sid = stream_ids ? uint64_t(stream_ids[b]) : uint64_t(b);
+    const float* row = logits + i * 2 * D;
+    float* out = actions + i * D;
+    for (int k = 0; k < D; k += 2) {
+      const uint4 w = philox4x32_10(uint32_t(ctr), uint32_t(ctr >> 32), uint32_t(sid), uint32_t(sid >> 32),
+                                    uint32_t(seed), uint32_t(seed >> 32) + uint32_t(k / 2));
+      for (int h = 0; h < 2 && k + h < D; ++h) {
+        const uint32_t x0 = h ? w.z : w.x, x1 = h ? w.w : w.y;
+        const float u1 = float((x0 >> 8) + 1u) * 0x1p-24f, u2 = float(x1 >> 8) * 0x1p-24f;
+        const float z = sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
+        const float mu = row[k + h], l = row[D + k + h];
+        out[k + h] = (isfinite(mu) && isfinite(l)) ? mu + expf(l) * z : __int_as_float(0x7fffffff);
+      }
+    }
+  }
+}
+
 }  // namespace tb
 
 using namespace tb;
+
+extern "C" int tb_sample_gaussian_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed,
+                                      uint64_t step, const uint64_t* seed_step, const int64_t* stream_ids,
+                                      float* actions, void* stream) {
+  TB_REQUIRE(T >= 0 && B >= 0, "sample_gaussian: negative size T=%lld B=%lld", (long long)T, (long long)B);
+  TB_REQUIRE(A >= 2 && A % 2 == 0 && A / 2 <= TB_MAX_CONTINUOUS_DIM,
+             "sample_gaussian: A = %lld must be 2D with 1 <= D <= %d", (long long)A, TB_MAX_CONTINUOUS_DIM);
+  if (T == 0 || B == 0) return 0;
+  TB_REQUIRE(T <= INT64_MAX / B && T * B <= INT64_MAX / A, "sample_gaussian: size overflow T=%lld B=%lld A=%lld",
+             (long long)T, (long long)B, (long long)A);
+  TB_REQUIRE(logits && actions, "sample_gaussian: null pointer");
+  const int64_t N = T * B;
+  const int threads = 256;
+  int64_t blocks = (N + threads - 1) / threads;
+  if (blocks > int64_t(kNumSMs) * 16) blocks = int64_t(kNumSMs) * 16;
+  ProfScope prof("sample_gaussian", (cudaStream_t)stream);
+  sample_gaussian_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(logits, N, B, int(A / 2), seed, step,
+                                                                                 seed_step, stream_ids, actions);
+  return check_launch("sample_gaussian_kernel");
+}
 
 extern "C" int tb_sample_actions_f32(const float* logits, int64_t T, int64_t B, int64_t A, uint64_t seed, uint64_t step,
                                      const int64_t* stream_ids, int64_t* actions, void* stream) {

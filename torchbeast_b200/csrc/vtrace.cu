@@ -443,7 +443,87 @@ struct LossArgs {
   const float* trust_beta; float* kl; float* trust_out;
   // factored action space (impala_loss_kernel<0, *, *, *, true> only): actions are [T,B,D], row segments as in seg
   ActionSegments seg;
+  // A diagonal-Gaussian policy (impala_loss_kernel<kGaussianRows, ...>) adds no field: its rows are (mu, log sigma)
+  // of width A = 2D, and `actions` carries the address of its float32 [T,B,D] actions (gaussian_actions), so the
+  // struct, and every kernel that takes it, keeps the layout it had before Gaussian rows existed.
 };
+
+// ---- continuous (diagonal-Gaussian) action spaces (impala_loss_kernel<kGaussianRows, ...>) ---------------------------
+// A row of width A = 2D is (mu_0 .. mu_{D-1}, l_0 .. l_{D-1}), sigma_k = expf(l_k).  Every sum over k runs in index
+// order and starts from the k = 0 term; a non-finite input makes the quantity NaN (include/torchbeast_b200.h,
+// "continuous (diagonal-Gaussian) action spaces").
+constexpr float kHalfLog2Pi = TB_GAUSSIAN_HALF_LOG_2PI;
+constexpr int kGaussianRows = -1;  // impala_loss_kernel's row-width argument for Gaussian rows
+
+__device__ __forceinline__ const float* gaussian_actions(const LossArgs& p) {
+  return reinterpret_cast<const float*>(p.actions);
+}
+
+__device__ __forceinline__ bool gaussian_finite(float mu, float l) { return isfinite(mu) && isfinite(l); }
+
+// log pi(a) = sum_k (-0.5 z_k^2 - l_k - c), z_k = (a_k - mu_k) expf(-l_k)
+__device__ __forceinline__ float alp_gaussian(const float* __restrict__ row, int D, const float* __restrict__ act) {
+  float lp = 0.0f;
+  bool ok = true;
+  for (int k = 0; k < D; ++k) {
+    const float mu = row[k], l = row[D + k], a = act[k];
+    ok = ok && gaussian_finite(mu, l) && isfinite(a);
+    const float z = (a - mu) * expf(-l);
+    const float term = (-0.5f * (z * z) - l) - kHalfLog2Pi;
+    lp = k == 0 ? term : lp + term;
+  }
+  return ok ? lp : __int_as_float(0x7fffffff);
+}
+
+// KL(pi || mu_b) of row i: sum_k ((lb_k - l_k) + 0.5 (expf(2 (l_k - lb_k)) + ((mu_k - mub_k) expf(-lb_k))^2) - 0.5)
+__device__ __forceinline__ float trust_kl_gaussian(const LossArgs& p, int64_t i) {
+  const int D = int(p.A / 2);
+  const float* trow = p.tlogits + i * p.A;
+  const float* brow = p.blogits + i * p.A;
+  float kl = 0.0f;
+  bool ok = true;
+  for (int k = 0; k < D; ++k) {
+    const float mu = trow[k], l = trow[D + k], mub = brow[k], lb = brow[D + k];
+    ok = ok && gaussian_finite(mu, l) && gaussian_finite(mub, lb);
+    const float dm = (mu - mub) * expf(-lb);
+    const float term = ((lb - l) + 0.5f * (expf(2.0f * (l - lb)) + dm * dm)) - 0.5f;
+    kl = k == 0 ? term : kl + term;
+  }
+  return ok ? kl : __int_as_float(0x7fffffff);
+}
+
+// The entropy term ent = sum_k -(l_k + 0.5 + c) of row i, and with grad_logits its gradient row: mu_k gets
+// -adv z_k expf(-l_k), l_k gets adv (1 - z_k^2) - entropy_cost, each times column_weights[b] when kWeighted.  A row or
+// action with a non-finite entry gets NaN for the term and the whole gradient row.
+template <bool kWeighted>
+__device__ __forceinline__ float gaussian_entropy_grad(const LossArgs& p, int64_t i, int64_t b, float adv) {
+  const int D = int(p.A / 2);
+  const float* row = p.tlogits + i * p.A;
+  const float* act = gaussian_actions(p) + i * D;
+  float ent = 0.0f;
+  bool ok = true;
+  for (int k = 0; k < D; ++k) {
+    const float l = row[D + k];
+    ok = ok && gaussian_finite(row[k], l) && isfinite(act[k]);
+    const float term = -((l + 0.5f) + kHalfLog2Pi);
+    ent = k == 0 ? term : ent + term;
+  }
+  const float nan = __int_as_float(0x7fffffff);
+  if (p.grad_logits) {
+    float* g = p.grad_logits + i * p.A;
+    const float wb = kWeighted ? __ldg(p.column_weights + b) : 1.0f;
+    for (int k = 0; k < D; ++k) {
+      const float mu = row[k], l = row[D + k];
+      const float s = expf(-l), z = (act[k] - mu) * s;
+      float gm = ((-adv) * z) * s, gl = adv * (1.0f - z * z) - p.entropy_cost;
+      if (!ok) gm = gl = nan;
+      if constexpr (kWeighted) { gm *= wb; gl *= wb; }
+      g[k] = gm;
+      g[D + k] = gl;
+    }
+  }
+  return ok ? ent : nan;
+}
 
 // ---- factored action spaces (impala_loss_kernel<0, *, *, *, true>) -----------------------------------------------------
 // Each segment is a row of its own for alp_dyn, the code the flat rows use; the sums over segments run in index order from
@@ -543,13 +623,15 @@ __device__ __forceinline__ float trust_kl(const LossArgs& p, int64_t i, int64_t 
 
 // rho of row i under the trust region: expf(lr) where kl_i <= beta, else 0 (a NaN kl too).  kl_i is formed and written
 // to p.kl here, or, with `written`, read back from there (pass 1 of the split layout wrote it in this thread).
-template <int A, bool kFactored = false>
+template <int A, bool kFactored = false, bool kGaussian = false>
 __device__ __forceinline__ float trust_rho(const LossArgs& p, int64_t i, int64_t Ause, float lr, bool written) {
   float kl;
   if (written) {
     kl = p.kl[i];
   } else {
-    if constexpr (kFactored) kl = trust_kl_factored(p, i); else kl = trust_kl<A>(p, i, Ause);
+    if constexpr (kGaussian) kl = trust_kl_gaussian(p, i);
+    else if constexpr (kFactored) kl = trust_kl_factored(p, i);
+    else kl = trust_kl<A>(p, i, Ause);
     p.kl[i] = kl;
   }
   const float rho = expf(lr);
@@ -611,10 +693,16 @@ __device__ __forceinline__ float discount_of(const LossArgs& p, int64_t i) {
 // code.  kTrust: row (t, b) with kl_t = KL(pi_t || mu_t) > beta (or NaN) runs the V-trace and the policy gradient with
 // rho_t = 0 (include/torchbeast_b200.h, tb_impala_loss_f32); the other instantiations compile no trust code.  kFactored
 // (with A = 0 only): actions are [T,B,D] and every row quantity is formed per segment (LossArgs::seg); the other
-// instantiations compile none of that code.
-template <int A, bool kPopArt = false, bool kWeighted = false, bool kTrust = false, bool kFactored = false>
+// instantiations compile none of that code.  AT = kGaussianRows: diagonal-Gaussian rows (mu, log sigma) on the
+// dynamic-A path (A = 0 below), whose actions are float32 [T,B,D] (gaussian_actions); the other instantiations compile
+// none of that code.  The row kind rides on AT rather than on a sixth flag so that the categorical instantiations keep
+// the names they had before Gaussian rows existed.
+template <int AT, bool kPopArt = false, bool kWeighted = false, bool kTrust = false, bool kFactored = false>
 __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
+  constexpr bool kGaussian = AT == kGaussianRows;
+  constexpr int A = kGaussian ? 0 : AT;
   static_assert(!kFactored || A == 0, "factored rows take the dynamic-A path");
+  static_assert(!kGaussian || !kFactored, "a row is factored or Gaussian");
   if (p.hp) load_hparams(p);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* sA = reinterpret_cast<float*>(smem_raw);
@@ -657,7 +745,10 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         for (int64_t t = t1 - 1; t >= t0; --t) {
           const int64_t i = t * B + b;
           float tlp, blp;
-          if constexpr (kFactored) {
+          if constexpr (kGaussian) {
+            tlp = alp_gaussian(p.tlogits + i * Ause, int(Ause / 2), gaussian_actions(p) + i * (Ause / 2));
+            blp = alp_gaussian(p.blogits + i * Ause, int(Ause / 2), gaussian_actions(p) + i * (Ause / 2));
+          } else if constexpr (kFactored) {
             tlp = alp_factored(p.seg, p.tlogits + i * Ause, p.actions + i * p.seg.D);
             blp = alp_factored(p.seg, p.blogits + i * Ause, p.actions + i * p.seg.D);
           } else {
@@ -667,7 +758,7 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
           }
           const float lr = tlp - blp;
           p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
-          const float rho = kTrust ? trust_rho<A, kFactored>(p, i, Ause, lr, false) : expf(lr);  // kl read back in pass 3
+          const float rho = kTrust ? trust_rho<A, kFactored, kGaussian>(p, i, Ause, lr, false) : expf(lr);  // kl read back in pass 3
           const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
           const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
           const float delta = rb * (r + g * v_next - v);
@@ -701,21 +792,25 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
     float acc = acc_in;
     for (int64_t t = t1 - 1; t >= t0; --t) {
       const int64_t i = t * B + b;
-      const int64_t act = kFactored ? 0 : p.actions[i];
+      const int64_t act = (kFactored || kGaussian) ? 0 : p.actions[i];
       const float* trow = p.tlogits + i * Ause;
       float m, logs;
-      const float tlp = kFactored ? alp_factored(p.seg, trow, p.actions + i * p.seg.D)
-                                  : alp_row<float, A>(trow, Ause, act, &m, &logs);
+      float tlp;
+      if constexpr (kGaussian) tlp = alp_gaussian(trow, int(Ause / 2), gaussian_actions(p) + i * (Ause / 2));
+      else if constexpr (kFactored) tlp = alp_factored(p.seg, trow, p.actions + i * p.seg.D);
+      else tlp = alp_row<float, A>(trow, Ause, act, &m, &logs);
       float lr;
       if (W > 1) {
         lr = p.log_rhos[i];  // written by this same thread in pass 1
       } else {
-        const float blp = kFactored ? alp_factored(p.seg, p.blogits + i * Ause, p.actions + i * p.seg.D)
-                                    : alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
+        float blp;
+        if constexpr (kGaussian) blp = alp_gaussian(p.blogits + i * Ause, int(Ause / 2), gaussian_actions(p) + i * (Ause / 2));
+        else if constexpr (kFactored) blp = alp_factored(p.seg, p.blogits + i * Ause, p.actions + i * p.seg.D);
+        else blp = alp_row<float, A>(p.blogits + i * Ause, Ause, act, nullptr, nullptr);
         lr = tlp - blp;
         p.talp[i] = tlp; p.balp[i] = blp; p.log_rhos[i] = lr;
       }
-      const float rho = kTrust ? trust_rho<A, kFactored>(p, i, Ause, lr, W > 1) : expf(lr);
+      const float rho = kTrust ? trust_rho<A, kFactored, kGaussian>(p, i, Ause, lr, W > 1) : expf(lr);
       const float g = discount_of(p, i), r = reward_of(p, i), v = kPopArt ? pop_value(t, b) : p.values[i];
       const float rb = p.has_clip_rho ? fminf(rho, p.clip_rho) : rho;
       const float rp = p.has_clip_pg ? fminf(rho, p.clip_pg) : rho;
@@ -754,7 +849,9 @@ __global__ void __launch_bounds__(512) impala_loss_kernel(LossArgs p) {
         s_bl += 0.5 * double(d * d);
       }
       float ent_row = 0.0f;
-      if constexpr (kFactored) {
+      if constexpr (kGaussian) {
+        ent_row = gaussian_entropy_grad<kWeighted>(p, i, b, adv);
+      } else if constexpr (kFactored) {
         ent_row = factored_entropy_grad<kWeighted>(p, i, b, adv);
       } else if constexpr (A != 0) {
         float lp[A], pr[A];
@@ -1120,18 +1217,24 @@ __global__ void pg_loss_kernel(const F* __restrict__ logits, const int64_t* __re
   if (grid_sum3(s, 0.0, 0.0, ws, tot)) out[0] = F(tot[0]);
 }
 
-// One fused-loss launch: the flat kernel of the row width p.A (TB_DISPATCH_A), or with `factored` the dynamic-A kernel
-// that reads p.seg.
+// What a loss row means: a flat categorical, a factored one (p.seg) or a diagonal Gaussian (gaussian_actions).
+enum class RowKind { kFlat, kFactored, kGaussian };
+
+// One fused-loss launch: the flat kernel of the row width p.A (TB_DISPATCH_A), or the dynamic-A kernel of a factored or
+// Gaussian row.
 template <bool kPopArt, bool kWeighted, bool kTrust>
-static void launch_loss_kernel(const LossArgs& p, bool factored, dim3 grid, dim3 block, size_t smem, cudaStream_t st) {
-  if (factored)
+static void launch_loss_kernel(const LossArgs& p, RowKind kind, dim3 grid, dim3 block, size_t smem, cudaStream_t st) {
+  if (kind == RowKind::kFactored)
     impala_loss_kernel<0, kPopArt, kWeighted, kTrust, true><<<grid, block, smem, st>>>(p);
+  else if (kind == RowKind::kGaussian)
+    impala_loss_kernel<kGaussianRows, kPopArt, kWeighted, kTrust><<<grid, block, smem, st>>>(p);
   else
     TB_DISPATCH_A(p.A, (impala_loss_kernel<kA, kPopArt, kWeighted, kTrust><<<grid, block, smem, st>>>(p)));
 }
 
-// tb_impala_loss_f32 and, with seg non-NULL, tb_impala_loss_factored_f32.  The kernel instantiation follows from which
-// of column_weights, task and trust_beta are non-NULL.
+// tb_impala_loss_f32, with seg non-NULL tb_impala_loss_factored_f32, and with gactions non-NULL (actions then NULL)
+// tb_impala_loss_gaussian_f32.  The kernel instantiation follows from which of column_weights, task and trust_beta are
+// non-NULL.
 static int impala_loss(const float* blogits, const float* tlogits, const int64_t* actions, const float* rewards,
                        const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
                        int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost, float entropy_cost,
@@ -1140,7 +1243,7 @@ static int impala_loss(const float* blogits, const float* tlogits, const int64_t
                        int64_t K, double* task_sums, const float* trust_beta, float* kl_out, float* trust_out,
                        float* vs, float* pg_adv, float* log_rhos, float* behavior_alp, float* target_alp,
                        float* losses_out, float* grad_logits, float* grad_values, int zero_tail, void* workspace,
-                       void* stream, const ActionSegments* seg) {
+                       void* stream, const ActionSegments* seg, const float* gactions = nullptr) {
 
   if (task) {
     TB_REQUIRE(!column_weights, "impala_loss_popart: column_weights are not supported with PopArt (task)");
@@ -1169,11 +1272,12 @@ static int impala_loss(const float* blogits, const float* tlogits, const int64_t
     }
     return 0;
   }
-  TB_REQUIRE(blogits && tlogits && actions && rewards && (done || discounts) && values && bootstrap,
+  TB_REQUIRE(blogits && tlogits && (actions || gactions) && rewards && (done || discounts) && values && bootstrap,
              "impala_loss: null input pointer");
   TB_REQUIRE(vs && pg_adv && log_rhos && behavior_alp && target_alp, "impala_loss: null output pointer");
   LossArgs p;
-  p.blogits = blogits; p.tlogits = tlogits; p.actions = actions; p.rewards = rewards; p.done = done;
+  p.blogits = blogits; p.tlogits = tlogits; p.rewards = rewards; p.done = done;
+  p.actions = gactions ? reinterpret_cast<const int64_t*>(gactions) : actions;
   p.discounts = discounts; p.values = values; p.bootstrap = bootstrap; p.T = T; p.B = B; p.A = A;
   p.discounting = discounting; p.baseline_cost = baseline_cost; p.entropy_cost = entropy_cost;
   p.clip_rewards = clip_rewards; p.clip_rho = clip_rho; p.clip_pg = clip_pg_rho;
@@ -1186,6 +1290,7 @@ static int impala_loss(const float* blogits, const float* tlogits, const int64_t
   p.column_weights = column_weights;
   p.trust_beta = trust_beta; p.kl = kl_out; p.trust_out = trust_out;
   if (seg) p.seg = *seg;
+  const RowKind kind = seg ? RowKind::kFactored : gactions ? RowKind::kGaussian : RowKind::kFlat;
   const int64_t tiles = (B + kWarp - 1) / kWarp;
   int W = pick_warps(T, tiles);
   p.wide = (W == 1);
@@ -1202,10 +1307,10 @@ static int impala_loss(const float* blogits, const float* tlogits, const int64_t
     ProfScope prof(trust_beta ? "impala_loss_popart_trust" : "impala_loss_popart", (cudaStream_t)stream);
     const size_t pop_smem = smem + size_t(2) * kPopArtMaxTasks * sizeof(float);
     if (trust_beta) {
-      launch_loss_kernel<true, false, true>(p, seg, grid, block, pop_smem, (cudaStream_t)stream);
+      launch_loss_kernel<true, false, true>(p, kind, grid, block, pop_smem, (cudaStream_t)stream);
       TB_TRY(check_launch("impala_loss_kernel<popart, trust>"));
     } else {
-      launch_loss_kernel<true, false, false>(p, seg, grid, block, pop_smem, (cudaStream_t)stream);
+      launch_loss_kernel<true, false, false>(p, kind, grid, block, pop_smem, (cudaStream_t)stream);
       TB_TRY(check_launch("impala_loss_kernel<popart>"));
     }
     popart_task_sums_kernel<<<unsigned(K), kPopArtStatsThreads, 0, (cudaStream_t)stream>>>(vs, task, T * B, int(K),
@@ -1215,19 +1320,19 @@ static int impala_loss(const float* blogits, const float* tlogits, const int64_t
   if (trust_beta) {
     ProfScope prof("impala_loss_trust", (cudaStream_t)stream);
     if (column_weights) {
-      launch_loss_kernel<false, true, true>(p, seg, grid, block, smem, (cudaStream_t)stream);
+      launch_loss_kernel<false, true, true>(p, kind, grid, block, smem, (cudaStream_t)stream);
       return check_launch("impala_loss_kernel<weighted, trust>");
     }
-    launch_loss_kernel<false, false, true>(p, seg, grid, block, smem, (cudaStream_t)stream);
+    launch_loss_kernel<false, false, true>(p, kind, grid, block, smem, (cudaStream_t)stream);
     return check_launch("impala_loss_kernel<trust>");
   }
   if (column_weights) {
     ProfScope prof("impala_loss_weighted", (cudaStream_t)stream);
-    launch_loss_kernel<false, true, false>(p, seg, grid, block, smem, (cudaStream_t)stream);
+    launch_loss_kernel<false, true, false>(p, kind, grid, block, smem, (cudaStream_t)stream);
     return check_launch("impala_loss_kernel<weighted>");
   }
   ProfScope prof("impala_loss_fwd_bwd", (cudaStream_t)stream);
-  launch_loss_kernel<false, false, false>(p, seg, grid, block, smem, (cudaStream_t)stream);
+  launch_loss_kernel<false, false, false>(p, kind, grid, block, smem, (cudaStream_t)stream);
   return check_launch("impala_loss_kernel");
 }
 
@@ -1297,6 +1402,24 @@ int tb_impala_loss_factored_f32(const float* blogits, const float* tlogits, cons
                      baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, column_weights, task, mu, nu,
                      K, task_sums, trust_beta, kl_out, trust_out, vs, pg_adv, log_rhos, behavior_alp, target_alp,
                      losses_out, grad_logits, grad_values, zero_tail, workspace, stream, &seg);
+}
+
+int tb_impala_loss_gaussian_f32(const float* blogits, const float* tlogits, const float* actions, const float* rewards,
+                                const uint8_t* done, const float* discounts, const float* values, const float* bootstrap,
+                                int64_t T, int64_t B, int64_t A, float discounting, float baseline_cost,
+                                float entropy_cost, int clip_rewards, float clip_rho, float clip_pg_rho,
+                                const tb_hparams* hp, const float* column_weights, const int64_t* task, const double* mu,
+                                const double* nu, int64_t K, double* task_sums, const float* trust_beta, float* kl_out,
+                                float* trust_out, float* vs, float* pg_adv, float* log_rhos, float* behavior_alp,
+                                float* target_alp, float* losses_out, float* grad_logits, float* grad_values,
+                                int zero_tail, void* workspace, void* stream) {
+  TB_REQUIRE(A >= 2 && A % 2 == 0 && A / 2 <= TB_MAX_CONTINUOUS_DIM,
+             "impala_loss_gaussian: A = %lld must be 2D with 1 <= D <= %d", (long long)A, TB_MAX_CONTINUOUS_DIM);
+  TB_REQUIRE(actions || T == 0 || B == 0, "impala_loss_gaussian: null actions");
+  return impala_loss(blogits, tlogits, nullptr, rewards, done, discounts, values, bootstrap, T, B, A, discounting,
+                     baseline_cost, entropy_cost, clip_rewards, clip_rho, clip_pg_rho, hp, column_weights, task, mu, nu,
+                     K, task_sums, trust_beta, kl_out, trust_out, vs, pg_adv, log_rhos, behavior_alp, target_alp,
+                     losses_out, grad_logits, grad_values, zero_tail, workspace, stream, nullptr, actions);
 }
 
 // The kernel instantiation follows from which of column_weights, task and trust_beta are non-NULL, as in the loss.

@@ -168,6 +168,11 @@ def impala_loss_fwd_bwd(
     With `action_space` (component sizes (A_1, ..., A_D) summing to A; torchbeast_b200.action_space) the policy is
     factored: `actions` are int64 [T, B, D] and tb_impala_loss_factored_f32 forms every row quantity per component
     (the rules are stated in include/torchbeast_b200.h).  UPGO takes flat rows only.
+
+    With `action_space` a Gaussian(D) (torchbeast_b200.action_space) the policy is a diagonal Gaussian: the logits are
+    the (mu, log sigma) rows [T, B, 2D], `actions` are float32 [T, B, D] and tb_impala_loss_gaussian_f32 forms the
+    log-densities, the entropy, the trust region's KL and the gradients (the rules are stated in
+    include/torchbeast_b200.h).  UPGO takes categorical rows only.
     """
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, bootstrap_value)
     _lib.require_cuda(*tensors)
@@ -217,7 +222,7 @@ def impala_loss_popart(
     of popart_update (SUM all-reduce it first when data-parallel).  With `trust_region` (see impala_loss_fwd_bwd) it
     returns (ImpalaLoss, task_sums, TrustRegion), task_sums from the masked vs.  With `upgo_cost` (see
     impala_loss_fwd_bwd; its advantage is divided by sigma_k) an Upgo is appended last.  `action_space`: a factored
-    policy, as in impala_loss_fwd_bwd."""
+    or a Gaussian policy, as in impala_loss_fwd_bwd."""
     tensors = (behavior_policy_logits, target_policy_logits, actions, rewards, done, values, task, mu, nu)
     _lib.require_cuda(*tensors)
     T, B, A = target_policy_logits.shape
@@ -240,9 +245,19 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
                  action_space=None):
     """The tb_impala_loss_f32 call behind impala_loss_fwd_bwd and impala_loss_popart, on inputs they checked, and with
     `upgo_cost` the tb_upgo_loss_f32 call right behind it on the same inputs.  popart: None, or (task, mu, nu) with
-    values [T+1, B, K].  action_space: component sizes, for tb_impala_loss_factored_f32.  Returns (ImpalaLoss,
-    task_sums or None, TrustRegion or None, Upgo or None)."""
-    dims = _action_space.dims_of(None if action_space is None else tuple(action_space))
+    values [T+1, B, K].  action_space: component sizes, for tb_impala_loss_factored_f32, or a Gaussian(D), for
+    tb_impala_loss_gaussian_f32.  Returns (ImpalaLoss, task_sums or None, TrustRegion or None, Upgo or None)."""
+    D = _action_space.continuous_dim_of(action_space)
+    dims = None if D is not None else _action_space.dims_of(None if action_space is None else tuple(action_space))
+    if D is not None:
+        if upgo_cost is not None:
+            raise _lib.TorchBeastB200Error("UPGO (upgo_cost) is not built for a continuous action space Gaussian(%d)" % D)
+        T, B, A = target_policy_logits.shape
+        if A != 2 * D or tuple(actions.shape) != (T, B, D) or not actions.dtype.is_floating_point:
+            raise _lib.TorchBeastB200Error(
+                "a continuous action space Gaussian(%d) takes logits [T, B, 2D] and float actions [T, B, D] = %r, got "
+                "logits %r and %s actions %r" % (D, (T, B, D), tuple(target_policy_logits.shape), actions.dtype,
+                                                 tuple(actions.shape)))
     if dims is not None:
         if upgo_cost is not None:
             raise _lib.TorchBeastB200Error("UPGO (upgo_cost) is not built for a factored action space %r" % (dims,))
@@ -285,7 +300,8 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
     losses = torch.empty(4, dtype=f32, device=dev)
     gl = torch.empty((T + 1, B, A), dtype=f32, device=dev) if with_grads else None
     gv = torch.empty((T + 1, B) + ((K,) if popart is not None else ()), dtype=f32, device=dev) if with_grads else None
-    tl, act = target_policy_logits.detach().to(f32).contiguous(), actions.to(torch.int64).contiguous()
+    tl = target_policy_logits.detach().to(f32).contiguous()
+    act = actions.to(torch.int64 if D is None else f32).contiguous()
     rw, vals = rewards.to(f32).contiguous(), values.detach().to(f32).contiguous()
     disc_arg = 0.0 if hparams_dev is not None else float(discounting)
     p = _lib.ptr
@@ -295,7 +311,9 @@ def _impala_loss(behavior_policy_logits, target_policy_logits, actions, rewards,
             clip_rewards, _lib.clip_arg(clip_rho_threshold), _lib.clip_arg(clip_pg_rho_threshold), p(hparams_dev),
             p(cw), p(task), p(mu), p(nu), K, p(sums), p(beta), p(kl), p(kl_sums),
             *[p(o) for o in outs], p(losses), p(gl), p(gv), 1)
-    if dims is None:
+    if D is not None:
+        _lib.check(_lib.lib().tb_impala_loss_gaussian_f32(*args, p(ws), _lib.stream_ptr()), "tb_impala_loss_gaussian_f32")
+    elif dims is None:
         _lib.check(_lib.lib().tb_impala_loss_f32(*args, p(ws), _lib.stream_ptr()), "tb_impala_loss_f32")
     else:
         _lib.check(_lib.lib().tb_impala_loss_factored_f32(*args, ctypes.byref(_action_space.c_space(dims)), p(ws),
@@ -525,6 +543,10 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     A model with a factored action space (model.action_dims, torchbeast_b200.action_space) takes action [T+1, B, D] and
     runs the factored loss (tb_impala_loss_factored_f32) on every path above but UPGO and kickstarting.
 
+    A model with a continuous action space (model.continuous_dim, a Gaussian(D)) takes float32 action [T+1, B, D] and
+    policy_logits [T+1, B, 2D] and runs the Gaussian loss (tb_impala_loss_gaussian_f32) on every path above but UPGO,
+    kickstarting and legal-action masks.
+
     A batch with a legal_actions leaf (bool or uint8 [T+1, B, A], torchbeast_b200.legal_actions) learns over each
     step's legal actions on every path above: the learner's and the teacher's forwards mask their own logits, and one
     launch writes a masked copy of the behaviour logits (policy_logits[1:] or `behavior_logits`) under
@@ -560,7 +582,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev,
             column_weights=None if draw is None else draw.weights, trust_region=trust_region, upgo_cost=upgo_arg,
-            action_space=_action_space.dims_of_model(model))
+            action_space=_action_space.loss_space_of_model(model))
         if trust_region is not None or upgo_arg is not None:
             loss, *rest = loss
             trust = rest.pop(0) if trust_region is not None else None
@@ -575,7 +597,7 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             _popart_task(model, batch), pop.mu, pop.nu,
             discounting=flags.discounting, baseline_cost=flags.baseline_cost, entropy_cost=flags.entropy_cost,
             reward_clipping=flags.reward_clipping, hparams_dev=hparams_dev, trust_region=trust_region,
-            upgo_cost=upgo_arg, action_space=_action_space.dims_of_model(model))
+            upgo_cost=upgo_arg, action_space=_action_space.loss_space_of_model(model))
         loss, task_sums, *rest = res
         trust = rest.pop(0) if trust_region is not None else None
         upgo = rest.pop(0) if upgo_arg is not None else None
@@ -705,6 +727,9 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
       any other leaf; learn_step learns over each step's legal actions.
     * a model with a factored action space (torchbeast_b200.action_space) learns on action [T+1, B, D] on every path
       above; UPGO, kickstarting, a legal_actions leaf or a teacher with another space raise before anything is staged.
+    * a model with a continuous action space (Gaussian(D)) learns on float32 action [T+1, B, D] on every path above;
+      UPGO, kickstarting, a legal_actions leaf, a teacher with another space or integer actions raise before anything
+      is staged.
     * with flags.kickstart_cost, the teacher attached as model.teacher (torchbeast_b200.kickstart.Teacher) runs on the
       same (mixed) batch and its KL term joins the loss (learn_step); the teacher is part of the graph's structure.
     Returns the reference's stats dict."""

@@ -61,8 +61,9 @@ class PopArt(nn.Module):
         return (self.sigma()[task] * n + self.mu[task]).to(torch.float32)
 
 
-def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
-    core = 512 + num_actions + 1
+def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1, continuous_dim=None):
+    """continuous_dim D (a Gaussian(D) space, num_actions = 2D): the core takes D last-action columns, 512 + D + 1."""
+    core = 512 + (num_actions if continuous_dim is None else continuous_dim) + 1
     spec = [
         ("conv1.weight", (32, in_channels, 8, 8)), ("conv1.bias", (32,)),
         ("conv2.weight", (64, 32, 4, 4)), ("conv2.bias", (64,)),
@@ -84,6 +85,7 @@ def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1):
 
 ATARI_SHAPE = (4, 84, 84)
 LSTM_MAX_HIDDEN = 700  # TB_LSTM_MAX_HIDDEN
+HEADS_MAX_OUTPUTS = 31  # the fused policy / baseline heads take A < 32
 RESNET_CHANNELS = (16, 32, 32)   # the IMPALA paper's section widths
 
 
@@ -205,11 +207,18 @@ class FlatParamModule(nn.Module):
     # component sizes (A_1, ..., A_D) of a factored action space (torchbeast_b200.action_space), or None: one categorical
     # over num_actions choices.  num_actions is the policy-logit width either way.
     action_dims = None
+    # D of a continuous (Gaussian(D)) action space, whose policy rows are (mu, log sigma) of width num_actions = 2D
+    continuous_dim = None
 
     def _set_action_space(self, num_actions):
-        """num_actions: an int, or a tuple of component sizes (a factored space); sets num_actions to the logit width."""
+        """num_actions: an int, a tuple of component sizes (a factored space) or a Gaussian(D) (a continuous one); sets
+        num_actions to the logit width."""
         self.action_dims = action_space.dims_of(num_actions)
+        self.continuous_dim = action_space.continuous_dim_of(num_actions)
         self.num_actions = action_space.width(num_actions)
+        if self.continuous_dim is not None and self.num_actions > HEADS_MAX_OUTPUTS:
+            raise _lib.TorchBeastB200Error("the policy head takes at most %d outputs: Gaussian(D) needs D <= %d, got %r"
+                                           % (HEADS_MAX_OUTPUTS, HEADS_MAX_OUTPUTS // 2, num_actions))
 
     def _sample(self, logits, inputs):
         """Training-mode action [T, B] (factored: [T, B, D]) of the reference-compatible forwards
@@ -219,16 +228,22 @@ class FlatParamModule(nn.Module):
         if self.action_sampler is not None:
             if self.action_dims is not None:
                 return self.action_sampler.sample(logits, inputs.get("stream_ids"), action_dims=self.action_dims)
+            if self.continuous_dim is not None:
+                return self.action_sampler.sample(logits, inputs.get("stream_ids"), continuous_dim=self.continuous_dim)
             return self.action_sampler.sample(logits, inputs.get("stream_ids"))
         if self.action_dims is not None:
             return action_space.multinomial(logits, self.action_dims)
+        if self.continuous_dim is not None:
+            return action_space.gaussian_normal(logits, self.continuous_dim)
         return torch.multinomial(torch.softmax(logits.detach().view(T * B, A), dim=1), num_samples=1).view(T, B)
 
     def _greedy(self, logits):
-        """Eval-mode action: argmax over the row, or per segment of a factored space."""
+        """Eval-mode action: argmax over the row, or per segment of a factored space; the mean of a Gaussian one."""
         T, B = logits.shape[:2]
         if self.action_dims is not None:
             return action_space.greedy(logits, self.action_dims)
+        if self.continuous_dim is not None:
+            return action_space.gaussian_mean(logits, self.continuous_dim)
         return torch.argmax(logits.detach().view(T * B, self.num_actions), dim=1)  # don't sample when testing
 
     def _build_flat(self, spec, device):
@@ -411,16 +426,21 @@ class AtariNet(FlatParamModule):
         self._set_action_space(num_actions)
         num_actions = self.num_actions
         self.use_lstm = use_lstm
-        self.core_size = 512 + num_actions + 1
+        D = self.continuous_dim
+        self.core_size = 512 + (num_actions if D is None else D) + 1
         if self.action_dims is not None and use_lstm and self.core_size > LSTM_MAX_HIDDEN:
             raise _lib.TorchBeastB200Error(
                 "AtariNet with an LSTM needs 512 + sum(num_actions) + 1 <= %d, got %d for num_actions=%r"
                 % (LSTM_MAX_HIDDEN, self.core_size, self.action_dims))
+        if D is not None and use_lstm and self.core_size > LSTM_MAX_HIDDEN:
+            raise _lib.TorchBeastB200Error("AtariNet with an LSTM needs 512 + D + 1 <= %d, got %d for Gaussian(%d)"
+                                           % (LSTM_MAX_HIDDEN, self.core_size, D))
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
         popart = None if num_tasks is None else PopArt(num_tasks, device)
         self.num_values = 1 if popart is None else popart.num_tasks
-        self._build_flat(atarinet_param_spec(num_actions, use_lstm, num_values=self.num_values), device)
+        self._build_flat(atarinet_param_spec(num_actions, use_lstm, num_values=self.num_values, continuous_dim=D),
+                         device)
         self.reset_parameters_like_torch()
         if popart is not None:
             self.popart = popart  # registered after the parameters: its keys come last in the state_dict
@@ -435,7 +455,10 @@ class AtariNet(FlatParamModule):
         self._ws = None
         self._ws_key = None
         self._scratch_buf = self._scratch_key = None
-        count = _lib.lib().tb_atarinet_param_count(num_actions, self.num_values, int(use_lstm))
+        if D is None:
+            count = _lib.lib().tb_atarinet_param_count(num_actions, self.num_values, int(use_lstm))
+        else:
+            count = _lib.lib().tb_atarinet_param_count_continuous(num_actions, self.num_values, int(use_lstm))
         assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
 
     def initial_state(self, batch_size):
@@ -447,8 +470,9 @@ class AtariNet(FlatParamModule):
     def _workspace(self, T1, B):
         key = (T1, B, self._flat.device, self.precision)
         if self._ws_key != key:
-            nbytes = _lib.lib().tb_atarinet_workspace_bytes(T1, B, self.num_actions, int(self.use_lstm),
-                                                            self.PRECISIONS[self.precision])
+            ws_bytes = _lib.lib().tb_atarinet_workspace_bytes if self.continuous_dim is None \
+                else _lib.lib().tb_atarinet_workspace_bytes_continuous
+            nbytes = ws_bytes(T1, B, self.num_actions, int(self.use_lstm), self.PRECISIONS[self.precision])
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
             self._ws_key = key
         return self._ws
@@ -464,7 +488,14 @@ class AtariNet(FlatParamModule):
         dev = self._flat.device
         frame = frame.contiguous()
         reward = reward.to(torch.float32).contiguous()
-        last_action = last_action.to(torch.int64).contiguous()
+        D = self.continuous_dim
+        if D is not None:
+            if last_action.dtype != torch.float32 or tuple(last_action.shape) != (T1, B, D):
+                raise _lib.TorchBeastB200Error("last_action must be float32 [T, B, D] = %r for Gaussian(%d), got %s %r"
+                                               % ((T1, B, D), D, last_action.dtype, tuple(last_action.shape)))
+            last_action = last_action.contiguous()
+        else:
+            last_action = last_action.to(torch.int64).contiguous()
         logits = torch.empty(T1, B, self.num_actions, dtype=torch.float32, device=dev)
         baseline = torch.empty(self._baseline_shape(T1, B), dtype=torch.float32, device=dev)
         if self.use_lstm:
@@ -480,7 +511,10 @@ class AtariNet(FlatParamModule):
                 p(self._flat), T1, B, self.num_actions, self.num_values, int(self.use_lstm),
                 self.PRECISIONS[self.precision], p(ws), p(_scratch(self, 0, T1, B)) if unstacked else None, p(logits),
                 p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None)
-        if self.action_dims is None:
+        if D is not None:
+            _lib.check(_lib.lib().tb_atarinet_forward_continuous(*args, _lib.stream_ptr()),
+                       "tb_atarinet_forward_continuous")
+        elif self.action_dims is None:
             _lib.check(_lib.lib().tb_atarinet_forward(*args, _lib.stream_ptr()), "tb_atarinet_forward")
         else:
             D = len(self.action_dims)
@@ -497,12 +531,13 @@ class AtariNet(FlatParamModule):
         T1, B = g_baseline.shape[:2]
         ws = self._workspace(T1, B)
         p = _lib.ptr
+        name = "tb_atarinet_backward" if self.continuous_dim is None else "tb_atarinet_backward_continuous"
         _lib.check(
-            _lib.lib().tb_atarinet_backward(
+            getattr(_lib.lib(), name)(
                 p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), T1, B,
                 self.num_actions, self.num_values, int(self.use_lstm), self.PRECISIONS[self.precision], p(ws),
                 p(grads_out), int(phase), _lib.stream_ptr()),
-            "tb_atarinet_backward")
+            name)
 
     def grad_split(self):
         """Flat-gradient offset where the LSTM + heads slice starts (final after backward phase 1 for precision

@@ -34,7 +34,7 @@ class ActionSampler:
         self.seed = int(seed)
         self.step = int(step)
 
-    def sample(self, logits, stream_ids=None, action_dims=None):
+    def sample(self, logits, stream_ids=None, action_dims=None, continuous_dim=None):
         """logits: [T, B, A] float32 CUDA tensor -> int64 [T, B] actions; advances `step` by T.
 
         Row (t, b) uses counter step + t and stream id `stream_ids[b]` (int64 [B], any device; default: the column
@@ -42,7 +42,10 @@ class ActionSampler:
 
         action_dims (A_1, ..., A_D), summing to A: a factored policy (torchbeast_b200.action_space), sampled by
         tb_sample_actions_factored_f32 into int64 [T, B, D]; component k draws from its own segment of the row, and a
-        segment with no distribution gets -1."""
+        segment with no distribution gets -1.
+
+        continuous_dim D, with A = 2D: a Gaussian policy (torchbeast_b200.action_space.Gaussian), sampled by
+        tb_sample_gaussian_f32 into float32 [T, B, D]; a component with a non-finite mean or log-std gets NaN."""
         _lib.require_cuda(logits)
         if logits.dim() != 3 or logits.dtype != torch.float32:
             raise _lib.TorchBeastB200Error("logits must be float32 [T, B, A], got %s %r" % (logits.dtype, tuple(logits.shape)))
@@ -54,6 +57,10 @@ class ActionSampler:
             stream_ids = stream_ids.to(device=logits.device, dtype=torch.int64).contiguous()
         if action_dims is not None:
             actions = sample_factored(logits, action_dims, stream_ids, seed=self.seed, step=self.step)
+            self.step += T
+            return actions
+        if continuous_dim is not None:
+            actions = sample_gaussian(logits, continuous_dim, stream_ids, seed=self.seed, step=self.step)
             self.step += T
             return actions
         actions = torch.empty(T, B, dtype=torch.int64, device=logits.device)
@@ -80,4 +87,20 @@ def sample_factored(logits, action_dims, stream_ids=None, seed=0, step=0, seed_s
             _lib.ptr(logits), T, B, A, seed % 2 ** 64, step % 2 ** 64, _lib.ptr(seed_step), _lib.ptr(stream_ids),
             ctypes.byref(action_space.c_space(dims)), _lib.ptr(actions), _lib.stream_ptr()),
         "tb_sample_actions_factored_f32")
+    return actions
+
+
+def sample_gaussian(logits, continuous_dim, stream_ids=None, seed=0, step=0, seed_step=None):
+    """tb_sample_gaussian_f32 on contiguous float32 rows [T, B, 2D] (mu, log sigma) -> float32 [T, B, D], D =
+    continuous_dim.  (seed, step) and stream_ids as in sample_factored."""
+    T, B, A = logits.shape
+    if A != 2 * int(continuous_dim):
+        raise _lib.TorchBeastB200Error("a Gaussian(%d) policy takes rows [T, B, %d], got %r"
+                                       % (continuous_dim, 2 * int(continuous_dim), tuple(logits.shape)))
+    actions = torch.empty(T, B, int(continuous_dim), dtype=torch.float32, device=logits.device)
+    _lib.check(
+        _lib.lib().tb_sample_gaussian_f32(
+            _lib.ptr(logits), T, B, A, seed % 2 ** 64, step % 2 ** 64, _lib.ptr(seed_step), _lib.ptr(stream_ids),
+            _lib.ptr(actions), _lib.stream_ptr()),
+        "tb_sample_gaussian_f32")
     return actions

@@ -37,9 +37,15 @@ def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), e
     frame_format="unstacked": the frame leaf is [T+4, B, H, W], one newest frame per step after step 0's first three
     channels; the learner rebuilds the stacks on the GPU (include/torchbeast_b200.h, "unstacked rollouts").
     num_actions a tuple (A_1, ..., A_D): a factored action space (torchbeast_b200.action_space), whose policy_logits
-    are [T+1, B, sum A_k] and whose action and last_action are [T+1, B, D]."""
+    are [T+1, B, sum A_k] and whose action and last_action are [T+1, B, D].  num_actions a Gaussian(D): a continuous
+    space, whose policy_logits are the (mu, log sigma) rows [T+1, B, 2D] and whose action and last_action are float32
+    [T+1, B, D]."""
     dims = action_space.dims_of(num_actions)
+    D = action_space.continuous_dim_of(num_actions)
     act = (T + 1, B) if dims is None else (T + 1, B, len(dims))
+    act_dtype = torch.int64
+    if D is not None:
+        act, act_dtype = (T + 1, B, D), torch.float32
     num_actions = action_space.width(num_actions)
     if frame_format not in FRAME_FORMATS:
         raise ValueError("frame_format must be one of %s, got %r" % (FRAME_FORMATS, frame_format))
@@ -53,10 +59,10 @@ def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), e
         episode_step=((T1, B), torch.int32),
         policy_logits=((T1, B, num_actions), torch.float32),
         baseline=((T1, B), torch.float32),
-        action=(act, torch.int64),
+        action=(act, act_dtype),
     )
     if use_last_action:
-        spec["last_action"] = (act, torch.int64)
+        spec["last_action"] = (act, act_dtype)
     for name, shape, dtype in extra:
         spec[name] = (tuple(shape), dtype)
     return spec
