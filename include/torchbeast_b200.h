@@ -537,6 +537,74 @@ int tb_atarinet_backward_continuous(const float* grad_logits, const float* grad_
                                     const float* params, int64_t T1, int64_t B, int num_actions, int num_values,
                                     int use_lstm, int precision, void* workspace, float* grads, int phase, void* stream);
 
+/* ---- MLPNet: vector observations -------------------------------------------------------------------------------
+ * AtariNet with its conv trunk and fc replaced by dense layers, for float32 observation vectors of O features:
+ *   x = obs [T1*B, O];  with normalisation x = clamp((x - mean) * inv_std, -10, 10) (below);
+ *   x = relu(x W_i^T + b_i) for i = 0 .. L-1, W_i [H_i, H_{i-1}] (H_{-1} = O);
+ *   core_in = cat[x, clamp(reward, -1, 1), last-action encoding] of width F = H_{L-1} + 1 + E;
+ *   [2-layer LSTM of width F with done-reset]; policy [A, F] / baseline [num_values, F] heads.
+ * The last-action encoding is AtariNet's: one-hot over A (E = A, last_action int64 [T1,B]) with space == NULL and
+ * continuous_dim == 0; a K-hot (E = A, last_action int64 [T1,B,D]) with a factored space (tb_action_space, see
+ * "multi-discrete (factored) action spaces"); the raw values (E = D, last_action float32 [T1,B,D]) with continuous_dim
+ * = D > 0 and num_actions = 2D (see "continuous (diagonal-Gaussian) action spaces").  Giving both is rejected.
+ * Limits: 1 <= O <= TB_MLP_MAX_OBS; 1 to TB_MLP_MAX_LAYERS hidden widths, each a multiple of 8 in [8, TB_MLP_MAX_WIDTH]
+ * (the row stride rule of the bf16 operands); 1 <= A <= 31 (the heads); with the LSTM F <= TB_LSTM_MAX_HIDDEN.
+ * Parameters, in one flat fp32 buffer in this order: W_0, b_0, ..., W_{L-1}, b_{L-1}, then AtariNet's LSTM (with F),
+ * policy and baseline layout; tb_mlpnet_param_count counts them (-1: a rejected config).
+ *
+ * Observation normalisation (cfg->normalize != 0): obs_mean / obs_var are float64 [O].  The staged operand is, in fp32,
+ *   mean_f[j] = (float)obs_mean[j];  inv_std_f[j] = (float)(1.0 / sqrt(obs_var[j] + 1e-8))   (both formed in float64),
+ *   y = (x - mean_f[j]) * inv_std_f[j]  (two fp32 roundings, no FMA);  y < -10 ? -10 : (y > 10 ? 10 : y)
+ * so a NaN observation stays NaN.  The clip of 10 and the eps of 1e-8 are fixed (VecNormalize's defaults).  Without
+ * normalisation y = x.  precision 0 stages y as fp32 [N, O]; 1 and 2 as bf16 [N, ld] with ld = O rounded up to a
+ * multiple of 8 and columns [O, ld) zero: hi = bf16_rn(y), and at precision 2 the lo plane bf16_rn(y - hi) follows at
+ * N * ld elements.  tb_obs_stage runs that staging alone into `out`.
+ *
+ * tb_mlpnet_forward / tb_mlpnet_backward: the contract of tb_atarinet_forward / tb_atarinet_backward (phase 3) with
+ * float32 observations in place of the frames: reward, notdone, h0/c0/hN/cN [2,B,F] and the outputs as there;
+ * precision 0 = fp32 SIMT GEMMs, 1 = bf16, 2 = split-bf16 tensor-core GEMMs.  The backward reads only the workspace
+ * the forward left (tb_mlpnet_workspace_bytes bytes, 0: a rejected config) and overwrites grads; the observations and
+ * the statistics get no gradient.                                                                                    */
+#define TB_MLP_MAX_OBS 4096
+#define TB_MLP_MAX_LAYERS 4
+#define TB_MLP_MAX_WIDTH 512
+#define TB_OBS_NORM_EPS 1e-8
+#define TB_OBS_NORM_CLIP 10.0f
+typedef struct tb_mlp_config {
+  int obs_dim;                     /* O */
+  int num_layers;                  /* L */
+  int hidden[TB_MLP_MAX_LAYERS];   /* H_0 .. H_{L-1}; later entries are not read */
+  int num_actions;                 /* A: the policy width (2D for a continuous space) */
+  int num_values;                  /* value outputs (PopArt tasks), 1 .. 64 */
+  int use_lstm;
+  int normalize;                   /* stage the observations normalised by obs_mean / obs_var */
+} tb_mlp_config;
+int64_t tb_mlpnet_param_count(const tb_mlp_config* cfg, const tb_action_space* space, int continuous_dim);
+size_t tb_mlpnet_workspace_bytes(const tb_mlp_config* cfg, const tb_action_space* space, int continuous_dim, int64_t T1,
+                                 int64_t B, int precision);
+int tb_mlpnet_forward(const float* obs, const float* reward, const float* notdone, const void* last_action,
+                      const float* h0, const float* c0, const float* params, const double* obs_mean,
+                      const double* obs_var, const tb_mlp_config* cfg, const tb_action_space* space, int continuous_dim,
+                      int64_t T1, int64_t B, int precision, void* workspace, float* policy_logits, float* baseline,
+                      float* hN, float* cN, void* stream);
+int tb_mlpnet_backward(const float* grad_logits, const float* grad_baseline, const float* notdone, const float* params,
+                       const tb_mlp_config* cfg, const tb_action_space* space, int continuous_dim, int64_t T1,
+                       int64_t B, int precision, void* workspace, float* grads, void* stream);
+int tb_obs_stage(const float* obs, int64_t N, int O, const double* obs_mean, const double* obs_var, int precision,
+                 void* out, void* stream);
+/* Running observation statistics, per feature j (count, mean, var: float64 [O], initially 0, 0 and 1).
+ * tb_obs_norm_sums: sums [3, O] float64 = {number of finite entries, sum x, sum x^2} of feature j over the rows (t, b)
+ *   with t_begin <= t < T1 and b < Bf of obs [T1, B, O]; non-finite entries are skipped.  A fixed summation order and
+ *   no atomics: bit-identical from run to run.
+ * tb_obs_norm_update: merges sums into the statistics (parallel variance).  With n_b = sums[0][j] > 0:
+ *   m_b = S / n_b;  v_b = max(S2 / n_b - m_b^2, 0);  tot = count + n_b;  d = m_b - mean;
+ *   mean' = mean + d * n_b / tot;  var' = (var * count + v_b * n_b + d^2 * count * n_b / tot) / tot;  count' = tot;
+ *   a feature with n_b = 0 is unchanged.  So the first update takes the batch's own mean and variance.
+ * One launch each, no host synchronisation: both can be captured in a CUDA graph.                                    */
+int tb_obs_norm_sums(const float* obs, int64_t T1, int64_t B, int O, int64_t t_begin, int64_t Bf, double* sums,
+                     void* stream);
+int tb_obs_norm_update(const double* sums, double* count, double* mean, double* var, int O, void* stream);
+
 /* ---- stacked LSTM over the unroll with per-step done-reset -------------------------------------------
  * Replaces the reference's loop of seq_len-1 nn.LSTM calls and its autograd graph (monobeast.py:603-611,
  * polybeast_learner.py:241-249):   for t: state *= notdone_t;  y_t, state = LSTM(x_t, state).

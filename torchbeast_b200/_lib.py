@@ -51,6 +51,13 @@ _SIGNATURES = {
     "tb_atarinet_workspace_bytes_continuous": ([_i64, _i64, _int, _int, _int], _c.c_size_t),
     "tb_atarinet_forward_continuous": ([_vp] * 8 + [_i64, _i64, _int, _int, _int, _int] + [_vp] * 7, _int),
     "tb_atarinet_backward_continuous": ([_vp] * 4 + [_i64, _i64, _int, _int, _int, _int, _vp, _vp, _int, _vp], _int),
+    "tb_mlpnet_param_count": ([_vp, _vp, _int], _i64),
+    "tb_mlpnet_workspace_bytes": ([_vp, _vp, _int, _i64, _i64, _int], _c.c_size_t),
+    "tb_mlpnet_forward": ([_vp] * 11 + [_int, _i64, _i64, _int] + [_vp] * 6, _int),
+    "tb_mlpnet_backward": ([_vp] * 6 + [_int, _i64, _i64, _int, _vp, _vp, _vp], _int),
+    "tb_obs_stage": ([_vp, _i64, _int, _vp, _vp, _int, _vp, _vp], _int),
+    "tb_obs_norm_sums": ([_vp, _i64, _i64, _int, _i64, _i64, _vp, _vp], _int),
+    "tb_obs_norm_update": ([_vp] * 4 + [_int, _vp], _int),
     "tb_resnet_obs_range": ([_vp], _int),
     "tb_resnet_widths": ([_vp], _int),
     "tb_resnet_supported": ([_int] * 7, _int),

@@ -229,7 +229,12 @@ class GraphedActor:
         frame, history = inputs["frame"], model.frame_history
         obs = tuple(getattr(model, "observation_shape", nets.ATARI_SHAPE))
         newest = history is not None and frame.dim() == 4
-        if (frame.dim() != 5 and not newest) or (frame.dim() == 5 and tuple(frame.shape[2:]) != obs):
+        if len(obs) != 3:  # a vector observation (MLPNet): frame [1, B, O], and no frame_history
+            if history is not None or frame.dim() != 2 + len(obs) or tuple(frame.shape[2:]) != obs:
+                raise _lib.TorchBeastB200Error("GraphedActor takes observations [1, B, %s] for this net%s, got frame %r"
+                                               % (", ".join(map(str, obs)), "" if history is None else
+                                                  " and no frame_history", tuple(frame.shape)))
+        elif (frame.dim() != 5 and not newest) or (frame.dim() == 5 and tuple(frame.shape[2:]) != obs):
             raise _lib.TorchBeastB200Error("GraphedActor takes stacked frames [1, B, %d, %d, %d]; unstacked rollouts are a "
                                            "learner input, got frame %r" % (obs + (tuple(inputs["frame"].shape),)))
         if history is not None and obs != nets.ATARI_SHAPE:

@@ -520,6 +520,11 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
     `fresh_columns` (a replay-mixed batch, see torchbeast_b200.replay): the stats' episode returns come from columns
     [0, fresh_columns) only, so a replayed episode end is not counted twice; the losses cover the whole batch.
 
+    A model with running observation statistics (an MLPNet built with normalize_observations=True, model.obs_norm)
+    merges rows 1..T of the fresh columns [0, fresh_columns) of batch["frame"] into them after the optimizer step (two
+    launches; the sums SUM all-reduced when data-parallel), before the actor copy, which takes the new statistics.  The
+    step's own forward normalised with the statistics as they were before it.
+
     `draw` (a prioritised buffer's replay.Draw, or one built by hand): with `draw.weights` the loss is the importance-
     weighted one (impala_loss_fwd_bwd with column_weights), so the stats' loss values are the weighted sums; with
     `draw.buffer` its priorities are updated from the loss's vs and values at `draw.slots`, right after the loss.
@@ -615,6 +620,12 @@ def learn_step(flags, model, actor_model, batch, initial_agent_state, optimizer,
             popart_beta_dev = torch.full((1,), popart_beta(flags), dtype=torch.float64, device=task_sums.device)
         weight, bias = model.value_head()
         popart_update(task_sums, popart_beta_dev, pop.mu, pop.nu, weight, bias)
+    if getattr(model, "obs_norm", None) is not None:
+        obs_sums = model.obs_norm_sums(batch["frame"], fresh_columns)
+        if _dp_world() > 1:
+            import torch.distributed as dist
+            dist.all_reduce(obs_sums, op=dist.ReduceOp.SUM)  # every rank merges the global batch's rows
+        model.obs_norm_update(obs_sums)
     if scheduler is not None:
         scheduler.step()
     if actor_model is not None and actor_model is not model:
@@ -730,6 +741,9 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
     * a model with a continuous action space (Gaussian(D)) learns on float32 action [T+1, B, D] on every path above;
       UPGO, kickstarting, a legal_actions leaf, a teacher with another space or integer actions raise before anything
       is staged.
+    * an MLPNet (float32 observation vectors) learns on a float32 frame leaf [T+1, B, O] on every path above; a
+      frame_history, an unstacked or uint8 frame leaf or another O raise before anything is staged.  With
+      normalize_observations its running statistics are updated after each step (learn_step), inside the graph too.
     * with flags.kickstart_cost, the teacher attached as model.teacher (torchbeast_b200.kickstart.Teacher) runs on the
       same (mixed) batch and its KL term joins the loss (learn_step); the teacher is part of the graph's structure.
     Returns the reference's stats dict."""
@@ -740,6 +754,8 @@ def learn(flags, model, actor_model, batch, initial_agent_state, optimizer, sche
     _check_legal(batch)
     teacher = _teacher_for(model, actor_model, kickstart_cost(flags))
     _action_space.check_learner(model, flags, batch, teacher_of(model))
+    if hasattr(model, "check_batch"):  # MLPNet: a float32 [T+1, B, O] frame leaf
+        model.check_batch(batch)
     needs_last_action = getattr(model, "needs_last_action", False) or (
         teacher is not None and getattr(teacher.net, "needs_last_action", False))
     slot = None
@@ -920,8 +936,10 @@ class GraphedLearner:
             self.mixing = self.replay.mixing(self.fresh_columns)
             replay_saved = self.replay.save(3)  # the two warm-up steps and the upload replay below each insert once
         # warm up on a side stream (allocations, one-time attribute calls), then capture
+        self.obs_norm = getattr(model, "obs_norm", None)
         snapshot = (model.flat_params.clone(), optimizer.snapshot(),
-                    None if self.popart is None else (self.popart.mu.clone(), self.popart.nu.clone()))
+                    None if self.popart is None else (self.popart.mu.clone(), self.popart.nu.clone()),
+                    None if self.obs_norm is None else tuple(t.clone() for t in self.obs_norm.tensors()))
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -951,6 +969,9 @@ class GraphedLearner:
         if self.popart is not None:
             self.popart.mu.copy_(snapshot[2][0])
             self.popart.nu.copy_(snapshot[2][1])
+        if self.obs_norm is not None:
+            for dst, src in zip(self.obs_norm.tensors(), snapshot[3]):
+                dst.copy_(src)
         if actor_model is not None and hasattr(actor_model, "copy_params_from"):
             actor_model.copy_params_from(model)
         if replay_saved is not None:
@@ -965,6 +986,7 @@ class GraphedLearner:
             draw = self.replay.last_draw if self.replay.prioritized else None
         return learn_step(self.flags, self.model, self.actor, batch, state, self.opt, None, stats_sync=False,
                           hparams_dev=self.hparams, popart_beta_dev=self.popart_beta, draw=draw,
+                          fresh_columns=self.fresh_columns if self.replay is not None else None,
                           trust_beta_dev=self.trust_beta, upgo_cost_dev=self.upgo_cost,
                           kickstart_cost_dev=self.kickstart_cost)
 

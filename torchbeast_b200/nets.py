@@ -61,6 +61,37 @@ class PopArt(nn.Module):
         return (self.sigma()[task] * n + self.mu[task]).to(torch.float32)
 
 
+class ObsNorm(nn.Module):
+    """Running observation statistics of an MLPNet built with normalize_observations=True: float64 [O] buffers `mean`,
+    `var` and `count` (state_dict keys obs_norm.mean, obs_norm.var, obs_norm.count), starting at 0, 1 and 0.  The net
+    stages x as clamp((x - mean) * rsqrt(var + 1e-8), -10, 10) (include/torchbeast_b200.h, "MLPNet"); learn() merges
+    each step's fresh observations into them after the optimizer step."""
+
+    KEYS = ("obs_norm.mean", "obs_norm.var", "obs_norm.count")
+    CLIP = 10.0   # TB_OBS_NORM_CLIP
+    EPS = 1e-8    # TB_OBS_NORM_EPS
+
+    def __init__(self, size, device):
+        super().__init__()
+        self.register_buffer("mean", torch.zeros(size, dtype=torch.float64, device=device))
+        self.register_buffer("var", torch.ones(size, dtype=torch.float64, device=device))
+        self.register_buffer("count", torch.zeros(size, dtype=torch.float64, device=device))
+
+    def _apply(self, fn, recurse=True):
+        # the statistics stay float64 through .float() and the like
+        super()._apply(fn, recurse)
+        for key, buf in list(self._buffers.items()):
+            self._buffers[key] = buf.to(torch.float64)
+        return self
+
+    def copy_from(self, other):
+        for name in ("mean", "var", "count"):
+            getattr(self, name).copy_(getattr(other, name), non_blocking=True)
+
+    def tensors(self):
+        return self.mean, self.var, self.count
+
+
 def atarinet_param_spec(num_actions, use_lstm, in_channels=4, num_values=1, continuous_dim=None):
     """continuous_dim D (a Gaussian(D) space, num_actions = 2D): the core takes D last-action columns, 512 + D + 1."""
     core = 512 + (num_actions if continuous_dim is None else continuous_dim) + 1
@@ -284,6 +315,8 @@ class FlatParamModule(nn.Module):
                 self._buffers[key] = fn(buf)
         if getattr(self, "popart", None) is not None:
             self.popart._apply(fn)
+        if getattr(self, "obs_norm", None) is not None:
+            self.obs_norm._apply(fn)
         return self
 
     @property
@@ -312,11 +345,13 @@ class FlatParamModule(nn.Module):
 
     def copy_params_from(self, other):
         """actor_model.load_state_dict(model.state_dict()) as ONE device copy (monobeast.py:295), plus the PopArt
-        statistics when both nets have them."""
+        statistics and the observation statistics when both nets have them."""
         self._flat.copy_(other._flat, non_blocking=True)
         if getattr(self, "popart", None) is not None and getattr(other, "popart", None) is not None:
             self.popart.mu.copy_(other.popart.mu, non_blocking=True)
             self.popart.nu.copy_(other.popart.nu, non_blocking=True)
+        if getattr(self, "obs_norm", None) is not None and getattr(other, "obs_norm", None) is not None:
+            self.obs_norm.copy_from(other.obs_norm)
 
     def _aliased_sibling(self, state_dict):
         """The FlatParamModule whose live flat buffer EVERY tensor of `state_dict` aliases at this module's own
@@ -342,15 +377,16 @@ class FlatParamModule(nn.Module):
         """Reference checkpoints / state_dicts load key by key; `actor.load_state_dict(model.state_dict())`
         (monobeast.py:295) is recognised by aliasing and becomes ONE device copy.  The dict itself carries nothing
         but tensors, so torch.save / torch.load(weights_only=True) / copy.deepcopy behave as for any nn.Module."""
-        stats = ("popart.mu", "popart.nu")
-        has_stats = getattr(self, "popart", None) is not None and all(k in state_dict for k in stats)
+        stats = (("popart.mu", "popart.nu") if getattr(self, "popart", None) is not None else ()) + (
+            ObsNorm.KEYS if getattr(self, "obs_norm", None) is not None else ())
+        has_stats = bool(stats) and all(k in state_dict for k in stats)
         params = {k: v for k, v in state_dict.items() if k not in stats} if has_stats else state_dict
         src = self._aliased_sibling(params)
         if src is not None:
             self.copy_params_from(src)
-            if has_stats:  # from any net with the same number of tasks (its statistics may be host tensors)
-                self.popart.mu.copy_(state_dict["popart.mu"])
-                self.popart.nu.copy_(state_dict["popart.nu"])
+            if has_stats:  # from any net with the same statistics' sizes (they may be host tensors)
+                for k in stats:
+                    self.get_buffer(k).copy_(state_dict[k])
             return torch.nn.modules.module._IncompatibleKeys([], [])
         return super().load_state_dict(state_dict, strict=strict)
 
@@ -814,6 +850,294 @@ class ResNet(FlatParamModule):
         T, B = baseline.shape[:2]
         action = self._sample(logits, inputs) if self.training else self._greedy(logits)
         return (action.view((T, B) + action.shape[2:]), logits, baseline), ((hN, cN) if self.use_lstm else tuple())
+
+
+class MLPConfig(ctypes.Structure):
+    """tb_mlp_config (include/torchbeast_b200.h)."""
+    _fields_ = [("obs_dim", ctypes.c_int), ("num_layers", ctypes.c_int), ("hidden", ctypes.c_int * 4),
+                ("num_actions", ctypes.c_int), ("num_values", ctypes.c_int), ("use_lstm", ctypes.c_int),
+                ("normalize", ctypes.c_int)]
+
+
+MLP_MAX_OBS = 4096     # TB_MLP_MAX_OBS
+MLP_MAX_LAYERS = 4     # TB_MLP_MAX_LAYERS
+MLP_MAX_WIDTH = 512    # TB_MLP_MAX_WIDTH
+
+
+def mlpnet_param_spec(obs_dim, hidden, num_actions, use_lstm, num_values=1, continuous_dim=None):
+    """State_dict order / shapes of MLPNet: torso.i.weight [H_i, H_{i-1}] (H_{-1} = obs_dim) and torso.i.bias [H_i],
+    then AtariNet's core.*, policy.* and baseline.* with the core width hidden[-1] + E + 1 (E = num_actions, or D for a
+    Gaussian(D) space)."""
+    spec, fan_in = [], obs_dim
+    for i, h in enumerate(hidden):
+        spec += [("torso.%d.weight" % i, (h, fan_in)), ("torso.%d.bias" % i, (h,))]
+        fan_in = h
+    core = hidden[-1] + (num_actions if continuous_dim is None else continuous_dim) + 1
+    if use_lstm:
+        for layer in range(2):
+            spec += [
+                ("core.weight_ih_l%d" % layer, (4 * core, core)), ("core.weight_hh_l%d" % layer, (4 * core, core)),
+                ("core.bias_ih_l%d" % layer, (4 * core,)), ("core.bias_hh_l%d" % layer, (4 * core,)),
+            ]
+    spec += [
+        ("policy.weight", (num_actions, core)), ("policy.bias", (num_actions,)),
+        ("baseline.weight", (num_values, core)), ("baseline.bias", (num_values,)),
+    ]
+    return spec
+
+
+class _MLPNetFunction(torch.autograd.Function):
+    """Autograd bridge of MLPNet, as _AtariNetFunction's."""
+
+    @staticmethod
+    def forward(ctx, module, frame, reward, notdone, last_action, h0, c0, *params):
+        logits, baseline, hN, cN = module._launch_forward(frame, reward, notdone, last_action, h0, c0)
+        ctx.module, ctx.notdone, ctx.shape = module, notdone, baseline.shape
+        ctx.mark_non_differentiable(hN, cN)
+        return logits, baseline, hN, cN
+
+    @staticmethod
+    def backward(ctx, g_logits, g_baseline, _ghn, _gcn):
+        module = ctx.module
+        T1, B = ctx.shape[:2]
+        if g_logits is None:
+            g_logits = torch.zeros(T1, B, module.num_actions, device=module._flat.device)
+        if g_baseline is None:
+            g_baseline = torch.zeros(module._baseline_shape(T1, B), device=module._flat.device)
+        grads = torch.empty_like(module._flat)
+        module._launch_backward(g_logits.contiguous(), g_baseline.contiguous(), ctx.notdone, grads)
+        return (None,) * 7 + tuple(grads[off:off + n].view(shape) for _, off, n, shape in module._views)
+
+
+class MLPNet(FlatParamModule):
+    """CUDA MLP net for float32 observation vectors [T, B, O] (include/torchbeast_b200.h, "MLPNet"): AtariNet with
+    its conv trunk and fc replaced by dense layers.  [normalise] -> relu(x W_i^T + b_i) per hidden width ->
+    cat[x, clip(reward), last-action encoding] -> optional 2-layer LSTM -> policy / baseline heads.
+
+    observation_size: O (an int or (O,)), 1 .. 4096.  hidden: 1 to 4 widths, each a multiple of 8 in [8, 512].
+    num_actions: an int, a tuple of component sizes or a Gaussian(D), as for AtariNet; num_tasks: PopArt heads.
+    normalize_observations: keep running float64 statistics (model.obs_norm, ObsNorm) and stage the observations as
+    clamp((x - mean) * rsqrt(var + 1e-8), -10, 10); learn() updates them from each step's fresh rows 1..T.
+    precision: "bf16x3" (default), "bf16" or "fp32", as for AtariNet.  A frame_history and unstacked frames do not
+    apply to vector observations."""
+
+    PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2}
+    DEFAULT_PRECISION = "bf16x3"
+    needs_last_action = True
+
+    def __init__(self, observation_size, num_actions, hidden=(256, 256), use_lstm=False, device=None, precision=None,
+                 num_tasks=None, normalize_observations=False):
+        super().__init__()
+        obs = observation_size if isinstance(observation_size, (tuple, list, torch.Size)) else (observation_size,)
+        if len(obs) != 1 or isinstance(obs[0], bool) or not isinstance(obs[0], int) or not 1 <= obs[0] <= MLP_MAX_OBS:
+            raise _lib.TorchBeastB200Error("MLPNet observation_size must be an int O in [1, %d] (or (O,)), got %r"
+                                           % (MLP_MAX_OBS, observation_size))
+        self.observation_shape = (int(obs[0]),)
+        try:
+            hid = tuple(hidden)
+        except TypeError:
+            hid = ()
+        if not 1 <= len(hid) <= MLP_MAX_LAYERS or not all(
+                isinstance(h, int) and not isinstance(h, bool) and 8 <= h <= MLP_MAX_WIDTH and h % 8 == 0 for h in hid):
+            raise _lib.TorchBeastB200Error(
+                "MLPNet hidden must be 1 to %d widths, each a multiple of 8 in [8, %d], got %r"
+                % (MLP_MAX_LAYERS, MLP_MAX_WIDTH, hidden))
+        self.hidden = hid
+        self._set_action_space(num_actions)
+        num_actions = self.num_actions
+        if num_actions > HEADS_MAX_OUTPUTS:
+            raise _lib.TorchBeastB200Error("the policy head takes at most %d outputs, got num_actions=%r"
+                                           % (HEADS_MAX_OUTPUTS, num_actions))
+        self.use_lstm = use_lstm
+        D = self.continuous_dim
+        self.core_size = hid[-1] + (num_actions if D is None else D) + 1
+        if use_lstm and self.core_size > LSTM_MAX_HIDDEN:
+            raise _lib.TorchBeastB200Error("MLPNet with an LSTM needs H_last + %s + 1 <= %d, got %d"
+                                           % ("D" if D is not None else "sum(num_actions)" if self.action_dims
+                                              else "num_actions", LSTM_MAX_HIDDEN, self.core_size))
+        if device is None:
+            device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+        popart = None if num_tasks is None else PopArt(num_tasks, device)
+        self.num_values = 1 if popart is None else popart.num_tasks
+        self._build_flat(mlpnet_param_spec(self.observation_shape[0], hid, num_actions, use_lstm,
+                                           num_values=self.num_values, continuous_dim=D), device)
+        self.reset_parameters_like_torch()
+        if popart is not None:
+            self.popart = popart  # registered after the parameters: its keys come next in the state_dict
+        self.obs_norm = ObsNorm(self.observation_shape[0], device) if normalize_observations else None
+        if use_lstm:
+            self.core.num_layers = 2
+            self.core.hidden_size = self.core_size
+            self.core.input_size = self.core_size
+        self.precision = precision or self.DEFAULT_PRECISION
+        if self.precision not in self.PRECISIONS:
+            raise _lib.TorchBeastB200Error("precision must be one of %s" % sorted(self.PRECISIONS))
+        self._ws = None
+        self._ws_key = None
+        self._scratch_buf = self._scratch_key = None
+        count = _lib.lib().tb_mlpnet_param_count(*self._c_args())
+        assert count == self._total, "parameter layout disagrees with the C-ABI (%d vs %d)" % (count, self._total)
+
+    def _c_args(self):
+        """(config, action space, continuous_dim) as the tb_mlpnet_* entries take them."""
+        cfg = MLPConfig()
+        cfg.obs_dim, cfg.num_layers = self.observation_shape[0], len(self.hidden)
+        for i, h in enumerate(self.hidden):
+            cfg.hidden[i] = h
+        cfg.num_actions, cfg.num_values = self.num_actions, self.num_values
+        cfg.use_lstm, cfg.normalize = int(bool(self.use_lstm)), int(self.obs_norm is not None)
+        self._cfg = cfg  # kept alive for the call
+        space = None if self.action_dims is None else ctypes.byref(action_space.c_space(self.action_dims))
+        return ctypes.byref(cfg), space, int(self.continuous_dim or 0)
+
+    def initial_state(self, batch_size):
+        if not self.use_lstm:
+            return tuple()
+        return tuple(torch.zeros(2, batch_size, self.core_size, device=self._flat.device) for _ in range(2))
+
+    def _workspace(self, T1, B):
+        key = (T1, B, self._flat.device, self.precision)
+        if self._ws_key != key:
+            nbytes = _lib.lib().tb_mlpnet_workspace_bytes(*self._c_args(), T1, B, self.PRECISIONS[self.precision])
+            if nbytes == 0:
+                raise _lib.TorchBeastB200Error("tb_mlpnet_workspace_bytes: %s" % _lib.lib().tb_last_error().decode())
+            self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self._flat.device)
+            self._ws_key = key
+        return self._ws
+
+    def check_frame(self, frame, what="frame"):
+        """Raises unless `frame` is float32 [T, B, O] and no frame_history is attached (before anything is launched)."""
+        O = self.observation_shape[0]
+        if self.frame_history is not None:
+            raise _lib.TorchBeastB200Error("a frame_history rebuilds (4, 84, 84) stacks; MLPNet takes float32 "
+                                           "observations [T,B,%d]: detach the history (model.frame_history = None)" % O)
+        if not isinstance(frame, torch.Tensor) or frame.dtype != torch.float32 or frame.dim() != 3 \
+                or frame.shape[2] != O:
+            raise _lib.TorchBeastB200Error("MLPNet takes %s float32 [T,B,%d] (unstacked and uint8 frames do not apply), "
+                                           "got %s" % (what, O, "%s %r" % (frame.dtype, tuple(frame.shape))
+                                                       if isinstance(frame, torch.Tensor) else type(frame).__name__))
+
+    def check_batch(self, batch):
+        """learn()'s check of a rollout batch's frame leaf, before anything is staged."""
+        if isinstance(batch, dict) and "frame" in batch:
+            self.check_frame(batch["frame"], "a frame leaf")
+
+    def _launch_forward(self, frame, reward, notdone, last_action, h0, c0):
+        self.check_frame(frame)
+        _lib.require_cuda(frame, reward, last_action, self._flat)
+        T1, B = frame.shape[:2]
+        if tuple(reward.shape[:2]) != (T1, B):
+            raise _lib.TorchBeastB200Error("reward must be [T, B] = %r, got %r" % ((T1, B), tuple(reward.shape)))
+        dev = self._flat.device
+        frame = frame.contiguous()
+        reward = reward.to(torch.float32).contiguous()
+        D = self.continuous_dim
+        if D is not None:
+            if last_action.dtype != torch.float32 or tuple(last_action.shape) != (T1, B, D):
+                raise _lib.TorchBeastB200Error("last_action must be float32 [T, B, D] = %r for Gaussian(%d), got %s %r"
+                                               % ((T1, B, D), D, last_action.dtype, tuple(last_action.shape)))
+            last_action = last_action.contiguous()
+        else:
+            want = (T1, B) if self.action_dims is None else (T1, B, len(self.action_dims))
+            if tuple(last_action.shape) != want:
+                raise _lib.TorchBeastB200Error("last_action must be int64 %r for num_actions=%r, got %r"
+                                               % (want, self.action_dims or self.num_actions,
+                                                  tuple(last_action.shape)))
+            last_action = last_action.to(torch.int64).contiguous()
+        logits = torch.empty(T1, B, self.num_actions, dtype=torch.float32, device=dev)
+        baseline = torch.empty(self._baseline_shape(T1, B), dtype=torch.float32, device=dev)
+        if self.use_lstm:
+            hN = torch.empty(2, B, self.core_size, dtype=torch.float32, device=dev)
+            cN = torch.empty_like(hN)
+            h0 = h0.to(torch.float32).contiguous(); c0 = c0.to(torch.float32).contiguous()
+        else:
+            hN = cN = torch.empty(0, device=dev)
+            h0 = c0 = notdone = None
+        mean = var = None
+        if self.obs_norm is not None:
+            mean, var = self.obs_norm.mean, self.obs_norm.var
+        p = _lib.ptr
+        _lib.check(
+            _lib.lib().tb_mlpnet_forward(
+                p(frame), p(reward), p(notdone), p(last_action), p(h0), p(c0), p(self._flat), p(mean), p(var),
+                *self._c_args(), T1, B, self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(logits),
+                p(baseline), p(hN) if self.use_lstm else None, p(cN) if self.use_lstm else None, _lib.stream_ptr()),
+            "tb_mlpnet_forward")
+        return logits, baseline, hN, cN
+
+    def _launch_backward(self, g_logits, g_baseline, notdone, grads_out):
+        T1, B = g_baseline.shape[:2]
+        p = _lib.ptr
+        _lib.check(
+            _lib.lib().tb_mlpnet_backward(
+                p(g_logits), p(g_baseline), p(notdone) if self.use_lstm else None, p(self._flat), *self._c_args(), T1,
+                B, self.PRECISIONS[self.precision], p(self._workspace(T1, B)), p(grads_out), _lib.stream_ptr()),
+            "tb_mlpnet_backward")
+
+    _notdone = staticmethod(AtariNet._notdone)
+
+    # ---- learner fast path (no autograd graph) ----------------------------------------------
+    @torch.no_grad()
+    def learner_forward(self, inputs, core_state=()):
+        notdone = self._notdone(inputs["done"]) if self.use_lstm else None
+        h0, c0 = core_state if self.use_lstm else (None, None)
+        logits, baseline, hN, cN = self._launch_forward(inputs["frame"], inputs["reward"], notdone,
+                                                        inputs["last_action"], h0, c0)
+        self._saved_notdone = notdone
+        return LearnerOutputs(mask_policy(logits, inputs), baseline, (hN, cN) if self.use_lstm else tuple())
+
+    @torch.no_grad()
+    def learner_backward(self, grad_logits, grad_baseline):
+        """Writes d loss / d params into flat_grad (and points every .grad at its slice)."""
+        fg = self.attach_grads()
+        self._launch_backward(grad_logits, grad_baseline, self._saved_notdone, fg)
+        return fg
+
+    # ---- running observation statistics -------------------------------------------------------
+    @torch.no_grad()
+    def obs_norm_sums(self, frame, fresh_columns=None):
+        """float64 [3, O] = per feature {finite entries, sum x, sum x^2} over rows 1..T of columns [0, fresh_columns)
+        (default: all) of a rollout's frame leaf [T+1, B, O] (tb_obs_norm_sums): row 0 repeats the previous rollout's
+        last frame, and replayed columns were counted when they were fresh."""
+        self.check_frame(frame)
+        _lib.require_cuda(frame)
+        T1, B, O = frame.shape
+        Bf = B if fresh_columns is None else int(fresh_columns)
+        frame = frame.contiguous()
+        sums = torch.empty(3, O, dtype=torch.float64, device=frame.device)
+        _lib.check(_lib.lib().tb_obs_norm_sums(_lib.ptr(frame), T1, B, O, 1, Bf, _lib.ptr(sums),
+                                               _lib.stream_ptr()), "tb_obs_norm_sums")
+        return sums
+
+    @torch.no_grad()
+    def obs_norm_update(self, sums):
+        """Merge obs_norm_sums' output (SUM all-reduced first when data-parallel) into model.obs_norm
+        (tb_obs_norm_update)."""
+        n = self.obs_norm
+        _lib.require_cuda(sums)
+        if sums.dtype != torch.float64 or tuple(sums.shape) != (3, n.mean.numel()) or not sums.is_contiguous():
+            raise _lib.TorchBeastB200Error("obs_norm_update takes contiguous float64 [3, %d], got %s %r"
+                                           % (n.mean.numel(), sums.dtype, tuple(sums.shape)))
+        _lib.check(_lib.lib().tb_obs_norm_update(_lib.ptr(sums), _lib.ptr(n.count), _lib.ptr(n.mean), _lib.ptr(n.var),
+                                                 n.mean.numel(), _lib.stream_ptr()), "tb_obs_norm_update")
+
+    # ---- reference-compatible forward ---------------------------------------------------------
+    def forward(self, inputs, core_state=()):
+        frame, done = inputs["frame"], inputs.get("done")
+        notdone = self._notdone(done) if self.use_lstm else None
+        h0, c0 = core_state if self.use_lstm else (None, None)
+        params = [v[0] for v in self._views]
+        if torch.is_grad_enabled() and any(q.requires_grad for q in params):
+            logits, baseline, hN, cN = _MLPNetFunction.apply(self, frame, inputs["reward"], notdone,
+                                                             inputs["last_action"], h0, c0, *params)
+        else:
+            logits, baseline, hN, cN = self._launch_forward(frame, inputs["reward"], notdone, inputs["last_action"],
+                                                            h0, c0)
+        logits = mask_policy(logits, inputs)  # with inputs["legal_actions"]: the sampler and argmax pick legal actions
+        T, B = baseline.shape[:2]
+        action = self._sample(logits, inputs) if self.training else self._greedy(logits)
+        out = dict(policy_logits=logits, baseline=baseline, action=action.view((T, B) + action.shape[2:]))
+        return out, ((hN, cN) if self.use_lstm else tuple())
 
 
 Net = AtariNet

@@ -44,8 +44,9 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
     `inference_batcher` yields DynamicBatcher batches (actorpool.cc:224-340): `batch.get_inputs()` returns
     `(batched_env_outputs, agent_state)` with [T=1, B, ...] leaves, B = 1 .. 512 actors; the forward of the SAME CUDA
     kernels the learner uses runs under `lock` on flags.actor_device, and `batch.set_outputs(((action, policy_logits,
-    baseline), core_state))` receives CPU tensors, like the reference.  Works for polybeast's Net (ResNet) and for AtariNet
-    (whose `last_action` input is batched_env_outputs[5] if the nest carries one, else zeros).
+    baseline), core_state))` receives CPU tensors, like the reference.  Works for polybeast's Net (ResNet), for AtariNet
+    and for MLPNet (float32 observations [1, B, O]); the last two take `last_action` from batched_env_outputs[5] if the
+    nest carries one, else zeros.
 
     A sampler attached as `model.action_sampler` (torchbeast_b200.sampling) replaces torch.multinomial in training mode;
     its step advances by one per call, safely across inference threads because the forward runs under `lock`.  The
@@ -63,7 +64,10 @@ def inference(flags, inference_batcher, model, lock=threading.Lock()):  # noqa: 
         for batch in inference_batcher:
             batched_env_outputs, agent_state = batch.get_inputs()
             frame, reward, done, *rest = batched_env_outputs
-            if frame.dim() != 5 or tuple(frame.shape[2:]) != obs:
+            if frame.dim() != 2 + len(obs) or tuple(frame.shape[2:]) != obs:
+                if len(obs) != 3:  # a vector observation (MLPNet)
+                    raise _lib.TorchBeastB200Error("inference takes observations [1, B, %s] for this net, got frame %r"
+                                                   % (", ".join(map(str, obs)), tuple(frame.shape)))
                 raise _lib.TorchBeastB200Error("inference takes stacked frames [1, B, %d, %d, %d]; unstacked rollouts are a "
                                                "learner input, got frame %r" % (obs + (tuple(frame.shape),)))
             inputs = dict(frame=frame.to(device, non_blocking=True), reward=reward.to(device, non_blocking=True),

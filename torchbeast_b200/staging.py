@@ -32,14 +32,16 @@ LEAF_ORDER = ("frame", "reward", "done", "episode_return", "episode_step", "poli
 FRAME_FORMATS = ("stacked", "unstacked")
 
 
-def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), extra=(), frame_format="stacked"):
+def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), extra=(), frame_format="stacked",
+             frame_dtype=torch.uint8):
     """Leaf name -> (shape, dtype) of one [T+1, B, ...] rollout batch (monobeast.py:299-316 buffers / the B2 nest).
     frame_format="unstacked": the frame leaf is [T+4, B, H, W], one newest frame per step after step 0's first three
     channels; the learner rebuilds the stacks on the GPU (include/torchbeast_b200.h, "unstacked rollouts").
     num_actions a tuple (A_1, ..., A_D): a factored action space (torchbeast_b200.action_space), whose policy_logits
     are [T+1, B, sum A_k] and whose action and last_action are [T+1, B, D].  num_actions a Gaussian(D): a continuous
     space, whose policy_logits are the (mu, log sigma) rows [T+1, B, 2D] and whose action and last_action are float32
-    [T+1, B, D]."""
+    [T+1, B, D].  frame_dtype: the frame leaf's dtype, e.g. torch.float32 with frame_shape=(O,) for an MLPNet's
+    observation vectors."""
     dims = action_space.dims_of(num_actions)
     D = action_space.continuous_dim_of(num_actions)
     act = (T + 1, B) if dims is None else (T + 1, B, len(dims))
@@ -52,7 +54,7 @@ def spec_for(T, B, num_actions, use_last_action=True, frame_shape=(4, 84, 84), e
     T1 = T + 1
     frame = (T1, B) + tuple(frame_shape) if frame_format == "stacked" else (T1 + 3, B) + tuple(frame_shape[1:])
     spec = collections.OrderedDict(
-        frame=(frame, torch.uint8),
+        frame=(frame, frame_dtype),
         reward=((T1, B), torch.float32),
         done=((T1, B), torch.bool),
         episode_return=((T1, B), torch.float32),
